@@ -1,9 +1,10 @@
 #!/usr/bin/env python
 """Headline benchmark: frames/sec of the SIVO perception front-end -- Bayesian SegNet(T) on the left image plus
 the ORB extractor on the left and right images -- on synthetic 1242x375 stereo frames (centre-cropped to the
-net's 1024x352 like System::TrackStereo does), N x B200.
+net's 1024x352 like System::TrackStereo does), N x H100.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--model basic|standard] [--T 6]
+                  [--dump-outputs DIR]
 
 One "step" = one stereo frame through both operators.  `value` times the operators with the cropped inputs
 already resident in HBM; `e2e` times the reference-facing calls (segmentImage / operator()) on HOST buffers,
@@ -16,6 +17,7 @@ import json
 import os
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
@@ -45,7 +47,36 @@ def parse_args():
                     help="--impl reference: full frames per step if (warmup + steps) of them fit this budget, else bounded samples")
     ap.add_argument("--sustain-seconds", type=float, default=3.0,
                     help="extra sustained leg on rank 0 (N=1): frames back to back for this long, own clock samples (0 = skip)")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed as DIR/<name>.npy (float32 / float64, rank 0)")
+    args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    return args
+
+
+def model_cache_dir():
+    """Generated model files are cached outside the source tree (which may be read-only), one directory per user."""
+    return os.path.join(tempfile.gettempdir(), f"sivo_b200_models_{os.getuid()}")
+
+
+def dump_outputs(out_dir, rec, conf, ent, kp_cap):
+    """Writes what the timed device step hands its caller for one frame -- the operator's double confidence / entropy maps and
+    the packed record (classes, single-precision maps, both extractors' keypoints and descriptors) -- as .npy files, so that
+    two builds can be compared output for output (about 10 MB at 1024x352)."""
+    from sivo_b200 import record
+    os.makedirs(out_dir, exist_ok=True)
+    r = record.unpack(rec.cpu().numpy(), NET_H, NET_W, kp_cap)
+    arrays = {"classes": r["classes"].astype(np.float32),
+              "confidence": conf.cpu().numpy().reshape(NET_H, NET_W), "entropy": ent.cpu().numpy().reshape(NET_H, NET_W),
+              "record_confidence_f32": r["confidence"], "record_entropy_f32": r["entropy"]}
+    for side in ("left", "right"):
+        kp = r["kp_" + side]
+        # one row per keypoint: x, y, size, angle, response, octave, class_id
+        arrays[f"keypoints_{side}"] = np.stack([kp[f].astype(np.float64) for f in kp.dtype.names], 1).reshape(-1, len(kp.dtype.names))
+        arrays[f"descriptors_{side}"] = r["desc_" + side].astype(np.float32)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(a))
 
 
 def model_files(kind, T, cache_dir):
@@ -78,7 +109,7 @@ def frames(n, start=0):
 
 
 class ClockSampler:
-    """SM clock and throttle reasons sampled DURING the timed region (B200_PROFILING.md): NVML from a thread every 2 ms
+    """SM clock and throttle reasons sampled DURING the timed region: NVML from a thread every 2 ms
     (the timed regions last tens of milliseconds, too short for `nvidia-smi -lms`), nvidia-smi as the fallback."""
 
     REASONS = {0x8: "hw_slowdown", 0x40: "hw_thermal_slowdown", 0x20: "sw_thermal_slowdown", 0x4: "sw_power_cap"}
@@ -192,7 +223,7 @@ def run_reference(args, rank, world):
     import gen_prototxt
     from sivo_b200.prototxt import load_net
     T = args.T or (6 if args.model == "basic" else (12 if world == 1 else 6))  # the GPU arm's rule: configs[1] / [2] / [3]
-    net, proto, model, weights = model_files(args.model, T, os.path.join("/tmp", "sivo_b200_models"))
+    net, proto, model, weights = model_files(args.model, T, model_cache_dir())
     weights = weights or load_weights(net, model)
     cores = os.cpu_count() or 1
     fr = frames(1)
@@ -280,17 +311,14 @@ def main():
     except Exception:
         pass
     if world > 1:
-        # The gather overlaps the next frame's convolutions, whose grids are sized to the 148 SMs (conv_decode1: 288 CTAs = two
-        # waves of 144).  A default NCCL all-gather takes a dozen SMs and would push them into a third wave, so keep it to a
-        # few channels: 3.5 MB per rank needs little bandwidth (measured at N=2 with the earlier 6.4 MB record: 8 channels 1278 fps,
-        # 2: 1425, 1: 1443).
-        # measured with the 3.5 MB record (profiles/r2_scaling.md): N=8 2 channels 9972 frames/s, 4 channels 10396 (N=1 1324)
+        # The gather overlaps the next frame's convolutions, whose grids are sized to the SM count.  A default NCCL all-gather
+        # takes a dozen SMs away from them, so keep it to a few channels: 3.5 MB per rank needs little bandwidth.
         nch = "1" if world <= 2 else ("2" if world <= 4 else "4")
         os.environ.setdefault("NCCL_MAX_NCHANNELS", nch)
         os.environ.setdefault("NCCL_MAX_CTAS", nch)
         dist.init_process_group("nccl", device_id=dev)
     T = args.T or (6 if args.model == "basic" else (12 if world == 1 else 6))
-    cache = os.path.join("/tmp", "sivo_b200_models")
+    cache = model_cache_dir()
     if rank == 0:
         net, proto, model, weights = model_files(args.model, T, cache)
     if world > 1:
@@ -357,7 +385,7 @@ def main():
         #   orb_l, orb_r (the handles' own streams, highest priority): wait side[k] -> extractor(i)
         #   side : wait seg[k] -> [all-gather of record k] -> side[k]
         # The extractors start with the frame, i.e. under SegNet's small early launches that leave SMs idle, and the main stream
-        # waits for them before the next frame: measured (profiles/r2_notes.md), letting SegNet run ahead instead (joining the
+        # waits for them before the next frame: letting SegNet run ahead instead (joining the
         # extractors on the side stream, SIVO_BENCH_JOIN=side) starves their 13 short dependent kernels behind 0.2 ms CTAs.
         if side_used[k]:
             stream.wait_event(ev_side[k])
@@ -516,6 +544,8 @@ def main():
     prof_value = dict(prof)  # the sustained leg and the e2e variants call device_step / the extractors again
     dev_ms = e0.elapsed_time(e1)
     elapsed = max(wall, dev_ms / 1e3)  # the ORB streams are the library's own; wall brackets everything (synced both sides)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, d_rec[(args.warmup + args.steps - 1) % NBUF], d_conf, d_ent, kp_cap)
     # ---- e2e: host buffers through the operator calls, three call patterns (the first is the headline)
     e2e_times = {}
     E2E_REPEATS = 3  # each measurement is exactly --steps frames; the median of three damps host-thread scheduling jitter
@@ -583,21 +613,14 @@ def main():
         except Exception:
             pass
         # the kernel is timed alone, by CUDA events, in a pass of <= 10 frames (milliseconds): burst regime -> the burst peak
-        peak = peaks.get("bf16_tflops") or 1650.0
+        # fallback: the H100 SXM data sheet's dense FP16 rate (989 TFLOP/s at 700 W), an upper bound that is not reached
+        peak = peaks.get("bf16_tflops") or 989.0
         which = "measured burst (MEASURED_PEAKS.json bf16_tflops): kernel timed alone in a <=10-frame pass" if peaks.get("bf16_tflops") \
-            else "fallback 1.65 PF burst (B200_PROFILING.md)"
-        peak_sus = peaks.get("bf16_tflops_sustained") or 1400.0
+            else "fallback: H100 SXM data-sheet dense FP16, 989 TFLOP/s"
+        peak_sus = peaks.get("bf16_tflops_sustained") or 989.0
         ach = op_flops[dom] / (op_ms[dom] * 1e-3) / 1e12
         ach_all = fl["exec"] / (np.mean(conv_ms) * 1e-3) / 1e12
-        traffic = None
-        for tf in ("r2_traffic.json", "r1_traffic.json"):  # dram bytes of that kernel from the committed `ncu --set full` capture
-            try:
-                tj = json.load(open(os.path.join(ROOT, "profiles", tf)))
-                traffic = tj.get(args.model, {}).get("dram_bytes_per_launch")
-                if traffic:
-                    break
-            except Exception:
-                pass
+        traffic = None  # DRAM bytes of the kernel: not measured
         # ---- sustained leg: >= --sustain-seconds of back-to-back work with its own clock samples, against the SUSTAINED peak
         sustained = None
         if args.sustain_seconds > 0 and world == 1:
@@ -624,10 +647,10 @@ def main():
                                   "conv_tflops_executed": tf_s, "frac_of_sustained_peak": tf_s / peak_sus,
                                   "conv_tflops_algorithmic": fl["dedup"] * n_done / dt / 1e12, "clocks": sm.stop()}
             sustained["peak"] = peak_sus
-            sustained["peak_source"] = "MEASURED_PEAKS.json bf16_tflops_sustained" if peaks.get("bf16_tflops_sustained") else "fallback 1.4 PF"
+            sustained["peak_source"] = "MEASURED_PEAKS.json bf16_tflops_sustained" if peaks.get("bf16_tflops_sustained") else "fallback: H100 SXM data-sheet dense FP16"
             sustained["note"] = "conv_tflops_executed = executed conv FLOPs per frame x frames / wall seconds of the whole leg (non-conv kernels and, in full_step, the extractors included)"
         roof = {"bound": "tensor", "achieved": ach, "peak": peak, "unit": "TFLOP/s", "frac": ach / peak, "traffic": traffic,
-                "kernel": f"tcgen05 convolution launch '{names[dom]}'", "peak_source": which,
+                "kernel": f"wgmma convolution launch '{names[dom]}'", "peak_source": which,
                 "kernel_ms": float(op_ms[dom]), "kernel_gflop": op_flops[dom] / 1e9, "kernel_gflop_algorithmic": op_alg[dom] / 1e9,
                 "flops_counted": "executed multiply-adds x 2 (see kernel_gflop_algorithmic / algorithmic_gflop_per_frame for the reference's operation count)",
                 "all_conv_launches": {"achieved": ach_all, "frac": ach_all / peak, "ms_per_frame": float(np.mean(conv_ms)),

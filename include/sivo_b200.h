@@ -1,4 +1,4 @@
-/* sivo_b200 -- C ABI of the B200-native SIVO perception front-end (libsivo_b200.so).
+/* sivo_b200 -- C ABI of the H100-native (sm_90a) SIVO perception front-end (libsivo_b200.so).
  *
  * The reference has no FFI on this path: the "plugin API" is two C++ classes.  The shim classes in
  * integration/ keep their public signatures and forward to the entry points below, so src/sivo.cc,

@@ -6,7 +6,7 @@ ComputeKeyPointsOctTree :752-847, DistributeOctTree :544-750, DivideNode :488-54
 computeOrbDescriptor :104-150, operator() :1019-1083).
 
 The arithmetic that lives in un-vendored OpenCV (`find_package(OpenCV 3.0)`, CMakeLists.txt:37-43 --
-version not pinned, sources not under /root/reference) is restated from OpenCV's published algorithms:
+version not pinned, sources not in the reference tree) is restated from OpenCV's published algorithms:
   cv::FAST (9_16, cornerScore, 3x3 NMS)      -> fast_score_map / cell_keypoints
   cv::resize INTER_LINEAR 8-bit fixed point   -> resize_linear_u8
   cv::copyMakeBorder BORDER_REFLECT_101       -> reflect101

@@ -33,7 +33,7 @@ class SegnetOptions(C.Structure):
 
 
 def build(verbose: bool = False) -> str:
-    """Compiles the library in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+    """Compiles the library in-tree with nvcc for sm_90a (cross-compiles without a GPU)."""
     r = subprocess.run(["make", "-C", os.path.join(_HERE, "csrc"), "-j8"], capture_output=True, text=True)
     if verbose or r.returncode:
         print(r.stdout[-4000:], r.stderr[-4000:])

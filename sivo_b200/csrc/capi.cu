@@ -30,7 +30,7 @@ struct sivo_orb { Orb* impl; };
 extern "C" {
 
 const char* sivo_last_error(void) { return g_last_error.c_str(); }
-const char* sivo_version(void) { return "sivo_b200 0.1 (sm_100a)"; }
+const char* sivo_version(void) { return "sivo_b200 0.1 (sm_90a)"; }
 
 int sivo_segnet_create_ex(const char* prototxt, const char* caffemodel, const sivo_segnet_options* opt, sivo_segnet_t** out) {
   return guarded([&] {
@@ -526,11 +526,6 @@ int sivo_dbg_conv(int device, int engine, int precision, const float* in, int n,
     op.bn_shift.alloc(sh.size() * 4);
     SIVO_CUDA(cudaMemcpy(op.w_simt.p, ws.data(), ws.size() * 4, cudaMemcpyHostToDevice));
     SIVO_CUDA(cudaMemcpy(op.w_tc.p, wt.data(), wt.size() * 2, cudaMemcpyHostToDevice));
-    if ((k == 7 || k == 3) && cin == 64 && cout == 64) {
-      std::vector<__half> wp = conv_tc_pair_weights(weight, k);
-      op.w_tc_pair.alloc(wp.size() * 2);
-      SIVO_CUDA(cudaMemcpy(op.w_tc_pair.p, wp.data(), wp.size() * 2, cudaMemcpyHostToDevice));
-    }
     SIVO_CUDA(cudaMemcpy(op.bias.p, b.data(), b.size() * 4, cudaMemcpyHostToDevice));
     SIVO_CUDA(cudaMemcpy(op.bn_scale.p, sc.data(), sc.size() * 4, cudaMemcpyHostToDevice));
     SIVO_CUDA(cudaMemcpy(op.bn_shift.p, sh.data(), sh.size() * 4, cudaMemcpyHostToDevice));

@@ -1,28 +1,28 @@
-// tcgen05 implicit-GEMM convolution for sm_100a -- replaces cuDNN's fp32 `cudnnConvolutionForward`
+// Hopper (sm_90a) implicit-GEMM convolution on wgmma -- replaces cuDNN's fp32 `cudnnConvolutionForward`
 // (caffe/src/caffe/layers/cudnn_conv_layer.cu:21-37) and the layers fused around it for every SegNet convolution
 // (Basic: all eight 7x7 layers + the 1x1 classifier; Standard: all 26 3x3 layers).
 //
 // GEMM view per CTA:  D[128 pixels x N couts] += A[128 pixels x 64 cin] * B[64 cin x N couts]  per filter tap,
-// M = 128 consecutive pixels of one output row, R = 4 (or 2) output rows -- a "row block" -- per accumulator stage.
+// M = 128 consecutive pixels of one output row, two output rows -- a "row block" -- per accumulator set.
 //
-//  * Activations are NHWC half, so one pixel's 64 input channels are one 128-byte row: exactly a
-//    SWIZZLE_128B K-major UMMA operand row.  A TMA box {64 ch, 128+K-1 px, 1 row} of the input lands one
-//    *halo row* in shared memory; out-of-image coordinates are zero-filled by TMA = the conv's zero padding.
-//  * The A operand of tap (kh, kw) for output row r is the same halo row shifted by kw pixels: the UMMA
-//    shared-memory descriptor simply starts kw*128 bytes later (the swizzle phase follows the absolute address), so
-//    each input row is fetched from L2 once per K rows of output instead of K*K times.
-//  * A CTA walks down a 128-px-wide column strip one row block at a time with a ring of halo rows: every input row is
-//    loaded once per CTA (plus the K-1 overlap between vertically adjacent CTAs) and released as soon as its last tap
-//    row has been issued.
-//  * Weights stream through a TMA ring, one tile per tap (k_conv_tc: {64 cin x N cout}, [tap][cout][cin]) or per pair of
-//    vertically adjacent taps (k_conv_tc_pair: two stacked tiles, N = 128, [kw][kh][cout][cin]).
+//  * Activations are NHWC half, so one pixel's 64 input channels are one 128-byte row: exactly a SWIZZLE_128B K-major
+//    wgmma operand row.  A TMA box {64 ch, 128+K-1 px, 1 row} of the input lands one *halo row* in shared memory;
+//    out-of-image coordinates are zero-filled by TMA = the conv's zero padding.
+//  * The A operand of tap (kh, kw) for output row r is the same halo row shifted by kw pixels: the shared-memory matrix
+//    descriptor simply starts kw*128 bytes later (the swizzle phase follows the absolute address), so each input row is
+//    fetched from L2 once per K rows of output instead of K*K times.
+//  * A CTA walks down a 128-px-wide column strip one row block at a time with a ring of halo rows (mbarrier full / empty
+//    pairs): every input row is loaded once per CTA (plus the K-1 overlap between vertically adjacent CTAs) and released
+//    as soon as its last tap row has retired.
+//  * Weights stream through a TMA ring, one {64 cin x N cout} tile per tap, [tap][cout][cin].
 //  * The 3-channel first layer reads a window-folded view of the zero-padded 8-channel image (KW = 1, see conv_tc_plan).
-//  * Accumulators live in TMEM (2 stages x R x N fp32 columns) so the epilogue of block j overlaps the MMAs of block
-//    j+1.  384 threads: warp 0 = halo-row TMA producer, warp 1 = weight TMA producer, warps 2-3 = MMA issuers (+ TMEM
-//    alloc), warps 4-11 = epilogue (two per TMEM lane quarter; setmaxnreg 56 / 216): tcgen05.ld -> bias / BN affine / ReLU
-//    -> half, then store | dropout | max-unpool scatter | 2x2 max-pool + argmax | 1x1 classifier -> float logits.
-//  * Constants (bias, BN, classifier weights) are kernel parameters; stores are 4-lane transposed (quad_transpose): the
-//    MMAs keep the shared-memory / L1 data path busy, so the epilogue must stay off it (DESIGN.md 4.1).
+//  * 384 threads = three warpgroups.  Warpgroup 0 produces (warp 0: halo rows, warp 1: weights; setmaxnreg 40);
+//    warpgroups 1 and 2 consume (setmaxnreg 232): consumer g owns pixels [64 g, 64 g + 64) of the tile, issues the
+//    m64nNk16 wgmma of both rows of the block into register accumulators, and runs the epilogue on them -- bias / BN
+//    affine / ReLU -> half, then store | dropout | max-unpool scatter | 2x2 max-pool + argmax | 1x1 classifier -> float
+//    logits -- while the other consumer's MMAs keep the tensor core busy.
+//  * Constants (bias, BN, classifier weights) are kernel parameters: the epilogue reads them from the constant bank and
+//    leaves the shared-memory data path to the MMA operand reads.
 #include <cuda.h>
 #include <cuda_fp16.h>
 
@@ -40,20 +40,17 @@ namespace sivo {
 
 namespace {
 
-constexpr int kTcThreads = 12 * 32;  // warps: 0 halo TMA, 1 weight TMA, 2-3 MMA issuers, 4-11 epilogue (two per TMEM lane quarter)
-constexpr int kEpiWarps = 8;
+constexpr int kTcThreads = 3 * 128;  // warpgroup 0: TMA producers, warpgroups 1-2: wgmma consumers + epilogue
+constexpr int kRows = 2;             // output rows per row block (accumulator set)
 constexpr int kSlotBytes = 17 * 1024;  // one halo row: (128 + K - 1) px * 128 B, padded to a 1024-B multiple
 constexpr int kMaxBStages = 6;
+constexpr int kEmptyArrivals = 8;    // every consumer warp releases a ring slot once its MMAs that read it retired
 
 struct TcParams {
   int H, W, N_batch;       // spatial size and batch of input == output
   int cout_total;          // channel stride of the output tensor
-  int n_tile;              // UMMA N (16 for the float logits layer, else 64 or 128)
+  int n_tile;              // wgmma N (16 for the float logits layer, else 64 or 128)
   int chunks;              // Cin / 64
-  int w_rep;               // weight tensor replicas in global memory (spreads the L2 hot spot all CTAs hammer)
-  int dbg_noepi;           // timing experiment only: 1 = epilogue does nothing, 2 = TMEM loads only, 3 = no global stores
-  int dbg_noshift;         // timing experiment only: ignore the kw shift of the A operand (wrong results)
-  int dbg_noload;          // timing experiment only: halo rows are loaded once per ring slot and then reused (wrong results)
   int b_stages;            // weight ring depth (as many of kMaxBStages as fit in shared memory)
   int out_f32;             // 1: 16-channel float output (logits); 2: n_tile-wide float output (split-operand fp32 mode)
   int split;               // split-operand fp32 mode: A = [hi Cin | lo Cin] half planes of the float input, B K-axis = per real chunk
@@ -63,11 +60,10 @@ struct TcParams {
   float rz_comp;           // split mode: expected truncation loss per accumulate step relative to the running sum (see seg_rows);
                            // each flushed segment of m steps is scaled by 1 + rz_comp * m before it is added (0 = off)
   int seg_rows;            // split mode: tap rows per accumulation segment.  The tensor core adds into its fp32 accumulator with
-                           // truncation (measured: ~2^-25 relative per accumulate step, always towards zero, so it grows linearly
-                           // with the chain length: 1.4e-5 for a 7x7x64 layer); the block's MMAs are therefore cut into segments
-                           // of (A chunk, seg_rows tap rows) that each start a fresh accumulator, and the epilogue sums the
-                           // segments in registers with round-to-nearest adds.
-  int pairs_per_cta;       // row blocks (R output rows each) one CTA walks
+                           // truncation towards zero, so the loss grows linearly with the chain length; the block's MMAs are
+                           // therefore cut into segments of (A chunk, seg_rows tap rows) that each start a fresh accumulator,
+                           // and the epilogue sums the segments in registers with round-to-nearest adds.
+  int pairs_per_cta;       // row blocks one CTA walks
   int strips;              // ceil(W / 128)
   int relu, has_bn, has_drop;
   float slope;
@@ -91,8 +87,7 @@ struct TcParams {
   float* cls_out;          // [N][H][W][16]
 };
 
-// Per-layer constants, passed by value as a kernel parameter so that the epilogue reads them from the constant bank
-// (FFMA operands / LDC) instead of through L1 or shared memory, whose data path the MMA operand reads saturate.
+// Per-layer constants, passed by value as a kernel parameter so that the epilogue reads them from the constant bank.
 constexpr int kMaxCout = 512;
 struct TcConsts {
   float bias[kMaxCout], bn_scale[kMaxCout], bn_shift[kMaxCout];
@@ -124,7 +119,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
         : "r"(addr), "r"(parity)
         : "memory");
     if (done) return;
-    if (spin > (1u << 26)) asm volatile("trap;");  // inline: a __trap() call stub pins the whole kernel to the setmaxnreg minimum
+    if (spin > (1u << 26)) asm volatile("trap;");
   }
 }
 
@@ -141,327 +136,247 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, u
       : "memory");
 }
 
-// K-major SWIZZLE_128B operand descriptor (cute::UMMA::SmemDescriptor): rows of 128 B, 8-row groups 1024 B apart.
-// High word: stride byte offset 1024 >> 4 (bits 32-45), version 1 (bits 46-47), base_offset 0 (bits 49-51),
-// layout SWIZZLE_128B = 2 (bits 61-63).  base_offset stays 0 even for operands that start kw*128 B into a
-// 1024-B-aligned halo row: measured on B200 (profiles/r1_notes.md) the XOR phase follows the absolute
-// shared-memory address bits [7:9]; writing (addr >> 7) & 7 there gives wrong products.
-constexpr uint32_t kDescHi = (1024u >> 4) | (1u << 14) | (2u << 29);
-
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "elect.sync _|p, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(pred));
-  return pred != 0;
+// K-major SWIZZLE_128B wgmma matrix descriptor: rows of 128 B, 8-row groups 1024 B apart.  High word: stride byte offset
+// 1024 >> 4 (bits 32-45), base offset 0 (bits 49-51), layout SWIZZLE_128B = 1 (bits 62-63).  Low word: start address >> 4
+// (bits 0-13), leading byte offset 1 (unused by swizzled K-major layouts).  A K step of 16 halfs advances the start by
+// 32 B (>> 4: 2); a tap column shifts an A operand by one 128-B row (8).  The XOR phase of the swizzle follows the
+// absolute shared-memory address, as TMA wrote it, so an operand may start at any 128-B row of a 1024-B-aligned halo row.
+constexpr uint32_t kDescHi = (1024u >> 4) | (1u << 30);
+__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
+  return (static_cast<uint64_t>(kDescHi) << 32) | (((smem_addr & 0x3FFFFu) >> 4) | (1u << 16));
 }
 
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
+// D[64 x N] (+)= A[64 x 16] * B[16 x N], both operands K-major in shared memory, fp32 accumulators in registers
+// (fragment layout: d[4 j + 2 h + e] = row 16 warp + lane / 4 + 8 h, column 8 j + 2 (lane % 4) + e)
+__device__ __forceinline__ void wgmma(float (&d)[8], uint64_t a, uint64_t b) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, 1, 1, 1, 0, 0;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(a), "l"(b));
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
+__device__ __forceinline__ void wgmma(float (&d)[32], uint64_t a, uint64_t b) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]),
-        "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]),
-        "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+      "%24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, 1, 1, 1, 0, 0;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a), "l"(b));
 }
-
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[32]) {
+__device__ __forceinline__ void wgmma(float (&d)[64], uint64_t a, uint64_t b) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+      "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, "
+      "%47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, 1, 1, 1, 0, 0;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+        "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+        "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+        "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
+        "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a), "l"(b));
 }
-
-// 4 x 4 transpose of 16-byte elements across each aligned group of four lanes: on entry lane c (of its group) holds
-// e[0..3] = chunks 0..3 of its own pixel; on return e[j] = chunk c of the group's pixel j.  After it, one store
-// instruction writes 64 contiguous bytes per pixel for 8 pixels instead of 16 bytes for 32: the epilogue's global
-// stores share the L1 / shared-memory data path with the MMA operand reads, and a warp store that touches 32
-// different lines holds that path four times longer (profiles/r1_notes.md).
-template <typename V4>
-__device__ __forceinline__ void quad_transpose(V4 (&e)[4], int lane) {
-  static_assert(sizeof(V4) == 16, "16-byte elements");
-  const bool odd = lane & 1, hi = lane & 2;
-  auto xchg = [](V4 v, int m) {
-    uint4 u = *reinterpret_cast<uint4*>(&v);
-    u.x = __shfl_xor_sync(0xffffffffu, u.x, m);
-    u.y = __shfl_xor_sync(0xffffffffu, u.y, m);
-    u.z = __shfl_xor_sync(0xffffffffu, u.z, m);
-    u.w = __shfl_xor_sync(0xffffffffu, u.w, m);
-    return *reinterpret_cast<V4*>(&u);
-  };
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// Ties the accumulator registers to the preceding wait: the compiler must not move their reads (or the zeroing of a
+// fresh segment) across it.
+template <int R, int F>
+__device__ __forceinline__ void fence_acc(float (&d)[R][F]) {
 #pragma unroll
-  for (int s = 0; s < 4; s += 2) {
-    const V4 got = xchg(odd ? e[s] : e[s + 1], 1);
-    if (odd) e[s] = got; else e[s + 1] = got;
-  }
+  for (int r = 0; r < R; ++r)
 #pragma unroll
-  for (int s = 0; s < 2; ++s) {
-    const V4 got = xchg(hi ? e[s] : e[s + 2], 2);
-    if (hi) e[s] = got; else e[s + 2] = got;
-  }
+    for (int i = 0; i < F; ++i) asm volatile("" : "+f"(d[r][i])::"memory");
 }
 
-// One output row of the epilogue for one thread (= one pixel x of row y): reads its accumulator columns from TMEM and
-// applies the runtime-selected tail (see the file header).  `trow` = TMEM address of this row's first column for the
-// thread's lane quarter, `n0` = first output channel of the CTA's tile.  Bias / BN / classifier constants come from the
-// kernel parameters (constant bank): loads through L1 or shared memory would compete with the MMA operand reads.
-// Must be called by all 32 lanes (warp shuffles); out-of-image pixels are masked at the stores.
-__device__ __forceinline__ void epilogue_row(const TcParams& p, const TcConsts& cst, uint32_t trow, int img, int y, int x, int n0, int lane) {
-    if (p.dbg_noepi == 1) return;
-    if (p.dbg_noepi == 2) {
-      for (int cc = 0; cc < p.n_tile; cc += 32) { uint32_t v[32]; tmem_ld32(trow + cc, v); if (v[0] == 0x12345678u && v[31] == 0x9abcdef0u) p.cls_out[0] = 1.f; }
-      return;
+__device__ __forceinline__ float affine(const TcParams& p, const TcConsts& cst, float v, int c) {
+  float t = __fadd_rn(v, cst.bias[c]);
+  if (p.has_bn) t = __fadd_rn(__fmul_rn(t, cst.bn_scale[c]), cst.bn_shift[c]);
+  if (p.relu) t = t > 0.f ? t : __fmul_rn(p.slope, t);
+  return t;
+}
+
+// Fused 1x1 classifier, one quad lane's share: partial logits over its 16 channels (8 j + 2 Q + e) of pixel h.
+template <int Q>
+__device__ __forceinline__ void cls_partial(const TcParams& p, const TcConsts& cst, const float (&a)[32], int h, float (&l)[16]) {
+#pragma unroll
+  for (int jj = 0; jj < 16; ++jj) l[jj] = 0.f;
+#pragma unroll
+  for (int j = 0; j < 8; ++j)
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const int c = 8 * j + 2 * Q + e;
+      const float hv = __half2float(__float2half_rn(affine(p, cst, a[4 * j + 2 * h + e], c)));
+#pragma unroll
+      for (int jj = 0; jj < 16; ++jj) l[jj] = fmaf(hv, cst.cls_w[c * 16 + jj], l[jj]);
     }
-    if (p.dbg_noepi == 3) x += 1 << 20;  // every store is predicated off by the x < W test
-    const int cl = lane & 3;          // this lane's 16-byte chunk after the transpose
-    const int xg = x - cl;            // first pixel of the lane's group of four
-    const bool row_ok = y < p.H && img < p.N_batch;  // img >= N: the odd image out of an image-pair tile (PK2)
-    if (p.out_f32 == 1) {  // 16-channel float logits (the convolution feeding Softmax)
-      uint32_t v[32];
-      tmem_ld16(trow, v);
-      float4 e[4];
+}
+
+// Epilogue of one row block for one consumer thread.  The thread holds, per output row r, pixels m0 and m0 + 8 of its
+// consumer's 64 (h = 0, 1) and channels 8 j + 2 q + e (q = lane % 4) of each: acc[r][4 j + 2 h + e].  `x_m0` = image column
+// of pixel m0, `y0` = first row of the block, `n0` = first output channel of the CTA's tile.  Called by all 32 lanes
+// (warp shuffles); out-of-image pixels are masked at the stores.
+template <int N>
+__device__ __forceinline__ void epilogue_block(const TcParams& p, const TcConsts& cst, const float (&acc)[kRows][N / 2], int img,
+                                               int y0, int x_m0, int n0, int lane) {
+  const int q = lane & 3;
+  const bool img_ok = img < p.N_batch;  // img >= N: the odd image out of an image-pair tile (PK2)
+  if (p.pool_out) {  // both rows of the block: 2x2 max with first-maximum argmax; the horizontal neighbour is pixel m + 1 = lane ^ 4
 #pragma unroll
-      for (int i = 0; i < 16; ++i) {
-        float t = __fadd_rn(__uint_as_float(v[i]), cst.bias[i]);
-        if (p.has_bn) t = __fadd_rn(__fmul_rn(t, cst.bn_scale[i]), cst.bn_shift[i]);
-        if (p.relu) t = t > 0.f ? t : __fmul_rn(p.slope, t);
-        reinterpret_cast<float*>(&e[i >> 2])[i & 3] = t;
-      }
-      quad_transpose(e, lane);
+    for (int h = 0; h < 2; ++h) {
+      const int x = x_m0 + 8 * h;
+      const bool writer = ((x & 1) == 0) && y0 + 1 < p.H && x + 1 < p.W && img_ok;
+      const size_t o = ((static_cast<size_t>(img) * (p.H >> 1) + (y0 >> 1)) * (p.W >> 1) + (x >> 1)) * p.cout_total + n0;
 #pragma unroll
-      for (int j = 0; j < 4; ++j)
-        if (row_ok && xg + j < p.W)
-          *reinterpret_cast<float4*>(reinterpret_cast<float*>(p.out) + ((static_cast<size_t>(img) * p.H + y) * p.W + xg + j) * 16 + 4 * cl) = e[j];
-      return;
-    }
-    if (p.has_cls) {  // conv (+bias) -> half rounding (as the unfused path stores it) -> 1x1 classifier -> float logits
-      float l[16];
+      for (int j = 0; j < N / 8; ++j) {
+        const int c = 8 * j + 2 * q;
+        const __half2 ha = __floats2half2_rn(affine(p, cst, acc[0][4 * j + 2 * h], n0 + c), affine(p, cst, acc[0][4 * j + 2 * h + 1], n0 + c + 1));
+        const __half2 hc = __floats2half2_rn(affine(p, cst, acc[1][4 * j + 2 * h], n0 + c), affine(p, cst, acc[1][4 * j + 2 * h + 1], n0 + c + 1));
+        const uint32_t a = *reinterpret_cast<const uint32_t*>(&ha), cc = *reinterpret_cast<const uint32_t*>(&hc);
+        const uint32_t b = __shfl_xor_sync(0xffffffffu, a, 4), d = __shfl_xor_sync(0xffffffffu, cc, 4);
+        // window in scan order: a = (y, x), b = (y, x+1), c = (y+1, x), d = (y+1, x+1); two channels per register
+        uint32_t best = a, arg = 0;
+        const uint32_t cand[3] = {b, cc, d};
 #pragma unroll
-      for (int jj = 0; jj < 16; ++jj) l[jj] = cst.cls_b[jj];
-#pragma unroll
-      for (int cc = 0; cc < 64; cc += 32) {
-        uint32_t v[32];
-        tmem_ld32(trow + cc, v);
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          float t = __fadd_rn(__uint_as_float(v[i]), cst.bias[cc + i]);
-          if (p.has_bn) t = __fadd_rn(__fmul_rn(t, cst.bn_scale[cc + i]), cst.bn_shift[cc + i]);
-          if (p.relu) t = t > 0.f ? t : __fmul_rn(p.slope, t);
-          const float hv = __half2float(__float2half_rn(t));
-#pragma unroll
-          for (int jj = 0; jj < 16; ++jj) l[jj] = fmaf(hv, cst.cls_w[(cc + i) * 16 + jj], l[jj]);
+        for (int k = 0; k < 3; ++k) {
+          // strict '>' per half (false on NaN, like __hgt): 0xFFFF where the candidate wins
+          const uint32_t sel = __hgt2_mask(*reinterpret_cast<const __half2*>(&cand[k]), *reinterpret_cast<const __half2*>(&best));
+          best = (best & ~sel) | (cand[k] & sel);
+          const uint32_t selb = __byte_perm(sel, 0u, 0x4420);  // the two half masks as two byte masks (bytes 0 and 1)
+          arg = (arg & ~selb) | ((0x0101u * static_cast<uint32_t>(k + 1)) & selb);
+        }
+        if (writer) {
+          *reinterpret_cast<uint32_t*>(p.pool_out + o + c) = best;
+          *reinterpret_cast<uint16_t*>(p.pool_mask + o + c) = static_cast<uint16_t>(arg);
         }
       }
-      float4 e[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) e[i] = make_float4(l[4 * i], l[4 * i + 1], l[4 * i + 2], l[4 * i + 3]);
-      quad_transpose(e, lane);
-#pragma unroll
-      for (int j = 0; j < 4; ++j)
-        if (row_ok && xg + j < p.W)
-          *reinterpret_cast<float4*>(p.cls_out + ((static_cast<size_t>(img) * p.H + y) * p.W + xg + j) * 16 + 4 * cl) = e[j];
-      return;
     }
-    uint32_t bits[4] = {0, 0, 0, 0};
-    // max-unpool: fetch the 2-bit mask codes of the first 64 channels before touching TMEM, so the (DRAM / L2) latency
-    // of the mask overlaps the accumulator loads.  Already in the transposed arrangement: lane (group, cl) reads the 8
-    // codes of channels [8 cl, 8 cl + 8) of each of its group's four pixels.
-    uint2 mrow[2][4] = {};
-    const size_t mask_row = (static_cast<size_t>(img % p.mask_n) * p.H + y) * p.W;
-    if (p.unpool_mask && row_ok) {
+    return;
+  }
 #pragma unroll
-      for (int h = 0; h < 2; ++h)
+  for (int r = 0; r < kRows; ++r) {
+    const int y = y0 + r;
+    const bool row_ok = y < p.H && img_ok;
+    if constexpr (N == 64) if (p.has_cls) {  // conv (+bias) -> half rounding (as the unfused path stores it) -> 1x1 classifier -> float logits
 #pragma unroll
-        for (int j = 0; j < 4; ++j)
-          if (xg + j < p.W && h * 32 < p.n_tile)
-            mrow[h][j] = __ldg(reinterpret_cast<const uint2*>(p.unpool_mask + (mask_row + xg + j) * p.cout_total + n0 + h * 32 + 8 * cl));
-    }
-    const bool inside = row_ok && x < p.W;
-    for (int cc = 0; cc < p.n_tile; cc += 32) {
-      uint32_t v[32];
-      tmem_ld32(trow + cc, v);
-      const int c0 = n0 + cc;
-      if (p.has_drop && inside && ((c0 & 127) == 0 || cc == 0))
-        dropout_bits128(p.seed, *p.frame, p.drop_layer, img, static_cast<uint32_t>(y * p.W + x), c0 >> 7, bits);
-      const int wsel = (c0 >> 5) & 3;  // selects, not a dynamically indexed (= local-memory) array
-      const uint32_t keep = !p.has_drop ? 0xFFFFFFFFu : wsel == 0 ? bits[0] : wsel == 1 ? bits[1] : wsel == 2 ? bits[2] : bits[3];
-      uint4 e[4];
-#pragma unroll
-      for (int i = 0; i < 32; i += 2) {
-        float f[2];
-#pragma unroll
-        for (int k = 0; k < 2; ++k) {
-          const int c = c0 + i + k;
-          float t = __fadd_rn(__uint_as_float(v[i + k]), cst.bias[c]);
-          if (p.has_bn) t = __fadd_rn(__fmul_rn(t, cst.bn_scale[c]), cst.bn_shift[c]);
-          if (p.relu) t = t > 0.f ? t : __fmul_rn(p.slope, t);
-          f[k] = t;
+      for (int h = 0; h < 2; ++h) {
+        float l[16];
+        switch (q) {  // one copy per quad lane, so that the classifier weights are compile-time constant-bank operands
+          case 0: cls_partial<0>(p, cst, acc[r], h, l); break;
+          case 1: cls_partial<1>(p, cst, acc[r], h, l); break;
+          case 2: cls_partial<2>(p, cst, acc[r], h, l); break;
+          default: cls_partial<3>(p, cst, acc[r], h, l); break;
         }
-        __half2 h = __floats2half2_rn(f[0], f[1]);
+#pragma unroll
+        for (int jj = 0; jj < 16; ++jj) {  // the four lanes of a pixel hold a quarter of its channels each
+          l[jj] += __shfl_xor_sync(0xffffffffu, l[jj], 1);
+          l[jj] += __shfl_xor_sync(0xffffffffu, l[jj], 2);
+          l[jj] = __fadd_rn(l[jj], cst.cls_b[jj]);
+        }
+        const int x = x_m0 + 8 * h;
+        const float4 v = q == 0 ? make_float4(l[0], l[1], l[2], l[3]) : q == 1 ? make_float4(l[4], l[5], l[6], l[7])
+                       : q == 2 ? make_float4(l[8], l[9], l[10], l[11]) : make_float4(l[12], l[13], l[14], l[15]);
+        if (row_ok && x < p.W) *reinterpret_cast<float4*>(p.cls_out + ((static_cast<size_t>(img) * p.H + y) * p.W + x) * 16 + 4 * q) = v;
+      }
+      continue;
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int x = x_m0 + 8 * h;
+      const bool inside = row_ok && x < p.W;
+      const size_t pix = (static_cast<size_t>(img) * p.H + y) * p.W + x;
+      if (p.out_f32) {  // float logits / split-mode output (the split epilogue passes accumulators already scaled by 2^-s)
+#pragma unroll
+        for (int j = 0; j < N / 8; ++j) {
+          const int c = n0 + 8 * j + 2 * q;
+          const float2 v = make_float2(affine(p, cst, acc[r][4 * j + 2 * h], c), affine(p, cst, acc[r][4 * j + 2 * h + 1], c + 1));
+          if (inside) *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + pix * p.cout_total + c) = v;
+        }
+        continue;
+      }
+      uint32_t bits[4] = {0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu};
+      if (p.has_drop && inside)  // a tile never straddles a 128-channel group (n0 is a multiple of N <= 128)
+        dropout_bits128(p.seed, *p.frame, p.drop_layer, img, static_cast<uint32_t>(y * p.W + x), n0 >> 7, bits);
+      const size_t mask_pix = (static_cast<size_t>(img % p.mask_n) * p.H + y) * p.W + x;
+#pragma unroll
+      for (int j = 0; j < N / 8; ++j) {
+        const int c = n0 + 8 * j + 2 * q;
+        __half2 hv = __floats2half2_rn(affine(p, cst, acc[r][4 * j + 2 * h], c), affine(p, cst, acc[r][4 * j + 2 * h + 1], c + 1));
         if (p.has_drop) {  // y = x * keep * 2 on the stored half value (exact)
-          __half2 sc = __floats2half2_rn((keep >> i) & 1u ? p.drop_scale : 0.f, (keep >> (i + 1)) & 1u ? p.drop_scale : 0.f);
-          h = __hmul2(h, sc);
+          const int wsel = (c >> 5) & 3;  // selects, not a dynamically indexed (= local-memory) array
+          const uint32_t keep = wsel == 0 ? bits[0] : wsel == 1 ? bits[1] : wsel == 2 ? bits[2] : bits[3];
+          const int bit = c & 31;
+          hv = __hmul2(hv, __floats2half2_rn((keep >> bit) & 1u ? p.drop_scale : 0.f, (keep >> (bit + 1)) & 1u ? p.drop_scale : 0.f));
         }
-        reinterpret_cast<uint32_t*>(&e[i >> 3])[(i >> 1) & 3] = *reinterpret_cast<uint32_t*>(&h);
-      }
-      quad_transpose(e, lane);  // e[j] = channels [c0 + 8 cl, c0 + 8 cl + 8) of pixel xg + j
-      if (p.unpool_mask) {
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          uint2 m;
-          if (cc == 0) m = mrow[0][j];
-          else if (cc == 32) m = mrow[1][j];
-          else {
-            m = make_uint2(0u, 0u);
-            if (row_ok && xg + j < p.W)
-              m = __ldg(reinterpret_cast<const uint2*>(p.unpool_mask + (mask_row + xg + j) * p.cout_total + c0 + 8 * cl));
-          }
-          if (!(row_ok && xg + j < p.W)) continue;
-          const uint32_t ew[4] = {e[j].x, e[j].y, e[j].z, e[j].w};         // half2 i = channels 2i, 2i+1 -> mask bytes 2i, 2i+1
-          // the last block's epilogue is exposed at the end of every CTA, so its instruction count matters: one address per
-          // output pixel (the four positions are constant offsets from it) and the eight mask bytes compared four at a time
-          __half* const ob = static_cast<__half*>(p.out) +
-              ((static_cast<size_t>(img) * 2 * p.H + 2 * y) * (2 * p.W) + 2 * (xg + j)) * p.cout_total + c0 + 8 * cl;
+        const uint32_t w = *reinterpret_cast<const uint32_t*>(&hv);
+        if (!inside) continue;
+        if (p.unpool_mask) {
+          // the value goes to the 2x2 position its mask byte names, zeros to the other three
+          const uint32_t m = __ldg(reinterpret_cast<const uint16_t*>(p.unpool_mask + mask_pix * p.cout_total + c));
+          __half* const ob = static_cast<__half*>(p.out) + ((static_cast<size_t>(img) * 2 * p.H + 2 * y) * (2 * p.W) + 2 * x) * p.cout_total + c;
           const size_t row_step = static_cast<size_t>(2 * p.W) * p.cout_total;
 #pragma unroll
           for (int pos = 0; pos < 4; ++pos) {
-            const uint32_t eq0 = __vcmpeq4(m.x, 0x01010101u * pos), eq1 = __vcmpeq4(m.y, 0x01010101u * pos);  // 0xFF per matching byte
-            // bytes (2i, 2i+1) of the mask widen to the two halves of word i
-            const uint32_t s0 = ew[0] & __byte_perm(eq0, 0u, 0x1100), s1 = ew[1] & __byte_perm(eq0, 0u, 0x3322);
-            const uint32_t s2 = ew[2] & __byte_perm(eq1, 0u, 0x1100), s3 = ew[3] & __byte_perm(eq1, 0u, 0x3322);
-            *reinterpret_cast<uint4*>(ob + (pos >> 1) * row_step + (pos & 1) * p.cout_total) = make_uint4(s0, s1, s2, s3);
+            const uint32_t sel = ((m & 0xFFu) == static_cast<uint32_t>(pos) ? 0x0000FFFFu : 0u) | ((m >> 8) == static_cast<uint32_t>(pos) ? 0xFFFF0000u : 0u);
+            *reinterpret_cast<uint32_t*>(ob + (pos >> 1) * row_step + (pos & 1) * p.cout_total) = w & sel;
           }
+        } else {
+          *reinterpret_cast<uint32_t*>(static_cast<__half*>(p.out) + pix * p.cout_total + c) = w;
         }
-      } else {
-#pragma unroll
-        for (int j = 0; j < 4; ++j)
-          if (row_ok && xg + j < p.W)
-            *reinterpret_cast<uint4*>(static_cast<__half*>(p.out) + ((static_cast<size_t>(img) * p.H + y) * p.W + xg + j) * p.cout_total + c0 + 8 * cl) = e[j];
       }
-    }
-}
-
-// Two vertically adjacent output rows (y even) with the pooling epilogue: bias / BN / ReLU -> half (the value the
-// unfused path would store) -> 2x2 max with first-maximum argmax; the horizontal neighbour lives in the adjacent lane.
-__device__ __forceinline__ void epilogue_pool_rows(const TcParams& p, const TcConsts& cst, uint32_t trow0, uint32_t trow1, int img, int y, int x, int n0, int lane) {
-  if (p.dbg_noepi) return;
-  const bool writer = (lane & 1) == 0 && y + 1 < p.H && x + 1 < p.W && img < p.N_batch;
-  for (int cc = 0; cc < p.n_tile; cc += 32) {
-    uint32_t v0[32], v1[32];
-    tmem_ld32(trow0 + cc, v0);
-    tmem_ld32(trow1 + cc, v1);
-    const int c0 = n0 + cc;
-    uint32_t outv[16], outm[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) outm[i] = 0;
-#pragma unroll
-    for (int i = 0; i < 32; i += 2) {
-      __half2 h[2];
-#pragma unroll
-      for (int r = 0; r < 2; ++r) {
-        float f[2];
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int c = c0 + i + e;
-          float t = __fadd_rn(__uint_as_float(r ? v1[i + e] : v0[i + e]), cst.bias[c]);
-          if (p.has_bn) t = __fadd_rn(__fmul_rn(t, cst.bn_scale[c]), cst.bn_shift[c]);
-          if (p.relu) t = t > 0.f ? t : __fmul_rn(p.slope, t);
-          f[e] = t;
-        }
-        h[r] = __floats2half2_rn(f[0], f[1]);
-      }
-      const uint32_t a = *reinterpret_cast<uint32_t*>(&h[0]), c = *reinterpret_cast<uint32_t*>(&h[1]);
-      const uint32_t b = __shfl_xor_sync(0xffffffffu, a, 1), d = __shfl_xor_sync(0xffffffffu, c, 1);
-      // window in scan order: a = (y, x), b = (y, x+1), c = (y+1, x), d = (y+1, x+1); two channels per register
-      uint32_t best = a, arg = 0;
-      const uint32_t cand[3] = {b, c, d};
-#pragma unroll
-      for (int k = 0; k < 3; ++k) {
-        // strict '>' per half (false on NaN, like __hgt): 0xFFFF where the candidate wins
-        const uint32_t sel = __hgt2_mask(*reinterpret_cast<const __half2*>(&cand[k]), *reinterpret_cast<const __half2*>(&best));
-        best = (best & ~sel) | (cand[k] & sel);
-        const uint32_t selb = __byte_perm(sel, 0u, 0x4420);  // the two half masks as two byte masks (bytes 0 and 1)
-        arg = (arg & ~selb) | ((0x0101u * static_cast<uint32_t>(k + 1)) & selb);
-      }
-      outv[i >> 1] = best;
-      outm[i >> 2] |= arg << (((i >> 1) & 1) * 16);  // two mask bytes per half2, four per 32-bit word
-    }
-    if (writer) {
-      const size_t o = ((static_cast<size_t>(img) * (p.H >> 1) + (y >> 1)) * (p.W >> 1) + (x >> 1)) * p.cout_total + c0;
-      uint4* dv = reinterpret_cast<uint4*>(p.pool_out + o);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) dv[i] = make_uint4(outv[4 * i], outv[4 * i + 1], outv[4 * i + 2], outv[4 * i + 3]);
-      uint4* dm = reinterpret_cast<uint4*>(p.pool_mask + o);
-      dm[0] = make_uint4(outm[0], outm[1], outm[2], outm[3]);
-      dm[1] = make_uint4(outm[4], outm[5], outm[6], outm[7]);
     }
   }
 }
 
 // ROLL = true : one 64-channel chunk (Cin == 64); halo rows persist in the ring while the CTA walks down its
 //               strip, so each input row is fetched once per CTA.
-// ROLL = false: Cin = 64 * NC; per (row pair, chunk) the kRows+K-1 halo rows of that chunk are fetched, used by
+// ROLL = false: Cin = 64 * NC; per (row block, chunk) the kRows+K-1 halo rows of that chunk are fetched, used by
 //               the K*K taps and released; the ring double-buffers chunks.
 // KW < K : the kernel is K x KW over a *window-folded* input (KW = 1: every pixel's 64 "channels" are the 8-pixel x
 //               8-channel window starting at it, so a 3-channel K x K layer is a K x 1 layer; see conv_tc_plan).
 // PK2 (only with !ROLL): layers at most 64 pixels wide (Standard's conv5_x at 22x64) would fill half of every 128-pixel M tile.
-//               Two images share a tile instead (rows 0-63: image 2z, rows 64-127: image 2z+1), and because the kw shift of a
+//               Two images share a tile instead (consumer 0: image 2z, consumer 1: image 2z+1), and because the kw shift of a
 //               shared-memory row would run from one image into the other, the shift is done by TMA: per (chunk, kw) the halo rows
 //               are fetched as two 64-pixel boxes starting at pixel kw - 1 (out-of-range pixels and images zero-filled), so the
 //               A operand of tap (kh, kw) is an unshifted, fully populated tile.  3x the halo traffic, which these small layers
 //               have to spare; weights arrive in (kw, kh) order.
-template <int K, bool ROLL, int kRows, int KW = K, bool PK2 = false>
+// SPLIT: split-operand fp32 mode (see TcParams::split / seg_rows); N <= 64 so that the segment sums fit in registers.
+template <int K, bool ROLL, int KW, bool PK2, int N, bool SPLIT>
 __global__ void __launch_bounds__(kTcThreads, 1)
 k_conv_tc(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const __grid_constant__ TcParams p,
           const __grid_constant__ TcConsts cst) {
   asm volatile("griddepcontrol.launch_dependents;");  // the next kernel's CTAs may be scheduled as soon as all of ours have started
-  constexpr int RK = kRows + K - 1;                  // halo rows one row pair reads (per chunk)
-  // rows are released as soon as their last tap row is issued; !ROLL double-buffers chunks where that fits (K = 7: RK + 2)
+  static_assert(!PK2 || (!ROLL && KW == K), "image-pair tiles use the chunked kernel");
+  static_assert(!SPLIT || (!ROLL && N <= 64), "split mode: chunked kernel, segment sums in registers");
+  constexpr int RK = kRows + K - 1;                  // halo rows one row block reads (per chunk)
+  // rows are released as soon as their last tap row retired; !ROLL double-buffers chunks where that fits (K = 7: RK + 2)
   constexpr int kSlots = ROLL ? RK : (K == 7 ? RK + 2 : 2 * RK);
   constexpr int kPad = (K - 1) / 2, kPadW = (KW - 1) / 2;
+  constexpr int F = N / 2;                           // accumulator registers per thread per output row
+  constexpr int b_bytes = N * 128;
+  constexpr int b_stride = (b_bytes + 1023) & ~1023;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
   uint8_t* a_slots = smem;
   uint8_t* b_stages = smem + kSlots * kSlotBytes;
-  const int b_bytes = p.n_tile * 128;
-  const int b_stride = (b_bytes + 1023) & ~1023;
   const int kBStages = p.b_stages;
   uint64_t* bars = reinterpret_cast<uint64_t*>(b_stages + kBStages * b_stride);
   uint64_t* a_full = bars;                       // [kSlots]
   uint64_t* a_empty = a_full + kSlots;           // [kSlots]
   uint64_t* b_full = a_empty + kSlots;           // [kBStages]
   uint64_t* b_empty = b_full + kBStages;         // [kBStages]
-  uint64_t* t_full = b_empty + kBStages;         // [2]
-  uint64_t* t_empty = t_full + 2;                // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(t_empty + 2);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int strip = blockIdx.x % p.strips, rowblk = blockIdx.x / p.strips;
-  static_assert(!PK2 || (!ROLL && KW == K), "image-pair tiles use the chunked kernel");
   constexpr int UPC = PK2 ? KW * RK : RK;          // halo units per (row block, chunk)
-  const int n0 = blockIdx.y * p.n_tile;
+  const int n0 = blockIdx.y * N;
   const int img = PK2 ? 2 * blockIdx.z : blockIdx.z;
   const int x0 = strip * 128;
   const int NC = ROLL ? 1 : p.chunks;
@@ -470,35 +385,23 @@ k_conv_tc(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUt
   const int npairs = min(p.pairs_per_cta, total_pairs - pair0);
   const int y_base = pair0 * kRows;              // first output row of this CTA
   const int n_units = ROLL ? npairs * kRows + K - 1 : npairs * NC * UPC;
-  uint32_t tmem_cols = 32;
-  while (tmem_cols < static_cast<uint32_t>(2 * kRows * p.n_tile)) tmem_cols <<= 1;
 
   if (threadIdx.x == 0) {
-    // two MMA issuer warps (each owns half of the output rows): every consumer-side release needs both commits
-    for (int i = 0; i < kSlots; ++i) { mbar_init(a_full + i, 1); mbar_init(a_empty + i, 2); }
-    for (int i = 0; i < kBStages; ++i) { mbar_init(b_full + i, 1); mbar_init(b_empty + i, 2); }
-    for (int i = 0; i < 2; ++i) { mbar_init(t_full + i, 2); mbar_init(t_empty + i, kEpiWarps); }
+    for (int i = 0; i < kSlots; ++i) { mbar_init(a_full + i, 1); mbar_init(a_empty + i, kEmptyArrivals); }
+    for (int i = 0; i < kBStages; ++i) { mbar_init(b_full + i, 1); mbar_init(b_empty + i, kEmptyArrivals); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(tmem_cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
-  // everything above touched only this CTA's shared / tensor memory; the producing kernel's results are needed from here on
+  // everything above touched only this CTA's shared memory; the producing kernel's results are needed from here on
   asm volatile("griddepcontrol.wait;" ::: "memory");
 
-  // 384 threads start with 168 registers each; the TMA / MMA-issue warpgroup needs few, the two epilogue warpgroups
-  // (32 accumulator words + packed outputs + masks per thread) need many: 128 x 56 + 256 x 216 = 62 464 <= 65 536
-  if (warp < 4) {
-  asm volatile("setmaxnreg.dec.sync.aligned.u32 56;" ::: "memory");
-  if (warp == 0) {
-    // ===== halo-row producer =====
-    if (lane == 0) {
+  if (wg == 0) {
+    // 384 threads start with 168 registers each; the producers need few, the consumers (2 rows x N/2 accumulators, the
+    // split sums, the epilogue's packed outputs) many: 128 x 40 + 256 x 232 = 64 512 <= 65 536
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+    if (warp == 0 && lane == 0) {
+      // ===== halo-row producer =====
       asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_a)) : "memory");
       for (int u = 0; u < n_units; ++u) {
         const int slot = u % kSlots;
@@ -523,12 +426,9 @@ k_conv_tc(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUt
         mbar_expect_tx(a_full + slot, static_cast<uint32_t>((128 + KW - 1) * 128));
         tma_load_4d(a_slots + slot * kSlotBytes, &map_a, a_full + slot, a_ch, x0 - kPadW, yy, img);
       }
-    }
-  } else if (warp == 1) {
-    // ===== weight producer =====
-    if (lane == 0) {
+    } else if (warp == 1 && lane == 0) {
+      // ===== weight producer =====
       asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_b)) : "memory");
-      const int w_replica = static_cast<int>((blockIdx.x + blockIdx.z) % static_cast<unsigned>(p.w_rep));
       uint32_t it = 0;
       for (int j = 0; j < npairs; ++j)
         for (int ch = 0; ch < NC; ++ch) {
@@ -541,620 +441,108 @@ k_conv_tc(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUt
               mbar_expect_tx(b_full + st, static_cast<uint32_t>(b_bytes));
               const int kc = p.split ? (3 * (ch >> 1) + ((ch & 1) ? 2 : rep)) * 64 : ch * 64;
               const int tap_w = PK2 ? (tap % K) * K + tap / K : tap;  // PK2 consumes taps kw-major: (kw, kh) -> kh * K + kw
-              tma_load_3d(b_stages + st * b_stride, &map_b, b_full + st, kc, n0, tap_w + w_replica * K * KW);
+              tma_load_3d(b_stages + st * b_stride, &map_b, b_full + st, kc, n0, tap_w);
             }
         }
     }
-  } else if (warp == 2 || warp == 3) {
-    // ===== MMA issuers: warp 2 owns output rows [0, kRows/2), warp 3 the rest.  The loops are warp-uniform (all 32
-    // lanes wait on the barriers) and one elected lane issues, so addresses stay in uniform registers: with N = 64 an
-    // MMA retires every 32 tensor cycles and a single issuing thread running ~14 instructions per MMA was the limiter
-    // (profiles/r1_notes.md).
-    constexpr int kMine = kRows / 2;
-    const int r_first = (warp - 2) * kMine;
-    const uint32_t idesc = (1u << 4) | (static_cast<uint32_t>(p.n_tile >> 3) << 17) | (8u << 24);  // f16 x f16 -> f32, M = 128
-    const uint32_t a_base = smem_u32(a_slots), b_base = smem_u32(b_stages);
-    int st = 0;
-    uint32_t b_phase = 0;
-    int waited = 0;  // halo units whose TMA has been observed
-    int seg = 0;  // accumulation segments issued so far (== row blocks unless split mode cuts a block into several)
-    const int S = p.split ? p.seg_rows : K;
-    for (int j = 0; j < npairs; ++j) {
-      int acc = seg & 1;
-      for (int ch = 0; ch < NC; ++ch)
-      for (int kwo = 0; kwo < (PK2 ? KW : 1); ++kwo) {  // PK2: the kw shift is done by TMA, one set of halo rows per tap column
-        const int base_u = ROLL ? j * kRows : PK2 ? ((j * NC + ch) * KW + kwo) * RK : (j * NC + ch) * RK;
-        for (int kh = 0; kh < K; ++kh) {
-          const bool seg_start = p.split ? (kh % S == 0) : (ch == 0 && kwo == 0 && kh == 0);
-          const bool seg_end = p.split ? (kh % S == S - 1 || kh == K - 1) : (ch == NC - 1 && kwo == (PK2 ? KW - 1 : 0) && kh == K - 1);
-          if (seg_start) {
-            acc = seg & 1;
-            mbar_wait(t_empty + acc, ((seg >> 1) & 1) ^ 1);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          }
-          while (waited <= base_u + kh + kRows - 1 && waited < n_units) {
-            mbar_wait(a_full + waited % kSlots, (waited / kSlots) & 1);
-            ++waited;
-          }
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          uint32_t a_row_lo[kMine], d_row[kMine];
-#pragma unroll
-          for (int m = 0; m < kMine; ++m) {
-            const int unit = base_u + r_first + m + kh;
-            a_row_lo[m] = (((a_base + (unit % kSlots) * kSlotBytes) & 0x3FFFFu) >> 4) | (1u << 16);
-            d_row[m] = tmem_base + static_cast<uint32_t>((acc * kRows + r_first + m) * p.n_tile);
-          }
-          const uint32_t first_row = p.split ? (kh % S ? 1u : 0u) : ((ch | kwo | kh) ? 1u : 0u);  // 0: the segment's first MMAs clear
-          const uint32_t kw_step = (p.dbg_noshift || PK2) ? 0u : 8u;
-          const int nrep = p.split && !(ch & 1) ? 2 : 1;
-#pragma unroll
-          for (int kw = 0; kw < (PK2 ? 1 : KW); ++kw)
-          for (int rep = 0; rep < nrep; ++rep) {
-            mbar_wait(b_full + st, b_phase);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            // descriptors: the high word is constant; the low word is (address >> 4) | LBO; a K step of 16 halfs
-            // advances it by 32 B >> 4 = 2, a tap column by 128 B >> 4 = 8
-            const uint32_t b_lo = (((b_base + st * b_stride) & 0x3FFFFu) >> 4) | (1u << 16);
-            if (elect_one()) {
-              // K step outer, row inner: consecutive MMAs go to different accumulators (an MMA chain on one
-              // accumulator is serialised by the accumulate dependency; see profiles/r1_notes.md)
-#pragma unroll
-              for (int k = 0; k < 4; ++k) {
-#pragma unroll
-                for (int m = 0; m < kMine; ++m)
-                  umma_f16(d_row[m], (static_cast<uint64_t>(kDescHi) << 32) | (a_row_lo[m] + kw_step * kw + 2 * k),
-                           (static_cast<uint64_t>(kDescHi) << 32) | (b_lo + 2 * k), idesc, first_row | static_cast<uint32_t>(kw | k | rep));
-              }
-              umma_commit(b_empty + st);  // weight stage is free once both issuers' MMAs retire
-            }
-            __syncwarp();
-            if (++st == kBStages) { st = 0; b_phase ^= 1; }
-          }
-          // halo row base_u + kh is only read by tap rows <= kh of this block.  ROLL: rows >= kRows are also the next block's, so
-          // only kh < kRows goes back to the producer now (the next block's rows stream in behind the MMAs); !ROLL: every
-          // chunk fetches its own rows, so row kh is dead after tap row kh
-          if ((!ROLL || kh < kRows) && elect_one()) umma_commit(a_empty + (base_u + kh) % kSlots);
-          __syncwarp();
-          if (seg_end) {
-            if (elect_one()) umma_commit(t_full + acc);
-            __syncwarp();
-            ++seg;
-          }
-        }
-        if (elect_one()) {
-          if (ROLL && K < kRows)  // fewer tap rows than output rows: release the rest of this block's own rows
-            for (int i = K; i < kRows; ++i) umma_commit(a_empty + (base_u + i) % kSlots);
-          if (!ROLL)  // the chunk's remaining halo rows (last read by tap row K - 1) are dead
-            for (int i = K; i < RK; ++i) umma_commit(a_empty + (base_u + i) % kSlots);
-        }
-        __syncwarp();
-      }
-    }
+    return;
   }
-  } else {
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 216;" ::: "memory");
-    // ===== epilogue: TMEM -> registers -> bias / BN / ReLU / dropout -> half (or float logits) -> global =====
-    // Measured (profiles/r1_notes.md): with four epilogue warps the stores + arithmetic of block j outlast the MMAs of
-    // block j+1 (30 % of the frame's conv time).  Eight warps -- warps w and w+4 share a TMEM lane quarter and split the
-    // rows of a block between them -- halve the epilogue's duration so it fits under the MMAs again.
-    const int q = warp & 3;           // TMEM lane quarter this warp may access
-    const int eset = (warp - 4) >> 2;  // 0: first half of the block's rows, 1: second half
-    const int x = PK2 ? ((q * 32 + lane) & 63) : x0 + q * 32 + lane;  // PK2: tile rows 64-127 are the second image
-    const int img_e = PK2 ? img + ((q * 32 + lane) >> 6) : img;
-    if (!ROLL && kRows == 2 && p.split) {
-      // split-operand fp32 mode: a block arrives as NC * ceil(K / seg_rows) accumulation segments; each epilogue warp owns one
-      // of the block's two rows, sums the segments in registers (round-to-nearest) and finishes the row after the last one
-      const int segs = NC * ((K + p.seg_rows - 1) / p.seg_rows);
-      const int y_row = eset;  // kRows == 2: set 0 takes row 0, set 1 row 1
-      int seg = 0;
-      for (int j = 0; j < npairs; ++j) {
-        float accr[128];
-#pragma unroll
-        for (int i = 0; i < 128; ++i) accr[i] = 0.f;
-        const int segs_per_chunk = (K + p.seg_rows - 1) / p.seg_rows;
-        for (int sg = 0; sg < segs; ++sg, ++seg) {
-          const int acc = seg & 1;
-          // accumulate steps of this segment: (tap rows) x KW x 4 K steps x (2 weight tiles for a hi chunk, 1 for a lo chunk).
-          // The tensor core truncates each add towards zero: mean loss 0.36 x 2^-23 of the running sum per step (half an ulp,
-          // ulp / |x| averaging 0.72 x 2^-23 over a binade), and a sum growing from 0 averages ~0.6 of its final value, so the
-          // segment comes back short by ~0.216 x 2^-23 x m of itself: scaled back up here (leaves the zero-mean part).
-          const int ch_s = sg / segs_per_chunk, kh0 = (sg % segs_per_chunk) * p.seg_rows;
-          const int m_steps = min(p.seg_rows, K - kh0) * KW * 4 * ((ch_s & 1) ? 1 : 2);
-          const float comp = 1.f + p.rz_comp * static_cast<float>(m_steps);
-          mbar_wait(t_full + acc, (seg >> 1) & 1);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t trow = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>((acc * kRows + y_row) * p.n_tile);
-          if (p.n_tile == 16) {
-            uint32_t v[32];
-            tmem_ld16(trow, v);
-#pragma unroll
-            for (int i = 0; i < 16; ++i) accr[i] = __fmaf_rn(__uint_as_float(v[i]), comp, accr[i]);
-          } else {
-#pragma unroll
-            for (int cc = 0; cc < 128; cc += 32)
-              if (cc < p.n_tile) {
-                uint32_t v[32];
-                tmem_ld32(trow + cc, v);
-#pragma unroll
-                for (int i = 0; i < 32; ++i) accr[cc + i] = __fmaf_rn(__uint_as_float(v[i]), comp, accr[cc + i]);
-              }
-          }
-          asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-          __syncwarp();
-          if (lane == 0) mbar_arrive(t_empty + acc);
-        }
-        // finish the row: x 2^-s, bias, BN affine, ReLU in fp32 (as the reference), float NHWC store (4-lane transposed)
-        const int y = y_base + j * kRows + y_row;
-        const bool row_ok = y < p.H;
-        const int cl = lane & 3, xg = x - cl;
-        if (p.n_tile == 16) {
-          float4 e[4];
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            float t = __fadd_rn(__fmul_rn(accr[i], p.acc_scale), cst.bias[i]);
-            if (p.has_bn) t = __fadd_rn(__fmul_rn(t, cst.bn_scale[i]), cst.bn_shift[i]);
-            if (p.relu) t = t > 0.f ? t : __fmul_rn(p.slope, t);
-            reinterpret_cast<float*>(&e[i >> 2])[i & 3] = t;
-          }
-          quad_transpose(e, lane);
-#pragma unroll
-          for (int jj = 0; jj < 4; ++jj)
-            if (row_ok && xg + jj < p.W)
-              *reinterpret_cast<float4*>(reinterpret_cast<float*>(p.out) + ((static_cast<size_t>(img) * p.H + y) * p.W + xg + jj) * 16 + 4 * cl) = e[jj];
-        } else {
-#pragma unroll
-          for (int cc = 0; cc < 128; cc += 32)
-            if (cc < p.n_tile) {
-              const int c0 = n0 + cc;
-              float4 ea[4], eb[4];
-#pragma unroll
-              for (int i = 0; i < 32; ++i) {
-                float t = __fadd_rn(__fmul_rn(accr[cc + i], p.acc_scale), cst.bias[c0 + i]);
-                if (p.has_bn) t = __fadd_rn(__fmul_rn(t, cst.bn_scale[c0 + i]), cst.bn_shift[c0 + i]);
-                if (p.relu) t = t > 0.f ? t : __fmul_rn(p.slope, t);
-                if (i < 16) reinterpret_cast<float*>(&ea[i >> 2])[i & 3] = t;
-                else reinterpret_cast<float*>(&eb[(i - 16) >> 2])[i & 3] = t;
-              }
-              quad_transpose(ea, lane);  // ea[jj] = channels [c0 + 4 cl, +4) of pixel xg + jj; eb the same 16 channels further
-              quad_transpose(eb, lane);
-#pragma unroll
-              for (int jj = 0; jj < 4; ++jj)
-                if (row_ok && xg + jj < p.W) {
-                  float* o = reinterpret_cast<float*>(p.out) + ((static_cast<size_t>(img) * p.H + y) * p.W + xg + jj) * p.cout_total + c0 + 4 * cl;
-                  *reinterpret_cast<float4*>(o) = ea[jj];
-                  *reinterpret_cast<float4*>(o + 16) = eb[jj];
-                }
-            }
-        }
-      }
-    } else
-    for (int j = 0; j < npairs; ++j) {
-      const int acc = j & 1;
-      mbar_wait(t_full + acc, (j >> 1) & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      constexpr int kPer = kRows / 2;  // rows per epilogue set
-      if (p.pool_out) {
-        if (kRows == 4 || eset == 0) {  // a row pair per set (kRows == 2: one pair, taken by set 0)
-          const int r = kRows == 4 ? 2 * eset : 0;
-          const uint32_t trow = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>((acc * kRows + r) * p.n_tile);
-          epilogue_pool_rows(p, cst, trow, trow + p.n_tile, img_e, y_base + j * kRows + r, x, n0, lane);
-        }
-      } else {
-#pragma unroll
-        for (int rr = 0; rr < kPer; ++rr) {
-          const int r = eset * kPer + rr;
-          const int y = y_base + j * kRows + r;
-          const uint32_t trow = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>((acc * kRows + r) * p.n_tile);
-          epilogue_row(p, cst, trow, img_e, y, x, n0, lane);
-        }
-      }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(t_empty + acc);
-    }
-  }
-  __syncthreads();
-  if (warp == 2) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(tmem_cols) : "memory");
-  }
-}
 
-// ---------------------------------------------------------------------------------------------------------------
-// Paired-tap variant (64 -> 64 channels, 4-row blocks).  With N = 64 every MMA re-reads its 16 KB A tile from shared
-// memory for 8 KB of weights: 192 B/clk of operand traffic against the SM's 128 B/clk, i.e. <= 67 % of the tensor
-// rate.  But output row r at tap row kh and output row r-1 at tap row kh+1 read the SAME input row, so with the four
-// accumulators laid out in decreasing row order one N = 128 MMA whose B tile stacks W(kh, kw) over W(kh+1, kw)
-// updates acc(r) | acc(r-1) from a single A read.  Per (tap-row pair, kw) that is 5 MMA groups (N = 64, 128, 128,
-// 128, 64) instead of 8: A traffic 80 KB instead of 128 KB per 1024 tensor cycles (141 B/clk), and 20 instead of 32
-// instructions.  Weights come as [kw][kh][cout][cin] so one TMA box of 128 rows lands both taps of a pair.
-// TRIPLE (K = 7): the last three tap rows (4, 5, 6) are stacked as well -- input row i of that group feeds acc(r) for every
-// r with 0 <= i - r <= 2, one MMA of N = 64 / 128 / 192 / 192 / 128 / 64 per (input row, kw): 1664 tensor cycles instead of
-// 1152 + 768 for a pair plus a single.  The weight stages grow to 24 KB (three 64-row boxes); the halo ring shrinks from
-// K + 3 to 9 slots to pay for it (a block keeps at most 6 rows live, the rest is prefetch depth).
-// NW = accumulator width = output channels per tap tile: 64 for the 64 -> 64 layers; 16 for conv_decode1 composed with the 1x1
-// classifier (float logits straight from the accumulators; needs TRIPLE: its weight boxes are one tap each).
-template <int K, bool TRIPLE = false, int NW = 64>
-__global__ void __launch_bounds__(kTcThreads, 1)
-k_conv_tc_pair(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const __grid_constant__ TcParams p,
-               const __grid_constant__ TcConsts cst) {
-  asm volatile("griddepcontrol.launch_dependents;");
-  static_assert(!TRIPLE || K == 7, "the triple group is taps 4..6 of a 7-row filter");
-  static_assert(NW == 64 || (NW == 16 && TRIPLE), "accumulator width");
-  constexpr int kTapBytes = NW * 128;            // one tap's weight tile: NW rows of 64 half
-  constexpr uint32_t kTapLo = kTapBytes >> 4;    // the same in descriptor units
-  constexpr int kRows = 4, RK = kRows + K - 1, kSlots = TRIPLE ? 9 : RK, kPad = (K - 1) / 2, NP = TRIPLE ? 3 : (K + 1) / 2;
-  constexpr int kBBytes = (TRIPLE ? 3 : 2) * kTapBytes;  // stacked weight tiles: stage stride
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-  uint8_t* a_slots = smem;
-  uint8_t* b_stages = smem + kSlots * kSlotBytes;
-  const int kBStages = p.b_stages;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(b_stages + kBStages * kBBytes);
-  uint64_t* a_full = bars;
-  uint64_t* a_empty = a_full + kSlots;
-  uint64_t* b_full = a_empty + kSlots;
-  uint64_t* b_empty = b_full + kBStages;
-  uint64_t* t_full = b_empty + kBStages;
-  uint64_t* t_empty = t_full + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(t_empty + 2);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int strip = blockIdx.x % p.strips, rowblk = blockIdx.x / p.strips;
-  const int img = blockIdx.z;
-  const int x0 = strip * 128;
-  const int total_pairs = (p.H + kRows - 1) / kRows;
-  const int pair0 = rowblk * p.pairs_per_cta;
-  const int npairs = min(p.pairs_per_cta, total_pairs - pair0);
-  const int y_base = pair0 * kRows;
-  const int n_units = npairs * kRows + K - 1;
-  constexpr uint32_t tmem_cols = 2 * kRows * NW;  // 2 stages x 4 rows x NW columns (512 or 128)
-
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < kSlots; ++i) { mbar_init(a_full + i, 1); mbar_init(a_empty + i, 1); }
-    for (int i = 0; i < kBStages; ++i) { mbar_init(b_full + i, 1); mbar_init(b_empty + i, 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(t_full + i, 1); mbar_init(t_empty + i, kEpiWarps); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(tmem_cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
-  // everything above touched only this CTA's shared / tensor memory; the producing kernel's results are needed from here on
-  asm volatile("griddepcontrol.wait;" ::: "memory");
-
-  if (warp < 4) {
-  asm volatile("setmaxnreg.dec.sync.aligned.u32 56;" ::: "memory");
-  if (warp == 0) {
-    if (lane == 0) {
-      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_a)) : "memory");
-      for (int u = 0; u < n_units; ++u) {
-        const int slot = u % kSlots;
-        mbar_wait(a_empty + slot, ((static_cast<uint32_t>(u / kSlots)) & 1) ^ 1);
-        mbar_expect_tx(a_full + slot, static_cast<uint32_t>((128 + K - 1) * 128));
-        tma_load_4d(a_slots + slot * kSlotBytes, &map_a, a_full + slot, 0, x0 - kPad, y_base - kPad + u, img);
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+  // ===== consumers: warpgroup g = wg - 1 owns tile rows (pixels) [64 g, 64 g + 64) =====
+  const int g = wg - 1;
+  const int m0 = 16 * (warp & 3) + (lane >> 2);    // this thread's accumulator rows: m0 and m0 + 8
+  const int img_c = PK2 ? img + g : img;
+  const int x_m0 = (PK2 ? 0 : x0 + 64 * g) + m0;
+  // PK2: the second image's 64-pixel box sits 64 rows into the slot; otherwise pixel 64 g of the halo row is 64 g rows in
+  const uint32_t a_base = smem_u32(a_slots) + static_cast<uint32_t>(g * 64 * 128), b_base = smem_u32(b_stages);
+  const bool releaser = lane == 0;
+  float acc[kRows][F];
+  float accr[SPLIT ? kRows : 1][SPLIT ? F : 1];
+  int st = 0;
+  uint32_t b_phase = 0;
+  int waited = 0;  // halo units whose TMA has been observed
+  const int S = p.split ? p.seg_rows : K;
+  for (int j = 0; j < npairs; ++j) {
+#pragma unroll
+    for (int r = 0; r < kRows; ++r)
+#pragma unroll
+      for (int i = 0; i < F; ++i) {
+        acc[r][i] = 0.f;
+        if (SPLIT) accr[r][i] = 0.f;
       }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_b)) : "memory");
-      const int w_replica = static_cast<int>((blockIdx.x + blockIdx.z) % static_cast<unsigned>(p.w_rep));
-      int st = 0;
-      uint32_t ph = 0;
-      for (int j = 0; j < npairs; ++j)
-        for (int pp = 0; pp < NP; ++pp)
-          for (int kw = 0; kw < K; ++kw) {
-            mbar_wait(b_empty + st, ph ^ 1);
-            if (TRIPLE) {  // 64-row boxes: two for a pair, three for the triple group
-              const int nt = pp == 2 ? 3 : 2;
-              mbar_expect_tx(b_full + st, static_cast<uint32_t>(nt * kTapBytes));
-              for (int t = 0; t < nt; ++t)
-                tma_load_3d(b_stages + st * kBBytes + t * kTapBytes, &map_b, b_full + st, 0, (kw * K + 2 * pp + t) * NW, w_replica);
-            } else {
-              mbar_expect_tx(b_full + st, static_cast<uint32_t>(kBBytes));
-              // rows (kw*K + 2pp)*64 .. +127 of the [kw][kh][cout] x cin matrix; the odd last tap row drags in 64 rows it
-              // never uses (the next kw's first tap, or zero fill past the end)
-              tma_load_3d(b_stages + st * kBBytes, &map_b, b_full + st, 0, (kw * K + 2 * pp) * 64, w_replica);
-            }
-            if (++st == kBStages) { st = 0; ph ^= 1; }
-          }
-    }
-  } else if (warp == 2) {
-    // ===== MMA issuer (one warp: with N = 128 an MMA lasts 64 tensor cycles and costs 1-2 issue instructions) =====
-    // one, two or three tap tiles wide (the names keep the NW = 64 widths)
-    const uint32_t idesc64 = (1u << 4) | (static_cast<uint32_t>(NW >> 3) << 17) | (8u << 24);
-    const uint32_t idesc128 = (1u << 4) | (static_cast<uint32_t>(2 * NW >> 3) << 17) | (8u << 24);
-    const uint32_t idesc192 = (1u << 4) | (static_cast<uint32_t>(3 * NW >> 3) << 17) | (8u << 24);
-    const uint32_t a_base = smem_u32(a_slots), b_base = smem_u32(b_stages);
-    int st = 0;
-    uint32_t b_phase = 0;
-    int waited = 0;
-    for (int j = 0; j < npairs; ++j) {
-      const int acc = j & 1;
-      mbar_wait(t_empty + acc, ((j >> 1) & 1) ^ 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const int base_u = j * kRows;
-      const uint32_t d0 = tmem_base + static_cast<uint32_t>(acc * kRows * NW);  // column of acc(row 3); acc(r) sits at d0 + (3 - r) * NW
-      for (int pp = 0; pp < NP; ++pp) {
-        const int kh0 = 2 * pp;
-        const bool triple = TRIPLE && pp == 2;
-        const bool paired = kh0 + 1 < K;
-        const int last_unit = base_u + kh0 + (triple ? 2 : paired ? 1 : 0) + kRows - 1;
-        while (waited <= last_unit && waited < n_units) {
+    for (int ch = 0; ch < NC; ++ch)
+    for (int kwo = 0; kwo < (PK2 ? KW : 1); ++kwo) {  // PK2: the kw shift is done by TMA, one set of halo rows per tap column
+      const int base_u = ROLL ? j * kRows : PK2 ? ((j * NC + ch) * KW + kwo) * RK : (j * NC + ch) * RK;
+      for (int kh = 0; kh < K; ++kh) {
+        while (waited <= base_u + kh + kRows - 1 && waited < n_units) {
           mbar_wait(a_full + waited % kSlots, (waited / kSlots) & 1);
           ++waited;
         }
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        uint32_t a_lo[kRows + 2];
+        uint32_t a_row[kRows];
 #pragma unroll
-        for (int i = 0; i <= kRows + 1; ++i)
-          a_lo[i] = (((a_base + ((base_u + kh0 + i) % kSlots) * kSlotBytes) & 0x3FFFFu) >> 4) | (1u << 16);
+        for (int r = 0; r < kRows; ++r) a_row[r] = a_base + ((base_u + r + kh) % kSlots) * kSlotBytes;
+        const int nrep = p.split && !(ch & 1) ? 2 : 1;
+        int prev_st = -1;
 #pragma unroll
-        for (int kw = 0; kw < K; ++kw) {
+        for (int kw = 0; kw < (PK2 ? 1 : KW); ++kw)
+        for (int rep = 0; rep < nrep; ++rep) {
           mbar_wait(b_full + st, b_phase);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t b_lo = (((b_base + st * kBBytes) & 0x3FFFFu) >> 4) | (1u << 16);
-          if (elect_one()) {
-            const uint64_t hi = static_cast<uint64_t>(kDescHi) << 32;
-            if (pp == 0 && kw == 0) {
-              // first tap pair of the block: plain N = 64 MMAs so that each accumulator's first MMA can clear it
+          const uint32_t b_addr = b_base + st * b_stride;
+          const uint32_t a_shift = PK2 ? 0u : static_cast<uint32_t>(kw * 128);
+          wgmma_fence();
+          // K step outer, row inner: consecutive MMAs go to different accumulators
 #pragma unroll
-              for (int t = 0; t < 2; ++t)
+          for (int k = 0; k < 4; ++k)
 #pragma unroll
-                for (int r = 0; r < kRows; ++r)
-#pragma unroll
-                  for (int k = 0; k < 4; ++k)
-                    umma_f16(d0 + (3 - r) * NW, hi | (a_lo[r + t] + 2 * k), hi | (b_lo + kTapLo * t + 2 * k), idesc64,
-                             static_cast<uint32_t>(t | k));
-            } else if (triple) {
-              // input row i of the group (block row 4 + i) x taps 4..6: acc(r) for r = i, i-1, i-2 where they exist.
-              // Accumulators sit in decreasing row order, weights in increasing tap order, so each MMA is one contiguous
-              // D range and one contiguous B range: (first acc column, first B row / 64, N)
-#pragma unroll
-              for (int k = 0; k < 4; ++k) {
-                const uint32_t ak = 8 * kw + 2 * k;
-                umma_f16(d0 + 3 * NW, hi | (a_lo[0] + ak), hi | (b_lo + 2 * k), idesc64, 1u);          // row 4: acc0 <- W4
-                umma_f16(d0 + 2 * NW, hi | (a_lo[1] + ak), hi | (b_lo + 2 * k), idesc128, 1u);         // row 5: acc1|acc0 <- W4|W5
-                umma_f16(d0 + 1 * NW, hi | (a_lo[2] + ak), hi | (b_lo + 2 * k), idesc192, 1u);         // row 6: acc2|acc1|acc0 <- W4|W5|W6
-                umma_f16(d0, hi | (a_lo[3] + ak), hi | (b_lo + 2 * k), idesc192, 1u);                  // row 7: acc3|acc2|acc1 <- W4|W5|W6
-                umma_f16(d0, hi | (a_lo[4] + ak), hi | (b_lo + kTapLo + 2 * k), idesc128, 1u);         // row 8: acc3|acc2 <- W5|W6
-                umma_f16(d0, hi | (a_lo[5] + ak), hi | (b_lo + 2 * kTapLo + 2 * k), idesc64, 1u);      // row 9: acc3 <- W6
-              }
-            } else if (paired) {
-#pragma unroll
-              for (int k = 0; k < 4; ++k) umma_f16(d0 + 3 * NW, hi | (a_lo[0] + 8 * kw + 2 * k), hi | (b_lo + 2 * k), idesc64, 1u);
-#pragma unroll
-              for (int i = 1; i < kRows; ++i)
-#pragma unroll
-                for (int k = 0; k < 4; ++k)
-                  umma_f16(d0 + (3 - i) * NW, hi | (a_lo[i] + 8 * kw + 2 * k), hi | (b_lo + 2 * k), idesc128, 1u);
-#pragma unroll
-              for (int k = 0; k < 4; ++k) umma_f16(d0, hi | (a_lo[kRows] + 8 * kw + 2 * k), hi | (b_lo + kTapLo + 2 * k), idesc64, 1u);
-            } else {
-#pragma unroll
-              for (int r = 0; r < kRows; ++r)
-#pragma unroll
-                for (int k = 0; k < 4; ++k)
-                  umma_f16(d0 + (3 - r) * NW, hi | (a_lo[r] + 8 * kw + 2 * k), hi | (b_lo + 2 * k), idesc64, 1u);
-            }
-            umma_commit(b_empty + st);
-          }
-          __syncwarp();
+            for (int r = 0; r < kRows; ++r) wgmma(acc[r], make_desc(a_row[r] + a_shift + 32 * k), make_desc(b_addr + 32 * k));
+          wgmma_commit();
+          // keep one group in flight: the previous one has retired, so its weight stage goes back to the producer
+          wgmma_wait<1>();
+          if (prev_st >= 0 && releaser) mbar_arrive(b_empty + prev_st);
+          prev_st = st;
           if (++st == kBStages) { st = 0; b_phase ^= 1; }
         }
-        // halo rows base_u + kh0 (and + kh0 + 1) are read by no later tap row of this block and by no later block
-        if (elect_one()) {
-          if (kh0 < kRows) umma_commit(a_empty + (base_u + kh0) % kSlots);
-          if (paired && kh0 + 1 < kRows) umma_commit(a_empty + (base_u + kh0 + 1) % kSlots);
+        wgmma_wait<0>();
+        fence_acc(acc);
+        if (releaser) {
+          mbar_arrive(b_empty + prev_st);
+          // halo row base_u + kh is only read by tap rows <= kh of this block.  ROLL: rows >= kRows are also the next block's, so
+          // only kh < kRows goes back to the producer now; !ROLL: every chunk fetches its own rows, so row kh is dead after tap row kh
+          if (!ROLL || kh < kRows) mbar_arrive(a_empty + (base_u + kh) % kSlots);
         }
-        __syncwarp();
-      }
-      if (elect_one()) {
-        for (int i = K; i < kRows; ++i) umma_commit(a_empty + (base_u + i) % kSlots);  // K < 4: rows no tap row released
-        umma_commit(t_full + acc);
-      }
-      __syncwarp();
-    }
-  }
-  } else {
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 216;" ::: "memory");
-    const int q = warp & 3;
-    const int eset = (warp - 4) >> 2;  // two warps per TMEM lane quarter: rows {0,1} and {2,3}
-    const int x = x0 + q * 32 + lane;
-    for (int j = 0; j < npairs; ++j) {
-      const int acc = j & 1;
-      mbar_wait(t_full + acc, (j >> 1) & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      if (p.pool_out) {  // accumulators sit in decreasing row order: row r+1 is 64 columns below row r
-        const int r = 2 * eset;
-        const uint32_t trow = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>((acc * kRows + (3 - r)) * NW);
-        epilogue_pool_rows(p, cst, trow, trow - NW, img, y_base + j * kRows + r, x, 0, lane);
-      } else {
+        if (SPLIT && (kh % S == S - 1 || kh == K - 1)) {
+          // segment done: accumulate steps (tap rows) x KW x 4 K steps x (2 weight tiles for a hi chunk, 1 for a lo chunk).
+          // The tensor core truncates each add towards zero: mean loss 0.36 x 2^-23 of the running sum per step (half an ulp,
+          // ulp / |x| averaging 0.72 x 2^-23 over a binade), and a sum growing from 0 averages ~0.6 of its final value, so the
+          // segment comes back short by ~0.216 x 2^-23 x m of itself: scaled back up here (leaves the zero-mean part).
+          const int kh0 = (kh / S) * S;
+          const int m_steps = min(S, K - kh0) * KW * 4 * ((ch & 1) ? 1 : 2);
+          const float comp = 1.f + p.rz_comp * static_cast<float>(m_steps);
 #pragma unroll
-        for (int rr = 0; rr < 2; ++rr) {
-          const int r = 2 * eset + rr;
-          const int y = y_base + j * kRows + r;
-          const uint32_t trow = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>((acc * kRows + (3 - r)) * NW);
-          epilogue_row(p, cst, trow, img, y, x, 0, lane);
-        }
-      }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(t_empty + acc);
-    }
-  }
-  __syncthreads();
-  if (warp == 2) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(tmem_cols) : "memory");
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// Full-stack variant for the composed 64 -> 16 layer (Basic: conv_decode1 x the 1x1 classifier as ONE 7x7 convolution with
-// 16 output columns, see conv_tc_set_composed_classifier).  With N = 16 per tap an MMA is bound by its 4 KB A read, so ALL
-// seven tap rows are stacked along N: input row i of a block feeds acc(r) for every output row r with 0 <= i - r <= 6, one
-// MMA of N = 16 x (number of such rows) <= 112 per (input row, kw, K step).  Accumulators sit in decreasing row order and
-// the weights in increasing tap order, so each MMA covers one contiguous TMEM column range and one contiguous weight range.
-//  * R = 16 output rows per block, 2 accumulator stages x 16 rows x 16 columns = all 512 TMEM columns.
-//  * The composed weights (49 taps x 16 x 64 half = 98 KB) stay resident in shared memory: no weight ring.
-//  * Every input row is consumed by 28 consecutive MMAs and then dead: the halo ring is pure prefetch depth (7 slots).
-//  * Model: per (kw, K step) a block issues MMAs of N = 16, 32, .., 96, 112 x 10, 96, .., 16 for its 22 input rows =
-//    1152 cycles (N = 112: 56 tensor cycles against 60 of shared-memory operand reads) -> 32 K cycles per 16 x 128 px.
-// K = 3: the same for a 3x3 layer with <= 16 float outputs (Standard's conv1_1_D): N = 16, 32, 48 x 14, 32, 16 per (kw, K step).
-constexpr int kStackRows = 16, kStackSlots = 7;
-template <int K>
-__global__ void __launch_bounds__(kTcThreads, 1)
-k_conv_tc_stack16(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const __grid_constant__ TcParams p,
-                  const __grid_constant__ TcConsts cst) {
-  asm volatile("griddepcontrol.launch_dependents;");
-  constexpr int R = kStackRows, kSlots = kStackSlots, kPad = (K - 1) / 2, NW = 16;
-  constexpr int kTapBytes = NW * 128, kKwBytes = K * kTapBytes, kWBytes = K * kKwBytes;  // 2 KB, 14 KB, 98 KB
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-  uint8_t* w_smem = smem;                         // [kw][kh][16][64] half, K-major SWIZZLE_128B rows
-  uint8_t* a_slots = smem + ((kWBytes + 1023) & ~1023);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(a_slots + kSlots * kSlotBytes);
-  uint64_t* a_full = bars;
-  uint64_t* a_empty = a_full + kSlots;
-  uint64_t* w_full = a_empty + kSlots;
-  uint64_t* t_full = w_full + 1;
-  uint64_t* t_empty = t_full + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(t_empty + 2);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int strip = blockIdx.x % p.strips, rowblk = blockIdx.x / p.strips;
-  const int img = blockIdx.z;
-  const int x0 = strip * 128;
-  const int total_blocks = (p.H + R - 1) / R;
-  const int blk0 = rowblk * p.pairs_per_cta;
-  const int nblk = min(p.pairs_per_cta, total_blocks - blk0);
-  constexpr uint32_t tmem_cols = 2 * R * NW;  // 512
-
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < kSlots; ++i) { mbar_init(a_full + i, 1); mbar_init(a_empty + i, 1); }
-    mbar_init(w_full, 1);
-    for (int i = 0; i < 2; ++i) { mbar_init(t_full + i, 1); mbar_init(t_empty + i, kEpiWarps); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(tmem_cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
-  asm volatile("griddepcontrol.wait;" ::: "memory");
-
-  if (warp < 4) {
-  asm volatile("setmaxnreg.dec.sync.aligned.u32 56;" ::: "memory");
-  if (warp == 0) {
-    // ===== halo-row producer: R + 6 input rows per block, in order, through the ring =====
-    if (lane == 0) {
-      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_a)) : "memory");
-      uint32_t u = 0;
-      for (int j = 0; j < nblk; ++j) {
-        const int y0 = (blk0 + j) * R;
-        for (int i = 0; i < R + K - 1; ++i, ++u) {
-          const int slot = u % kSlots;
-          mbar_wait(a_empty + slot, ((u / kSlots) & 1) ^ 1);
-          if (p.dbg_noload && u >= static_cast<uint32_t>(kSlots)) { mbar_arrive(a_full + slot); continue; }
-          mbar_expect_tx(a_full + slot, static_cast<uint32_t>((128 + K - 1) * 128));
-          tma_load_4d(a_slots + slot * kSlotBytes, &map_a, a_full + slot, 0, x0 - kPad, y0 - kPad + i, img);
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===== weights: loaded once, resident =====
-    if (lane == 0) {
-      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_b)) : "memory");
-      mbar_expect_tx(w_full, static_cast<uint32_t>(kWBytes));
-      for (int kw = 0; kw < K; ++kw)  // one box {64 cin, 7 taps x 16 rows} per tap column
-        tma_load_3d(w_smem + kw * kKwBytes, &map_b, w_full, 0, kw * K * NW, 0);
-    }
-  } else if (warp == 2) {
-    // ===== MMA issuer =====
-    const uint32_t a_base = smem_u32(a_slots), w_base = smem_u32(w_smem);
-    const uint64_t hi = static_cast<uint64_t>(kDescHi) << 32;
-    mbar_wait(w_full, 0);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    uint32_t u = 0;
-    for (int j = 0; j < nblk; ++j) {
-      const int acc = j & 1;
-      mbar_wait(t_empty + acc, ((j >> 1) & 1) ^ 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t d0 = tmem_base + static_cast<uint32_t>(acc * R * NW);  // acc(r) sits at d0 + (R - 1 - r) * NW
-      for (int i = 0; i < R + K - 1; ++i, ++u) {
-        const int slot = u % kSlots;
-        mbar_wait(a_full + slot, (u / kSlots) & 1);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const int r_hi = min(R - 1, i), r_lo = max(0, i - (K - 1));
-        const int cnt = r_hi - r_lo + 1;             // output rows this input row feeds
-        const int kh_lo = i - r_hi;                  // tap row meeting acc(r_hi); acc(r_hi - t) meets tap kh_lo + t
-        const uint32_t d = d0 + static_cast<uint32_t>((R - 1 - r_hi) * NW);
-        const uint32_t a_lo = (((a_base + slot * kSlotBytes) & 0x3FFFFu) >> 4) | (1u << 16);
-        const uint32_t b_lo = (((w_base + kh_lo * kTapBytes) & 0x3FFFFu) >> 4) | (1u << 16);
-        const uint32_t idesc = (1u << 4) | (static_cast<uint32_t>((cnt * NW) >> 3) << 17) | (8u << 24);
-        if (elect_one()) {
-          if (i < R) {
-            // acc(i) meets its first tap here (kh = 0, kw = 0, K step 0): that MMA must clear it, the rest of the stack accumulates
-            const uint32_t idesc1 = (1u << 4) | (static_cast<uint32_t>(NW >> 3) << 17) | (8u << 24);
-            umma_f16(d, hi | a_lo, hi | b_lo, idesc1, 0u);
-            if (cnt > 1) {
-              const uint32_t idesc_r = (1u << 4) | (static_cast<uint32_t>(((cnt - 1) * NW) >> 3) << 17) | (8u << 24);
-              umma_f16(d + NW, hi | a_lo, hi | (b_lo + (kTapBytes >> 4)), idesc_r, 1u);
+          for (int r = 0; r < kRows; ++r)
+#pragma unroll
+            for (int i = 0; i < F; ++i) {
+              accr[r][i] = __fmaf_rn(acc[r][i], comp, accr[r][i]);
+              acc[r][i] = 0.f;
             }
-#pragma unroll
-            for (int k = 1; k < 4; ++k) umma_f16(d, hi | (a_lo + 2 * k), hi | (b_lo + 2 * k), idesc, 1u);
-          } else {
-#pragma unroll
-            for (int k = 0; k < 4; ++k) umma_f16(d, hi | (a_lo + 2 * k), hi | (b_lo + 2 * k), idesc, 1u);
-          }
-#pragma unroll
-          for (int kw = 1; kw < K; ++kw)
-#pragma unroll
-            for (int k = 0; k < 4; ++k)
-              umma_f16(d, hi | (a_lo + 8 * kw + 2 * k), hi | (b_lo + kw * (kKwBytes >> 4) + 2 * k), idesc, 1u);
-          umma_commit(a_empty + slot);   // the row is dead once these MMAs retire
-          if (i == R + K - 2) umma_commit(t_full + acc);
         }
-        __syncwarp();
+      }
+      if (releaser) {
+        if (ROLL && K < kRows)  // fewer tap rows than output rows: release the rest of this block's own rows
+          for (int i = K; i < kRows; ++i) mbar_arrive(a_empty + (base_u + i) % kSlots);
+        if (!ROLL)  // the chunk's remaining halo rows (last read by tap row K - 1) are dead
+          for (int i = K; i < RK; ++i) mbar_arrive(a_empty + (base_u + i) % kSlots);
       }
     }
-  }
-  } else {
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 216;" ::: "memory");
-    // ===== epilogue: 16 float logits per pixel straight from the accumulators (+ composed bias), 4-lane transposed stores =====
-    const int q = warp & 3;
-    const int eset = (warp - 4) >> 2;  // two warps per TMEM lane quarter: rows [0, 8) and [8, 16) of the block
-    const int x = x0 + q * 32 + lane;
-    for (int j = 0; j < nblk; ++j) {
-      const int acc = j & 1;
-      mbar_wait(t_full + acc, (j >> 1) & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll 2
-      for (int rr = 0; rr < R / 2; ++rr) {
-        const int r = eset * (R / 2) + rr;
-        const int y = (blk0 + j) * R + r;
-        const uint32_t trow = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>(acc * R * NW + (R - 1 - r) * NW);
-        epilogue_row(p, cst, trow, img, y, x, 0, lane);
-      }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(t_empty + acc);
+    const int y0 = y_base + j * kRows;
+    if (SPLIT) {
+#pragma unroll
+      for (int r = 0; r < kRows; ++r)
+#pragma unroll
+        for (int i = 0; i < F; ++i) acc[r][i] = __fmul_rn(accr[r][i], p.acc_scale);  // x 2^-s (exact)
     }
-  }
-  __syncthreads();
-  if (warp == 2) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(tmem_cols) : "memory");
+    epilogue_block<N>(p, cst, acc, img_c, y0, x_m0, n0, lane);
   }
 }
 
@@ -1191,15 +579,11 @@ struct ConvTcPlan {
   TcConsts cst;
   dim3 grid;
   size_t smem;
-  int k, rows;
+  int k;
   int kw;             // filter width the kernel walks (== k, or 1 for a window-folded layer)
   bool roll;
-  bool pair = false;  // paired-tap kernel (64 -> 64 channels, 4-row blocks)
-  bool triple = false;  // ... with taps 4..6 stacked three-high (K = 7)
-  bool nw16 = false;    // ... with 16-wide accumulators: conv composed with the 1x1 classifier
-  bool pk2 = false;     // two images per 128-pixel M tile (layers at most 64 pixels wide, chunked 3x3 kernel)
-  bool stack16 = false; // composed 64 -> 16 layer on the full-stack kernel (all seven tap rows stacked along N, resident weights)
-  DevBuf w_replicas;  // private replicated copy of the weights (w_rep > 1)
+  bool pk2 = false;   // two images per 128-pixel M tile (layers at most 64 pixels wide, chunked 3x3 kernel)
+  DevBuf w_own;       // weights the plan owns (the composed classifier)
 };
 
 namespace {
@@ -1207,14 +591,13 @@ namespace {
 void conv_tc_dispatch(const ConvTcPlan& plan, cudaStream_t s, bool configure) {
   auto go = [&](auto kern) {
     // the limit is per kernel function, not per launch: always raise it to the full 227 KB so that plans of different
-    // sizes that share an instantiation (e.g. the 16-wide logits tile and a 64-wide layer) cannot lower it for each other
+    // sizes that share an instantiation cannot lower it for each other
     if (configure) SIVO_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     else {
       // Programmatic dependent launch: the CTAs of this launch may start while the previous kernel of the stream is still
-      // draining (on SMs it has already left, or never used) and run their prologue -- barrier init, TMEM allocation,
-      // descriptor prefetch -- up to griddepcontrol.wait, which returns once that kernel has completed and flushed.
-      // Opt-in (SIVO_B200_PDL=1): measured on B200 it shaves ~20 us off a lone SegNet frame (1.22 -> 1.20 ms) but the early
-      // CTAs sit on SMs the concurrent extractor kernels could have used, so the three-call frame gets no faster.
+      // draining (on SMs it has already left, or never used) and run their prologue -- barrier init, descriptor
+      // prefetch -- up to griddepcontrol.wait, which returns once that kernel has completed and flushed.  Opt-in
+      // (SIVO_B200_PDL=1): the early CTAs sit on SMs the concurrent extractor kernels could have used.
       static const bool pdl = [] { const char* e = std::getenv("SIVO_B200_PDL"); return e && e[0] == '1'; }();
       cudaLaunchConfig_t cfg = {};
       cfg.gridDim = plan.grid;
@@ -1229,44 +612,47 @@ void conv_tc_dispatch(const ConvTcPlan& plan, cudaStream_t s, bool configure) {
       SIVO_CUDA(cudaLaunchKernelEx(&cfg, kern, plan.map_a, plan.map_b, plan.p, plan.cst));
     }
   };
+  // per (K, ROLL, KW, PK2): the three tile widths
+  auto by_n = [&](auto k16, auto k64, auto k128) {
+    if (plan.p.n_tile == 16) go(k16); else if (plan.p.n_tile == 64) go(k64); else go(k128);
+  };
   const int K = plan.k;
-  if (plan.stack16) { if (plan.k == 7) go(k_conv_tc_stack16<7>); else go(k_conv_tc_stack16<3>); }
-  else if (plan.pair && plan.nw16) go(k_conv_tc_pair<7, true, 16>);
-  else if (plan.pair) { if (K == 7 && plan.triple) go(k_conv_tc_pair<7, true>); else if (K == 7) go(k_conv_tc_pair<7>); else go(k_conv_tc_pair<3>); }
-  else if (plan.kw == 1 && K > 1) {  // window-folded first layer (K x 1)
-    if (!plan.roll) fail(SIVO_EINVAL, "window-folded convolution needs the rolling kernel");
-    if (plan.rows == 4) { if (K == 7) go(k_conv_tc<7, true, 4, 1>); else go(k_conv_tc<3, true, 4, 1>); }
-    else { if (K == 7) go(k_conv_tc<7, true, 2, 1>); else go(k_conv_tc<3, true, 2, 1>); }
+  if (plan.p.split) {
+    if (plan.p.n_tile == 16) { if (K == 7) go(k_conv_tc<7, false, 7, false, 16, true>); else if (K == 3) go(k_conv_tc<3, false, 3, false, 16, true>); else go(k_conv_tc<1, false, 1, false, 16, true>); }
+    else { if (K == 7) go(k_conv_tc<7, false, 7, false, 64, true>); else if (K == 3) go(k_conv_tc<3, false, 3, false, 64, true>); else go(k_conv_tc<1, false, 1, false, 64, true>); }
+  } else if (plan.kw == 1 && K > 1) {  // window-folded first layer (K x 1), 64-wide tiles
+    if (K == 7) go(k_conv_tc<7, true, 1, false, 64, false>); else go(k_conv_tc<3, true, 1, false, 64, false>);
+  } else if (plan.pk2) {
+    if (plan.p.n_tile == 64) go(k_conv_tc<3, false, 3, true, 64, false>); else go(k_conv_tc<3, false, 3, true, 128, false>);
+  } else if (plan.roll) {
+    if (K == 7) by_n(k_conv_tc<7, true, 7, false, 16, false>, k_conv_tc<7, true, 7, false, 64, false>, k_conv_tc<7, true, 7, false, 128, false>);
+    else if (K == 3) by_n(k_conv_tc<3, true, 3, false, 16, false>, k_conv_tc<3, true, 3, false, 64, false>, k_conv_tc<3, true, 3, false, 128, false>);
+    else by_n(k_conv_tc<1, true, 1, false, 16, false>, k_conv_tc<1, true, 1, false, 64, false>, k_conv_tc<1, true, 1, false, 128, false>);
+  } else {
+    if (K == 7) by_n(k_conv_tc<7, false, 7, false, 16, false>, k_conv_tc<7, false, 7, false, 64, false>, k_conv_tc<7, false, 7, false, 128, false>);
+    else if (K == 3) by_n(k_conv_tc<3, false, 3, false, 16, false>, k_conv_tc<3, false, 3, false, 64, false>, k_conv_tc<3, false, 3, false, 128, false>);
+    else by_n(k_conv_tc<1, false, 1, false, 16, false>, k_conv_tc<1, false, 1, false, 64, false>, k_conv_tc<1, false, 1, false, 128, false>);
   }
-  else if (plan.roll && plan.rows == 4) { if (K == 7) go(k_conv_tc<7, true, 4>); else if (K == 3) go(k_conv_tc<3, true, 4>); else go(k_conv_tc<1, true, 4>); }
-  else if (plan.roll) { if (K == 7) go(k_conv_tc<7, true, 2>); else if (K == 3) go(k_conv_tc<3, true, 2>); else go(k_conv_tc<1, true, 2>); }
-  else if (plan.pk2) go(k_conv_tc<3, false, 2, 3, true>);
-  else { if (K == 7) go(k_conv_tc<7, false, 2>); else if (K == 3) go(k_conv_tc<3, false, 2>); else go(k_conv_tc<1, false, 2>); }
 }
-}  // namespace
 
-namespace {
-void conv_tc_use_stack16(ConvTcPlan& plan, int K);  // below
-// Upper bound on the row blocks one CTA walks.  Long-lived CTAs (one wave of 144 CTAs x 8 blocks = 0.19 ms) amortise the
-// prologue best, but while they run no SM frees up, so the extractors' short dependent kernels -- highest stream priority
-// notwithstanding -- each wait for a whole CTA lifetime; SIVO_B200_TC_MAX_PPC trades the two (unit: row blocks of this kernel;
-// the 16-row full-stack blocks count `scale` x as much).
-int tc_max_ppc(int scale = 1) {
-  static const int v = [] { const char* e = std::getenv("SIVO_B200_TC_MAX_PPC"); return e ? std::max(1, atoi(e)) : 24; }();
-  return std::max(1, v / scale);
+int num_sms() {
+  int dev = 0, n = 0;
+  SIVO_CUDA(cudaGetDevice(&dev));
+  SIVO_CUDA(cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev));
+  return std::max(1, n);
 }
-// Output rows per accumulator stage.  4 rows share each weight tile (TMEM: 2 stages x rows x n_tile <= 512 columns), but
-// a layer too small to give every SM a 4-row block runs 2-row blocks instead: twice the CTAs, half the work each.
-int tc_rows(int K, bool roll, int n_tile, int columns = 1 << 30, int H = 1 << 20) {
-  if (!(roll && n_tile <= 64)) return 2;
-  return static_cast<long>(columns) * ceil_div(H, 4) < 148 ? 2 : 4;
+// Upper bound on the row blocks one CTA walks.  Long-lived CTAs amortise the prologue best, but while they run no SM
+// frees up, so the extractors' short dependent kernels -- highest stream priority notwithstanding -- each wait for a
+// whole CTA lifetime; SIVO_B200_TC_MAX_PPC trades the two (unit: 2-row blocks).
+int tc_max_ppc() {
+  static const int v = [] { const char* e = std::getenv("SIVO_B200_TC_MAX_PPC"); return e ? std::max(1, atoi(e)) : 48; }();
+  return v;
 }
 size_t tc_smem_bytes(int K, bool roll, int n_tile, int stages) {
-  const int rows = tc_rows(K, roll, n_tile);  // the 4-row variant is the larger footprint
-  const int rk = rows + K - 1;
+  const int rk = kRows + K - 1;
   const int slots = roll ? rk : (K == 7 ? rk + 2 : 2 * rk);  // k_conv_tc's kSlots
   const int b_stride = (n_tile * 128 + 1023) & ~1023;
-  return 1024 + static_cast<size_t>(slots) * kSlotBytes + static_cast<size_t>(stages) * b_stride + (2 * slots + 2 * stages + 4) * 8 + 16 + 64 * 16 * 4;  // barriers, TMEM slot, fused-classifier weights
+  return 1024 + static_cast<size_t>(slots) * kSlotBytes + static_cast<size_t>(stages) * b_stride + (2 * slots + 2 * stages) * 8;
 }
 int tc_stages(int K, bool roll, int n_tile) {  // deepest weight ring that fits (0 = configuration does not fit)
   for (int st = kMaxBStages; st >= 3; --st)
@@ -1275,9 +661,22 @@ int tc_stages(int K, bool roll, int n_tile) {  // deepest weight ring that fits 
 }
 int tc_pick_n(const Op& op, const TensorView& out, bool roll) {
   if (out.dt == DType::F32 && out.cs <= 16) return 16;  // the float logits layer
+  if (op.split || op.fold_kw) return 64;                // split: the segment sums must fit in registers next to the accumulators
   int n = (op.cout_p % 128 == 0) ? 128 : 64;
   if (!tc_stages(op.k, roll, n)) n = 64;
   return n;
+}
+// row blocks per CTA: minimise (waves over the SMs) x (blocks per CTA + ~1 block of prologue / halo overhead)
+int tc_blocks_per_cta(long columns, int total_pairs, double overhead) {
+  const int sms = num_sms();
+  int ppc = 1;
+  double best_cost = 1e30;
+  for (int c = 1; c <= std::min(total_pairs, tc_max_ppc()); ++c) {
+    const long ctas = columns * ceil_div(total_pairs, c);
+    const double cost = static_cast<double>((ctas + sms - 1) / sms) * (c + overhead);
+    if (cost < best_cost - 1e-9) { best_cost = cost; ppc = c; }
+  }
+  return ppc;
 }
 }  // namespace
 
@@ -1310,6 +709,7 @@ std::shared_ptr<ConvTcPlan> conv_tc_plan(const Op& op, const TensorView& in, con
   const int K = op.k;
   const int KW = op.fold_kw ? 1 : K;
   const bool roll = (in.cs == 64 || op.fold_kw) && !op.split;
+  const int n_tile = tc_pick_n(op, out, roll);
   if (op.fold_kw) {
     // window-folded input: `in` is the zero-padded 8-channel image [N][H][W + 8][8] half (3 zero pixels left, 5 right);
     // "pixel" x of the operand is the 128-byte window of 8 pixels x 8 channels starting at padded pixel x, i.e. image
@@ -1326,40 +726,27 @@ std::shared_ptr<ConvTcPlan> conv_tc_plan(const Op& op, const TensorView& in, con
                           static_cast<cuuint64_t>(in.n)};
     cuuint64_t strides[3] = {static_cast<cuuint64_t>(in.cs) * 2, static_cast<cuuint64_t>(in.w) * in.cs * 2,
                              static_cast<cuuint64_t>(in.h) * in.w * in.cs * 2};
-    const char* pk2_env = std::getenv("SIVO_B200_TC_PK2");
-    plan->pk2 = !roll && !op.split && K == 3 && in.w <= 64 && in.n >= 2 && !(pk2_env && pk2_env[0] == '0');
+    plan->pk2 = !roll && !op.split && K == 3 && in.w <= 64 && in.n >= 2 && n_tile != 16;
     cuuint32_t box[4] = {64, static_cast<cuuint32_t>(plan->pk2 ? 64 : 128 + K - 1), 1, 1};
     encode(&plan->map_a, in.p, 4, dims, strides, box);
   }
-  const int n_tile = tc_pick_n(op, out, roll);
-  int w_rep = 1;
-  if (const char* e = std::getenv("SIVO_B200_TC_WREP")) w_rep = std::max(1, std::min(16, atoi(e)));
-  {  // weights: [replica][tap][cout_p][cin_p] half, dims (cin, cout, replica * tap)
-    const size_t one = static_cast<size_t>(K) * KW * op.cout_p * op.cin_p * 2 * (op.split ? 3 : 1);
-    void* wbase = const_cast<void*>(w_tc);
-    if (w_rep > 1) {
-      plan->w_replicas.alloc(one * w_rep);
-      for (int r = 0; r < w_rep; ++r)
-        SIVO_CUDA(cudaMemcpy(plan->w_replicas.as<uint8_t>() + r * one, w_tc, one, cudaMemcpyDeviceToDevice));
-      wbase = plan->w_replicas.p;
-    }
+  {  // weights: [tap][cout_p][cin_p] half, dims (cin, cout, tap)
     const int kext = op.split ? 3 * op.cin_p : op.cin_p;  // split: [W_hi | W_lo | W_hi] per 64-channel chunk along K
-    cuuint64_t dims[3] = {static_cast<cuuint64_t>(kext), static_cast<cuuint64_t>(op.cout_p), static_cast<cuuint64_t>(K * KW * w_rep)};
+    cuuint64_t dims[3] = {static_cast<cuuint64_t>(kext), static_cast<cuuint64_t>(op.cout_p), static_cast<cuuint64_t>(K * KW)};
     cuuint64_t strides[2] = {static_cast<cuuint64_t>(kext) * 2, static_cast<cuuint64_t>(op.cout_p) * kext * 2};
     cuuint32_t box[3] = {64, static_cast<cuuint32_t>(n_tile), 1};
-    encode(&plan->map_b, wbase, 3, dims, strides, box);
+    encode(&plan->map_b, const_cast<void*>(w_tc), 3, dims, strides, box);
   }
   TcParams& p = plan->p;
   p.H = in.h; p.W = op.fold_kw ? in.w - 8 : in.w; p.N_batch = in.n;
   p.cout_total = out.cs;
   p.n_tile = n_tile;
   p.chunks = op.fold_kw ? 1 : in.cs / 64;
-  p.w_rep = w_rep;
   p.out_f32 = out.dt == DType::F32 ? (n_tile == 16 ? 1 : 2) : 0;
   p.split = op.split ? 1 : 0;
   p.cin_real = op.cin;
   p.acc_scale = op.split ? op.acc_scale : 1.f;
-  p.seg_rows = 1;  // a segment per (chunk, tap row): 7x7 56 / 28 accumulate steps, 3x3 24 / 12, 1x1 8 / 4 (measured: profiles/r2_parity.md)
+  p.seg_rows = 1;  // a segment per (chunk, tap row): 7x7 56 / 28 accumulate steps, 3x3 24 / 12, 1x1 8 / 4
   if (const char* e = std::getenv("SIVO_B200_SPLIT_SEG")) p.seg_rows = std::max(1, std::min(K, atoi(e)));
   p.rz_comp = 0.216f * 1.1920929e-7f;  // x 2^-23
   if (const char* e = std::getenv("SIVO_B200_SPLIT_RZ")) p.rz_comp = static_cast<float>(atof(e)) * 1.1920929e-7f;
@@ -1367,17 +754,8 @@ std::shared_ptr<ConvTcPlan> conv_tc_plan(const Op& op, const TensorView& in, con
   const int cout_tiles = p.out_f32 == 1 ? 1 : op.cout_p / n_tile;
   const int n_z = plan->pk2 ? ceil_div(in.n, 2) : in.n;  // PK2: an image pair per tile
   const int columns = p.strips * n_z * cout_tiles;
-  const int rows = tc_rows(K, roll, n_tile, columns, in.h);
-  const int total_pairs = ceil_div(in.h, rows);
-  // row blocks per CTA: minimise (waves of 148 SMs) x (blocks per CTA + ~1 block of prologue / halo overhead)
-  int ppc = 1;
-  double best_cost = 1e30;
-  for (int c = 1; c <= std::min(total_pairs, tc_max_ppc()); ++c) {
-    const long ctas = static_cast<long>(columns) * ceil_div(total_pairs, c);
-    const double cost = static_cast<double>((ctas + 147) / 148) * (c + (roll ? (K - 1.0) / rows * 0.5 + 0.5 : 0.3));
-    if (cost < best_cost - 1e-9) { best_cost = cost; ppc = c; }
-  }
-  p.pairs_per_cta = ppc;
+  const int total_pairs = ceil_div(in.h, kRows);
+  p.pairs_per_cta = tc_blocks_per_cta(columns, total_pairs, roll ? (K - 1.0) / kRows * 0.5 + 0.5 : 0.3);
   p.relu = op.relu; p.has_bn = op.has_bn; p.slope = op.slope;
   std::memset(&plan->cst, 0, sizeof(TcConsts));
   if (static_cast<int>(op.h_bias.size()) != op.cout_p || (op.has_bn && (static_cast<int>(op.h_bn_scale.size()) != op.cout_p ||
@@ -1391,65 +769,14 @@ std::shared_ptr<ConvTcPlan> conv_tc_plan(const Op& op, const TensorView& in, con
   p.out = out.p;
   p.has_drop = 0; p.seed = 0; p.frame = nullptr; p.drop_layer = 0; p.drop_scale = 2.f;
   p.unpool_mask = nullptr; p.mask_n = 1;
-  p.dbg_noshift = 0;
-  p.dbg_noepi = 0;
-  if (const char* e = std::getenv("SIVO_B200_TC_NOEPI")) p.dbg_noepi = atoi(e);
-  if (const char* e = std::getenv("SIVO_B200_TC_NOSHIFT")) p.dbg_noshift = e[0] == '1';
-  p.dbg_noload = 0;
-  if (const char* e = std::getenv("SIVO_B200_TC_NOLOAD")) p.dbg_noload = e[0] == '1';
   p.pool_out = nullptr; p.pool_mask = nullptr;
   p.has_cls = 0; p.cls_out = nullptr;
-  plan->grid = dim3(p.strips * ceil_div(total_pairs, ppc), cout_tiles, n_z);
+  plan->grid = dim3(p.strips * ceil_div(total_pairs, p.pairs_per_cta), cout_tiles, n_z);
   p.b_stages = tc_stages(K, roll, n_tile);
-  if (const char* e = std::getenv("SIVO_B200_TC_BSTAGES")) p.b_stages = std::max(2, std::min(p.b_stages, atoi(e)));  // experiment knob
   plan->smem = tc_smem_bytes(K, roll, n_tile, p.b_stages);
-  const char* pair_env = std::getenv("SIVO_B200_TC_PAIR");
-  if (roll && !op.fold_kw && rows == 4 && n_tile == 64 && op.cout_p == 64 && !p.out_f32 && (K == 7 || K == 3) && op.w_tc_pair.p &&
-      !(pair_env && pair_env[0] == '0')) {  // default on: ~2 % faster than the N = 64 kernel (profiles/r1_notes.md)
-    // paired-tap kernel: weights as one [K*K*64 rows][64 cin] matrix in (kw, kh, cout) row order, 128-row boxes
-    const size_t one = static_cast<size_t>(K) * K * 64 * 128;
-    void* wbase = op.w_tc_pair.p;
-    if (w_rep > 1) {
-      plan->w_replicas.alloc(one * w_rep);
-      for (int r = 0; r < w_rep; ++r)
-        SIVO_CUDA(cudaMemcpy(plan->w_replicas.as<uint8_t>() + r * one, op.w_tc_pair.p, one, cudaMemcpyDeviceToDevice));
-      wbase = plan->w_replicas.p;
-    }
-    const char* triple_env = std::getenv("SIVO_B200_TC_TRIPLE");
-    plan->triple = K == 7 && !(triple_env && triple_env[0] == '0');
-    cuuint64_t dims[3] = {64, static_cast<cuuint64_t>(K) * K * 64, static_cast<cuuint64_t>(w_rep)};
-    cuuint64_t strides[2] = {128, one};
-    cuuint32_t box[3] = {64, static_cast<cuuint32_t>(plan->triple ? 64 : 128), 1};
-    encode(&plan->map_b, wbase, 3, dims, strides, box);
-    plan->pair = true;
-    const int slots = plan->triple ? 9 : rows + K - 1;
-    const size_t stage = plan->triple ? 24576 : 16384;
-    int st = plan->triple ? 3 : 6;
-    auto bytes = [&](int n) { return 1024 + static_cast<size_t>(slots) * kSlotBytes + static_cast<size_t>(n) * stage + (2 * slots + 2 * n + 4) * 8 + 16; };
-    while (st > 2 && bytes(st) > 227 * 1024) --st;
-    if (bytes(st) > 227 * 1024) fail(SIVO_EINVAL, "paired-tap kernel does not fit in shared memory");
-    p.b_stages = st;
-    plan->smem = bytes(st);
-  }
   plan->k = K;
   plan->kw = KW;
   plan->roll = roll;
-  plan->rows = rows;
-  const char* stack_env = std::getenv("SIVO_B200_STACK16");
-  if (roll && !op.fold_kw && !op.split && p.out_f32 == 1 && (K == 3 || K == 7) && op.cin == 64 && op.cout <= 16 &&
-      op.h_w_raw.size() == static_cast<size_t>(op.cout) * 64 * K * K && !(stack_env && stack_env[0] == '0')) {
-    // the float logits layer (Standard: conv1_1_D, 64 -> 15, 3x3): all K tap rows stacked along N on the full-stack kernel
-    std::vector<__half> w(static_cast<size_t>(K) * K * 16 * 64, __float2half_rn(0.f));
-    for (int o = 0; o < op.cout; ++o)
-      for (int i = 0; i < 64; ++i)
-        for (int kh = 0; kh < K; ++kh)
-          for (int kw = 0; kw < K; ++kw)
-            w[((static_cast<size_t>(kw) * K + kh) * 16 + o) * 64 + i] =
-                __float2half_rn(op.h_w_raw[((static_cast<size_t>(o) * 64 + i) * K + kh) * K + kw]);
-    plan->w_replicas.alloc(w.size() * sizeof(__half));
-    SIVO_CUDA(cudaMemcpy(plan->w_replicas.p, w.data(), w.size() * sizeof(__half), cudaMemcpyHostToDevice));
-    conv_tc_use_stack16(*plan, K);
-  }
   conv_tc_dispatch(*plan, nullptr, true);
   return plan;
 }
@@ -1466,18 +793,6 @@ void conv_tc_set_unpool(ConvTcPlan& plan, const uint8_t* mask, int mask_n, void*
   plan.p.unpool_mask = mask;
   plan.p.mask_n = mask_n;
   plan.p.out = out_2h_2w;
-}
-
-std::vector<__half> conv_tc_pair_weights(const float* w_cout_cin_k_k, int K) {
-  // [kw][kh][cout = 64][cin = 64] half from Caffe's (cout, cin, kh, kw) float blob
-  std::vector<__half> out(static_cast<size_t>(K) * K * 64 * 64);
-  for (int kw = 0; kw < K; ++kw)
-    for (int kh = 0; kh < K; ++kh)
-      for (int co = 0; co < 64; ++co)
-        for (int ci = 0; ci < 64; ++ci)
-          out[((static_cast<size_t>(kw) * K + kh) * 64 + co) * 64 + ci] =
-              __float2half_rn(w_cout_cin_k_k[((static_cast<size_t>(co) * 64 + ci) * K + kh) * K + kw]);
-  return out;
 }
 
 std::vector<__half> conv_tc_split_weights(const float* W, int cout, int cin, int K, int cout_p, int cin_p, float* acc_scale) {
@@ -1525,35 +840,9 @@ void conv_tc_set_classifier(ConvTcPlan& plan, const float* w_cin_by_cout, int st
   plan.p.cls_out = logits;
 }
 
-namespace {
-// Points a plan whose weights sit in plan.w_replicas as [kw][kh][16][64] half at the full-stack kernel (k_conv_tc_stack16<K>).
-void conv_tc_use_stack16(ConvTcPlan& plan, int K) {
-  TcParams& p = plan.p;
-  cuuint64_t dims[3] = {64, static_cast<cuuint64_t>(K) * K * 16, 1};
-  cuuint64_t strides[2] = {128, static_cast<cuuint64_t>(K) * K * 16 * 128};
-  cuuint32_t box_s[3] = {64, static_cast<cuuint32_t>(K * 16), 1};  // one box per tap column: K taps x 16 rows
-  encode(&plan.map_b, plan.w_replicas.p, 3, dims, strides, box_s);
-  plan.stack16 = true;
-  plan.pair = plan.triple = plan.nw16 = false;
-  const int total_blocks = ceil_div(p.H, kStackRows);
-  const int columns = p.strips * p.N_batch;
-  int ppc = 1;
-  double best_cost = 1e30;
-  for (int c = 1; c <= std::min(total_blocks, tc_max_ppc(2)); ++c) {  // (waves of 148 SMs) x (blocks per CTA + weight load / prologue)
-    const long ctas = static_cast<long>(columns) * ceil_div(total_blocks, c);
-    const double cost = static_cast<double>((ctas + 147) / 148) * (c + 0.35);
-    if (cost < best_cost - 1e-9) { best_cost = cost; ppc = c; }
-  }
-  p.pairs_per_cta = ppc;
-  plan.grid = dim3(p.strips * ceil_div(total_blocks, ppc), 1, p.N_batch);
-  const size_t wbytes = (static_cast<size_t>(K) * K * 16 * 128 + 1023) & ~static_cast<size_t>(1023);
-  plan.smem = 1024 + wbytes + static_cast<size_t>(kStackSlots) * kSlotBytes + (2 * kStackSlots + 1 + 4) * 8 + 16;
-}
-}  // namespace
-
 bool conv_tc_can_compose_classifier(const ConvTcPlan& plan) {
-  return plan.pair && plan.triple && plan.k == 7 && !plan.p.out_f32 && !plan.p.unpool_mask && !plan.p.has_drop && !plan.p.pool_out &&
-         !plan.p.has_cls && !plan.p.relu && !plan.p.has_bn && plan.p.cout_total == 64;
+  return plan.roll && plan.k == 7 && plan.kw == 7 && plan.p.n_tile == 64 && !plan.p.out_f32 && !plan.p.unpool_mask &&
+         !plan.p.has_drop && !plan.p.pool_out && !plan.p.has_cls && !plan.p.relu && !plan.p.has_bn && plan.p.cout_total == 64;
 }
 
 void conv_tc_set_composed_classifier(ConvTcPlan& plan, const Op& conv, const float* wc, const float* bc, int n_cls, float* logits) {
@@ -1561,7 +850,7 @@ void conv_tc_set_composed_classifier(ConvTcPlan& plan, const Op& conv, const flo
   if (n_cls > 16 || conv.h_w_raw.size() != static_cast<size_t>(64) * 64 * K * K || conv.h_bias.size() < 64)
     fail(SIVO_EINVAL, "composed classifier: unexpected layer shapes");
   // W'[o][i][kh][kw] = sum_c wc[o][c] W[c][i][kh][kw] in double, rounded once to half; rows o >= n_cls stay zero.
-  // Device layout [kw][kh][16][64]: one 16-row TMA box per tap, K-major rows like every other B tile.
+  // Device layout [kh][kw][16][64]: the [tap][cout][cin] layout of every other weight tensor, 16-row tiles.
   std::vector<__half> w(static_cast<size_t>(K) * K * 16 * 64, __float2half_rn(0.f));
   const float* W = conv.h_w_raw.data();
   for (int o = 0; o < n_cls; ++o)
@@ -1570,14 +859,14 @@ void conv_tc_set_composed_classifier(ConvTcPlan& plan, const Op& conv, const flo
         for (int kw = 0; kw < K; ++kw) {
           double acc = 0.0;
           for (int c = 0; c < 64; ++c) acc += static_cast<double>(wc[o * 64 + c]) * W[((static_cast<size_t>(c) * 64 + i) * K + kh) * K + kw];
-          w[((static_cast<size_t>(kw) * K + kh) * 16 + o) * 64 + i] = __float2half_rn(static_cast<float>(acc));
+          w[((static_cast<size_t>(kh) * K + kw) * 16 + o) * 64 + i] = __float2half_rn(static_cast<float>(acc));
         }
-  plan.w_replicas.alloc(w.size() * sizeof(__half));
-  SIVO_CUDA(cudaMemcpy(plan.w_replicas.p, w.data(), w.size() * sizeof(__half), cudaMemcpyHostToDevice));
-  cuuint64_t dims[3] = {64, static_cast<cuuint64_t>(K) * K * 16, 1};
-  cuuint64_t strides[2] = {128, static_cast<cuuint64_t>(K) * K * 16 * 128};
+  plan.w_own.alloc(w.size() * sizeof(__half));
+  SIVO_CUDA(cudaMemcpy(plan.w_own.p, w.data(), w.size() * sizeof(__half), cudaMemcpyHostToDevice));
+  cuuint64_t dims[3] = {64, 16, static_cast<cuuint64_t>(K) * K};
+  cuuint64_t strides[2] = {128, 16 * 128};
   cuuint32_t box[3] = {64, 16, 1};
-  encode(&plan.map_b, plan.w_replicas.p, 3, dims, strides, box);
+  encode(&plan.map_b, plan.w_own.p, 3, dims, strides, box);
   std::memset(&plan.cst, 0, sizeof(TcConsts));
   for (int o = 0; o < n_cls; ++o) {
     double acc = bc[o];
@@ -1589,15 +878,9 @@ void conv_tc_set_composed_classifier(ConvTcPlan& plan, const Op& conv, const flo
   p.n_tile = 16;
   p.cout_total = 16;
   p.out = logits;
-  p.w_rep = 1;
-  const char* stack_env = std::getenv("SIVO_B200_STACK16");
-  if (!(stack_env && stack_env[0] == '0')) {
-    conv_tc_use_stack16(plan, K);
-  } else {
-    p.b_stages = 6;
-    plan.nw16 = true;
-    plan.smem = 1024 + static_cast<size_t>(9) * kSlotBytes + static_cast<size_t>(p.b_stages) * 3 * 16 * 128 + (2 * 9 + 2 * p.b_stages + 4) * 8 + 16;
-  }
+  p.b_stages = tc_stages(K, true, 16);
+  plan.smem = tc_smem_bytes(K, true, 16, p.b_stages);
+  plan.grid.y = 1;
   conv_tc_dispatch(plan, nullptr, true);
 }
 

@@ -63,9 +63,8 @@ struct OrbSelected {  // one retained keypoint, level coordinates
 // Programmatic dependent launch for the extractor's chain of short dependent kernels: every kernel starts with
 // `griddepcontrol.launch_dependents; griddepcontrol.wait;` (ORB_PDL_PROLOGUE), so the next grid of the stream is scheduled while
 // this one drains and only its launch latency -- not its work -- overlaps (the wait returns once the previous grid has completed
-// and flushed).  Opt-in (SIVO_B200_ORB_PDL=1; without the attribute the prologue is a no-op): measured on B200 it does not
-// shorten a lone extractor call (0.336 vs 0.312 ms for the concurrent pair) and costs the full frame 10 % (0.855 vs 0.75 ms) --
-// the early CTAs of the next small kernel sit on SMs the convolution CTAs need (profiles/r2_notes.md).
+// and flushed).  Opt-in (SIVO_B200_ORB_PDL=1; without the attribute the prologue is a no-op): the early CTAs of the next small
+// kernel sit on SMs the convolution CTAs need.
 #define ORB_PDL_PROLOGUE() asm volatile("griddepcontrol.launch_dependents;\n\tgriddepcontrol.wait;" ::: "memory")
 template <class... KArgs, class... Args>
 inline void orb_launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args... args) {

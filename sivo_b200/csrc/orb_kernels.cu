@@ -1,7 +1,7 @@
 // ORB extractor kernels.  All integer / byte work, bit-exact against oracle/orb_oracle.py (which is pinned
 // to cv2): pyramid (cv::resize INTER_LINEAR fixed point + REFLECT_101 border), FAST-9/16 score map,
 // per-cell threshold / 3x3 NMS / ordered compaction, 7x7 sigma-2 fixed-point blur, IC angle, rBRIEF.
-// Everything here is latency/launch bound on B200 (~8 MB touched per image), so the design goal is few
+// Everything here is latency/launch bound on the GPU (~8 MB touched per image), so the design goal is few
 // launches over all 8 levels at once rather than bandwidth tricks.
 #include "orb.h"
 

@@ -73,11 +73,6 @@ void SegNet::prepare_conv(Op& op, const std::vector<Blob>& cb, const std::vector
         }
     op.w_tc.alloc(wt.size() * sizeof(__half));
     SIVO_CUDA(cudaMemcpy(op.w_tc.p, wt.data(), wt.size() * sizeof(__half), cudaMemcpyHostToDevice));
-    if (!op.expand_k && (K == 7 || K == 3) && cin == 64 && cout == 64 && op.cin_p == 64 && op.cout_p == 64) {
-      std::vector<__half> wp = conv_tc_pair_weights(W, K);
-      op.w_tc_pair.alloc(wp.size() * sizeof(__half));
-      SIVO_CUDA(cudaMemcpy(op.w_tc_pair.p, wp.data(), wp.size() * sizeof(__half), cudaMemcpyHostToDevice));
-    }
   }
   if (op.split) {
     if (taps != K * K) fail(SIVO_EINVAL, "layer '%s': split-operand mode does not take folded / expanded first layers", op.layer.c_str());

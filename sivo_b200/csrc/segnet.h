@@ -40,8 +40,8 @@ struct Op {
   int expand_k = 0, expand_blk = 0;  // > 0: a KxK conv over 3 channels run as a 1x1 conv over the tap-expanded input
   bool relu = false, has_bn = false;
   float slope = 0.f;
-  DevBuf w_simt, w_tc, w_tc_pair, bias, bn_scale, bn_shift;  // w_tc_pair: [kw][kh][cout][cin] half for the paired-tap kernel
-  // split-operand fp32 mode (precision fp32 on the tcgen05 engine): x = hi + lo and w * 2^s = hi + lo in half, and
+  DevBuf w_simt, w_tc, bias, bn_scale, bn_shift;
+  // split-operand fp32 mode (precision fp32 on the tensor-core engine): x = hi + lo and w * 2^s = hi + lo in half, and
   // x * w ~= (x_hi w_hi + x_hi w_lo + x_lo w_hi) * 2^-s accumulated in fp32 -- three MMAs per tap, ~2^-22 relative per product.
   // w_tc holds [tap][cout_p][3 cin_p] = per 64-channel chunk [W_hi | W_lo | W_hi]; a_split the [hi Cin | lo Cin] planes of the input.
   bool split = false;
@@ -128,7 +128,7 @@ class SegNet {
   float* rec_ent32_ = nullptr;
 };
 
-// conv_tc.cu -- tcgen05 implicit-GEMM convolution
+// conv_tc.cu -- wgmma implicit-GEMM convolution
 bool conv_tc_supported(const Op& op, const TensorView& in, const TensorView& out);
 std::shared_ptr<ConvTcPlan> conv_tc_plan(const Op& op, const TensorView& in, const TensorView& out, const void* w_tc);
 void conv_tc_launch(const ConvTcPlan& plan, const Op& op, cudaStream_t s);
@@ -144,8 +144,6 @@ void conv_tc_set_pool(ConvTcPlan& plan, void* pooled, uint8_t* mask);
 bool conv_tc_can_fuse_classifier(const ConvTcPlan& plan);
 // host-side weight layout of the split-operand fp32 mode: [tap][cout_p][3 cin_p] half + the accumulator scale 2^-s
 std::vector<__half> conv_tc_split_weights(const float* w_cout_cin_k_k, int cout, int cin, int K, int cout_p, int cin_p, float* acc_scale);
-// host-side weight layout of the paired-tap kernel (64 -> 64 channels)
-std::vector<__half> conv_tc_pair_weights(const float* w_cout_cin_k_k, int K);
 // Experimental (SIVO_B200_COMPOSE=1): conv (64 -> 64, 7x7, no BN / ReLU) followed by the 1x1 classifier run as ONE 64 -> 16
 // convolution with composed weights; logits come straight from the accumulators.  wc = [n_cls][64], bc = [n_cls] (host).
 bool conv_tc_can_compose_classifier(const ConvTcPlan& plan);

@@ -1,4 +1,4 @@
-// SegNet layer kernels, SIMT set: the strict-fp32 engine, the correctness anchor for the tcgen05
+// SegNet layer kernels, SIMT set: the strict-fp32 engine, the correctness anchor for the tensor-core
 // convolution (conv_tc.cu), and every bandwidth-bound layer.  Semantics follow the Caffe layers the
 // reference executes (SURVEY 2b); each kernel cites the layer it replaces.
 #include <cuda_fp16.h>
@@ -661,7 +661,7 @@ void launch_input_lrn_pad8(const uint8_t* bgr, TensorView out, int size, float a
 }
 
 // Split-operand fp32 mode: float NHWC [px][C] -> half [px][hi C | lo C] with hi = half(x), lo = half(x - hi) (both roundings
-// to nearest; x - hi is exact in fp32), the A operand planes of the tcgen05 convolution (conv_tc.cu, TcParams::split).
+// to nearest; x - hi is exact in fp32), the A operand planes of the tensor-core convolution (conv_tc.cu, TcParams::split).
 __global__ void k_split_hilo(const float4* __restrict__ in, uint2* __restrict__ out, size_t npix, int c4) {
   const size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= npix * c4) return;

@@ -115,15 +115,15 @@ def test_conv_simt_matches_oracle(k, cin, cout, prec):
                                               (3, 64, 128, 2, 11, 96), (7, 64, 64, 3, 44, 128), (3, 64, 64, 1, 64, 300),
                                               (1, 64, 15, 2, 10, 140), (3, 64, 15, 1, 12, 128), (3, 128, 128, 2, 11, 96),
                                               (3, 256, 64, 1, 22, 64), (3, 512, 512, 2, 11, 32), (1, 128, 64, 1, 6, 130),
-                                              # 4-row blocks (columns x ceil(H/4) >= 148): the paired / TRIPLE stacked-tap kernels
+                                              # full-size layers: many row blocks per CTA
                                               (7, 64, 64, 2, 176, 512), (7, 64, 64, 1, 352, 300), (3, 64, 64, 1, 160, 512),
                                               (3, 64, 64, 2, 90, 520),
                                               # at most 64 pixels wide, Cin > 64: two images per M tile, kw shift by TMA (PK2)
                                               (3, 128, 128, 3, 22, 64), (3, 512, 512, 12, 22, 64), (3, 256, 256, 2, 11, 33), (3, 128, 64, 5, 6, 20)])
 def test_conv_tcgen05_matches_oracle(k, cin, cout, n, h, w):
     """The tensor-core convolution against torch fp32 on identical half-rounded operands; sizes cover partial
-    strips (W not a multiple of 128), an odd height, several images, both UMMA N tiles, and shapes large enough to take the
-    4-row paired-tap (K = 3) and paired + TRIPLE stacked-tap (K = 7) kernels the full-size nets run."""
+    strips (W not a multiple of 128), an odd height, several images, the 16 / 64 / 128-wide wgmma N tiles, and the
+    full-size shapes the nets run."""
     import torch.nn.functional as F
     rng = np.random.default_rng(5)
     x = rng.normal(0, 1, size=(n, cin, h, w)).astype(np.float32)
@@ -146,8 +146,8 @@ def test_conv_tcgen05_matches_oracle(k, cin, cout, n, h, w):
                                               (1, 64, 15, 2, 10, 140), (3, 64, 15, 1, 12, 128), (3, 128, 128, 2, 11, 96),
                                               (3, 256, 64, 1, 22, 64), (3, 512, 512, 2, 11, 32), (7, 64, 64, 1, 60, 300)])
 def test_conv_tcgen05_split_operand_mode_is_fp32_grade(k, cin, cout, n, h, w):
-    """precision fp32 on the tcgen05 engine: x = hi + lo, w = hi + lo in half, x*w ~ hi*hi + hi*lo + lo*hi accumulated in fp32
-    (TMEM).  Compared with a float64 convolution of the same fp32 inputs; the bar is caffe's own conv tolerance (1e-4,
+    """precision fp32 on the tensor-core engine: x = hi + lo, w = hi + lo in half, x*w ~ hi*hi + hi*lo + lo*hi accumulated in fp32
+    (registers).  Compared with a float64 convolution of the same fp32 inputs; the bar is caffe's own conv tolerance (1e-4,
     test_convolution_layer.cpp) with two orders of margin, and torch's fp32 convolution is measured next to it."""
     import torch.nn.functional as F
     rng = np.random.default_rng(6)

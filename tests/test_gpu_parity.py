@@ -5,8 +5,8 @@ activations, logits std ~2.5, entropy spread over [0, log2 15] -- no saturated `
 
 north_star bar: classes bit-exact given the dropout seed, confidence / entropy within 1e-4.  Two modes are held to it:
 
-  strict  precision fp32 on the tcgen05 engine: split-operand mode (x = hi + lo, w = hi + lo in half, three MMAs per tap,
-          fp32 accumulation in TMEM, fp32 bias / BN / ReLU / pool / unpool / dropout) -- MUST meet 1e-4, and every class
+  strict  precision fp32 on the tensor-core engine: split-operand mode (x = hi + lo, w = hi + lo in half, three MMAs per tap,
+          fp32 accumulation in registers, fp32 bias / BN / ReLU / pool / unpool / dropout) -- MUST meet 1e-4, and every class
           mismatch must be a tie (top-2 margin of the oracle's mean softmax below 1e-5).
   fast    precision fp16 (the default, benchmarked mode): half operands and half activation storage.  It cannot meet 1e-4
           (half rounding alone is 2^-11 per stored value); the test states its measured gap and bounds it.
@@ -57,8 +57,7 @@ def run_mode(mode, proto, model, T, img, frame, keep_blobs=False):
 
 def check(mode, r_hand, flip_rate):
     if mode == "fast":
-        # measured on B200 (profiles/r2_parity.md): entropy max 3e-3 (Basic) .. 1.2e-2 (Standard), class mismatches ~1e-3 of
-        # the pixels, all near-ties.  Pooling flips: two window entries that round to the same half tie on the device and
+        # expected: entropy max ~3e-3 (Basic) .. ~1e-2 (Standard), class mismatches ~1e-3 of the pixels, all near-ties.  Pooling flips: two window entries that round to the same half tie on the device and
         # not in the fp32 oracle, ~1 % of the windows (each checked to be such a tie by check_masks_are_ties)
         assert r_hand["ent_max"] < 3e-2 and r_hand["conf_max"] < 1e-2 and r_hand["ent_q99"] < 1e-2
         assert r_hand["class_mismatch_px"] < 5e-3 * r_hand["px"] and r_hand["max_margin_of_mismatch"] < 1e-2

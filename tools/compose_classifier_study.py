@@ -1,4 +1,4 @@
-"""CPU study for the round-2 question (profiles/r1_notes.md): how does composing conv_decode1 with the 1x1 classifier
+"""CPU study: how does composing conv_decode1 with the 1x1 classifier
 (logits = (Wc W) * x + Wc b + bc, half weights, fp32 accumulation) compare with today's two-step fp16 path, both measured
 against the same two convolutions evaluated in float64 on the same (half-rounded) input?  Oracle only; no GPU."""
 import os

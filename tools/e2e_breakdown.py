@@ -1,4 +1,4 @@
-"""Where the end-to-end frame time goes (one B200): segmentImage alone, the two extractor calls alone, all three
+"""Where the end-to-end frame time goes (one GPU): segmentImage alone, the two extractor calls alone, all three
 concurrently -- page-locked host buffers, as bench.py's e2e arm.  Prints ms per frame."""
 import os
 import sys

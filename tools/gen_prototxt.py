@@ -1,8 +1,8 @@
 """Emits the two Bayesian SegNet topologies as Caffe prototxt text from a compact description, so the
-bench and tests have model files on the GPU box (where /root/reference does not exist).  The layer names,
+bench and tests have model files without the reference tree.  The layer names,
 blob names and hyper-parameters are the ones `Net::CopyTrainedLayersFrom` matches weights against
-(config/bayesian_segnet/{basic,standard}/kitti/*.prototxt in the reference); tests/test_prototxt.py checks,
-when /root/reference is present, that these parse to the same layer list as the shipped files.
+(config/bayesian_segnet/{basic,standard}/kitti/*.prototxt in the reference); tests/test_host.py checks that these parse to
+the reference's layer list (stored in tests/golden/reference_topology.json.gz).
 
 usage: python tools/gen_prototxt.py   -> configs/bayesian_segnet_basic.prototxt, configs/bayesian_segnet.prototxt
 """
