@@ -90,6 +90,31 @@ int sivo_segnet_set_record_outputs(sivo_segnet_t* h, uint8_t* classes_device, fl
  * reduction; the double maps stay the operator's outputs (bayesian_segnet.cpp:192-203, 262-276 compute in double). */
 int sivo_segnet_run_device_maps(sivo_segnet_t* h, const uint8_t* bgr_device, uint8_t* classes_device, double* confidence_device,
                                 double* entropy_device, float* confidence_f32_device, float* entropy_f32_device, void* stream);
+/* ---- latency mode (SURVEY 8e): one frame's Monte-Carlo samples split across GPUs ------------------------------------
+ * A shard handle owns the samples [sample_begin, sample_begin + sample_count) of a frame of opt->T samples (0 = the prototxt's
+ * batch): it runs the sample-invariant prefix once and the rest of the net for its own samples only, and sample n of the shard
+ * draws exactly the dropout masks sample sample_begin + n draws in a whole-frame handle with the same seed and frame counter.
+ * Each rank sums its samples' softmax (sivo_segnet_run_partial_device), the sums are added across ranks (e.g. one reduce),
+ * and one rank turns the total into the operator's maps (sivo_segnet_finalize_device).  A handle from sivo_segnet_create_ex is
+ * the shard [0, T).  SIVO_EINVAL for sample_begin < 0, sample_count < 1 or sample_begin + sample_count > T, and for T <= 1 as
+ * in sivo_segnet_create.  sivo_segnet_run, _run_device and _run_device_maps refuse a shard that owns fewer than T samples
+ * (SIVO_EINVAL).  The frame counter advances per sivo_segnet_run_partial_device exactly as per sivo_segnet_run_device, so
+ * shards created alike and pinned with sivo_segnet_set_frame stay in lockstep. */
+int sivo_segnet_create_shard(const char* prototxt, const char* caffemodel, const sivo_segnet_options* opt, int sample_begin,
+                             int sample_count, sivo_segnet_t** out);
+/* The handle's sample range and the frame's sample count T (the mean divides by T); any output may be NULL. */
+int sivo_segnet_samples(const sivo_segnet_t* h, int* sample_begin, int* sample_count, int* T_total);
+/* bgr_device as in sivo_segnet_run_device.  sum_device: height*width x 16 doubles, pixel-major, overwritten with the sum over
+ * the shard's samples of the per-sample softmax (the per-sample arithmetic of the one-pass reduction; channels >= n_classes
+ * are 0).  On `stream` (NULL = the handle's own), no host synchronisation.  SIVO_EINVAL for a NULL image or sum; SIVO_EFORMAT
+ * if the net has more than 16 classes. */
+int sivo_segnet_run_partial_device(sivo_segnet_t* h, const uint8_t* bgr_device, double* sum_device, void* stream);
+/* sum_device: the sum over ALL T samples of the frame (e.g. the shards' sums after a reduction over ranks), layout as above.
+ * Writes what sivo_segnet_run_device_maps writes, any output may be NULL; the shard [0, T) followed by this call gives the same
+ * bits as sivo_segnet_run_device_maps.  The maps become the ones sivo_segnet_semantic_keys reads.  Does not touch the frame
+ * counter.  On `stream` (NULL = the handle's own), no host synchronisation; SIVO_EINVAL for a NULL sum. */
+int sivo_segnet_finalize_device(sivo_segnet_t* h, const double* sum_device, uint8_t* classes_device, double* confidence_device,
+                                double* entropy_device, float* confidence_f32_device, float* entropy_f32_device, void* stream);
 /* Test hook: copies blob `name` (any top in the prototxt; needs keep_blobs) to `out` as float NCHW.
  * `*n`, `*c`, `*hh`, `*ww` receive its shape; `out` may be NULL to query the shape only. */
 int sivo_segnet_blob(sivo_segnet_t* h, const char* name, float* out, size_t cap, int* n, int* c, int* hh,

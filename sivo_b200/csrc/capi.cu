@@ -43,6 +43,45 @@ int sivo_segnet_create_ex(const char* prototxt, const char* caffemodel, const si
   });
 }
 
+int sivo_segnet_create_shard(const char* prototxt, const char* caffemodel, const sivo_segnet_options* opt, int sample_begin,
+                             int sample_count, sivo_segnet_t** out) {
+  return guarded([&] {
+    if (!out) fail(SIVO_EINVAL, "null output handle");
+    *out = nullptr;
+    if (sample_begin < 0 || sample_count < 1)
+      fail(SIVO_EINVAL, "sample range: begin %d must be >= 0 and count %d >= 1", sample_begin, sample_count);
+    sivo_segnet_options o{};
+    if (opt) o = *opt;
+    auto* impl = new SegNet(prototxt ? prototxt : "", caffemodel ? caffemodel : "", o, sample_begin, sample_count);
+    *out = new sivo_segnet{impl};
+  });
+}
+
+int sivo_segnet_samples(const sivo_segnet_t* h, int* sample_begin, int* sample_count, int* T_total) {
+  return guarded([&] {
+    if (!h) fail(SIVO_EINVAL, "null handle");
+    if (sample_begin) *sample_begin = h->impl->sample_begin();
+    if (sample_count) *sample_count = h->impl->sample_count();
+    if (T_total) *T_total = h->impl->T();
+  });
+}
+
+int sivo_segnet_run_partial_device(sivo_segnet_t* h, const uint8_t* bgr_device, double* sum_device, void* stream) {
+  return guarded([&] {
+    if (!h || !bgr_device || !sum_device) fail(SIVO_EINVAL, "null handle, image or sum buffer");
+    h->impl->run_partial(bgr_device, sum_device, static_cast<cudaStream_t>(stream));
+  });
+}
+
+int sivo_segnet_finalize_device(sivo_segnet_t* h, const double* sum_device, uint8_t* classes_device, double* confidence_device,
+                                double* entropy_device, float* confidence_f32_device, float* entropy_f32_device, void* stream) {
+  return guarded([&] {
+    if (!h || !sum_device) fail(SIVO_EINVAL, "null handle or sum buffer");
+    h->impl->finalize(sum_device, classes_device, confidence_device, entropy_device, confidence_f32_device, entropy_f32_device,
+                      static_cast<cudaStream_t>(stream));
+  });
+}
+
 int sivo_segnet_create(const char* prototxt, const char* caffemodel, int device, uint64_t seed, sivo_segnet_t** out) {
   sivo_segnet_options o{};
   o.device = device;

@@ -71,7 +71,8 @@ struct TcParams {
   // dropout fused into the epilogue (decoder convs of Basic: decdrop4 / decdrop3)
   uint64_t seed;
   const uint64_t* frame;
-  int drop_layer;
+  uint32_t drop_nl;        // sample0 | layer << 16: local image i draws the keep bits of dropout layer `layer`, global sample
+                           // sample0 + i (a shard handle owns samples [sample0, sample0 + N_batch) of the frame)
   float drop_scale;
   // max-unpool fused into the epilogue (decoder convs): the output tensor is 2H x 2W and every pixel's channel
   // lands in the 2x2 position its pooling mask names, zeros elsewhere (upsample_layer.cpp:74-103)
@@ -303,7 +304,7 @@ __device__ __forceinline__ void epilogue_block(const TcParams& p, const TcConsts
       }
       uint32_t bits[4] = {0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu};
       if (p.has_drop && inside)  // a tile never straddles a 128-channel group (n0 is a multiple of N <= 128)
-        dropout_bits128(p.seed, *p.frame, p.drop_layer, img, static_cast<uint32_t>(y * p.W + x), n0 >> 7, bits);
+        dropout_bits128_nl(p.seed, *p.frame, p.drop_nl + img, static_cast<uint32_t>(y * p.W + x), n0 >> 7, bits);
       const size_t mask_pix = (static_cast<size_t>(img % p.mask_n) * p.H + y) * p.W + x;
 #pragma unroll
       for (int j = 0; j < N / 8; ++j) {
@@ -767,7 +768,7 @@ std::shared_ptr<ConvTcPlan> conv_tc_plan(const Op& op, const TensorView& in, con
     std::copy(op.h_bn_shift.begin(), op.h_bn_shift.end(), plan->cst.bn_shift);
   }
   p.out = out.p;
-  p.has_drop = 0; p.seed = 0; p.frame = nullptr; p.drop_layer = 0; p.drop_scale = 2.f;
+  p.has_drop = 0; p.seed = 0; p.frame = nullptr; p.drop_nl = 0; p.drop_scale = 2.f;
   p.unpool_mask = nullptr; p.mask_n = 1;
   p.pool_out = nullptr; p.pool_mask = nullptr;
   p.has_cls = 0; p.cls_out = nullptr;
@@ -781,11 +782,14 @@ std::shared_ptr<ConvTcPlan> conv_tc_plan(const Op& op, const TensorView& in, con
   return plan;
 }
 
-void conv_tc_set_dropout(ConvTcPlan& plan, uint64_t seed, const uint64_t* frame_dev, int layer, float scale) {
+void conv_tc_set_dropout(ConvTcPlan& plan, uint64_t seed, const uint64_t* frame_dev, int layer, float scale, int sample0) {
   plan.p.has_drop = 1;
   plan.p.seed = seed;
   plan.p.frame = frame_dev;
-  plan.p.drop_layer = layer;
+  if (sample0 < 0 || sample0 + plan.p.N_batch > (1 << 16) || layer < 0 || layer > 255)
+    fail(SIVO_EINVAL, "conv_tc_set_dropout: samples [%d, %d) / layer %d outside the keep-bit counter's fields", sample0,
+         sample0 + plan.p.N_batch, layer);
+  plan.p.drop_nl = static_cast<uint32_t>(sample0) | (static_cast<uint32_t>(layer) << 16);
   plan.p.drop_scale = scale;
 }
 

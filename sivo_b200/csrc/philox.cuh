@@ -25,12 +25,19 @@ __host__ __device__ __forceinline__ void philox4x32_10(uint32_t c0, uint32_t c1,
   out[0] = c0; out[1] = c1; out[2] = c2; out[3] = c3;
 }
 
+// The same with the sample / layer part of the counter word given whole: nl = n | layer << 16 (n < 2^16, so a caller may add
+// a sample offset to it).  The fields are disjoint, so the group is added rather than or-ed: the same word, and in the
+// convolution epilogue one IADD3 with the caller's addition (no extra register pressure).
+__host__ __device__ __forceinline__ void dropout_bits128_nl(uint64_t seed, uint64_t frame, uint32_t nl, uint32_t pix, int g,
+                                                            uint32_t out[4]) {
+  philox4x32_10(pix, nl + (static_cast<uint32_t>(g) << 24), static_cast<uint32_t>(frame), static_cast<uint32_t>(frame >> 32),
+                static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32), out);
+}
+
 // 128 keep bits for channels [128*g, 128*g+128) of pixel `pix` in sample `n` of dropout layer `layer`
 __host__ __device__ __forceinline__ void dropout_bits128(uint64_t seed, uint64_t frame, int layer, int n,
                                                          uint32_t pix, int g, uint32_t out[4]) {
-  philox4x32_10(pix, static_cast<uint32_t>(n) | (static_cast<uint32_t>(layer) << 16) | (static_cast<uint32_t>(g) << 24),
-                static_cast<uint32_t>(frame), static_cast<uint32_t>(frame >> 32), static_cast<uint32_t>(seed),
-                static_cast<uint32_t>(seed >> 32), out);
+  dropout_bits128_nl(seed, frame, static_cast<uint32_t>(n) | (static_cast<uint32_t>(layer) << 16), pix, g, out);
 }
 
 }  // namespace sivo

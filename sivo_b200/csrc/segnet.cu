@@ -233,7 +233,7 @@ void SegNet::build(const NetSpec& net, const WeightMap& weights) {
         op.flops = 2.0 * iv.c * ly.kernel * ly.kernel * op.cout * iv.h * iv.w * iv.n;  // algorithmic, whatever the mapping
         op.flops_exec = op.split ? 3.0 * op.flops : op.flops;
         flops_dedup += op.flops;
-        flops_naive += op.flops / iv.n * T_;
+        flops_naive += op.flops / iv.n * ns_;
         if (logits && !opt_.keep_blobs && op.k == 1 && op.cin == 64 && op.cout <= 16 && !op.relu && !bn && !ops_.empty() &&
             ops_.back().kind == Op::Conv && ops_.back().use_tc && ops_.back().out == in && conv_tc_can_fuse_classifier(*ops_.back().tc)) {
           // 1x1 classifier straight after a tensor-core convolution: computed in that convolution's epilogue from the
@@ -348,10 +348,10 @@ void SegNet::build(const NetSpec& net, const WeightMap& weights) {
         }
         if (ly.dropout_ratio != 0.5f)
           fail(SIVO_EFORMAT, "layer '%s': dropout_ratio %.3f (the keep-bit rule is specified for 0.5)", ly.name.c_str(), ly.dropout_ratio);
-        if (!ops_.empty() && ops_.back().kind == Op::Conv && ops_.back().use_tc && ops_.back().out == in && iv.n == T_ &&
+        if (!ops_.empty() && ops_.back().kind == Op::Conv && ops_.back().use_tc && ops_.back().out == in && iv.n == ns_ &&
             iv.dt == DType::F16 && ly.tops[0] == ly.bottoms[0]) {
           // in-place sampling Dropout right after a tensor-core convolution: applied in its epilogue registers
-          conv_tc_set_dropout(*ops_.back().tc, opt_.seed, d_frame_.as<uint64_t>(), drop_idx++, 1.f / (1.f - ly.dropout_ratio));
+          conv_tc_set_dropout(*ops_.back().tc, opt_.seed, d_frame_.as<uint64_t>(), drop_idx++, 1.f / (1.f - ly.dropout_ratio), s0_);
           ops_.back().layer += "+" + ly.name;
           break;
         }
@@ -361,7 +361,7 @@ void SegNet::build(const NetSpec& net, const WeightMap& weights) {
         op.in = in;
         op.drop_layer = drop_idx++;
         op.drop_scale = 1.f / (1.f - ly.dropout_ratio);
-        op.out = add_tensor(ly.tops[0], T_, iv.c, iv.h, iv.w, iv.cs, act_);
+        op.out = add_tensor(ly.tops[0], ns_, iv.c, iv.h, iv.w, iv.cs, act_);
         ops_.push_back(std::move(op));
         break;
       }
@@ -381,7 +381,9 @@ void SegNet::build(const NetSpec& net, const WeightMap& weights) {
   if (!saw_softmax) fail(SIVO_EFORMAT, "prototxt: no Softmax output layer ('prob')");
 }
 
-SegNet::SegNet(const std::string& prototxt, const std::string& caffemodel, const sivo_segnet_options& opt) : opt_(opt) {
+SegNet::SegNet(const std::string& prototxt, const std::string& caffemodel, const sivo_segnet_options& opt, int sample_begin,
+               int sample_count)
+    : opt_(opt) {
   // checkConfig (bayesian_segnet.cpp:80-89)
   if (prototxt.empty()) fail(SIVO_EINVAL, "model_file (.prototxt file) is empty!");
   if (caffemodel.empty()) fail(SIVO_EINVAL, "weights_file (.caffemodel file) is empty!");
@@ -390,6 +392,12 @@ SegNet::SegNet(const std::string& prototxt, const std::string& caffemodel, const
   // bayesian_segnet.cpp:65-70
   if (net.dims[1] != 3) fail(SIVO_EINVAL, "Input layer must have 3 channels!");
   if (T_ <= 1) fail(SIVO_EINVAL, "Input layer must have a batch size greater than 1!");
+  if (sample_count == 0) sample_count = T_;
+  if (sample_begin < 0 || sample_count < 1 || sample_begin > T_ - sample_count)
+    fail(SIVO_EINVAL, "sample range [%d, %d + %d) is not a non-empty part of the frame's %d samples", sample_begin, sample_begin,
+         sample_count, T_);
+  s0_ = sample_begin;
+  ns_ = sample_count;
   H_ = net.dims[2];
   W_ = net.dims[3];
   if (H_ <= 0 || W_ <= 0) fail(SIVO_EFORMAT, "prototxt: bad input geometry %dx%d", W_, H_);
@@ -478,6 +486,7 @@ void SegNet::enqueue(const uint8_t* bgr_dev, uint8_t* classes_dev, double* conf_
         d.seed = opt_.seed;
         d.frame_dev = d_frame_.as<uint64_t>();
         d.layer = op.drop_layer;
+        d.sample0 = s0_;
         launch_dropout(tensors_[op.in]->v, tensors_[op.out]->v, d, op.drop_scale, s);
         break;
       }
@@ -486,15 +495,19 @@ void SegNet::enqueue(const uint8_t* bgr_dev, uint8_t* classes_dev, double* conf_
         d.seed = opt_.seed;
         d.frame_dev = d_frame_.as<uint64_t>();
         d.layer = op.drop_layer;
+        d.sample0 = s0_;
         const Tensor& mt = *tensors_[op.in2];
-        launch_dropout_unpool(tensors_[op.in]->v, T_, mt.buf.as<uint8_t>(), mt.v.n, tensors_[op.out]->v, d, op.drop_scale, s);
+        launch_dropout_unpool(tensors_[op.in]->v, ns_, mt.buf.as<uint8_t>(), mt.v.n, tensors_[op.out]->v, d, op.drop_scale, s);
         break;
       }
       case Op::Reduce: {
-        if (skip_reduce_) break;
+        if (reduce_ == ReduceMode::Skip) break;
         const TensorView& lv = tensors_[op.in]->v;
-        launch_mc_reduce(static_cast<const float*>(lv.p), lv.n, lv.c, lv.cs, lv.h * lv.w, classes_dev, conf_dev, ent_dev, s, 0, -1,
-                         d_frame_.as<FrameArgs>());
+        if (reduce_ == ReduceMode::Partial)
+          launch_mc_partial(static_cast<const float*>(lv.p), lv.n, lv.c, lv.cs, lv.h * lv.w, s, d_frame_.as<FrameArgs>());
+        else
+          launch_mc_reduce(static_cast<const float*>(lv.p), lv.n, lv.c, lv.cs, lv.h * lv.w, classes_dev, conf_dev, ent_dev, s, 0, -1,
+                           d_frame_.as<FrameArgs>());
         break;
       }
     }
@@ -540,17 +553,62 @@ void SegNet::semantic_keys(const sivo_keypoint* kps, int n, int max_static_class
   if (n_keep) *n_keep = kept;
 }
 
+void SegNet::require_whole_frame(const char* what) const {
+  if (ns_ < T_)
+    fail(SIVO_EINVAL, "%s: this handle is a latency-mode shard owning samples [%d, %d) of %d; run it with "
+                      "sivo_segnet_run_partial_device and turn the sum over all shards into maps with sivo_segnet_finalize_device",
+         what, s0_, s0_ + ns_, T_);
+}
+
 void SegNet::run_device(const uint8_t* bgr_dev, uint8_t* classes_dev, double* conf_dev, double* ent_dev, cudaStream_t s, float* conf32_dev,
                         float* ent32_dev) {
+  require_whole_frame("run_device");
   SIVO_CUDA(cudaSetDevice(device_));
   if (!s) s = stream_;
   last_classes_ = classes_dev; last_conf_ = conf_dev; last_ent_ = ent_dev; last_stream_ = s;
+  FrameArgs fa{};
+  fa.frame = frame_++;
+  fa.bgr = bgr_dev; fa.classes = classes_dev; fa.conf = conf_dev; fa.ent = ent_dev; fa.conf32 = conf32_dev; fa.ent32 = ent32_dev;
+  launch_frame(fa, s);
+}
+
+void SegNet::run_partial(const uint8_t* bgr_dev, double* sum_dev, cudaStream_t s) {
+  if (!bgr_dev || !sum_dev) fail(SIVO_EINVAL, "run_partial: null image or sum buffer");
+  const TensorView& lv = tensors_[ops_.back().in]->v;  // the op list ends with the Reduce op (build() checks for the Softmax)
+  if (lv.cs != 16 || lv.c > 16)
+    fail(SIVO_EFORMAT, "run_partial: the partial sum needs the 16-channel logits layout (at most 16 classes, this net has %d)", lv.c);
+  SIVO_CUDA(cudaSetDevice(device_));
+  if (!s) s = stream_;
+  FrameArgs fa{};
+  fa.frame = frame_++;  // advances exactly as run_device does, so the shards of one frame stay in lockstep
+  fa.bgr = bgr_dev; fa.sum = sum_dev;
+  reduce_ = ReduceMode::Partial;
+  try {
+    launch_frame(fa, s);
+  } catch (...) {
+    reduce_ = ReduceMode::Full;
+    throw;
+  }
+  reduce_ = ReduceMode::Full;
+}
+
+void SegNet::finalize(const double* sum_dev, uint8_t* classes_dev, double* conf_dev, double* ent_dev, float* conf32_dev, float* ent32_dev,
+                      cudaStream_t s) {
+  if (!sum_dev) fail(SIVO_EINVAL, "finalize: null sum buffer");
+  SIVO_CUDA(cudaSetDevice(device_));
+  if (!s) s = stream_;
+  launch_mc_finalize(sum_dev, T_, n_classes_, H_ * W_, classes_dev, conf_dev, ent_dev, conf32_dev, ent32_dev, s);
+  last_classes_ = classes_dev; last_conf_ = conf_dev; last_ent_ = ent_dev; last_stream_ = s;  // semantic_keys reads these maps
+}
+
+void SegNet::launch_frame(FrameArgs fa, cudaStream_t s) {
+  const uint8_t* bgr_dev = fa.bgr;
+  uint8_t* classes_dev = fa.classes;
+  double* conf_dev = fa.conf;
+  double* ent_dev = fa.ent;
   // Everything that changes per frame -- the dropout frame counter and the caller's pointers -- goes to the device by value,
   // outside the captured graph (pipelined callers may issue the next frame before this one has started), so one graph per
   // stream serves every pointer set a caller cycles through
-  FrameArgs fa;
-  fa.frame = frame_++;
-  fa.bgr = bgr_dev; fa.classes = classes_dev; fa.conf = conf_dev; fa.ent = ent_dev; fa.conf32 = conf32_dev; fa.ent32 = ent32_dev;
   launch_set_frame_args(d_frame_.as<FrameArgs>(), fa, s);
   if (profiling_) {
     while (events_.size() < ops_.size() + 1) {
@@ -581,7 +639,7 @@ void SegNet::run_device(const uint8_t* bgr_dev, uint8_t* classes_dev, double* co
   if (graphs_enabled && graph_ok_ && all_tc) {
     // the graph's kernels read the image / result pointers from FrameArgs: the key is the stream (and the op-list variant) only
     const void* key[5] = {nullptr, nullptr, nullptr, nullptr,
-                          reinterpret_cast<const void*>(reinterpret_cast<uintptr_t>(s) ^ (skip_reduce_ ? 1u : 0u))};
+                          reinterpret_cast<const void*>(reinterpret_cast<uintptr_t>(s) ^ static_cast<uintptr_t>(reduce_))};
     cudaGraphExec_t graph_exec_ = nullptr;
     for (size_t i = 0; i < graphs_.size(); ++i)
       if (memcmp(key, graphs_[i].key, sizeof key) == 0) {
@@ -629,6 +687,7 @@ void SegNet::run_device(const uint8_t* bgr_dev, uint8_t* classes_dev, double* co
 }
 
 void SegNet::run_host(const uint8_t* bgr, int rows, int cols, size_t stride, uint8_t* classes, double* conf, double* ent) {
+  require_whole_frame("segmentImage");
   if (!bgr) fail(SIVO_EINVAL, "segmentImage: null image");
   // resizeImage (bayesian_segnet.cpp:142-162): exact size passes through, larger is centre-cropped;
   // smaller yields an empty Mat in the reference (and a crash downstream) -- here an error.
@@ -676,14 +735,14 @@ void SegNet::run_host(const uint8_t* bgr, int rows, int cols, size_t stride, uin
       SIVO_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
       band_ev_.push_back(e);
     }
-    skip_reduce_ = true;
+    reduce_ = ReduceMode::Skip;
     try {
       run_device(d_bgr_.as<uint8_t>(), d_classes_.as<uint8_t>(), d_conf_.as<double>(), d_ent_.as<double>(), stream_);
     } catch (...) {
-      skip_reduce_ = false;
+      reduce_ = ReduceMode::Full;
       throw;
     }
-    skip_reduce_ = false;
+    reduce_ = ReduceMode::Full;
     for (int b = 0; b < n_bands; ++b) {
       const int r0 = static_cast<int>(static_cast<long>(H_) * b / n_bands), r1 = static_cast<int>(static_cast<long>(H_) * (b + 1) / n_bands);
       const size_t p0 = static_cast<size_t>(r0) * W_, np = static_cast<size_t>(r1 - r0) * W_;

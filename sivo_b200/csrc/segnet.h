@@ -58,11 +58,16 @@ struct Op {
 
 class SegNet {
  public:
-  SegNet(const std::string& prototxt, const std::string& caffemodel, const sivo_segnet_options& opt);
+  // sample_count 0: the whole frame, samples [0, T).  Otherwise a latency-mode shard owning samples
+  // [sample_begin, sample_begin + sample_count) of a frame of T (= opt.T or the prototxt's batch) samples.
+  SegNet(const std::string& prototxt, const std::string& caffemodel, const sivo_segnet_options& opt, int sample_begin = 0,
+         int sample_count = 0);
   ~SegNet();
   int width() const { return W_; }
   int height() const { return H_; }
   int T() const { return T_; }
+  int sample_begin() const { return s0_; }
+  int sample_count() const { return ns_; }
   int classes() const { return n_classes_; }
   void set_frame(uint64_t f) { frame_ = f; }
   void run_host(const uint8_t* bgr, int rows, int cols, size_t stride, uint8_t* classes, double* conf, double* ent);
@@ -74,6 +79,11 @@ class SegNet {
   // conf32 / ent32 (optional): single-precision copies of the two maps, e.g. straight into the packed multi-GPU record
   void run_device(const uint8_t* bgr_dev, uint8_t* classes_dev, double* conf_dev, double* ent_dev, cudaStream_t s, float* conf32_dev = nullptr,
                   float* ent32_dev = nullptr);
+  // latency mode: the shard's samples through the net, then sum_dev[H*W][16] (double) = their sum of per-sample softmax
+  void run_partial(const uint8_t* bgr_dev, double* sum_dev, cudaStream_t s);
+  // the maps from a sum over all T samples of the frame (e.g. the shards' sums reduced over ranks); any output may be NULL
+  void finalize(const double* sum_dev, uint8_t* classes_dev, double* conf_dev, double* ent_dev, float* conf32_dev, float* ent32_dev,
+                cudaStream_t s);
   void semantic_keys(const sivo_keypoint* kps, int n, int max_static_class, uint8_t* kp_class, double* kp_conf, double* kp_entropy,
                      int* keep_idx, int* n_keep);
   void blob(const std::string& name, float* out, size_t cap, int* n, int* c, int* h, int* w);
@@ -90,9 +100,13 @@ class SegNet {
   void build(const NetSpec& net, const WeightMap& weights);
   void prepare_conv(Op& op, const std::vector<Blob>& conv_blobs, const std::vector<Blob>* bn_blobs);
   void enqueue(const uint8_t* bgr_dev, uint8_t* classes_dev, double* conf_dev, double* ent_dev, cudaStream_t s, bool timed);
+  // one frame of the op list (graph replay or plain launches) with the per-frame arguments `fa`, ending as reduce_ says
+  void launch_frame(FrameArgs fa, cudaStream_t s);
+  void require_whole_frame(const char* what) const;
 
   sivo_segnet_options opt_;
-  int device_ = 0, T_ = 0, H_ = 0, W_ = 0, n_classes_ = 0;
+  // T_: samples of the frame (the mean divides by it); this handle runs samples [s0_, s0_ + ns_) (ns_ = T_ unless a shard)
+  int device_ = 0, T_ = 0, H_ = 0, W_ = 0, n_classes_ = 0, s0_ = 0, ns_ = 0;
   DType act_ = DType::F16;
   uint64_t frame_ = 0;
   bool profiling_ = false;
@@ -119,7 +133,10 @@ class SegNet {
   bool graph_ok_ = true;
   // segmentImage read-back overlap: the MC reduction runs in row bands and each band's slices of the three maps start their
   // device-to-host copy on a second stream while the next band is reduced
-  bool skip_reduce_ = false;      // set by run_host around run_device: the op list stops before the Reduce op
+  // how the op list's Reduce op runs: the full MC reduction; skipped (set by run_host around run_device when it reduces in row
+  // bands); or the latency-mode partial sum (run_partial).  Each is its own captured graph.
+  enum class ReduceMode : uintptr_t { Full = 0, Skip = 1, Partial = 2 };
+  ReduceMode reduce_ = ReduceMode::Full;
   cudaStream_t copy_stream_ = nullptr;
   std::vector<cudaEvent_t> band_ev_;
   // device-resident copies run_host leaves for a packed multi-GPU record (set_record_outputs)
@@ -133,7 +150,8 @@ bool conv_tc_supported(const Op& op, const TensorView& in, const TensorView& out
 std::shared_ptr<ConvTcPlan> conv_tc_plan(const Op& op, const TensorView& in, const TensorView& out, const void* w_tc);
 void conv_tc_launch(const ConvTcPlan& plan, const Op& op, cudaStream_t s);
 // fuses the sampling Dropout that follows the convolution in place into its epilogue
-void conv_tc_set_dropout(ConvTcPlan& plan, uint64_t seed, const uint64_t* frame_dev, int layer, float scale);
+// (sample0: global MC sample index of the batch's image 0, so that a shard handle draws the masks of its own samples)
+void conv_tc_set_dropout(ConvTcPlan& plan, uint64_t seed, const uint64_t* frame_dev, int layer, float scale, int sample0);
 // fuses the max-unpool (Upsample) that consumes the convolution's output into its epilogue; `out_2h_2w` is the
 // unpooled tensor the convolution then writes instead of its own output
 void conv_tc_set_unpool(ConvTcPlan& plan, const uint8_t* mask, int mask_n, void* out_2h_2w);

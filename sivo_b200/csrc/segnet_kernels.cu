@@ -192,7 +192,7 @@ __global__ void k_unpool(const AT* __restrict__ in, const uint8_t* __restrict__ 
 // ---- test-time dropout sampling (dropout_layer.cpp:31-46): y = x * keep * 1/(1-ratio).
 template <typename AT>
 __global__ void k_dropout(const AT* __restrict__ in, int in_n, AT* __restrict__ out, int N, int HW, int cs, int C,
-                          uint64_t seed, const uint64_t* __restrict__ frame, int layer, float scale) {
+                          uint64_t seed, const uint64_t* __restrict__ frame, int layer, int n0, float scale) {
   size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;  // one thread per (n, pix, 32-ch word)
   int words = (cs + 31) / 32;
   size_t total = static_cast<size_t>(N) * HW * words;
@@ -202,7 +202,7 @@ __global__ void k_dropout(const AT* __restrict__ in, int in_n, AT* __restrict__ 
   uint32_t pix = r % HW;
   int n = r / HW;
   uint32_t bits[4];
-  dropout_bits128(seed, *frame, layer, n, pix, wd >> 2, bits);
+  dropout_bits128(seed, *frame, layer, n0 + n, pix, wd >> 2, bits);
   uint32_t b = bits[wd & 3];
   const AT* s = in + (static_cast<size_t>(n % in_n) * HW + pix) * cs + wd * 32;
   AT* d = out + (static_cast<size_t>(n) * HW + pix) * cs + wd * 32;
@@ -218,7 +218,7 @@ __global__ void k_dropout(const AT* __restrict__ in, int in_n, AT* __restrict__ 
 // is scattered straight into the 2x2 block its pooling mask names (dropout -> upsample pair of the decoder entry).
 template <bool UNPOOL>
 __global__ void k_dropout_h8(const uint4* __restrict__ in, int in_n, uint4* __restrict__ out, int N, int Hi, int Wi, int cs,
-                             uint64_t seed, const uint64_t* __restrict__ frame, int layer, float scale,
+                             uint64_t seed, const uint64_t* __restrict__ frame, int layer, int n0, float scale,
                              const uint8_t* __restrict__ mask, int mask_n) {
   const size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   const int chunks = cs >> 3;
@@ -229,7 +229,7 @@ __global__ void k_dropout_h8(const uint4* __restrict__ in, int in_n, uint4* __re
   const uint32_t pix = static_cast<uint32_t>(r % HW);
   const int n = static_cast<int>(r / HW);
   uint32_t bits[4];
-  dropout_bits128(seed, *frame, layer, n, pix, ch >> 4, bits);
+  dropout_bits128(seed, *frame, layer, n0 + n, pix, ch >> 4, bits);
   const uint32_t b = (bits[(ch >> 2) & 3] >> ((ch & 3) * 8)) & 0xFFu;
   const uint4 v = __ldg(in + (static_cast<size_t>(n % in_n) * HW + pix) * chunks + ch);
   const uint32_t w[4] = {v.x, v.y, v.z, v.w};
@@ -329,20 +329,15 @@ __global__ void k_mc_reduce(const float* __restrict__ logits, int T, int cs, int
 // Same reduction with four lanes per pixel (one float4 = 4 classes each): a warp reads 512 contiguous bytes per
 // sample and there are 4x more threads in flight, which is what this HBM-bound pass needs.  The softmax max / sum and
 // the final argmax / entropy are combined with xor-shuffles inside the 4-lane group (first maximum still wins).
-__global__ void k_mc_reduce_quad(const float* __restrict__ logits, int T, int C, int hw, uint8_t* __restrict__ classes,
-                                 double* __restrict__ conf, double* __restrict__ entropy, int pix0, int pix_end,
-                                 const FrameArgs* __restrict__ args) {
-  float *conf32 = nullptr, *ent32 = nullptr;
-  if (args) { classes = args->classes; conf = args->conf; entropy = args->ent; conf32 = args->conf32; ent32 = args->ent32; }
-  // Instruction diet (ncu: the first version was issue-bound at 3400 instructions per warp, 0.8 TB/s): one IEEE
-  // reciprocal per sample instead of C divisions (p = e * (1/sum), <= 1 ulp from e/sum), mean = acc * (1/T) in double,
-  // and log2 evaluated in float on the double mean (relative error < 2^-22, i.e. < 1e-6 on the entropy, against the
-  // 1e-4 the contract allows); the products and the sums stay in double like computeEntropy (bayesian_segnet.cpp:38-44).
-  const int gid = blockIdx.x * blockDim.x + threadIdx.x;
-  const int pix = pix0 + (gid >> 2), q = gid & 3;
-  const bool live = pix < pix_end;
-  const int pp = live ? pix : hw - 1;
-  double acc[4] = {0.0, 0.0, 0.0, 0.0};
+// Instruction diet (ncu: the first version was issue-bound at 3400 instructions per warp, 0.8 TB/s): one IEEE
+// reciprocal per sample instead of C divisions (p = e * (1/sum), <= 1 ulp from e/sum), mean = acc * (1/T) in double,
+// and log2 evaluated in float on the double mean (relative error < 2^-22, i.e. < 1e-6 on the entropy, against the
+// 1e-4 the contract allows); the products and the sums stay in double like computeEntropy (bayesian_segnet.cpp:38-44).
+// The two halves below are shared by the one-pass kernel and the latency-mode pair (partial sum / finalize), so all three
+// perform the same operations in the same order.
+
+// lane q of pixel pp: acc[j] += softmax(logits[t][pp])[4q + j] in double, samples t = 0 .. T-1 in order
+__device__ __forceinline__ void quad_softmax_sum(const float* __restrict__ logits, int T, int C, int hw, int pp, int q, double (&acc)[4]) {
   constexpr int kBatch = 6;  // samples whose loads are issued together (memory-level parallelism: the pass is HBM-bound)
   for (int t0 = 0; t0 < T; t0 += kBatch) {
   float4 vb[kBatch];
@@ -372,6 +367,11 @@ __global__ void k_mc_reduce_quad(const float* __restrict__ logits, int T, int C,
     for (int j = 0; j < 4; ++j) acc[j] += static_cast<double>(__fmul_rn(x[j], inv));
   }
   }
+}
+
+// mean = acc / T, first-max argmax and entropy across the 4-lane group; lane 0 of a live pixel writes the maps
+__device__ __forceinline__ void quad_finalize(const double (&acc)[4], int T, int C, int q, int pix, bool live, uint8_t* classes,
+                                              double* conf, double* entropy, float* conf32, float* ent32) {
   const double inv_t = 1.0 / static_cast<double>(T);
   double best = -1.0, ent = 0.0;
   int arg = 0;
@@ -397,6 +397,50 @@ __global__ void k_mc_reduce_quad(const float* __restrict__ logits, int T, int C,
     if (conf32) conf32[pix] = static_cast<float>(best);
     if (ent32) ent32[pix] = static_cast<float>(ent);
   }
+}
+
+__global__ void k_mc_reduce_quad(const float* __restrict__ logits, int T, int C, int hw, uint8_t* __restrict__ classes,
+                                 double* __restrict__ conf, double* __restrict__ entropy, int pix0, int pix_end,
+                                 const FrameArgs* __restrict__ args) {
+  float *conf32 = nullptr, *ent32 = nullptr;
+  if (args) { classes = args->classes; conf = args->conf; entropy = args->ent; conf32 = args->conf32; ent32 = args->ent32; }
+  const int gid = blockIdx.x * blockDim.x + threadIdx.x;
+  const int pix = pix0 + (gid >> 2), q = gid & 3;
+  const bool live = pix < pix_end;
+  const int pp = live ? pix : hw - 1;
+  double acc[4] = {0.0, 0.0, 0.0, 0.0};
+  quad_softmax_sum(logits, T, C, hw, pp, q, acc);
+  quad_finalize(acc, T, C, q, pix, live, classes, conf, entropy, conf32, ent32);
+}
+
+// Latency mode, first half: the shard's sum of per-sample softmax, [hw][16] double (lane q owns channels 4q .. 4q+3)
+__global__ void k_mc_partial_quad(const float* __restrict__ logits, int T, int C, int hw, const FrameArgs* __restrict__ args) {
+  double* __restrict__ sum = args->sum;
+  const int gid = blockIdx.x * blockDim.x + threadIdx.x;
+  const int pix = gid >> 2, q = gid & 3;
+  const bool live = pix < hw;
+  const int pp = live ? pix : hw - 1;
+  double acc[4] = {0.0, 0.0, 0.0, 0.0};
+  quad_softmax_sum(logits, T, C, hw, pp, q, acc);
+  if (live) {
+    double2* o = reinterpret_cast<double2*>(sum + static_cast<size_t>(pix) * 16 + 4 * q);
+    o[0] = make_double2(acc[0], acc[1]);
+    o[1] = make_double2(acc[2], acc[3]);
+  }
+}
+
+// Latency mode, second half: the maps from the sum over all T_total samples of the frame
+__global__ void k_mc_finalize_quad(const double* __restrict__ sum, int T_total, int C, int hw, uint8_t* __restrict__ classes,
+                                   double* __restrict__ conf, double* __restrict__ entropy, float* __restrict__ conf32,
+                                   float* __restrict__ ent32) {
+  const int gid = blockIdx.x * blockDim.x + threadIdx.x;
+  const int pix = gid >> 2, q = gid & 3;
+  const bool live = pix < hw;
+  const int pp = live ? pix : hw - 1;
+  const double2* s = reinterpret_cast<const double2*>(sum + static_cast<size_t>(pp) * 16 + 4 * q);
+  const double2 a = __ldg(s), b = __ldg(s + 1);
+  const double acc[4] = {a.x, a.y, b.x, b.y};
+  quad_finalize(acc, T_total, C, q, pix, live, classes, conf, entropy, conf32, ent32);
 }
 
 __global__ void k_mc_reduce_generic(const float* __restrict__ logits, int T, int C, int cs, int hw,
@@ -717,7 +761,8 @@ void launch_dropout(TensorView in, TensorView out, const DropoutParams& d, float
   if (in.dt == DType::F16 && out.dt == DType::F16 && out.cs % 8 == 0 && out.c == out.cs && in.cs == out.cs) {
     const size_t total = static_cast<size_t>(out.n) * out.h * out.w * (out.cs / 8);
     k_dropout_h8<false><<<blocks_for(total, 256), 256, 0, s>>>(static_cast<const uint4*>(in.p), in.n, static_cast<uint4*>(out.p), out.n,
-                                                            out.h, out.w, out.cs, d.seed, d.frame_dev, d.layer, scale, nullptr, 1);
+                                                            out.h, out.w, out.cs, d.seed, d.frame_dev, d.layer, d.sample0, scale,
+                                                            nullptr, 1);
     SIVO_CUDA(cudaGetLastError());
     return;
   }
@@ -725,7 +770,8 @@ void launch_dropout(TensorView in, TensorView out, const DropoutParams& d, float
   size_t total = static_cast<size_t>(out.n) * out.h * out.w * words;
   DISPATCH_AT(in.dt, (k_dropout<AT><<<blocks_for(total, 256), 256, 0, s>>>(static_cast<const AT*>(in.p), in.n,
                                                                            static_cast<AT*>(out.p), out.n, out.h * out.w,
-                                                                           out.cs, out.c, d.seed, d.frame_dev, d.layer, scale)));
+                                                                           out.cs, out.c, d.seed, d.frame_dev, d.layer, d.sample0,
+                                                                           scale)));
   SIVO_CUDA(cudaGetLastError());
 }
 
@@ -736,7 +782,7 @@ void launch_dropout_unpool(TensorView in, int T, const uint8_t* mask, int mask_n
     fail(SIVO_EINVAL, "dropout+unpool: unexpected tensor layout");
   const size_t total = static_cast<size_t>(T) * in.h * in.w * (in.cs / 8);
   k_dropout_h8<true><<<blocks_for(total, 256), 256, 0, s>>>(static_cast<const uint4*>(in.p), in.n, static_cast<uint4*>(out.p), T, in.h, in.w,
-                                                         in.cs, d.seed, d.frame_dev, d.layer, scale, mask, mask_n);
+                                                         in.cs, d.seed, d.frame_dev, d.layer, d.sample0, scale, mask, mask_n);
   SIVO_CUDA(cudaGetLastError());
 }
 
@@ -753,6 +799,19 @@ void launch_mc_reduce(const float* logits, int T, int C, int cs, int hw, uint8_t
   if (pix0 != 0 || npix != hw) fail(SIVO_EINVAL, "mc_reduce: pixel ranges need the 16-channel logits layout");
   if (C == 15) k_mc_reduce<15><<<blocks_for(hw, 128), 128, 0, s>>>(logits, T, cs, hw, classes, conf, entropy, args);
   else k_mc_reduce_generic<<<blocks_for(hw, 128), 128, 0, s>>>(logits, T, C, cs, hw, classes, conf, entropy, args);
+  SIVO_CUDA(cudaGetLastError());
+}
+
+void launch_mc_partial(const float* logits, int T, int C, int cs, int hw, cudaStream_t s, const FrameArgs* args) {
+  if (cs != 16 || C > 16) fail(SIVO_EFORMAT, "mc_partial: the latency-mode partial sum needs the 16-channel logits layout (C <= 16)");
+  k_mc_partial_quad<<<blocks_for(static_cast<size_t>(hw) * 4, 256), 256, 0, s>>>(logits, T, C, hw, args);
+  SIVO_CUDA(cudaGetLastError());
+}
+
+void launch_mc_finalize(const double* sum, int T_total, int C, int hw, uint8_t* classes, double* conf, double* entropy, float* conf32,
+                        float* ent32, cudaStream_t s) {
+  if (C > 16) fail(SIVO_EFORMAT, "mc_finalize: the latency-mode sum layout holds at most 16 classes");
+  k_mc_finalize_quad<<<blocks_for(static_cast<size_t>(hw) * 4, 256), 256, 0, s>>>(sum, T_total, C, hw, classes, conf, entropy, conf32, ent32);
   SIVO_CUDA(cudaGetLastError());
 }
 

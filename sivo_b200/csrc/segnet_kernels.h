@@ -41,12 +41,14 @@ struct FrameArgs {
   double* ent;
   float* conf32;         // optional single-precision copies of the two maps (the packed multi-GPU record carries those)
   float* ent32;
+  double* sum;           // latency mode: [H*W][16] per-pixel sum of the shard's per-sample softmax (k_mc_partial_quad)
 };
 
 struct DropoutParams {
   uint64_t seed = 0;
   const uint64_t* frame_dev = nullptr;  // device scalar, so a captured graph replays with a new frame
   int layer = 0;
+  int sample0 = 0;  // global MC sample index of local sample 0 (a shard handle owns samples [sample0, sample0 + N))
 };
 
 // `args` != nullptr: the image / result pointers are read from *args on the device instead of the by-value arguments
@@ -78,6 +80,13 @@ void launch_dropout(TensorView in, TensorView out, const DropoutParams& d, float
 // pix0 / npix restrict the pass to pixels [pix0, pix0 + npix) (npix < 0: all of them)
 void launch_mc_reduce(const float* logits, int T, int C, int cs, int hw, uint8_t* classes, double* conf,
                       double* entropy, cudaStream_t s, int pix0 = 0, int npix = -1, const FrameArgs* args = nullptr);
+// Latency mode, the MC reduction cut in two.  Partial: sum[pix][16] (double) = sum over the T local samples of softmax(logits),
+// channels >= C zero; the sum pointer is read from args->sum.  Finalize: the maps of launch_mc_reduce from a sum over all
+// T_total samples of the frame.  Both need the 16-channel logits layout; partial over [0, T) then finalize equals
+// launch_mc_reduce bit for bit.
+void launch_mc_partial(const float* logits, int T, int C, int cs, int hw, cudaStream_t s, const FrameArgs* args);
+void launch_mc_finalize(const double* sum, int T_total, int C, int hw, uint8_t* classes, double* conf, double* entropy, float* conf32,
+                        float* ent32, cudaStream_t s);
 void launch_dropout_bits(uint64_t seed, const uint64_t* frame_dev, int layer, int T, int C, int H, int W,
                          uint8_t* keep_nchw, cudaStream_t s);
 // layout converters for the test hooks (float NCHW host order <-> NHWC activation)

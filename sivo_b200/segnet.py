@@ -20,22 +20,48 @@ class BayesianSegNetParams:
     use_gpu: bool = True  # kept for signature parity; this backend is GPU only
 
 
+def sample_ranges(T: int, G: int):
+    """Latency mode: the T Monte-Carlo samples of a frame split over G ranks as contiguous (begin, count) blocks whose sizes
+    differ by at most one, larger blocks first -- e.g. T=6, G=4 -> [(0, 2), (2, 2), (4, 1), (5, 1)]."""
+    if T < 1 or G < 1:
+        raise ValueError(f"sample_ranges: T={T} and G={G} must both be >= 1")
+    if G > T:
+        raise ValueError(f"sample_ranges: {G} ranks for {T} samples would leave a rank without a sample")
+    base, extra = divmod(T, G)
+    out, b = [], 0
+    for g in range(G):
+        n = base + (1 if g < extra else 0)
+        out.append((b, n))
+        b += n
+    return out
+
+
 class BayesianSegNet:
     def __init__(self, params: BayesianSegNetParams, device: int = 0, seed: int = 1234, T: int = 0,
-                 precision: str = "fp16", engine: str = "auto", keep_blobs: bool = False):
+                 precision: str = "fp16", engine: str = "auto", keep_blobs: bool = False, samples=None):
+        """`samples` = (begin, count): a latency-mode shard that runs only the samples [begin, begin + count) of a frame of T;
+        run it with run_partial() and turn the sum over all shards into maps with finalize()."""
         self._h = C.c_void_p()
         opt = L.SegnetOptions(device=device, T=T, seed=seed,
                               precision={"fp16": L.PRECISION_FP16, "fp32": L.PRECISION_FP32}[precision],
                               engine={"auto": L.ENGINE_AUTO, "simt": L.ENGINE_SIMT, "tcgen05": L.ENGINE_TCGEN05}[engine],
                               keep_blobs=int(keep_blobs), reserved=0)
-        rc = L.lib().sivo_segnet_create_ex(params.model_file.encode(), params.weights_file.encode(), C.byref(opt),
-                                           C.byref(self._h))
+        if samples is None:
+            rc = L.lib().sivo_segnet_create_ex(params.model_file.encode(), params.weights_file.encode(), C.byref(opt),
+                                               C.byref(self._h))
+        else:
+            begin, count = samples
+            rc = L.lib().sivo_segnet_create_shard(params.model_file.encode(), params.weights_file.encode(), C.byref(opt),
+                                                  int(begin), int(count), C.byref(self._h))
         if rc == L.EINVAL:  # the reference throws std::invalid_argument (bayesian_segnet.cpp:66,68,82,86)
             raise ValueError(L.lib().sivo_last_error().decode())
         L.check(rc)
         w, h, t, nc = C.c_int(), C.c_int(), C.c_int(), C.c_int()
         L.check(L.lib().sivo_segnet_geometry(self._h, C.byref(w), C.byref(h), C.byref(t), C.byref(nc)))
         self.width, self.height, self.T, self.n_classes = w.value, h.value, t.value, nc.value
+        b, n = C.c_int(), C.c_int()
+        L.check(L.lib().sivo_segnet_samples(self._h, C.byref(b), C.byref(n), None))
+        self.sample_begin, self.sample_count = b.value, n.value
 
     def __del__(self):
         if getattr(self, "_h", None) and self._h.value and L is not None and getattr(L, "lib", None):
@@ -115,6 +141,19 @@ class BayesianSegNet:
         """run_device plus single-precision copies of the two maps (the packed multi-GPU record's layout); any pointer may be 0."""
         L.check(L.lib().sivo_segnet_run_device_maps(self._h, C.c_void_p(bgr_ptr), C.c_void_p(classes_ptr), C.c_void_p(conf_ptr),
                                                     C.c_void_p(ent_ptr), C.c_void_p(conf32_ptr), C.c_void_p(ent32_ptr), C.c_void_p(stream)))
+
+    def run_partial(self, bgr_ptr: int, sum_ptr: int, stream: int = 0):
+        """Latency mode: this handle's samples of the frame at bgr_ptr (device, height x width x 3 u8); sum_ptr (device,
+        height*width x 16 float64) receives their sum of per-sample softmax.  Advances the frame counter like run_device."""
+        L.check(L.lib().sivo_segnet_run_partial_device(self._h, C.c_void_p(bgr_ptr), C.c_void_p(sum_ptr), C.c_void_p(stream)))
+
+    def finalize(self, sum_ptr: int, classes_ptr: int, conf_ptr: int, ent_ptr: int, conf32_ptr: int = 0, ent32_ptr: int = 0,
+                 stream: int = 0):
+        """Latency mode: the maps of run_device_maps from sum_ptr = the sum over ALL T samples (e.g. reduced over the ranks'
+        run_partial sums); any output pointer may be 0."""
+        L.check(L.lib().sivo_segnet_finalize_device(self._h, C.c_void_p(sum_ptr), C.c_void_p(classes_ptr), C.c_void_p(conf_ptr),
+                                                    C.c_void_p(ent_ptr), C.c_void_p(conf32_ptr), C.c_void_p(ent32_ptr),
+                                                    C.c_void_p(stream)))
 
     def blob(self, name: str) -> np.ndarray:
         n, c, h, w = C.c_int(), C.c_int(), C.c_int(), C.c_int()
