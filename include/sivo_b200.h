@@ -8,6 +8,7 @@
  *                             ctor                             src/bayesian_segnet/bayesian_segnet.cpp:46-78
  *                             segmentImage                     src/bayesian_segnet/bayesian_segnet.cpp:299-318
  *                             getInputGeometry                 include/bayesian_segnet/bayesian_segnet.hpp:139
+ *                             computeVariance                  src/bayesian_segnet/bayesian_segnet.cpp:205-260
  *   sivo_orb_*      replaces  SIVO::ORBextractor              include/orbslam/ORBextractor.h:46-125
  *                             ctor                             src/orbslam/ORBextractor.cc:412-475
  *                             operator()                       src/orbslam/ORBextractor.cc:1019-1083
@@ -115,6 +116,28 @@ int sivo_segnet_run_partial_device(sivo_segnet_t* h, const uint8_t* bgr_device, 
  * counter.  On `stream` (NULL = the handle's own), no host synchronisation; SIVO_EINVAL for a NULL sum. */
 int sivo_segnet_finalize_device(sivo_segnet_t* h, const double* sum_device, uint8_t* classes_device, double* confidence_device,
                                 double* entropy_device, float* confidence_f32_device, float* entropy_f32_device, void* stream);
+/* ---- Monte-Carlo variance (BayesianSegNet::computeVariance, bayesian_segnet.cpp:205-260) ------------------------------
+ * Per pixel, with c = classes[row * width + col] (normally the class map the same frame's run returned) and p_t the softmax
+ * probability of class c in sample t of the LAST FRAME RUN ON THE HANDLE: avg = sum_t p_t / T and variance = sum_t (p_t - avg)^2
+ * / (T - 1), the sample variance, summed in double in sample order.  Two rules the reference leaves open: a class >= n_classes
+ * (e.g. VOID = 255) gives 0, and p_t is computed with the per-sample arithmetic of the reduction the handle runs, so for the
+ * argmax class avg is the mean `confidence` reports.  The samples never leave the device, so only these calls can compute it.
+ * They do not touch the frame counter.  SIVO_EINVAL for a NULL buffer or a handle that has not run a frame yet.
+ *
+ * Host form: classes (u8) and variance (double) are row-major height x width host buffers; returns when done.  SIVO_EINVAL on
+ * a latency-mode shard owning fewer than T samples. */
+int sivo_segnet_variance(sivo_segnet_t* h, const uint8_t* classes, double* variance);
+/* The same with device buffers on `stream` (NULL = the handle's own), no host synchronisation.  The call must be ordered after
+ * the run whose samples it reads (the same stream, or a stream that waits on it) and before the handle's next run, which
+ * overwrites them. */
+int sivo_segnet_variance_device(sivo_segnet_t* h, const uint8_t* classes_device, double* variance_device, void* stream);
+/* Latency mode: moments_device (height*width x 2 doubles, pixel-major) = (sum p_t, sum p_t^2) of class c over this shard's
+ * samples of its last sivo_segnet_run_partial_device ((0, 0) where c >= n_classes); ordered as above.  SIVO_EFORMAT if the
+ * net's logits do not have the 16-channel layout (more than 16 classes), as sivo_segnet_run_partial_device. */
+int sivo_segnet_variance_partial_device(sivo_segnet_t* h, const uint8_t* classes_device, double* moments_device, void* stream);
+/* moments_device: the moments summed over ALL T samples of the frame (e.g. reduced over the ranks).  variance_device =
+ * max(0, (S2 - S1^2 / T) / (T - 1)); agrees with the two-pass form to rounding (about 1e-16 for probabilities). */
+int sivo_segnet_variance_finalize_device(sivo_segnet_t* h, const double* moments_device, double* variance_device, void* stream);
 /* Test hook: copies blob `name` (any top in the prototxt; needs keep_blobs) to `out` as float NCHW.
  * `*n`, `*c`, `*hh`, `*ww` receive its shape; `out` may be NULL to query the shape only. */
 int sivo_segnet_blob(sivo_segnet_t* h, const char* name, float* out, size_t cap, int* n, int* c, int* hh,
@@ -234,6 +257,9 @@ int sivo_dbg_lrn(int device, const float* in, int n, int c, int h, int w, int si
                  float k, float* out);
 int sivo_dbg_mc_reduce(int device, const float* logits, int T, int c, int h, int w, uint8_t* classes,
                        double* confidence, double* entropy);
+/* logits float NCHW [T][c][h][w] (T >= 2) laid out as sivo_dbg_mc_reduce does (c <= 16: the 16-channel layout and the quad
+ * kernel; c > 16: the generic kernel); classes / variance h x w. */
+int sivo_dbg_mc_variance(int device, const float* logits, int T, int c, int h, int w, const uint8_t* classes, double* variance);
 int sivo_dbg_dropout_mask(int device, uint64_t seed, uint64_t frame, int layer, int T, int c, int h, int w,
                           uint8_t* keep);
 

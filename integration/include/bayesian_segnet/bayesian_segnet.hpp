@@ -44,6 +44,10 @@ class BayesianSegNet {
 
     void segmentImage(const cv::Mat &image, MatXu &classes, MatXd &confidence, MatXd &entropy);
     cv::Size getInputGeometry() { return this->input_geometry; }
+    // Private and never called in the reference (bayesian_segnet.hpp, bayesian_segnet.cpp:205-260); public here because the
+    // Monte-Carlo samples stay on the device and only the library can compute it.  Per pixel, the sample variance over the
+    // last segmentImage's T samples of the softmax probability of classes(row, col); 0 where that class does not exist.
+    MatXd computeVariance(const MatXu &classes);
     cv::Mat generateConfidenceImage(const MatXd &confidence);
     cv::Mat generateVarianceImage(MatXd &variance);
     cv::Mat generateEntropyImage(MatXd &entropy);

@@ -42,6 +42,15 @@ void BayesianSegNet::segmentImage(const cv::Mat &image, MatXu &classes, MatXd &c
     if (rc != SIVO_OK) throw std::runtime_error(sivo_last_error());
 }
 
+MatXd BayesianSegNet::computeVariance(const MatXu &classes) {
+    if (classes.rows() != input_geometry.height || classes.cols() != input_geometry.width)
+        throw std::invalid_argument("computeVariance: the class map must have the network's input geometry");
+    MatXd variance(input_geometry.height, input_geometry.width);
+    int rc = sivo_segnet_variance(this->handle, classes.data(), variance.data());
+    if (rc != SIVO_OK) throw std::runtime_error(sivo_last_error());
+    return variance;
+}
+
 cv::Mat BayesianSegNet::resizeImage(const cv::Mat &image) {
     if (image.size() == this->input_geometry) return image;
     cv::Mat out;

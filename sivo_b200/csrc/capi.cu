@@ -82,6 +82,34 @@ int sivo_segnet_finalize_device(sivo_segnet_t* h, const double* sum_device, uint
   });
 }
 
+int sivo_segnet_variance(sivo_segnet_t* h, const uint8_t* classes, double* variance) {
+  return guarded([&] {
+    if (!h) fail(SIVO_EINVAL, "null handle");
+    h->impl->variance_host(classes, variance);
+  });
+}
+
+int sivo_segnet_variance_device(sivo_segnet_t* h, const uint8_t* classes_device, double* variance_device, void* stream) {
+  return guarded([&] {
+    if (!h) fail(SIVO_EINVAL, "null handle");
+    h->impl->variance_device(classes_device, variance_device, static_cast<cudaStream_t>(stream));
+  });
+}
+
+int sivo_segnet_variance_partial_device(sivo_segnet_t* h, const uint8_t* classes_device, double* moments_device, void* stream) {
+  return guarded([&] {
+    if (!h) fail(SIVO_EINVAL, "null handle");
+    h->impl->variance_partial(classes_device, moments_device, static_cast<cudaStream_t>(stream));
+  });
+}
+
+int sivo_segnet_variance_finalize_device(sivo_segnet_t* h, const double* moments_device, double* variance_device, void* stream) {
+  return guarded([&] {
+    if (!h) fail(SIVO_EINVAL, "null handle");
+    h->impl->variance_finalize(moments_device, variance_device, static_cast<cudaStream_t>(stream));
+  });
+}
+
 int sivo_segnet_create(const char* prototxt, const char* caffemodel, int device, uint64_t seed, sivo_segnet_t** out) {
   sivo_segnet_options o{};
   o.device = device;
@@ -506,6 +534,22 @@ int sivo_dbg_mc_reduce(int device, const float* logits, int T, int c, int h, int
     if (classes) SIVO_CUDA(cudaMemcpy(classes, bc.p, static_cast<size_t>(h) * w, cudaMemcpyDeviceToHost));
     if (confidence) SIVO_CUDA(cudaMemcpy(confidence, bf.p, static_cast<size_t>(h) * w * 8, cudaMemcpyDeviceToHost));
     if (entropy) SIVO_CUDA(cudaMemcpy(entropy, be.p, static_cast<size_t>(h) * w * 8, cudaMemcpyDeviceToHost));
+  });
+}
+
+int sivo_dbg_mc_variance(int device, const float* logits, int T, int c, int h, int w, const uint8_t* classes, double* variance) {
+  return guarded([&] {
+    if (!logits || !classes || !variance || T < 2 || c <= 0 || h <= 0 || w <= 0) fail(SIVO_EINVAL, "mc_variance: bad arguments");
+    SIVO_CUDA(cudaSetDevice(device));
+    const size_t hw = static_cast<size_t>(h) * w;
+    DevBuf bl, bc(hw), bv(hw * sizeof(double));
+    int cs = (c + 15) / 16 * 16;  // the layout sivo_dbg_mc_reduce uses: C <= 16 takes the quad kernel, C > 16 the generic one
+    TensorView vl = make_view(bl, T, c, h, w, cs, DType::F32);
+    upload_nchw(logits, vl);
+    SIVO_CUDA(cudaMemcpy(bc.p, classes, hw, cudaMemcpyHostToDevice));
+    launch_mc_variance(static_cast<const float*>(vl.p), T, c, cs, static_cast<int>(hw), bc.as<uint8_t>(), bv.as<double>(), nullptr);
+    SIVO_CUDA(cudaDeviceSynchronize());
+    SIVO_CUDA(cudaMemcpy(variance, bv.p, hw * sizeof(double), cudaMemcpyDeviceToHost));
   });
 }
 

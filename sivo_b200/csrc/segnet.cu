@@ -570,6 +570,7 @@ void SegNet::run_device(const uint8_t* bgr_dev, uint8_t* classes_dev, double* co
   fa.frame = frame_++;
   fa.bgr = bgr_dev; fa.classes = classes_dev; fa.conf = conf_dev; fa.ent = ent_dev; fa.conf32 = conf32_dev; fa.ent32 = ent32_dev;
   launch_frame(fa, s);
+  run_stream_ = s;
 }
 
 void SegNet::run_partial(const uint8_t* bgr_dev, double* sum_dev, cudaStream_t s) {
@@ -590,6 +591,57 @@ void SegNet::run_partial(const uint8_t* bgr_dev, double* sum_dev, cudaStream_t s
     throw;
   }
   reduce_ = ReduceMode::Full;
+  run_stream_ = s;
+}
+
+const TensorView& SegNet::last_logits(const char* what) const {
+  if (!run_stream_) fail(SIVO_EINVAL, "%s: the handle has not run a frame yet (the variance reads the last frame's samples)", what);
+  return tensors_[ops_.back().in]->v;  // the op list ends with the Reduce op (build() checks for the Softmax)
+}
+
+void SegNet::variance_device(const uint8_t* classes_dev, double* variance_dev, cudaStream_t s) {
+  if (!classes_dev || !variance_dev) fail(SIVO_EINVAL, "variance: null class map or variance buffer");
+  require_whole_frame("variance");
+  const TensorView& lv = last_logits("variance");
+  SIVO_CUDA(cudaSetDevice(device_));
+  if (!s) s = stream_;
+  launch_mc_variance(static_cast<const float*>(lv.p), lv.n, lv.c, lv.cs, lv.h * lv.w, classes_dev, variance_dev, s);
+}
+
+void SegNet::variance_host(const uint8_t* classes, double* variance) {
+  if (!classes || !variance) fail(SIVO_EINVAL, "computeVariance: null class map or variance buffer");
+  require_whole_frame("computeVariance");
+  last_logits("computeVariance");
+  SIVO_CUDA(cudaSetDevice(device_));
+  const size_t hw = static_cast<size_t>(H_) * W_;
+  if (!d_var_classes_.p) d_var_classes_.alloc(hw);
+  if (!d_var_.p) d_var_.alloc(hw * sizeof(double));
+  // the caller's buffers are plain host memory: staged through the pinned buffers segmentImage uses, on the last run's stream
+  cudaStream_t s = run_stream_;
+  const bool pc = is_pinned_host(classes), pv = is_pinned_host(variance);
+  if (!pc) memcpy(h_classes_.p, classes, hw);
+  SIVO_CUDA(cudaMemcpyAsync(d_var_classes_.p, pc ? classes : h_classes_.p, hw, cudaMemcpyHostToDevice, s));
+  variance_device(d_var_classes_.as<uint8_t>(), d_var_.as<double>(), s);
+  SIVO_CUDA(cudaMemcpyAsync(pv ? variance : h_conf_.p, d_var_.p, hw * sizeof(double), cudaMemcpyDeviceToHost, s));
+  SIVO_CUDA(cudaStreamSynchronize(s));
+  if (!pv) memcpy(variance, h_conf_.p, hw * sizeof(double));
+}
+
+void SegNet::variance_partial(const uint8_t* classes_dev, double* moments_dev, cudaStream_t s) {
+  if (!classes_dev || !moments_dev) fail(SIVO_EINVAL, "variance_partial: null class map or moments buffer");
+  const TensorView& lv = last_logits("variance_partial");
+  if (lv.cs != 16 || lv.c > 16)
+    fail(SIVO_EFORMAT, "variance_partial: the moments need the 16-channel logits layout (at most 16 classes, this net has %d)", lv.c);
+  SIVO_CUDA(cudaSetDevice(device_));
+  if (!s) s = stream_;
+  launch_mc_variance_partial(static_cast<const float*>(lv.p), lv.n, lv.c, lv.cs, lv.h * lv.w, classes_dev, moments_dev, s);
+}
+
+void SegNet::variance_finalize(const double* moments_dev, double* variance_dev, cudaStream_t s) {
+  if (!moments_dev || !variance_dev) fail(SIVO_EINVAL, "variance_finalize: null moments or variance buffer");
+  SIVO_CUDA(cudaSetDevice(device_));
+  if (!s) s = stream_;
+  launch_mc_variance_finalize(moments_dev, T_, H_ * W_, variance_dev, s);
 }
 
 void SegNet::finalize(const double* sum_dev, uint8_t* classes_dev, double* conf_dev, double* ent_dev, float* conf32_dev, float* ent32_dev,

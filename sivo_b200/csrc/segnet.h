@@ -84,6 +84,15 @@ class SegNet {
   // the maps from a sum over all T samples of the frame (e.g. the shards' sums reduced over ranks); any output may be NULL
   void finalize(const double* sum_dev, uint8_t* classes_dev, double* conf_dev, double* ent_dev, float* conf32_dev, float* ent32_dev,
                 cudaStream_t s);
+  // computeVariance over the samples of the last run (the logits feeding the Reduce op): per pixel the sample variance of the
+  // probability of class classes[pix] (0 where it is >= the class count).  The device forms run on `s` (NULL = the handle's
+  // own stream), which must be ordered after that run and before the next; the host form synchronises.
+  void variance_host(const uint8_t* classes, double* variance);
+  void variance_device(const uint8_t* classes_dev, double* variance_dev, cudaStream_t s);
+  // latency mode: moments_dev[H*W][2] = (sum p, sum p^2) over this shard's samples; the variance from the moments summed over
+  // all T samples of the frame
+  void variance_partial(const uint8_t* classes_dev, double* moments_dev, cudaStream_t s);
+  void variance_finalize(const double* moments_dev, double* variance_dev, cudaStream_t s);
   void semantic_keys(const sivo_keypoint* kps, int n, int max_static_class, uint8_t* kp_class, double* kp_conf, double* kp_entropy,
                      int* keep_idx, int* n_keep);
   void blob(const std::string& name, float* out, size_t cap, int* n, int* c, int* h, int* w);
@@ -103,6 +112,8 @@ class SegNet {
   // one frame of the op list (graph replay or plain launches) with the per-frame arguments `fa`, ending as reduce_ says
   void launch_frame(FrameArgs fa, cudaStream_t s);
   void require_whole_frame(const char* what) const;
+  // the logits of the last run's samples (the Reduce op's input); fails if the handle has not run yet
+  const TensorView& last_logits(const char* what) const;
 
   sivo_segnet_options opt_;
   // T_: samples of the frame (the mean divides by it); this handle runs samples [s0_, s0_ + ns_) (ns_ = T_ unless a shard)
@@ -122,6 +133,10 @@ class SegNet {
   const double* last_conf_ = nullptr;
   const double* last_ent_ = nullptr;
   cudaStream_t last_stream_ = nullptr;
+  // stream of the last run_device / run_partial; non-NULL once a frame has been issued, so that the logits tensor holds its
+  // samples (the variance reads them)
+  cudaStream_t run_stream_ = nullptr;
+  DevBuf d_var_classes_, d_var_;  // device staging of the host-buffer variance call
   DevBuf d_kp_, d_kp_out_;
   PinnedBuf h_kp_, h_kp_out_;
   std::vector<cudaEvent_t> events_;

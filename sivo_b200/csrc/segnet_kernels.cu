@@ -336,35 +336,48 @@ __global__ void k_mc_reduce(const float* __restrict__ logits, int T, int cs, int
 // The two halves below are shared by the one-pass kernel and the latency-mode pair (partial sum / finalize), so all three
 // perform the same operations in the same order.
 
+constexpr int kQuadBatch = 6;  // samples whose loads are issued together (memory-level parallelism: the pass is HBM-bound)
+
+__device__ __forceinline__ float4 quad_load(const float* __restrict__ logits, int t, int hw, int pp, int q) {
+  return __ldcs(reinterpret_cast<const float4*>(logits + (static_cast<size_t>(t) * hw + pp) * 16) + q);
+}
+
+// lane q of one sample's pixel (logits v = channels 4q .. 4q+3): p[j] = softmax[4q + j] in float, 0 for channels >= C.
+// Every lane of the 4-lane group must call it (the max and the sum travel by xor-shuffles).
+__device__ __forceinline__ void quad_softmax(const float4 v, int C, int q, float (&p)[4]) {
+  float x[4] = {v.x, v.y, v.z, v.w};
+  float m = -INFINITY;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) if (q * 4 + j < C) m = fmaxf(m, x[j]);
+  m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
+  m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+  float sum = 0.f;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    x[j] = (q * 4 + j < C) ? __expf(__fsub_rn(x[j], m)) : 0.f;  // ex2.approx: <= 2 ulp on an argument in [-88, 0], 2e-7 on a probability
+    sum = __fadd_rn(sum, x[j]);
+  }
+  sum = __fadd_rn(sum, __shfl_xor_sync(0xffffffffu, sum, 1));
+  sum = __fadd_rn(sum, __shfl_xor_sync(0xffffffffu, sum, 2));
+  const float inv = __frcp_rn(sum);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) p[j] = __fmul_rn(x[j], inv);
+}
+
 // lane q of pixel pp: acc[j] += softmax(logits[t][pp])[4q + j] in double, samples t = 0 .. T-1 in order
 __device__ __forceinline__ void quad_softmax_sum(const float* __restrict__ logits, int T, int C, int hw, int pp, int q, double (&acc)[4]) {
-  constexpr int kBatch = 6;  // samples whose loads are issued together (memory-level parallelism: the pass is HBM-bound)
-  for (int t0 = 0; t0 < T; t0 += kBatch) {
-  float4 vb[kBatch];
+  for (int t0 = 0; t0 < T; t0 += kQuadBatch) {
+  float4 vb[kQuadBatch];
 #pragma unroll
-  for (int b = 0; b < kBatch; ++b)
-    if (t0 + b < T) vb[b] = __ldcs(reinterpret_cast<const float4*>(logits + (static_cast<size_t>(t0 + b) * hw + pp) * 16) + q);
+  for (int b = 0; b < kQuadBatch; ++b)
+    if (t0 + b < T) vb[b] = quad_load(logits, t0 + b, hw, pp, q);
 #pragma unroll
-  for (int b = 0; b < kBatch; ++b) {
+  for (int b = 0; b < kQuadBatch; ++b) {
     if (t0 + b >= T) break;
-    const float4 v = vb[b];
-    float x[4] = {v.x, v.y, v.z, v.w};
-    float m = -INFINITY;
+    float p[4];
+    quad_softmax(vb[b], C, q, p);
 #pragma unroll
-    for (int j = 0; j < 4; ++j) if (q * 4 + j < C) m = fmaxf(m, x[j]);
-    m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
-    m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
-    float sum = 0.f;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      x[j] = (q * 4 + j < C) ? __expf(__fsub_rn(x[j], m)) : 0.f;  // ex2.approx: <= 2 ulp on an argument in [-88, 0], 2e-7 on a probability
-      sum = __fadd_rn(sum, x[j]);
-    }
-    sum = __fadd_rn(sum, __shfl_xor_sync(0xffffffffu, sum, 1));
-    sum = __fadd_rn(sum, __shfl_xor_sync(0xffffffffu, sum, 2));
-    const float inv = __frcp_rn(sum);
-#pragma unroll
-    for (int j = 0; j < 4; ++j) acc[j] += static_cast<double>(__fmul_rn(x[j], inv));
+    for (int j = 0; j < 4; ++j) acc[j] += static_cast<double>(p[j]);
   }
   }
 }
@@ -471,6 +484,129 @@ __global__ void k_mc_reduce_generic(const float* __restrict__ logits, int T, int
   if (entropy) entropy[i] = ent;
   if (conf32) conf32[i] = static_cast<float>(best);
   if (ent32) ent32[i] = static_cast<float>(ent);
+}
+
+// ---- Monte-Carlo sample variance (computeVariance, bayesian_segnet.cpp:205-260): per pixel, with c = classes[pixel] and p_t
+// the softmax probability of class c in sample t, avg = sum_t p_t / T and var = sum_t (p_t - avg)^2 / (T - 1), both sums in
+// double in sample order with every square rounded before it is added (std::pow(x, 2), no fused multiply-add).  p_t comes from
+// the per-sample arithmetic of the reduction kernel the same logits layout selects, and avg is formed as that kernel forms
+// the mean, so for the argmax class avg is the mean `confidence` reports.  A class >= C (VOID = 255) gives 0: the reference
+// leaves that element unwritten.  Run after the frame, outside its graph; the logits stay valid until the handle's next run.
+
+__device__ __forceinline__ float pick4(const float (&p)[4], int j) { return j == 0 ? p[0] : j == 1 ? p[1] : j == 2 ? p[2] : p[3]; }
+
+// 16-channel logits, C <= 16, four lanes per pixel as k_mc_reduce_quad (lane c >> 2 owns class c).  The first kRegT samples'
+// p_t stay in registers between the mean pass and the deviation pass; a sample beyond them is loaded again in the second.
+template <int kRegT>
+__global__ void k_mc_variance_quad(const float* __restrict__ logits, int T, int C, int hw, const uint8_t* __restrict__ classes,
+                                   double* __restrict__ variance) {
+  const int gid = blockIdx.x * blockDim.x + threadIdx.x;
+  const int pix = gid >> 2, q = gid & 3;
+  const bool live = pix < hw;
+  const int pp = live ? pix : hw - 1;
+  const int c = __ldg(classes + pp), j = c & 3;
+  float reg[kRegT];
+  double s = 0.0;
+#pragma unroll
+  for (int t0 = 0; t0 < kRegT; t0 += kQuadBatch) {
+    float4 vb[kQuadBatch];
+#pragma unroll
+    for (int b = 0; b < kQuadBatch; ++b)
+      if (t0 + b < kRegT && t0 + b < T) vb[b] = quad_load(logits, t0 + b, hw, pp, q);
+#pragma unroll
+    for (int b = 0; b < kQuadBatch; ++b)
+      if (t0 + b < kRegT && t0 + b < T) {
+        float p[4];
+        quad_softmax(vb[b], C, q, p);
+        reg[t0 + b] = pick4(p, j);
+        s += static_cast<double>(reg[t0 + b]);
+      }
+  }
+  for (int t = kRegT; t < T; ++t) {
+    float p[4];
+    quad_softmax(quad_load(logits, t, hw, pp, q), C, q, p);
+    s += static_cast<double>(pick4(p, j));
+  }
+  const double avg = s * (1.0 / static_cast<double>(T));  // quad_finalize's mean
+  double d2 = 0.0;
+#pragma unroll
+  for (int t = 0; t < kRegT; ++t)
+    if (t < T) {
+      const double d = static_cast<double>(reg[t]) - avg;
+      d2 = __dadd_rn(d2, __dmul_rn(d, d));
+    }
+  for (int t = kRegT; t < T; ++t) {
+    float p[4];
+    quad_softmax(quad_load(logits, t, hw, pp, q), C, q, p);
+    const double d = static_cast<double>(pick4(p, j)) - avg;
+    d2 = __dadd_rn(d2, __dmul_rn(d, d));
+  }
+  if (live && q == (c < C ? c >> 2 : 0)) variance[pix] = c < C ? d2 / static_cast<double>(T - 1) : 0.0;
+}
+
+// softmax probability of class c at one pixel with the arithmetic of k_mc_reduce<15> / k_mc_reduce_generic
+__device__ __forceinline__ float generic_prob(const float* __restrict__ s, int C, int c) {
+  float m = -INFINITY;
+  for (int k = 0; k < C; ++k) m = fmaxf(m, s[k]);
+  float sum = 0.f;
+  for (int k = 0; k < C; ++k) sum = __fadd_rn(sum, expf(__fsub_rn(s[k], m)));
+  return __fdiv_rn(expf(__fsub_rn(s[c], m)), sum);
+}
+
+// any C and channel stride (the layouts launch_mc_reduce does not give to the quad kernel); one thread per pixel, the
+// deviation pass reads the logits again
+__global__ void k_mc_variance_generic(const float* __restrict__ logits, int T, int C, int cs, int hw, const uint8_t* __restrict__ classes,
+                                      double* __restrict__ variance) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= hw) return;
+  const int c = classes[i];
+  if (c >= C) { variance[i] = 0.0; return; }
+  double a = 0.0;
+  for (int t = 0; t < T; ++t) a += static_cast<double>(generic_prob(logits + (static_cast<size_t>(t) * hw + i) * cs, C, c));
+  const double avg = a / static_cast<double>(T);  // the generic kernels' mean
+  double d2 = 0.0;
+  for (int t = 0; t < T; ++t) {
+    const double d = static_cast<double>(generic_prob(logits + (static_cast<size_t>(t) * hw + i) * cs, C, c)) - avg;
+    d2 = __dadd_rn(d2, __dmul_rn(d, d));
+  }
+  variance[i] = d2 / static_cast<double>(T - 1);
+}
+
+// Latency mode, first half: moments[pix] = (sum p_t, sum p_t^2) over the shard's T local samples, class c's p_t as in
+// k_mc_variance_quad; (0, 0) for c >= C
+__global__ void k_mc_variance_partial(const float* __restrict__ logits, int T, int C, int hw, const uint8_t* __restrict__ classes,
+                                      double2* __restrict__ moments) {
+  const int gid = blockIdx.x * blockDim.x + threadIdx.x;
+  const int pix = gid >> 2, q = gid & 3;
+  const bool live = pix < hw;
+  const int pp = live ? pix : hw - 1;
+  const int c = __ldg(classes + pp), j = c & 3;
+  double s1 = 0.0, s2 = 0.0;
+  for (int t0 = 0; t0 < T; t0 += kQuadBatch) {
+    float4 vb[kQuadBatch];
+#pragma unroll
+    for (int b = 0; b < kQuadBatch; ++b)
+      if (t0 + b < T) vb[b] = quad_load(logits, t0 + b, hw, pp, q);
+#pragma unroll
+    for (int b = 0; b < kQuadBatch; ++b) {
+      if (t0 + b >= T) break;
+      float p[4];
+      quad_softmax(vb[b], C, q, p);
+      const double x = static_cast<double>(pick4(p, j));
+      s1 += x;
+      s2 = __dadd_rn(s2, __dmul_rn(x, x));
+    }
+  }
+  if (live && q == (c < C ? c >> 2 : 0)) moments[pix] = c < C ? make_double2(s1, s2) : make_double2(0.0, 0.0);
+}
+
+// Latency mode, second half: variance = max(0, (S2 - S1^2 / T) / (T - 1)) from the moments summed over all T samples
+__global__ void k_mc_variance_finalize(const double2* __restrict__ moments, int T, int hw, double* __restrict__ variance) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= hw) return;
+  const double2 m = __ldg(moments + i);
+  const double v = (m.y - m.x * m.x / static_cast<double>(T)) / static_cast<double>(T - 1);
+  variance[i] = fmax(0.0, v);
 }
 
 // ---- tap expansion for the 3-channel first convolution: out[y][x][kh*blk + kw*4 + c] = in[y+kh-pad][x+kw-pad][c]
@@ -812,6 +948,32 @@ void launch_mc_finalize(const double* sum, int T_total, int C, int hw, uint8_t* 
                         float* ent32, cudaStream_t s) {
   if (C > 16) fail(SIVO_EFORMAT, "mc_finalize: the latency-mode sum layout holds at most 16 classes");
   k_mc_finalize_quad<<<blocks_for(static_cast<size_t>(hw) * 4, 256), 256, 0, s>>>(sum, T_total, C, hw, classes, conf, entropy, conf32, ent32);
+  SIVO_CUDA(cudaGetLastError());
+}
+
+void launch_mc_variance(const float* logits, int T, int C, int cs, int hw, const uint8_t* classes, double* variance, cudaStream_t s) {
+  if (T < 2) fail(SIVO_EINVAL, "mc_variance: the sample variance needs at least 2 samples (T = %d)", T);
+  if (cs == 16 && C <= 16) {  // the layout launch_mc_reduce gives to k_mc_reduce_quad
+    const unsigned grid = blocks_for(static_cast<size_t>(hw) * 4, 256);
+    if (T <= 6) k_mc_variance_quad<6><<<grid, 256, 0, s>>>(logits, T, C, hw, classes, variance);
+    else if (T <= 12) k_mc_variance_quad<12><<<grid, 256, 0, s>>>(logits, T, C, hw, classes, variance);
+    else k_mc_variance_quad<24><<<grid, 256, 0, s>>>(logits, T, C, hw, classes, variance);
+  } else {
+    k_mc_variance_generic<<<blocks_for(hw, 128), 128, 0, s>>>(logits, T, C, cs, hw, classes, variance);
+  }
+  SIVO_CUDA(cudaGetLastError());
+}
+
+void launch_mc_variance_partial(const float* logits, int T, int C, int cs, int hw, const uint8_t* classes, double* moments, cudaStream_t s) {
+  if (cs != 16 || C > 16) fail(SIVO_EFORMAT, "mc_variance_partial: the latency-mode moments need the 16-channel logits layout (C <= 16)");
+  k_mc_variance_partial<<<blocks_for(static_cast<size_t>(hw) * 4, 256), 256, 0, s>>>(logits, T, C, hw, classes,
+                                                                                     reinterpret_cast<double2*>(moments));
+  SIVO_CUDA(cudaGetLastError());
+}
+
+void launch_mc_variance_finalize(const double* moments, int T_total, int hw, double* variance, cudaStream_t s) {
+  if (T_total < 2) fail(SIVO_EINVAL, "mc_variance_finalize: the sample variance needs at least 2 samples (T = %d)", T_total);
+  k_mc_variance_finalize<<<blocks_for(hw, 256), 256, 0, s>>>(reinterpret_cast<const double2*>(moments), T_total, hw, variance);
   SIVO_CUDA(cudaGetLastError());
 }
 

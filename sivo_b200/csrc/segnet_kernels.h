@@ -87,6 +87,13 @@ void launch_mc_reduce(const float* logits, int T, int C, int cs, int hw, uint8_t
 void launch_mc_partial(const float* logits, int T, int C, int cs, int hw, cudaStream_t s, const FrameArgs* args);
 void launch_mc_finalize(const double* sum, int T_total, int C, int hw, uint8_t* classes, double* conf, double* entropy, float* conf32,
                         float* ent32, cudaStream_t s);
+// Monte-Carlo sample variance of the probability of class classes[pix] over the T samples of `logits` (layout as in
+// launch_mc_reduce, whose per-sample arithmetic it repeats); variance[pix] = 0 where classes[pix] >= C.  Needs T >= 2.
+void launch_mc_variance(const float* logits, int T, int C, int cs, int hw, const uint8_t* classes, double* variance, cudaStream_t s);
+// Latency mode: moments[pix][2] (double) = (sum p_t, sum p_t^2) over the T local samples (16-channel layout only), and the
+// variance from moments summed over all T_total samples of the frame.
+void launch_mc_variance_partial(const float* logits, int T, int C, int cs, int hw, const uint8_t* classes, double* moments, cudaStream_t s);
+void launch_mc_variance_finalize(const double* moments, int T_total, int hw, double* variance, cudaStream_t s);
 void launch_dropout_bits(uint64_t seed, const uint64_t* frame_dev, int layer, int T, int C, int H, int W,
                          uint8_t* keep_nchw, cudaStream_t s);
 // layout converters for the test hooks (float NCHW host order <-> NHWC activation)

@@ -155,6 +155,30 @@ class BayesianSegNet:
                                                     C.c_void_p(ent_ptr), C.c_void_p(conf32_ptr), C.c_void_p(ent32_ptr),
                                                     C.c_void_p(stream)))
 
+    def computeVariance(self, classes: np.ndarray) -> np.ndarray:
+        """bayesian_segnet.cpp:205-260 after segmentImage / segment_on_device: float64 [H, W], per pixel the sample variance
+        over the last frame's T samples of the softmax probability of class classes[row, col] (0 where it is >= n_classes)."""
+        classes = np.ascontiguousarray(classes)
+        if classes.dtype != np.uint8 or classes.shape != (self.height, self.width):
+            raise ValueError(f"computeVariance expects a {self.height}x{self.width} uint8 class map")
+        var = np.empty((self.height, self.width), np.float64)
+        L.check(L.lib().sivo_segnet_variance(self._h, classes.ctypes.data_as(C.c_void_p), var.ctypes.data_as(C.c_void_p)))
+        return var
+
+    def variance_device(self, classes_ptr: int, var_ptr: int, stream: int = 0):
+        """computeVariance on device buffers (height*width u8 in, float64 out), ordered on `stream` after the run it reads."""
+        L.check(L.lib().sivo_segnet_variance_device(self._h, C.c_void_p(classes_ptr), C.c_void_p(var_ptr), C.c_void_p(stream)))
+
+    def variance_partial(self, classes_ptr: int, moments_ptr: int, stream: int = 0):
+        """Latency mode: moments_ptr (device, height*width x 2 float64) receives (sum p, sum p^2) of the given class over this
+        shard's samples of its last run_partial."""
+        L.check(L.lib().sivo_segnet_variance_partial_device(self._h, C.c_void_p(classes_ptr), C.c_void_p(moments_ptr),
+                                                            C.c_void_p(stream)))
+
+    def variance_finalize(self, moments_ptr: int, var_ptr: int, stream: int = 0):
+        """Latency mode: the variance map from the moments summed over ALL T samples of the frame."""
+        L.check(L.lib().sivo_segnet_variance_finalize_device(self._h, C.c_void_p(moments_ptr), C.c_void_p(var_ptr), C.c_void_p(stream)))
+
     def blob(self, name: str) -> np.ndarray:
         n, c, h, w = C.c_int(), C.c_int(), C.c_int(), C.c_int()
         L.check(L.lib().sivo_segnet_blob(self._h, name.encode(), None, C.c_size_t(0), C.byref(n), C.byref(c), C.byref(h), C.byref(w)))

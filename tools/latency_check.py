@@ -23,6 +23,7 @@ def main():
     ap.add_argument("--T", type=int, default=6)
     ap.add_argument("--precision", default="fp16", choices=["fp16", "fp32"])
     ap.add_argument("--frame", type=int, default=41)
+    ap.add_argument("--variance", action="store_true", help="also check the latency-mode variance map")
     args = ap.parse_args()
 
     import torch
@@ -60,13 +61,17 @@ def main():
     torch.cuda.set_stream(stream)
     shard.set_frame(args.frame)
     shard.run_partial(d_bgr.data_ptr(), d_sum.data_ptr(), stream.cuda_stream)
-    if nccl:
-        dist.reduce(d_sum, dst=0)  # enqueued behind run_partial on the current stream
-    else:
-        h_sum = d_sum.cpu()
-        dist.reduce(h_sum, dst=0)
-        if rank == 0:
-            d_sum.copy_(h_sum)
+
+    def reduce_to_rank0(t):
+        if nccl:
+            dist.reduce(t, dst=0)  # enqueued behind the library's work on the current stream
+        else:
+            h = t.cpu()
+            dist.reduce(h, dst=0)
+            if rank == 0:
+                t.copy_(h)
+
+    reduce_to_rank0(d_sum)
     ok = True
     if rank == 0:
         maps = lambda: (torch.empty(hw, dtype=torch.uint8, device=dev), torch.empty(hw, dtype=torch.float64, device=dev),
@@ -89,6 +94,27 @@ def main():
               f"samples {ranges}: class mismatches {int(diff.sum())} (near-tie pixels {int(tie.sum())}), |d confidence| {d_conf:.1e}, "
               f"|d entropy| {d_ent:.1e}")
         print("LATENCY OK" if ok else "LATENCY FAILED")
+    if args.variance:
+        d_cls = s_cls if rank == 0 else torch.empty(hw, dtype=torch.uint8, device=dev)
+        if nccl:
+            dist.broadcast(d_cls, src=0)
+        else:
+            h_cls = d_cls.cpu()
+            dist.broadcast(h_cls, src=0)
+            d_cls.copy_(h_cls)
+        d_mom = torch.empty(hw * 2, dtype=torch.float64, device=dev)
+        shard.variance_partial(d_cls.data_ptr(), d_mom.data_ptr(), stream.cuda_stream)
+        reduce_to_rank0(d_mom)
+        if rank == 0:
+            s_var, u_var = torch.empty(hw, dtype=torch.float64, device=dev), torch.empty(hw, dtype=torch.float64, device=dev)
+            shard.variance_finalize(d_mom.data_ptr(), s_var.data_ptr(), stream.cuda_stream)
+            full.variance_device(d_cls.data_ptr(), u_var.data_ptr(), stream.cuda_stream)
+            torch.cuda.synchronize(dev)
+            d_var = float((s_var - u_var).abs().max())
+            ok_var = d_var <= 1e-12 and bool((s_var >= 0).all())
+            print(f"variance over {world} shards: |d variance| {d_var:.1e} (whole-frame max {float(u_var.max()):.3g})")
+            print("VARIANCE OK" if ok_var else "VARIANCE FAILED")
+            ok = ok and ok_var
     dist.barrier()
     dist.destroy_process_group()
     sys.exit(0 if ok else 1)
