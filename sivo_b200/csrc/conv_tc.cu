@@ -353,7 +353,6 @@ template <int K, bool ROLL, int KW, bool PK2, int N, bool SPLIT>
 __global__ void __launch_bounds__(kTcThreads, 1)
 k_conv_tc(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const __grid_constant__ TcParams p,
           const __grid_constant__ TcConsts cst) {
-  asm volatile("griddepcontrol.launch_dependents;");  // the next kernel's CTAs may be scheduled as soon as all of ours have started
   static_assert(!PK2 || (!ROLL && KW == K), "image-pair tiles use the chunked kernel");
   static_assert(!SPLIT || (!ROLL && N <= 64), "split mode: chunked kernel, segment sums in registers");
   constexpr int RK = kRows + K - 1;                  // halo rows one row block reads (per chunk)
@@ -394,8 +393,6 @@ k_conv_tc(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUt
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
   __syncthreads();
-  // everything above touched only this CTA's shared memory; the producing kernel's results are needed from here on
-  asm volatile("griddepcontrol.wait;" ::: "memory");
 
   if (wg == 0) {
     // 384 threads start with 168 registers each; the producers need few, the consumers (2 rows x N/2 accumulators, the
@@ -594,24 +591,7 @@ void conv_tc_dispatch(const ConvTcPlan& plan, cudaStream_t s, bool configure) {
     // the limit is per kernel function, not per launch: always raise it to the full 227 KB so that plans of different
     // sizes that share an instantiation cannot lower it for each other
     if (configure) SIVO_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    else {
-      // Programmatic dependent launch: the CTAs of this launch may start while the previous kernel of the stream is still
-      // draining (on SMs it has already left, or never used) and run their prologue -- barrier init, descriptor
-      // prefetch -- up to griddepcontrol.wait, which returns once that kernel has completed and flushed.  Opt-in
-      // (SIVO_B200_PDL=1): the early CTAs sit on SMs the concurrent extractor kernels could have used.
-      static const bool pdl = [] { const char* e = std::getenv("SIVO_B200_PDL"); return e && e[0] == '1'; }();
-      cudaLaunchConfig_t cfg = {};
-      cfg.gridDim = plan.grid;
-      cfg.blockDim = dim3(kTcThreads);
-      cfg.dynamicSmemBytes = plan.smem;
-      cfg.stream = s;
-      cudaLaunchAttribute attr[1];
-      attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-      attr[0].val.programmaticStreamSerializationAllowed = 1;
-      cfg.attrs = attr;
-      cfg.numAttrs = pdl ? 1 : 0;
-      SIVO_CUDA(cudaLaunchKernelEx(&cfg, kern, plan.map_a, plan.map_b, plan.p, plan.cst));
-    }
+    else kern<<<plan.grid, kTcThreads, plan.smem, s>>>(plan.map_a, plan.map_b, plan.p, plan.cst);
   };
   // per (K, ROLL, KW, PK2): the three tile widths
   auto by_n = [&](auto k16, auto k64, auto k128) {
@@ -644,11 +624,8 @@ int num_sms() {
 }
 // Upper bound on the row blocks one CTA walks.  Long-lived CTAs amortise the prologue best, but while they run no SM
 // frees up, so the extractors' short dependent kernels -- highest stream priority notwithstanding -- each wait for a
-// whole CTA lifetime; SIVO_B200_TC_MAX_PPC trades the two (unit: 2-row blocks).
-int tc_max_ppc() {
-  static const int v = [] { const char* e = std::getenv("SIVO_B200_TC_MAX_PPC"); return e ? std::max(1, atoi(e)) : 48; }();
-  return v;
-}
+// whole CTA lifetime; this cap trades the two (unit: 2-row blocks).
+constexpr int kTcMaxPpc = 48;
 size_t tc_smem_bytes(int K, bool roll, int n_tile, int stages) {
   const int rk = kRows + K - 1;
   const int slots = roll ? rk : (K == 7 ? rk + 2 : 2 * rk);  // k_conv_tc's kSlots
@@ -672,7 +649,7 @@ int tc_blocks_per_cta(long columns, int total_pairs, double overhead) {
   const int sms = num_sms();
   int ppc = 1;
   double best_cost = 1e30;
-  for (int c = 1; c <= std::min(total_pairs, tc_max_ppc()); ++c) {
+  for (int c = 1; c <= std::min(total_pairs, kTcMaxPpc); ++c) {
     const long ctas = columns * ceil_div(total_pairs, c);
     const double cost = static_cast<double>((ctas + sms - 1) / sms) * (c + overhead);
     if (cost < best_cost - 1e-9) { best_cost = cost; ppc = c; }
@@ -682,7 +659,6 @@ int tc_blocks_per_cta(long columns, int total_pairs, double overhead) {
 }  // namespace
 
 bool conv_tc_supported(const Op& op, const TensorView& in, const TensorView& out) {
-  if (const char* e = std::getenv("SIVO_B200_NO_TC")) if (e[0] == '1') return false;
   if (in.dt != DType::F16) return false;
   if (op.k != 1 && op.k != 3 && op.k != 7) return false;
   if (op.cout_p > kMaxCout) return false;
@@ -748,9 +724,7 @@ std::shared_ptr<ConvTcPlan> conv_tc_plan(const Op& op, const TensorView& in, con
   p.cin_real = op.cin;
   p.acc_scale = op.split ? op.acc_scale : 1.f;
   p.seg_rows = 1;  // a segment per (chunk, tap row): 7x7 56 / 28 accumulate steps, 3x3 24 / 12, 1x1 8 / 4
-  if (const char* e = std::getenv("SIVO_B200_SPLIT_SEG")) p.seg_rows = std::max(1, std::min(K, atoi(e)));
   p.rz_comp = 0.216f * 1.1920929e-7f;  // x 2^-23
-  if (const char* e = std::getenv("SIVO_B200_SPLIT_RZ")) p.rz_comp = static_cast<float>(atof(e)) * 1.1920929e-7f;
   p.strips = ceil_div(p.W, 128);
   const int cout_tiles = p.out_f32 == 1 ? 1 : op.cout_p / n_tile;
   const int n_z = plan->pk2 ? ceil_div(in.n, 2) : in.n;  // PK2: an image pair per tile

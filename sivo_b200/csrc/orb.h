@@ -23,7 +23,7 @@ struct OrbLevel {
   int w, h;            // level image size
   int pitch;           // bytes per row of the bordered buffer ((w + 38) rounded up to 16)
   size_t img_off;      // offset of the bordered buffer in the pyramid arena
-  size_t flat_off;     // offset of the w*h planes (score map, blurred image) in their arenas
+  size_t flat_off;     // offset of the w*h blurred image in its arena
   int cell_begin, cell_end;
 };
 
@@ -60,36 +60,13 @@ struct OrbSelected {  // one retained keypoint, level coordinates
   short pad;
 };
 
-// Programmatic dependent launch for the extractor's chain of short dependent kernels: every kernel starts with
-// `griddepcontrol.launch_dependents; griddepcontrol.wait;` (ORB_PDL_PROLOGUE), so the next grid of the stream is scheduled while
-// this one drains and only its launch latency -- not its work -- overlaps (the wait returns once the previous grid has completed
-// and flushed).  Opt-in (SIVO_B200_ORB_PDL=1; without the attribute the prologue is a no-op): the early CTAs of the next small
-// kernel sit on SMs the convolution CTAs need.
-#define ORB_PDL_PROLOGUE() asm volatile("griddepcontrol.launch_dependents;\n\tgriddepcontrol.wait;" ::: "memory")
-template <class... KArgs, class... Args>
-inline void orb_launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args... args) {
-  static const bool pdl = [] { const char* e = std::getenv("SIVO_B200_ORB_PDL"); return e && e[0] == '1'; }();
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid;
-  cfg.blockDim = block;
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = s;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = pdl ? 1 : 0;
-  SIVO_CUDA(cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...));
-}
-
 // ---- kernels (orb_kernels.cu)
 void orb_launch_pyramid(const uint8_t* gray, int rows, int cols, size_t gray_pitch, uint8_t* pyr, const OrbLevelTable& t,
                         cudaStream_t s);
 void hamming_best2(int device, const uint8_t* query, int nq, const uint8_t* train, int nt, const int* cand_off, const int* cand_idx,
                    const int* train_level, int* out5);
-void orb_launch_score(const uint8_t* pyr, uint8_t* score, const OrbLevelTable& t, int t_min, cudaStream_t s);
-// score == nullptr: the cells score their own pixels from `pyr` (no score-map pass)
-void orb_launch_cells(const uint8_t* score, const uint8_t* pyr, const OrbLevelTable& t, const OrbCell* cells, int ncells, int ini_th,
+// the cells score their own pixels from `pyr`
+void orb_launch_cells(const uint8_t* pyr, const OrbLevelTable& t, const OrbCell* cells, int ncells, int ini_th,
                       int min_th, int* cell_count, uint32_t* cell_items, cudaStream_t s);
 void orb_launch_compact(const OrbLevelTable& t, const OrbCell* cells, int ncells, const int* cell_count,
                         const uint32_t* cell_items, int* cell_offset, int* level_offsets, uint32_t* cand, int cand_cap,
@@ -173,7 +150,7 @@ class Orb {
   std::vector<OrbCell> cells_;
   cudaStream_t stream_ = nullptr;
   cudaEvent_t ev_[4] = {nullptr, nullptr, nullptr, nullptr};
-  DevBuf d_gray_, d_pyr_, d_score_, d_blur_, d_cells_, d_cell_count_, d_cell_items_, d_cell_offset_, d_level_off_, d_cand_,
+  DevBuf d_gray_, d_pyr_, d_blur_, d_cells_, d_cell_count_, d_cell_items_, d_cell_offset_, d_level_off_, d_cand_,
       d_sel_, d_umax_, d_angles_, d_desc_;
   PinnedBuf h_gray_, h_cand_, h_level_off_, h_sel_, h_angles_, h_desc_, h_pyr_;
   size_t pyr_bytes_ = 0, flat_bytes_ = 0;

@@ -1,6 +1,6 @@
 // Host side of the ORB operator: constructor tables, the per-level cell grid, the quad-tree keypoint
 // distribution (order dependent and tiny -- stays on the host), and the two-phase device schedule
-//   [pyramid, score, cells, compact, blur] -> candidates D2H -> quad tree -> selection H2D -> [angle+rBRIEF] -> D2H.
+//   [pyramid, cells, compact, blur] -> candidates D2H -> quad tree -> selection H2D -> [angle+rBRIEF] -> D2H.
 #include <algorithm>
 #include <chrono>
 #include <cmath>
@@ -303,8 +303,7 @@ Orb::Orb(int nfeatures, float scale_factor, int nlevels, int ini_th, int min_th,
     // they slot in ahead of the next wave of a long convolution kernel running on the same GPU
     int lo = 0, hi = 0;
     SIVO_CUDA(cudaDeviceGetStreamPriorityRange(&lo, &hi));
-    const char* e = std::getenv("SIVO_B200_ORB_PRIO");  // A/B switch: 0 = default priority
-    SIVO_CUDA(cudaStreamCreateWithPriority(&stream_, cudaStreamNonBlocking, (e && e[0] == '0') ? lo : hi));
+    SIVO_CUDA(cudaStreamCreateWithPriority(&stream_, cudaStreamNonBlocking, hi));
   }
   for (auto& e : ev_) SIVO_CUDA(cudaEventCreate(&e));
   d_umax_.alloc(sizeof(tab_.umax));
@@ -420,7 +419,6 @@ void Orb::ensure(int rows, int cols) {
   h_gray_.ensure(static_cast<size_t>(rows) * cols);
   d_pyr_.alloc(pyr_bytes_);
   h_pyr_.ensure(pyr_bytes_);
-  d_score_.alloc(flat_bytes_);
   d_blur_.alloc(flat_bytes_);
   d_cells_.alloc(std::max<size_t>(1, ncells) * sizeof(OrbCell));
   if (ncells) SIVO_CUDA(cudaMemcpy(d_cells_.p, cells_.data(), ncells * sizeof(OrbCell), cudaMemcpyHostToDevice));
@@ -653,10 +651,8 @@ void Orb::enqueue_front(const uint8_t* src, size_t src_pitch, cudaStream_t s) {
   const int ncells = static_cast<int>(cells_.size());
   orb_launch_pyramid(src, rows_, cols_, src_pitch, d_pyr_.as<uint8_t>(), lt_, s);
   if (ev_pyr_) SIVO_CUDA(cudaEventRecord(ev_pyr_, s));  // the level images are final: their read-back can start on the copy stream
-  static const bool fused_score = [] { const char* e = std::getenv("SIVO_B200_ORB_FUSED_SCORE"); return !(e && e[0] == '0'); }();
-  if (!fused_score) orb_launch_score(d_pyr_.as<uint8_t>(), d_score_.as<uint8_t>(), lt_, std::min(ini_th_, min_th_), s);
-  orb_launch_cells(fused_score ? nullptr : d_score_.as<uint8_t>(), d_pyr_.as<uint8_t>(), lt_, d_cells_.as<OrbCell>(), ncells, ini_th_, min_th_,
-                   d_cell_count_.as<int>(), d_cell_items_.as<uint32_t>(), s);
+  orb_launch_cells(d_pyr_.as<uint8_t>(), lt_, d_cells_.as<OrbCell>(), ncells, ini_th_, min_th_, d_cell_count_.as<int>(),
+                   d_cell_items_.as<uint32_t>(), s);
   compacted_ = false;  // the device tree reads the cell lists directly; the host path and the test hook compact on demand
 }
 

@@ -1,5 +1,5 @@
 // ORB extractor kernels.  All integer / byte work, bit-exact against oracle/orb_oracle.py (which is pinned
-// to cv2): pyramid (cv::resize INTER_LINEAR fixed point + REFLECT_101 border), FAST-9/16 score map,
+// to cv2): pyramid (cv::resize INTER_LINEAR fixed point + REFLECT_101 border), FAST-9/16 score,
 // per-cell threshold / 3x3 NMS / ordered compaction, 7x7 sigma-2 fixed-point blur, IC angle, rBRIEF.
 // Everything here is latency/launch bound on the GPU (~8 MB touched per image), so the design goal is few
 // launches over all 8 levels at once rather than bandwidth tricks.
@@ -22,7 +22,6 @@ __device__ __forceinline__ int reflect101(int i, int n) {
 
 // ---- level 0: copyMakeBorder(image, 19, BORDER_REFLECT_101) (ORBextractor.cc:1112-1119)
 __global__ void k_level0(const uint8_t* __restrict__ gray, size_t gpitch, uint8_t* __restrict__ dst, OrbLevel lv) {
-  ORB_PDL_PROLOGUE();
   int bx = blockIdx.x * blockDim.x + threadIdx.x, by = blockIdx.y;
   if (bx >= lv.w + 2 * kEdge) return;
   int x = reflect101(bx - kEdge, lv.w), y = reflect101(by - kEdge, lv.h);
@@ -48,7 +47,6 @@ __device__ __forceinline__ Coef lin_coef(int d, int dn, int sn) {
 }
 
 __global__ void k_resize(uint8_t* __restrict__ pyr, OrbLevel src, OrbLevel dst) {
-  ORB_PDL_PROLOGUE();
   int bx = blockIdx.x * blockDim.x + threadIdx.x, by = blockIdx.y;
   if (bx >= dst.w + 2 * kEdge) return;
   int dx = reflect101(bx - kEdge, dst.w), dy = reflect101(by - kEdge, dst.h);
@@ -63,8 +61,8 @@ __global__ void k_resize(uint8_t* __restrict__ pyr, OrbLevel src, OrbLevel dst) 
 }
 
 // ---- FAST-9/16 corner score (cv::FAST's cornerScore<16>): S = max over the 16 contiguous 9-arcs of
-// min(+-(ring - p)) - 1; p is a corner at threshold t iff S >= t.  One thread per pixel, all levels in
-// one launch (grid.y = level).  Only [19, w-19) x [19, h-19) can ever be a keypoint (cell interiors).
+// min(+-(ring - p)) - 1; p is a corner at threshold t iff S >= t.  Only [19, w-19) x [19, h-19) can ever be a
+// keypoint (cell interiors).
 // `t_min` = the smallest threshold any consumer applies (min(iniThFAST, minThFAST)): a 9-arc covers at least two of the four
 // compass points, so a pixel with fewer than two compass points brighter than p + t_min and fewer than two darker than
 // p - t_min has S < t_min, is zeroed by every threshold, and gets 0 without the full score (most pixels).
@@ -103,13 +101,6 @@ __device__ __forceinline__ int fast_score_at(const uint8_t* __restrict__ pyr, co
   return max(best - 1, 0);
 }
 
-__global__ void k_fast_score(const uint8_t* __restrict__ pyr, uint8_t* __restrict__ score, OrbLevelTable t, int t_min) {
-  const OrbLevel lv = t.lv[blockIdx.y];
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= lv.w * lv.h) return;
-  score[lv.flat_off + i] = static_cast<uint8_t>(fast_score_at(pyr, lv, i % lv.w, i / lv.w, t_min));
-}
-
 // ---- one block per 30-px cell: cv::FAST(cell, iniThFAST, NMS) with the minThFAST retry when the cell
 // comes back empty (ORBextractor.cc:793-807), emitted in sub-image row-major order.
 constexpr int kCellThreads = 256;
@@ -132,12 +123,11 @@ __device__ int block_exclusive_scan(int flag, int* s_warp, int& total) {
   return base + within;
 }
 
-// score == nullptr: the cell computes its own FAST scores from the pyramid (cell interiors tile the level without overlap, so
-// this is the same work as the score-map kernel minus one launch and the 1.1 MB map written and read back)
-__global__ void __launch_bounds__(kCellThreads) k_cells(const uint8_t* __restrict__ score, const uint8_t* __restrict__ pyr, OrbLevelTable t,
+// The cell computes its own FAST scores from the pyramid (cell interiors tile the level without overlap, so no pixel is
+// scored twice and no score map is written and read back)
+__global__ void __launch_bounds__(kCellThreads) k_cells(const uint8_t* __restrict__ pyr, OrbLevelTable t,
                                                         const OrbCell* __restrict__ cells, int ini_th, int min_th,
                                                         int* __restrict__ cell_count, uint32_t* __restrict__ cell_items) {
-  ORB_PDL_PROLOGUE();
   __shared__ uint8_t s[(kCellMaxDim + 2) * (kCellMaxDim + 2)];
   __shared__ int s_warp[kCellThreads / 32];
   __shared__ int s_any;
@@ -150,13 +140,10 @@ __global__ void __launch_bounds__(kCellThreads) k_cells(const uint8_t* __restric
     return;
   }
   const int sw = iw + 2;
-  const uint8_t* sc = score + lv.flat_off;
   for (int e = threadIdx.x; e < (ih + 2) * sw; e += kCellThreads) {
     int x = e % sw - 1, y = e / sw - 1;
     uint8_t v = 0;
-    if (x >= 0 && x < iw && y >= 0 && y < ih)
-      v = score ? sc[static_cast<size_t>(iy0 + y) * lv.w + ix0 + x]
-                : static_cast<uint8_t>(fast_score_at(pyr, lv, ix0 + x, iy0 + y, min(ini_th, min_th)));
+    if (x >= 0 && x < iw && y >= 0 && y < ih) v = static_cast<uint8_t>(fast_score_at(pyr, lv, ix0 + x, iy0 + y, min(ini_th, min_th)));
     s[e] = v;  // outside the sub-image's 3-px apron the score is 0 by construction of cv::FAST
   }
   if (threadIdx.x == 0) s_any = 0;
@@ -265,7 +252,6 @@ __global__ void k_gather_cells(const int* __restrict__ cell_count, const int* __
 // blurs (`mvImagePyramid[level].clone()`, ORBextractor.cc:1060-1062).
 // One thread = four horizontally adjacent pixels: 10 bytes per source row serve four 7-tap row sums.
 __global__ void k_blur(const uint8_t* __restrict__ pyr, uint8_t* __restrict__ blur, OrbLevelTable t) {
-  ORB_PDL_PROLOGUE();
   const OrbLevel lv = t.lv[blockIdx.y];
   const int wq = (lv.w + 3) >> 2;
   int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -325,7 +311,6 @@ __global__ void k_describe(const uint8_t* __restrict__ pyr, const uint8_t* __res
                            float* __restrict__ angles, uint8_t* __restrict__ desc, const uint32_t* __restrict__ sel_packed,
                            const int* __restrict__ level_count, OrbTreeParams prm, sivo_keypoint* __restrict__ kps,
                            int* __restrict__ n_out, long long* __restrict__ n_out_i64, int* __restrict__ out_error) {
-  ORB_PDL_PROLOGUE();
   int wid = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   OrbSelected kp;
   uint32_t packed = 0;
@@ -424,22 +409,16 @@ void orb_launch_pyramid(const uint8_t* gray, int rows, int cols, size_t gray_pit
   for (int l = 0; l < t.nlevels; ++l) {
     const OrbLevel& lv = t.lv[l];
     dim3 grid(ceil_div(lv.w + 2 * kEdge, 128), lv.h + 2 * kEdge);
-    if (l == 0) orb_launch_pdl(k_level0, grid, dim3(128), 0, s, gray, gray_pitch, pyr, lv);
-    else orb_launch_pdl(k_resize, grid, dim3(128), 0, s, pyr, t.lv[l - 1], lv);
+    if (l == 0) k_level0<<<grid, 128, 0, s>>>(gray, gray_pitch, pyr, lv);
+    else k_resize<<<grid, 128, 0, s>>>(pyr, t.lv[l - 1], lv);
   }
   SIVO_CUDA(cudaGetLastError());
 }
 
-void orb_launch_score(const uint8_t* pyr, uint8_t* score, const OrbLevelTable& t, int t_min, cudaStream_t s) {
-  dim3 grid(ceil_div(t.lv[0].w * t.lv[0].h, 128), t.nlevels);
-  k_fast_score<<<grid, 128, 0, s>>>(pyr, score, t, t_min);
-  SIVO_CUDA(cudaGetLastError());
-}
-
-void orb_launch_cells(const uint8_t* score, const uint8_t* pyr, const OrbLevelTable& t, const OrbCell* cells, int ncells, int ini_th,
-                      int min_th, int* cell_count, uint32_t* cell_items, cudaStream_t s) {
+void orb_launch_cells(const uint8_t* pyr, const OrbLevelTable& t, const OrbCell* cells, int ncells, int ini_th, int min_th,
+                      int* cell_count, uint32_t* cell_items, cudaStream_t s) {
   if (ncells == 0) return;
-  orb_launch_pdl(k_cells, dim3(ncells), dim3(kCellThreads), 0, s, score, pyr, t, cells, ini_th, min_th, cell_count, cell_items);
+  k_cells<<<ncells, kCellThreads, 0, s>>>(pyr, t, cells, ini_th, min_th, cell_count, cell_items);
   SIVO_CUDA(cudaGetLastError());
 }
 
@@ -455,7 +434,7 @@ void orb_launch_compact(const OrbLevelTable& t, const OrbCell* cells, int ncells
 
 void orb_launch_blur(const uint8_t* pyr, uint8_t* blur, const OrbLevelTable& t, cudaStream_t s) {
   dim3 grid(ceil_div(((t.lv[0].w + 3) / 4) * t.lv[0].h, 128), t.nlevels);
-  orb_launch_pdl(k_blur, grid, dim3(128), 0, s, pyr, blur, t);
+  k_blur<<<grid, 128, 0, s>>>(pyr, blur, t);
   SIVO_CUDA(cudaGetLastError());
 }
 
@@ -470,8 +449,8 @@ void orb_launch_describe_dev(const uint8_t* pyr, const uint8_t* blur, const OrbL
                              const int* level_count, const OrbTreeParams& prm, int cap, const int* umax, sivo_keypoint* kps,
                              uint8_t* desc, int* n_out, long long* n_out_i64, int* error, cudaStream_t s) {
   if (cap == 0) return;
-  orb_launch_pdl(k_describe, dim3(ceil_div(cap * 32, 128)), dim3(128), 0, s, pyr, blur, t, static_cast<const OrbSelected*>(nullptr), cap, umax,
-                 static_cast<float*>(nullptr), desc, sel_packed, level_count, prm, kps, n_out, n_out_i64, error);
+  k_describe<<<ceil_div(cap * 32, 128), 128, 0, s>>>(pyr, blur, t, nullptr, cap, umax, nullptr, desc, sel_packed, level_count, prm, kps, n_out,
+                                                     n_out_i64, error);
   SIVO_CUDA(cudaGetLastError());
 }
 

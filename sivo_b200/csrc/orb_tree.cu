@@ -143,7 +143,6 @@ __global__ void __launch_bounds__(kTreeThreads, 1)
 k_distribute(const uint32_t* __restrict__ cand, const int* __restrict__ level_off, const uint32_t* __restrict__ cell_items,
              const int* __restrict__ cell_count, OrbTreeParams prm, uint32_t* __restrict__ out_sel, int* __restrict__ out_count,
              int* __restrict__ out_error) {
-  ORB_PDL_PROLOGUE();
   extern __shared__ __align__(16) uint8_t tree_raw[];
   TreeSmem& s = *reinterpret_cast<TreeSmem*>(tree_raw);
   const int l = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -472,8 +471,7 @@ void orb_tree_configure() {
 
 void orb_launch_distribute(const uint32_t* cand, const int* level_off, const uint32_t* cell_items, const int* cell_count,
                            const OrbTreeParams& prm, int nlevels, uint32_t* sel_packed, int* level_count, int* error, cudaStream_t s) {
-  orb_launch_pdl(k_distribute, dim3(nlevels), dim3(kTreeThreads), sizeof(TreeSmem), s, cand, level_off, cell_items, cell_count, prm, sel_packed,
-                 level_count, error);
+  k_distribute<<<nlevels, kTreeThreads, sizeof(TreeSmem), s>>>(cand, level_off, cell_items, cell_count, prm, sel_packed, level_count, error);
   SIVO_CUDA(cudaGetLastError());
 }
 

@@ -32,14 +32,12 @@ int SegNet::add_tensor(const std::string& name, int n, int c, int h, int w, int 
 }
 
 void SegNet::prepare_conv(Op& op, const std::vector<Blob>& cb, const std::vector<Blob>* bn) {
-  // K is the layer's kernel size; a tap-expanded layer (expand_k > 0) stores it as one tap over expand_k*blk channels
-  const int K = op.expand_k ? op.expand_k : op.k, cin = (op.expand_k || op.fold_kw) ? 3 : op.cin, cout = op.cout;
-  const int taps = op.expand_k ? 1 : op.fold_kw ? K : K * K;
+  const int K = op.k, cin = op.fold_kw ? 3 : op.cin, cout = op.cout;
+  const int taps = op.fold_kw ? K : K * K;
   auto slot = [&](int t, int ci, int& tap, int& cidx) {
-    if (op.expand_k) { tap = 0; cidx = (t / K) * op.expand_blk + (t % K) * 4 + ci; }
     // tap row kh; "channel" = window pixel * 8 + c.  The window of output pixel x starts at image pixel x - 3, tap column
     // kw reads image pixel x + kw - (K-1)/2, i.e. window pixel kw + 3 - (K-1)/2
-    else if (op.fold_kw) { tap = t / K; cidx = (t % K + 3 - (K - 1) / 2) * 8 + ci; }
+    if (op.fold_kw) { tap = t / K; cidx = (t % K + 3 - (K - 1) / 2) * 8 + ci; }
     else { tap = t; cidx = ci; }
   };
   if (cb.empty() || cb[0].shape.size() != 4 || cb[0].shape[0] != cout || cb[0].shape[1] != cin || cb[0].shape[2] != K ||
@@ -75,7 +73,7 @@ void SegNet::prepare_conv(Op& op, const std::vector<Blob>& cb, const std::vector
     SIVO_CUDA(cudaMemcpy(op.w_tc.p, wt.data(), wt.size() * sizeof(__half), cudaMemcpyHostToDevice));
   }
   if (op.split) {
-    if (taps != K * K) fail(SIVO_EINVAL, "layer '%s': split-operand mode does not take folded / expanded first layers", op.layer.c_str());
+    if (taps != K * K) fail(SIVO_EINVAL, "layer '%s': split-operand mode does not take window-folded first layers", op.layer.c_str());
     std::vector<__half> wt = conv_tc_split_weights(W, cout, cin, K, op.cout_p, op.cin_p, &op.acc_scale);
     op.w_tc.alloc(wt.size() * sizeof(__half));
     SIVO_CUDA(cudaMemcpy(op.w_tc.p, wt.data(), wt.size() * sizeof(__half), cudaMemcpyHostToDevice));
@@ -154,46 +152,31 @@ void SegNet::build(const NetSpec& net, const WeightMap& weights) {
         op.in = in;
         op.k = ly.kernel; op.pad = ly.pad; op.cin = iv.c; op.cout = ly.num_output;
         op.cin_p = iv.cs;
-        const char* no_tc = std::getenv("SIVO_B200_NO_TC");
         if (iv.cs == 4 && iv.c == 3 && act_ == DType::F16 && opt_.engine != SIVO_ENGINE_SIMT && (ly.kernel == 7 || ly.kernel == 3) &&
-            ly.num_output % 64 == 0 && !(no_tc && no_tc[0] == '1')) {
-          // 3-channel first layer: expand the KxK taps into channels once, then it is a 1x1 tensor-core convolution
-          const char* no_fold = std::getenv("SIVO_B200_NO_FOLD");
+            ly.num_output % 64 == 0) {
+          // 3-channel first layer: zero-pad to 8-channel pixels; the convolution's TMA reads overlapping 8-pixel windows of it
+          // (K x 1 layer)
           Op ex;
-          ex.kind = Op::Expand;
+          ex.kind = Op::Pad8;
           ex.in = in;
-          ex.k = ly.kernel;
-          if (no_fold && no_fold[0] == '1') {
-            // (A/B switch) materialise the taps as channels once, then it is a 1x1 tensor-core convolution
-            const int blk = (ly.kernel * 4 + 15) / 16 * 16, cs_e = round_up(ly.kernel * blk, 64);
-            ex.layer = ly.name + "/expand";
-            ex.expand_blk = blk;
-            ex.out = add_tensor("__expand_" + ly.name, iv.n, cs_e, iv.h, iv.w, cs_e, act_);
-            ops_.push_back(std::move(ex));
-            op.in = ops_.back().out;
-            op.expand_k = ly.kernel; op.expand_blk = blk;
-            op.k = 1; op.pad = 0; op.cin = cs_e; op.cin_p = cs_e;
-          } else {
-            // zero-pad to 8-channel pixels; the convolution's TMA reads overlapping 8-pixel windows of it (K x 1 layer)
-            ex.layer = ly.name + "/pad8";
-            ex.out = add_tensor("__pad8_" + ly.name, iv.n, 8, iv.h, iv.w + 8, 8, act_);
-            const size_t no = ops_.size();
-            if (!opt_.keep_blobs && no >= 2 && ops_[no - 1].kind == Op::LRN && ops_[no - 1].out == in && ops_[no - 2].kind == Op::Input &&
-                ops_[no - 2].out == ops_[no - 1].in && iv.n == 1) {
-              // input -> LRN -> pad8 collapse into one pass (the 'data' and 'norm' blobs are not materialised)
-              ex.kind = Op::InputPad8;
-              ex.lrn_size = ops_[no - 1].lrn_size; ex.lrn_alpha = ops_[no - 1].lrn_alpha;
-              ex.lrn_beta = ops_[no - 1].lrn_beta; ex.lrn_k = ops_[no - 1].lrn_k;
-              ex.layer = "input+" + ops_[no - 1].layer + "+" + ex.layer;
-              tensors_[ops_[no - 1].out]->elided = tensors_[ops_[no - 2].out]->elided = true;
-              ops_.pop_back();
-              ops_.pop_back();
-            }
-            ops_.push_back(std::move(ex));
-            op.in = ops_.back().out;
-            op.fold_kw = ly.kernel;
-            op.cin = 64; op.cin_p = 64;
+          ex.layer = ly.name + "/pad8";
+          ex.out = add_tensor("__pad8_" + ly.name, iv.n, 8, iv.h, iv.w + 8, 8, act_);
+          const size_t no = ops_.size();
+          if (!opt_.keep_blobs && no >= 2 && ops_[no - 1].kind == Op::LRN && ops_[no - 1].out == in && ops_[no - 2].kind == Op::Input &&
+              ops_[no - 2].out == ops_[no - 1].in && iv.n == 1) {
+            // input -> LRN -> pad8 collapse into one pass (the 'data' and 'norm' blobs are not materialised)
+            ex.kind = Op::InputPad8;
+            ex.lrn_size = ops_[no - 1].lrn_size; ex.lrn_alpha = ops_[no - 1].lrn_alpha;
+            ex.lrn_beta = ops_[no - 1].lrn_beta; ex.lrn_k = ops_[no - 1].lrn_k;
+            ex.layer = "input+" + ops_[no - 1].layer + "+" + ex.layer;
+            tensors_[ops_[no - 1].out]->elided = tensors_[ops_[no - 2].out]->elided = true;
+            ops_.pop_back();
+            ops_.pop_back();
           }
+          ops_.push_back(std::move(ex));
+          op.in = ops_.back().out;
+          op.fold_kw = ly.kernel;
+          op.cin = 64; op.cin_p = 64;
         }
         const TensorView civ = tensors_[op.in]->v;  // the tensor the convolution actually reads
         op.cout_p = round_up(op.cout, 64);
@@ -222,8 +205,7 @@ void SegNet::build(const NetSpec& net, const WeightMap& weights) {
         if (it == weights.end()) fail(SIVO_EFORMAT, "caffemodel has no blobs for layer '%s'", ly.name.c_str());
         // fp32 activations on the tensor-core engine: split-operand mode (three half MMAs per tap, fp32 accumulation)
         TensorView split_in = civ;
-        if (act_ == DType::F32 && opt_.engine != SIVO_ENGINE_SIMT && !op.fold_kw && !op.expand_k && civ.cs % 64 == 0 && civ.c == civ.cs &&
-            !(no_tc && no_tc[0] == '1')) {
+        if (act_ == DType::F32 && opt_.engine != SIVO_ENGINE_SIMT && !op.fold_kw && civ.cs % 64 == 0 && civ.c == civ.cs) {
           split_in.dt = DType::F16;
           split_in.cs = 2 * civ.cs;
           op.split = true;
@@ -429,8 +411,6 @@ SegNet::SegNet(const std::string& prototxt, const std::string& caffemodel, const
 SegNet::~SegNet() {
   cudaSetDevice(device_);
   for (auto& g : graphs_) cudaGraphExecDestroy(g.exec);
-  for (auto e : band_ev_) cudaEventDestroy(e);
-  if (copy_stream_) cudaStreamDestroy(copy_stream_);
   for (auto e : events_) cudaEventDestroy(e);
   if (stream_) cudaStreamDestroy(stream_);
 }
@@ -444,12 +424,11 @@ void SegNet::enqueue(const uint8_t* bgr_dev, uint8_t* classes_dev, double* conf_
       case Op::Input:
         launch_input_u8(bgr_dev, tensors_[op.out]->v, s, d_frame_.as<FrameArgs>());
         break;
-      case Op::Expand:
+      case Op::Pad8:
+        launch_pad8(tensors_[op.in]->v, tensors_[op.out]->v, s);
+        break;
       case Op::InputPad8:
-        if (op.kind == Op::InputPad8)
-          launch_input_lrn_pad8(bgr_dev, tensors_[op.out]->v, op.lrn_size, op.lrn_alpha, op.lrn_beta, op.lrn_k, s, d_frame_.as<FrameArgs>());
-        else if (op.expand_blk) launch_expand_taps(tensors_[op.in]->v, tensors_[op.out]->v, op.k, op.expand_blk, s);
-        else launch_pad8(tensors_[op.in]->v, tensors_[op.out]->v, s);
+        launch_input_lrn_pad8(bgr_dev, tensors_[op.out]->v, op.lrn_size, op.lrn_alpha, op.lrn_beta, op.lrn_k, s, d_frame_.as<FrameArgs>());
         break;
       case Op::LRN:
         launch_lrn(tensors_[op.in]->v, tensors_[op.out]->v, op.lrn_size, op.lrn_alpha, op.lrn_beta, op.lrn_k, s);
@@ -501,12 +480,11 @@ void SegNet::enqueue(const uint8_t* bgr_dev, uint8_t* classes_dev, double* conf_
         break;
       }
       case Op::Reduce: {
-        if (reduce_ == ReduceMode::Skip) break;
         const TensorView& lv = tensors_[op.in]->v;
         if (reduce_ == ReduceMode::Partial)
           launch_mc_partial(static_cast<const float*>(lv.p), lv.n, lv.c, lv.cs, lv.h * lv.w, s, d_frame_.as<FrameArgs>());
         else
-          launch_mc_reduce(static_cast<const float*>(lv.p), lv.n, lv.c, lv.cs, lv.h * lv.w, classes_dev, conf_dev, ent_dev, s, 0, -1,
+          launch_mc_reduce(static_cast<const float*>(lv.p), lv.n, lv.c, lv.cs, lv.h * lv.w, classes_dev, conf_dev, ent_dev, s,
                            d_frame_.as<FrameArgs>());
         break;
       }
@@ -687,14 +665,11 @@ void SegNet::launch_frame(FrameArgs fa, cudaStream_t s) {
   // memory (the frame counter read by the dropout code), so the captured kernels and their arguments never change.
   bool all_tc = true;
   for (const Op& op : ops_) if (op.kind == Op::Conv && !op.use_tc) all_tc = false;  // the SIMT launcher sets attributes per launch
-  static const bool graphs_enabled = [] { const char* e = std::getenv("SIVO_B200_NO_GRAPH"); return !(e && e[0] == '1'); }();
-  if (graphs_enabled && graph_ok_ && all_tc) {
+  if (graph_ok_ && all_tc) {
     // the graph's kernels read the image / result pointers from FrameArgs: the key is the stream (and the op-list variant) only
-    const void* key[5] = {nullptr, nullptr, nullptr, nullptr,
-                          reinterpret_cast<const void*>(reinterpret_cast<uintptr_t>(s) ^ static_cast<uintptr_t>(reduce_))};
     cudaGraphExec_t graph_exec_ = nullptr;
     for (size_t i = 0; i < graphs_.size(); ++i)
-      if (memcmp(key, graphs_[i].key, sizeof key) == 0) {
+      if (graphs_[i].stream == s && graphs_[i].reduce == reduce_) {
         std::rotate(graphs_.begin(), graphs_.begin() + i, graphs_.begin() + i + 1);  // move to front
         graph_exec_ = graphs_.front().exec;
         break;
@@ -720,14 +695,11 @@ void SegNet::launch_frame(FrameArgs fa, cudaStream_t s) {
         graph_ok_ = false;
         graph_exec_ = nullptr;
       } else {
-        if (graphs_.size() >= kMaxGraphs) {  // a caller cycling through more buffers than this re-captures the oldest
+        if (graphs_.size() >= kMaxGraphs) {  // a caller cycling through more streams than this re-captures the oldest
           cudaGraphExecDestroy(graphs_.back().exec);
           graphs_.pop_back();
         }
-        GraphEntry ge;
-        memcpy(ge.key, key, sizeof key);
-        ge.exec = graph_exec_;
-        graphs_.insert(graphs_.begin(), ge);
+        graphs_.insert(graphs_.begin(), GraphEntry{s, reduce_, graph_exec_});
       }
     }
     if (graph_exec_) {
@@ -768,48 +740,12 @@ void SegNet::run_host(const uint8_t* bgr, int rows, int cols, size_t stride, uin
   uint8_t* hc = pc ? classes : h_classes_.as<uint8_t>();
   double* hf = pf ? conf : h_conf_.as<double>();
   double* he = pe ? ent : h_ent_.as<double>();
-  static const int n_bands = [] { const char* e = std::getenv("SIVO_B200_READBACK_BANDS"); return e ? std::max(1, std::min(16, atoi(e))) : 1; }();  // opt-in: measured no gain with the extractors' copies sharing the D2H engine
-  const Op& last = ops_.back();
-  const TensorView* lv = last.kind == Op::Reduce ? &tensors_[last.in]->v : nullptr;
-  const bool to_record = rec_classes_ || rec_conf32_ || rec_ent32_;
-  const bool banded = n_bands > 1 && !to_record && !profiling_ && lv && lv->cs == 16 && lv->c <= 16 && (classes || conf || ent) && H_ >= n_bands;
-  if (!banded) {
-    run_device(d_bgr_.as<uint8_t>(), d_classes_.as<uint8_t>(), d_conf_.as<double>(), d_ent_.as<double>(), stream_, rec_conf32_, rec_ent32_);
-    if (classes) SIVO_CUDA(cudaMemcpyAsync(hc, d_classes_.p, hw, cudaMemcpyDeviceToHost, stream_));
-    if (conf) SIVO_CUDA(cudaMemcpyAsync(hf, d_conf_.p, hw * sizeof(double), cudaMemcpyDeviceToHost, stream_));
-    if (ent) SIVO_CUDA(cudaMemcpyAsync(he, d_ent_.p, hw * sizeof(double), cudaMemcpyDeviceToHost, stream_));
-    if (rec_classes_) SIVO_CUDA(cudaMemcpyAsync(rec_classes_, d_classes_.p, hw, cudaMemcpyDeviceToDevice, stream_));
-    SIVO_CUDA(cudaStreamSynchronize(stream_));
-  } else {
-    if (!copy_stream_) SIVO_CUDA(cudaStreamCreateWithFlags(&copy_stream_, cudaStreamNonBlocking));
-    while (static_cast<int>(band_ev_.size()) < n_bands) {
-      cudaEvent_t e;
-      SIVO_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-      band_ev_.push_back(e);
-    }
-    reduce_ = ReduceMode::Skip;
-    try {
-      run_device(d_bgr_.as<uint8_t>(), d_classes_.as<uint8_t>(), d_conf_.as<double>(), d_ent_.as<double>(), stream_);
-    } catch (...) {
-      reduce_ = ReduceMode::Full;
-      throw;
-    }
-    reduce_ = ReduceMode::Full;
-    for (int b = 0; b < n_bands; ++b) {
-      const int r0 = static_cast<int>(static_cast<long>(H_) * b / n_bands), r1 = static_cast<int>(static_cast<long>(H_) * (b + 1) / n_bands);
-      const size_t p0 = static_cast<size_t>(r0) * W_, np = static_cast<size_t>(r1 - r0) * W_;
-      launch_mc_reduce(static_cast<const float*>(lv->p), lv->n, lv->c, lv->cs, lv->h * lv->w, d_classes_.as<uint8_t>(), d_conf_.as<double>(),
-                       d_ent_.as<double>(), stream_, static_cast<int>(p0), static_cast<int>(np));
-      SIVO_CUDA(cudaEventRecord(band_ev_[b], stream_));
-      SIVO_CUDA(cudaStreamWaitEvent(copy_stream_, band_ev_[b], 0));
-      if (classes) SIVO_CUDA(cudaMemcpyAsync(hc + p0, d_classes_.as<uint8_t>() + p0, np, cudaMemcpyDeviceToHost, copy_stream_));
-      if (conf) SIVO_CUDA(cudaMemcpyAsync(hf + p0, d_conf_.as<double>() + p0, np * sizeof(double), cudaMemcpyDeviceToHost, copy_stream_));
-      if (ent) SIVO_CUDA(cudaMemcpyAsync(he + p0, d_ent_.as<double>() + p0, np * sizeof(double), cudaMemcpyDeviceToHost, copy_stream_));
-    }
-    launches = static_cast<int>(ops_.size()) - 1 + n_bands;  // the bands replace the single Reduce launch of the op list
-    SIVO_CUDA(cudaStreamSynchronize(copy_stream_));
-    SIVO_CUDA(cudaStreamSynchronize(stream_));
-  }
+  run_device(d_bgr_.as<uint8_t>(), d_classes_.as<uint8_t>(), d_conf_.as<double>(), d_ent_.as<double>(), stream_, rec_conf32_, rec_ent32_);
+  if (classes) SIVO_CUDA(cudaMemcpyAsync(hc, d_classes_.p, hw, cudaMemcpyDeviceToHost, stream_));
+  if (conf) SIVO_CUDA(cudaMemcpyAsync(hf, d_conf_.p, hw * sizeof(double), cudaMemcpyDeviceToHost, stream_));
+  if (ent) SIVO_CUDA(cudaMemcpyAsync(he, d_ent_.p, hw * sizeof(double), cudaMemcpyDeviceToHost, stream_));
+  if (rec_classes_) SIVO_CUDA(cudaMemcpyAsync(rec_classes_, d_classes_.p, hw, cudaMemcpyDeviceToDevice, stream_));
+  SIVO_CUDA(cudaStreamSynchronize(stream_));
   if (classes && !pc) memcpy(classes, h_classes_.p, hw);
   if (conf && !pf) memcpy(conf, h_conf_.p, hw * sizeof(double));
   if (ent && !pe) memcpy(ent, h_ent_.p, hw * sizeof(double));

@@ -26,7 +26,7 @@ struct Tensor {
 };
 
 struct Op {
-  enum Kind { Input, LRN, Expand, InputPad8, DropoutUnpool, Conv, Pool, Unpool, Dropout, Reduce } kind = Input;
+  enum Kind { Input, LRN, Pad8, InputPad8, DropoutUnpool, Conv, Pool, Unpool, Dropout, Reduce } kind = Input;
   std::string layer;
   int in = -1, in2 = -1, out = -1, out2 = -1;
   // LRN
@@ -34,10 +34,9 @@ struct Op {
   float lrn_alpha = 1.f, lrn_beta = 0.75f, lrn_k = 1.f;
   // Conv
   int k = 0, pad = 0, cin = 0, cout = 0, cin_p = 0, cout_p = 0;
-  std::vector<float> h_w_raw;  // the caffemodel's (cout, cin, k, k) floats, unrounded (composed-classifier experiment)
+  std::vector<float> h_w_raw;  // the caffemodel's (cout, cin, k, k) floats, unrounded (the composed classifier's input)
   std::vector<float> h_bias, h_bn_scale, h_bn_shift, h_w;  // host copies (the tensor-core kernels take them as kernel parameters)
-  int fold_kw = 0;                  // > 0: KxK conv over 3 channels run as a Kx1 conv over the window-folded padded input (conv_tc.cu)
-  int expand_k = 0, expand_blk = 0;  // > 0: a KxK conv over 3 channels run as a 1x1 conv over the tap-expanded input
+  int fold_kw = 0;  // > 0: KxK conv over 3 channels run as a Kx1 conv over the window-folded padded input (conv_tc.cu)
   bool relu = false, has_bn = false;
   float slope = 0.f;
   DevBuf w_simt, w_tc, bias, bn_scale, bn_shift;
@@ -140,20 +139,15 @@ class SegNet {
   DevBuf d_kp_, d_kp_out_;
   PinnedBuf h_kp_, h_kp_out_;
   std::vector<cudaEvent_t> events_;
-  // the op list captured once as a CUDA graph (one launch per frame); re-captured if the buffers or the stream change
-  // captured op lists, one per (input, outputs, stream) pointer set the caller has used; most recently used first
-  struct GraphEntry { const void* key[5]; cudaGraphExec_t exec; };
+  // how the op list's Reduce op runs: the full MC reduction, or the latency-mode partial sum (run_partial)
+  enum class ReduceMode { Full, Partial };
+  ReduceMode reduce_ = ReduceMode::Full;
+  // the op list captured as CUDA graphs (one launch per frame), one per (stream, ReduceMode) the caller has used, most recently
+  // used first.  The kernels read the per-frame pointers from FrameArgs, so every buffer set replays the same graph.
+  struct GraphEntry { cudaStream_t stream; ReduceMode reduce; cudaGraphExec_t exec; };
   std::vector<GraphEntry> graphs_;
   static constexpr size_t kMaxGraphs = 32;
   bool graph_ok_ = true;
-  // segmentImage read-back overlap: the MC reduction runs in row bands and each band's slices of the three maps start their
-  // device-to-host copy on a second stream while the next band is reduced
-  // how the op list's Reduce op runs: the full MC reduction; skipped (set by run_host around run_device when it reduces in row
-  // bands); or the latency-mode partial sum (run_partial).  Each is its own captured graph.
-  enum class ReduceMode : uintptr_t { Full = 0, Skip = 1, Partial = 2 };
-  ReduceMode reduce_ = ReduceMode::Full;
-  cudaStream_t copy_stream_ = nullptr;
-  std::vector<cudaEvent_t> band_ev_;
   // device-resident copies run_host leaves for a packed multi-GPU record (set_record_outputs)
   uint8_t* rec_classes_ = nullptr;
   float* rec_conf32_ = nullptr;
@@ -177,8 +171,9 @@ void conv_tc_set_pool(ConvTcPlan& plan, void* pooled, uint8_t* mask);
 bool conv_tc_can_fuse_classifier(const ConvTcPlan& plan);
 // host-side weight layout of the split-operand fp32 mode: [tap][cout_p][3 cin_p] half + the accumulator scale 2^-s
 std::vector<__half> conv_tc_split_weights(const float* w_cout_cin_k_k, int cout, int cin, int K, int cout_p, int cin_p, float* acc_scale);
-// Experimental (SIVO_B200_COMPOSE=1): conv (64 -> 64, 7x7, no BN / ReLU) followed by the 1x1 classifier run as ONE 64 -> 16
-// convolution with composed weights; logits come straight from the accumulators.  wc = [n_cls][64], bc = [n_cls] (host).
+// The composed classifier (default; SIVO_B200_COMPOSE=0 keeps the two-step form): conv (64 -> 64, 7x7, no BN / ReLU) followed by
+// the 1x1 classifier run as ONE 64 -> 16 convolution with composed weights; logits come straight from the accumulators.
+// wc = [n_cls][64], bc = [n_cls] (host).
 bool conv_tc_can_compose_classifier(const ConvTcPlan& plan);
 void conv_tc_set_composed_classifier(ConvTcPlan& plan, const Op& conv, const float* wc, const float* bc, int n_cls, float* logits);
 void conv_tc_set_classifier(ConvTcPlan& plan, const float* w_cin_by_cout, int stride, const float* bias, int n_bias, float* logits);  // host pointers

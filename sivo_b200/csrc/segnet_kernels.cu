@@ -277,56 +277,8 @@ __global__ void k_dropout_bits(uint64_t seed, const uint64_t* frame, int layer, 
 
 // ---- Softmax over channels (softmax_layer.cpp:27-60, fp32) fused with the Monte-Carlo reduction the
 // reference runs on the host in double (bayesian_segnet.cpp:278-318): mean over T, first-max argmax, max,
-// -sum p log2 p with 0 log 0 := 0 (computeEntropy :38-44).  One thread per pixel; `prob` never exists.
-template <int C>
-__global__ void k_mc_reduce(const float* __restrict__ logits, int T, int cs, int hw, uint8_t* __restrict__ classes,
-                            double* __restrict__ conf, double* __restrict__ entropy, const FrameArgs* __restrict__ args) {
-  float *conf32 = nullptr, *ent32 = nullptr;
-  if (args) { classes = args->classes; conf = args->conf; entropy = args->ent; conf32 = args->conf32; ent32 = args->ent32; }
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= hw) return;
-  double acc[C];
-#pragma unroll
-  for (int c = 0; c < C; ++c) acc[c] = 0.0;
-  for (int t = 0; t < T; ++t) {
-    const float* s = logits + (static_cast<size_t>(t) * hw + i) * cs;
-    float x[16];
-    if (cs == 16) {  // one 64-byte pixel: four 128-bit loads instead of 15 strided scalar ones
-      const float4* s4 = reinterpret_cast<const float4*>(s);
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const float4 v = __ldg(s4 + q);
-        x[4 * q] = v.x; x[4 * q + 1] = v.y; x[4 * q + 2] = v.z; x[4 * q + 3] = v.w;
-      }
-    } else {
-#pragma unroll
-      for (int c = 0; c < C; ++c) x[c] = s[c];
-    }
-    float m = -INFINITY;
-#pragma unroll
-    for (int c = 0; c < C; ++c) m = fmaxf(m, x[c]);
-    float sum = 0.f;
-#pragma unroll
-    for (int c = 0; c < C; ++c) { x[c] = expf(__fsub_rn(x[c], m)); sum = __fadd_rn(sum, x[c]); }
-#pragma unroll
-    for (int c = 0; c < C; ++c) acc[c] += static_cast<double>(__fdiv_rn(x[c], sum));
-  }
-  double best = -1.0, ent = 0.0;
-  int arg = 0;
-#pragma unroll
-  for (int c = 0; c < C; ++c) {
-    double pm = acc[c] / static_cast<double>(T);
-    if (pm > best) { best = pm; arg = c; }
-    if (pm != 0.0) ent += -1.0 * pm * log2(pm);
-  }
-  if (classes) classes[i] = static_cast<uint8_t>(arg);
-  if (conf) conf[i] = best;
-  if (entropy) entropy[i] = ent;
-  if (conf32) conf32[i] = static_cast<float>(best);
-  if (ent32) ent32[i] = static_cast<float>(ent);
-}
-
-// Same reduction with four lanes per pixel (one float4 = 4 classes each): a warp reads 512 contiguous bytes per
+// -sum p log2 p with 0 log 0 := 0 (computeEntropy :38-44); `prob` never exists.
+// 16-channel logits (C <= 16): four lanes per pixel (one float4 = 4 classes each): a warp reads 512 contiguous bytes per
 // sample and there are 4x more threads in flight, which is what this HBM-bound pass needs.  The softmax max / sum and
 // the final argmax / entropy are combined with xor-shuffles inside the 4-lane group (first maximum still wins).
 // Instruction diet (ncu: the first version was issue-bound at 3400 instructions per warp, 0.8 TB/s): one IEEE
@@ -413,13 +365,12 @@ __device__ __forceinline__ void quad_finalize(const double (&acc)[4], int T, int
 }
 
 __global__ void k_mc_reduce_quad(const float* __restrict__ logits, int T, int C, int hw, uint8_t* __restrict__ classes,
-                                 double* __restrict__ conf, double* __restrict__ entropy, int pix0, int pix_end,
-                                 const FrameArgs* __restrict__ args) {
+                                 double* __restrict__ conf, double* __restrict__ entropy, const FrameArgs* __restrict__ args) {
   float *conf32 = nullptr, *ent32 = nullptr;
   if (args) { classes = args->classes; conf = args->conf; entropy = args->ent; conf32 = args->conf32; ent32 = args->ent32; }
   const int gid = blockIdx.x * blockDim.x + threadIdx.x;
-  const int pix = pix0 + (gid >> 2), q = gid & 3;
-  const bool live = pix < pix_end;
+  const int pix = gid >> 2, q = gid & 3;
+  const bool live = pix < hw;
   const int pp = live ? pix : hw - 1;
   double acc[4] = {0.0, 0.0, 0.0, 0.0};
   quad_softmax_sum(logits, T, C, hw, pp, q, acc);
@@ -544,7 +495,7 @@ __global__ void k_mc_variance_quad(const float* __restrict__ logits, int T, int 
   if (live && q == (c < C ? c >> 2 : 0)) variance[pix] = c < C ? d2 / static_cast<double>(T - 1) : 0.0;
 }
 
-// softmax probability of class c at one pixel with the arithmetic of k_mc_reduce<15> / k_mc_reduce_generic
+// softmax probability of class c at one pixel with the arithmetic of k_mc_reduce_generic
 __device__ __forceinline__ float generic_prob(const float* __restrict__ s, int C, int c) {
   float m = -INFINITY;
   for (int k = 0; k < C; ++k) m = fmaxf(m, s[k]);
@@ -607,46 +558,6 @@ __global__ void k_mc_variance_finalize(const double2* __restrict__ moments, int 
   const double2 m = __ldg(moments + i);
   const double v = (m.y - m.x * m.x / static_cast<double>(T)) / static_cast<double>(T - 1);
   variance[i] = fmax(0.0, v);
-}
-
-// ---- tap expansion for the 3-channel first convolution: out[y][x][kh*blk + kw*4 + c] = in[y+kh-pad][x+kw-pad][c]
-// (zero outside the image = the convolution's zero padding), so that conv1 becomes a 1x1 convolution over
-// K*blk channels that the tensor-core kernel can run (K*K*3 = 147 of 256 K-slots useful for the 7x7 layer).
-template <typename AT>
-__global__ void k_expand_taps(const AT* __restrict__ in, AT* __restrict__ out, int N, int H, int W, int K, int blk, int cs_out) {
-  size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;  // one thread per (n, y, x, kh-or-pad-block)
-  const int groups = cs_out / blk;
-  size_t total = static_cast<size_t>(N) * H * W * groups;
-  if (i >= total) return;
-  const int g = i % groups;
-  size_t r = i / groups;
-  const int x = r % W;
-  r /= W;
-  const int y = r % H;
-  const int n = r / H;
-  AT* d = out + ((static_cast<size_t>(n) * H + y) * W + x) * cs_out + g * blk;
-  const int pad = (K - 1) / 2;
-  const int yy = y + g - pad;
-  const bool row_ok = g < K && yy >= 0 && yy < H;
-  if (sizeof(AT) == 2) {  // half: one 4-channel pixel = 8 bytes; write the block as 16-byte vectors
-    const uint2* src = reinterpret_cast<const uint2*>(in) + (static_cast<size_t>(n) * H + yy) * W;
-    uint4* dst = reinterpret_cast<uint4*>(d);
-    for (int q = 0; q < blk / 8; ++q) {
-      uint2 a = make_uint2(0u, 0u), b = make_uint2(0u, 0u);
-      const int xa = x + 2 * q - pad, xb = xa + 1;
-      if (row_ok && 2 * q < K && xa >= 0 && xa < W) a = __ldg(src + xa);
-      if (row_ok && 2 * q + 1 < K && xb >= 0 && xb < W) b = __ldg(src + xb);
-      dst[q] = make_uint4(a.x, a.y, b.x, b.y);
-    }
-    return;
-  }
-  for (int j = 0; j < blk; ++j) {
-    const int kw = j >> 2, c = j & 3;
-    const int xx = x + kw - pad;
-    float v = 0.f;
-    if (row_ok && kw < K && xx >= 0 && xx < W) v = ld_act(in + ((static_cast<size_t>(n) * H + yy) * W + xx) * 4 + c);
-    st_act(d + j, v);
-  }
 }
 
 // Window-folded first layer (conv_tc.cu): the 4-channel half image, zero-padded to [H][W + 8] pixels of 8 channels.
@@ -797,13 +708,6 @@ void launch_conv_simt(const ConvParams& p, cudaStream_t s) {
   }
 }
 
-void launch_expand_taps(TensorView in, TensorView out, int K, int blk, cudaStream_t s) {
-  size_t total = static_cast<size_t>(out.n) * out.h * out.w * (out.cs / blk);
-  DISPATCH_AT(in.dt, (k_expand_taps<AT><<<blocks_for(total, 256), 256, 0, s>>>(static_cast<const AT*>(in.p), static_cast<AT*>(out.p),
-                                                                               out.n, out.h, out.w, K, blk, out.cs)));
-  SIVO_CUDA(cudaGetLastError());
-}
-
 __global__ void k_keypoint_lookup(const sivo_keypoint* __restrict__ kps, int n, const uint8_t* __restrict__ classes,
                                   const double* __restrict__ conf, const double* __restrict__ ent, int H, int W,
                                   uint8_t* __restrict__ out_class, double* __restrict__ out_conf, double* __restrict__ out_ent) {
@@ -923,18 +827,12 @@ void launch_dropout_unpool(TensorView in, int T, const uint8_t* mask, int mask_n
 }
 
 void launch_mc_reduce(const float* logits, int T, int C, int cs, int hw, uint8_t* classes, double* conf, double* entropy,
-                      cudaStream_t s, int pix0, int npix, const FrameArgs* args) {
-  if (npix < 0) { pix0 = 0; npix = hw; }
-  if (pix0 < 0 || pix0 + npix > hw) fail(SIVO_EINVAL, "mc_reduce: pixel range outside the map");
-  if (npix == 0) return;
-  if (cs == 16 && C <= 16) {
-    k_mc_reduce_quad<<<blocks_for(static_cast<size_t>(npix) * 4, 256), 256, 0, s>>>(logits, T, C, hw, classes, conf, entropy, pix0, pix0 + npix, args);
-    SIVO_CUDA(cudaGetLastError());
-    return;
-  }
-  if (pix0 != 0 || npix != hw) fail(SIVO_EINVAL, "mc_reduce: pixel ranges need the 16-channel logits layout");
-  if (C == 15) k_mc_reduce<15><<<blocks_for(hw, 128), 128, 0, s>>>(logits, T, cs, hw, classes, conf, entropy, args);
-  else k_mc_reduce_generic<<<blocks_for(hw, 128), 128, 0, s>>>(logits, T, C, cs, hw, classes, conf, entropy, args);
+                      cudaStream_t s, const FrameArgs* args) {
+  if (hw == 0) return;
+  if (cs == 16 && C <= 16)
+    k_mc_reduce_quad<<<blocks_for(static_cast<size_t>(hw) * 4, 256), 256, 0, s>>>(logits, T, C, hw, classes, conf, entropy, args);
+  else
+    k_mc_reduce_generic<<<blocks_for(hw, 128), 128, 0, s>>>(logits, T, C, cs, hw, classes, conf, entropy, args);
   SIVO_CUDA(cudaGetLastError());
 }
 

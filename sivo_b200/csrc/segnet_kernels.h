@@ -55,14 +55,12 @@ struct DropoutParams {
 void launch_input_u8(const uint8_t* bgr_hwc, TensorView out, cudaStream_t s, const FrameArgs* args = nullptr);
 void launch_lrn(TensorView in, TensorView out, int size, float alpha, float beta, float k, cudaStream_t s);
 void launch_conv_simt(const ConvParams& p, cudaStream_t s);
-// 4-channel input -> K*blk-channel tap-expanded tensor (see k_expand_taps)
-void launch_expand_taps(TensorView in, TensorView out, int K, int blk, cudaStream_t s);
-// [N][H][W][4] half -> zero-padded [N][H][W + 8][8] half (3 zero pixels left, 5 right, channels 4..7 zero)
 void launch_dropout_unpool(TensorView in, int T, const uint8_t* mask, int mask_n, TensorView out, const DropoutParams& d, float scale,
                            cudaStream_t s);
 // per-keypoint gather from the three result maps (Frame.cc:181-186 indexing); out-of-map keypoints get (255, 0, 0)
 void launch_keypoint_lookup(const sivo_keypoint* kps, int n, const uint8_t* classes, const double* conf, const double* ent, int H, int W,
                             uint8_t* out_class, double* out_conf, double* out_ent, cudaStream_t s);
+// [N][H][W][4] half -> zero-padded [N][H][W + 8][8] half (3 zero pixels left, 5 right, channels 4..7 zero)
 void launch_pad8(TensorView in, TensorView out, cudaStream_t s);
 // the three steps input_u8 -> lrn -> pad8 in one pass (same arithmetic, so the same half values)
 void launch_input_lrn_pad8(const uint8_t* bgr, TensorView out, int size, float alpha, float beta, float k, cudaStream_t s,
@@ -76,10 +74,9 @@ void launch_pool(TensorView in, TensorView out, uint8_t* mask, cudaStream_t s);
 void launch_unpool(TensorView in, const uint8_t* mask, int mask_n, TensorView out, cudaStream_t s);
 // in.n may be 1 (broadcast to out.n samples)
 void launch_dropout(TensorView in, TensorView out, const DropoutParams& d, float scale, cudaStream_t s);
-// logits: float [T, H, W, 16]
-// pix0 / npix restrict the pass to pixels [pix0, pix0 + npix) (npix < 0: all of them)
+// logits: float [T, H, W, cs] (cs = 16 for up to 16 classes)
 void launch_mc_reduce(const float* logits, int T, int C, int cs, int hw, uint8_t* classes, double* conf,
-                      double* entropy, cudaStream_t s, int pix0 = 0, int npix = -1, const FrameArgs* args = nullptr);
+                      double* entropy, cudaStream_t s, const FrameArgs* args = nullptr);
 // Latency mode, the MC reduction cut in two.  Partial: sum[pix][16] (double) = sum over the T local samples of softmax(logits),
 // channels >= C zero; the sum pointer is read from args->sum.  Finalize: the maps of launch_mc_reduce from a sum over all
 // T_total samples of the frame.  Both need the 16-channel logits layout; partial over [0, T) then finalize equals
