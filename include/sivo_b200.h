@@ -152,6 +152,19 @@ int sivo_segnet_blob(sivo_segnet_t* h, const char* name, float* out, size_t cap,
  * order mvKeysSemantic / mDescriptorsSemantic are built in.  Any output pointer may be NULL. */
 int sivo_segnet_semantic_keys(sivo_segnet_t* h, const sivo_keypoint* kps, int n, int max_static_class, uint8_t* kp_class,
                               double* kp_conf, double* kp_entropy, int* keep_idx, int* n_keep);
+/* The same selection for a device-resident pipeline: keypoints, count and every output are DEVICE buffers, e.g. what
+ * sivo_orb_enqueue_device leaves (kps_device, and its int64 *count_device, read on the device).  The maps are those of the
+ * handle's last run (sivo_segnet_run / _run_device / _run_device_maps / _finalize_device) as they stand when the call is made.
+ * cap = capacity of the caller's buffers (kp_class / kp_conf / kp_entropy / keep_idx hold cap entries each; sivo_orb_capacity
+ * suffices for an extractor's output).  If *count_device > cap (or < 0) nothing is written except *n_keep_device = -1.  Otherwise
+ * the per-key values and keep_idx[0 .. *n_keep_device) equal the host form's bit for bit (keep_idx ascending).  Any output may
+ * be NULL.  Runs on `stream` (NULL = the stream of the handle's last run) with no host synchronisation and no host staging; the
+ * stream must be ordered after the run that wrote the maps and after the producer of the keypoints (e.g. sivo_orb_stream_wait),
+ * and before the next run overwrites the maps.  SIVO_EINVAL for a NULL handle, keypoint or count pointer, a negative cap, or a
+ * handle with no maps on the device yet. */
+int sivo_segnet_semantic_keys_device(sivo_segnet_t* h, const sivo_keypoint* kps_device, const long long* count_device, int cap,
+                                     int max_static_class, uint8_t* kp_class_device, double* kp_conf_device,
+                                     double* kp_entropy_device, int* keep_idx_device, long long* n_keep_device, void* stream);
 int sivo_segnet_set_profiling(sivo_segnet_t* h, int on);
 /* Per-stage device times (ms) of the last run: conv, other layers, MC reduction, total; counts kernels. */
 int sivo_segnet_last_timing(const sivo_segnet_t* h, float* conv_ms, float* other_ms, float* reduce_ms,
@@ -235,6 +248,23 @@ int sivo_stereo_hamming(int device, const sivo_keypoint* left, const uint8_t* de
 int sivo_stereo_match(const sivo_orb_t* left, const sivo_orb_t* right, const sivo_keypoint* kp_left, const uint8_t* desc_left,
                       int n_left, const sivo_keypoint* kp_right, const uint8_t* desc_right, int n_right, float mb, float mbf,
                       float* u_right, float* depth);
+/* The same on device-resident inputs and outputs, e.g. the buffers sivo_orb_enqueue_device filled for `left` / `right`.
+ * Output j (u_right_device[j], depth_device[j]) belongs to left keypoint keep_idx_device[j] for j < *n_left_device, or to left
+ * keypoint j when keep_idx_device is NULL: pass sivo_segnet_semantic_keys_device's keep_idx / n_keep to match mvKeysSemantic.
+ * The values equal sivo_stereo_match's on the same keypoints gathered on the host (-1 where unmatched), median cut included.
+ * Counts (int64) are read on the device and clamped to the extractors' capacities; a negative *n_left_device (the -1 of
+ * sivo_segnet_semantic_keys_device) writes nothing.  The output buffers need sivo_orb_capacity(left) floats.  Keypoints whose
+ * octave is outside [0, nlevels) are left unmatched.
+ * Ordering: the call makes `stream` (NULL = the left extractor's stream) wait for everything enqueued so far on both extractors'
+ * streams, so no manual wait is needed after sivo_orb_enqueue_device; keep_idx / n_keep must be ordered before it on `stream`.  The
+ * call reads both pyramids and writes the left extractor's SAD scratch, so the next sivo_orb_enqueue_device on either extractor
+ * must be ordered after it (sivo_orb_wait_for_stream(extractor, stream)), and calls that share a left extractor must be ordered
+ * among themselves.  No host synchronisation.  SIVO_EINVAL for NULL handles or buffers (keep_idx_device may be NULL), extractors
+ * that have not run, extractors on different devices or with different nlevels, and mb / mbf <= 0. */
+int sivo_stereo_match_device(sivo_orb_t* left, sivo_orb_t* right, const sivo_keypoint* kp_left_device, const uint8_t* desc_left_device,
+                             const int* keep_idx_device, const long long* n_left_device, const sivo_keypoint* kp_right_device,
+                             const uint8_t* desc_right_device, const long long* n_right_device, float mb, float mbf,
+                             float* u_right_device, float* depth_device, void* stream);
 
 /* Best / second-best match over per-query candidate lists -- the inner loop of ORBmatcher::SearchByProjection
  * (ORBmatcher.cc:79-113), its last-frame / keyframe variants (:1278-, :1420-), SearchForTriangulation (:631-) and

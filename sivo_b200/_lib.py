@@ -56,6 +56,9 @@ def lib() -> C.CDLL:
         _lib.sivo_version.restype = C.c_char_p
         _lib.sivo_segnet_destroy.restype = None
         _lib.sivo_orb_destroy.restype = None
+        vp, i32, f32 = C.c_void_p, C.c_int, C.c_float
+        _lib.sivo_segnet_semantic_keys_device.argtypes = [vp, vp, vp, i32, i32, vp, vp, vp, vp, vp, vp]
+        _lib.sivo_stereo_match_device.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, f32, f32, vp, vp, vp]
     return _lib
 
 

@@ -20,6 +20,9 @@ void stereo_hamming(int device, const sivo_keypoint* left, const uint8_t* dl, in
                     int* best_idx, int* best_dist);
 void stereo_match(const Orb& left, const Orb& right, const sivo_keypoint* kl, const uint8_t* dl, int nl, const sivo_keypoint* kr,
                   const uint8_t* dr, int nr, float mb, float mbf, float* u_right, float* depth);
+void stereo_match_device(Orb& left, Orb& right, const sivo_keypoint* kl, const uint8_t* dl, const int* keep_idx, const long long* n_left,
+                         const sivo_keypoint* kr, const uint8_t* dr, const long long* n_right, float mb, float mbf, float* u_right,
+                         float* depth, cudaStream_t s);
 }  // namespace sivo
 
 using namespace sivo;
@@ -203,6 +206,16 @@ int sivo_segnet_semantic_keys(sivo_segnet_t* h, const sivo_keypoint* kps, int n,
   return guarded([&] {
     if (!h) fail(SIVO_EINVAL, "null handle");
     h->impl->semantic_keys(kps, n, max_static_class, kp_class, kp_conf, kp_entropy, keep_idx, n_keep);
+  });
+}
+
+int sivo_segnet_semantic_keys_device(sivo_segnet_t* h, const sivo_keypoint* kps_device, const long long* count_device, int cap,
+                                     int max_static_class, uint8_t* kp_class_device, double* kp_conf_device, double* kp_entropy_device,
+                                     int* keep_idx_device, long long* n_keep_device, void* stream) {
+  return guarded([&] {
+    if (!h) fail(SIVO_EINVAL, "null handle");
+    h->impl->semantic_keys_device(kps_device, count_device, cap, max_static_class, kp_class_device, kp_conf_device, kp_entropy_device,
+                                  keep_idx_device, n_keep_device, static_cast<cudaStream_t>(stream));
   });
 }
 
@@ -446,6 +459,19 @@ int sivo_stereo_match(const sivo_orb_t* left, const sivo_orb_t* right, const siv
     if (!left || !right || !u_right || !depth || (n_left && (!kp_left || !desc_left)) || (n_right && (!kp_right || !desc_right)))
       fail(SIVO_EINVAL, "null argument");
     stereo_match(*left->impl, *right->impl, kp_left, desc_left, n_left, kp_right, desc_right, n_right, mb, mbf, u_right, depth);
+  });
+}
+
+int sivo_stereo_match_device(sivo_orb_t* left, sivo_orb_t* right, const sivo_keypoint* kp_left_device, const uint8_t* desc_left_device,
+                             const int* keep_idx_device, const long long* n_left_device, const sivo_keypoint* kp_right_device,
+                             const uint8_t* desc_right_device, const long long* n_right_device, float mb, float mbf, float* u_right_device,
+                             float* depth_device, void* stream) {
+  return guarded([&] {
+    if (!left || !right || !kp_left_device || !desc_left_device || !n_left_device || !kp_right_device || !desc_right_device ||
+        !n_right_device || !u_right_device || !depth_device)
+      fail(SIVO_EINVAL, "null argument");
+    stereo_match_device(*left->impl, *right->impl, kp_left_device, desc_left_device, keep_idx_device, n_left_device, kp_right_device,
+                        desc_right_device, n_right_device, mb, mbf, u_right_device, depth_device, static_cast<cudaStream_t>(stream));
   });
 }
 

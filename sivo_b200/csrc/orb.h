@@ -127,6 +127,12 @@ class Orb {
   int device_tree_status();
   int capacity() const { return sel_cap_; }
   bool device_tree() const { return device_tree_; }
+  cudaStream_t stream() const { return stream_; }
+  // device copies of tables().scale / inv_scale, and capacity() ints of scratch for the device stereo form's SAD distances
+  // (a frame's stereo call on this handle as the left extractor is ordered before its next enqueue_device, like the pyramid)
+  const float* dev_scale() const { return d_scales_.as<float>(); }
+  const float* dev_inv_scale() const { return d_scales_.as<float>() + nlevels_; }
+  int* stereo_sad() const { return d_stereo_sad_.as<int>(); }
   float device_ms = 0, tree_ms = 0;
   int launches = 0;
 
@@ -151,7 +157,7 @@ class Orb {
   cudaStream_t stream_ = nullptr;
   cudaEvent_t ev_[4] = {nullptr, nullptr, nullptr, nullptr};
   DevBuf d_gray_, d_pyr_, d_blur_, d_cells_, d_cell_count_, d_cell_items_, d_cell_offset_, d_level_off_, d_cand_,
-      d_sel_, d_umax_, d_angles_, d_desc_;
+      d_sel_, d_umax_, d_angles_, d_desc_, d_scales_, d_stereo_sad_;
   PinnedBuf h_gray_, h_cand_, h_level_off_, h_sel_, h_angles_, h_desc_, h_pyr_;
   size_t pyr_bytes_ = 0, flat_bytes_ = 0;
   int cand_cap_ = 0, sel_cap_ = 0;

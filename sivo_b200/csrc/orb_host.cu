@@ -315,6 +315,13 @@ Orb::Orb(int nfeatures, float scale_factor, int nlevels, int ini_th, int min_th,
   h_sel_.ensure(sel_cap_ * sizeof(OrbSelected));
   h_angles_.ensure(sel_cap_ * sizeof(float));
   h_desc_.ensure(static_cast<size_t>(sel_cap_) * 32);
+  d_stereo_sad_.alloc(sel_cap_ * sizeof(int));
+  {
+    std::vector<float> sc(tab_.scale);
+    sc.insert(sc.end(), tab_.inv_scale.begin(), tab_.inv_scale.end());
+    d_scales_.alloc(sc.size() * sizeof(float));
+    SIVO_CUDA(cudaMemcpy(d_scales_.p, sc.data(), sc.size() * sizeof(float), cudaMemcpyHostToDevice));
+  }
   {
     // device quad tree (orb_tree.cu): default; the host tree remains for inputs beyond its shared-memory caps and as the
     // cross-check in the tests (SIVO_B200_ORB_DEVICE_TREE=0 forces it)

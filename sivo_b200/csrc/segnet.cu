@@ -531,6 +531,16 @@ void SegNet::semantic_keys(const sivo_keypoint* kps, int n, int max_static_class
   if (n_keep) *n_keep = kept;
 }
 
+void SegNet::semantic_keys_device(const sivo_keypoint* kps_dev, const long long* count_dev, int cap, int max_static_class, uint8_t* kp_class_dev,
+                                  double* kp_conf_dev, double* kp_entropy_dev, int* keep_idx_dev, long long* n_keep_dev, cudaStream_t s) {
+  if (!kps_dev || !count_dev || cap < 0) fail(SIVO_EINVAL, "semantic_keys: null keypoints or count, or negative capacity %d", cap);
+  if (!last_classes_ || !last_conf_ || !last_ent_) fail(SIVO_EINVAL, "semantic_keys: no segmentation result on the device yet (or a map pointer was NULL)");
+  SIVO_CUDA(cudaSetDevice(device_));
+  if (!s) s = last_stream_;
+  launch_semantic_keys(kps_dev, count_dev, cap, last_classes_, last_conf_, last_ent_, H_, W_, max_static_class, kp_class_dev, kp_conf_dev,
+                       kp_entropy_dev, keep_idx_dev, n_keep_dev, s);
+}
+
 void SegNet::require_whole_frame(const char* what) const {
   if (ns_ < T_)
     fail(SIVO_EINVAL, "%s: this handle is a latency-mode shard owning samples [%d, %d) of %d; run it with "

@@ -94,6 +94,9 @@ class SegNet {
   void variance_finalize(const double* moments_dev, double* variance_dev, cudaStream_t s);
   void semantic_keys(const sivo_keypoint* kps, int n, int max_static_class, uint8_t* kp_class, double* kp_conf, double* kp_entropy,
                      int* keep_idx, int* n_keep);
+  // the same on device buffers with a device-resident count (<= cap), on `s` (NULL = the stream of the last run); no host sync
+  void semantic_keys_device(const sivo_keypoint* kps_dev, const long long* count_dev, int cap, int max_static_class, uint8_t* kp_class_dev,
+                            double* kp_conf_dev, double* kp_entropy_dev, int* keep_idx_dev, long long* n_keep_dev, cudaStream_t s);
   void blob(const std::string& name, float* out, size_t cap, int* n, int* c, int* h, int* w);
   void set_profiling(bool on) { profiling_ = on; }
   float conv_ms = 0, other_ms = 0, reduce_ms = 0, total_ms = 0;

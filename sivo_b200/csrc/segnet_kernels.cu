@@ -728,6 +728,64 @@ void launch_keypoint_lookup(const sivo_keypoint* kps, int n, const uint8_t* clas
   SIVO_CUDA(cudaGetLastError());
 }
 
+// SelectSemanticKeys with a device-resident count: the lookup of k_keypoint_lookup plus the ordered compaction of the kept keys.
+// One block walks the keys in chunks of kSemThreads with a running offset; within a chunk a key's slot is the number of kept keys
+// before it (warp ballots, then the per-warp totals), so keep_idx comes out ascending, exactly as the host loop builds it.
+constexpr int kSemThreads = 512;
+
+__global__ void __launch_bounds__(kSemThreads) k_semantic_keys(const sivo_keypoint* __restrict__ kps, const long long* __restrict__ count,
+                                                              int cap, const uint8_t* __restrict__ classes, const double* __restrict__ conf,
+                                                              const double* __restrict__ ent, int H, int W, int max_static_class,
+                                                              uint8_t* __restrict__ out_class, double* __restrict__ out_conf,
+                                                              double* __restrict__ out_ent, int* __restrict__ keep_idx,
+                                                              long long* __restrict__ n_keep) {
+  __shared__ int warp_kept[kSemThreads / 32];
+  const long long n64 = *count;
+  if (n64 < 0 || n64 > cap) {
+    if (threadIdx.x == 0 && n_keep) *n_keep = -1;
+    return;
+  }
+  const int n = static_cast<int>(n64);
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  int base = 0;  // kept keys in the chunks before this one (the same value in every thread)
+  for (int c0 = 0; c0 < n; c0 += kSemThreads) {
+    const int i = c0 + tid;
+    bool keep = false;
+    if (i < n) {
+      const int col = static_cast<int>(kps[i].x), row = static_cast<int>(kps[i].y);  // static_cast<int>(pt.x / pt.y): truncation
+      const bool ok = col >= 0 && col < W && row >= 0 && row < H;
+      const size_t o = ok ? static_cast<size_t>(row) * W + col : 0;
+      const uint8_t c = ok ? classes[o] : static_cast<uint8_t>(255);
+      if (out_class) out_class[i] = c;
+      if (out_conf) out_conf[i] = ok ? conf[o] : 0.0;
+      if (out_ent) out_ent[i] = ok ? ent[o] : 0.0;
+      keep = c != 255 && static_cast<int>(c) <= max_static_class;  // `detection <= Classes::TERRAIN` (Frame.cc:190)
+    }
+    const unsigned ballot = __ballot_sync(0xffffffffu, keep);
+    if (lane == 0) warp_kept[warp] = __popc(ballot);
+    __syncthreads();
+    int before = 0, total = 0;
+#pragma unroll
+    for (int w = 0; w < kSemThreads / 32; ++w) {
+      const int k = warp_kept[w];
+      before += w < warp ? k : 0;
+      total += k;
+    }
+    if (keep && keep_idx) keep_idx[base + before + __popc(ballot & ((1u << lane) - 1u))] = i;
+    base += total;
+    __syncthreads();  // warp_kept is rewritten by the next chunk
+  }
+  if (tid == 0 && n_keep) *n_keep = base;
+}
+
+void launch_semantic_keys(const sivo_keypoint* kps, const long long* count, int cap, const uint8_t* classes, const double* conf,
+                          const double* ent, int H, int W, int max_static_class, uint8_t* out_class, double* out_conf, double* out_ent,
+                          int* keep_idx, long long* n_keep, cudaStream_t s) {
+  k_semantic_keys<<<1, kSemThreads, 0, s>>>(kps, count, cap, classes, conf, ent, H, W, max_static_class, out_class, out_conf, out_ent,
+                                            keep_idx, n_keep);
+  SIVO_CUDA(cudaGetLastError());
+}
+
 void launch_pad8(TensorView in, TensorView out, cudaStream_t s) {
   if (in.dt != DType::F16 || in.cs != 4 || out.cs != 8 || out.w != in.w + 8) fail(SIVO_EINVAL, "pad8: unexpected tensor layout");
   const size_t total = static_cast<size_t>(out.n) * out.h * out.w;

@@ -60,6 +60,11 @@ void launch_dropout_unpool(TensorView in, int T, const uint8_t* mask, int mask_n
 // per-keypoint gather from the three result maps (Frame.cc:181-186 indexing); out-of-map keypoints get (255, 0, 0)
 void launch_keypoint_lookup(const sivo_keypoint* kps, int n, const uint8_t* classes, const double* conf, const double* ent, int H, int W,
                             uint8_t* out_class, double* out_conf, double* out_ent, cudaStream_t s);
+// the same lookup for *count (device) keypoints, one block, plus keep_idx[0..*n_keep) = the kept keys in ascending order;
+// *count outside [0, cap] writes nothing but *n_keep = -1.  Any output may be NULL.
+void launch_semantic_keys(const sivo_keypoint* kps, const long long* count, int cap, const uint8_t* classes, const double* conf,
+                          const double* ent, int H, int W, int max_static_class, uint8_t* out_class, double* out_conf, double* out_ent,
+                          int* keep_idx, long long* n_keep, cudaStream_t s);
 // [N][H][W][4] half -> zero-padded [N][H][W + 8][8] half (3 zero pixels left, 5 right, channels 4..7 zero)
 void launch_pad8(TensorView in, TensorView out, cudaStream_t s);
 // the three steps input_u8 -> lrn -> pad8 in one pass (same arithmetic, so the same half values)

@@ -49,26 +49,28 @@ __global__ void k_stereo_hamming(const sivo_keypoint* __restrict__ kl, const uin
 // ---- the whole of Frame::ComputeStereoMatches (Frame.cc:444-629) for one left keypoint per warp: Hamming search as
 // above, then the 11x11 SAD slide over +-5 px on the keypoint's pyramid level (windows are centred-intensity
 // differences of u8 pixels, so every L1 distance is an exact integer), parabola sub-pixel fit, disparity gate.
-// The median-based outlier cut (:617-628) needs all matches and runs on the host over the returned SAD distances.
+// The median-based outlier cut (:617-628) needs all matches: the host form does it on the host over the returned SAD distances,
+// the device form in k_stereo_median_cut.
 __device__ __forceinline__ float c_roundf(float v) { return v >= 0.f ? floorf(__fadd_rn(v, 0.5f)) : -floorf(__fadd_rn(-v, 0.5f)); }
 
-__global__ void k_stereo_match(const sivo_keypoint* __restrict__ kl, const uint8_t* __restrict__ dl, int nl,
-                               const sivo_keypoint* __restrict__ kr, const uint8_t* __restrict__ dr, int nr,
-                               const float* __restrict__ scale, const float* __restrict__ inv_scale, const uint8_t* __restrict__ pyr_l,
-                               OrbLevelTable lt_l, const uint8_t* __restrict__ pyr_r, OrbLevelTable lt_r, float mb, float mbf,
-                               float* __restrict__ u_right, float* __restrict__ depth, int* __restrict__ sad_dist) {
-  const int wid = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  if (wid >= nl) return;
-  const sivo_keypoint L = kl[wid];
+// The per-keypoint body shared by both forms; every lane of the warp calls it with the same left keypoint L and descriptor row.
+// kCheckOctave: skip right keypoints whose octave is outside [0, nlevels) (the host form validated them on the host).
+template <bool kCheckOctave>
+__device__ __forceinline__ void stereo_match_key(const sivo_keypoint L, const uint8_t* __restrict__ dl_key, const sivo_keypoint* __restrict__ kr,
+                                                 const uint8_t* __restrict__ dr, int nr, const float* __restrict__ scale,
+                                                 const float* __restrict__ inv_scale, const uint8_t* __restrict__ pyr_l, const OrbLevelTable& lt_l,
+                                                 const uint8_t* __restrict__ pyr_r, const OrbLevelTable& lt_r, float mb, float mbf, int lane,
+                                                 float& out_u, float& out_z, int& out_sad) {
   const int rows = lt_l.lv[0].h;
   const int row = static_cast<int>(L.y);
   const float min_d = 0.f, max_d = __fdiv_rn(mbf, mb);
   const float min_u = __fsub_rn(L.x, max_d), max_u = __fsub_rn(L.x, min_d);
-  const ulonglong4 a = *reinterpret_cast<const ulonglong4*>(dl + static_cast<size_t>(wid) * 32);
+  const ulonglong4 a = *reinterpret_cast<const ulonglong4*>(dl_key);
   unsigned best = (static_cast<unsigned>(kThHigh) << 20) | 0xFFFFFu;
   if (max_u >= 0.f && row >= 0 && row < rows) {
     for (int i = lane; i < nr; i += 32) {
       const sivo_keypoint R = kr[i];
+      if (kCheckOctave && static_cast<unsigned>(R.octave) >= static_cast<unsigned>(lt_l.nlevels)) continue;
       const float band = __fmul_rn(2.0f, scale[R.octave]);
       const int maxr = static_cast<int>(ceilf(__fadd_rn(R.y, band)));
       const int minr = static_cast<int>(floorf(__fsub_rn(R.y, band)));
@@ -82,8 +84,9 @@ __global__ void k_stereo_match(const sivo_keypoint* __restrict__ kl, const uint8
   }
 #pragma unroll
   for (int o = 16; o; o >>= 1) best = min(best, __shfl_xor_sync(0xffffffffu, best, o));
-  float out_u = -1.f, out_z = -1.f;
-  int out_sad = -1;
+  out_u = -1.f;
+  out_z = -1.f;
+  out_sad = -1;
   const int hd = best >> 20;
   if (hd < (kThHigh + 50) / 2) {  // thOrbDist = (TH_HIGH + TH_LOW) / 2 (:448)
     const int ir = best & 0xFFFFFu;
@@ -139,10 +142,129 @@ __global__ void k_stereo_match(const sivo_keypoint* __restrict__ kl, const uint8
       }
     }
   }
+}
+
+__global__ void k_stereo_match(const sivo_keypoint* __restrict__ kl, const uint8_t* __restrict__ dl, int nl,
+                               const sivo_keypoint* __restrict__ kr, const uint8_t* __restrict__ dr, int nr,
+                               const float* __restrict__ scale, const float* __restrict__ inv_scale, const uint8_t* __restrict__ pyr_l,
+                               OrbLevelTable lt_l, const uint8_t* __restrict__ pyr_r, OrbLevelTable lt_r, float mb, float mbf,
+                               float* __restrict__ u_right, float* __restrict__ depth, int* __restrict__ sad_dist) {
+  const int wid = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (wid >= nl) return;
+  float out_u, out_z;
+  int out_sad;
+  stereo_match_key<false>(kl[wid], dl + static_cast<size_t>(wid) * 32, kr, dr, nr, scale, inv_scale, pyr_l, lt_l, pyr_r, lt_r, mb, mbf,
+                          lane, out_u, out_z, out_sad);
   if (lane == 0) {
     u_right[wid] = out_u;
     depth[wid] = out_z;
     sad_dist[wid] = out_sad;
+  }
+}
+
+// Device form: counts and (optionally) the left keypoint indices live on the device.  Warp j handles left keypoint keep_idx[j]
+// (j when keep_idx is NULL) for j < min(*n_left, cap_l); right keypoints [0, min(*n_right, cap_r)).  A left keypoint whose octave
+// or index is out of range stays unmatched.  Same arithmetic as k_stereo_match through stereo_match_key.
+__global__ void k_stereo_match_dev(const sivo_keypoint* __restrict__ kl, const uint8_t* __restrict__ dl, const int* __restrict__ keep_idx,
+                                   const long long* __restrict__ n_left, int cap_l, const sivo_keypoint* __restrict__ kr,
+                                   const uint8_t* __restrict__ dr, const long long* __restrict__ n_right, int cap_r,
+                                   const float* __restrict__ scale, const float* __restrict__ inv_scale, const uint8_t* __restrict__ pyr_l,
+                                   OrbLevelTable lt_l, const uint8_t* __restrict__ pyr_r, OrbLevelTable lt_r, float mb, float mbf,
+                                   float* __restrict__ u_right, float* __restrict__ depth, int* __restrict__ sad_dist) {
+  const int wid = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (wid >= cap_l || wid >= *n_left) return;
+  const long long nr64 = *n_right;
+  const int nr = nr64 < 0 ? 0 : static_cast<int>(min(nr64, static_cast<long long>(cap_r)));
+  const int k = keep_idx ? keep_idx[wid] : wid;
+  float out_u = -1.f, out_z = -1.f;
+  int out_sad = -1;
+  if (k >= 0 && k < cap_l) {
+    const sivo_keypoint L = kl[k];
+    if (static_cast<unsigned>(L.octave) < static_cast<unsigned>(lt_l.nlevels))
+      stereo_match_key<true>(L, dl + static_cast<size_t>(k) * 32, kr, dr, nr, scale, inv_scale, pyr_l, lt_l, pyr_r, lt_r, mb, mbf, lane,
+                             out_u, out_z, out_sad);
+  }
+  if (lane == 0) {
+    u_right[wid] = out_u;
+    depth[wid] = out_z;
+    sad_dist[wid] = out_sad;
+  }
+}
+
+// ---- median-based outlier cut (Frame.cc:617-628) on the device, one block.  m = number of matched keys (SAD >= 0); the median
+// is the SAD at index m / 2 of the ascending order.  Every SAD is an integer <= 121 * 510 < 2^16, so an exact two-pass radix
+// select (high byte, then low byte, 256-bin shared histograms) finds it without sorting.  th = 1.5f * 1.4f * median in float as
+// on the host; every matched key with (float) sad >= th -- exactly the tail the host loop walks -- is unmatched (-1).
+constexpr int kCutThreads = 1024;
+
+// warp 0: the bin holding the element of rank `k` (0-based, ascending) of the 256-bin histogram, and its rank within that bin
+__device__ __forceinline__ void hist_select(const int* hist, int k, int lane, int* bin, int* rank_in_bin) {
+  int c[8], sum = 0;
+#pragma unroll
+  for (int b = 0; b < 8; ++b) { c[b] = hist[lane * 8 + b]; sum += c[b]; }
+  int incl = sum;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int v = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += v;
+  }
+  int before = incl - sum;
+  if (k >= before && k < incl) {
+#pragma unroll
+    for (int b = 0; b < 8; ++b) {
+      if (k < before + c[b]) { *bin = lane * 8 + b; *rank_in_bin = k - before; break; }
+      before += c[b];
+    }
+  }
+}
+
+__global__ void __launch_bounds__(kCutThreads) k_stereo_median_cut(const long long* __restrict__ n_left, int cap, const int* __restrict__ sad,
+                                                                   float* __restrict__ u_right, float* __restrict__ depth) {
+  __shared__ int hist[256];
+  __shared__ int s_m, s_bin, s_rank;
+  const long long n64 = *n_left;
+  const int n = n64 < 0 ? 0 : static_cast<int>(min(n64, static_cast<long long>(cap)));
+  const int tid = threadIdx.x, lane = tid & 31;
+  if (tid < 256) hist[tid] = 0;
+  __syncthreads();
+  for (int i = tid; i < n; i += kCutThreads) {
+    const int s = sad[i];
+    if (s >= 0) atomicAdd(&hist[s >> 8], 1);
+  }
+  __syncthreads();
+  if (tid < 32) {
+    int m = 0;
+#pragma unroll
+    for (int b = 0; b < 8; ++b) m += hist[lane * 8 + b];
+#pragma unroll
+    for (int o = 16; o; o >>= 1) m += __shfl_xor_sync(0xffffffffu, m, o);
+    if (lane == 0) s_m = m;
+    if (m > 0) hist_select(hist, m / 2, lane, &s_bin, &s_rank);
+  }
+  __syncthreads();
+  if (s_m == 0) return;  // nothing matched: nothing to cut
+  const int hi = s_bin;
+  if (tid < 256) hist[tid] = 0;
+  __syncthreads();
+  for (int i = tid; i < n; i += kCutThreads) {
+    const int s = sad[i];
+    if (s >= 0 && (s >> 8) == hi) atomicAdd(&hist[s & 255], 1);
+  }
+  __syncthreads();
+  if (tid < 32) {
+    const int k = s_rank;
+    __syncwarp();  // every lane has read the rank before one of them overwrites it
+    hist_select(hist, k, lane, &s_bin, &s_rank);
+  }
+  __syncthreads();
+  const float median = static_cast<float>((hi << 8) | s_bin);
+  const float th = 1.5f * 1.4f * median;
+  for (int i = tid; i < n; i += kCutThreads) {
+    const int s = sad[i];
+    if (s >= 0 && static_cast<float>(s) >= th) {
+      u_right[i] = -1.f;
+      depth[i] = -1.f;
+    }
   }
 }
 
@@ -339,5 +461,27 @@ void stereo_match(const Orb& left, const Orb& right, const sivo_keypoint* kl, co
     u_right[v[i].second] = -1.f;
     depth[v[i].second] = -1.f;
   }
+}
+
+// ComputeStereoMatches on device-resident keypoints, descriptors and counts, enqueued on `s` (NULL: the left extractor's stream)
+// without a host synchronisation.  `s` first waits for everything enqueued so far on both extractors' streams (their pyramids
+// are read).  The SAD distances go to the left extractor's scratch.
+void stereo_match_device(Orb& left, Orb& right, const sivo_keypoint* kl, const uint8_t* dl, const int* keep_idx, const long long* n_left,
+                         const sivo_keypoint* kr, const uint8_t* dr, const long long* n_right, float mb, float mbf, float* u_right,
+                         float* depth, cudaStream_t s) {
+  if (!left.has_run() || !right.has_run()) fail(SIVO_EINVAL, "stereo: run both extractors first");
+  if (left.device() != right.device() || left.nlevels() != right.nlevels()) fail(SIVO_EINVAL, "stereo: extractors differ");
+  if (!(mb > 0.f) || !(mbf > 0.f)) fail(SIVO_EINVAL, "stereo: bad arguments");
+  SIVO_CUDA(cudaSetDevice(left.device()));
+  if (!s) s = left.stream();
+  left.stream_wait(s);
+  right.stream_wait(s);
+  const int cap_l = left.capacity(), cap_r = right.capacity();
+  k_stereo_match_dev<<<ceil_div(cap_l * 32, 128), 128, 0, s>>>(kl, dl, keep_idx, n_left, cap_l, kr, dr, n_right, cap_r, left.dev_scale(),
+                                                               left.dev_inv_scale(), left.dev_pyramid(), left.levels(), right.dev_pyramid(),
+                                                               right.levels(), mb, mbf, u_right, depth, left.stereo_sad());
+  SIVO_CUDA(cudaGetLastError());
+  k_stereo_median_cut<<<1, kCutThreads, 0, s>>>(n_left, cap_l, left.stereo_sad(), u_right, depth);
+  SIVO_CUDA(cudaGetLastError());
 }
 }  // namespace sivo

@@ -203,6 +203,17 @@ def stereo_match(left: ORBextractor, right: ORBextractor, kp_left, desc_left, kp
     return u, z
 
 
+def stereo_match_device(left: ORBextractor, right: ORBextractor, kp_left_ptr: int, desc_left_ptr: int, keep_idx_ptr: int,
+                        n_left_ptr: int, kp_right_ptr: int, desc_right_ptr: int, n_right_ptr: int, mb: float, mbf: float,
+                        u_right_ptr: int, depth_ptr: int, stream: int = 0):
+    """stereo_match on device buffers (sivo_stereo_match_device): output j belongs to left keypoint keep_idx[j] (keep_idx_ptr 0:
+    keypoint j) for j < the int64 count at n_left_ptr; float32 outputs of left.capacity() entries.  `stream` (0 = the left
+    extractor's stream) first waits for both extractors' work; the next enqueue_device on either must be ordered after this call
+    (wait_for_stream).  No host synchronisation."""
+    L.check(L.lib().sivo_stereo_match_device(left._h, right._h, kp_left_ptr, desc_left_ptr, keep_idx_ptr or None, n_left_ptr, kp_right_ptr,
+                                             desc_right_ptr, n_right_ptr, mb, mbf, u_right_ptr, depth_ptr, stream or None))
+
+
 def hamming_best2(query_desc, train_desc, cand_offsets, cand_idx, train_level=None, device: int = 0) -> np.ndarray:
     """Inner loop of ORBmatcher::SearchByProjection & co (ORBmatcher.cc:79-113) for all queries at once.
     Returns int32 [n_query, 5] = (bestIdx, bestDist, bestLevel, bestDist2, bestLevel2)."""

@@ -129,6 +129,16 @@ class BayesianSegNet:
                                                   ent.ctypes.data_as(C.c_void_p), keep.ctypes.data_as(C.c_void_p), C.byref(m)))
         return cls, conf, ent, keep[:m.value].copy()
 
+    def semantic_keys_device(self, kps_ptr: int, count_ptr: int, cap: int, max_static_class: int = 8, class_ptr: int = 0,
+                             conf_ptr: int = 0, ent_ptr: int = 0, keep_ptr: int = 0, n_keep_ptr: int = 0, stream: int = 0):
+        """semantic_keys on device buffers (sivo_segnet_semantic_keys_device): kps_ptr holds the keypoint records and count_ptr
+        their int64 count (e.g. what ORBextractor.enqueue_device wrote), cap the capacity of the output buffers (u8 classes,
+        float64 confidence / entropy, int32 keep indices; 0 = not wanted).  *n_keep_ptr (int64) receives the kept count, or -1
+        if the count exceeds cap.  Enqueued on `stream` (0 = the stream of the last run) without a host synchronisation."""
+        L.check(L.lib().sivo_segnet_semantic_keys_device(self._h, kps_ptr, count_ptr, int(cap), int(max_static_class), class_ptr or None,
+                                                         conf_ptr or None, ent_ptr or None, keep_ptr or None, n_keep_ptr or None,
+                                                         stream or None))
+
     def run_device(self, bgr_ptr: int, classes_ptr: int, conf_ptr: int, ent_ptr: int, stream: int = 0):
         L.check(L.lib().sivo_segnet_run_device(self._h, C.c_void_p(bgr_ptr), C.c_void_p(classes_ptr), C.c_void_p(conf_ptr),
                                                C.c_void_p(ent_ptr), C.c_void_p(stream)))
