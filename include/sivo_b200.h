@@ -266,6 +266,52 @@ int sivo_stereo_match_device(sivo_orb_t* left, sivo_orb_t* right, const sivo_key
                              const uint8_t* desc_right_device, const long long* n_right_device, float mb, float mbf,
                              float* u_right_device, float* depth_device, void* stream);
 
+/* ---- SIVO's information-based map-point selection (Tracking::StereoInitialization, Tracking.cc:470-520, threshold 0;
+ * Tracking::CreateNewKeyFrame, Tracking.cc:953-1000, threshold mThEntropyReduction) -----------------------------------
+ * For semantic key j with keypoint k, depth z = depth[j], classification entropy H and s2 = sigma2[k.octave] (the left
+ * extractor's GetScaleSigmaSquares):
+ *   valid iff z > 0 (NaN is invalid) and 0 <= octave < nlevels; an invalid key gets world = NaN x 3, reduction = NaN.
+ *   world = Frame::UnprojectStereo (Frame.cc:631-645) in float: x = ((u - cx) * z) * invfx, y = ((v - cy) * z) * invfy,
+ *           w_r = ((Rwc[r][0] * x + Rwc[r][1] * y) + Rwc[r][2] * z) + Ow[r], every operation rounded to float (cv::gemm).
+ *   J     = computeStereoJacobianPose(fx, fy, mb, wX, wY, wZ) (sivo_helpers.cpp:64-88) in double, all zeros when wZ == 0.  As in
+ *           the reference, it is given the WORLD point where the helper expects camera coordinates (equal at the identity pose).
+ *   M     = [[S, S J^T], [J S, (J S) J^T + s2 I]] (9 x 9; S = sigma_cw), products summed over k in ascending order.
+ *   MI    = 0.5 * log2((det S * det M33) / det M): det of the 3 x 3 by cofactors along the first row, of the 6 x 6 / 9 x 9 by LU
+ *           with partial pivoting (the first row with the largest |a|; a zero pivot column is skipped).
+ *   reduction = MI - H; key j is selected iff reduction > threshold (a NaN is never selected).
+ * Steps 2-5 use no fused multiply-add, so every intermediate is the IEEE float / double result of the operation as written;
+ * log2 is within an ulp of glibc's.  selected[0 .. n_selected) = the selected j, ascending: the order in which the reference
+ * creates map points.  CreateNewKeyFrame's test for an existing map point stays with the caller (filter the selected list).
+ * Any output may be NULL; the camera is copied at call time.  SIVO_EINVAL for a NULL handle, input or camera, or n < 0. */
+typedef struct sivo_info_camera {          /* the Frame's own members */
+  float fx, fy, cx, cy, invfx, invfy, mb;  /* Frame.cc:166-172 */
+  float Rwc[9];                            /* mRwc, row-major */
+  float Ow[3];                             /* mOw */
+  double sigma_cw[36];                     /* mSigmacw, row-major 6x6 */
+} sivo_info_camera;
+
+/* Host buffers gathered per semantic key: kps = mvKeysSemantic, depth = mvDepth, entropy = mEntropy at ((int) y, (int) x); world
+ * 3n floats, reduction n doubles, selected n ints.  Returns when done. */
+int sivo_info_select(const sivo_orb_t* left, const sivo_keypoint* kps, const float* depth, const double* entropy, int n,
+                     const sivo_info_camera* cam, double threshold, float* world, double* reduction, int* selected, int* n_selected);
+/* The same selection on device buffers, e.g. the Frame tail's: semantic key j < *n_keep_device is extractor key keep_idx_device[j]
+ * (j when keep_idx_device is NULL) of kps_device; its entropy is kp_entropy_device[keep_idx[j]] as sivo_segnet_semantic_keys_device
+ * writes it, its depth depth_device[j] as sivo_stereo_match_device writes it.  Outputs as in the host form, each with room for
+ * sivo_orb_capacity(left) keys; the values equal the host form's on the same keys gathered on the host, bit for bit.
+ * *n_keep_device (int64) is read on the device and clamped to the capacity; a negative count (the -1 of
+ * sivo_segnet_semantic_keys_device) writes nothing except *n_selected_device = -1.  A key index outside the capacity is invalid.
+ * Ordering: runs on `stream` (NULL = the left extractor's stream) with no host synchronisation and no waits of its own, so every
+ * input must be ordered before it on `stream` (on the Frame tail's stream they are).  The per-key decisions go to scratch on the
+ * left extractor, so calls that share a left extractor must be ordered among themselves, and its next sivo_orb_enqueue_device
+ * must be ordered after this call (sivo_orb_wait_for_stream(left, stream) after it). */
+int sivo_info_select_device(const sivo_orb_t* left, const sivo_keypoint* kps_device, const double* kp_entropy_device,
+                            const int* keep_idx_device, const long long* n_keep_device, const float* depth_device,
+                            const sivo_info_camera* cam, double threshold, float* world_device, double* reduction_device,
+                            int* selected_device, long long* n_selected_device, void* stream);
+/* Test hook: the host form's world points and the three determinants per key (det S, det M33, det M; NaN for an invalid key). */
+int sivo_dbg_info_terms(const sivo_orb_t* left, const sivo_keypoint* kps, const float* depth, int n, const sivo_info_camera* cam,
+                        float* world, double* det_state, double* det_meas, double* det_joint);
+
 /* Best / second-best match over per-query candidate lists -- the inner loop of ORBmatcher::SearchByProjection
  * (ORBmatcher.cc:79-113), its last-frame / keyframe variants (:1278-, :1420-), SearchForTriangulation (:631-) and
  * SearchBySim3 (next row 4).  Query i's candidates are cand_idx[cand_offsets[i] .. cand_offsets[i+1]) (indices into the

@@ -2,3 +2,4 @@
 Host-side mirrors of the reference's two operators over the C-ABI of libsivo_b200.so."""
 from .segnet import BayesianSegNet, BayesianSegNetParams, sample_ranges  # noqa: F401
 from .orb import ORBextractor, distribute_octtree, stereo_hamming, stereo_match, stereo_match_device, KP_DTYPE  # noqa: F401
+from .info import InfoCamera, info_select, info_select_device, make_camera  # noqa: F401

@@ -32,6 +32,12 @@ class SegnetOptions(C.Structure):
                 ("engine", C.c_int32), ("keep_blobs", C.c_int32), ("reserved", C.c_int32)]
 
 
+class InfoCamera(C.Structure):
+    """sivo_info_camera: the Frame members the information selection reads (Rwc row-major, Sigma_cw row-major 6x6)."""
+    _fields_ = [("fx", C.c_float), ("fy", C.c_float), ("cx", C.c_float), ("cy", C.c_float), ("invfx", C.c_float),
+                ("invfy", C.c_float), ("mb", C.c_float), ("Rwc", C.c_float * 9), ("Ow", C.c_float * 3), ("sigma_cw", C.c_double * 36)]
+
+
 def build(verbose: bool = False) -> str:
     """Compiles the library in-tree with nvcc for sm_90a (cross-compiles without a GPU)."""
     r = subprocess.run(["make", "-C", os.path.join(_HERE, "csrc"), "-j8"], capture_output=True, text=True)
@@ -59,6 +65,9 @@ def lib() -> C.CDLL:
         vp, i32, f32 = C.c_void_p, C.c_int, C.c_float
         _lib.sivo_segnet_semantic_keys_device.argtypes = [vp, vp, vp, i32, i32, vp, vp, vp, vp, vp, vp]
         _lib.sivo_stereo_match_device.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, f32, f32, vp, vp, vp]
+        _lib.sivo_info_select.argtypes = [vp, vp, vp, vp, i32, vp, C.c_double, vp, vp, vp, vp]
+        _lib.sivo_info_select_device.argtypes = [vp, vp, vp, vp, vp, vp, vp, C.c_double, vp, vp, vp, vp, vp]
+        _lib.sivo_dbg_info_terms.argtypes = [vp, vp, vp, i32, vp, vp, vp, vp, vp]
     return _lib
 
 

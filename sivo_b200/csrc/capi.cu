@@ -23,6 +23,13 @@ void stereo_match(const Orb& left, const Orb& right, const sivo_keypoint* kl, co
 void stereo_match_device(Orb& left, Orb& right, const sivo_keypoint* kl, const uint8_t* dl, const int* keep_idx, const long long* n_left,
                          const sivo_keypoint* kr, const uint8_t* dr, const long long* n_right, float mb, float mbf, float* u_right,
                          float* depth, cudaStream_t s);
+void info_select(const Orb& left, const sivo_keypoint* kps, const float* depth, const double* entropy, int n, const sivo_info_camera& cam,
+                 double threshold, float* world, double* reduction, int* selected, int* n_selected);
+void info_terms(const Orb& left, const sivo_keypoint* kps, const float* depth, int n, const sivo_info_camera& cam, float* world,
+                double* det_state, double* det_meas, double* det_joint);
+void info_select_device(const Orb& left, const sivo_keypoint* kps, const double* kp_entropy, const int* keep_idx, const long long* n_keep,
+                        const float* depth, const sivo_info_camera& cam, double threshold, float* world, double* reduction, int* selected,
+                        long long* n_selected, cudaStream_t s);
 }  // namespace sivo
 
 using namespace sivo;
@@ -472,6 +479,34 @@ int sivo_stereo_match_device(sivo_orb_t* left, sivo_orb_t* right, const sivo_key
       fail(SIVO_EINVAL, "null argument");
     stereo_match_device(*left->impl, *right->impl, kp_left_device, desc_left_device, keep_idx_device, n_left_device, kp_right_device,
                         desc_right_device, n_right_device, mb, mbf, u_right_device, depth_device, static_cast<cudaStream_t>(stream));
+  });
+}
+
+// ---------------------------------------------------------------------------------------- information selection
+int sivo_info_select(const sivo_orb_t* left, const sivo_keypoint* kps, const float* depth, const double* entropy, int n,
+                     const sivo_info_camera* cam, double threshold, float* world, double* reduction, int* selected, int* n_selected) {
+  return guarded([&] {
+    if (!left || !cam || n < 0 || (n && (!kps || !depth || !entropy))) fail(SIVO_EINVAL, "info_select: null argument or n < 0");
+    info_select(*left->impl, kps, depth, entropy, n, *cam, threshold, world, reduction, selected, n_selected);
+  });
+}
+
+int sivo_info_select_device(const sivo_orb_t* left, const sivo_keypoint* kps_device, const double* kp_entropy_device,
+                            const int* keep_idx_device, const long long* n_keep_device, const float* depth_device,
+                            const sivo_info_camera* cam, double threshold, float* world_device, double* reduction_device,
+                            int* selected_device, long long* n_selected_device, void* stream) {
+  return guarded([&] {
+    if (!left || !kps_device || !kp_entropy_device || !n_keep_device || !depth_device || !cam) fail(SIVO_EINVAL, "info_select: null argument");
+    info_select_device(*left->impl, kps_device, kp_entropy_device, keep_idx_device, n_keep_device, depth_device, *cam, threshold, world_device,
+                       reduction_device, selected_device, n_selected_device, static_cast<cudaStream_t>(stream));
+  });
+}
+
+int sivo_dbg_info_terms(const sivo_orb_t* left, const sivo_keypoint* kps, const float* depth, int n, const sivo_info_camera* cam,
+                        float* world, double* det_state, double* det_meas, double* det_joint) {
+  return guarded([&] {
+    if (!left || !cam || n < 0 || (n && (!kps || !depth))) fail(SIVO_EINVAL, "info_terms: null argument or n < 0");
+    info_terms(*left->impl, kps, depth, n, *cam, world, det_state, det_meas, det_joint);
   });
 }
 

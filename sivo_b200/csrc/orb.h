@@ -2,6 +2,7 @@
 // orb_kernels.cu.  One instance = one CUDA stream + its own workspace, so two instances can run
 // concurrently from two threads as Frame.cc:126-129 does.
 #pragma once
+#include <algorithm>
 #include <condition_variable>
 #include <cstdlib>
 #include <functional>
@@ -87,6 +88,42 @@ void orb_launch_distribute(const uint32_t* cand, const int* level_off, const uin
 void orb_tree_configure();  // raises k_distribute's dynamic shared-memory limit on the current device
 void orb_upload_pattern();  // copies the rBRIEF pair table into constant memory (once per device)
 
+// Per-thread, per-device workspace of the host-buffer stereo / Hamming / information-selection entry points: one arena that only
+// grows and one non-blocking stream (stereo.cu).  Each such call takes its buffers after begin() and synchronises before it
+// returns, so the calls of one thread share it.
+// (Allocating and freeing half a dozen buffers per call and running on the legacy default stream synchronises the whole device,
+// i.e. serialises every per-frame call against the SegNet graph and the extractors' streams.)
+struct StereoWs {
+  int device = -1;
+  cudaStream_t stream = nullptr;
+  DevBuf arena;
+  size_t used = 0;
+  void begin(int dev, size_t bytes_needed) {
+    SIVO_CUDA(cudaSetDevice(dev));
+    if (device != dev) {
+      if (stream) { cudaSetDevice(device); cudaStreamDestroy(stream); cudaSetDevice(dev); }
+      arena.release();
+      SIVO_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
+      device = dev;
+    }
+    if (arena.bytes < bytes_needed) {
+      SIVO_CUDA(cudaStreamSynchronize(stream));
+      arena.alloc(bytes_needed + bytes_needed / 2);
+    }
+    used = 0;
+  }
+  template <class T> T* take(size_t count) {
+    used = (used + 255) & ~static_cast<size_t>(255);
+    T* p = reinterpret_cast<T*>(arena.as<uint8_t>() + used);
+    used += std::max<size_t>(count, 1) * sizeof(T);
+    if (used > arena.bytes) fail(SIVO_ENOMEM, "stereo workspace accounting");
+    return p;
+  }
+  ~StereoWs() { if (stream) { cudaSetDevice(device); cudaStreamDestroy(stream); } }
+};
+StereoWs& stereo_ws();
+inline size_t pad256(size_t b) { return (std::max<size_t>(b, 1) + 255) & ~static_cast<size_t>(255); }
+
 // ---- host (orb_host.cu)
 struct OrbTables {
   std::vector<float> scale, inv_scale, sigma2, inv_sigma2;
@@ -133,6 +170,8 @@ class Orb {
   const float* dev_scale() const { return d_scales_.as<float>(); }
   const float* dev_inv_scale() const { return d_scales_.as<float>() + nlevels_; }
   int* stereo_sad() const { return d_stereo_sad_.as<int>(); }
+  // capacity() bytes of scratch for the device information selection's per-key decisions (ordered like stereo_sad())
+  uint8_t* info_flags() const { return d_info_flags_.as<uint8_t>(); }
   float device_ms = 0, tree_ms = 0;
   int launches = 0;
 
@@ -157,7 +196,7 @@ class Orb {
   cudaStream_t stream_ = nullptr;
   cudaEvent_t ev_[4] = {nullptr, nullptr, nullptr, nullptr};
   DevBuf d_gray_, d_pyr_, d_blur_, d_cells_, d_cell_count_, d_cell_items_, d_cell_offset_, d_level_off_, d_cand_,
-      d_sel_, d_umax_, d_angles_, d_desc_, d_scales_, d_stereo_sad_;
+      d_sel_, d_umax_, d_angles_, d_desc_, d_scales_, d_stereo_sad_, d_info_flags_;
   PinnedBuf h_gray_, h_cand_, h_level_off_, h_sel_, h_angles_, h_desc_, h_pyr_;
   size_t pyr_bytes_ = 0, flat_bytes_ = 0;
   int cand_cap_ = 0, sel_cap_ = 0;

@@ -316,6 +316,7 @@ Orb::Orb(int nfeatures, float scale_factor, int nlevels, int ini_th, int min_th,
   h_angles_.ensure(sel_cap_ * sizeof(float));
   h_desc_.ensure(static_cast<size_t>(sel_cap_) * 32);
   d_stereo_sad_.alloc(sel_cap_ * sizeof(int));
+  d_info_flags_.alloc(sel_cap_);
   {
     std::vector<float> sc(tab_.scale);
     sc.insert(sc.end(), tab_.inv_scale.begin(), tab_.inv_scale.end());

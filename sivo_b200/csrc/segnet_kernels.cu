@@ -4,6 +4,7 @@
 #include <cuda_fp16.h>
 
 #include "common.h"
+#include "compact.cuh"
 #include "philox.cuh"
 #include "segnet_kernels.h"
 
@@ -729,8 +730,8 @@ void launch_keypoint_lookup(const sivo_keypoint* kps, int n, const uint8_t* clas
 }
 
 // SelectSemanticKeys with a device-resident count: the lookup of k_keypoint_lookup plus the ordered compaction of the kept keys.
-// One block walks the keys in chunks of kSemThreads with a running offset; within a chunk a key's slot is the number of kept keys
-// before it (warp ballots, then the per-warp totals), so keep_idx comes out ascending, exactly as the host loop builds it.
+// One block walks the keys in chunks of kSemThreads with a running offset (compact_chunk), so keep_idx comes out ascending,
+// exactly as the host loop builds it.
 constexpr int kSemThreads = 512;
 
 __global__ void __launch_bounds__(kSemThreads) k_semantic_keys(const sivo_keypoint* __restrict__ kps, const long long* __restrict__ count,
@@ -761,19 +762,7 @@ __global__ void __launch_bounds__(kSemThreads) k_semantic_keys(const sivo_keypoi
       if (out_ent) out_ent[i] = ok ? ent[o] : 0.0;
       keep = c != 255 && static_cast<int>(c) <= max_static_class;  // `detection <= Classes::TERRAIN` (Frame.cc:190)
     }
-    const unsigned ballot = __ballot_sync(0xffffffffu, keep);
-    if (lane == 0) warp_kept[warp] = __popc(ballot);
-    __syncthreads();
-    int before = 0, total = 0;
-#pragma unroll
-    for (int w = 0; w < kSemThreads / 32; ++w) {
-      const int k = warp_kept[w];
-      before += w < warp ? k : 0;
-      total += k;
-    }
-    if (keep && keep_idx) keep_idx[base + before + __popc(ballot & ((1u << lane) - 1u))] = i;
-    base += total;
-    __syncthreads();  // warp_kept is rewritten by the next chunk
+    base = compact_chunk<kSemThreads>(keep, i, base, lane, warp, warp_kept, keep_idx);
   }
   if (tid == 0 && n_keep) *n_keep = base;
 }

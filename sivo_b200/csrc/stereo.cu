@@ -268,43 +268,12 @@ __global__ void __launch_bounds__(kCutThreads) k_stereo_median_cut(const long lo
   }
 }
 
-// Per-thread, per-device workspace of the stereo / Hamming entry points: one arena that only grows and one non-blocking stream.
-// (Allocating and freeing half a dozen buffers per call and running on the legacy default stream synchronises the whole device,
-// i.e. serialises every per-frame call against the SegNet graph and the extractors' streams.)
-struct StereoWs {
-  int device = -1;
-  cudaStream_t stream = nullptr;
-  DevBuf arena;
-  size_t used = 0;
-  void begin(int dev, size_t bytes_needed) {
-    SIVO_CUDA(cudaSetDevice(dev));
-    if (device != dev) {
-      if (stream) { cudaSetDevice(device); cudaStreamDestroy(stream); cudaSetDevice(dev); }
-      arena.release();
-      SIVO_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
-      device = dev;
-    }
-    if (arena.bytes < bytes_needed) {
-      SIVO_CUDA(cudaStreamSynchronize(stream));
-      arena.alloc(bytes_needed + bytes_needed / 2);
-    }
-    used = 0;
-  }
-  template <class T> T* take(size_t count) {
-    used = (used + 255) & ~static_cast<size_t>(255);
-    T* p = reinterpret_cast<T*>(arena.as<uint8_t>() + used);
-    used += std::max<size_t>(count, 1) * sizeof(T);
-    if (used > arena.bytes) fail(SIVO_ENOMEM, "stereo workspace accounting");
-    return p;
-  }
-  ~StereoWs() { if (stream) { cudaSetDevice(device); cudaStreamDestroy(stream); } }
-};
+}  // namespace
+
 StereoWs& stereo_ws() {
   static thread_local StereoWs ws;
   return ws;
 }
-inline size_t pad256(size_t b) { return (std::max<size_t>(b, 1) + 255) & ~static_cast<size_t>(255); }
-}  // namespace
 
 void stereo_hamming(int device, const sivo_keypoint* left, const uint8_t* dl, int nl, const sivo_keypoint* right,
                     const uint8_t* dr, int nr, const float* scale, int nlevels, int rows, float min_d, float max_d,
