@@ -23,6 +23,7 @@
 //    logits -- while the other consumer's MMAs keep the tensor core busy.
 //  * Constants (bias, BN, classifier weights) are kernel parameters: the epilogue reads them from the constant bank and
 //    leaves the shared-memory data path to the MMA operand reads.
+//  * The 64 -> 16 float-logits layers (K = 3, 7) run on k_conv_stack instead: tap rows stacked along N, resident weights.
 #include <cuda.h>
 #include <cuda_fp16.h>
 
@@ -64,6 +65,7 @@ struct TcParams {
                            // therefore cut into segments of (A chunk, seg_rows tap rows) that each start a fresh accumulator,
                            // and the epilogue sums the segments in registers with round-to-nearest adds.
   int pairs_per_cta;       // row blocks one CTA walks
+  int rows_per_cta;        // k_conv_stack: output rows one CTA emits, a piece of the flattened (image, strip, row) range
   int strips;              // ceil(W / 128)
   int relu, has_bn, has_drop;
   float slope;
@@ -183,6 +185,29 @@ __device__ __forceinline__ void wgmma(float (&d)[64], uint64_t a, uint64_t b) {
         "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
       : "l"(a), "l"(b));
 }
+// k_conv_stack's MMA: D[64 x 16 K] += A[64 x 16] * B[16 x 16 K], column block j into ring slot acc[j].  The slots keep fixed
+// registers: HGMMA takes its accumulators as one register range, and ptxas serialises every wgmma of a kernel whose MMAs
+// name different sub-ranges or orders of the same registers.
+#define SIVO_ACC8(s) "+f"(acc[s][0]), "+f"(acc[s][1]), "+f"(acc[s][2]), "+f"(acc[s][3]), "+f"(acc[s][4]), "+f"(acc[s][5]), \
+                     "+f"(acc[s][6]), "+f"(acc[s][7])
+__device__ __forceinline__ void wgmma_stack(float (&acc)[7][8], uint64_t a, uint64_t b) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n112k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+      "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, "
+      "%47, %48, %49, %50, %51, %52, %53, %54, %55}, %56, %57, 1, 1, 1, 0, 0;"
+      : SIVO_ACC8(0), SIVO_ACC8(1), SIVO_ACC8(2), SIVO_ACC8(3), SIVO_ACC8(4), SIVO_ACC8(5), SIVO_ACC8(6)
+      : "l"(a), "l"(b));
+}
+__device__ __forceinline__ void wgmma_stack(float (&acc)[3][8], uint64_t a, uint64_t b) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n48k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, "
+      "%24, %25, 1, 1, 1, 0, 0;"
+      : SIVO_ACC8(0), SIVO_ACC8(1), SIVO_ACC8(2)
+      : "l"(a), "l"(b));
+}
+#undef SIVO_ACC8
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
@@ -544,6 +569,183 @@ k_conv_tc(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUt
   }
 }
 
+// k_conv_stack's shared memory: the resident weights (per kw the tap rows kh = 0 .. K-1, 0 .. K-2 of [16 cout][64 cin] half:
+// 2 K - 1 blocks of 2 KB), then as many halo-row slots as fit, then the mbarriers.
+__host__ __device__ constexpr int stack_w_bytes(int K) { return K * (2 * K - 1) * 16 * 128; }
+__host__ __device__ constexpr int stack_slots(int K) { return (227 * 1024 - 1024 - 256 - stack_w_bytes(K)) / kSlotBytes; }
+__host__ __device__ constexpr int stack_smem_bytes(int K) {
+  return 1024 + stack_w_bytes(K) + stack_slots(K) * kSlotBytes + (2 * stack_slots(K) + 2) * 8;
+}
+
+// Epilogue of one output row of k_conv_stack for one consumer thread: pixels m0 and m0 + 8 (h = 0, 1), channels 8 j + 2 q + e.
+__device__ __forceinline__ void epilogue_row16(const TcParams& p, const TcConsts& cst, const float (&a)[8], int img, int y, int x_m0, int q) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int x = x_m0 + 8 * h;
+    const size_t pix = (static_cast<size_t>(img) * p.H + y) * p.W + x;
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const int c = 8 * j + 2 * q;
+      const float2 v = make_float2(affine(p, cst, a[4 * j + 2 * h], c), affine(p, cst, a[4 * j + 2 * h + 1], c + 1));
+      if (x < p.W) *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + pix * p.cout_total + c) = v;
+    }
+  }
+}
+
+// One input row of k_conv_stack at phase PH: its MMAs, then output row r - (K - 1) (slot K-1-PH) moved out to `v` and its
+// slot zeroed.  The epilogue runs on `v` outside the phase switch, once.
+template <int K, int PH>
+__device__ __forceinline__ void stack_row(float (&acc)[K][8], uint32_t a_row, uint32_t w_base, float (&v)[8]) {
+  if constexpr (PH < K) {
+    constexpr int kKwBytes = (2 * K - 1) * 16 * 128;  // the resident rows of one tap column
+    wgmma_fence();
+#pragma unroll
+    for (int kw = 0; kw < K; ++kw)
+#pragma unroll
+      for (int k = 0; k < 4; ++k)  // B = tap rows PH .. PH + K - 1 (mod K) of tap column kw
+        wgmma_stack(acc, make_desc(a_row + kw * 128 + 32 * k), make_desc(w_base + kw * kKwBytes + PH * 16 * 128 + 32 * k));
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_acc(acc);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      v[i] = acc[K - 1 - PH][i];
+      acc[K - 1 - PH][i] = 0.f;
+    }
+  }
+}
+
+// Cin = 64 -> 16 float channels, K x K (K = 3, 7): the float-logits layers (the composed classifier, Standard's conv1_1_D).
+// An m64n16k16 MMA reads a 2 KB A tile for 16 output columns, which makes the 16-wide k_conv_tc tile bound by shared-memory
+// operand reads.  Here the K tap rows are stacked along N instead: ONE m64n{16K}k16 per (kw, K step) of input row i computes
+// the contributions of all K tap rows of tap column kw, tap row kh to output row i + pad - kh.  A operand reads drop K-fold
+// and the layer is bound by the tensor rate.
+//  * Output rows live in a ring of K accumulator slots of 8 fp32 per thread (64 pixels x 16 channels), counted downwards:
+//    relative output row y (from the run's first row) sits in slot (-y) mod K, so at phase ph = r mod K of relative input row
+//    r, slot j takes tap row (ph + j) mod K.  The slots keep fixed registers and the weights rotate instead: per tap column
+//    the rows kh = 0 .. K-1, 0 .. K-2 are resident, and phase ph's B operand is the K-row window starting at row ph.  The
+//    phase selects one of K copies of the issue code.  After input row r, output row r - (K - 1) (slot K-1-ph) is complete:
+//    it is stored and its slot zeroed for the row that enters next.  Per output pixel the adds run in the order of k_conv_tc
+//    -- tap row kh ascending, then kw, then the 4 K steps -- onto a zeroed accumulator, out-of-image rows included
+//    (zero-filled by TMA), so the results are the same bits.
+//  * The weights (182 KB for K = 7, 30 KB for K = 3) are loaded once per CTA: per kw one TMA box {64 cin, 16 cout, 1, K kh}
+//    out of the [kh][kw][cout][cin] tensor, which lands [kh][16][64]; the weight warp copies rows 0 .. K-2 behind it.  What
+//    is left of shared memory holds the halo ring (2 slots for K = 7, 11 for K = 3).
+//  * A CTA emits rows [b R, b R + R) of the flattened (image, strip, row) range; each maximal run of rows within one strip
+//    first walks K - 1 warm-up input rows, whose MMAs only feed rows that are not emitted.  Every input row is read by one
+//    step and then released, so the halo ring is pure prefetch.
+template <int K>
+__global__ void __launch_bounds__(kTcThreads, 1)
+k_conv_stack(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const __grid_constant__ TcParams p,
+             const __grid_constant__ TcConsts cst) {
+  constexpr int kPad = (K - 1) / 2;
+  constexpr int kSlots = stack_slots(K);
+  constexpr int kBlock = 16 * 128;                  // one tap row: [16 cout][64 cin] half
+  constexpr int kKwBytes = (2 * K - 1) * kBlock;    // one tap column
+  static_assert(stack_smem_bytes(K) <= 227 * 1024 && kSlots >= 2 && K <= 7, "weights + halo ring must fit in shared memory");
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
+  uint8_t* w_smem = smem;
+  uint8_t* a_slots = smem + stack_w_bytes(K);
+  uint64_t* a_full = reinterpret_cast<uint64_t*>(a_slots + kSlots * kSlotBytes);  // [kSlots]
+  uint64_t* a_empty = a_full + kSlots;                                             // [kSlots]
+  uint64_t* w_full = a_empty + kSlots;   // TMA landed tap rows 0 .. K-1 of every column
+  uint64_t* w_ready = w_full + 1;        // ... and the copies of rows 0 .. K-2 behind them
+
+  const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const long rows = static_cast<long>(p.N_batch) * p.strips * p.H;
+  const long t_begin = static_cast<long>(blockIdx.x) * p.rows_per_cta;
+  const long t_end = min(t_begin + p.rows_per_cta, rows);
+
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < kSlots; ++i) { mbar_init(a_full + i, 1); mbar_init(a_empty + i, kEmptyArrivals); }
+    mbar_init(w_full, 1);
+    mbar_init(w_ready, 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+  }
+  __syncthreads();
+
+  if (wg == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+    if (warp == 0 && lane == 0) {
+      // ===== halo-row producer: per run, input rows y_start - pad .. y_end - 1 + pad =====
+      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_a)) : "memory");
+      uint32_t u = 0;
+      for (long t = t_begin; t < t_end;) {
+        const int col = static_cast<int>(t / p.H), y_start = static_cast<int>(t % p.H);
+        const int n_out = static_cast<int>(min(static_cast<long>(p.H - y_start), t_end - t));
+        const int img = col / p.strips, x0 = (col % p.strips) * 128;
+        for (int r = 0; r < n_out + K - 1; ++r, ++u) {
+          const int slot = u % kSlots;
+          mbar_wait(a_empty + slot, ((u / kSlots) & 1) ^ 1);
+          mbar_expect_tx(a_full + slot, static_cast<uint32_t>((128 + K - 1) * 128));
+          tma_load_4d(a_slots + slot * kSlotBytes, &map_a, a_full + slot, 0, x0 - kPad, y_start - kPad + r, img);
+        }
+        t += n_out;
+      }
+    } else if (warp == 1) {
+      // ===== weights, once: TMA lands rows 0 .. K-1 of each tap column, the warp copies rows 0 .. K-2 behind them (whole
+      // 1 KB swizzle groups, so the SWIZZLE_128B phase is the same at the copy), and every window of K consecutive rows
+      // is the B operand of one phase =====
+      if (lane == 0) {
+        mbar_expect_tx(w_full, static_cast<uint32_t>(K * K * kBlock));
+        for (int kw = 0; kw < K; ++kw) tma_load_4d(w_smem + kw * kKwBytes, &map_b, w_full, 0, 0, kw, 0);
+      }
+      mbar_wait(w_full, 0);
+      for (int kw = 0; kw < K; ++kw) {
+        const uint4* src = reinterpret_cast<const uint4*>(w_smem + kw * kKwBytes);
+        uint4* dst = reinterpret_cast<uint4*>(w_smem + kw * kKwBytes + K * kBlock);
+        for (int i = lane; i < (K - 1) * kBlock / 16; i += 32) dst[i] = src[i];
+      }
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes, read by wgmma
+      __syncwarp();
+      if (lane == 0) mbar_arrive(w_ready);
+    }
+    return;
+  }
+
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+  // ===== consumers: warpgroup g = wg - 1 owns pixels [64 g, 64 g + 64) of the strip =====
+  const int g = wg - 1;
+  const int m0 = 16 * (warp & 3) + (lane >> 2);
+  const uint32_t a_base = smem_u32(a_slots) + static_cast<uint32_t>(g * 64 * 128), w_base = smem_u32(w_smem);
+  const bool releaser = lane == 0;
+  mbar_wait(w_ready, 0);
+  float acc[K][8];
+  uint32_t u = 0;
+  for (long t = t_begin; t < t_end;) {
+    const int col = static_cast<int>(t / p.H), y_start = static_cast<int>(t % p.H);
+    const int n_out = static_cast<int>(min(static_cast<long>(p.H - y_start), t_end - t));
+    const int img = col / p.strips, x_m0 = (col % p.strips) * 128 + 64 * g + m0;
+    const int n_in = n_out + K - 1;
+#pragma unroll
+    for (int s = 0; s < K; ++s)
+#pragma unroll
+      for (int i = 0; i < 8; ++i) acc[s][i] = 0.f;
+    for (int r = 0; r < n_in; ++r) {  // input row y_start - pad + r: its tap row kh feeds relative output row r - kh
+      const int slot = u % kSlots;
+      mbar_wait(a_full + slot, (u / kSlots) & 1);
+      const uint32_t a_row = a_base + slot * kSlotBytes;
+      float v[8];
+      switch (r % K) {
+        case 0: stack_row<K, 0>(acc, a_row, w_base, v); break;
+        case 1: stack_row<K, 1>(acc, a_row, w_base, v); break;
+        case 2: stack_row<K, 2>(acc, a_row, w_base, v); break;
+        case 3: stack_row<K, 3>(acc, a_row, w_base, v); break;
+        case 4: stack_row<K, 4>(acc, a_row, w_base, v); break;
+        case 5: stack_row<K, 5>(acc, a_row, w_base, v); break;
+        default: stack_row<K, 6>(acc, a_row, w_base, v); break;
+      }
+      if (releaser) mbar_arrive(a_empty + slot);
+      ++u;
+      // output row y_start + r - (K - 1) got its last tap row (rows before y_start are warm-up, not emitted)
+      if (r >= K - 1) epilogue_row16(p, cst, v, img, y_start + r - (K - 1), x_m0, lane & 3);
+    }
+    t += n_out;
+  }
+}
+
 // ---- host: tensor maps through the driver entry point (no -lcuda at link time)
 using EncodeFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                               const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -581,6 +783,8 @@ struct ConvTcPlan {
   int kw;             // filter width the kernel walks (== k, or 1 for a window-folded layer)
   bool roll;
   bool pk2 = false;   // two images per 128-pixel M tile (layers at most 64 pixels wide, chunked 3x3 kernel)
+  bool stack = false; // k_conv_stack: 64 -> 16 float logits, K = 3 / 7
+  double rows_ratio = 1.0;  // k_conv_stack: input rows it runs the MMAs of / output rows (the warm-up rows of every run)
   DevBuf w_own;       // weights the plan owns (the composed classifier)
 };
 
@@ -605,9 +809,11 @@ void conv_tc_dispatch(const ConvTcPlan& plan, cudaStream_t s, bool configure) {
     if (K == 7) go(k_conv_tc<7, true, 1, false, 64, false>); else go(k_conv_tc<3, true, 1, false, 64, false>);
   } else if (plan.pk2) {
     if (plan.p.n_tile == 64) go(k_conv_tc<3, false, 3, true, 64, false>); else go(k_conv_tc<3, false, 3, true, 128, false>);
+  } else if (plan.stack) {  // 64 -> 16 float logits, K = 3 / 7
+    if (K == 7) go(k_conv_stack<7>); else go(k_conv_stack<3>);
   } else if (plan.roll) {
-    if (K == 7) by_n(k_conv_tc<7, true, 7, false, 16, false>, k_conv_tc<7, true, 7, false, 64, false>, k_conv_tc<7, true, 7, false, 128, false>);
-    else if (K == 3) by_n(k_conv_tc<3, true, 3, false, 16, false>, k_conv_tc<3, true, 3, false, 64, false>, k_conv_tc<3, true, 3, false, 128, false>);
+    if (K == 7) { if (plan.p.n_tile == 64) go(k_conv_tc<7, true, 7, false, 64, false>); else go(k_conv_tc<7, true, 7, false, 128, false>); }
+    else if (K == 3) { if (plan.p.n_tile == 64) go(k_conv_tc<3, true, 3, false, 64, false>); else go(k_conv_tc<3, true, 3, false, 128, false>); }
     else by_n(k_conv_tc<1, true, 1, false, 16, false>, k_conv_tc<1, true, 1, false, 64, false>, k_conv_tc<1, true, 1, false, 128, false>);
   } else {
     if (K == 7) by_n(k_conv_tc<7, false, 7, false, 16, false>, k_conv_tc<7, false, 7, false, 64, false>, k_conv_tc<7, false, 7, false, 128, false>);
@@ -655,6 +861,35 @@ int tc_blocks_per_cta(long columns, int total_pairs, double overhead) {
     if (cost < best_cost - 1e-9) { best_cost = cost; ppc = c; }
   }
   return ppc;
+}
+// Output rows per k_conv_stack CTA at most: bounds how long the extractors' dependent kernels wait for an SM (see kTcMaxPpc).
+// Basic T=6 at 352 x 1024 (6 x 8 x 352 = 16 896 rows) is then one wave of 128-row CTAs on 132 SMs.
+constexpr int kStackMaxRows = 128;
+// Points a K = 3 / 7, 64 -> 16 float-logits plan at k_conv_stack.  `w` = [kh][kw][cout_rows][64] half, couts 0..15 used.
+void plan_stack(ConvTcPlan& plan, void* w, int cout_rows) {
+  const int K = plan.k;
+  cuuint64_t dims[4] = {64, static_cast<cuuint64_t>(cout_rows), static_cast<cuuint64_t>(K), static_cast<cuuint64_t>(K)};
+  cuuint64_t strides[3] = {128, static_cast<cuuint64_t>(cout_rows) * 128, static_cast<cuuint64_t>(K) * cout_rows * 128};
+  cuuint32_t box[4] = {64, 16, 1, static_cast<cuuint32_t>(K)};  // one tap column: [kh][16][64]
+  encode(&plan.map_b, w, 4, dims, strides, box);
+  TcParams& p = plan.p;
+  p.n_tile = 16;
+  p.out_f32 = 1;
+  // equal pieces of the flattened (image, strip, row) range, in as few waves over the SMs as kStackMaxRows allows
+  const long rows = static_cast<long>(p.N_batch) * p.strips * p.H;
+  const long sms = num_sms();
+  const long waves = (rows + sms * kStackMaxRows - 1) / (sms * kStackMaxRows);
+  p.rows_per_cta = static_cast<int>((rows + waves * sms - 1) / (waves * sms));
+  const long ctas = (rows + p.rows_per_cta - 1) / p.rows_per_cta;
+  long runs = 0;  // maximal runs of rows within one strip: each costs K - 1 warm-up input rows
+  for (long b = 0; b < ctas; ++b) {
+    const long t0 = b * p.rows_per_cta, t1 = std::min(t0 + p.rows_per_cta, rows);
+    runs += (t1 - 1) / p.H - t0 / p.H + 1;
+  }
+  plan.rows_ratio = static_cast<double>(rows + (K - 1) * runs) / static_cast<double>(rows);
+  plan.grid = dim3(static_cast<unsigned>(ctas), 1, 1);
+  plan.smem = stack_smem_bytes(K);
+  plan.stack = true;
 }
 }  // namespace
 
@@ -752,6 +987,7 @@ std::shared_ptr<ConvTcPlan> conv_tc_plan(const Op& op, const TensorView& in, con
   plan->k = K;
   plan->kw = KW;
   plan->roll = roll;
+  if (roll && n_tile == 16 && K > 1) plan_stack(*plan, const_cast<void*>(w_tc), op.cout_p);
   conv_tc_dispatch(*plan, nullptr, true);
   return plan;
 }
@@ -828,7 +1064,7 @@ void conv_tc_set_composed_classifier(ConvTcPlan& plan, const Op& conv, const flo
   if (n_cls > 16 || conv.h_w_raw.size() != static_cast<size_t>(64) * 64 * K * K || conv.h_bias.size() < 64)
     fail(SIVO_EINVAL, "composed classifier: unexpected layer shapes");
   // W'[o][i][kh][kw] = sum_c wc[o][c] W[c][i][kh][kw] in double, rounded once to half; rows o >= n_cls stay zero.
-  // Device layout [kh][kw][16][64]: the [tap][cout][cin] layout of every other weight tensor, 16-row tiles.
+  // Device layout [kh][kw][16][64]: the [tap][cout][cin] layout of every other weight tensor, 16 couts per tap.
   std::vector<__half> w(static_cast<size_t>(K) * K * 16 * 64, __float2half_rn(0.f));
   const float* W = conv.h_w_raw.data();
   for (int o = 0; o < n_cls; ++o)
@@ -841,26 +1077,19 @@ void conv_tc_set_composed_classifier(ConvTcPlan& plan, const Op& conv, const flo
         }
   plan.w_own.alloc(w.size() * sizeof(__half));
   SIVO_CUDA(cudaMemcpy(plan.w_own.p, w.data(), w.size() * sizeof(__half), cudaMemcpyHostToDevice));
-  cuuint64_t dims[3] = {64, 16, static_cast<cuuint64_t>(K) * K};
-  cuuint64_t strides[2] = {128, 16 * 128};
-  cuuint32_t box[3] = {64, 16, 1};
-  encode(&plan.map_b, plan.w_own.p, 3, dims, strides, box);
   std::memset(&plan.cst, 0, sizeof(TcConsts));
   for (int o = 0; o < n_cls; ++o) {
     double acc = bc[o];
     for (int c = 0; c < 64; ++c) acc += static_cast<double>(wc[o * 64 + c]) * conv.h_bias[c];
     plan.cst.bias[o] = static_cast<float>(acc);
   }
-  TcParams& p = plan.p;
-  p.out_f32 = 1;
-  p.n_tile = 16;
-  p.cout_total = 16;
-  p.out = logits;
-  p.b_stages = tc_stages(K, true, 16);
-  plan.smem = tc_smem_bytes(K, true, 16, p.b_stages);
-  plan.grid.y = 1;
+  plan.p.cout_total = 16;
+  plan.p.out = logits;
+  plan_stack(plan, plan.w_own.p, 16);
   conv_tc_dispatch(plan, nullptr, true);
 }
+
+double conv_tc_rows_ratio(const ConvTcPlan& plan) { return plan.rows_ratio; }
 
 void conv_tc_launch(const ConvTcPlan& plan, const Op& op, cudaStream_t s) {
   (void)op;

@@ -229,7 +229,8 @@ void SegNet::build(const NetSpec& net, const WeightMap& weights) {
           if (!(compose && compose[0] == '0') && !conv.relu && !conv.has_bn && conv_tc_can_compose_classifier(*conv.tc)) {
             conv_tc_set_composed_classifier(*conv.tc, conv, op.h_w_raw.data(), op.h_bias.data(), op.cout,
                                             static_cast<float*>(tensors_[op.out]->v.p));
-            conv.flops_exec = 2.0 * conv.cin * conv.k * conv.k * 16 * iv.h * iv.w * iv.n;  // the 16-wide composed layer
+            // the 16-wide composed layer, warm-up rows included
+            conv.flops_exec = 2.0 * conv.cin * conv.k * conv.k * 16 * iv.h * iv.w * iv.n * conv_tc_rows_ratio(*conv.tc);
             conv.layer += "*" + ly.name;  // '*': composed, not merely fused
           } else {
             conv_tc_set_classifier(*conv.tc, op.h_w.data(), op.cout_p, op.h_bias.data(), std::min(16, op.cout_p),
@@ -251,6 +252,7 @@ void SegNet::build(const NetSpec& net, const WeightMap& weights) {
         } else if (opt_.engine != SIVO_ENGINE_SIMT && act_ == DType::F16 &&
             conv_tc_supported(op, civ, tensors_[op.out]->v)) {
           op.tc = conv_tc_plan(op, civ, tensors_[op.out]->v, op.w_tc.p);
+          op.flops_exec *= conv_tc_rows_ratio(*op.tc);
           op.use_tc = true;
         } else if (op.fold_kw) {
           fail(SIVO_EINVAL, "layer '%s': window-folded first layer is not supported by the tensor-core kernel", ly.name.c_str());

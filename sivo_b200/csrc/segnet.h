@@ -161,6 +161,8 @@ class SegNet {
 bool conv_tc_supported(const Op& op, const TensorView& in, const TensorView& out);
 std::shared_ptr<ConvTcPlan> conv_tc_plan(const Op& op, const TensorView& in, const TensorView& out, const void* w_tc);
 void conv_tc_launch(const ConvTcPlan& plan, const Op& op, cudaStream_t s);
+// input rows whose MMAs the plan's kernel runs per output row: > 1 for the tap-row-stacked float-logits kernel (warm-up rows)
+double conv_tc_rows_ratio(const ConvTcPlan& plan);
 // fuses the sampling Dropout that follows the convolution in place into its epilogue
 // (sample0: global MC sample index of the batch's image 0, so that a shard handle draws the masks of its own samples)
 void conv_tc_set_dropout(ConvTcPlan& plan, uint64_t seed, const uint64_t* frame_dev, int layer, float scale, int sample0);
