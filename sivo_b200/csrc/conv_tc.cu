@@ -20,7 +20,10 @@
 //    warpgroups 1 and 2 consume (setmaxnreg 232): consumer g owns pixels [64 g, 64 g + 64) of the tile, issues the
 //    m64nNk16 wgmma of both rows of the block into register accumulators, and runs the epilogue on them -- bias / BN
 //    affine / ReLU -> half, then store | dropout | max-unpool scatter | 2x2 max-pool + argmax | 1x1 classifier -> float
-//    logits -- while the other consumer's MMAs keep the tensor core busy.
+//    logits.  Both consumers read every weight stage, so they reach a block's epilogue together and no MMA is issued
+//    while it runs.  The 64-wide store / dropout / unpool epilogues are therefore deferred: a block's outputs are
+//    converted and staged in registers (16 B per lane after a quad transpose), and their stores are issued one slice per
+//    tap row between the next block's MMA commits, so they drain under the tensor core's work.
 //  * Constants (bias, BN, classifier weights) are kernel parameters: the epilogue reads them from the constant bank and
 //    leaves the shared-memory data path to the MMA operand reads.
 //  * The 64 -> 16 float-logits layers (K = 3, 7) run on k_conv_stack instead: tap rows stacked along N, resident weights.
@@ -32,6 +35,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <mutex>
+#include <type_traits>
 #include <vector>
 
 #include "philox.cuh"
@@ -361,6 +365,100 @@ __device__ __forceinline__ void epilogue_block(const TcParams& p, const TcConsts
   }
 }
 
+// Deferred epilogue (store / dropout / max-unpool, N = 64): the half outputs of one row block, staged in registers so that
+// their stores can be issued while the next row block's MMAs run.  Chunk i = (2 r + h) * N/32 + J holds channels
+// 8 (4 J + q) .. + 7 of pixel (y0 + r, x_m0 + 8 h): 16 bytes per lane, 64 contiguous bytes per quad.
+template <int N>
+struct EpiStage {
+  static constexpr int kChunks = kRows * 2 * (N / 32);
+  uint4 v[kChunks];
+  uint2 m[kChunks];  // unpool: the chunk's 8 mask bytes
+  int y0, img;
+};
+
+// 4 x 4 word transpose within a quad: lane q holds w[k] = channels 8 k + 2 q, +1 of a 32-channel group and gets back
+// channels 8 q .. 8 q + 7 (lane q' sends w[q' ^ x] across xor distance x, which is the word lane q' ^ x keeps).
+__device__ __forceinline__ uint4 quad_transpose(const uint32_t (&w)[4], int q) {
+  auto pick = [](const uint32_t (&a)[4], int i) { return i == 0 ? a[0] : i == 1 ? a[1] : i == 2 ? a[2] : a[3]; };
+  uint32_t r[4];  // r[x] = word q of column q ^ x
+  r[0] = pick(w, q);
+#pragma unroll
+  for (int x = 1; x < 4; ++x) r[x] = __shfl_xor_sync(0xffffffffu, pick(w, q ^ x), x);
+  return make_uint4(pick(r, q), pick(r, q ^ 1), pick(r, q ^ 2), pick(r, q ^ 3));
+}
+
+// Converts one row block's accumulators into its staged outputs with the arithmetic of epilogue_block (bias / BN /
+// ReLU -> half, dropout keep bits x scale) and issues the unpool mask loads.  Called by all 32 lanes (warp shuffles).
+template <int N>
+__device__ __forceinline__ void epilogue_stage(const TcParams& p, const TcConsts& cst, const float (&acc)[kRows][N / 2], int img,
+                                               int y0, int x_m0, int n0, int q, EpiStage<N>& e) {
+  e.y0 = y0;
+  e.img = img;
+  const bool img_ok = img < p.N_batch;
+#pragma unroll
+  for (int r = 0; r < kRows; ++r) {
+    const int y = y0 + r;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int x = x_m0 + 8 * h;
+      const bool inside = y < p.H && img_ok && x < p.W;
+      uint32_t bits[4] = {0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu};
+      if (p.has_drop && inside)
+        dropout_bits128_nl(p.seed, *p.frame, p.drop_nl + img, static_cast<uint32_t>(y * p.W + x), n0 >> 7, bits);
+      uint32_t w[N / 8];
+#pragma unroll
+      for (int j = 0; j < N / 8; ++j) {
+        const int c = n0 + 8 * j + 2 * q;
+        __half2 hv = __floats2half2_rn(affine(p, cst, acc[r][4 * j + 2 * h], c), affine(p, cst, acc[r][4 * j + 2 * h + 1], c + 1));
+        if (p.has_drop) {
+          const int wsel = (c >> 5) & 3;
+          const uint32_t keep = wsel == 0 ? bits[0] : wsel == 1 ? bits[1] : wsel == 2 ? bits[2] : bits[3];
+          const int bit = c & 31;
+          hv = __hmul2(hv, __floats2half2_rn((keep >> bit) & 1u ? p.drop_scale : 0.f, (keep >> (bit + 1)) & 1u ? p.drop_scale : 0.f));
+        }
+        w[j] = *reinterpret_cast<const uint32_t*>(&hv);
+      }
+      const size_t mask_pix = (static_cast<size_t>(img % p.mask_n) * p.H + y) * p.W + x;
+#pragma unroll
+      for (int J = 0; J < N / 32; ++J) {
+        const int i = (2 * r + h) * (N / 32) + J;
+        const uint32_t wj[4] = {w[4 * J], w[4 * J + 1], w[4 * J + 2], w[4 * J + 3]};
+        e.v[i] = quad_transpose(wj, q);
+        e.m[i] = make_uint2(0u, 0u);
+        if (p.unpool_mask && inside)
+          e.m[i] = __ldg(reinterpret_cast<const uint2*>(p.unpool_mask + mask_pix * p.cout_total + n0 + 8 * (4 * J + q)));
+      }
+    }
+  }
+}
+
+// Issues the stores of staged chunk i (a compile-time index after unrolling): one 16-byte store, or four for unpool,
+// where each channel's value goes to the 2x2 position its mask byte names and zeros to the other three.
+template <int N>
+__device__ __forceinline__ void epilogue_flush(const TcParams& p, const EpiStage<N>& e, int i, int x_m0, int n0, int q) {
+  const int r = i / (2 * (N / 32)), h = (i / (N / 32)) & 1, J = i % (N / 32);
+  // opaque copies: the addresses are computed here, not at staging time and kept live (in spilled registers) across the MMAs
+  int y0 = e.y0, img = e.img;
+  asm volatile("" : "+r"(y0), "+r"(img));
+  const int y = y0 + r, x = x_m0 + 8 * h;
+  if (!(y < p.H && img < p.N_batch && x < p.W)) return;
+  const int c = n0 + 8 * (4 * J + q);
+  const uint4 v = e.v[i];
+  if (p.unpool_mask) {
+    __half* const ob = static_cast<__half*>(p.out) + ((static_cast<size_t>(img) * 2 * p.H + 2 * y) * (2 * p.W) + 2 * x) * p.cout_total + c;
+    const size_t row_step = static_cast<size_t>(2 * p.W) * p.cout_total;
+#pragma unroll
+    for (int pos = 0; pos < 4; ++pos) {
+      const uint32_t lo = __vcmpeq4(e.m[i].x, 0x01010101u * pos), hi = __vcmpeq4(e.m[i].y, 0x01010101u * pos);  // 0xFF per matching byte
+      const uint4 o = make_uint4(v.x & __byte_perm(lo, 0u, 0x1100), v.y & __byte_perm(lo, 0u, 0x3322),
+                                 v.z & __byte_perm(hi, 0u, 0x1100), v.w & __byte_perm(hi, 0u, 0x3322));
+      *reinterpret_cast<uint4*>(ob + (pos >> 1) * row_step + (pos & 1) * p.cout_total) = o;
+    }
+  } else {
+    *reinterpret_cast<uint4*>(static_cast<__half*>(p.out) + ((static_cast<size_t>(img) * p.H + y) * p.W + x) * p.cout_total + c) = v;
+  }
+}
+
 // ROLL = true : one 64-channel chunk (Cin == 64); halo rows persist in the ring while the CTA walks down its
 //               strip, so each input row is fetched once per CTA.
 // ROLL = false: Cin = 64 * NC; per (row block, chunk) the kRows+K-1 halo rows of that chunk are fetched, used by
@@ -480,92 +578,128 @@ k_conv_tc(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUt
   // PK2: the second image's 64-pixel box sits 64 rows into the slot; otherwise pixel 64 g of the halo row is 64 g rows in
   const uint32_t a_base = smem_u32(a_slots) + static_cast<uint32_t>(g * 64 * 128), b_base = smem_u32(b_stages);
   const bool releaser = lane == 0;
-  float acc[kRows][F];
-  float accr[SPLIT ? kRows : 1][SPLIT ? F : 1];
-  int st = 0;
-  uint32_t b_phase = 0;
-  int waited = 0;  // halo units whose TMA has been observed
-  const int S = p.split ? p.seg_rows : K;
-  for (int j = 0; j < npairs; ++j) {
-#pragma unroll
-    for (int r = 0; r < kRows; ++r)
-#pragma unroll
-      for (int i = 0; i < F; ++i) {
-        acc[r][i] = 0.f;
-        if (SPLIT) accr[r][i] = 0.f;
-      }
-    for (int ch = 0; ch < NC; ++ch)
-    for (int kwo = 0; kwo < (PK2 ? KW : 1); ++kwo) {  // PK2: the kw shift is done by TMA, one set of halo rows per tap column
-      const int base_u = ROLL ? j * kRows : PK2 ? ((j * NC + ch) * KW + kwo) * RK : (j * NC + ch) * RK;
-      for (int kh = 0; kh < K; ++kh) {
-        while (waited <= base_u + kh + kRows - 1 && waited < n_units) {
-          mbar_wait(a_full + waited % kSlots, (waited / kSlots) & 1);
-          ++waited;
-        }
-        uint32_t a_row[kRows];
-#pragma unroll
-        for (int r = 0; r < kRows; ++r) a_row[r] = a_base + ((base_u + r + kh) % kSlots) * kSlotBytes;
-        const int nrep = p.split && !(ch & 1) ? 2 : 1;
-        int prev_st = -1;
-#pragma unroll
-        for (int kw = 0; kw < (PK2 ? 1 : KW); ++kw)
-        for (int rep = 0; rep < nrep; ++rep) {
-          mbar_wait(b_full + st, b_phase);
-          const uint32_t b_addr = b_base + st * b_stride;
-          const uint32_t a_shift = PK2 ? 0u : static_cast<uint32_t>(kw * 128);
-          wgmma_fence();
-          // K step outer, row inner: consecutive MMAs go to different accumulators
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-#pragma unroll
-            for (int r = 0; r < kRows; ++r) wgmma(acc[r], make_desc(a_row[r] + a_shift + 32 * k), make_desc(b_addr + 32 * k));
-          wgmma_commit();
-          // keep one group in flight: the previous one has retired, so its weight stage goes back to the producer
-          wgmma_wait<1>();
-          if (prev_st >= 0 && releaser) mbar_arrive(b_empty + prev_st);
-          prev_st = st;
-          if (++st == kBStages) { st = 0; b_phase ^= 1; }
-        }
-        wgmma_wait<0>();
-        fence_acc(acc);
-        if (releaser) {
-          mbar_arrive(b_empty + prev_st);
-          // halo row base_u + kh is only read by tap rows <= kh of this block.  ROLL: rows >= kRows are also the next block's, so
-          // only kh < kRows goes back to the producer now; !ROLL: every chunk fetches its own rows, so row kh is dead after tap row kh
-          if (!ROLL || kh < kRows) mbar_arrive(a_empty + (base_u + kh) % kSlots);
-        }
-        if (SPLIT && (kh % S == S - 1 || kh == K - 1)) {
-          // segment done: accumulate steps (tap rows) x KW x 4 K steps x (2 weight tiles for a hi chunk, 1 for a lo chunk).
-          // The tensor core truncates each add towards zero: mean loss 0.36 x 2^-23 of the running sum per step (half an ulp,
-          // ulp / |x| averaging 0.72 x 2^-23 over a binade), and a sum growing from 0 averages ~0.6 of its final value, so the
-          // segment comes back short by ~0.216 x 2^-23 x m of itself: scaled back up here (leaves the zero-mean part).
-          const int kh0 = (kh / S) * S;
-          const int m_steps = min(S, K - kh0) * KW * 4 * ((ch & 1) ? 1 : 2);
-          const float comp = 1.f + p.rz_comp * static_cast<float>(m_steps);
-#pragma unroll
-          for (int r = 0; r < kRows; ++r)
-#pragma unroll
-            for (int i = 0; i < F; ++i) {
-              accr[r][i] = __fmaf_rn(acc[r][i], comp, accr[r][i]);
-              acc[r][i] = 0.f;
-            }
-        }
-      }
-      if (releaser) {
-        if (ROLL && K < kRows)  // fewer tap rows than output rows: release the rest of this block's own rows
-          for (int i = K; i < kRows; ++i) mbar_arrive(a_empty + (base_u + i) % kSlots);
-        if (!ROLL)  // the chunk's remaining halo rows (last read by tap row K - 1) are dead
-          for (int i = K; i < RK; ++i) mbar_arrive(a_empty + (base_u + i) % kSlots);
-      }
-    }
-    const int y0 = y_base + j * kRows;
-    if (SPLIT) {
+  const int q = lane & 3;
+  // N = 64 store / dropout / unpool epilogues are deferred: block j's outputs are staged in registers, and their stores go
+  // out one slice per tap row of block j + 1, right after that tap row's first MMA group is committed, so they drain while
+  // the tensor core works (the last block's are flushed at the end).  The walk is instantiated once per epilogue kind so
+  // that the staged registers are not live next to the immediate epilogues (pool, classifier), which would then spill.
+  constexpr bool kDefer = N == 64 && !SPLIT;
+  auto walk = [&](auto defer_tag) {
+    constexpr bool D = decltype(defer_tag)::value;
+    float acc[kRows][F];
+    float accr[SPLIT ? kRows : 1][SPLIT ? F : 1];
+    EpiStage<D ? N : 32> ep;
+    bool pending = false;
+    int st = 0;
+    uint32_t b_phase = 0;
+    int waited = 0;  // halo units whose TMA has been observed
+    const int S = p.split ? p.seg_rows : K;
+    for (int j = 0; j < npairs; ++j) {
 #pragma unroll
       for (int r = 0; r < kRows; ++r)
 #pragma unroll
-        for (int i = 0; i < F; ++i) acc[r][i] = __fmul_rn(accr[r][i], p.acc_scale);  // x 2^-s (exact)
+        for (int i = 0; i < F; ++i) {
+          acc[r][i] = 0.f;
+          if (SPLIT) accr[r][i] = 0.f;
+        }
+      for (int ch = 0; ch < NC; ++ch)
+      for (int kwo = 0; kwo < (PK2 ? KW : 1); ++kwo) {  // PK2: the kw shift is done by TMA, one set of halo rows per tap column
+        const int base_u = ROLL ? j * kRows : PK2 ? ((j * NC + ch) * KW + kwo) * RK : (j * NC + ch) * RK;
+        for (int kh = 0; kh < K; ++kh) {
+          while (waited <= base_u + kh + kRows - 1 && waited < n_units) {
+            mbar_wait(a_full + waited % kSlots, (waited / kSlots) & 1);
+            ++waited;
+          }
+          uint32_t a_row[kRows];
+#pragma unroll
+          for (int r = 0; r < kRows; ++r) a_row[r] = a_base + ((base_u + r + kh) % kSlots) * kSlotBytes;
+          const int nrep = p.split && !(ch & 1) ? 2 : 1;
+          int prev_st = -1;
+#pragma unroll
+          for (int kw = 0; kw < (PK2 ? 1 : KW); ++kw)
+          for (int rep = 0; rep < nrep; ++rep) {
+            mbar_wait(b_full + st, b_phase);
+            const uint32_t b_addr = b_base + st * b_stride;
+            const uint32_t a_shift = PK2 ? 0u : static_cast<uint32_t>(kw * 128);
+            wgmma_fence();
+            // K step outer, row inner: consecutive MMAs go to different accumulators
+#pragma unroll
+            for (int k = 0; k < 4; ++k)
+#pragma unroll
+              for (int r = 0; r < kRows; ++r) wgmma(acc[r], make_desc(a_row[r] + a_shift + 32 * k), make_desc(b_addr + 32 * k));
+            wgmma_commit();
+            if constexpr (D) {
+              if (kw == 0 && rep == 0 && ch == 0 && kwo == 0 && pending) {
+                // the previous block's chunks i with i K / 8 == kh: every chunk goes out during the first chunk's K tap rows
+#pragma unroll
+                for (int i = 0; i < EpiStage<N>::kChunks; ++i)
+                  if ((i * K) / EpiStage<N>::kChunks == kh) epilogue_flush<N>(p, ep, i, x_m0, n0, q);
+              }
+            }
+            // keep one group in flight: the previous one has retired, so its weight stage goes back to the producer
+            wgmma_wait<1>();
+            if (prev_st >= 0 && releaser) mbar_arrive(b_empty + prev_st);
+            prev_st = st;
+            if (++st == kBStages) { st = 0; b_phase ^= 1; }
+          }
+          wgmma_wait<0>();
+          fence_acc(acc);
+          if (releaser) {
+            mbar_arrive(b_empty + prev_st);
+            // halo row base_u + kh is only read by tap rows <= kh of this block.  ROLL: rows >= kRows are also the next block's, so
+            // only kh < kRows goes back to the producer now; !ROLL: every chunk fetches its own rows, so row kh is dead after tap row kh
+            if (!ROLL || kh < kRows) mbar_arrive(a_empty + (base_u + kh) % kSlots);
+          }
+          if (SPLIT && (kh % S == S - 1 || kh == K - 1)) {
+            // segment done: accumulate steps (tap rows) x KW x 4 K steps x (2 weight tiles for a hi chunk, 1 for a lo chunk).
+            // The tensor core truncates each add towards zero: mean loss 0.36 x 2^-23 of the running sum per step (half an ulp,
+            // ulp / |x| averaging 0.72 x 2^-23 over a binade), and a sum growing from 0 averages ~0.6 of its final value, so the
+            // segment comes back short by ~0.216 x 2^-23 x m of itself: scaled back up here (leaves the zero-mean part).
+            const int kh0 = (kh / S) * S;
+            const int m_steps = min(S, K - kh0) * KW * 4 * ((ch & 1) ? 1 : 2);
+            const float comp = 1.f + p.rz_comp * static_cast<float>(m_steps);
+#pragma unroll
+            for (int r = 0; r < kRows; ++r)
+#pragma unroll
+              for (int i = 0; i < F; ++i) {
+                accr[r][i] = __fmaf_rn(acc[r][i], comp, accr[r][i]);
+                acc[r][i] = 0.f;
+              }
+          }
+        }
+        if (releaser) {
+          if (ROLL && K < kRows)  // fewer tap rows than output rows: release the rest of this block's own rows
+            for (int i = K; i < kRows; ++i) mbar_arrive(a_empty + (base_u + i) % kSlots);
+          if (!ROLL)  // the chunk's remaining halo rows (last read by tap row K - 1) are dead
+            for (int i = K; i < RK; ++i) mbar_arrive(a_empty + (base_u + i) % kSlots);
+        }
+      }
+      const int y0 = y_base + j * kRows;
+      if (SPLIT) {
+#pragma unroll
+        for (int r = 0; r < kRows; ++r)
+#pragma unroll
+          for (int i = 0; i < F; ++i) acc[r][i] = __fmul_rn(accr[r][i], p.acc_scale);  // x 2^-s (exact)
+      }
+      if constexpr (D) {
+        epilogue_stage<N>(p, cst, acc, img_c, y0, x_m0, n0, q, ep);
+        pending = true;
+      } else {
+        epilogue_block<N>(p, cst, acc, img_c, y0, x_m0, n0, lane);
+      }
     }
-    epilogue_block<N>(p, cst, acc, img_c, y0, x_m0, n0, lane);
+    if constexpr (D) {
+      if (pending) {
+#pragma unroll
+        for (int i = 0; i < EpiStage<N>::kChunks; ++i) epilogue_flush<N>(p, ep, i, x_m0, n0, q);
+      }
+    }
+  };
+  if constexpr (kDefer) {
+    if (!p.pool_out && !p.has_cls && !p.out_f32) walk(std::true_type{});
+    else walk(std::false_type{});
+  } else {
+    walk(std::false_type{});
   }
 }
 
