@@ -329,6 +329,11 @@ int sivo_dbg_unpool(int device, const float* in, const int* mask, int n, int c, 
 int sivo_dbg_conv(int device, int engine, int precision, const float* in, int n, int cin, int h, int w,
                   const float* weight, const float* bias, const float* bn_scale, const float* bn_shift,
                   int cout, int k, int pad, int relu, float* out);
+/* The 7x7 float-logits convolution over the max-unpool of `pooled` (float NCHW [n][64][h][w]) by `mask` (sivo_dbg_unpool's
+ * convention, [mask_n][64][h][w], image i takes mask i % mask_n), unpooled as the kernel loads its input rows: out = float
+ * NCHW [n][cout][2h][2w], cout <= 16, k = 7, no ReLU.  Equals sivo_dbg_unpool followed by sivo_dbg_conv bit for bit. */
+int sivo_dbg_conv_unpooled(int device, const float* pooled, const int* mask, int n, int mask_n, int h, int w, const float* weight,
+                           const float* bias, const float* bn_scale, const float* bn_shift, int cout, int k, float* out);
 int sivo_dbg_lrn(int device, const float* in, int n, int c, int h, int w, int size, float alpha, float beta,
                  float k, float* out);
 int sivo_dbg_mc_reduce(int device, const float* logits, int T, int c, int h, int w, uint8_t* classes,

@@ -532,6 +532,42 @@ void download_nchw(TensorView v, float* dst) {
   launch_act_to_nchw(v, tmp.as<float>(), nullptr);
   SIVO_CUDA(cudaMemcpy(dst, tmp.p, count * sizeof(float), cudaMemcpyDeviceToHost));
 }
+// the convolution op of the conv test hooks, weights through the same preparation the executor uses
+Op dbg_conv_op(DType dt, int cin, int cs_in, const float* weight, const float* bias, const float* bn_scale, const float* bn_shift,
+               int cout, int k, int pad, int relu) {
+  Op op;
+  op.kind = Op::Conv;
+  op.layer = "dbg_conv";
+  op.k = k; op.pad = pad; op.cin = cin; op.cout = cout; op.cin_p = cs_in; op.cout_p = (cout + 63) / 64 * 64;
+  op.relu = relu != 0;
+  auto th = [&](float x) { return dt == DType::F16 ? __half2float(__float2half_rn(x)) : x; };
+  std::vector<float> ws(static_cast<size_t>(k) * k * op.cin_p * op.cout_p, 0.f);
+  std::vector<__half> wt(static_cast<size_t>(k) * k * op.cout_p * op.cin_p, __float2half_rn(0.f));
+  for (int co = 0; co < cout; ++co)
+    for (int ci = 0; ci < cin; ++ci)
+      for (int t = 0; t < k * k; ++t) {
+        float v = weight[(static_cast<size_t>(co) * cin + ci) * k * k + t];
+        ws[(static_cast<size_t>(t) * op.cin_p + ci) * op.cout_p + co] = th(v);
+        wt[(static_cast<size_t>(t) * op.cout_p + co) * op.cin_p + ci] = __float2half_rn(v);
+      }
+  std::vector<float> b(op.cout_p, 0.f), sc(op.cout_p, 1.f), sh(op.cout_p, 0.f);
+  if (bias) std::copy(bias, bias + cout, b.begin());
+  if (bn_scale) std::copy(bn_scale, bn_scale + cout, sc.begin());
+  if (bn_shift) std::copy(bn_shift, bn_shift + cout, sh.begin());
+  op.h_bias = b; op.h_bn_scale = sc; op.h_bn_shift = sh;
+  op.w_simt.alloc(ws.size() * 4);
+  op.w_tc.alloc(wt.size() * 2);
+  op.bias.alloc(b.size() * 4);
+  op.bn_scale.alloc(sc.size() * 4);
+  op.bn_shift.alloc(sh.size() * 4);
+  SIVO_CUDA(cudaMemcpy(op.w_simt.p, ws.data(), ws.size() * 4, cudaMemcpyHostToDevice));
+  SIVO_CUDA(cudaMemcpy(op.w_tc.p, wt.data(), wt.size() * 2, cudaMemcpyHostToDevice));
+  SIVO_CUDA(cudaMemcpy(op.bias.p, b.data(), b.size() * 4, cudaMemcpyHostToDevice));
+  SIVO_CUDA(cudaMemcpy(op.bn_scale.p, sc.data(), sc.size() * 4, cudaMemcpyHostToDevice));
+  SIVO_CUDA(cudaMemcpy(op.bn_shift.p, sh.data(), sh.size() * 4, cudaMemcpyHostToDevice));
+  op.has_bn = bn_scale != nullptr;
+  return op;
+}
 }  // namespace
 
 int sivo_dbg_pool(int device, const float* in, int n, int c, int h, int w, float* out, int* mask) {
@@ -642,38 +678,7 @@ int sivo_dbg_conv(int device, int engine, int precision, const float* in, int n,
     DType odt = (cout % 8) ? DType::F32 : dt;
     TensorView vo = make_view(bo, n, cout, h, w, cs_out, odt);
     upload_nchw(in, vi);
-    Op op;
-    op.kind = Op::Conv;
-    op.layer = "dbg_conv";
-    op.k = k; op.pad = pad; op.cin = cin; op.cout = cout; op.cin_p = cs_in; op.cout_p = (cout + 63) / 64 * 64;
-    op.relu = relu != 0;
-    // weights through the same preparation the executor uses
-    auto th = [&](float x) { return dt == DType::F16 ? __half2float(__float2half_rn(x)) : x; };
-    std::vector<float> ws(static_cast<size_t>(k) * k * op.cin_p * op.cout_p, 0.f);
-    std::vector<__half> wt(static_cast<size_t>(k) * k * op.cout_p * op.cin_p, __float2half_rn(0.f));
-    for (int co = 0; co < cout; ++co)
-      for (int ci = 0; ci < cin; ++ci)
-        for (int t = 0; t < k * k; ++t) {
-          float v = weight[(static_cast<size_t>(co) * cin + ci) * k * k + t];
-          ws[(static_cast<size_t>(t) * op.cin_p + ci) * op.cout_p + co] = th(v);
-          wt[(static_cast<size_t>(t) * op.cout_p + co) * op.cin_p + ci] = __float2half_rn(v);
-        }
-    std::vector<float> b(op.cout_p, 0.f), sc(op.cout_p, 1.f), sh(op.cout_p, 0.f);
-    if (bias) std::copy(bias, bias + cout, b.begin());
-    if (bn_scale) std::copy(bn_scale, bn_scale + cout, sc.begin());
-    if (bn_shift) std::copy(bn_shift, bn_shift + cout, sh.begin());
-    op.h_bias = b; op.h_bn_scale = sc; op.h_bn_shift = sh;
-    op.w_simt.alloc(ws.size() * 4);
-    op.w_tc.alloc(wt.size() * 2);
-    op.bias.alloc(b.size() * 4);
-    op.bn_scale.alloc(sc.size() * 4);
-    op.bn_shift.alloc(sh.size() * 4);
-    SIVO_CUDA(cudaMemcpy(op.w_simt.p, ws.data(), ws.size() * 4, cudaMemcpyHostToDevice));
-    SIVO_CUDA(cudaMemcpy(op.w_tc.p, wt.data(), wt.size() * 2, cudaMemcpyHostToDevice));
-    SIVO_CUDA(cudaMemcpy(op.bias.p, b.data(), b.size() * 4, cudaMemcpyHostToDevice));
-    SIVO_CUDA(cudaMemcpy(op.bn_scale.p, sc.data(), sc.size() * 4, cudaMemcpyHostToDevice));
-    SIVO_CUDA(cudaMemcpy(op.bn_shift.p, sh.data(), sh.size() * 4, cudaMemcpyHostToDevice));
-    op.has_bn = bn_scale != nullptr;
+    Op op = dbg_conv_op(dt, cin, cs_in, weight, bias, bn_scale, bn_shift, cout, k, pad, relu);
     // tensors for the tc plan live in a scratch vector; run on the default stream
     if (engine == SIVO_ENGINE_TCGEN05 && dt == DType::F32) {  // split-operand fp32 mode
       TensorView vs = vi;
@@ -703,6 +708,34 @@ int sivo_dbg_conv(int device, int engine, int precision, const float* in, int n,
       p.k = k; p.pad = pad; p.cin_p = op.cin_p; p.cout_p = op.cout_p; p.relu = op.relu; p.slope = 0.f;
       launch_conv_simt(p, nullptr);
     }
+    SIVO_CUDA(cudaDeviceSynchronize());
+    download_nchw(vo, out);
+    SIVO_CUDA(cudaDeviceSynchronize());
+  });
+}
+
+int sivo_dbg_conv_unpooled(int device, const float* pooled, const int* mask, int n, int mask_n, int h, int w, const float* weight,
+                           const float* bias, const float* bn_scale, const float* bn_shift, int cout, int k, float* out) {
+  return guarded([&] {
+    if (!pooled || !mask || !weight || !out) fail(SIVO_EINVAL, "conv_unpooled: null argument");
+    if (n < 1 || mask_n < 1 || mask_n > n || h < 1 || w < 1 || cout < 1 || cout > 16 || k != 7)
+      fail(SIVO_EINVAL, "conv_unpooled: needs n, h, w >= 1, 1 <= mask_n <= n, 1 <= cout <= 16 and k = 7");
+    SIVO_CUDA(cudaSetDevice(device));
+    const size_t mask_cnt = static_cast<size_t>(mask_n) * 64 * h * w;
+    DevBuf bp, bo, bm(mask_cnt), bmi(mask_cnt * sizeof(int));
+    TensorView vp = make_view(bp, n, 64, h, w, 64, DType::F16);
+    TensorView vo = make_view(bo, n, cout, 2 * h, 2 * w, 16, DType::F32);
+    upload_nchw(pooled, vp);
+    SIVO_CUDA(cudaMemcpy(bmi.p, mask, mask_cnt * sizeof(int), cudaMemcpyHostToDevice));
+    launch_mask_from_nchw(bmi.as<int>(), mask_n, 64, h, w, bm.as<uint8_t>(), nullptr);
+    Op op = dbg_conv_op(DType::F16, 64, 64, weight, bias, bn_scale, bn_shift, cout, k, (k - 1) / 2, 0);
+    TensorView vu = vp;  // the unpooled input's shape: the plan is made for it, and then reads the pooled tensor instead
+    vu.h = 2 * h;
+    vu.w = 2 * w;
+    if (!conv_tc_supported(op, vu, vo)) fail(SIVO_EINVAL, "conv_unpooled: shape not supported by the tensor-core kernel");
+    op.tc = conv_tc_plan(op, vu, vo, op.w_tc.p);
+    conv_tc_set_unpool_input(*op.tc, vp.p, bm.as<uint8_t>(), mask_n, h, w);
+    conv_tc_launch(*op.tc, op, nullptr);
     SIVO_CUDA(cudaDeviceSynchronize());
     download_nchw(vo, out);
     SIVO_CUDA(cudaDeviceSynchronize());

@@ -27,6 +27,7 @@
 //  * Constants (bias, BN, classifier weights) are kernel parameters: the epilogue reads them from the constant bank and
 //    leaves the shared-memory data path to the MMA operand reads.
 //  * The 64 -> 16 float-logits layers (K = 3, 7) run on k_conv_stack instead: tap rows stacked along N, resident weights.
+//    Fed by a max-unpool (Basic's composed classifier), it unpools the pooled tensor as it loads its halo rows.
 #include <cuda.h>
 #include <cuda_fp16.h>
 
@@ -92,6 +93,9 @@ struct TcParams {
   // the 64-channel output itself is then never written
   int has_cls;
   float* cls_out;          // [N][H][W][16]
+  // k_conv_stack<K, true>: the input is the max-unpool of this pooled tensor [N][H/2][W/2][64] by unpool_mask (same shape,
+  // batch mask_n), expanded as the halo rows are loaded; the 2H x 2W unpooled tensor is never stored
+  const __half* unpool_in;
 };
 
 // Per-layer constants, passed by value as a kernel parameter so that the epilogue reads them from the constant bank.
@@ -749,6 +753,80 @@ __device__ __forceinline__ void stack_row(float (&acc)[K][8], uint32_t a_row, ui
   }
 }
 
+// The halo producer of k_conv_stack<K, true>, run by all four warps of warpgroup 0: each halo row -- input row y of the
+// 2H x 2W unpooled tensor, pixels x0 - pad .. x0 + 127 + pad -- is expanded from pooled row y / 2 straight into its ring
+// slot.  Per pooled pixel j and 8-channel chunk c, one thread loads the 16 bytes of values and the 8 mask bytes and writes
+// the 16-byte chunks of pixels 2 j and 2 j + 1: each channel keeps its value where its mask code is 2 (y & 1) + dx and is
+// zero elsewhere, the select epilogue_flush scatters with, so the slot holds the bits the unpooled tensor would.  Chunks go
+// to their SWIZZLE_128B position (the slots are 1 KB aligned); rows and pixels outside the image are written as zeros,
+// since slots are reused (TMA's zero fill in the plain kernel).  A row's loads are issued before the wait for its slot, so
+// their latency hides under the consumers' MMAs of the previous row.
+template <int K>
+__device__ __forceinline__ void stack_unpool_producer(const TcParams& p, uint8_t* a_slots, uint64_t* a_full, uint64_t* a_empty,
+                                                      long t_begin, long t_end) {
+  constexpr int kPad = (K - 1) / 2;
+  constexpr int kSlots = stack_slots(K);
+  constexpr int kHalo = 128 + K - 1;
+  constexpr int kLeft = (kPad + 1) / 2;                  // pooled pixels the halo reaches left of x0 / 2
+  constexpr int kPooled = kLeft + (127 + kPad) / 2 + 1;  // pooled pixels per halo row (68 for K = 7)
+  constexpr int kSteps = (kPooled * 8 + 127) / 128;      // (pixel, chunk) pairs per thread
+  // thread: chunk c of pooled pixels j = jt + 16 s (halo-relative jr = jr0 + 16 s); the addresses of steps s differ by
+  // compile-time strides, so a row needs one pointer per tensor
+  const int tid = threadIdx.x, c = tid & 7, lane = tid & 31, jr0 = tid >> 3;
+  const int Hp = p.H >> 1, Wp = p.W >> 1;
+  // halo pixel of (jr0, dx): image pixel x0 - pad + px = 2 j + dx.  Its swizzle phase px & 7 is the same for every step.
+  const int px0 = 2 * jr0 + kPad - 2 * kLeft;
+  uint32_t u = 0;
+  for (long t = t_begin; t < t_end;) {
+    const int col = static_cast<int>(t / p.H), y_start = static_cast<int>(t % p.H);
+    const int n_out = static_cast<int>(min(static_cast<long>(p.H - y_start), t_end - t));
+    const int img = col / p.strips, jt = (col % p.strips) * 64 - kLeft + jr0;
+    uint32_t live = 0;  // steps whose pooled pixel is inside the image
+#pragma unroll
+    for (int s = 0; s < kSteps; ++s)
+      if (jr0 + 16 * s < kPooled && jt + 16 * s >= 0 && jt + 16 * s < Wp) live |= 1u << s;
+    const long v_img = static_cast<long>(img) * Hp, m_img = static_cast<long>(img % p.mask_n) * Hp;
+    for (int r = 0; r < n_out + K - 1; ++r, ++u) {
+      const int y = y_start - kPad + r;
+      const uint32_t row_live = y >= 0 && y < p.H ? live : 0u;
+      const __half* const vp = p.unpool_in + ((v_img + (y >> 1)) * Wp + jt) * 64 + 8 * c;
+      const uint8_t* const mp = p.unpool_mask + ((m_img + (y >> 1)) * Wp + jt) * 64 + 8 * c;
+      uint4 v[kSteps];
+      uint2 m[kSteps];
+#pragma unroll
+      for (int s = 0; s < kSteps; ++s) {
+        v[s] = make_uint4(0u, 0u, 0u, 0u);
+        m[s] = make_uint2(0u, 0u);
+        if (row_live & (1u << s)) {
+          v[s] = __ldg(reinterpret_cast<const uint4*>(vp + s * 16 * 64));
+          m[s] = __ldg(reinterpret_cast<const uint2*>(mp + s * 16 * 64));
+        }
+      }
+      const int slot = u % kSlots;
+      mbar_wait(a_empty + slot, ((u / kSlots) & 1) ^ 1);
+      uint8_t* const dst = a_slots + slot * kSlotBytes;
+#pragma unroll
+      for (int dx = 0; dx < 2; ++dx) {
+        const int px = px0 + dx;
+        uint8_t* const d = dst + px * 128 + ((c ^ (px & 7)) << 4);
+        const uint32_t code = 0x01010101u * static_cast<uint32_t>(2 * (y & 1) + dx);
+#pragma unroll
+        for (int s = 0; s < kSteps; ++s) {
+          if (jr0 + 16 * s >= kPooled || px + 32 * s < 0 || px + 32 * s >= kHalo) continue;
+          const uint32_t lo = __vcmpeq4(m[s].x, code), hi = __vcmpeq4(m[s].y, code);  // 0xFF per matching byte
+          const uint4 o = make_uint4(v[s].x & __byte_perm(lo, 0u, 0x1100), v[s].y & __byte_perm(lo, 0u, 0x3322),
+                                     v[s].z & __byte_perm(hi, 0u, 0x1100), v[s].w & __byte_perm(hi, 0u, 0x3322));
+          *reinterpret_cast<uint4*>(d + s * 32 * 128) = o;
+        }
+      }
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes, read by wgmma
+      __syncwarp();
+      if (lane == 0) mbar_arrive(a_full + slot);
+    }
+    t += n_out;
+  }
+}
+
 // Cin = 64 -> 16 float channels, K x K (K = 3, 7): the float-logits layers (the composed classifier, Standard's conv1_1_D).
 // An m64n16k16 MMA reads a 2 KB A tile for 16 output columns, which makes the 16-wide k_conv_tc tile bound by shared-memory
 // operand reads.  Here the K tap rows are stacked along N instead: ONE m64n{16K}k16 per (kw, K step) of input row i computes
@@ -768,7 +846,10 @@ __device__ __forceinline__ void stack_row(float (&acc)[K][8], uint32_t a_row, ui
 //  * A CTA emits rows [b R, b R + R) of the flattened (image, strip, row) range; each maximal run of rows within one strip
 //    first walks K - 1 warm-up input rows, whose MMAs only feed rows that are not emitted.  Every input row is read by one
 //    step and then released, so the halo ring is pure prefetch.
-template <int K>
+//  * UNPOOL: the input is a max-unpool (Basic's upsample1 -> conv_decode1); the four producer warps expand each halo row
+//    from the pooled tensor and its mask (stack_unpool_producer) instead of one TMA box, so the unpooled tensor, three
+//    quarters zeros, is neither written nor read back.  The consumers are unchanged.
+template <int K, bool UNPOOL = false>
 __global__ void __launch_bounds__(kTcThreads, 1)
 k_conv_stack(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const __grid_constant__ TcParams p,
              const __grid_constant__ TcConsts cst) {
@@ -792,7 +873,8 @@ k_conv_stack(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ 
   const long t_end = min(t_begin + p.rows_per_cta, rows);
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < kSlots; ++i) { mbar_init(a_full + i, 1); mbar_init(a_empty + i, kEmptyArrivals); }
+    // UNPOOL: each of the four producer warps arrives once it has written its share of a halo row
+    for (int i = 0; i < kSlots; ++i) { mbar_init(a_full + i, UNPOOL ? 4 : 1); mbar_init(a_empty + i, kEmptyArrivals); }
     mbar_init(w_full, 1);
     mbar_init(w_ready, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -801,8 +883,11 @@ k_conv_stack(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ 
   __syncthreads();
 
   if (wg == 0) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
-    if (warp == 0 && lane == 0) {
+    // UNPOOL: the expanding producers keep a row's loads in flight (30 registers of values and masks per thread):
+    // 128 x 80 + 256 x 208 = 63 488 <= 64 512
+    if constexpr (UNPOOL) asm volatile("setmaxnreg.dec.sync.aligned.u32 80;" ::: "memory");
+    else asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+    if (warp == 0 && lane == 0 && !UNPOOL) {
       // ===== halo-row producer: per run, input rows y_start - pad .. y_end - 1 + pad =====
       asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_a)) : "memory");
       uint32_t u = 0;
@@ -836,10 +921,12 @@ k_conv_stack(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ 
       __syncwarp();
       if (lane == 0) mbar_arrive(w_ready);
     }
+    if constexpr (UNPOOL) stack_unpool_producer<K>(p, a_slots, a_full, a_empty, t_begin, t_end);
     return;
   }
 
-  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+  if constexpr (UNPOOL) asm volatile("setmaxnreg.inc.sync.aligned.u32 208;" ::: "memory");
+  else asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
   // ===== consumers: warpgroup g = wg - 1 owns pixels [64 g, 64 g + 64) of the strip =====
   const int g = wg - 1;
   const int m0 = 16 * (warp & 3) + (lane >> 2);
@@ -944,7 +1031,8 @@ void conv_tc_dispatch(const ConvTcPlan& plan, cudaStream_t s, bool configure) {
   } else if (plan.pk2) {
     if (plan.p.n_tile == 64) go(k_conv_tc<3, false, 3, true, 64, false>); else go(k_conv_tc<3, false, 3, true, 128, false>);
   } else if (plan.stack) {  // 64 -> 16 float logits, K = 3 / 7
-    if (K == 7) go(k_conv_stack<7>); else go(k_conv_stack<3>);
+    if (K == 7) { if (plan.p.unpool_in) go(k_conv_stack<7, true>); else go(k_conv_stack<7>); }
+    else go(k_conv_stack<3>);
   } else if (plan.roll) {
     if (K == 7) { if (plan.p.n_tile == 64) go(k_conv_tc<7, true, 7, false, 64, false>); else go(k_conv_tc<7, true, 7, false, 128, false>); }
     else if (K == 3) { if (plan.p.n_tile == 64) go(k_conv_tc<3, true, 3, false, 64, false>); else go(k_conv_tc<3, true, 3, false, 128, false>); }
@@ -1112,7 +1200,7 @@ std::shared_ptr<ConvTcPlan> conv_tc_plan(const Op& op, const TensorView& in, con
   }
   p.out = out.p;
   p.has_drop = 0; p.seed = 0; p.frame = nullptr; p.drop_nl = 0; p.drop_scale = 2.f;
-  p.unpool_mask = nullptr; p.mask_n = 1;
+  p.unpool_mask = nullptr; p.mask_n = 1; p.unpool_in = nullptr;
   p.pool_out = nullptr; p.pool_mask = nullptr;
   p.has_cls = 0; p.cls_out = nullptr;
   plan->grid = dim3(p.strips * ceil_div(total_pairs, p.pairs_per_cta), cout_tiles, n_z);
@@ -1141,6 +1229,16 @@ void conv_tc_set_unpool(ConvTcPlan& plan, const uint8_t* mask, int mask_n, void*
   plan.p.unpool_mask = mask;
   plan.p.mask_n = mask_n;
   plan.p.out = out_2h_2w;
+}
+
+void conv_tc_set_unpool_input(ConvTcPlan& plan, const void* pooled, const uint8_t* mask, int mask_n, int h, int w) {
+  if (!plan.stack || plan.k != 7 || 2 * h != plan.p.H || 2 * w != plan.p.W || !pooled || !mask || mask_n < 1)
+    fail(SIVO_EINVAL, "conv_tc_set_unpool_input: needs a 7x7 float-logits plan over the %d x %d unpooled input (got %d x %d pooled)",
+         plan.p.H, plan.p.W, h, w);
+  plan.p.unpool_in = static_cast<const __half*>(pooled);
+  plan.p.unpool_mask = mask;
+  plan.p.mask_n = mask_n;
+  conv_tc_dispatch(plan, nullptr, true);
 }
 
 std::vector<__half> conv_tc_split_weights(const float* W, int cout, int cin, int K, int cout_p, int cin_p, float* acc_scale) {

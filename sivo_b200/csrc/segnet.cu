@@ -122,7 +122,7 @@ void SegNet::build(const NetSpec& net, const WeightMap& weights) {
     auto it = by_name_.find(name);
     if (it == by_name_.end()) fail(SIVO_EFORMAT, "prototxt: blob '%s' is used before it is produced", name.c_str());
     // a fused kernel consumes this blob in registers and never writes it: a second consumer would read uninitialised memory
-    if (tensors_[it->second]->elided)
+    if (tensors_[it->second]->elided || tensors_[it->second]->derived_from >= 0)
       fail(SIVO_EFORMAT, "prototxt: blob '%s' has more than one consumer; the fused pool / unpool / dropout / classifier paths need a "
                          "single-consumer chain (create the net with keep_blobs to run it unfused)", name.c_str());
     return it->second;
@@ -232,6 +232,26 @@ void SegNet::build(const NetSpec& net, const WeightMap& weights) {
             // the 16-wide composed layer, warm-up rows included
             conv.flops_exec = 2.0 * conv.cin * conv.k * conv.k * 16 * iv.h * iv.w * iv.n * conv_tc_rows_ratio(*conv.tc);
             conv.layer += "*" + ly.name;  // '*': composed, not merely fused
+            Op* up = ops_.size() >= 2 ? &ops_[ops_.size() - 2] : nullptr;
+            if (up && up->kind == Op::Conv && up->use_tc && up->out2 == conv.in) {
+              // the input is scattered by the previous convolution's fused unpool (Basic: conv_decode2 -> upsample1), three
+              // quarters zeros: take that fusion back.  The previous convolution stores its own pooled-resolution output, and
+              // the composed kernel unpools it as it loads its halo rows.  The unpooled tensor is derived, never written.
+              Tensor& pooled = *tensors_[up->out];
+              Tensor& unpooled = *tensors_[conv.in];
+              const Tensor& mask = *tensors_[up->in2];
+              conv_tc_set_unpool(*up->tc, nullptr, 1, pooled.v.p);
+              pooled.elided = false;
+              conv_tc_set_unpool_input(*conv.tc, pooled.v.p, mask.buf.as<uint8_t>(), mask.v.n, pooled.v.h, pooled.v.w);
+              unpooled.derived_from = up->out;
+              unpooled.derived_mask = up->in2;
+              unpooled.buf.release();
+              unpooled.v.p = nullptr;
+              const size_t plus = up->layer.rfind('+');  // the unpool is the last layer fused into it
+              conv.layer = up->layer.substr(plus + 1) + "+" + conv.layer;
+              up->layer.erase(plus);
+              up->in2 = up->out2 = -1;
+            }
           } else {
             conv_tc_set_classifier(*conv.tc, op.h_w.data(), op.cout_p, op.h_bias.data(), std::min(16, op.cout_p),
                                    static_cast<float*>(tensors_[op.out]->v.p));
@@ -302,6 +322,8 @@ void SegNet::build(const NetSpec& net, const WeightMap& weights) {
           conv_tc_set_unpool(*ops_.back().tc, mt.buf.as<uint8_t>(), mt.v.n, tensors_[up]->v.p);
           tensors_[in]->elided = true;
           ops_.back().layer += "+" + ly.name;
+          ops_.back().in2 = m;  // recorded so that a consumer that unpools on load can take the fusion back
+          ops_.back().out2 = up;
           break;
         }
         if (!opt_.keep_blobs && !ops_.empty() && ops_.back().kind == Op::Dropout && ops_.back().out == in && iv.dt == DType::F16 &&
@@ -766,7 +788,7 @@ void SegNet::run_host(const uint8_t* bgr, int rows, int cols, size_t stride, uin
 void SegNet::blob(const std::string& name, float* out, size_t cap, int* n, int* c, int* h, int* w) {
   auto it = by_name_.find(name);
   if (it == by_name_.end()) fail(SIVO_EINVAL, "no blob named '%s'", name.c_str());
-  const Tensor& t = *tensors_[it->second];
+  Tensor& t = *tensors_[it->second];
   if (t.elided && out)
     fail(SIVO_EINVAL, "blob '%s' is not materialised in this build (a fused kernel consumes it); create the net with keep_blobs", name.c_str());
   if (n) *n = t.v.n;
@@ -777,6 +799,14 @@ void SegNet::blob(const std::string& name, float* out, size_t cap, int* n, int* 
   size_t count = static_cast<size_t>(t.v.n) * t.v.c * t.v.h * t.v.w;
   if (cap < count) fail(SIVO_ERANGE, "blob '%s' has %zu values, buffer holds %zu", name.c_str(), count, cap);
   SIVO_CUDA(cudaSetDevice(device_));
+  if (t.derived_from >= 0) {  // computed from the last run's tensors it derives from, with the unpool kernel of the unfused build
+    if (!t.buf.p) {
+      t.buf.alloc(t.v.bytes());
+      t.v.p = t.buf.p;
+    }
+    const Tensor& mt = *tensors_[t.derived_mask];
+    launch_unpool(tensors_[t.derived_from]->v, mt.buf.as<uint8_t>(), mt.v.n, t.v, stream_);
+  }
   DevBuf tmp(count * sizeof(float));
   if (t.is_mask) {
     launch_mask_to_nchw(t.buf.as<uint8_t>(), t.v.n, t.v.c, t.v.h, t.v.w, tmp.as<int>(), stream_);

@@ -23,6 +23,9 @@ struct Tensor {
   DevBuf buf;
   bool is_mask = false;  // u8 2-bit argmax codes, dims = pooled dims
   bool elided = false;   // a fusion consumes this blob in registers: it is never written (blob() refuses to read it)
+  // >= 0: the max-unpool of tensor `derived_from` by mask tensor `derived_mask`, which its consumer expands as it loads: no
+  // kernel writes it, and blob() computes it on demand into a buffer allocated on that first read
+  int derived_from = -1, derived_mask = -1;
 };
 
 struct Op {
@@ -169,6 +172,9 @@ void conv_tc_set_dropout(ConvTcPlan& plan, uint64_t seed, const uint64_t* frame_
 // fuses the max-unpool (Upsample) that consumes the convolution's output into its epilogue; `out_2h_2w` is the
 // unpooled tensor the convolution then writes instead of its own output
 void conv_tc_set_unpool(ConvTcPlan& plan, const uint8_t* mask, int mask_n, void* out_2h_2w);
+// makes a 7x7 float-logits (k_conv_stack) plan read the max-unpool of `pooled` ([n][h][w][64] half, the plan's input being
+// 2h x 2w) by `mask` (same layout, batch mask_n) instead of its input tensor: the unpool is done as the halo rows are loaded
+void conv_tc_set_unpool_input(ConvTcPlan& plan, const void* pooled, const uint8_t* mask, int mask_n, int h, int w);
 // fuses the 2x2/2 max pool (+ argmax mask) that consumes the convolution's output into its epilogue
 bool conv_tc_can_fuse_pool(const ConvTcPlan& plan);
 void conv_tc_set_pool(ConvTcPlan& plan, void* pooled, uint8_t* mask);
