@@ -312,6 +312,97 @@ int sivo_info_select_device(const sivo_orb_t* left, const sivo_keypoint* kps_dev
 int sivo_dbg_info_terms(const sivo_orb_t* left, const sivo_keypoint* kps, const float* depth, int n, const sivo_info_camera* cam,
                         float* world, double* det_state, double* det_meas, double* det_joint);
 
+/* ---- map points matched to a frame's semantic keys by projection: ORBmatcher::SearchByProjection(F, vpMapPoints, th) after
+ * Frame::isInFrustum (Tracking::SearchLocalPoints, Tracking.cc:1033-1085) and SearchByProjection(CurrentFrame, LastFrame, th)
+ * (Tracking::TrackWithMotionModel, Tracking.cc:704-746), with the Frame's grid (Frame.cc:205-223, 326-404) ------------------
+ * Every operation is the IEEE float / double operation as written (no contracted multiply-add).  The rules, which
+ * oracle/track_oracle.py restates:
+ *   grid      key j goes to cell (round((x - min_x) * wInv), round((y - min_y) * hInv)), round = half away from zero, wInv =
+ *             64.f / (max_x - min_x), hInv = 48.f / (max_y - min_y) in float; dropped outside 64 x 48; ascending j per cell.
+ *   area      GetFeaturesInArea(x, y, r, minLevel, maxLevel): cells floor(((x - min_x) - r) * wInv) .. ceil(((x - min_x) + r) *
+ *             wInv) with Frame.cc:334-358's early returns and clamps (same in y); walk ix ascending, then iy, then the cell's
+ *             keys; levels filtered only when minLevel > 0 || maxLevel >= 0; kept iff |kp.x - x| < r && |kp.y - y| < r.
+ *   Pc        ((R[r][0] X + R[r][1] Y) + R[r][2] Z) + t[r] in float (cv::gemm's 3 x 3 float form).
+ *   frustum   (local-map search, isInFrustum(pMP, 0.5) + PredictScale) out if Pc_z < 0; invz = 1.0f / Pc_z; u = (fx Pc_x) invz + cx,
+ *             v likewise; out unless min_x <= u <= max_x and min_y <= v <= max_y; dist = (float) sqrt of ((0 + a0 a0) + a1 a1) + a2 a2
+ *             in double over a = pos - Ow in float (cv::norm); out unless 0.8f min_distance <= dist <= 1.2f max_distance; viewCos =
+ *             (float)(((0 + a0 n0) + a1 n1) + a2 n2 in double / dist) (Mat::dot's scalar path for three floats, not pinnable
+ *             against Python: only a viewCos within an ulp of 0.5 or 0.998 can depend on it); out if viewCos < 0.5f; level =
+ *             ceil(logf(max_distance / dist) / logf(scale_factor)) clamped to [0, nlevels).  MapPoint.cc sees `using namespace
+ *             std` through MapPoint.h -> KeyFrame.h -> ORBVocabulary.h -> DBoW2's TemplatedVocabulary.h, so PredictScale's log is
+ *             the float overload; logf here is the correctly rounded float logarithm, within an ulp of glibc's.  projXR = u -
+ *             mbf invz.
+ *   local     per point in order, if in view: r = viewCos > 0.998 ? 2.5f : 4.0f, times th when th != 1; radius = r scale[level];
+ *             candidates = area(u, v, radius, level - 1, level) minus keys held by an observed point and keys with u_right > 0
+ *             and |projXR - u_right| > radius; best / second fold as ORBmatcher.cc:86-113; accepted iff bestDist <= 100 and not
+ *             (bestLevel == bestLevel2 && bestDist > nnratio bestDist2); an accepted point takes its key (F.mvpMapPoints[bestIdx] =
+ *             pMP), which blocks the key for every later point iff the point is observed.
+ *   last      twc = -Rcw^T tcw (each entry the double sum of the three products, rounded to float: cv::gemm with GEMM_1_T); tlc =
+ *             Rlw twc + tlw in the Pc form; forward iff tlc_z > mb, backward iff -tlc_z > mb.  Per point in order: invzc = (float)
+ *             (1.0 / Pc_z) in double, out if invzc < 0; u, v with invzc, out of bounds as above; o = octave; radius = th scale[o];
+ *             area(u, v, radius, o, -1) forward, (0, o) backward, else (o - 1, o + 1); the stereo gate uses ur = u - mbf invzc;
+ *             best distance only, accepted iff <= 100; the key is taken as above (a key taken by an unobserved point can be taken
+ *             again: the last writer wins).  Rotation check: rot = angle - key angle, + 360 if negative; bin = roundf(rot * (1.f /
+ *             30)), 30 -> 0 (so only bins 0..12 are used, as in the reference); ComputeThreeMaxima with its 0.1f * max1 rule; every
+ *             entry of every other bin frees its key and decrements the count, duplicates included.
+ *   NaN       a point whose u, v, viewCos or level quotient is NaN is not in view (the reference converts a NaN to int there).
+ * Map-point order and claims make the result sequential; the device walks the points in order in one block and re-searches only
+ * the points whose best (or, local, second-best) key an earlier point took. */
+typedef struct sivo_track_frame {          /* the current Frame's members */
+  float fx, fy, cx, cy, mb, mbf;
+  float min_x, max_x, min_y, max_y;        /* mnMinX, mnMaxX, mnMinY, mnMaxY (ComputeImageBounds) */
+  float Rcw[9], tcw[3], Ow[3];             /* mRcw row-major, mtcw, mOw */
+} sivo_track_frame;
+
+typedef struct sivo_map_point {            /* 80 bytes, one per map point */
+  uint8_t desc[32];                        /* GetDescriptor */
+  float pos[3], normal[3];                 /* GetWorldPos, GetNormal */
+  float min_distance, max_distance;        /* mfMinDistance, mfMaxDistance: the search applies 0.8f / 1.2f itself */
+  int32_t observed;                        /* Observations() > 0 */
+  int32_t octave;                          /* last-frame search: LastFrame.mvKeysSemantic[i].octave */
+  float angle;                             /* last-frame search: LastFrame.mvKeysSemantic[i].angle */
+  int32_t reserved;
+} sivo_map_point;
+
+/* SearchLocalPoints' isInFrustum loop and SearchByProjection(F, vpMapPoints, th) on device buffers.  Semantic key j <
+ * *n_keep_device is extractor key keep_idx_device[j] (j when NULL) of kps_device / desc_device (the Frame tail's buffers);
+ * u_right_device[j] is its mvRight.  blocked_device[j] (u8, may be NULL) = mvpMapPoints[j] && Observations() > 0 on entry.  The
+ * points are mvpLocalMapPoints in order, without the ones SearchLocalPoints skips (already seen by the frame, bad).  Outputs (any
+ * may be NULL): in_view_device[i] (u8, n_points) = isInFrustum's result (the caller's IncreaseVisible); match_device[j] (int,
+ * sivo_orb_capacity(left)) = the point this call gave key j, or -1; *n_matches_device (int64) = SearchByProjection's return.
+ * *n_keep_device is clamped to the capacity; a negative count writes only *n_matches_device = -1.  A key index outside the
+ * capacity is in no cell.  Runs on `stream` (NULL = the left extractor's stream) with no waits of its own and no host
+ * synchronisation.  Scratch lives on the left extractor: calls sharing it must be ordered among themselves and before its next
+ * sivo_orb_enqueue_device.  SIVO_EINVAL for NULL handles or inputs, n_points < 0, th <= 0, nnratio not finite, or max <= min in
+ * the bounds. */
+int sivo_search_local_points_device(const sivo_orb_t* left, const sivo_keypoint* kps_device, const uint8_t* desc_device,
+                                    const int* keep_idx_device, const long long* n_keep_device, const float* u_right_device,
+                                    const uint8_t* blocked_device, const sivo_map_point* points_device, int n_points,
+                                    const sivo_track_frame* frame, float th, float nnratio, uint8_t* in_view_device, int* match_device,
+                                    long long* n_matches_device, void* stream);
+/* SearchByProjection(CurrentFrame, LastFrame, th) (stereo) on device buffers, keys as above.  The points are the last frame's
+ * non-NULL, non-outlier map points in key order, each with its key's octave and angle; no key is blocked on entry (Tracking
+ * clears mvpMapPoints before both calls).  Rlw / tlw: the last frame's pose (host, row-major 3 x 3 and 3).  match_device /
+ * n_matches_device as above.  A point whose octave is outside [0, nlevels) is never matched (the host form refuses it). */
+int sivo_search_last_frame_device(const sivo_orb_t* left, const sivo_keypoint* kps_device, const uint8_t* desc_device,
+                                  const int* keep_idx_device, const long long* n_keep_device, const float* u_right_device,
+                                  const sivo_map_point* points_device, int n_points, const sivo_track_frame* frame, const float* Rlw,
+                                  const float* tlw, float th, int* match_device, long long* n_matches_device, void* stream);
+/* Host forms: n keys gathered per semantic key (mvKeysSemantic, mDescriptorsSemantic n x 32, mvRight, blocked may be NULL), points
+ * on the host; outputs in_view (n_points), match (n), *n_matches, any may be NULL.  They stage the inputs and run the device
+ * forms' kernels, then synchronise.  SIVO_EINVAL as above and for n < 0; SIVO_ERANGE for a last-frame octave outside [0, nlevels). */
+int sivo_search_local_points(const sivo_orb_t* left, const sivo_keypoint* kps, const uint8_t* desc, const float* u_right,
+                             const uint8_t* blocked, int n, const sivo_map_point* points, int n_points, const sivo_track_frame* frame,
+                             float th, float nnratio, uint8_t* in_view, int* match, int* n_matches);
+int sivo_search_last_frame(const sivo_orb_t* left, const sivo_keypoint* kps, const uint8_t* desc, const float* u_right, int n,
+                           const sivo_map_point* points, int n_points, const sivo_track_frame* frame, const float* Rlw,
+                           const float* tlw, float th, int* match, int* n_matches);
+/* Test hook: GetFeaturesInArea on the device grid of n host keys within the bounds.  Query q is (xyr[3 q], xyr[3 q + 1],
+ * xyr[3 q + 2], levels[2 q], levels[2 q + 1]); its list is idx[offsets[q] .. offsets[q + 1]).  SIVO_ERANGE (offsets written) if
+ * idx_cap is too small. */
+int sivo_dbg_features_in_area(const sivo_orb_t* left, const sivo_keypoint* kps, int n, float min_x, float max_x, float min_y,
+                              float max_y, const float* xyr, const int* levels, int n_query, int* offsets, int* idx, int idx_cap);
+
 /* Best / second-best match over per-query candidate lists -- the inner loop of ORBmatcher::SearchByProjection
  * (ORBmatcher.cc:79-113), its last-frame / keyframe variants (:1278-, :1420-), SearchForTriangulation (:631-) and
  * SearchBySim3 (next row 4).  Query i's candidates are cand_idx[cand_offsets[i] .. cand_offsets[i+1]) (indices into the

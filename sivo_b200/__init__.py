@@ -3,3 +3,5 @@ Host-side mirrors of the reference's two operators over the C-ABI of libsivo_b20
 from .segnet import BayesianSegNet, BayesianSegNetParams, sample_ranges  # noqa: F401
 from .orb import ORBextractor, distribute_octtree, stereo_hamming, stereo_match, stereo_match_device, KP_DTYPE  # noqa: F401
 from .info import InfoCamera, info_select, info_select_device, make_camera  # noqa: F401
+from .track import (MAP_POINT_DTYPE, TrackFrame, make_frame, map_points, search_last_frame, search_last_frame_device,  # noqa: F401
+                    search_local_points, search_local_points_device)

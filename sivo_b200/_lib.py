@@ -68,6 +68,11 @@ def lib() -> C.CDLL:
         _lib.sivo_info_select.argtypes = [vp, vp, vp, vp, i32, vp, C.c_double, vp, vp, vp, vp]
         _lib.sivo_info_select_device.argtypes = [vp, vp, vp, vp, vp, vp, vp, C.c_double, vp, vp, vp, vp, vp]
         _lib.sivo_dbg_info_terms.argtypes = [vp, vp, vp, i32, vp, vp, vp, vp, vp]
+        _lib.sivo_search_local_points_device.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, i32, vp, f32, f32, vp, vp, vp, vp]
+        _lib.sivo_search_last_frame_device.argtypes = [vp, vp, vp, vp, vp, vp, vp, i32, vp, vp, vp, f32, vp, vp, vp]
+        _lib.sivo_search_local_points.argtypes = [vp, vp, vp, vp, vp, i32, vp, i32, vp, f32, f32, vp, vp, vp]
+        _lib.sivo_search_last_frame.argtypes = [vp, vp, vp, vp, i32, vp, i32, vp, vp, vp, f32, vp, vp]
+        _lib.sivo_dbg_features_in_area.argtypes = [vp, vp, i32, f32, f32, f32, f32, vp, vp, i32, vp, vp, i32]
         _lib.sivo_dbg_conv_unpooled.argtypes = [i32, vp, vp, i32, i32, i32, i32, vp, vp, vp, vp, i32, i32, vp]
     return _lib
 

@@ -30,6 +30,20 @@ void info_terms(const Orb& left, const sivo_keypoint* kps, const float* depth, i
 void info_select_device(const Orb& left, const sivo_keypoint* kps, const double* kp_entropy, const int* keep_idx, const long long* n_keep,
                         const float* depth, const sivo_info_camera& cam, double threshold, float* world, double* reduction, int* selected,
                         long long* n_selected, cudaStream_t s);
+void search_local_points(const Orb& left, const sivo_keypoint* kps, const uint8_t* desc, const float* u_right, const uint8_t* blocked, int n,
+                         const sivo_map_point* pts, int n_points, const sivo_track_frame& f, float th, float nnratio, uint8_t* in_view,
+                         int* match, int* n_matches);
+void search_last_frame(const Orb& left, const sivo_keypoint* kps, const uint8_t* desc, const float* u_right, int n, const sivo_map_point* pts,
+                       int n_points, const sivo_track_frame& f, const float* Rlw, const float* tlw, float th, int* match, int* n_matches);
+void search_local_points_device(const Orb& left, const sivo_keypoint* kps, const uint8_t* desc, const int* keep_idx, const long long* n_keep,
+                                const float* u_right, const uint8_t* blocked, const sivo_map_point* pts, int n_points,
+                                const sivo_track_frame& f, float th, float nnratio, uint8_t* in_view, int* match, long long* n_matches,
+                                cudaStream_t s);
+void search_last_frame_device(const Orb& left, const sivo_keypoint* kps, const uint8_t* desc, const int* keep_idx, const long long* n_keep,
+                              const float* u_right, const sivo_map_point* pts, int n_points, const sivo_track_frame& f, const float* Rlw,
+                              const float* tlw, float th, int* match, long long* n_matches, cudaStream_t s);
+void features_in_area(const Orb& left, const sivo_keypoint* kps, int n, const sivo_track_frame& f, const float* xyr, const int* levels, int nq,
+                      int* offsets, int* idx, int idx_cap);
 }  // namespace sivo
 
 using namespace sivo;
@@ -507,6 +521,65 @@ int sivo_dbg_info_terms(const sivo_orb_t* left, const sivo_keypoint* kps, const 
   return guarded([&] {
     if (!left || !cam || n < 0 || (n && (!kps || !depth))) fail(SIVO_EINVAL, "info_terms: null argument or n < 0");
     info_terms(*left->impl, kps, depth, n, *cam, world, det_state, det_meas, det_joint);
+  });
+}
+
+// ---------------------------------------------------------------------------------------- projection searches
+int sivo_search_local_points_device(const sivo_orb_t* left, const sivo_keypoint* kps_device, const uint8_t* desc_device,
+                                    const int* keep_idx_device, const long long* n_keep_device, const float* u_right_device,
+                                    const uint8_t* blocked_device, const sivo_map_point* points_device, int n_points,
+                                    const sivo_track_frame* frame, float th, float nnratio, uint8_t* in_view_device, int* match_device,
+                                    long long* n_matches_device, void* stream) {
+  return guarded([&] {
+    if (!left || !kps_device || !desc_device || !n_keep_device || !u_right_device || !frame || (n_points > 0 && !points_device))
+      fail(SIVO_EINVAL, "search_local_points: null argument");
+    search_local_points_device(*left->impl, kps_device, desc_device, keep_idx_device, n_keep_device, u_right_device, blocked_device,
+                               points_device, n_points, *frame, th, nnratio, in_view_device, match_device, n_matches_device,
+                               static_cast<cudaStream_t>(stream));
+  });
+}
+
+int sivo_search_last_frame_device(const sivo_orb_t* left, const sivo_keypoint* kps_device, const uint8_t* desc_device,
+                                  const int* keep_idx_device, const long long* n_keep_device, const float* u_right_device,
+                                  const sivo_map_point* points_device, int n_points, const sivo_track_frame* frame, const float* Rlw,
+                                  const float* tlw, float th, int* match_device, long long* n_matches_device, void* stream) {
+  return guarded([&] {
+    if (!left || !kps_device || !desc_device || !n_keep_device || !u_right_device || !frame || !Rlw || !tlw ||
+        (n_points > 0 && !points_device))
+      fail(SIVO_EINVAL, "search_last_frame: null argument");
+    search_last_frame_device(*left->impl, kps_device, desc_device, keep_idx_device, n_keep_device, u_right_device, points_device, n_points,
+                             *frame, Rlw, tlw, th, match_device, n_matches_device, static_cast<cudaStream_t>(stream));
+  });
+}
+
+int sivo_search_local_points(const sivo_orb_t* left, const sivo_keypoint* kps, const uint8_t* desc, const float* u_right,
+                             const uint8_t* blocked, int n, const sivo_map_point* points, int n_points, const sivo_track_frame* frame,
+                             float th, float nnratio, uint8_t* in_view, int* match, int* n_matches) {
+  return guarded([&] {
+    if (!left || !frame || n < 0 || (n && (!kps || !desc || !u_right)) || (n_points > 0 && !points))
+      fail(SIVO_EINVAL, "search_local_points: null argument or n < 0");
+    search_local_points(*left->impl, kps, desc, u_right, blocked, n, points, n_points, *frame, th, nnratio, in_view, match, n_matches);
+  });
+}
+
+int sivo_search_last_frame(const sivo_orb_t* left, const sivo_keypoint* kps, const uint8_t* desc, const float* u_right, int n,
+                           const sivo_map_point* points, int n_points, const sivo_track_frame* frame, const float* Rlw,
+                           const float* tlw, float th, int* match, int* n_matches) {
+  return guarded([&] {
+    if (!left || !frame || !Rlw || !tlw || n < 0 || (n && (!kps || !desc || !u_right)) || (n_points > 0 && !points))
+      fail(SIVO_EINVAL, "search_last_frame: null argument or n < 0");
+    search_last_frame(*left->impl, kps, desc, u_right, n, points, n_points, *frame, Rlw, tlw, th, match, n_matches);
+  });
+}
+
+int sivo_dbg_features_in_area(const sivo_orb_t* left, const sivo_keypoint* kps, int n, float min_x, float max_x, float min_y,
+                              float max_y, const float* xyr, const int* levels, int n_query, int* offsets, int* idx, int idx_cap) {
+  return guarded([&] {
+    if (!left || !offsets || n < 0 || n_query < 0 || (n && !kps) || (n_query && (!xyr || !levels)) || (idx_cap > 0 && !idx))
+      fail(SIVO_EINVAL, "features_in_area: null argument or negative count");
+    sivo_track_frame f{};
+    f.min_x = min_x; f.max_x = max_x; f.min_y = min_y; f.max_y = max_y;
+    features_in_area(*left->impl, kps, n, f, xyr, levels, n_query, offsets, idx, idx_cap);
   });
 }
 

@@ -1,0 +1,34 @@
+// The best / second-best fold of ORBmatcher's candidate loops (SearchByProjection, ORBmatcher.cc:79-113 and :1352-1376), shared
+// by k_hamming_best2 (stereo.cu) and the projection searches (track.cu):
+//   for idx in candidates (in order): dist = DescriptorDistance(q, train[idx]);
+//     if (dist < bestDist) { bestDist2 = bestDist; bestLevel2 = bestLevel; bestDist = dist; bestLevel = level[idx]; bestIdx = idx; }
+//     else if (dist < bestDist2) { bestLevel2 = level[idx]; bestDist2 = dist; }
+#pragma once
+#include <cuda_runtime.h>
+
+namespace sivo {
+
+struct Best2 {
+  int dist = 256, level = -1, idx = -1;    // bestDist, bestLevel, bestIdx
+  int dist2 = 256, level2 = -1, idx2 = -1;  // bestDist2, bestLevel2 and the candidate that set them last
+};
+
+// Folds lane k's candidate (d, idx, lvl) for k = 0 .. n-1 in lane order; every lane of the warp calls it with the same `b` and
+// ends with the same `b`.  A lane without a candidate passes d >= 256, which can change neither distance, so it is skipped.
+__device__ __forceinline__ void best2_fold_warp(Best2& b, int d, int idx, int lvl, int n) {
+  unsigned live = __ballot_sync(0xffffffffu, d < 256);
+  if (n < 32) live &= (1u << n) - 1u;
+  while (live) {
+    const int k = __ffs(live) - 1;
+    live &= live - 1u;
+    const int dk = __shfl_sync(0xffffffffu, d, k), ik = __shfl_sync(0xffffffffu, idx, k), lk = __shfl_sync(0xffffffffu, lvl, k);
+    if (dk < b.dist) {
+      b.dist2 = b.dist; b.level2 = b.level; b.idx2 = b.idx;
+      b.dist = dk; b.level = lk; b.idx = ik;
+    } else if (dk < b.dist2) {
+      b.level2 = lk; b.dist2 = dk; b.idx2 = ik;
+    }
+  }
+}
+
+}  // namespace sivo

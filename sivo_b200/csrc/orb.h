@@ -172,6 +172,9 @@ class Orb {
   int* stereo_sad() const { return d_stereo_sad_.as<int>(); }
   // capacity() bytes of scratch for the device information selection's per-key decisions (ordered like stereo_sad())
   uint8_t* info_flags() const { return d_info_flags_.as<uint8_t>(); }
+  // at least `bytes` of scratch for the device projection searches (track.cu), ordered like stereo_sad(); it grows by a
+  // stream-ordered reallocation on `s`, so no call synchronises the host
+  uint8_t* track_scratch(size_t bytes, cudaStream_t s);
   float device_ms = 0, tree_ms = 0;
   int launches = 0;
 
@@ -198,6 +201,8 @@ class Orb {
   DevBuf d_gray_, d_pyr_, d_blur_, d_cells_, d_cell_count_, d_cell_items_, d_cell_offset_, d_level_off_, d_cand_,
       d_sel_, d_umax_, d_angles_, d_desc_, d_scales_, d_stereo_sad_, d_info_flags_;
   PinnedBuf h_gray_, h_cand_, h_level_off_, h_sel_, h_angles_, h_desc_, h_pyr_;
+  void* d_track_ = nullptr;  // cudaMallocAsync'd by track_scratch()
+  size_t track_bytes_ = 0;
   size_t pyr_bytes_ = 0, flat_bytes_ = 0;
   int cand_cap_ = 0, sel_cap_ = 0;
   mutable std::vector<uint32_t> last_cand_;  // last call's packed candidates (x | y << 12 | resp << 24), all levels (test hook)

@@ -353,6 +353,7 @@ Orb::~Orb() {
   if (copy_stream_) cudaStreamDestroy(copy_stream_);
   if (ev_wait2_) cudaEventDestroy(ev_wait2_);
   if (stream_) cudaStreamDestroy(stream_);
+  if (d_track_) cudaFree(d_track_);
 }
 
 void Orb::level_size(int rows, int cols, int level, int* w, int* h) const {

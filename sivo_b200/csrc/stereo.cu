@@ -6,6 +6,7 @@
 #include <algorithm>
 #include <vector>
 
+#include "match_fold.cuh"
 #include "orb.h"
 
 namespace sivo {
@@ -313,8 +314,8 @@ void stereo_hamming(int device, const sivo_keypoint* left, const uint8_t* dl, in
 //   for idx in candidates (in order): dist = DescriptorDistance(q, train[idx]);
 //     if (dist < bestDist) { bestDist2 = bestDist; bestLevel2 = bestLevel; bestDist = dist; bestLevel = level[idx]; bestIdx = idx; }
 //     else if (dist < bestDist2) { bestLevel2 = level[idx]; bestDist2 = dist; }
-// One warp per query: the lanes compute 32 distances at a time, lane 0 folds them in candidate order so that ties fall
-// exactly as in the sequential loop.
+// One warp per query: the lanes compute 32 distances at a time, the warp folds them in candidate order (best2_fold_warp,
+// match_fold.cuh) so that ties fall exactly as in the sequential loop.
 namespace {
 __global__ void k_hamming_best2(const uint8_t* __restrict__ query, int nq, const uint8_t* __restrict__ train,
                                 const int* __restrict__ cand_off, const int* __restrict__ cand_idx, const int* __restrict__ level,
@@ -323,7 +324,7 @@ __global__ void k_hamming_best2(const uint8_t* __restrict__ query, int nq, const
   if (wid >= nq) return;
   const ulonglong4 a = *reinterpret_cast<const ulonglong4*>(query + static_cast<size_t>(wid) * 32);
   const int b = cand_off[wid], e = cand_off[wid + 1];
-  int best_dist = 256, best_level = -1, best_dist2 = 256, best_level2 = -1, best_idx = -1;
+  Best2 best;
   for (int base = b; base < e; base += 32) {
     const int i = base + lane;
     int d = 0x7FFFFFFF, idx = -1, lvl = -1;
@@ -333,16 +334,11 @@ __global__ void k_hamming_best2(const uint8_t* __restrict__ query, int nq, const
       d = __popcll(a.x ^ t.x) + __popcll(a.y ^ t.y) + __popcll(a.z ^ t.z) + __popcll(a.w ^ t.w);
       lvl = level ? level[idx] : 0;
     }
-    const int n = min(32, e - base);
-    for (int k = 0; k < n; ++k) {  // warp-uniform fold in candidate order
-      const int dk = __shfl_sync(0xffffffffu, d, k), ik = __shfl_sync(0xffffffffu, idx, k), lk = __shfl_sync(0xffffffffu, lvl, k);
-      if (dk < best_dist) { best_dist2 = best_dist; best_level2 = best_level; best_dist = dk; best_level = lk; best_idx = ik; }
-      else if (dk < best_dist2) { best_level2 = lk; best_dist2 = dk; }
-    }
+    best2_fold_warp(best, d, idx, lvl, min(32, e - base));  // warp-uniform fold in candidate order
   }
   if (lane == 0) {
     int* o = out + static_cast<size_t>(wid) * 5;
-    o[0] = best_idx; o[1] = best_dist; o[2] = best_level; o[3] = best_dist2; o[4] = best_level2;
+    o[0] = best.idx; o[1] = best.dist; o[2] = best.level; o[3] = best.dist2; o[4] = best.level2;
   }
 }
 }  // namespace

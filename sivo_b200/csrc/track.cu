@@ -1,0 +1,635 @@
+// Map points matched to a frame's semantic keys by projection: the Frame's grid (AssignFeaturesToGrid / PosInGrid /
+// GetFeaturesInArea, Frame.cc:205-223, 326-404), Frame::isInFrustum + MapPoint::PredictScale (Frame.cc:267-324, MapPoint.cc:439-453)
+// and the two per-frame forms of ORBmatcher::SearchByProjection (ORBmatcher.cc:44-127, 1278-1418).  The rules are spelled out in
+// include/sivo_b200.h and oracle/track_oracle.py.  This file is compiled with -fmad=false: every float / double intermediate is the
+// correctly rounded result of the operation as written.
+//
+// Three launches per search, all on the caller's stream:
+//   k_track_grid       one block: gathers the semantic keys (position, level, mvRight, descriptor, angle) and builds the 64 x 48
+//                      cell CSR (cell index ix * 48 + iy, so the cells of one column of a window are contiguous) by a counting
+//                      sort, each cell's short list then sorted by key index.
+//   k_track_project    one warp per point: projection and window, then the fold over the window's candidates in
+//                      GetFeaturesInArea order with only the entry mask applied (best and second-best recorded).
+//   k_track_ordered    one warp walks the points in order with the per-key blocked / owner state in shared memory.  A fold's
+//                      result depends on a removed candidate only if that candidate was its best or its second-best, so only
+//                      the points whose recorded best (local: or second) key an earlier point took are searched again.  The
+//                      last-frame search then runs the rotation histogram and ComputeThreeMaxima.
+#include <cmath>
+
+#include "match_fold.cuh"
+#include "orb.h"
+
+namespace sivo {
+namespace {
+constexpr int kCols = 64, kRows = 48, kCells = kCols * kRows;  // FRAME_GRID_COLS / _ROWS
+constexpr int kThHigh = 100;                                   // ORBmatcher::TH_HIGH
+constexpr int kHisto = 30;                                     // ORBmatcher::HISTO_LENGTH
+constexpr int kGridThreads = 1024;
+constexpr int kProjectThreads = 128;
+
+struct TrackParams {
+  float fx, fy, cx, cy, mbf;
+  float min_x, max_x, min_y, max_y, w_inv, h_inv;
+  float rcw[9], tcw[3], ow[3];
+  float scale[kOrbMaxLevels];
+  float log_scale;  // Frame::mfLogScaleFactor
+  float th, nnratio;
+  int nlevels;
+  int last_frame;  // 0: local-map search, 1: last-frame search
+  int forward, backward;
+};
+
+struct TrackKey {  // one semantic key as the area walk reads it
+  float x, y, ur;
+  int octave;
+};
+
+struct TrackWin {  // one point's projection and window
+  float u, v, rad, xr;
+  int lmin, lmax, in_view, pad;
+};
+
+struct TrackBufs {  // scratch of one call, carved from one allocation
+  int* cell_start;  // kCells + 1
+  int* cell_keys;   // cap
+  int* cell_of;     // cap
+  TrackKey* keys;   // cap
+  uint4* desc;      // 2 cap
+  float* angle;     // cap
+  TrackWin* win;    // n_points
+  Best2* fold;      // n_points
+  int* hist;        // n_points
+};
+
+size_t align256(size_t b) { return (b + 255) & ~static_cast<size_t>(255); }
+
+size_t scratch_bytes(int cap, int np) {
+  const size_t c = std::max(cap, 1), p = std::max(np, 1);
+  return align256((kCells + 1) * sizeof(int)) + 2 * align256(c * sizeof(int)) + align256(c * sizeof(TrackKey)) + align256(c * 32) +
+         align256(c * sizeof(float)) + align256(p * sizeof(TrackWin)) + align256(p * sizeof(Best2)) + align256(p * sizeof(int));
+}
+
+TrackBufs carve(uint8_t* base, int cap, int np) {
+  const size_t c = std::max(cap, 1), p = std::max(np, 1);
+  TrackBufs b;
+  size_t off = 0;
+  auto take = [&](size_t bytes) { uint8_t* q = base + off; off += align256(bytes); return q; };
+  b.cell_start = reinterpret_cast<int*>(take((kCells + 1) * sizeof(int)));
+  b.cell_keys = reinterpret_cast<int*>(take(c * sizeof(int)));
+  b.cell_of = reinterpret_cast<int*>(take(c * sizeof(int)));
+  b.keys = reinterpret_cast<TrackKey*>(take(c * sizeof(TrackKey)));
+  b.desc = reinterpret_cast<uint4*>(take(c * 32));
+  b.angle = reinterpret_cast<float*>(take(c * sizeof(float)));
+  b.win = reinterpret_cast<TrackWin*>(take(p * sizeof(TrackWin)));
+  b.fold = reinterpret_cast<Best2*>(take(p * sizeof(Best2)));
+  b.hist = reinterpret_cast<int*>(take(p * sizeof(int)));
+  return b;
+}
+
+__device__ __forceinline__ int clamp_count(const long long* n_keep, int cap) {
+  const long long n = *n_keep;
+  return n < 0 ? -1 : static_cast<int>(min(n, static_cast<long long>(cap)));
+}
+
+// ---- grid
+__global__ void __launch_bounds__(kGridThreads, 1) k_track_grid(const TrackParams p, const sivo_keypoint* __restrict__ kps,
+                                                                const uint8_t* __restrict__ desc, const int* __restrict__ keep_idx,
+                                                                const long long* __restrict__ n_keep, int cap,
+                                                                const float* __restrict__ u_right, TrackBufs b) {
+  __shared__ int cnt[kCells];
+  __shared__ int warp_sum[kGridThreads / 32];
+  const int n = clamp_count(n_keep, cap);
+  if (n < 0) return;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  for (int c = tid; c < kCells; c += kGridThreads) cnt[c] = 0;
+  __syncthreads();
+  for (int j = tid; j < n; j += kGridThreads) {
+    const int k = keep_idx ? keep_idx[j] : j;
+    int cell = -1;
+    TrackKey key{__int_as_float(0x7fc00000), __int_as_float(0x7fc00000), -1.f, -1};
+    float ang = 0.f;
+    uint4 d0 = make_uint4(0, 0, 0, 0), d1 = d0;
+    if (k >= 0 && k < cap) {
+      const sivo_keypoint kp = kps[k];
+      key = TrackKey{kp.x, kp.y, u_right[j], kp.octave};
+      ang = kp.angle;
+      d0 = reinterpret_cast<const uint4*>(desc + static_cast<size_t>(k) * 32)[0];
+      d1 = reinterpret_cast<const uint4*>(desc + static_cast<size_t>(k) * 32)[1];
+      // PosInGrid: round half away from zero; the comparisons in float keep a NaN or huge coordinate out of the int conversion
+      const float gx = roundf((kp.x - p.min_x) * p.w_inv), gy = roundf((kp.y - p.min_y) * p.h_inv);
+      if (gx >= 0.f && gx < static_cast<float>(kCols) && gy >= 0.f && gy < static_cast<float>(kRows)) {
+        cell = static_cast<int>(gx) * kRows + static_cast<int>(gy);
+        atomicAdd(&cnt[cell], 1);
+      }
+    }
+    b.keys[j] = key;
+    b.desc[2 * j] = d0;
+    b.desc[2 * j + 1] = d1;
+    b.angle[j] = ang;
+    b.cell_of[j] = cell;
+  }
+  __syncthreads();
+  // exclusive scan of the 3072 counts: three consecutive cells per thread
+  constexpr int kPer = kCells / kGridThreads;
+  int local[kPer], sum = 0;
+#pragma unroll
+  for (int q = 0; q < kPer; ++q) { local[q] = cnt[tid * kPer + q]; sum += local[q]; }
+  int incl = sum;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int v = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += v;
+  }
+  if (lane == 31) warp_sum[warp] = incl;
+  __syncthreads();
+  int before = 0;
+  for (int w = 0; w < warp; ++w) before += warp_sum[w];
+  int run = before + incl - sum;
+#pragma unroll
+  for (int q = 0; q < kPer; ++q) {
+    const int c = tid * kPer + q;
+    b.cell_start[c] = run;
+    cnt[c] = run;  // becomes the scatter cursor
+    run += local[q];
+  }
+  if (tid == kGridThreads - 1) b.cell_start[kCells] = run;
+  __syncthreads();
+  for (int j = tid; j < n; j += kGridThreads) {
+    const int c = b.cell_of[j];
+    if (c >= 0) b.cell_keys[atomicAdd(&cnt[c], 1)] = j;
+  }
+  __syncthreads();
+  // each cell's list in ascending key order (the lists are a few keys long)
+  for (int c = tid; c < kCells; c += kGridThreads) {
+    const int s = b.cell_start[c], e = b.cell_start[c + 1];
+    for (int i = s + 1; i < e; ++i) {
+      const int v = b.cell_keys[i];
+      int q = i - 1;
+      while (q >= s && b.cell_keys[q] > v) { b.cell_keys[q + 1] = b.cell_keys[q]; --q; }
+      b.cell_keys[q + 1] = v;
+    }
+  }
+}
+
+// ---- GetFeaturesInArea: visits the window's candidates 32 at a time in the reference's order.  visit(ok, j, n_in_chunk) is
+// called by every lane of the warp for every chunk; lane i holds the chunk's i-th key (ok: it passes the level and position
+// filters).  Returns without visiting when an early return of Frame.cc:334-358 applies.
+template <class Visit>
+__device__ __forceinline__ void walk_area(const TrackParams& p, const TrackBufs& b, float x, float y, float r, int min_level,
+                                          int max_level, int lane, Visit&& visit) {
+  const int min_cx = max(0, static_cast<int>(floorf(((x - p.min_x) - r) * p.w_inv)));
+  if (min_cx >= kCols) return;
+  const int max_cx = min(kCols - 1, static_cast<int>(ceilf(((x - p.min_x) + r) * p.w_inv)));
+  if (max_cx < 0) return;
+  const int min_cy = max(0, static_cast<int>(floorf(((y - p.min_y) - r) * p.h_inv)));
+  if (min_cy >= kRows) return;
+  const int max_cy = min(kRows - 1, static_cast<int>(ceilf(((y - p.min_y) + r) * p.h_inv)));
+  if (max_cy < 0) return;
+  const bool check_levels = min_level > 0 || max_level >= 0;
+  for (int ix = min_cx; ix <= max_cx; ++ix) {
+    const int s = b.cell_start[ix * kRows + min_cy], e = b.cell_start[ix * kRows + max_cy + 1];
+    for (int base = s; base < e; base += 32) {
+      const int i = base + lane;
+      int j = -1;
+      bool ok = false;
+      if (i < e) {
+        j = b.cell_keys[i];
+        const TrackKey k = b.keys[j];
+        ok = !(check_levels && (k.octave < min_level || (max_level >= 0 && k.octave > max_level))) && fabsf(k.x - x) < r &&
+             fabsf(k.y - y) < r;
+      }
+      visit(ok, j, min(32, e - base));
+    }
+  }
+}
+
+// The candidate loop of both searches over the window `w` with the key mask `blocked` (NULL: none): the stereo gate, the
+// distance and the fold in candidate order.
+__device__ __forceinline__ Best2 search_window(const TrackParams& p, const TrackBufs& b, const TrackWin& w, const uint4 q0, const uint4 q1,
+                                               const uint8_t* blocked, int lane) {
+  Best2 best;
+  walk_area(p, b, w.u, w.v, w.rad, w.lmin, w.lmax, lane, [&](bool ok, int j, int n) {
+    int d = 0x7FFFFFFF, lvl = -1;
+    if (ok && !(blocked && blocked[j])) {
+      const TrackKey k = b.keys[j];
+      if (!(k.ur > 0.f && fabsf(w.xr - k.ur) > w.rad)) {
+        const uint4 t0 = b.desc[2 * j], t1 = b.desc[2 * j + 1];
+        d = __popc(q0.x ^ t0.x) + __popc(q0.y ^ t0.y) + __popc(q0.z ^ t0.z) + __popc(q0.w ^ t0.w) + __popc(q1.x ^ t1.x) +
+            __popc(q1.y ^ t1.y) + __popc(q1.z ^ t1.z) + __popc(q1.w ^ t1.w);
+        lvl = k.octave;
+      }
+    }
+    best2_fold_warp(best, d, j, lvl, n);
+  });
+  return best;
+}
+
+// Pc = Rcw P + tcw as cv::gemm computes it for 3 x 3 floats
+__device__ __forceinline__ void to_camera(const TrackParams& p, const float* P, float* pc) {
+#pragma unroll
+  for (int r = 0; r < 3; ++r) pc[r] = ((p.rcw[3 * r] * P[0] + p.rcw[3 * r + 1] * P[1]) + p.rcw[3 * r + 2] * P[2]) + p.tcw[r];
+}
+
+// The projection and window of one point; in_view = 0 when it is not searched.
+__device__ TrackWin project(const TrackParams& p, const sivo_map_point& mp) {
+  TrackWin w{0.f, 0.f, 0.f, 0.f, 0, 0, 0, 0};
+  float pc[3];
+  to_camera(p, mp.pos, pc);
+  if (!p.last_frame) {
+    // Frame::isInFrustum(pMP, 0.5)
+    if (pc[2] < 0.0f) return w;
+    const float invz = 1.0f / pc[2];
+    const float u = p.fx * pc[0] * invz + p.cx, v = p.fy * pc[1] * invz + p.cy;
+    if (isnan(u) || isnan(v)) return w;
+    if (u < p.min_x || u > p.max_x || v < p.min_y || v > p.max_y) return w;
+    const float max_d = 1.2f * mp.max_distance, min_d = 0.8f * mp.min_distance;
+    const float a0 = mp.pos[0] - p.ow[0], a1 = mp.pos[1] - p.ow[1], a2 = mp.pos[2] - p.ow[2];
+    double ss = 0.0;
+    ss = ss + static_cast<double>(a0) * a0;
+    ss = ss + static_cast<double>(a1) * a1;
+    ss = ss + static_cast<double>(a2) * a2;
+    const float dist = static_cast<float>(sqrt(ss));
+    if (dist < min_d || dist > max_d) return w;
+    double dot = 0.0;
+    dot = dot + static_cast<double>(a0) * mp.normal[0];
+    dot = dot + static_cast<double>(a1) * mp.normal[1];
+    dot = dot + static_cast<double>(a2) * mp.normal[2];
+    const float view_cos = static_cast<float>(dot / static_cast<double>(dist));
+    if (isnan(view_cos) || view_cos < 0.5f) return w;
+    // MapPoint::PredictScale(dist, F)
+    const float ratio = mp.max_distance / dist;
+    const float lq = static_cast<float>(log(static_cast<double>(ratio))) / p.log_scale;
+    if (isnan(lq)) return w;
+    const float c = ceilf(lq);
+    const int level = c < 0.f ? 0 : (c >= static_cast<float>(p.nlevels) ? p.nlevels - 1 : static_cast<int>(c));
+    // ORBmatcher::SearchByProjection(F, vpMapPoints, th)
+    float r = static_cast<double>(view_cos) > 0.998 ? 2.5f : 4.0f;
+    if (p.th != 1.0f) r *= p.th;
+    w = TrackWin{u, v, r * p.scale[level], u - p.mbf * invz, level - 1, level, 1, 0};
+    return w;
+  }
+  // SearchByProjection(CurrentFrame, LastFrame, th)
+  const float invzc = static_cast<float>(1.0 / static_cast<double>(pc[2]));
+  if (invzc < 0) return w;
+  const float u = p.fx * pc[0] * invzc + p.cx, v = p.fy * pc[1] * invzc + p.cy;
+  if (isnan(u) || isnan(v)) return w;
+  if (u < p.min_x || u > p.max_x || v < p.min_y || v > p.max_y) return w;
+  const int o = mp.octave;
+  if (o < 0 || o >= p.nlevels) return w;
+  const float radius = p.th * p.scale[o];
+  int lmin = o - 1, lmax = o + 1;
+  if (p.forward) { lmin = o; lmax = -1; }
+  else if (p.backward) { lmin = 0; lmax = o; }
+  w = TrackWin{u, v, radius, u - p.mbf * invzc, lmin, lmax, 1, 0};
+  return w;
+}
+
+__device__ __forceinline__ void load_desc(const sivo_map_point* mp, uint4& q0, uint4& q1) {
+  q0 = reinterpret_cast<const uint4*>(mp->desc)[0];
+  q1 = reinterpret_cast<const uint4*>(mp->desc)[1];
+}
+
+// ---- the unconstrained pass: one warp per point
+__global__ void __launch_bounds__(kProjectThreads) k_track_project(const TrackParams p, const long long* __restrict__ n_keep,
+                                                                   const sivo_map_point* __restrict__ pts, int n_points,
+                                                                   const uint8_t* __restrict__ blocked, TrackBufs b,
+                                                                   uint8_t* __restrict__ in_view) {
+  const int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (i >= n_points || *n_keep < 0) return;
+  const TrackWin w = project(p, pts[i]);
+  Best2 best;
+  if (w.in_view) {
+    uint4 q0, q1;
+    load_desc(pts + i, q0, q1);
+    best = search_window(p, b, w, q0, q1, blocked, lane);
+  }
+  if (lane == 0) {
+    b.win[i] = w;
+    b.fold[i] = best;
+    if (in_view) in_view[i] = static_cast<uint8_t>(w.in_view);
+  }
+}
+
+// ---- the ordered pass: one warp, the key state in dynamic shared memory (owner: cap ints, blocked: cap bytes)
+__global__ void __launch_bounds__(32) k_track_ordered(const TrackParams p, const long long* __restrict__ n_keep, int cap,
+                                                      const sivo_map_point* __restrict__ pts, int n_points,
+                                                      const uint8_t* __restrict__ blocked_in, TrackBufs b, int* __restrict__ match,
+                                                      long long* __restrict__ n_matches) {
+  extern __shared__ int owner[];
+  __shared__ int hist_count[kHisto];
+  uint8_t* blocked = reinterpret_cast<uint8_t*>(owner + cap);
+  const int lane = threadIdx.x;
+  const int n = clamp_count(n_keep, cap);
+  if (n < 0) {
+    if (lane == 0 && n_matches) *n_matches = -1;
+    return;
+  }
+  for (int j = lane; j < n; j += 32) {
+    owner[j] = -1;
+    blocked[j] = blocked_in ? blocked_in[j] : 0;
+  }
+  if (lane < kHisto) hist_count[lane] = 0;
+  __syncwarp();
+  int count = 0, n_hist = 0;
+  for (int base = 0; base < n_points; base += 32) {
+    const int mine = base + lane;
+    Best2 f;
+    int view = 0;
+    if (mine < n_points) {
+      f = b.fold[mine];
+      view = b.win[mine].in_view;
+    }
+    const int m = min(32, n_points - base);
+    for (int k = 0; k < m; ++k) {
+      if (!__shfl_sync(0xffffffffu, view, k)) continue;
+      const int i = base + k;
+      Best2 r;
+      r.idx = __shfl_sync(0xffffffffu, f.idx, k);
+      if (r.idx < 0) continue;  // no candidate at all; taking keys only removes candidates
+      r.idx2 = __shfl_sync(0xffffffffu, f.idx2, k);
+      if (blocked[r.idx] || (!p.last_frame && r.idx2 >= 0 && blocked[r.idx2])) {
+        uint4 q0, q1;
+        load_desc(pts + i, q0, q1);
+        r = search_window(p, b, b.win[i], q0, q1, blocked, lane);
+        if (r.idx < 0) continue;
+      } else {
+        r.dist = __shfl_sync(0xffffffffu, f.dist, k);
+        r.level = __shfl_sync(0xffffffffu, f.level, k);
+        r.dist2 = __shfl_sync(0xffffffffu, f.dist2, k);
+        r.level2 = __shfl_sync(0xffffffffu, f.level2, k);
+      }
+      if (r.dist > kThHigh) continue;
+      if (!p.last_frame && r.level == r.level2 && static_cast<float>(r.dist) > p.nnratio * static_cast<float>(r.dist2)) continue;
+      ++count;
+      const sivo_map_point& mp = pts[i];
+      if (lane == 0) {
+        owner[r.idx] = i;
+        if (mp.observed > 0) blocked[r.idx] = 1;
+      }
+      if (p.last_frame) {
+        float rot = mp.angle - b.angle[r.idx];
+        if (rot < 0.0f) rot += 360.0f;
+        int bin = static_cast<int>(roundf(rot * (1.0f / kHisto)));
+        if (bin == kHisto) bin = 0;
+        if (lane == 0) {
+          b.hist[n_hist] = r.idx | (bin << 24);
+          ++hist_count[bin];
+        }
+        ++n_hist;
+      }
+      __syncwarp();
+    }
+  }
+  if (p.last_frame) {
+    __syncwarp();
+    __shared__ int keep_bin[3];
+    if (lane == 0) {  // ComputeThreeMaxima (ORBmatcher.cc:1545-1577)
+      int max1 = 0, max2 = 0, max3 = 0, ind1 = -1, ind2 = -1, ind3 = -1;
+      for (int i = 0; i < kHisto; ++i) {
+        const int s = hist_count[i];
+        if (s > max1) { max3 = max2; max2 = max1; max1 = s; ind3 = ind2; ind2 = ind1; ind1 = i; }
+        else if (s > max2) { max3 = max2; max2 = s; ind3 = ind2; ind2 = i; }
+        else if (s > max3) { max3 = s; ind3 = i; }
+      }
+      if (max2 < 0.1f * static_cast<float>(max1)) { ind2 = -1; ind3 = -1; }
+      else if (max3 < 0.1f * static_cast<float>(max1)) ind3 = -1;
+      keep_bin[0] = ind1; keep_bin[1] = ind2; keep_bin[2] = ind3;
+    }
+    __syncwarp();
+    int culled = 0;
+    for (int e = lane; e < n_hist; e += 32) {
+      const int v = b.hist[e], bin = v >> 24;
+      if (bin != keep_bin[0] && bin != keep_bin[1] && bin != keep_bin[2]) {
+        owner[v & 0xFFFFFF] = -1;
+        ++culled;
+      }
+    }
+#pragma unroll
+    for (int o = 16; o; o >>= 1) culled += __shfl_xor_sync(0xffffffffu, culled, o);
+    count -= culled;
+    __syncwarp();
+  }
+  if (match)
+    for (int j = lane; j < n; j += 32) match[j] = owner[j];
+  if (lane == 0 && n_matches) *n_matches = count;
+}
+
+// test hook kernels: per-query list lengths, then the lists
+__global__ void k_area_lists(const TrackParams p, TrackBufs b, const float* __restrict__ xyr, const int* __restrict__ levels, int nq,
+                             const int* __restrict__ offsets, int* __restrict__ out) {
+  const int q = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (q >= nq) return;
+  int pos = offsets ? offsets[q] : 0;
+  walk_area(p, b, xyr[3 * q], xyr[3 * q + 1], xyr[3 * q + 2], levels[2 * q], levels[2 * q + 1], lane, [&](bool ok, int j, int) {
+    const unsigned m = __ballot_sync(0xffffffffu, ok);
+    if (ok && offsets) out[pos + __popc(m & ((1u << lane) - 1u))] = j;
+    pos += __popc(m);
+  });
+  if (!offsets && lane == 0) out[q] = pos;
+}
+
+TrackParams make_params(const Orb& left, const sivo_track_frame& f) {
+  if (!(f.max_x > f.min_x) || !(f.max_y > f.min_y)) fail(SIVO_EINVAL, "track: image bounds need max > min");
+  TrackParams p{};
+  p.fx = f.fx; p.fy = f.fy; p.cx = f.cx; p.cy = f.cy; p.mbf = f.mbf;
+  p.min_x = f.min_x; p.max_x = f.max_x; p.min_y = f.min_y; p.max_y = f.max_y;
+  p.w_inv = static_cast<float>(kCols) / (f.max_x - f.min_x);
+  p.h_inv = static_cast<float>(kRows) / (f.max_y - f.min_y);
+  for (int i = 0; i < 9; ++i) p.rcw[i] = f.Rcw[i];
+  for (int i = 0; i < 3; ++i) { p.tcw[i] = f.tcw[i]; p.ow[i] = f.Ow[i]; }
+  p.nlevels = left.nlevels();
+  for (int l = 0; l < p.nlevels; ++l) p.scale[l] = left.tables().scale[l];
+  p.log_scale = static_cast<float>(std::log(static_cast<double>(left.tables().scale.size() > 1 ? left.tables().scale[1] : 1.0f)));
+  return p;
+}
+
+// the forward / backward decision of the last-frame search (ORBmatcher.cc:1290-1301)
+void last_frame_direction(TrackParams& p, const sivo_track_frame& f, const float* Rlw, const float* tlw) {
+  float twc[3], tlc[3];
+  for (int r = 0; r < 3; ++r) {
+    double s = 0.0;
+    s = s + static_cast<double>(f.Rcw[r]) * f.tcw[0];
+    s = s + static_cast<double>(f.Rcw[3 + r]) * f.tcw[1];
+    s = s + static_cast<double>(f.Rcw[6 + r]) * f.tcw[2];
+    twc[r] = -static_cast<float>(s);
+  }
+  for (int r = 0; r < 3; ++r) tlc[r] = ((Rlw[3 * r] * twc[0] + Rlw[3 * r + 1] * twc[1]) + Rlw[3 * r + 2] * twc[2]) + tlw[r];
+  p.forward = tlc[2] > f.mb;
+  p.backward = -tlc[2] > f.mb;
+}
+
+size_t ordered_smem(int cap) { return static_cast<size_t>(std::max(cap, 1)) * (sizeof(int) + 1); }
+
+void launch_search(const TrackParams& p, const sivo_keypoint* kps, const uint8_t* desc, const int* keep_idx, const long long* n_keep,
+                   int cap, const float* u_right, const uint8_t* blocked, const sivo_map_point* pts, int n_points, const TrackBufs& b,
+                   uint8_t* in_view, int* match, long long* n_matches, cudaStream_t s) {
+  const size_t smem = ordered_smem(cap);
+  if (smem > 200 * 1024) fail(SIVO_EINVAL, "track: capacity %d exceeds the ordered pass's shared memory", cap);
+  SIVO_CUDA(cudaFuncSetAttribute(k_track_ordered, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+  k_track_grid<<<1, kGridThreads, 0, s>>>(p, kps, desc, keep_idx, n_keep, cap, u_right, b);
+  SIVO_CUDA(cudaGetLastError());
+  if (n_points > 0) {
+    k_track_project<<<ceil_div(n_points, kProjectThreads / 32), kProjectThreads, 0, s>>>(p, n_keep, pts, n_points, blocked, b, in_view);
+    SIVO_CUDA(cudaGetLastError());
+  }
+  k_track_ordered<<<1, 32, smem, s>>>(p, n_keep, cap, pts, n_points, blocked, b, match, n_matches);
+  SIVO_CUDA(cudaGetLastError());
+}
+
+void check_args(int n_points, float th, float nnratio) {
+  if (n_points < 0 || !(th > 0.f) || !std::isfinite(th) || !std::isfinite(nnratio)) fail(SIVO_EINVAL, "track: bad arguments");
+}
+
+// The host forms: stage the gathered keys and the points on the host-call workspace, run the device forms' kernels, download.
+void search_host(const Orb& left, bool last, const sivo_keypoint* kps, const uint8_t* desc, const float* u_right, const uint8_t* blocked,
+                 int n, const sivo_map_point* pts, int n_points, const sivo_track_frame& f, const float* Rlw, const float* tlw, float th,
+                 float nnratio, uint8_t* in_view, int* match, int* n_matches) {
+  if (n < 0) fail(SIVO_EINVAL, "track: n = %d", n);
+  check_args(n_points, th, nnratio);
+  TrackParams p = make_params(left, f);
+  p.th = th;
+  p.nnratio = nnratio;
+  p.last_frame = last;
+  if (last) {
+    last_frame_direction(p, f, Rlw, tlw);
+    for (int i = 0; i < n_points; ++i)
+      if (pts[i].octave < 0 || pts[i].octave >= p.nlevels) fail(SIVO_ERANGE, "track: point %d has octave %d", i, pts[i].octave);
+  }
+  StereoWs& ws = stereo_ws();
+  ws.begin(left.device(), pad256(n * sizeof(sivo_keypoint)) + pad256(static_cast<size_t>(n) * 32) + 2 * pad256(n * sizeof(float)) +
+                              pad256(n) + pad256(n_points * sizeof(sivo_map_point)) + pad256(n_points) + pad256(n * sizeof(int)) +
+                              2 * pad256(sizeof(long long)) + scratch_bytes(n, n_points) + 4096);
+  cudaStream_t st = ws.stream;
+  sivo_keypoint* d_kps = ws.take<sivo_keypoint>(n);
+  uint8_t* d_desc = ws.take<uint8_t>(static_cast<size_t>(n) * 32);
+  float* d_ur = ws.take<float>(n);
+  uint8_t* d_blocked = blocked ? ws.take<uint8_t>(n) : nullptr;
+  sivo_map_point* d_pts = ws.take<sivo_map_point>(n_points);
+  uint8_t* d_view = ws.take<uint8_t>(n_points);
+  int* d_match = ws.take<int>(n);
+  long long* d_count = ws.take<long long>(1);
+  long long* d_nm = ws.take<long long>(1);
+  const TrackBufs b = carve(ws.take<uint8_t>(scratch_bytes(n, n_points)), n, n_points);
+  const long long count = n;
+  if (n) {
+    SIVO_CUDA(cudaMemcpyAsync(d_kps, kps, n * sizeof(sivo_keypoint), cudaMemcpyHostToDevice, st));
+    SIVO_CUDA(cudaMemcpyAsync(d_desc, desc, static_cast<size_t>(n) * 32, cudaMemcpyHostToDevice, st));
+    SIVO_CUDA(cudaMemcpyAsync(d_ur, u_right, n * sizeof(float), cudaMemcpyHostToDevice, st));
+    if (blocked) SIVO_CUDA(cudaMemcpyAsync(d_blocked, blocked, n, cudaMemcpyHostToDevice, st));
+  }
+  if (n_points) SIVO_CUDA(cudaMemcpyAsync(d_pts, pts, n_points * sizeof(sivo_map_point), cudaMemcpyHostToDevice, st));
+  SIVO_CUDA(cudaMemcpyAsync(d_count, &count, sizeof(long long), cudaMemcpyHostToDevice, st));
+  launch_search(p, d_kps, d_desc, nullptr, d_count, n, d_ur, d_blocked, d_pts, n_points, b, d_view, d_match, d_nm, st);
+  long long nm = 0;
+  if (in_view && n_points) SIVO_CUDA(cudaMemcpyAsync(in_view, d_view, n_points, cudaMemcpyDeviceToHost, st));
+  if (match && n) SIVO_CUDA(cudaMemcpyAsync(match, d_match, n * sizeof(int), cudaMemcpyDeviceToHost, st));
+  SIVO_CUDA(cudaMemcpyAsync(&nm, d_nm, sizeof(long long), cudaMemcpyDeviceToHost, st));
+  SIVO_CUDA(cudaStreamSynchronize(st));
+  if (n_matches) *n_matches = static_cast<int>(nm);
+}
+
+void search_device(const Orb& left, bool last, const sivo_keypoint* kps, const uint8_t* desc, const int* keep_idx, const long long* n_keep,
+                   const float* u_right, const uint8_t* blocked, const sivo_map_point* pts, int n_points, const sivo_track_frame& f,
+                   const float* Rlw, const float* tlw, float th, float nnratio, uint8_t* in_view, int* match, long long* n_matches,
+                   cudaStream_t s) {
+  check_args(n_points, th, nnratio);
+  TrackParams p = make_params(left, f);
+  p.th = th;
+  p.nnratio = nnratio;
+  p.last_frame = last;
+  if (last) last_frame_direction(p, f, Rlw, tlw);
+  SIVO_CUDA(cudaSetDevice(left.device()));
+  if (!s) s = left.stream();
+  const int cap = left.capacity();
+  const TrackBufs b = carve(const_cast<Orb&>(left).track_scratch(scratch_bytes(cap, n_points), s), cap, n_points);
+  launch_search(p, kps, desc, keep_idx, n_keep, cap, u_right, blocked, pts, n_points, b, in_view, match, n_matches, s);
+}
+}  // namespace
+
+uint8_t* Orb::track_scratch(size_t bytes, cudaStream_t s) {
+  if (track_bytes_ < bytes) {
+    if (d_track_) SIVO_CUDA(cudaFreeAsync(d_track_, s));
+    d_track_ = nullptr;
+    track_bytes_ = 0;
+    SIVO_CUDA(cudaMallocAsync(&d_track_, bytes + bytes / 2, s));
+    track_bytes_ = bytes + bytes / 2;
+  }
+  return static_cast<uint8_t*>(d_track_);
+}
+
+void search_local_points(const Orb& left, const sivo_keypoint* kps, const uint8_t* desc, const float* u_right, const uint8_t* blocked, int n,
+                         const sivo_map_point* pts, int n_points, const sivo_track_frame& f, float th, float nnratio, uint8_t* in_view,
+                         int* match, int* n_matches) {
+  search_host(left, false, kps, desc, u_right, blocked, n, pts, n_points, f, nullptr, nullptr, th, nnratio, in_view, match, n_matches);
+}
+
+void search_last_frame(const Orb& left, const sivo_keypoint* kps, const uint8_t* desc, const float* u_right, int n, const sivo_map_point* pts,
+                       int n_points, const sivo_track_frame& f, const float* Rlw, const float* tlw, float th, int* match, int* n_matches) {
+  search_host(left, true, kps, desc, u_right, nullptr, n, pts, n_points, f, Rlw, tlw, th, 0.f, nullptr, match, n_matches);
+}
+
+void search_local_points_device(const Orb& left, const sivo_keypoint* kps, const uint8_t* desc, const int* keep_idx, const long long* n_keep,
+                                const float* u_right, const uint8_t* blocked, const sivo_map_point* pts, int n_points,
+                                const sivo_track_frame& f, float th, float nnratio, uint8_t* in_view, int* match, long long* n_matches,
+                                cudaStream_t s) {
+  search_device(left, false, kps, desc, keep_idx, n_keep, u_right, blocked, pts, n_points, f, nullptr, nullptr, th, nnratio, in_view, match,
+                n_matches, s);
+}
+
+void search_last_frame_device(const Orb& left, const sivo_keypoint* kps, const uint8_t* desc, const int* keep_idx, const long long* n_keep,
+                              const float* u_right, const sivo_map_point* pts, int n_points, const sivo_track_frame& f, const float* Rlw,
+                              const float* tlw, float th, int* match, long long* n_matches, cudaStream_t s) {
+  search_device(left, true, kps, desc, keep_idx, n_keep, u_right, nullptr, pts, n_points, f, Rlw, tlw, th, 0.f, nullptr, match, n_matches, s);
+}
+
+// GetFeaturesInArea on the device grid of n host keys: lengths, host scan, lists
+void features_in_area(const Orb& left, const sivo_keypoint* kps, int n, const sivo_track_frame& f, const float* xyr, const int* levels, int nq,
+                      int* offsets, int* idx, int idx_cap) {
+  if (n < 0 || nq < 0) fail(SIVO_EINVAL, "features_in_area: negative counts");
+  const TrackParams p = make_params(left, f);
+  StereoWs& ws = stereo_ws();
+  ws.begin(left.device(), pad256(n * sizeof(sivo_keypoint)) + pad256(static_cast<size_t>(n) * 32) + pad256(n * sizeof(float)) +
+                              pad256(sizeof(long long)) + pad256(3 * sizeof(float) * nq) + pad256(2 * sizeof(int) * nq) +
+                              pad256((nq + 1) * sizeof(int)) + pad256(std::max(idx_cap, 0) * sizeof(int)) + scratch_bytes(n, 0) + 4096);
+  cudaStream_t st = ws.stream;
+  sivo_keypoint* d_kps = ws.take<sivo_keypoint>(n);
+  uint8_t* d_desc = ws.take<uint8_t>(static_cast<size_t>(n) * 32);
+  float* d_ur = ws.take<float>(n);
+  long long* d_count = ws.take<long long>(1);
+  float* d_xyr = ws.take<float>(3 * static_cast<size_t>(nq));
+  int* d_lv = ws.take<int>(2 * static_cast<size_t>(nq));
+  int* d_off = ws.take<int>(nq + 1);
+  int* d_idx = ws.take<int>(std::max(idx_cap, 0));
+  const TrackBufs b = carve(ws.take<uint8_t>(scratch_bytes(n, 0)), n, 0);
+  const long long count = n;
+  if (n) {
+    SIVO_CUDA(cudaMemcpyAsync(d_kps, kps, n * sizeof(sivo_keypoint), cudaMemcpyHostToDevice, st));
+    SIVO_CUDA(cudaMemsetAsync(d_desc, 0, static_cast<size_t>(n) * 32, st));
+    SIVO_CUDA(cudaMemsetAsync(d_ur, 0, n * sizeof(float), st));
+  }
+  SIVO_CUDA(cudaMemcpyAsync(d_count, &count, sizeof(long long), cudaMemcpyHostToDevice, st));
+  if (nq) {
+    SIVO_CUDA(cudaMemcpyAsync(d_xyr, xyr, 3 * sizeof(float) * nq, cudaMemcpyHostToDevice, st));
+    SIVO_CUDA(cudaMemcpyAsync(d_lv, levels, 2 * sizeof(int) * nq, cudaMemcpyHostToDevice, st));
+  }
+  k_track_grid<<<1, kGridThreads, 0, st>>>(p, d_kps, d_desc, nullptr, d_count, n, d_ur, b);
+  SIVO_CUDA(cudaGetLastError());
+  std::vector<int> len(std::max(nq, 1));
+  if (nq) {
+    k_area_lists<<<ceil_div(nq * 32, 128), 128, 0, st>>>(p, b, d_xyr, d_lv, nq, nullptr, d_off);
+    SIVO_CUDA(cudaGetLastError());
+    SIVO_CUDA(cudaMemcpyAsync(len.data(), d_off, nq * sizeof(int), cudaMemcpyDeviceToHost, st));
+  }
+  SIVO_CUDA(cudaStreamSynchronize(st));
+  offsets[0] = 0;
+  for (int q = 0; q < nq; ++q) offsets[q + 1] = offsets[q] + len[q];
+  if (offsets[nq] > idx_cap) fail(SIVO_ERANGE, "features_in_area: %d candidates, room for %d", offsets[nq], idx_cap);
+  if (!offsets[nq]) return;
+  SIVO_CUDA(cudaMemcpyAsync(d_off, offsets, (nq + 1) * sizeof(int), cudaMemcpyHostToDevice, st));
+  k_area_lists<<<ceil_div(nq * 32, 128), 128, 0, st>>>(p, b, d_xyr, d_lv, nq, d_off, d_idx);
+  SIVO_CUDA(cudaGetLastError());
+  SIVO_CUDA(cudaMemcpyAsync(idx, d_idx, offsets[nq] * sizeof(int), cudaMemcpyDeviceToHost, st));
+  SIVO_CUDA(cudaStreamSynchronize(st));
+}
+
+}  // namespace sivo
