@@ -346,8 +346,14 @@ int sivo_dbg_info_terms(const sivo_orb_t* left, const sivo_keypoint* kps, const 
  *             30)), 30 -> 0 (so only bins 0..12 are used, as in the reference); ComputeThreeMaxima with its 0.1f * max1 rule; every
  *             entry of every other bin frees its key and decrements the count, duplicates included.
  *   NaN       a point whose u, v, viewCos or level quotient is NaN is not in view (the reference converts a NaN to int there).
+ *   angles    key angles (kp.angle, both searches) and last-frame point angles must be finite and in [0, 360] (-0.0 included),
+ *             which keeps rot in [0, 360] and every bin in 0..12 (the reference asserts 0 <= bin < 30, ORBmatcher.cc:1390).  The
+ *             host forms return SIVO_ERANGE for any other angle.  The device forms put a key with such an angle in no cell (as
+ *             a key index outside the capacity) and do not search a last-frame point with one.  Extractor keys satisfy the rule.
  * Map-point order and claims make the result sequential; the device walks the points in order in one block and re-searches only
- * the points whose best (or, local, second-best) key an earlier point took. */
+ * the points whose best (or, local, second-best) key an earlier point took.  tests/test_gpu_track_edges.py holds the device
+ * forms to oracle/track_oracle.py on constructed worst cases: crowded windows, exact ties, every decision boundary, long claim
+ * chains, the limits and a seeded differential fuzz. */
 typedef struct sivo_track_frame {          /* the current Frame's members */
   float fx, fy, cx, cy, mb, mbf;
   float min_x, max_x, min_y, max_y;        /* mnMinX, mnMaxX, mnMinY, mnMaxY (ComputeImageBounds) */
@@ -383,14 +389,16 @@ int sivo_search_local_points_device(const sivo_orb_t* left, const sivo_keypoint*
 /* SearchByProjection(CurrentFrame, LastFrame, th) (stereo) on device buffers, keys as above.  The points are the last frame's
  * non-NULL, non-outlier map points in key order, each with its key's octave and angle; no key is blocked on entry (Tracking
  * clears mvpMapPoints before both calls).  Rlw / tlw: the last frame's pose (host, row-major 3 x 3 and 3).  match_device /
- * n_matches_device as above.  A point whose octave is outside [0, nlevels) is never matched (the host form refuses it). */
+ * n_matches_device as above.  A point whose octave is outside [0, nlevels), or whose angle breaks the angle rule, is never
+ * matched (the host form refuses it). */
 int sivo_search_last_frame_device(const sivo_orb_t* left, const sivo_keypoint* kps_device, const uint8_t* desc_device,
                                   const int* keep_idx_device, const long long* n_keep_device, const float* u_right_device,
                                   const sivo_map_point* points_device, int n_points, const sivo_track_frame* frame, const float* Rlw,
                                   const float* tlw, float th, int* match_device, long long* n_matches_device, void* stream);
 /* Host forms: n keys gathered per semantic key (mvKeysSemantic, mDescriptorsSemantic n x 32, mvRight, blocked may be NULL), points
  * on the host; outputs in_view (n_points), match (n), *n_matches, any may be NULL.  They stage the inputs and run the device
- * forms' kernels, then synchronise.  SIVO_EINVAL as above and for n < 0; SIVO_ERANGE for a last-frame octave outside [0, nlevels). */
+ * forms' kernels, then synchronise.  SIVO_EINVAL as above and for n < 0; SIVO_ERANGE for a last-frame octave outside [0, nlevels)
+ * and for an angle that breaks the angle rule.  At most 40,960 keys (the ordered pass keeps 5 bytes per key in shared memory). */
 int sivo_search_local_points(const sivo_orb_t* left, const sivo_keypoint* kps, const uint8_t* desc, const float* u_right,
                              const uint8_t* blocked, int n, const sivo_map_point* points, int n_points, const sivo_track_frame* frame,
                              float th, float nnratio, uint8_t* in_view, int* match, int* n_matches);

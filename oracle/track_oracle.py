@@ -16,6 +16,9 @@ order the reference writes it (no fused multiply-add).  The rules the reference 
 - PredictScale's log is the float overload (MapPoint.cc sees `using namespace std` through DBoW2's TemplatedVocabulary.h); here the
   correctly rounded float logarithm, float32(log(float64(ratio))).  mfLogScaleFactor likewise.
 - A point whose u, v, viewCos or level quotient is NaN is not in view (the reference converts the NaN to int).
+- Angles: a key or last-frame point angle takes part only if it is finite and in [0, 360] (angle_ok).  A key with another angle
+  goes in no cell; a last-frame point with one is not searched.  Within the rule the rotation bin is in 0..12; the reference
+  asserts bin in [0, HISTO_LENGTH) (ORBmatcher.cc:1390) and has no rule for angles that would break it.
 """
 from __future__ import annotations
 
@@ -104,10 +107,17 @@ def pos_in_grid(x, y, f: Frame):
     return int(gx), int(gy)
 
 
+def angle_ok(a) -> bool:
+    """The angle rule: finite and in [0, 360] (-0.0 included)."""
+    return bool(F32(0) <= F32(a) <= F32(360))
+
+
 def assign_features_to_grid(kps, f: Frame):
-    """Frame::AssignFeaturesToGrid -> grid[ix][iy] = ascending key indices."""
+    """Frame::AssignFeaturesToGrid -> grid[ix][iy] = ascending key indices; a key breaking the angle rule goes in no cell."""
     grid = [[[] for _ in range(ROWS)] for _ in range(COLS)]
     for j in range(len(kps)):
+        if not angle_ok(kps["angle"][j]):
+            continue
         c = pos_in_grid(kps["x"][j], kps["y"][j], f)
         if c is not None:
             grid[c[0]][c[1]].append(j)
@@ -263,6 +273,9 @@ def compute_three_maxima(counts):
 
 
 def rotation_bin(angle_last, angle_cur) -> int:
+    """The histogram bin of a match; both angles must satisfy the angle rule (the bin is then in 0..12)."""
+    if not (angle_ok(angle_last) and angle_ok(angle_cur)):
+        raise ValueError(f"angle outside [0, 360]: {angle_last}, {angle_cur}")
     rot = F32(angle_last) - F32(angle_cur)
     if rot < F32(0):
         rot = rot + F32(360)
@@ -286,6 +299,8 @@ def search_last_frame(kps, desc, u_right, points, f: Frame, Rlw, tlw, scale, th)
     hist = [[] for _ in range(HISTO_LENGTH)]
     nmatches = 0
     for i, mp in enumerate(points):
+        if not angle_ok(mp["angle"]):
+            continue
         pc = gemm_pc(f.Rcw, mp["pos"], f.tcw)
         with np.errstate(all="ignore"):
             invzc = F32(F64(1.0) / F64(pc[2]))

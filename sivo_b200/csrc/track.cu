@@ -86,6 +86,11 @@ TrackBufs carve(uint8_t* base, int cap, int np) {
   return b;
 }
 
+// The angle rule: a key or point angle takes part only if it is finite and in [0, 360].  With both angles in range, rot is in
+// [0, 360] and the rotation bin in 0..12, inside hist_count; a NaN or infinite angle, or one off by more than 360, would index
+// outside it.
+__host__ __device__ __forceinline__ bool angle_ok(float a) { return a >= 0.f && a <= 360.f; }
+
 __device__ __forceinline__ int clamp_count(const long long* n_keep, int cap) {
   const long long n = *n_keep;
   return n < 0 ? -1 : static_cast<int>(min(n, static_cast<long long>(cap)));
@@ -115,9 +120,10 @@ __global__ void __launch_bounds__(kGridThreads, 1) k_track_grid(const TrackParam
       ang = kp.angle;
       d0 = reinterpret_cast<const uint4*>(desc + static_cast<size_t>(k) * 32)[0];
       d1 = reinterpret_cast<const uint4*>(desc + static_cast<size_t>(k) * 32)[1];
-      // PosInGrid: round half away from zero; the comparisons in float keep a NaN or huge coordinate out of the int conversion
+      // PosInGrid: round half away from zero; the comparisons in float keep a NaN or huge coordinate out of the int conversion.
+      // A key whose angle breaks the angle rule goes in no cell.
       const float gx = roundf((kp.x - p.min_x) * p.w_inv), gy = roundf((kp.y - p.min_y) * p.h_inv);
-      if (gx >= 0.f && gx < static_cast<float>(kCols) && gy >= 0.f && gy < static_cast<float>(kRows)) {
+      if (angle_ok(kp.angle) && gx >= 0.f && gx < static_cast<float>(kCols) && gy >= 0.f && gy < static_cast<float>(kRows)) {
         cell = static_cast<int>(gx) * kRows + static_cast<int>(gy);
         atomicAdd(&cnt[cell], 1);
       }
@@ -275,7 +281,7 @@ __device__ TrackWin project(const TrackParams& p, const sivo_map_point& mp) {
   if (isnan(u) || isnan(v)) return w;
   if (u < p.min_x || u > p.max_x || v < p.min_y || v > p.max_y) return w;
   const int o = mp.octave;
-  if (o < 0 || o >= p.nlevels) return w;
+  if (o < 0 || o >= p.nlevels || !angle_ok(mp.angle)) return w;
   const float radius = p.th * p.scale[o];
   int lmin = o - 1, lmax = o + 1;
   if (p.forward) { lmin = o; lmax = -1; }
@@ -490,10 +496,14 @@ void search_host(const Orb& left, bool last, const sivo_keypoint* kps, const uin
   p.th = th;
   p.nnratio = nnratio;
   p.last_frame = last;
+  for (int j = 0; j < n; ++j)
+    if (!angle_ok(kps[j].angle)) fail(SIVO_ERANGE, "track: key %d has angle %g outside [0, 360]", j, kps[j].angle);
   if (last) {
     last_frame_direction(p, f, Rlw, tlw);
-    for (int i = 0; i < n_points; ++i)
+    for (int i = 0; i < n_points; ++i) {
       if (pts[i].octave < 0 || pts[i].octave >= p.nlevels) fail(SIVO_ERANGE, "track: point %d has octave %d", i, pts[i].octave);
+      if (!angle_ok(pts[i].angle)) fail(SIVO_ERANGE, "track: point %d has angle %g outside [0, 360]", i, pts[i].angle);
+    }
   }
   StereoWs& ws = stereo_ws();
   ws.begin(left.device(), pad256(n * sizeof(sivo_keypoint)) + pad256(static_cast<size_t>(n) * 32) + 2 * pad256(n * sizeof(float)) +

@@ -1,10 +1,15 @@
 """Compiles the unmodified C++ shim (integration/src/*.cpp) + tests/cpp/test_shim.cpp with g++ against integration/stubs
-(minimal OpenCV / Eigen look-alikes; the image has neither) and links it to libsivo_b200.so."""
+(minimal OpenCV / Eigen look-alikes; the image has neither) and links it to libsivo_b200.so.  The binaries go to a per-user
+directory under the system's temporary directory, keyed by the checkout's path, so the suite writes nothing into the tree
+(which may be read-only)."""
+import hashlib
 import os
 import subprocess
+import tempfile
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-BIN = os.path.join(ROOT, "tests", "cpp", "build", "test_shim")
+BUILD_DIR = os.path.join(tempfile.gettempdir(), f"sivo_b200_shim_{os.getuid()}_{hashlib.sha1(ROOT.encode()).hexdigest()[:12]}")
+BIN = os.path.join(BUILD_DIR, "test_shim")
 SOURCES = [os.path.join(ROOT, "integration", "src", "bayesian_segnet.cpp"), os.path.join(ROOT, "integration", "src", "ORBextractor.cc"),
            os.path.join(ROOT, "tests", "cpp", "test_shim.cpp")]
 

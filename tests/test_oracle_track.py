@@ -175,6 +175,53 @@ def test_rotation_bins_use_only_0_to_12():
     assert T.rotation_bin(0.0, 15.0) == 12 and T.rotation_bin(0.0, 0.0) == 0 and T.rotation_bin(15.0, 0.0) == 1
 
 
+BAD_ANGLES = (np.nan, np.inf, -np.inf, -400.0, 720.0, np.nextafter(np.float32(360), np.float32(400)), -np.float32(1e-45))
+GOOD_ANGLES = (-0.0, 0.0, 360.0, 359.99997, 1e-45)
+
+
+def test_angle_rule_keeps_every_rotation_bin_in_0_to_12():
+    for a in BAD_ANGLES:
+        assert not T.angle_ok(a), a
+        for args in ((a, 0.0), (0.0, a), (a, a)):
+            try:
+                T.rotation_bin(*args)
+            except ValueError:
+                continue
+            raise AssertionError(args)
+    for a in GOOD_ANGLES:
+        assert T.angle_ok(a), a
+        for b in GOOD_ANGLES:
+            assert 0 <= T.rotation_bin(a, b) <= 12, (a, b)
+    assert T.rotation_bin(-0.0, 0.0) == 0 and T.rotation_bin(0.0, -0.0) == 0
+    assert T.rotation_bin(360.0, 0.0) == 12 and T.rotation_bin(0.0, 360.0) == 0 and T.rotation_bin(360.0, 360.0) == 0
+
+
+def test_angle_rule_drops_keys_and_last_frame_points():
+    f = frame()
+    n = 2 * len(BAD_ANGLES) + len(GOOD_ANGLES)
+    angles = list(BAD_ANGLES) + list(GOOD_ANGLES) + list(BAD_ANGLES)
+    k = keys([(100 + 20 * i, 100) for i in range(n)], 0)
+    k["angle"] = angles
+    d = np.stack([desc_with([i]) for i in range(n)])
+    ur = np.full(n, -1, np.float32)
+    grid = T.assign_features_to_grid(k, f)
+    placed = sorted(j for col in grid for cell in col for j in cell)
+    assert placed == [j for j in range(n) if T.angle_ok(angles[j])]
+    # a key breaking the rule is no candidate of either search
+    pts = [point_at(f, 100 + 20 * i, 100, 10, desc_with([i]), angle=0.0) for i in range(n)]
+    view, match, nm = local(pts, k, d)
+    assert view.all() and nm == len(GOOD_ANGLES) and list(np.flatnonzero(match >= 0)) == placed
+    match, nm = T.search_last_frame(k, d, ur, np.array(pts, MP), f, np.eye(3), np.zeros(3), SCALE, 7)
+    assert nm == len(GOOD_ANGLES) and list(np.flatnonzero(match >= 0)) == placed
+    # a last-frame point breaking the rule is not searched; -0.0 and 360 are (bins 0 and 12, both kept)
+    k["angle"] = 0.0
+    for i, p in enumerate(pts):
+        p["angle"] = angles[i]
+    match, nm = T.search_last_frame(k, d, ur, np.array(pts, MP), f, np.eye(3), np.zeros(3), SCALE, 7)
+    good = [i for i in range(n) if T.angle_ok(angles[i])]
+    assert nm == len(good) and list(np.flatnonzero(match >= 0)) == good and [int(match[i]) for i in good] == good
+
+
 def test_last_frame_histogram_culls_every_entry_of_a_losing_bin():
     f = frame()
     n = 40

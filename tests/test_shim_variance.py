@@ -8,10 +8,11 @@ import numpy as np
 import pytest
 
 from conftest import make_model
+from shim_build import BUILD_DIR
 from test_shim import write_bin
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-BIN = os.path.join(ROOT, "tests", "cpp", "build", "test_shim_variance")
+BIN = os.path.join(BUILD_DIR, "test_shim_variance")  # outside the tree, as tests/shim_build.py builds
 SOURCES = [os.path.join(ROOT, "integration", "src", "bayesian_segnet.cpp"), os.path.join(ROOT, "tests", "cpp", "test_shim_variance.cpp")]
 
 
