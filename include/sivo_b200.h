@@ -411,6 +411,71 @@ int sivo_search_last_frame(const sivo_orb_t* left, const sivo_keypoint* kps, con
 int sivo_dbg_features_in_area(const sivo_orb_t* left, const sivo_keypoint* kps, int n, float min_x, float max_x, float min_y,
                               float max_y, const float* xyr, const int* levels, int n_query, int* offsets, int* idx, int idx_cap);
 
+/* ---- the frame pose: Optimizer::PoseOptimization (Optimizer.cc:273-491) with g2o's Levenberg-Marquardt, and the pose's
+ * marginal covariance (computeMarginals, :480-487), as Tracking runs it after each projection search ----------------------------
+ * Every operation is the IEEE float / double operation as written (no contracted multiply-add).  oracle/pose_oracle.py restates
+ * the rules and the reference facts kept (its header lists them with their g2o sources); in short:
+ *   edges     one per semantic key j with a map point (xw[3 j] not NaN), in key order; stereo iff u_right[j] >= 0 is not false
+ *             (mvRight < 0: mono).  Omega = I * mvInvLevelSigma2[octave] (the left extractor's table), Huber deltas sqrt(5.991f)
+ *             and sqrt(7.815f) in float.  Mono u = (x / z) fx + cx in double; stereo invz = (float)(1.0 / z), u = ((x invz) fx) +
+ *             cx, ur = u - mbf invz.  Jacobians as g2o's linearizeOplus, update [omega, upsilon]; robust weighting rho1 Omega only.
+ *   LM        tau 1e-5, lambda re-initialised per optimize(); <= 10 trials after a failure; scale = x . (lambda x + b) + 1e-3;
+ *             Terminate on qmax == 10, rho == 0 or a non-finite lambda; a failed factorisation sets tempChi = DBL_MAX and keeps
+ *             the last solved x (zeros before the first).  oplus = SE3Quat::exp(delta) * T with its theta < 1e-5 branch.
+ *   rounds    4 rounds of 10 iterations, each from the INPUT pose; only stereo edges are classified (outlier iff (float) chi2 >
+ *             7.815f), an inlier with the chi2 the last error pass left (possibly a rejected trial's), an outlier recomputed at
+ *             the round's estimate; stereo kernels removed after round 2; stop after a round when there are < 10 edges.  Below
+ *             3 edges: n_good = 0, the pose untouched.
+ *   result    Tcw = the quaternion's toRotationMatrix and t rounded to float; Ow = -Rcw^T tcw as Frame::UpdatePoseMatrices;
+ *             sigma_cw = the inverse of the last linearisation's H (LL^T in natural order, then MarginalCovarianceCholesky's
+ *             recursion), sigma_valid = 0 (sigma_cw zeros: keep the prior) when a pivot is not > 0 or the last round had no
+ *             inlier edge.  n_good = n_initial - n_bad of the last round run.
+ *   NaN rule  an edge is valid at a pose iff its chi2 and 1 / z^2 are finite; an invalid edge adds nothing to H, b or chi2 and
+ *             is an outlier when classified.
+ *   order     sums over edges run in a fixed tree: thread t of 256 sums edges t, t + 256, ...; xor shuffles 16 .. 1 in each warp;
+ *             the 8 warp totals folded by halves.  The reference sums in key order; the two agree to rounding.
+ * Not pinned to the reference (not buildable here): CHOLMOD's ordering, Eigen's operation orders, sin / cos / pow. */
+typedef struct sivo_pose_result {
+  float Tcw[12];                           /* 3 x 4 row-major [Rcw | tcw]: the next call's Tcw_in */
+  double q[4], t[3];                       /* the SE3Quat: quaternion (x, y, z, w) and translation */
+  float Rcw[9], tcw[3], Rwc[9], Ow[3];     /* sivo_track_frame's Rcw / tcw / Ow, sivo_info_camera's Rwc / Ow */
+  double sigma_cw[36];                     /* mSigmacw, row-major 6 x 6 [omega, upsilon] (sivo_info_camera.sigma_cw) */
+  int32_t sigma_valid, n_initial, n_bad, n_good, rounds_run, reserved;  /* n_good: PoseOptimization's return */
+} sivo_pose_result;
+
+/* PoseOptimization on device buffers.  Semantic key j < *n_keep_device is extractor key keep_idx_device[j] (j when NULL) of
+ * kps_device; u_right_device[j] is its mvRight, xw_device[3 j ..] its map point's world position (NaN x: no map point, e.g.
+ * filled by sivo_pose_gather_device).  Tcw_in_device: 12 floats, the frame's 3 x 4 pose (a sivo_pose_result's Tcw may be
+ * passed, that of result_device itself included: the pose is read before the result is written).  Writes *result_device and
+ * outlier_device[j] for j < the count (u8, sivo_orb_capacity(left) room; may be NULL): 0 for a key without a map point, where
+ * the reference leaves mvbOutlier as the caller had it, so the buffer is the call's whole output.  A key index outside the capacity, or a key with an octave outside the extractor's levels, has no edge.  The count is
+ * clamped to the capacity; a negative count (the -1 of sivo_segnet_semantic_keys_device) writes only result_device->n_good =
+ * -1.  One block runs the whole optimisation.  Runs on `stream` (NULL = the left extractor's stream) with no waits of its own
+ * and no host synchronisation; the edges live in the left extractor's projection-search scratch, so calls sharing it (both
+ * searches included) must be ordered among themselves and before its next sivo_orb_enqueue_device.  SIVO_EINVAL for NULL
+ * handles or inputs, or fx, fy, mbf not finite and positive, cx, cy not finite. */
+int sivo_pose_optimize_device(const sivo_orb_t* left, const sivo_keypoint* kps_device, const int* keep_idx_device,
+                              const long long* n_keep_device, const float* u_right_device, const float* xw_device, float fx, float fy,
+                              float cx, float cy, float mbf, const float* Tcw_in_device, sivo_pose_result* result_device,
+                              uint8_t* outlier_device, void* stream);
+/* For semantic keys j < *n_keep_device: if 0 <= match_device[j] < n_points, xw_device[3 j ..] = points_device[match[j]].pos; other
+ * entries are left alone, so matches of several searches merge into one array (as mvpMapPoints).  Same stream and ordering
+ * rules; SIVO_EINVAL for NULL handles or buffers or n_points < 0. */
+int sivo_pose_gather_device(const sivo_orb_t* left, const int* match_device, const long long* n_keep_device,
+                            const sivo_map_point* points_device, int n_points, float* xw_device, void* stream);
+/* Host form: n keys gathered per semantic key (mvKeysSemantic, mvRight, xw), the pose as 12 host floats; result and outlier (n)
+ * on the host.  It stages the inputs, runs the device form's kernel and synchronises.  SIVO_EINVAL as above and for n < 0;
+ * SIVO_ERANGE for a key with a point whose octave is outside the extractor's levels. */
+int sivo_pose_optimize(const sivo_orb_t* left, const sivo_keypoint* kps, const float* u_right, const float* xw, int n, float fx,
+                       float fy, float cx, float cy, float mbf, const float* Tcw_in, sivo_pose_result* result, uint8_t* outlier);
+/* Test hook: one linearisation pass of the kernel at pose7 = (qx, qy, qz, qw, tx, ty, tz) over the host keys' edges, with the
+ * stereo kernels on iff robust_stereo, edges j with level1[j] != 0 left out of the sums (level1 may be NULL).  Per key (NaN for a
+ * key without an edge): err[3 j ..], chi2[j], rho[2 j ..] = (rho0, rho1), jac[18 j ..] (3 x 6 row-major; a mono edge's third row
+ * zero).  H (36, row-major), b (6) and *chi (the robust chi2) as the kernel's reduction produces them.  Any output may be NULL. */
+int sivo_dbg_pose_system(const sivo_orb_t* left, const sivo_keypoint* kps, const float* u_right, const float* xw, int n, float fx,
+                         float fy, float cx, float cy, float mbf, const double* pose7, int robust_stereo, const uint8_t* level1,
+                         double* err, double* chi2, double* rho, double* jac, double* H, double* b, double* chi);
+
 /* Best / second-best match over per-query candidate lists -- the inner loop of ORBmatcher::SearchByProjection
  * (ORBmatcher.cc:79-113), its last-frame / keyframe variants (:1278-, :1420-), SearchForTriangulation (:631-) and
  * SearchBySim3 (next row 4).  Query i's candidates are cand_idx[cand_offsets[i] .. cand_offsets[i+1]) (indices into the

@@ -5,3 +5,4 @@ from .orb import ORBextractor, distribute_octtree, stereo_hamming, stereo_match,
 from .info import InfoCamera, info_select, info_select_device, make_camera  # noqa: F401
 from .track import (MAP_POINT_DTYPE, TrackFrame, make_frame, map_points, search_last_frame, search_last_frame_device,  # noqa: F401
                     search_local_points, search_local_points_device)
+from .pose import PoseResult, pose_gather_device, pose_optimize, pose_optimize_device  # noqa: F401

@@ -73,6 +73,10 @@ def lib() -> C.CDLL:
         _lib.sivo_search_local_points.argtypes = [vp, vp, vp, vp, vp, i32, vp, i32, vp, f32, f32, vp, vp, vp]
         _lib.sivo_search_last_frame.argtypes = [vp, vp, vp, vp, i32, vp, i32, vp, vp, vp, f32, vp, vp]
         _lib.sivo_dbg_features_in_area.argtypes = [vp, vp, i32, f32, f32, f32, f32, vp, vp, i32, vp, vp, i32]
+        _lib.sivo_pose_optimize_device.argtypes = [vp, vp, vp, vp, vp, vp, f32, f32, f32, f32, f32, vp, vp, vp, vp]
+        _lib.sivo_pose_gather_device.argtypes = [vp, vp, vp, vp, i32, vp, vp]
+        _lib.sivo_pose_optimize.argtypes = [vp, vp, vp, vp, i32, f32, f32, f32, f32, f32, vp, vp, vp]
+        _lib.sivo_dbg_pose_system.argtypes = [vp, vp, vp, vp, i32, f32, f32, f32, f32, f32, vp, i32, vp, vp, vp, vp, vp, vp, vp, vp]
         _lib.sivo_dbg_conv_unpooled.argtypes = [i32, vp, vp, i32, i32, i32, i32, vp, vp, vp, vp, i32, i32, vp]
     return _lib
 

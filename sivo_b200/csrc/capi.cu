@@ -44,6 +44,16 @@ void search_last_frame_device(const Orb& left, const sivo_keypoint* kps, const u
                               const float* tlw, float th, int* match, long long* n_matches, cudaStream_t s);
 void features_in_area(const Orb& left, const sivo_keypoint* kps, int n, const sivo_track_frame& f, const float* xyr, const int* levels, int nq,
                       int* offsets, int* idx, int idx_cap);
+void pose_optimize_device(const Orb& left, const sivo_keypoint* kps, const int* keep_idx, const long long* n_keep, const float* u_right,
+                          const float* xw, float fx, float fy, float cx, float cy, float mbf, const float* Tcw_in,
+                          sivo_pose_result* result, uint8_t* outlier, cudaStream_t s);
+void pose_gather_device(const Orb& left, const int* match, const long long* n_keep, const sivo_map_point* pts, int n_points, float* xw,
+                        cudaStream_t s);
+void pose_optimize(const Orb& left, const sivo_keypoint* kps, const float* u_right, const float* xw, int n, float fx, float fy, float cx,
+                   float cy, float mbf, const float* Tcw_in, sivo_pose_result* result, uint8_t* outlier);
+void pose_system(const Orb& left, const sivo_keypoint* kps, const float* u_right, const float* xw, int n, float fx, float fy, float cx,
+                 float cy, float mbf, const double* pose7, int robust_stereo, const uint8_t* level1, double* err, double* chi2, double* rho,
+                 double* jac, double* H, double* b, double* chi);
 }  // namespace sivo
 
 using namespace sivo;
@@ -580,6 +590,45 @@ int sivo_dbg_features_in_area(const sivo_orb_t* left, const sivo_keypoint* kps, 
     sivo_track_frame f{};
     f.min_x = min_x; f.max_x = max_x; f.min_y = min_y; f.max_y = max_y;
     features_in_area(*left->impl, kps, n, f, xyr, levels, n_query, offsets, idx, idx_cap);
+  });
+}
+
+// ---------------------------------------------------------------------------------------- frame pose
+int sivo_pose_optimize_device(const sivo_orb_t* left, const sivo_keypoint* kps_device, const int* keep_idx_device,
+                              const long long* n_keep_device, const float* u_right_device, const float* xw_device, float fx, float fy,
+                              float cx, float cy, float mbf, const float* Tcw_in_device, sivo_pose_result* result_device,
+                              uint8_t* outlier_device, void* stream) {
+  return guarded([&] {
+    if (!left || !kps_device || !n_keep_device || !u_right_device || !xw_device || !Tcw_in_device || !result_device)
+      fail(SIVO_EINVAL, "pose_optimize: null argument");
+    pose_optimize_device(*left->impl, kps_device, keep_idx_device, n_keep_device, u_right_device, xw_device, fx, fy, cx, cy, mbf,
+                         Tcw_in_device, result_device, outlier_device, static_cast<cudaStream_t>(stream));
+  });
+}
+
+int sivo_pose_gather_device(const sivo_orb_t* left, const int* match_device, const long long* n_keep_device,
+                            const sivo_map_point* points_device, int n_points, float* xw_device, void* stream) {
+  return guarded([&] {
+    if (!left || !match_device || !n_keep_device || !xw_device || (n_points > 0 && !points_device))
+      fail(SIVO_EINVAL, "pose_gather: null argument");
+    pose_gather_device(*left->impl, match_device, n_keep_device, points_device, n_points, xw_device, static_cast<cudaStream_t>(stream));
+  });
+}
+
+int sivo_pose_optimize(const sivo_orb_t* left, const sivo_keypoint* kps, const float* u_right, const float* xw, int n, float fx,
+                       float fy, float cx, float cy, float mbf, const float* Tcw_in, sivo_pose_result* result, uint8_t* outlier) {
+  return guarded([&] {
+    if (!left || !Tcw_in || !result || n < 0 || (n && (!kps || !u_right || !xw))) fail(SIVO_EINVAL, "pose_optimize: null argument or n < 0");
+    pose_optimize(*left->impl, kps, u_right, xw, n, fx, fy, cx, cy, mbf, Tcw_in, result, outlier);
+  });
+}
+
+int sivo_dbg_pose_system(const sivo_orb_t* left, const sivo_keypoint* kps, const float* u_right, const float* xw, int n, float fx,
+                         float fy, float cx, float cy, float mbf, const double* pose7, int robust_stereo, const uint8_t* level1,
+                         double* err, double* chi2, double* rho, double* jac, double* H, double* b, double* chi) {
+  return guarded([&] {
+    if (!left || !pose7 || n < 0 || (n && (!kps || !u_right || !xw))) fail(SIVO_EINVAL, "pose_system: null argument or n < 0");
+    pose_system(*left->impl, kps, u_right, xw, n, fx, fy, cx, cy, mbf, pose7, robust_stereo, level1, err, chi2, rho, jac, H, b, chi);
   });
 }
 

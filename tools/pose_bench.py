@@ -1,0 +1,273 @@
+#!/usr/bin/env python
+"""Frame-pose benchmark: Optimizer::PoseOptimization on the device (sivo_pose_optimize_device).  Prints one JSON line
+{"metric": "pose optimisation", ...}.
+
+  python tools/pose_bench.py [--steps 30] [--warmup 5] [--blocks-of 10]
+
+Reports:
+  (a) device_call_ms: the device call at 100 / 500 / 1000 / 2000 edges with 0 / 30 % gross outliers, CUDA events around the call,
+      median / p90 over --steps calls.  The scenes are synthetic (keys at random pixels and depths seen from a known pose, 0.5 px
+      noise times the octave's scale, about 60 % stereo, the initial pose moved by up to 0.01 rad / 5 cm), because a 1024x352 frame
+      holds fewer semantic keys with depth than the larger counts;
+  (b) host_call_ms: the host form on the same scenes, end to end (host wall time);
+  (c) frames/s of Tracking's device chain SegNet (Basic T=6) + ORB(2000) x2 + semantic keys + stereo + last-frame search +
+      local-map search, without and with the two optimisations appended the way Tracking runs them: last-frame search -> gather
+      -> pose -> the host reads the 512-byte result -> local-map search at that pose -> gather -> pose.  The host read makes
+      every frame of the "with" leg wait for its own first optimisation.  Synthetic 1024x352 frames; each frame's map points are
+      its own semantic keys with depth unprojected at a known pose (half as last-frame points, half as the local map, one in eight
+      moved by 0.5-2 m), found by a first pass of the front end.  The two legs alternate in blocks.
+The g2o host loop the kernel replaces (Eigen + CHOLMOD) is not built here: not measured.  Writes nothing into the source tree."""
+import argparse
+import gc
+import json
+import os
+import sys
+import time
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tools"))
+
+from bench import CROP_X, CROP_Y, NET_H, NET_W, frames, model_cache_dir, model_files  # noqa: E402
+
+FX, CX, CY, MBF = 718.856, 607.1928 - CROP_X, 185.2157 - CROP_Y, 386.1448  # KITTI00-02.yaml, principal point in the crop
+MB = MBF / FX
+EDGES = (100, 500, 1000, 2000)
+
+
+def rotation(ax, ay, az):
+    cx, sx, cy, sy, cz, sz = np.cos(ax), np.sin(ax), np.cos(ay), np.sin(ay), np.cos(az), np.sin(az)
+    return (np.array([[cz, -sz, 0], [sz, cz, 0], [0, 0, 1]]) @ np.array([[cy, 0, sy], [0, 1, 0], [-sy, 0, cy]])
+            @ np.array([[1, 0, 0], [0, cx, -sx], [0, sx, cx]]))
+
+
+def synthetic_scene(n, outliers, rng):
+    """Keys seen from a true pose, their points, u_right (< 0: mono) and the moved initial pose (3 x 4 float)."""
+    from sivo_b200 import KP_DTYPE
+    R, t = rotation(*rng.uniform(-0.2, 0.2, 3)), rng.uniform(-2, 2, 3)
+    u, v, z = rng.uniform(0, NET_W, n), rng.uniform(0, NET_H, n), rng.uniform(3, 40, n)
+    X = ((np.stack([(u - CX) * z / FX, (v - CY) * z / FX, z], 1) - t) @ R).astype(np.float32)
+    octave = rng.integers(0, 8, n)
+    sc = 1.2 ** octave
+    kps = np.zeros(n, KP_DTYPE)
+    kps["x"], kps["y"], kps["octave"] = u + 0.5 * sc * rng.standard_normal(n), v + 0.5 * sc * rng.standard_normal(n), octave
+    ur = np.where(rng.uniform(size=n) < 0.6, np.maximum(u - MBF / z + 0.5 * sc * rng.standard_normal(n), 0), -1).astype(np.float32)
+    bad = rng.permutation(n)[:int(round(outliers * n))]
+    X[bad] += rng.uniform(-5, 5, (len(bad), 3)).astype(np.float32)
+    Tin = np.concatenate([rotation(*rng.uniform(-0.01, 0.01, 3)) @ R, (t + rng.uniform(-0.05, 0.05, 3))[:, None]], 1)
+    return kps, ur, X, Tin.astype(np.float32)
+
+
+def frame_map(kps, desc, depth, scale, rng):
+    """Last-frame points and local-map points made from a frame's keys with depth at the identity pose."""
+    from oracle.track_oracle import map_points_from_keys
+    from sivo_b200 import map_points
+    f, idx = map_points_from_keys(kps, depth, np.eye(3), np.zeros(3), FX, FX, CX, CY, scale)
+    pts = map_points(desc[idx], f["pos"], f["normal"], f["min_distance"], f["max_distance"], 1, kps["octave"][idx], kps["angle"][idx])
+    bad = rng.uniform(size=len(pts)) < 0.125
+    pts["pos"][bad] += (rng.uniform(0.5, 2.0, (bad.sum(), 3)) * rng.choice([-1, 1], (bad.sum(), 3))).astype(np.float32)
+    return pts[0::2].copy(), pts[1::2].copy()
+
+
+def run(args):
+    import torch
+    from sivo_b200 import (BayesianSegNet, BayesianSegNetParams, KP_DTYPE, ORBextractor, make_frame, pose_gather_device, pose_optimize,
+                           pose_optimize_device, search_last_frame_device, search_local_points_device, stereo_match_device)
+    from sivo_b200.pose import frame_from_result, result_from_bytes
+    if not torch.cuda.is_available():
+        raise SystemExit("pose_bench.py needs a CUDA device (there is no CPU fallback for the product path)")
+    dev = torch.device("cuda", 0)
+    el, er = (ORBextractor(args.nfeatures, 1.2, 8, 20, 7) for _ in range(2))
+    cap = el.capacity()
+    u8, i32, i64, f32, f64 = torch.uint8, torch.int32, torch.int64, torch.float32, torch.float64
+    stream = torch.cuda.Stream(dev)
+    s = stream.cuda_stream
+    med = lambda v: float(np.median(v))
+    p90 = lambda v: float(np.percentile(v, 90))
+    rng = np.random.default_rng(0)
+
+    # (a) / (b)
+    kp_buf = torch.zeros(cap * 28, dtype=u8, device=dev)
+    n_buf = torch.zeros(1, dtype=i64, device=dev)
+    ur_buf = torch.zeros(cap, dtype=f32, device=dev)
+    xw_buf = torch.full((3 * cap,), float("nan"), dtype=f32, device=dev)
+    t_buf = torch.zeros(12, dtype=f32, device=dev)
+    res_buf = torch.zeros(512, dtype=u8, device=dev)
+    out_buf = torch.zeros(cap, dtype=u8, device=dev)
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    calls = {}
+    for n in EDGES:
+        for frac in (0.0, 0.3):
+            kps, ur, X, Tin = synthetic_scene(min(n, cap), frac, rng)
+            slots = np.zeros(cap, KP_DTYPE)
+            slots[:len(kps)] = kps
+            kp_buf.copy_(torch.from_numpy(slots.view(np.uint8).reshape(-1).copy()))
+            n_buf.fill_(len(kps))
+            ur_buf[:len(kps)].copy_(torch.from_numpy(ur))
+            xw_buf[:3 * len(kps)].copy_(torch.from_numpy(X.reshape(-1)))
+            t_buf.copy_(torch.from_numpy(Tin.reshape(-1)))
+            torch.cuda.synchronize(dev)
+            dev_ms, host_ms = [], []
+            gc.collect()
+            gc.disable()
+            for i in range(args.warmup + args.steps):
+                e0.record(stream)
+                pose_optimize_device(el, kp_buf.data_ptr(), 0, n_buf.data_ptr(), ur_buf.data_ptr(), xw_buf.data_ptr(), FX, FX, CX, CY, MBF,
+                                     t_buf.data_ptr(), res_buf.data_ptr(), out_buf.data_ptr(), s)
+                e1.record(stream)
+                e1.synchronize()
+                t0 = time.perf_counter()
+                hres, _ = pose_optimize(el, kps, ur, X, Tin, FX, FX, CX, CY, MBF)
+                t1 = time.perf_counter()
+                if i >= args.warmup:
+                    dev_ms.append(e0.elapsed_time(e1))
+                    host_ms.append(1e3 * (t1 - t0))
+            gc.enable()
+            dres = result_from_bytes(res_buf.cpu().numpy())
+            calls[f"{n}_edges_{int(frac * 100)}pct_outliers"] = {
+                "device_call_ms": {"median": med(dev_ms), "p90": p90(dev_ms)}, "host_call_ms": {"median": med(host_ms), "p90": p90(host_ms)},
+                "n_good": int(dres.n_good), "device_equals_host": bytes(dres) == bytes(hres)}
+
+    # (c) the chain
+    T = 6
+    _, proto, model, _ = model_files("basic", T, model_cache_dir())
+    seg = BayesianSegNet(BayesianSegNetParams(proto, model), seed=1234, T=T)
+    bounds = (0.0, float(NET_W), 0.0, float(NET_H))
+    frame0 = make_frame(FX, FX, CX, CY, MBF, bounds, rotation(0.001, -0.0015, 0.001), (0.01, -0.005, 0.01))
+    T0 = np.concatenate([np.array(frame0.Rcw, np.float32).reshape(3, 3), np.array(frame0.tcw, np.float32)[:, None]], 1)
+    fr = frames(6)
+    hw = NET_H * NET_W
+    d_cls, d_conf, d_ent = (torch.empty(hw, dtype=t, device=dev) for t in (u8, f64, f64))
+    B = []
+    for f in fr:
+        B.append({"in": [torch.from_numpy(np.ascontiguousarray(f[0][CROP_Y:CROP_Y + NET_H, CROP_X:CROP_X + NET_W])).to(dev), torch.from_numpy(f[1]).to(dev),
+                         torch.from_numpy(f[2]).to(dev)],
+                  "kp": [torch.zeros(cap * 28, dtype=u8, device=dev) for _ in range(2)],
+                  "desc": [torch.zeros(cap * 32, dtype=u8, device=dev) for _ in range(2)], "cnt": torch.zeros(2, dtype=i64, device=dev),
+                  "ent": torch.empty(cap, dtype=f64, device=dev), "keep": torch.empty(cap, dtype=i32, device=dev),
+                  "n": torch.empty(1, dtype=i64, device=dev), "u": torch.empty(cap, dtype=f32, device=dev),
+                  "z": torch.empty(cap, dtype=f32, device=dev), "m1": torch.empty(cap, dtype=i32, device=dev),
+                  "m2": torch.empty(cap, dtype=i32, device=dev), "nm": torch.empty(2, dtype=i64, device=dev),
+                  "view": torch.empty(cap, dtype=u8, device=dev), "xw": torch.empty(3 * cap, dtype=f32, device=dev),
+                  "T0": torch.from_numpy(T0.reshape(-1).copy()).to(dev), "r1": torch.empty(512, dtype=u8, device=dev),
+                  "r2": torch.empty(512, dtype=u8, device=dev), "o": torch.empty(cap, dtype=u8, device=dev),
+                  "r1_host": torch.empty(512, dtype=u8, pin_memory=True), "ev": torch.cuda.Event()})
+    torch.cuda.synchronize(dev)
+
+    def front(b):
+        bgr, gl, gr = b["in"]
+        seg.run_device_maps(bgr.data_ptr(), d_cls.data_ptr(), d_conf.data_ptr(), d_ent.data_ptr(), 0, 0, s)
+        for o, g, side in ((el, gl, 0), (er, gr, 1)):
+            o.enqueue_device(g.data_ptr(), NET_H, NET_W, NET_W, b["kp"][side].data_ptr(), b["desc"][side].data_ptr(), b["cnt"][side:].data_ptr())
+        el.stream_wait(s)
+        seg.semantic_keys_device(b["kp"][0].data_ptr(), b["cnt"][0:].data_ptr(), cap, 8, 0, 0, b["ent"].data_ptr(), b["keep"].data_ptr(),
+                                 b["n"].data_ptr(), s)
+        stereo_match_device(el, er, b["kp"][0].data_ptr(), b["desc"][0].data_ptr(), b["keep"].data_ptr(), b["n"].data_ptr(),
+                            b["kp"][1].data_ptr(), b["desc"][1].data_ptr(), b["cnt"][1:].data_ptr(), MB, MBF, b["u"].data_ptr(), b["z"].data_ptr(), s)
+
+    def last_search(b):
+        search_last_frame_device(el, b["kp"][0].data_ptr(), b["desc"][0].data_ptr(), b["keep"].data_ptr(), b["n"].data_ptr(), b["u"].data_ptr(),
+                                 b["last"].data_ptr(), b["n_last"], frame0, T0[:, :3], T0[:, 3], 7.0, b["m1"].data_ptr(), b["nm"][1:].data_ptr(), s)
+
+    def local_search(b, frame):
+        search_local_points_device(el, b["kp"][0].data_ptr(), b["desc"][0].data_ptr(), b["keep"].data_ptr(), b["n"].data_ptr(),
+                                   b["u"].data_ptr(), 0, b["local"].data_ptr(), b["n_local"], frame, 1.0, 0.8, b["view"].data_ptr(),
+                                   b["m2"].data_ptr(), b["nm"].data_ptr(), s)
+
+    def pose(b, t_in, res):
+        pose_optimize_device(el, b["kp"][0].data_ptr(), b["keep"].data_ptr(), b["n"].data_ptr(), b["u"].data_ptr(), b["xw"].data_ptr(),
+                             FX, FX, CX, CY, MBF, t_in.data_ptr(), res.data_ptr(), b["o"].data_ptr(), s)
+
+    def step(b, with_pose):
+        front(b)
+        last_search(b)
+        if with_pose:
+            with torch.cuda.stream(stream):
+                b["xw"].fill_(float("nan"))
+            pose_gather_device(el, b["m1"].data_ptr(), b["n"].data_ptr(), b["last"].data_ptr(), b["n_last"], b["xw"].data_ptr(), s)
+            pose(b, b["T0"], b["r1"])
+            with torch.cuda.stream(stream):
+                b["r1_host"].copy_(b["r1"], non_blocking=True)
+            stream.synchronize()  # Tracking's host read: the local-map search takes the pose as a host struct
+            frame = frame_from_result(result_from_bytes(b["r1_host"].numpy()), FX, FX, CX, CY, MBF, bounds)
+            local_search(b, frame)
+            pose_gather_device(el, b["m2"].data_ptr(), b["n"].data_ptr(), b["local"].data_ptr(), b["n_local"], b["xw"].data_ptr(), s)
+            pose(b, b["r1"], b["r2"])
+        else:
+            local_search(b, frame0)
+        el.wait_for_stream(s)  # the next enqueue_device overwrites what the tail, the searches and the optimisations read
+        er.wait_for_stream(s)
+        b["ev"].record(stream)
+
+    for b in B:  # first pass: the network's graph is captured, and each frame's keys give its map
+        front(b)
+        stream.synchronize()
+        m = int(b["n"].cpu()[0])
+        kidx = b["keep"][:m].cpu().numpy()
+        kps = b["kp"][0].cpu().numpy().view(KP_DTYPE)[kidx]
+        desc = b["desc"][0].cpu().numpy().reshape(-1, 32)[kidx]
+        last, local = frame_map(kps, desc, b["z"][:m].cpu().numpy(), el.GetScaleFactors(), rng)
+        b["last"], b["local"] = (torch.from_numpy(p.view(np.uint8).reshape(-1).copy()).to(dev) for p in (last, local))
+        b["n_last"], b["n_local"] = len(last), len(local)
+    torch.cuda.synchronize(dev)
+    fps_blocks = {"without_pose": [], "with_two_poses": []}
+    total = {k: [0, 0.0] for k in fps_blocks}
+    n_blocks = max(1, -(-(args.warmup + args.steps) // args.blocks_of))
+    i = 0
+    gc.collect()
+    gc.disable()
+    for blk in range(n_blocks + 2):
+        for name in (("without_pose", "with_two_poses") if blk % 2 == 0 else ("with_two_poses", "without_pose")):
+            torch.cuda.synchronize(dev)
+            t0 = time.perf_counter()
+            for _ in range(args.blocks_of):
+                step(B[i % len(B)], name == "with_two_poses")
+                if (i & 3) == 3:
+                    B[(i - 1) % len(B)]["ev"].synchronize()
+                i += 1
+            torch.cuda.synchronize(dev)
+            dt = time.perf_counter() - t0
+            if blk >= 2:
+                fps_blocks[name].append(args.blocks_of / dt)
+                total[name][0] += args.blocks_of
+                total[name][1] += dt
+    gc.enable()
+    if el.device_status() or er.device_status():
+        raise SystemExit("a pyramid level exceeded the device quad tree's capacity: the asynchronous outputs are not valid")
+    r2 = result_from_bytes(B[(i - 1) % len(B)]["r2"].cpu().numpy())
+
+    gpu, power = torch.cuda.get_device_name(dev), None
+    try:
+        import pynvml
+        pynvml.nvmlInit()
+        power = pynvml.nvmlDeviceGetEnforcedPowerLimit(pynvml.nvmlDeviceGetHandleByIndex(0)) / 1e3
+    except Exception:
+        pass
+    line = {"metric": "pose optimisation", "unit": "ms", "calls": calls,
+            "chain_fps": {name: {"overall": total[name][0] / total[name][1], "median_block": med(fps_blocks[name]),
+                                 "frames": total[name][0]} for name in fps_blocks},
+            "chain_last_second_optimisation": {"n_initial": int(r2.n_initial), "n_good": int(r2.n_good), "sigma_valid": int(r2.sigma_valid)},
+            "g2o_host_loop": "not measured (Eigen + CHOLMOD are not built here)", "calls_timed": args.steps, "warmup": args.warmup,
+            "gpu": gpu, "power_limit_w": power,
+            "workload": f"(a, b) synthetic scenes, 60 % stereo; (c) Bayesian SegNet Basic T={T} + ORB({args.nfeatures}) x2 + semantic keys + "
+                        "stereo + last-frame search (th 7) + local-map search (th 1), with / without gather + pose after each search, "
+                        "synthetic 1024x352 frames"}
+    print(json.dumps(line))
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=30, help="timed calls / frames per measurement")
+    ap.add_argument("--warmup", type=int, default=5)
+    ap.add_argument("--blocks-of", type=int, default=10, help="frames per alternating block of the chain legs")
+    ap.add_argument("--nfeatures", type=int, default=2000)
+    args = ap.parse_args()
+    if args.steps < 1 or args.blocks_of < 1:
+        ap.error("--steps and --blocks-of must be at least 1")
+    run(args)
+
+
+if __name__ == "__main__":
+    main()
