@@ -525,34 +525,33 @@ void SegNet::semantic_keys(const sivo_keypoint* kps, int n, int max_static_class
   if (!last_classes_ || !last_conf_ || !last_ent_) fail(SIVO_EINVAL, "semantic_keys: no segmentation result on the device yet (or a map pointer was NULL)");
   if (n == 0) return;
   SIVO_CUDA(cudaSetDevice(device_));
-  cudaStream_t s = last_stream_;
-  const size_t in_bytes = static_cast<size_t>(n) * sizeof(sivo_keypoint);
-  const size_t out_bytes = static_cast<size_t>(n) * 17;  // n doubles, n doubles, n bytes
+  cudaStream_t s = last_stream_;  // the last run's maps may still be in flight on it
+  // staging: in = int64 count | keypoints, out = int64 n_keep | conf | entropy | keep_idx | class
+  const size_t in_bytes = 8 + static_cast<size_t>(n) * sizeof(sivo_keypoint), out_bytes = 8 + static_cast<size_t>(n) * 21;
   if (d_kp_.bytes < in_bytes) d_kp_.alloc(in_bytes * 2);
   if (d_kp_out_.bytes < out_bytes) d_kp_out_.alloc(out_bytes * 2);
   h_kp_.ensure(in_bytes);
   h_kp_out_.ensure(out_bytes);
-  memcpy(h_kp_.p, kps, in_bytes);
+  *h_kp_.as<long long>() = n;
+  memcpy(h_kp_.as<long long>() + 1, kps, in_bytes - 8);
   SIVO_CUDA(cudaMemcpyAsync(d_kp_.p, h_kp_.p, in_bytes, cudaMemcpyHostToDevice, s));
-  double* o_conf = d_kp_out_.as<double>();
-  double* o_ent = o_conf + n;
-  uint8_t* o_cls = reinterpret_cast<uint8_t*>(o_ent + n);
-  launch_keypoint_lookup(d_kp_.as<sivo_keypoint>(), n, last_classes_, last_conf_, last_ent_, H_, W_, o_cls, o_conf, o_ent, s);
+  long long* o_n = d_kp_out_.as<long long>();
+  double* o_conf = reinterpret_cast<double*>(o_n + 1);
+  int* o_keep = reinterpret_cast<int*>(o_conf + 2 * n);
+  launch_semantic_keys(reinterpret_cast<const sivo_keypoint*>(d_kp_.as<long long>() + 1), d_kp_.as<long long>(), n, last_classes_,
+                       last_conf_, last_ent_, H_, W_, max_static_class, kp_class ? reinterpret_cast<uint8_t*>(o_keep + n) : nullptr,
+                       kp_conf ? o_conf : nullptr, kp_entropy ? o_conf + n : nullptr, keep_idx ? o_keep : nullptr,
+                       keep_idx || n_keep ? o_n : nullptr, s);
   SIVO_CUDA(cudaMemcpyAsync(h_kp_out_.p, d_kp_out_.p, out_bytes, cudaMemcpyDeviceToHost, s));
   SIVO_CUDA(cudaStreamSynchronize(s));
-  const double* hc = h_kp_out_.as<double>();
-  const double* he = hc + n;
-  const uint8_t* hk = reinterpret_cast<const uint8_t*>(he + n);
+  const long long kept = *h_kp_out_.as<long long>();
+  const double* hc = reinterpret_cast<const double*>(h_kp_out_.as<long long>() + 1);
+  const int* hk = reinterpret_cast<const int*>(hc + 2 * n);
   if (kp_conf) memcpy(kp_conf, hc, static_cast<size_t>(n) * sizeof(double));
-  if (kp_entropy) memcpy(kp_entropy, he, static_cast<size_t>(n) * sizeof(double));
-  if (kp_class) memcpy(kp_class, hk, n);
-  int kept = 0;
-  for (int i = 0; i < n; ++i)
-    if (hk[i] != 255 && static_cast<int>(hk[i]) <= max_static_class) {  // `detection <= Classes::TERRAIN` (Frame.cc:190)
-      if (keep_idx) keep_idx[kept] = i;
-      ++kept;
-    }
-  if (n_keep) *n_keep = kept;
+  if (kp_entropy) memcpy(kp_entropy, hc + n, static_cast<size_t>(n) * sizeof(double));
+  if (kp_class) memcpy(kp_class, hk + n, n);
+  if (keep_idx) memcpy(keep_idx, hk, static_cast<size_t>(kept) * sizeof(int));
+  if (n_keep) *n_keep = static_cast<int>(kept);
 }
 
 void SegNet::semantic_keys_device(const sivo_keypoint* kps_dev, const long long* count_dev, int cap, int max_static_class, uint8_t* kp_class_dev,

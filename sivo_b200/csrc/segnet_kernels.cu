@@ -709,29 +709,9 @@ void launch_conv_simt(const ConvParams& p, cudaStream_t s) {
   }
 }
 
-__global__ void k_keypoint_lookup(const sivo_keypoint* __restrict__ kps, int n, const uint8_t* __restrict__ classes,
-                                  const double* __restrict__ conf, const double* __restrict__ ent, int H, int W,
-                                  uint8_t* __restrict__ out_class, double* __restrict__ out_conf, double* __restrict__ out_ent) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const int col = static_cast<int>(kps[i].x), row = static_cast<int>(kps[i].y);  // static_cast<int>(pt.x / pt.y): truncation
-  const bool ok = col >= 0 && col < W && row >= 0 && row < H;
-  const size_t o = ok ? static_cast<size_t>(row) * W + col : 0;
-  out_class[i] = ok ? classes[o] : static_cast<uint8_t>(255);
-  out_conf[i] = ok ? conf[o] : 0.0;
-  out_ent[i] = ok ? ent[o] : 0.0;
-}
-
-void launch_keypoint_lookup(const sivo_keypoint* kps, int n, const uint8_t* classes, const double* conf, const double* ent, int H, int W,
-                            uint8_t* out_class, double* out_conf, double* out_ent, cudaStream_t s) {
-  if (n <= 0) return;
-  k_keypoint_lookup<<<blocks_for(n, 128), 128, 0, s>>>(kps, n, classes, conf, ent, H, W, out_class, out_conf, out_ent);
-  SIVO_CUDA(cudaGetLastError());
-}
-
-// SelectSemanticKeys with a device-resident count: the lookup of k_keypoint_lookup plus the ordered compaction of the kept keys.
-// One block walks the keys in chunks of kSemThreads with a running offset (compact_chunk), so keep_idx comes out ascending,
-// exactly as the host loop builds it.
+// SelectSemanticKeys with a device-resident count: the per-keypoint gather from the three maps plus the ordered compaction of the
+// kept keys.  One block walks the keys in chunks of kSemThreads with a running offset (compact_chunk), so keep_idx comes out
+// ascending, in keypoint order as Frame.cc builds it.
 constexpr int kSemThreads = 512;
 
 __global__ void __launch_bounds__(kSemThreads) k_semantic_keys(const sivo_keypoint* __restrict__ kps, const long long* __restrict__ count,

@@ -57,11 +57,9 @@ void launch_lrn(TensorView in, TensorView out, int size, float alpha, float beta
 void launch_conv_simt(const ConvParams& p, cudaStream_t s);
 void launch_dropout_unpool(TensorView in, int T, const uint8_t* mask, int mask_n, TensorView out, const DropoutParams& d, float scale,
                            cudaStream_t s);
-// per-keypoint gather from the three result maps (Frame.cc:181-186 indexing); out-of-map keypoints get (255, 0, 0)
-void launch_keypoint_lookup(const sivo_keypoint* kps, int n, const uint8_t* classes, const double* conf, const double* ent, int H, int W,
-                            uint8_t* out_class, double* out_conf, double* out_ent, cudaStream_t s);
-// the same lookup for *count (device) keypoints, one block, plus keep_idx[0..*n_keep) = the kept keys in ascending order;
-// *count outside [0, cap] writes nothing but *n_keep = -1.  Any output may be NULL.
+// per-keypoint gather from the three result maps (Frame.cc:181-186 indexing; out-of-map keypoints get (255, 0, 0)) for *count
+// (device) keypoints, one block, plus keep_idx[0..*n_keep) = the kept keys in ascending order; *count outside [0, cap] writes
+// nothing but *n_keep = -1.  Any output may be NULL.
 void launch_semantic_keys(const sivo_keypoint* kps, const long long* count, int cap, const uint8_t* classes, const double* conf,
                           const double* ent, int H, int W, int max_static_class, uint8_t* out_class, double* out_conf, double* out_ent,
                           int* keep_idx, long long* n_keep, cudaStream_t s);

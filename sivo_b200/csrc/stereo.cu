@@ -3,9 +3,6 @@
 // [floor(vR - 2 s), ceil(vR + 2 s)] must contain int(vL), octave within +-1, uR in [uL - maxD, uL - minD];
 // distance = ORBmatcher::DescriptorDistance (ORBmatcher.cc:1582-1596) as 4 x __popcll.  The reference keeps
 // the first strictly smaller distance walking candidates in increasing iR, i.e. (min dist, min iR).
-#include <algorithm>
-#include <vector>
-
 #include "match_fold.cuh"
 #include "orb.h"
 
@@ -13,20 +10,19 @@ namespace sivo {
 namespace {
 constexpr int kThHigh = 100;  // ORBmatcher::TH_HIGH (ORBmatcher.cc:37)
 
-__global__ void k_stereo_hamming(const sivo_keypoint* __restrict__ kl, const uint8_t* __restrict__ dl, int nl,
-                                 const sivo_keypoint* __restrict__ kr, const uint8_t* __restrict__ dr, int nr,
-                                 const float* __restrict__ scale, int rows, float min_d, float max_d,
-                                 int* __restrict__ best_idx, int* __restrict__ best_dist) {
-  int wid = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  if (wid >= nl) return;
-  const sivo_keypoint L = kl[wid];
+// The row-band Hamming search of left keypoint L (descriptor a) over right keypoints [0, nr), warp-wide: every lane calls it with
+// the same L and gets the warp's packed best (dist << 20 | idx), or (kThHigh << 20 | 0xFFFFF) if no candidate is below kThHigh.
+// Right keypoints whose octave is outside [0, nlevels) are skipped.
+__device__ __forceinline__ unsigned stereo_best_right(const sivo_keypoint L, const ulonglong4 a, const sivo_keypoint* __restrict__ kr,
+                                                      const uint8_t* __restrict__ dr, int nr, const float* __restrict__ scale, int nlevels,
+                                                      int rows, float min_d, float max_d, int lane) {
   const int row = static_cast<int>(L.y);
   const float min_u = __fsub_rn(L.x, max_d), max_u = __fsub_rn(L.x, min_d);
-  const ulonglong4 a = *reinterpret_cast<const ulonglong4*>(dl + static_cast<size_t>(wid) * 32);
   unsigned best = (static_cast<unsigned>(kThHigh) << 20) | 0xFFFFFu;  // dist:12 | idx:20
   if (max_u >= 0.f && row >= 0 && row < rows) {
     for (int i = lane; i < nr; i += 32) {
       const sivo_keypoint R = kr[i];
+      if (static_cast<unsigned>(R.octave) >= static_cast<unsigned>(nlevels)) continue;
       const float band = __fmul_rn(2.0f, scale[R.octave]);
       const int maxr = static_cast<int>(ceilf(__fadd_rn(R.y, band)));
       const int minr = static_cast<int>(floorf(__fsub_rn(R.y, band)));
@@ -40,6 +36,17 @@ __global__ void k_stereo_hamming(const sivo_keypoint* __restrict__ kl, const uin
   }
 #pragma unroll
   for (int o = 16; o; o >>= 1) best = min(best, __shfl_xor_sync(0xffffffffu, best, o));
+  return best;
+}
+
+__global__ void k_stereo_hamming(const sivo_keypoint* __restrict__ kl, const uint8_t* __restrict__ dl, int nl,
+                                 const sivo_keypoint* __restrict__ kr, const uint8_t* __restrict__ dr, int nr,
+                                 const float* __restrict__ scale, int nlevels, int rows, float min_d, float max_d,
+                                 int* __restrict__ best_idx, int* __restrict__ best_dist) {
+  int wid = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (wid >= nl) return;
+  const ulonglong4 a = *reinterpret_cast<const ulonglong4*>(dl + static_cast<size_t>(wid) * 32);
+  const unsigned best = stereo_best_right(kl[wid], a, kr, dr, nr, scale, nlevels, rows, min_d, max_d, lane);
   if (lane == 0) {
     int d = best >> 20;
     best_dist[wid] = d;
@@ -50,41 +57,18 @@ __global__ void k_stereo_hamming(const sivo_keypoint* __restrict__ kl, const uin
 // ---- the whole of Frame::ComputeStereoMatches (Frame.cc:444-629) for one left keypoint per warp: Hamming search as
 // above, then the 11x11 SAD slide over +-5 px on the keypoint's pyramid level (windows are centred-intensity
 // differences of u8 pixels, so every L1 distance is an exact integer), parabola sub-pixel fit, disparity gate.
-// The median-based outlier cut (:617-628) needs all matches: the host form does it on the host over the returned SAD distances,
-// the device form in k_stereo_median_cut.
+// The median-based outlier cut (:617-628) needs all matches: k_stereo_median_cut does it over the SAD distances.
 __device__ __forceinline__ float c_roundf(float v) { return v >= 0.f ? floorf(__fadd_rn(v, 0.5f)) : -floorf(__fadd_rn(-v, 0.5f)); }
 
-// The per-keypoint body shared by both forms; every lane of the warp calls it with the same left keypoint L and descriptor row.
-// kCheckOctave: skip right keypoints whose octave is outside [0, nlevels) (the host form validated them on the host).
-template <bool kCheckOctave>
+// The per-keypoint body; every lane of the warp calls it with the same left keypoint L and descriptor row.
 __device__ __forceinline__ void stereo_match_key(const sivo_keypoint L, const uint8_t* __restrict__ dl_key, const sivo_keypoint* __restrict__ kr,
                                                  const uint8_t* __restrict__ dr, int nr, const float* __restrict__ scale,
                                                  const float* __restrict__ inv_scale, const uint8_t* __restrict__ pyr_l, const OrbLevelTable& lt_l,
                                                  const uint8_t* __restrict__ pyr_r, const OrbLevelTable& lt_r, float mb, float mbf, int lane,
                                                  float& out_u, float& out_z, int& out_sad) {
-  const int rows = lt_l.lv[0].h;
-  const int row = static_cast<int>(L.y);
   const float min_d = 0.f, max_d = __fdiv_rn(mbf, mb);
-  const float min_u = __fsub_rn(L.x, max_d), max_u = __fsub_rn(L.x, min_d);
-  const ulonglong4 a = *reinterpret_cast<const ulonglong4*>(dl_key);
-  unsigned best = (static_cast<unsigned>(kThHigh) << 20) | 0xFFFFFu;
-  if (max_u >= 0.f && row >= 0 && row < rows) {
-    for (int i = lane; i < nr; i += 32) {
-      const sivo_keypoint R = kr[i];
-      if (kCheckOctave && static_cast<unsigned>(R.octave) >= static_cast<unsigned>(lt_l.nlevels)) continue;
-      const float band = __fmul_rn(2.0f, scale[R.octave]);
-      const int maxr = static_cast<int>(ceilf(__fadd_rn(R.y, band)));
-      const int minr = static_cast<int>(floorf(__fsub_rn(R.y, band)));
-      if (row < minr || row > maxr) continue;
-      if (R.octave < L.octave - 1 || R.octave > L.octave + 1) continue;
-      if (!(R.x >= min_u && R.x <= max_u)) continue;
-      const ulonglong4 b = *reinterpret_cast<const ulonglong4*>(dr + static_cast<size_t>(i) * 32);
-      unsigned d = __popcll(a.x ^ b.x) + __popcll(a.y ^ b.y) + __popcll(a.z ^ b.z) + __popcll(a.w ^ b.w);
-      if (d < static_cast<unsigned>(kThHigh)) best = min(best, (d << 20) | static_cast<unsigned>(i));
-    }
-  }
-#pragma unroll
-  for (int o = 16; o; o >>= 1) best = min(best, __shfl_xor_sync(0xffffffffu, best, o));
+  const unsigned best = stereo_best_right(L, *reinterpret_cast<const ulonglong4*>(dl_key), kr, dr, nr, scale, lt_l.nlevels, lt_l.lv[0].h,
+                                          min_d, max_d, lane);
   out_u = -1.f;
   out_z = -1.f;
   out_sad = -1;
@@ -145,33 +129,15 @@ __device__ __forceinline__ void stereo_match_key(const sivo_keypoint L, const ui
   }
 }
 
-__global__ void k_stereo_match(const sivo_keypoint* __restrict__ kl, const uint8_t* __restrict__ dl, int nl,
-                               const sivo_keypoint* __restrict__ kr, const uint8_t* __restrict__ dr, int nr,
+// Counts and (optionally) the left keypoint indices live on the device.  Warp j handles left keypoint keep_idx[j] (j when keep_idx
+// is NULL) for j < min(*n_left, cap_l); right keypoints [0, min(*n_right, cap_r)).  A left keypoint whose octave or index is out
+// of range stays unmatched.
+__global__ void k_stereo_match(const sivo_keypoint* __restrict__ kl, const uint8_t* __restrict__ dl, const int* __restrict__ keep_idx,
+                               const long long* __restrict__ n_left, int cap_l, const sivo_keypoint* __restrict__ kr,
+                               const uint8_t* __restrict__ dr, const long long* __restrict__ n_right, int cap_r,
                                const float* __restrict__ scale, const float* __restrict__ inv_scale, const uint8_t* __restrict__ pyr_l,
                                OrbLevelTable lt_l, const uint8_t* __restrict__ pyr_r, OrbLevelTable lt_r, float mb, float mbf,
                                float* __restrict__ u_right, float* __restrict__ depth, int* __restrict__ sad_dist) {
-  const int wid = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  if (wid >= nl) return;
-  float out_u, out_z;
-  int out_sad;
-  stereo_match_key<false>(kl[wid], dl + static_cast<size_t>(wid) * 32, kr, dr, nr, scale, inv_scale, pyr_l, lt_l, pyr_r, lt_r, mb, mbf,
-                          lane, out_u, out_z, out_sad);
-  if (lane == 0) {
-    u_right[wid] = out_u;
-    depth[wid] = out_z;
-    sad_dist[wid] = out_sad;
-  }
-}
-
-// Device form: counts and (optionally) the left keypoint indices live on the device.  Warp j handles left keypoint keep_idx[j]
-// (j when keep_idx is NULL) for j < min(*n_left, cap_l); right keypoints [0, min(*n_right, cap_r)).  A left keypoint whose octave
-// or index is out of range stays unmatched.  Same arithmetic as k_stereo_match through stereo_match_key.
-__global__ void k_stereo_match_dev(const sivo_keypoint* __restrict__ kl, const uint8_t* __restrict__ dl, const int* __restrict__ keep_idx,
-                                   const long long* __restrict__ n_left, int cap_l, const sivo_keypoint* __restrict__ kr,
-                                   const uint8_t* __restrict__ dr, const long long* __restrict__ n_right, int cap_r,
-                                   const float* __restrict__ scale, const float* __restrict__ inv_scale, const uint8_t* __restrict__ pyr_l,
-                                   OrbLevelTable lt_l, const uint8_t* __restrict__ pyr_r, OrbLevelTable lt_r, float mb, float mbf,
-                                   float* __restrict__ u_right, float* __restrict__ depth, int* __restrict__ sad_dist) {
   const int wid = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (wid >= cap_l || wid >= *n_left) return;
   const long long nr64 = *n_right;
@@ -182,8 +148,8 @@ __global__ void k_stereo_match_dev(const sivo_keypoint* __restrict__ kl, const u
   if (k >= 0 && k < cap_l) {
     const sivo_keypoint L = kl[k];
     if (static_cast<unsigned>(L.octave) < static_cast<unsigned>(lt_l.nlevels))
-      stereo_match_key<true>(L, dl + static_cast<size_t>(k) * 32, kr, dr, nr, scale, inv_scale, pyr_l, lt_l, pyr_r, lt_r, mb, mbf, lane,
-                             out_u, out_z, out_sad);
+      stereo_match_key(L, dl + static_cast<size_t>(k) * 32, kr, dr, nr, scale, inv_scale, pyr_l, lt_l, pyr_r, lt_r, mb, mbf, lane,
+                       out_u, out_z, out_sad);
   }
   if (lane == 0) {
     u_right[wid] = out_u;
@@ -194,8 +160,8 @@ __global__ void k_stereo_match_dev(const sivo_keypoint* __restrict__ kl, const u
 
 // ---- median-based outlier cut (Frame.cc:617-628) on the device, one block.  m = number of matched keys (SAD >= 0); the median
 // is the SAD at index m / 2 of the ascending order.  Every SAD is an integer <= 121 * 510 < 2^16, so an exact two-pass radix
-// select (high byte, then low byte, 256-bin shared histograms) finds it without sorting.  th = 1.5f * 1.4f * median in float as
-// on the host; every matched key with (float) sad >= th -- exactly the tail the host loop walks -- is unmatched (-1).
+// select (high byte, then low byte, 256-bin shared histograms) finds it without sorting.  th = 1.5f * 1.4f * median in float; every
+// matched key with (float) sad >= th -- exactly the tail the reference walks down the sorted distances -- is unmatched (-1).
 constexpr int kCutThreads = 1024;
 
 // warp 0: the bin holding the element of rank `k` (0-based, ascending) of the 256-bin histogram, and its rank within that bin
@@ -269,6 +235,18 @@ __global__ void __launch_bounds__(kCutThreads) k_stereo_median_cut(const long lo
   }
 }
 
+// Both forms: the match kernel over cap_l outputs, then the median cut over their SAD distances in `sad` (cap_l ints), on `s`.
+void launch_stereo(const Orb& left, const Orb& right, const sivo_keypoint* kl, const uint8_t* dl, const int* keep_idx, const long long* n_left,
+                   int cap_l, const sivo_keypoint* kr, const uint8_t* dr, const long long* n_right, int cap_r, float mb, float mbf,
+                   float* u_right, float* depth, int* sad, cudaStream_t s) {
+  k_stereo_match<<<ceil_div(cap_l * 32, 128), 128, 0, s>>>(kl, dl, keep_idx, n_left, cap_l, kr, dr, n_right, cap_r, left.dev_scale(),
+                                                           left.dev_inv_scale(), left.dev_pyramid(), left.levels(), right.dev_pyramid(),
+                                                           right.levels(), mb, mbf, u_right, depth, sad);
+  SIVO_CUDA(cudaGetLastError());
+  k_stereo_median_cut<<<1, kCutThreads, 0, s>>>(n_left, cap_l, sad, u_right, depth);
+  SIVO_CUDA(cudaGetLastError());
+}
+
 }  // namespace
 
 StereoWs& stereo_ws() {
@@ -301,7 +279,7 @@ void stereo_hamming(int device, const sivo_keypoint* left, const uint8_t* dl, in
     SIVO_CUDA(cudaMemcpyAsync(d_dr, dr, static_cast<size_t>(nr) * 32, cudaMemcpyHostToDevice, st));
   }
   SIVO_CUDA(cudaMemcpyAsync(d_sc, scale, nlevels * sizeof(float), cudaMemcpyHostToDevice, st));
-  k_stereo_hamming<<<ceil_div(nl * 32, 128), 128, 0, st>>>(d_kl, d_dl, nl, d_kr, d_dr, nr, d_sc, rows, min_d, max_d, d_bi, d_bd);
+  k_stereo_hamming<<<ceil_div(nl * 32, 128), 128, 0, st>>>(d_kl, d_dl, nl, d_kr, d_dr, nr, d_sc, nlevels, rows, min_d, max_d, d_bi, d_bd);
   SIVO_CUDA(cudaGetLastError());
   SIVO_CUDA(cudaMemcpyAsync(best_idx, d_bi, nl * sizeof(int), cudaMemcpyDeviceToHost, st));
   SIVO_CUDA(cudaMemcpyAsync(best_dist, d_bd, nl * sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -388,44 +366,29 @@ void stereo_match(const Orb& left, const Orb& right, const sivo_keypoint* kl, co
   for (int i = 0; i < nr; ++i) if (kr[i].octave < 0 || kr[i].octave >= nlev) fail(SIVO_EINVAL, "stereo: right octave out of range");
   StereoWs& ws = stereo_ws();
   ws.begin(left.device(), pad256(nl * sizeof(sivo_keypoint)) + pad256(static_cast<size_t>(nl) * 32) + pad256(nr * sizeof(sivo_keypoint)) +
-                              pad256(static_cast<size_t>(nr) * 32) + 2 * pad256(nlev * sizeof(float)) + 3 * pad256(nl * sizeof(float)) + 4096);
+                              pad256(static_cast<size_t>(nr) * 32) + pad256(2 * sizeof(long long)) + 3 * pad256(nl * sizeof(float)) + 4096);
   cudaStream_t st = ws.stream;
   sivo_keypoint* d_kl = ws.take<sivo_keypoint>(nl);
   uint8_t* d_dl = ws.take<uint8_t>(static_cast<size_t>(nl) * 32);
   sivo_keypoint* d_kr = ws.take<sivo_keypoint>(nr);
   uint8_t* d_dr = ws.take<uint8_t>(static_cast<size_t>(nr) * 32);
-  float* d_sc = ws.take<float>(nlev);
-  float* d_isc = ws.take<float>(nlev);
+  long long* d_n = ws.take<long long>(2);
   float* d_u = ws.take<float>(nl);
   float* d_z = ws.take<float>(nl);
   int* d_s = ws.take<int>(nl);
+  const long long counts[2] = {nl, nr};
   SIVO_CUDA(cudaMemcpyAsync(d_kl, kl, nl * sizeof(sivo_keypoint), cudaMemcpyHostToDevice, st));
   SIVO_CUDA(cudaMemcpyAsync(d_dl, dl, static_cast<size_t>(nl) * 32, cudaMemcpyHostToDevice, st));
   SIVO_CUDA(cudaMemcpyAsync(d_kr, kr, nr * sizeof(sivo_keypoint), cudaMemcpyHostToDevice, st));
   SIVO_CUDA(cudaMemcpyAsync(d_dr, dr, static_cast<size_t>(nr) * 32, cudaMemcpyHostToDevice, st));
-  SIVO_CUDA(cudaMemcpyAsync(d_sc, left.tables().scale.data(), nlev * sizeof(float), cudaMemcpyHostToDevice, st));
-  SIVO_CUDA(cudaMemcpyAsync(d_isc, left.tables().inv_scale.data(), nlev * sizeof(float), cudaMemcpyHostToDevice, st));
-  // the pyramids were written on the two extractors' own streams; their synchronous run() has returned, so they are complete
-  k_stereo_match<<<ceil_div(nl * 32, 128), 128, 0, st>>>(d_kl, d_dl, nl, d_kr, d_dr, nr, d_sc, d_isc, left.dev_pyramid(), left.levels(),
-                                                         right.dev_pyramid(), right.levels(), mb, mbf, d_u, d_z, d_s);
-  SIVO_CUDA(cudaGetLastError());
-  std::vector<int> sad(nl);
+  SIVO_CUDA(cudaMemcpyAsync(d_n, counts, sizeof(counts), cudaMemcpyHostToDevice, st));
+  // the pyramids were written on the two extractors' own streams; their synchronous run() has returned, so they are complete.
+  // The SAD distances go to this call's workspace: the left extractor's scratch holds capacity() entries and belongs to its
+  // device-form calls, which are not ordered with this one.
+  launch_stereo(left, right, d_kl, d_dl, nullptr, d_n, nl, d_kr, d_dr, d_n + 1, nr, mb, mbf, d_u, d_z, d_s, st);
   SIVO_CUDA(cudaMemcpyAsync(u_right, d_u, nl * sizeof(float), cudaMemcpyDeviceToHost, st));
   SIVO_CUDA(cudaMemcpyAsync(depth, d_z, nl * sizeof(float), cudaMemcpyDeviceToHost, st));
-  SIVO_CUDA(cudaMemcpyAsync(sad.data(), d_s, nl * sizeof(int), cudaMemcpyDeviceToHost, st));
   SIVO_CUDA(cudaStreamSynchronize(st));
-  // median-based outlier cut (Frame.cc:617-628)
-  std::vector<std::pair<int, int>> v;
-  for (int i = 0; i < nl; ++i) if (sad[i] >= 0) v.emplace_back(sad[i], i);
-  if (v.empty()) return;
-  std::sort(v.begin(), v.end());
-  const float median = static_cast<float>(v[v.size() / 2].first);
-  const float th = 1.5f * 1.4f * median;
-  for (int i = static_cast<int>(v.size()) - 1; i >= 0; --i) {
-    if (static_cast<float>(v[i].first) < th) break;
-    u_right[v[i].second] = -1.f;
-    depth[v[i].second] = -1.f;
-  }
 }
 
 // ComputeStereoMatches on device-resident keypoints, descriptors and counts, enqueued on `s` (NULL: the left extractor's stream)
@@ -441,12 +404,7 @@ void stereo_match_device(Orb& left, Orb& right, const sivo_keypoint* kl, const u
   if (!s) s = left.stream();
   left.stream_wait(s);
   right.stream_wait(s);
-  const int cap_l = left.capacity(), cap_r = right.capacity();
-  k_stereo_match_dev<<<ceil_div(cap_l * 32, 128), 128, 0, s>>>(kl, dl, keep_idx, n_left, cap_l, kr, dr, n_right, cap_r, left.dev_scale(),
-                                                               left.dev_inv_scale(), left.dev_pyramid(), left.levels(), right.dev_pyramid(),
-                                                               right.levels(), mb, mbf, u_right, depth, left.stereo_sad());
-  SIVO_CUDA(cudaGetLastError());
-  k_stereo_median_cut<<<1, kCutThreads, 0, s>>>(n_left, cap_l, left.stereo_sad(), u_right, depth);
-  SIVO_CUDA(cudaGetLastError());
+  launch_stereo(left, right, kl, dl, keep_idx, n_left, left.capacity(), kr, dr, n_right, right.capacity(), mb, mbf, u_right, depth,
+                left.stereo_sad(), s);
 }
 }  // namespace sivo

@@ -176,6 +176,37 @@ def test_semantic_keys_device_out_of_map_keys_count_above_cap_and_null_outputs(s
         assert (o.cls.cpu().numpy() == 77).all() and (o.keep.cpu().numpy() == -7).all() and (o.conf.cpu().numpy() == 7.0).all()
 
 
+def test_semantic_keys_host_form_reads_maps_still_in_flight(seg):
+    """The host form runs on the stream of the last run: it reads that run's maps although the host has not waited for them."""
+    (bgr_a, _, _), (bgr_b, gray_b, _) = synth(20), synth(21)
+    kps, _ = ORBextractor(2000, 1.2, 8, 20, 7)(gray_b, None)
+    maps = [torch.empty(H * W, dtype=t, device="cuda") for t in (torch.uint8, torch.float64, torch.float64)]
+    d_a, d_b = to_dev(bgr_a), to_dev(bgr_b)
+    side = torch.cuda.Stream()
+
+    def run(d_bgr, frame):
+        seg.set_frame(frame)
+        seg.run_device_maps(ptr(d_bgr), *(ptr(m) for m in maps), 0, 0, side.cuda_stream)
+
+    run(d_b, 41)  # first use of the stream: the network's graph is captured here
+    side.synchronize()
+    run(d_a, 40)
+    side.synchronize()
+    maps_a = [m.cpu().numpy().reshape(H, W) for m in maps]
+    xy = np.stack([kps["x"], kps["y"]], 1)
+    want_a = O.select_semantic_keys(xy, *maps_a)
+    # also sizes the call's staging buffers: allocating them in the call below would serialise it behind the side stream
+    assert all(np.array_equal(g, w) for g, w in zip(seg.semantic_keys(kps, 8), want_a))
+    with torch.cuda.stream(side):
+        torch.cuda._sleep(200_000_000)  # frame B's maps are written only after this spin
+    run(d_b, 41)
+    got = seg.semantic_keys(kps, 8)  # no host synchronisation before this call
+    side.synchronize()
+    want = O.select_semantic_keys(xy, *[m.cpu().numpy().reshape(H, W) for m in maps])
+    assert all(np.array_equal(g, w) for g, w in zip(got, want)) and len(want[3]) > 0
+    assert not np.array_equal(want_a[1], want[1])  # frame A's maps would show
+
+
 # ---------------------------------------------------------------------------------------------------------- stereo
 @pytest.mark.parametrize("nf", [1000, 2000])
 @pytest.mark.parametrize("baseline", sorted(BASELINES))
@@ -271,6 +302,22 @@ def test_stereo_device_edge_cases():
     sel = np.setdiff1d(np.arange(n), np.arange(0, n, 3)).astype(np.int32)
     hu, hz = stereo_match(el, er, kl[sel], dl[sel], kr, dr, mb, mbf)
     assert u[sel].tobytes() == hu.tobytes() and z[sel].tobytes() == hz.tobytes() and (hu >= 0).sum() > 20
+
+
+def test_stereo_host_form_takes_more_left_keys_than_the_capacity():
+    """The host form sizes its buffers from the call, not from the left extractor's capacity()."""
+    mb, mbf = BASELINES["kitti"]
+    _, gl, gr = synth(1)
+    el, er = extractors(1000)
+    kl, dl = el(gl, None)
+    kr, dr = er(gr, None)
+    kl2, dl2 = np.concatenate([kl, kl]), np.concatenate([dl, dl])
+    assert len(kl2) > el.capacity()
+    u, z = stereo_match(el, er, kl2, dl2, kr, dr, mb, mbf)
+    ru, rz = O.compute_stereo_matches(kl2, dl2, kr, dr, el._bordered, er._bordered, el.GetScaleFactors(), el.GetInverseScaleFactors(),
+                                      mb, mbf)
+    assert u.tobytes() == ru.tobytes() and z.tobytes() == rz.tobytes()
+    assert (u[len(kl):] >= 0).sum() > 50
 
 
 def test_error_codes(seg, model_dir):
