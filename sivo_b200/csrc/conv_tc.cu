@@ -233,7 +233,8 @@ __device__ __forceinline__ void fence_acc(float (&d)[R][F]) {
 __device__ __forceinline__ float affine(const TcParams& p, const TcConsts& cst, float v, int c) {
   float t = __fadd_rn(v, cst.bias[c]);
   if (p.has_bn) t = __fadd_rn(__fmul_rn(t, cst.bn_scale[c]), cst.bn_shift[c]);
-  if (p.relu) t = t > 0.f ? t : __fmul_rn(p.slope, t);
+  // a negative input gives +0 (Caffe's max(t, 0) + slope * min(t, 0)), not slope * t = -0
+  if (p.relu) t = t > 0.f ? t : (p.slope != 0.f ? __fmul_rn(p.slope, t) : 0.f);
   return t;
 }
 

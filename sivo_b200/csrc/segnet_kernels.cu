@@ -132,7 +132,7 @@ __global__ void __launch_bounds__(kConvThreads) k_conv_simt(ConvParams p, int CK
       if (co >= p.out.cs) continue;
       float v = __fadd_rn(acc[i][j], p.bias[co]);
       if (p.bn_scale) v = __fadd_rn(__fmul_rn(v, p.bn_scale[co]), p.bn_shift[co]);
-      if (p.relu) v = v > 0.f ? v : __fmul_rn(p.slope, v);
+      if (p.relu) v = v > 0.f ? v : (p.slope != 0.f ? __fmul_rn(p.slope, v) : 0.f);  // +0 for a negative input, as Caffe's ReLU
       st_act(out + static_cast<size_t>(gx) * p.out.cs + co, v);
     }
   }

@@ -6,7 +6,9 @@ import numpy as np
 import pytest
 import torch
 
+from oracle import conv_bounds as B
 from sivo_b200 import _lib as L
+from test_gpu_layers import interval_violations
 
 pytestmark = pytest.mark.gpu
 
@@ -47,6 +49,7 @@ def test_stacked_logits_conv_matches_oracle(k, n, h, w):
     ref = torch.relu(ref * torch.from_numpy(sc).view(1, -1, 1, 1) + torch.from_numpy(sh).view(1, -1, 1, 1)).numpy()
     err = np.abs(out - ref)
     assert err.max() < 2e-3 * max(1.0, float(np.abs(ref).max())), float(err.max())
+    assert interval_violations(xt.numpy(), wtt.numpy(), b, sc, sh, out, B.gamma_tc(k, 64), half=False) == 0
 
 
 @pytest.mark.parametrize("k", [3, 7])

@@ -6,6 +6,7 @@ import numpy as np
 import pytest
 import torch
 
+from oracle import conv_bounds as B
 from oracle import philox, segnet_oracle as S
 from sivo_b200 import _lib as L
 
@@ -14,6 +15,19 @@ pytestmark = pytest.mark.gpu
 
 def _p(a):
     return a.ctypes.data_as(C.c_void_p)
+
+
+def interval_violations(x, wt, b, sc, sh, out, gamma, relu=True, half=True, abs_per_input=0.0):
+    """Outputs outside the float64 interval of oracle/conv_bounds.py, over the whole output tensor."""
+    k = wt.shape[-1]
+    extra = abs_per_input * B.conv_abs(np.ones_like(x), wt, k // 2) if abs_per_input else None
+    cb = B.ConvBound(x, wt, k // 2, gamma, b, sc, sh, relu=relu, extra=extra)
+    lo, hi = cb.half_interval() if half else cb.float_interval()
+    bad = B.outside(out, lo, hi)
+    ratio, frac = cb.stats(out, half)
+    print(f"interval: {int(bad.sum())} of {bad.size} outside, max |out - f(r)| / bound {ratio:.3f}"
+          + (f", {frac:.2e} != half_rn(f(r))" if half else ""))
+    return int(bad.sum())
 
 
 def gpu_pool(x):
@@ -86,6 +100,39 @@ def test_mc_reduce_matches_oracle_and_first_max():
     assert abs(ent[0, 0] - np.log2(15)) < 1e-6
 
 
+# T across the 6-sample load batches of k_mc_reduce_quad; C up to 16 on the quad kernel, 17 and 21 on k_mc_reduce_generic
+@pytest.mark.parametrize("T", [2, 3, 6, 7, 12, 13, 24])
+@pytest.mark.parametrize("Cn", [1, 4, 5, 11, 15, 16, 17, 21])
+def test_mc_reduce_sweep_within_float64_bounds(T, Cn):
+    rng = np.random.default_rng(100 * T + Cn)
+    H, W = 5, 13  # hw = 65: not a multiple of 8
+    logits = rng.normal(0, 3, size=(T, Cn, H, W)).astype(np.float32)
+    logits[:, :, 0, 2] = rng.uniform(-80, 0, size=(T, Cn)).astype(np.float32)   # spread down to -80 below the max
+    logits[:, :, 0, 2][:, 0] = 0.0
+    if Cn > 12:  # classes 3 and 12 in different lanes of the quad kernel, identical and on top: 3 wins
+        logits[:, :, 0, 0] = -5.0
+        logits[:, 3, 0, 0] = logits[:, 12, 0, 0] = 4.0
+    if Cn > 5:  # classes 4 and 5 in the same lane
+        logits[:, :, 0, 1] = -5.0
+        logits[:, 4, 0, 1] = logits[:, 5, 0, 1] = 4.0
+    cls = np.empty((H, W), np.uint8)
+    conf = np.empty((H, W), np.float64)
+    ent = np.empty((H, W), np.float64)
+    L.check(L.lib().sivo_dbg_mc_reduce(0, _p(logits), T, Cn, H, W, _p(cls), _p(conf), _p(ent)))
+    rc, rf, re = S.mc_reduce(S.softmax_channels(torch.from_numpy(logits)).numpy())
+    bc, bconf, bent, conf_b, ent_b, margin = B.map_bounds(logits)
+    print(f"mc reduce T={T} C={Cn}: |d conf| {np.abs(conf - bconf).max():.2e} (bound {conf_b.max():.2e}), "
+          f"|d entropy| {np.abs(ent - bent).max():.2e} (bound {ent_b.max():.2e})")
+    if Cn > 12:
+        assert cls[0, 0] == 3
+    if Cn > 5:
+        assert cls[0, 1] == 4
+    sure = margin > 2 * conf_b
+    assert np.array_equal(cls[sure], bc[sure])
+    assert (np.abs(conf - bconf) <= conf_b).all() and (np.abs(ent - bent) <= ent_b).all()
+    assert np.abs(conf - rf).max() < 1e-6 and np.abs(ent - re).max() < 1e-5
+
+
 @pytest.mark.parametrize("k,cin,cout,prec", [(7, 3, 64, "fp32"), (7, 64, 64, "fp32"), (3, 64, 128, "fp32"), (1, 64, 15, "fp32"),
                                              (3, 3, 64, "fp16"), (7, 64, 64, "fp16"), (3, 128, 64, "fp16"), (3, 64, 15, "fp16")])
 def test_conv_simt_matches_oracle(k, cin, cout, prec):
@@ -109,6 +156,8 @@ def test_conv_simt_matches_oracle(k, cin, cout, prec):
         ref = ref.half().float()
     tol = 1e-4 if prec == "fp32" else 2e-3   # caffe's conv test: 1e-4 vs the naive loop; half storage: 1 ulp = 2^-11 rel
     assert np.abs(out - ref.numpy()).max() < tol * max(1.0, float(ref.abs().max()))
+    xs, ws = (x, wt) if prec == "fp32" else (xt.numpy(), wtt.numpy())
+    assert interval_violations(xs, ws, b, sc, sh, out, B.gamma_simt(k, cin), half=prec == "fp16" and cout % 8 == 0) == 0
 
 
 @pytest.mark.parametrize("k,cin,cout,n,h,w", [(7, 64, 64, 1, 8, 128), (7, 64, 64, 2, 22, 200), (3, 64, 64, 1, 16, 128),
@@ -140,6 +189,7 @@ def test_conv_tcgen05_matches_oracle(k, cin, cout, n, h, w):
     ref = (ref.half().float() if cout % 8 == 0 else ref).numpy()  # the 15-channel logits layer stays float
     err = np.abs(out - ref)
     assert err.max() < 2e-3 * max(1.0, float(np.abs(ref).max())), float(err.max())
+    assert interval_violations(xt.numpy(), wtt.numpy(), b, sc, sh, out, B.gamma_tc(k, cin), half=cout % 8 == 0) == 0
 
 
 @pytest.mark.parametrize("k,cin,cout,n,h,w", [(7, 64, 64, 2, 22, 200), (3, 64, 64, 1, 16, 128), (3, 64, 128, 2, 11, 96),
@@ -168,3 +218,4 @@ def test_conv_tcgen05_split_operand_mode_is_fp32_grade(k, cin, cout, n, h, w):
     err, err32 = float(np.abs(out - ref).max()) / scale, float(np.abs(r32 - ref).max()) / scale
     print(f"split conv k={k} {cin}->{cout}: max err {err:.2e} of scale (torch fp32: {err32:.2e})")
     assert err < 1e-5, err
+    assert interval_violations(x, wt, b, sc, sh, out, B.gamma_split(k, cin), half=False, abs_per_input=B.SPLIT_ABS) == 0

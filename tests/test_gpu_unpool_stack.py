@@ -7,7 +7,12 @@ import ctypes as C
 import numpy as np
 import pytest
 
+import torch
+
 from conftest import make_model
+from oracle import conv_bounds as B
+from oracle import segnet_oracle as S
+from test_gpu_layers import interval_violations
 from sivo_b200 import BayesianSegNet, BayesianSegNetParams
 from sivo_b200 import _lib as L
 from sivo_b200.synth import stereo_frame
@@ -61,6 +66,10 @@ def test_unpool_on_load_equals_unpool_then_conv(n, h, w, shared_mask):
     args = _case(n, 1 if shared_mask else n, h, w, seed=h * 1000 + w)
     got, want = _fused(*args), _two_kernels(*args)
     assert np.array_equal(got.view(np.uint32), want.view(np.uint32)), float(np.abs(got - want).max())
+    x, mask, wt, b, sc, sh = args
+    n_, _, h_, w_ = x.shape
+    up = S.unpool(torch.from_numpy(x).half().float(), torch.from_numpy(mask.astype(np.int64)).expand(n_, -1, -1, -1)).numpy()
+    assert interval_violations(up, B.half_rn(wt).astype(np.float32), b, sc, sh, got, B.gamma_tc(7, 64), relu=False, half=False) == 0
 
 
 def test_unpool_on_load_does_not_depend_on_the_row_split():
