@@ -7,7 +7,7 @@
 #include <cstring>
 #include <string>
 
-#include "orb.h"
+#include "frame_ops.h"
 #include "segnet.h"
 
 namespace sivo {
@@ -15,45 +15,6 @@ namespace {
 thread_local std::string g_last_error;
 }
 void set_last_error(const std::string& m) { g_last_error = m; }
-void stereo_hamming(int device, const sivo_keypoint* left, const uint8_t* dl, int nl, const sivo_keypoint* right,
-                    const uint8_t* dr, int nr, const float* scale, int nlevels, int rows, float min_d, float max_d,
-                    int* best_idx, int* best_dist);
-void stereo_match(const Orb& left, const Orb& right, const sivo_keypoint* kl, const uint8_t* dl, int nl, const sivo_keypoint* kr,
-                  const uint8_t* dr, int nr, float mb, float mbf, float* u_right, float* depth);
-void stereo_match_device(Orb& left, Orb& right, const sivo_keypoint* kl, const uint8_t* dl, const int* keep_idx, const long long* n_left,
-                         const sivo_keypoint* kr, const uint8_t* dr, const long long* n_right, float mb, float mbf, float* u_right,
-                         float* depth, cudaStream_t s);
-void info_select(const Orb& left, const sivo_keypoint* kps, const float* depth, const double* entropy, int n, const sivo_info_camera& cam,
-                 double threshold, float* world, double* reduction, int* selected, int* n_selected);
-void info_terms(const Orb& left, const sivo_keypoint* kps, const float* depth, int n, const sivo_info_camera& cam, float* world,
-                double* det_state, double* det_meas, double* det_joint);
-void info_select_device(const Orb& left, const sivo_keypoint* kps, const double* kp_entropy, const int* keep_idx, const long long* n_keep,
-                        const float* depth, const sivo_info_camera& cam, double threshold, float* world, double* reduction, int* selected,
-                        long long* n_selected, cudaStream_t s);
-void search_local_points(const Orb& left, const sivo_keypoint* kps, const uint8_t* desc, const float* u_right, const uint8_t* blocked, int n,
-                         const sivo_map_point* pts, int n_points, const sivo_track_frame& f, float th, float nnratio, uint8_t* in_view,
-                         int* match, int* n_matches);
-void search_last_frame(const Orb& left, const sivo_keypoint* kps, const uint8_t* desc, const float* u_right, int n, const sivo_map_point* pts,
-                       int n_points, const sivo_track_frame& f, const float* Rlw, const float* tlw, float th, int* match, int* n_matches);
-void search_local_points_device(const Orb& left, const sivo_keypoint* kps, const uint8_t* desc, const int* keep_idx, const long long* n_keep,
-                                const float* u_right, const uint8_t* blocked, const sivo_map_point* pts, int n_points,
-                                const sivo_track_frame& f, float th, float nnratio, uint8_t* in_view, int* match, long long* n_matches,
-                                cudaStream_t s);
-void search_last_frame_device(const Orb& left, const sivo_keypoint* kps, const uint8_t* desc, const int* keep_idx, const long long* n_keep,
-                              const float* u_right, const sivo_map_point* pts, int n_points, const sivo_track_frame& f, const float* Rlw,
-                              const float* tlw, float th, int* match, long long* n_matches, cudaStream_t s);
-void features_in_area(const Orb& left, const sivo_keypoint* kps, int n, const sivo_track_frame& f, const float* xyr, const int* levels, int nq,
-                      int* offsets, int* idx, int idx_cap);
-void pose_optimize_device(const Orb& left, const sivo_keypoint* kps, const int* keep_idx, const long long* n_keep, const float* u_right,
-                          const float* xw, float fx, float fy, float cx, float cy, float mbf, const float* Tcw_in,
-                          sivo_pose_result* result, uint8_t* outlier, cudaStream_t s);
-void pose_gather_device(const Orb& left, const int* match, const long long* n_keep, const sivo_map_point* pts, int n_points, float* xw,
-                        cudaStream_t s);
-void pose_optimize(const Orb& left, const sivo_keypoint* kps, const float* u_right, const float* xw, int n, float fx, float fy, float cx,
-                   float cy, float mbf, const float* Tcw_in, sivo_pose_result* result, uint8_t* outlier);
-void pose_system(const Orb& left, const sivo_keypoint* kps, const float* u_right, const float* xw, int n, float fx, float fy, float cx,
-                 float cy, float mbf, const double* pose7, int robust_stereo, const uint8_t* level1, double* err, double* chi2, double* rho,
-                 double* jac, double* H, double* b, double* chi);
 }  // namespace sivo
 
 using namespace sivo;

@@ -6,7 +6,8 @@
 #include <cmath>
 
 #include "compact.cuh"
-#include "orb.h"
+#include "frame_ops.h"
+#include "host_call.h"
 
 namespace sivo {
 
@@ -222,42 +223,33 @@ void info_host(const Orb& left, const sivo_keypoint* kps, const float* depth, co
   if (n < 0) fail(SIVO_EINVAL, "info_select: n = %d", n);
   const InfoParams p = make_params(left, cam, threshold);
   const bool dets = det_state || det_meas || det_joint;
-  StereoWs& ws = stereo_ws();
-  ws.begin(left.device(), pad256(n * sizeof(sivo_keypoint)) + pad256(n * sizeof(float)) + pad256(n * sizeof(double)) +
-                              pad256(sizeof(long long)) + pad256(3 * sizeof(float) * n) + pad256(n * sizeof(double)) + pad256(n) +
-                              pad256(n * sizeof(int)) + pad256(sizeof(long long)) + (dets ? 3 * pad256(n * sizeof(double)) : 0) + 4096);
-  cudaStream_t st = ws.stream;
-  sivo_keypoint* d_kps = ws.take<sivo_keypoint>(n);
-  float* d_depth = ws.take<float>(n);
-  double* d_ent = ws.take<double>(n);
-  long long* d_count = ws.take<long long>(1);
-  float* d_world = world ? ws.take<float>(3 * static_cast<size_t>(n)) : nullptr;
-  double* d_red = reduction ? ws.take<double>(n) : nullptr;
-  uint8_t* d_flags = ws.take<uint8_t>(n);
-  int* d_sel = selected ? ws.take<int>(n) : nullptr;
-  long long* d_nsel = selected || n_selected ? ws.take<long long>(1) : nullptr;
+  HostCall& hc = host_call();
+  hc.begin(left.device());
+  const sivo_keypoint* d_kps = hc.upload(kps, n);
+  const float* d_depth = hc.upload(depth, n);
+  double* d_ent = hc.upload(entropy, n);
+  if (!entropy && n) SIVO_CUDA(cudaMemsetAsync(d_ent, 0, n * sizeof(double), hc.stream));
+  const long long count = n;
+  const long long* d_count = hc.upload(&count, 1);
+  float* d_world = world ? hc.take<float>(3 * static_cast<size_t>(n)) : nullptr;
+  double* d_red = reduction ? hc.take<double>(n) : nullptr;
+  uint8_t* d_flags = hc.take<uint8_t>(n);
+  int* d_sel = selected ? hc.take<int>(n) : nullptr;
+  long long* d_nsel = selected || n_selected ? hc.take<long long>(1) : nullptr;
   double* d_det[3] = {nullptr, nullptr, nullptr};
   if (dets)
-    for (auto& d : d_det) d = ws.take<double>(n);
-  const long long count = n;
-  if (n) {
-    SIVO_CUDA(cudaMemcpyAsync(d_kps, kps, n * sizeof(sivo_keypoint), cudaMemcpyHostToDevice, st));
-    SIVO_CUDA(cudaMemcpyAsync(d_depth, depth, n * sizeof(float), cudaMemcpyHostToDevice, st));
-    if (entropy) SIVO_CUDA(cudaMemcpyAsync(d_ent, entropy, n * sizeof(double), cudaMemcpyHostToDevice, st));
-    else SIVO_CUDA(cudaMemsetAsync(d_ent, 0, n * sizeof(double), st));
-  }
-  SIVO_CUDA(cudaMemcpyAsync(d_count, &count, sizeof(long long), cudaMemcpyHostToDevice, st));
-  launch_info_select(p, d_kps, d_ent, nullptr, d_count, n, d_depth, d_world, d_red, d_flags, d_sel, d_nsel, d_det[0], d_det[1], d_det[2], st);
+    for (auto& d : d_det) d = hc.take<double>(n);
+  launch_info_select(p, d_kps, d_ent, nullptr, d_count, n, d_depth, d_world, d_red, d_flags, d_sel, d_nsel, d_det[0], d_det[1], d_det[2],
+                     hc.stream);
   long long nsel = 0;
-  if (n && world) SIVO_CUDA(cudaMemcpyAsync(world, d_world, 3 * sizeof(float) * n, cudaMemcpyDeviceToHost, st));
-  if (n && reduction) SIVO_CUDA(cudaMemcpyAsync(reduction, d_red, n * sizeof(double), cudaMemcpyDeviceToHost, st));
-  if (d_nsel) SIVO_CUDA(cudaMemcpyAsync(&nsel, d_nsel, sizeof(long long), cudaMemcpyDeviceToHost, st));
-  SIVO_CUDA(cudaStreamSynchronize(st));  // the selected list's length is known only now
-  if (selected && nsel > 0) SIVO_CUDA(cudaMemcpyAsync(selected, d_sel, nsel * sizeof(int), cudaMemcpyDeviceToHost, st));
+  hc.download(world, d_world, 3 * static_cast<size_t>(n));
+  hc.download(reduction, d_red, n);
+  if (d_nsel) hc.download(&nsel, d_nsel, 1);
+  hc.sync();  // the selected list's length is known only now
+  if (nsel > 0) hc.download(selected, d_sel, nsel);
   double* out_det[3] = {det_state, det_meas, det_joint};
-  for (int i = 0; i < 3; ++i)
-    if (n && out_det[i]) SIVO_CUDA(cudaMemcpyAsync(out_det[i], d_det[i], n * sizeof(double), cudaMemcpyDeviceToHost, st));
-  SIVO_CUDA(cudaStreamSynchronize(st));
+  for (int i = 0; i < 3; ++i) hc.download(out_det[i], d_det[i], n);
+  hc.sync();
   if (n_selected) *n_selected = static_cast<int>(nsel);
 }
 }  // namespace

@@ -64,8 +64,6 @@ struct OrbSelected {  // one retained keypoint, level coordinates
 // ---- kernels (orb_kernels.cu)
 void orb_launch_pyramid(const uint8_t* gray, int rows, int cols, size_t gray_pitch, uint8_t* pyr, const OrbLevelTable& t,
                         cudaStream_t s);
-void hamming_best2(int device, const uint8_t* query, int nq, const uint8_t* train, int nt, const int* cand_off, const int* cand_idx,
-                   const int* train_level, int* out5);
 // the cells score their own pixels from `pyr`
 void orb_launch_cells(const uint8_t* pyr, const OrbLevelTable& t, const OrbCell* cells, int ncells, int ini_th,
                       int min_th, int* cell_count, uint32_t* cell_items, cudaStream_t s);
@@ -87,42 +85,6 @@ void orb_launch_distribute(const uint32_t* cand, const int* level_off, const uin
                            const OrbTreeParams& prm, int nlevels, uint32_t* sel_packed, int* level_count, int* error, cudaStream_t s);
 void orb_tree_configure();  // raises k_distribute's dynamic shared-memory limit on the current device
 void orb_upload_pattern();  // copies the rBRIEF pair table into constant memory (once per device)
-
-// Per-thread, per-device workspace of the host-buffer stereo / Hamming / information-selection entry points: one arena that only
-// grows and one non-blocking stream (stereo.cu).  Each such call takes its buffers after begin() and synchronises before it
-// returns, so the calls of one thread share it.
-// (Allocating and freeing half a dozen buffers per call and running on the legacy default stream synchronises the whole device,
-// i.e. serialises every per-frame call against the SegNet graph and the extractors' streams.)
-struct StereoWs {
-  int device = -1;
-  cudaStream_t stream = nullptr;
-  DevBuf arena;
-  size_t used = 0;
-  void begin(int dev, size_t bytes_needed) {
-    SIVO_CUDA(cudaSetDevice(dev));
-    if (device != dev) {
-      if (stream) { cudaSetDevice(device); cudaStreamDestroy(stream); cudaSetDevice(dev); }
-      arena.release();
-      SIVO_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
-      device = dev;
-    }
-    if (arena.bytes < bytes_needed) {
-      SIVO_CUDA(cudaStreamSynchronize(stream));
-      arena.alloc(bytes_needed + bytes_needed / 2);
-    }
-    used = 0;
-  }
-  template <class T> T* take(size_t count) {
-    used = (used + 255) & ~static_cast<size_t>(255);
-    T* p = reinterpret_cast<T*>(arena.as<uint8_t>() + used);
-    used += std::max<size_t>(count, 1) * sizeof(T);
-    if (used > arena.bytes) fail(SIVO_ENOMEM, "stereo workspace accounting");
-    return p;
-  }
-  ~StereoWs() { if (stream) { cudaSetDevice(device); cudaStreamDestroy(stream); } }
-};
-StereoWs& stereo_ws();
-inline size_t pad256(size_t b) { return (std::max<size_t>(b, 1) + 255) & ~static_cast<size_t>(255); }
 
 // ---- host (orb_host.cu)
 struct OrbTables {

@@ -13,7 +13,8 @@
 #include <cfloat>
 #include <cmath>
 
-#include "orb.h"
+#include "frame_ops.h"
+#include "host_call.h"
 
 namespace sivo {
 namespace {
@@ -633,6 +634,13 @@ void launch_optimize(const PoseParams& p, const sivo_keypoint* kps, const int* k
   k_pose_optimize<<<1, kThreads, 0, s>>>(p, kps, keep_idx, n_keep, cap, u_right, xw, Tcw_in, edges, result, outlier);
   SIVO_CUDA(cudaGetLastError());
 }
+
+// the host forms refuse a key that has a point (xw not NaN) and an octave outside the extractor's levels
+void check_octaves(const char* who, const sivo_keypoint* kps, const float* xw, int n, int nlevels) {
+  for (int j = 0; j < n; ++j)
+    if (!std::isnan(xw[3 * j]) && (kps[j].octave < 0 || kps[j].octave >= nlevels))
+      fail(SIVO_ERANGE, "%s: key %d has octave %d", who, j, kps[j].octave);
+}
 }  // namespace
 
 void pose_optimize_device(const Orb& left, const sivo_keypoint* kps, const int* keep_idx, const long long* n_keep, const float* u_right,
@@ -661,34 +669,22 @@ void pose_optimize(const Orb& left, const sivo_keypoint* kps, const float* u_rig
                    float cy, float mbf, const float* Tcw_in, sivo_pose_result* result, uint8_t* outlier) {
   if (n < 0) fail(SIVO_EINVAL, "pose: n = %d", n);
   const PoseParams p = make_params(left, fx, fy, cx, cy, mbf);
-  for (int j = 0; j < n; ++j)
-    if (!std::isnan(xw[3 * j]) && (kps[j].octave < 0 || kps[j].octave >= p.nlevels))
-      fail(SIVO_ERANGE, "pose: key %d has octave %d", j, kps[j].octave);
-  StereoWs& ws = stereo_ws();
-  ws.begin(left.device(), pad256(n * sizeof(sivo_keypoint)) + pad256(n * sizeof(float)) + pad256(3 * sizeof(float) * n) +
-                              pad256(12 * sizeof(float)) + pad256(sizeof(sivo_pose_result)) + pad256(n) + pad256(sizeof(long long)) +
-                              pad256(edges_bytes(n)) + 4096);
-  cudaStream_t st = ws.stream;
-  sivo_keypoint* d_kps = ws.take<sivo_keypoint>(n);
-  float* d_ur = ws.take<float>(n);
-  float* d_xw = ws.take<float>(3 * static_cast<size_t>(n));
-  float* d_T = ws.take<float>(12);
-  sivo_pose_result* d_res = ws.take<sivo_pose_result>(1);
-  uint8_t* d_out = ws.take<uint8_t>(n);
-  long long* d_count = ws.take<long long>(1);
-  PoseEdge* d_edges = reinterpret_cast<PoseEdge*>(ws.take<uint8_t>(edges_bytes(n)));
+  check_octaves("pose", kps, xw, n, p.nlevels);
+  HostCall& hc = host_call();
+  hc.begin(left.device());
+  const sivo_keypoint* d_kps = hc.upload(kps, n);
+  const float* d_ur = hc.upload(u_right, n);
+  const float* d_xw = hc.upload(xw, 3 * static_cast<size_t>(n));
+  const float* d_T = hc.upload(Tcw_in, 12);
   const long long count = n;
-  if (n) {
-    SIVO_CUDA(cudaMemcpyAsync(d_kps, kps, n * sizeof(sivo_keypoint), cudaMemcpyHostToDevice, st));
-    SIVO_CUDA(cudaMemcpyAsync(d_ur, u_right, n * sizeof(float), cudaMemcpyHostToDevice, st));
-    SIVO_CUDA(cudaMemcpyAsync(d_xw, xw, 3 * sizeof(float) * n, cudaMemcpyHostToDevice, st));
-  }
-  SIVO_CUDA(cudaMemcpyAsync(d_T, Tcw_in, 12 * sizeof(float), cudaMemcpyHostToDevice, st));
-  SIVO_CUDA(cudaMemcpyAsync(d_count, &count, sizeof(long long), cudaMemcpyHostToDevice, st));
-  launch_optimize(p, d_kps, nullptr, d_count, n, d_ur, d_xw, d_T, d_edges, d_res, d_out, st);
-  SIVO_CUDA(cudaMemcpyAsync(result, d_res, sizeof(sivo_pose_result), cudaMemcpyDeviceToHost, st));
-  if (outlier && n) SIVO_CUDA(cudaMemcpyAsync(outlier, d_out, n, cudaMemcpyDeviceToHost, st));
-  SIVO_CUDA(cudaStreamSynchronize(st));
+  const long long* d_count = hc.upload(&count, 1);
+  sivo_pose_result* d_res = hc.take<sivo_pose_result>(1);
+  uint8_t* d_out = hc.take<uint8_t>(n);
+  PoseEdge* d_edges = reinterpret_cast<PoseEdge*>(hc.take<uint8_t>(edges_bytes(n)));
+  launch_optimize(p, d_kps, nullptr, d_count, n, d_ur, d_xw, d_T, d_edges, d_res, d_out, hc.stream);
+  hc.download(result, d_res, 1);
+  hc.download(outlier, d_out, n);
+  hc.sync();
 }
 
 void pose_system(const Orb& left, const sivo_keypoint* kps, const float* u_right, const float* xw, int n, float fx, float fy, float cx,
@@ -696,43 +692,29 @@ void pose_system(const Orb& left, const sivo_keypoint* kps, const float* u_right
                  double* jac, double* H, double* b, double* chi) {
   if (n < 0) fail(SIVO_EINVAL, "pose_system: n = %d", n);
   const PoseParams p = make_params(left, fx, fy, cx, cy, mbf);
-  for (int j = 0; j < n; ++j)
-    if (!std::isnan(xw[3 * j]) && (kps[j].octave < 0 || kps[j].octave >= p.nlevels))
-      fail(SIVO_ERANGE, "pose_system: key %d has octave %d", j, kps[j].octave);
-  StereoWs& ws = stereo_ws();
-  ws.begin(left.device(), pad256(n * sizeof(sivo_keypoint)) + pad256(n * sizeof(float)) + pad256(3 * sizeof(float) * n) + pad256(n) +
-                              pad256(7 * sizeof(double)) + pad256(24 * sizeof(double) * n) + pad256(43 * sizeof(double)) +
-                              pad256(edges_bytes(n)) + 4096);
-  cudaStream_t st = ws.stream;
-  sivo_keypoint* d_kps = ws.take<sivo_keypoint>(n);
-  float* d_ur = ws.take<float>(n);
-  float* d_xw = ws.take<float>(3 * static_cast<size_t>(n));
-  uint8_t* d_l1 = ws.take<uint8_t>(n);
-  double* d_pose = ws.take<double>(7);
-  double* d_per = ws.take<double>(24 * static_cast<size_t>(n));
-  double* d_Hb = ws.take<double>(43);
-  PoseEdge* d_edges = reinterpret_cast<PoseEdge*>(ws.take<uint8_t>(edges_bytes(n)));
-  if (n) {
-    SIVO_CUDA(cudaMemcpyAsync(d_kps, kps, n * sizeof(sivo_keypoint), cudaMemcpyHostToDevice, st));
-    SIVO_CUDA(cudaMemcpyAsync(d_ur, u_right, n * sizeof(float), cudaMemcpyHostToDevice, st));
-    SIVO_CUDA(cudaMemcpyAsync(d_xw, xw, 3 * sizeof(float) * n, cudaMemcpyHostToDevice, st));
-    if (level1) SIVO_CUDA(cudaMemcpyAsync(d_l1, level1, n, cudaMemcpyHostToDevice, st));
-  }
-  SIVO_CUDA(cudaMemcpyAsync(d_pose, pose7, 7 * sizeof(double), cudaMemcpyHostToDevice, st));
+  check_octaves("pose_system", kps, xw, n, p.nlevels);
+  HostCall& hc = host_call();
+  hc.begin(left.device());
+  const sivo_keypoint* d_kps = hc.upload(kps, n);
+  const float* d_ur = hc.upload(u_right, n);
+  const float* d_xw = hc.upload(xw, 3 * static_cast<size_t>(n));
+  const uint8_t* d_l1 = hc.upload(level1, n);
+  const double* d_pose = hc.upload(pose7, 7);
+  double* d_per = hc.take<double>(24 * static_cast<size_t>(n));
+  double* d_Hb = hc.take<double>(43);
+  PoseEdge* d_edges = reinterpret_cast<PoseEdge*>(hc.take<uint8_t>(edges_bytes(n)));
   double *d_err = d_per, *d_chi2 = d_per + 3 * static_cast<size_t>(n), *d_rho = d_per + 4 * static_cast<size_t>(n),
          *d_jac = d_per + 6 * static_cast<size_t>(n);
-  k_pose_system<<<1, kThreads, 0, st>>>(p, d_kps, n, d_ur, d_xw, level1 ? d_l1 : nullptr, d_pose, robust_stereo, d_edges, d_err, d_chi2,
-                                        d_rho, d_jac, d_Hb);
+  k_pose_system<<<1, kThreads, 0, hc.stream>>>(p, d_kps, n, d_ur, d_xw, level1 ? d_l1 : nullptr, d_pose, robust_stereo, d_edges, d_err,
+                                               d_chi2, d_rho, d_jac, d_Hb);
   SIVO_CUDA(cudaGetLastError());
   double Hb[43];
-  if (n) {
-    if (err) SIVO_CUDA(cudaMemcpyAsync(err, d_err, 3 * sizeof(double) * n, cudaMemcpyDeviceToHost, st));
-    if (chi2) SIVO_CUDA(cudaMemcpyAsync(chi2, d_chi2, sizeof(double) * n, cudaMemcpyDeviceToHost, st));
-    if (rho) SIVO_CUDA(cudaMemcpyAsync(rho, d_rho, 2 * sizeof(double) * n, cudaMemcpyDeviceToHost, st));
-    if (jac) SIVO_CUDA(cudaMemcpyAsync(jac, d_jac, 18 * sizeof(double) * n, cudaMemcpyDeviceToHost, st));
-  }
-  SIVO_CUDA(cudaMemcpyAsync(Hb, d_Hb, sizeof(Hb), cudaMemcpyDeviceToHost, st));
-  SIVO_CUDA(cudaStreamSynchronize(st));
+  hc.download(err, d_err, 3 * static_cast<size_t>(n));
+  hc.download(chi2, d_chi2, n);
+  hc.download(rho, d_rho, 2 * static_cast<size_t>(n));
+  hc.download(jac, d_jac, 18 * static_cast<size_t>(n));
+  hc.download(Hb, d_Hb, 43);
+  hc.sync();
   if (H) for (int i = 0; i < 36; ++i) H[i] = Hb[i];
   if (b) for (int i = 0; i < 6; ++i) b[i] = Hb[36 + i];
   if (chi) *chi = Hb[42];

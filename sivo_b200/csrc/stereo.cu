@@ -3,8 +3,9 @@
 // [floor(vR - 2 s), ceil(vR + 2 s)] must contain int(vL), octave within +-1, uR in [uL - maxD, uL - minD];
 // distance = ORBmatcher::DescriptorDistance (ORBmatcher.cc:1582-1596) as 4 x __popcll.  The reference keeps
 // the first strictly smaller distance walking candidates in increasing iR, i.e. (min dist, min iR).
+#include "frame_ops.h"
+#include "host_call.h"
 #include "match_fold.cuh"
-#include "orb.h"
 
 namespace sivo {
 namespace {
@@ -247,11 +248,16 @@ void launch_stereo(const Orb& left, const Orb& right, const sivo_keypoint* kl, c
   SIVO_CUDA(cudaGetLastError());
 }
 
+void check_octaves(const sivo_keypoint* left, int nl, const sivo_keypoint* right, int nr, int nlevels) {
+  for (int i = 0; i < nl; ++i) if (left[i].octave < 0 || left[i].octave >= nlevels) fail(SIVO_EINVAL, "stereo: left octave out of range");
+  for (int i = 0; i < nr; ++i) if (right[i].octave < 0 || right[i].octave >= nlevels) fail(SIVO_EINVAL, "stereo: right octave out of range");
+}
+
 }  // namespace
 
-StereoWs& stereo_ws() {
-  static thread_local StereoWs ws;
-  return ws;
+HostCall& host_call() {
+  static thread_local HostCall hc;
+  return hc;
 }
 
 void stereo_hamming(int device, const sivo_keypoint* left, const uint8_t* dl, int nl, const sivo_keypoint* right,
@@ -259,31 +265,22 @@ void stereo_hamming(int device, const sivo_keypoint* left, const uint8_t* dl, in
                     int* best_idx, int* best_dist) {
   if (nl < 0 || nr < 0 || nr >= (1 << 20)) fail(SIVO_EINVAL, "stereo: bad keypoint counts %d / %d", nl, nr);
   if (nl == 0) return;
-  for (int i = 0; i < nl; ++i) if (left[i].octave < 0 || left[i].octave >= nlevels) fail(SIVO_EINVAL, "stereo: left octave out of range");
-  for (int i = 0; i < nr; ++i) if (right[i].octave < 0 || right[i].octave >= nlevels) fail(SIVO_EINVAL, "stereo: right octave out of range");
-  StereoWs& ws = stereo_ws();
-  ws.begin(device, pad256(nl * sizeof(sivo_keypoint)) + pad256(static_cast<size_t>(nl) * 32) + pad256(nr * sizeof(sivo_keypoint)) +
-                       pad256(static_cast<size_t>(nr) * 32) + pad256(nlevels * sizeof(float)) + 2 * pad256(nl * sizeof(int)) + 4096);
-  cudaStream_t st = ws.stream;
-  sivo_keypoint* d_kl = ws.take<sivo_keypoint>(nl);
-  uint8_t* d_dl = ws.take<uint8_t>(static_cast<size_t>(nl) * 32);
-  sivo_keypoint* d_kr = ws.take<sivo_keypoint>(nr);
-  uint8_t* d_dr = ws.take<uint8_t>(static_cast<size_t>(nr) * 32);
-  float* d_sc = ws.take<float>(nlevels);
-  int* d_bi = ws.take<int>(nl);
-  int* d_bd = ws.take<int>(nl);
-  SIVO_CUDA(cudaMemcpyAsync(d_kl, left, nl * sizeof(sivo_keypoint), cudaMemcpyHostToDevice, st));
-  SIVO_CUDA(cudaMemcpyAsync(d_dl, dl, static_cast<size_t>(nl) * 32, cudaMemcpyHostToDevice, st));
-  if (nr) {
-    SIVO_CUDA(cudaMemcpyAsync(d_kr, right, nr * sizeof(sivo_keypoint), cudaMemcpyHostToDevice, st));
-    SIVO_CUDA(cudaMemcpyAsync(d_dr, dr, static_cast<size_t>(nr) * 32, cudaMemcpyHostToDevice, st));
-  }
-  SIVO_CUDA(cudaMemcpyAsync(d_sc, scale, nlevels * sizeof(float), cudaMemcpyHostToDevice, st));
-  k_stereo_hamming<<<ceil_div(nl * 32, 128), 128, 0, st>>>(d_kl, d_dl, nl, d_kr, d_dr, nr, d_sc, nlevels, rows, min_d, max_d, d_bi, d_bd);
+  check_octaves(left, nl, right, nr, nlevels);
+  HostCall& hc = host_call();
+  hc.begin(device);
+  const sivo_keypoint* d_kl = hc.upload(left, nl);
+  const uint8_t* d_dl = hc.upload(dl, static_cast<size_t>(nl) * 32);
+  const sivo_keypoint* d_kr = hc.upload(right, nr);
+  const uint8_t* d_dr = hc.upload(dr, static_cast<size_t>(nr) * 32);
+  const float* d_sc = hc.upload(scale, nlevels);
+  int* d_bi = hc.take<int>(nl);
+  int* d_bd = hc.take<int>(nl);
+  k_stereo_hamming<<<ceil_div(nl * 32, 128), 128, 0, hc.stream>>>(d_kl, d_dl, nl, d_kr, d_dr, nr, d_sc, nlevels, rows, min_d, max_d, d_bi,
+                                                                  d_bd);
   SIVO_CUDA(cudaGetLastError());
-  SIVO_CUDA(cudaMemcpyAsync(best_idx, d_bi, nl * sizeof(int), cudaMemcpyDeviceToHost, st));
-  SIVO_CUDA(cudaMemcpyAsync(best_dist, d_bd, nl * sizeof(int), cudaMemcpyDeviceToHost, st));
-  SIVO_CUDA(cudaStreamSynchronize(st));
+  hc.download(best_idx, d_bi, nl);
+  hc.download(best_dist, d_bd, nl);
+  hc.sync();
 }
 
 // ---- best / second-best descriptor match over per-query candidate lists: the inner loop shared by
@@ -329,25 +326,18 @@ void hamming_best2(int device, const uint8_t* query, int nq, const uint8_t* trai
   for (int i = 0; i < nq; ++i) if (cand_off[i + 1] < cand_off[i]) fail(SIVO_EINVAL, "hamming_best2: candidate offsets must not decrease");
   const int nc = cand_off[nq];
   for (int i = 0; i < nc; ++i) if (cand_idx[i] < 0 || cand_idx[i] >= nt) fail(SIVO_ERANGE, "hamming_best2: candidate %d names train descriptor %d of %d", i, cand_idx[i], nt);
-  StereoWs& ws = stereo_ws();
-  ws.begin(device, pad256(static_cast<size_t>(nq) * 32) + pad256(static_cast<size_t>(nt) * 32) + pad256((nq + 1) * sizeof(int)) +
-                       pad256(nc * sizeof(int)) + pad256(nt * sizeof(int)) + pad256(static_cast<size_t>(nq) * 5 * sizeof(int)) + 4096);
-  cudaStream_t st = ws.stream;
-  uint8_t* d_q = ws.take<uint8_t>(static_cast<size_t>(nq) * 32);
-  uint8_t* d_t = ws.take<uint8_t>(static_cast<size_t>(nt) * 32);
-  int* d_off = ws.take<int>(nq + 1);
-  int* d_idx = ws.take<int>(nc);
-  int* d_lvl = ws.take<int>(nt);
-  int* d_out = ws.take<int>(static_cast<size_t>(nq) * 5);
-  SIVO_CUDA(cudaMemcpyAsync(d_q, query, static_cast<size_t>(nq) * 32, cudaMemcpyHostToDevice, st));
-  if (nt) SIVO_CUDA(cudaMemcpyAsync(d_t, train, static_cast<size_t>(nt) * 32, cudaMemcpyHostToDevice, st));
-  SIVO_CUDA(cudaMemcpyAsync(d_off, cand_off, (nq + 1) * sizeof(int), cudaMemcpyHostToDevice, st));
-  if (nc) SIVO_CUDA(cudaMemcpyAsync(d_idx, cand_idx, nc * sizeof(int), cudaMemcpyHostToDevice, st));
-  if (train_level && nt) SIVO_CUDA(cudaMemcpyAsync(d_lvl, train_level, nt * sizeof(int), cudaMemcpyHostToDevice, st));
-  k_hamming_best2<<<ceil_div(nq * 32, 128), 128, 0, st>>>(d_q, nq, d_t, d_off, d_idx, train_level ? d_lvl : nullptr, d_out);
+  HostCall& hc = host_call();
+  hc.begin(device);
+  const uint8_t* d_q = hc.upload(query, static_cast<size_t>(nq) * 32);
+  const uint8_t* d_t = hc.upload(train, static_cast<size_t>(nt) * 32);
+  const int* d_off = hc.upload(cand_off, nq + 1);
+  const int* d_idx = hc.upload(cand_idx, nc);
+  const int* d_lvl = hc.upload(train_level, nt);
+  int* d_out = hc.take<int>(static_cast<size_t>(nq) * 5);
+  k_hamming_best2<<<ceil_div(nq * 32, 128), 128, 0, hc.stream>>>(d_q, nq, d_t, d_off, d_idx, train_level ? d_lvl : nullptr, d_out);
   SIVO_CUDA(cudaGetLastError());
-  SIVO_CUDA(cudaMemcpyAsync(out5, d_out, static_cast<size_t>(nq) * 5 * sizeof(int), cudaMemcpyDeviceToHost, st));
-  SIVO_CUDA(cudaStreamSynchronize(st));
+  hc.download(out5, d_out, static_cast<size_t>(nq) * 5);
+  hc.sync();
 }
 
 }  // namespace sivo
@@ -361,34 +351,25 @@ void stereo_match(const Orb& left, const Orb& right, const sivo_keypoint* kl, co
   if (nl < 0 || nr < 0 || nr >= (1 << 20) || !(mb > 0.f) || !(mbf > 0.f)) fail(SIVO_EINVAL, "stereo: bad arguments");
   for (int i = 0; i < nl; ++i) { u_right[i] = -1.f; depth[i] = -1.f; }
   if (nl == 0 || nr == 0) return;
-  const int nlev = left.nlevels();
-  for (int i = 0; i < nl; ++i) if (kl[i].octave < 0 || kl[i].octave >= nlev) fail(SIVO_EINVAL, "stereo: left octave out of range");
-  for (int i = 0; i < nr; ++i) if (kr[i].octave < 0 || kr[i].octave >= nlev) fail(SIVO_EINVAL, "stereo: right octave out of range");
-  StereoWs& ws = stereo_ws();
-  ws.begin(left.device(), pad256(nl * sizeof(sivo_keypoint)) + pad256(static_cast<size_t>(nl) * 32) + pad256(nr * sizeof(sivo_keypoint)) +
-                              pad256(static_cast<size_t>(nr) * 32) + pad256(2 * sizeof(long long)) + 3 * pad256(nl * sizeof(float)) + 4096);
-  cudaStream_t st = ws.stream;
-  sivo_keypoint* d_kl = ws.take<sivo_keypoint>(nl);
-  uint8_t* d_dl = ws.take<uint8_t>(static_cast<size_t>(nl) * 32);
-  sivo_keypoint* d_kr = ws.take<sivo_keypoint>(nr);
-  uint8_t* d_dr = ws.take<uint8_t>(static_cast<size_t>(nr) * 32);
-  long long* d_n = ws.take<long long>(2);
-  float* d_u = ws.take<float>(nl);
-  float* d_z = ws.take<float>(nl);
-  int* d_s = ws.take<int>(nl);
+  check_octaves(kl, nl, kr, nr, left.nlevels());
+  HostCall& hc = host_call();
+  hc.begin(left.device());
+  const sivo_keypoint* d_kl = hc.upload(kl, nl);
+  const uint8_t* d_dl = hc.upload(dl, static_cast<size_t>(nl) * 32);
+  const sivo_keypoint* d_kr = hc.upload(kr, nr);
+  const uint8_t* d_dr = hc.upload(dr, static_cast<size_t>(nr) * 32);
   const long long counts[2] = {nl, nr};
-  SIVO_CUDA(cudaMemcpyAsync(d_kl, kl, nl * sizeof(sivo_keypoint), cudaMemcpyHostToDevice, st));
-  SIVO_CUDA(cudaMemcpyAsync(d_dl, dl, static_cast<size_t>(nl) * 32, cudaMemcpyHostToDevice, st));
-  SIVO_CUDA(cudaMemcpyAsync(d_kr, kr, nr * sizeof(sivo_keypoint), cudaMemcpyHostToDevice, st));
-  SIVO_CUDA(cudaMemcpyAsync(d_dr, dr, static_cast<size_t>(nr) * 32, cudaMemcpyHostToDevice, st));
-  SIVO_CUDA(cudaMemcpyAsync(d_n, counts, sizeof(counts), cudaMemcpyHostToDevice, st));
+  const long long* d_n = hc.upload(counts, 2);
+  float* d_u = hc.take<float>(nl);
+  float* d_z = hc.take<float>(nl);
+  int* d_s = hc.take<int>(nl);
   // the pyramids were written on the two extractors' own streams; their synchronous run() has returned, so they are complete.
   // The SAD distances go to this call's workspace: the left extractor's scratch holds capacity() entries and belongs to its
   // device-form calls, which are not ordered with this one.
-  launch_stereo(left, right, d_kl, d_dl, nullptr, d_n, nl, d_kr, d_dr, d_n + 1, nr, mb, mbf, d_u, d_z, d_s, st);
-  SIVO_CUDA(cudaMemcpyAsync(u_right, d_u, nl * sizeof(float), cudaMemcpyDeviceToHost, st));
-  SIVO_CUDA(cudaMemcpyAsync(depth, d_z, nl * sizeof(float), cudaMemcpyDeviceToHost, st));
-  SIVO_CUDA(cudaStreamSynchronize(st));
+  launch_stereo(left, right, d_kl, d_dl, nullptr, d_n, nl, d_kr, d_dr, d_n + 1, nr, mb, mbf, d_u, d_z, d_s, hc.stream);
+  hc.download(u_right, d_u, nl);
+  hc.download(depth, d_z, nl);
+  hc.sync();
 }
 
 // ComputeStereoMatches on device-resident keypoints, descriptors and counts, enqueued on `s` (NULL: the left extractor's stream)

@@ -16,8 +16,9 @@
 //                      last-frame search then runs the rotation histogram and ComputeThreeMaxima.
 #include <cmath>
 
+#include "frame_ops.h"
+#include "host_call.h"
 #include "match_fold.cuh"
-#include "orb.h"
 
 namespace sivo {
 namespace {
@@ -505,36 +506,25 @@ void search_host(const Orb& left, bool last, const sivo_keypoint* kps, const uin
       if (!angle_ok(pts[i].angle)) fail(SIVO_ERANGE, "track: point %d has angle %g outside [0, 360]", i, pts[i].angle);
     }
   }
-  StereoWs& ws = stereo_ws();
-  ws.begin(left.device(), pad256(n * sizeof(sivo_keypoint)) + pad256(static_cast<size_t>(n) * 32) + 2 * pad256(n * sizeof(float)) +
-                              pad256(n) + pad256(n_points * sizeof(sivo_map_point)) + pad256(n_points) + pad256(n * sizeof(int)) +
-                              2 * pad256(sizeof(long long)) + scratch_bytes(n, n_points) + 4096);
-  cudaStream_t st = ws.stream;
-  sivo_keypoint* d_kps = ws.take<sivo_keypoint>(n);
-  uint8_t* d_desc = ws.take<uint8_t>(static_cast<size_t>(n) * 32);
-  float* d_ur = ws.take<float>(n);
-  uint8_t* d_blocked = blocked ? ws.take<uint8_t>(n) : nullptr;
-  sivo_map_point* d_pts = ws.take<sivo_map_point>(n_points);
-  uint8_t* d_view = ws.take<uint8_t>(n_points);
-  int* d_match = ws.take<int>(n);
-  long long* d_count = ws.take<long long>(1);
-  long long* d_nm = ws.take<long long>(1);
-  const TrackBufs b = carve(ws.take<uint8_t>(scratch_bytes(n, n_points)), n, n_points);
+  HostCall& hc = host_call();
+  hc.begin(left.device());
+  const sivo_keypoint* d_kps = hc.upload(kps, n);
+  const uint8_t* d_desc = hc.upload(desc, static_cast<size_t>(n) * 32);
+  const float* d_ur = hc.upload(u_right, n);
+  const uint8_t* d_blocked = blocked ? hc.upload(blocked, n) : nullptr;
+  const sivo_map_point* d_pts = hc.upload(pts, n_points);
   const long long count = n;
-  if (n) {
-    SIVO_CUDA(cudaMemcpyAsync(d_kps, kps, n * sizeof(sivo_keypoint), cudaMemcpyHostToDevice, st));
-    SIVO_CUDA(cudaMemcpyAsync(d_desc, desc, static_cast<size_t>(n) * 32, cudaMemcpyHostToDevice, st));
-    SIVO_CUDA(cudaMemcpyAsync(d_ur, u_right, n * sizeof(float), cudaMemcpyHostToDevice, st));
-    if (blocked) SIVO_CUDA(cudaMemcpyAsync(d_blocked, blocked, n, cudaMemcpyHostToDevice, st));
-  }
-  if (n_points) SIVO_CUDA(cudaMemcpyAsync(d_pts, pts, n_points * sizeof(sivo_map_point), cudaMemcpyHostToDevice, st));
-  SIVO_CUDA(cudaMemcpyAsync(d_count, &count, sizeof(long long), cudaMemcpyHostToDevice, st));
-  launch_search(p, d_kps, d_desc, nullptr, d_count, n, d_ur, d_blocked, d_pts, n_points, b, d_view, d_match, d_nm, st);
+  const long long* d_count = hc.upload(&count, 1);
+  uint8_t* d_view = hc.take<uint8_t>(n_points);
+  int* d_match = hc.take<int>(n);
+  long long* d_nm = hc.take<long long>(1);
+  const TrackBufs b = carve(hc.take<uint8_t>(scratch_bytes(n, n_points)), n, n_points);
+  launch_search(p, d_kps, d_desc, nullptr, d_count, n, d_ur, d_blocked, d_pts, n_points, b, d_view, d_match, d_nm, hc.stream);
   long long nm = 0;
-  if (in_view && n_points) SIVO_CUDA(cudaMemcpyAsync(in_view, d_view, n_points, cudaMemcpyDeviceToHost, st));
-  if (match && n) SIVO_CUDA(cudaMemcpyAsync(match, d_match, n * sizeof(int), cudaMemcpyDeviceToHost, st));
-  SIVO_CUDA(cudaMemcpyAsync(&nm, d_nm, sizeof(long long), cudaMemcpyDeviceToHost, st));
-  SIVO_CUDA(cudaStreamSynchronize(st));
+  hc.download(in_view, d_view, n_points);
+  hc.download(match, d_match, n);
+  hc.download(&nm, d_nm, 1);
+  hc.sync();
   if (n_matches) *n_matches = static_cast<int>(nm);
 }
 
@@ -597,40 +587,32 @@ void features_in_area(const Orb& left, const sivo_keypoint* kps, int n, const si
                       int* offsets, int* idx, int idx_cap) {
   if (n < 0 || nq < 0) fail(SIVO_EINVAL, "features_in_area: negative counts");
   const TrackParams p = make_params(left, f);
-  StereoWs& ws = stereo_ws();
-  ws.begin(left.device(), pad256(n * sizeof(sivo_keypoint)) + pad256(static_cast<size_t>(n) * 32) + pad256(n * sizeof(float)) +
-                              pad256(sizeof(long long)) + pad256(3 * sizeof(float) * nq) + pad256(2 * sizeof(int) * nq) +
-                              pad256((nq + 1) * sizeof(int)) + pad256(std::max(idx_cap, 0) * sizeof(int)) + scratch_bytes(n, 0) + 4096);
-  cudaStream_t st = ws.stream;
-  sivo_keypoint* d_kps = ws.take<sivo_keypoint>(n);
-  uint8_t* d_desc = ws.take<uint8_t>(static_cast<size_t>(n) * 32);
-  float* d_ur = ws.take<float>(n);
-  long long* d_count = ws.take<long long>(1);
-  float* d_xyr = ws.take<float>(3 * static_cast<size_t>(nq));
-  int* d_lv = ws.take<int>(2 * static_cast<size_t>(nq));
-  int* d_off = ws.take<int>(nq + 1);
-  int* d_idx = ws.take<int>(std::max(idx_cap, 0));
-  const TrackBufs b = carve(ws.take<uint8_t>(scratch_bytes(n, 0)), n, 0);
-  const long long count = n;
+  HostCall& hc = host_call();
+  hc.begin(left.device());
+  cudaStream_t st = hc.stream;
+  const sivo_keypoint* d_kps = hc.upload(kps, n);
+  uint8_t* d_desc = hc.take<uint8_t>(static_cast<size_t>(n) * 32);
+  float* d_ur = hc.take<float>(n);
   if (n) {
-    SIVO_CUDA(cudaMemcpyAsync(d_kps, kps, n * sizeof(sivo_keypoint), cudaMemcpyHostToDevice, st));
     SIVO_CUDA(cudaMemsetAsync(d_desc, 0, static_cast<size_t>(n) * 32, st));
     SIVO_CUDA(cudaMemsetAsync(d_ur, 0, n * sizeof(float), st));
   }
-  SIVO_CUDA(cudaMemcpyAsync(d_count, &count, sizeof(long long), cudaMemcpyHostToDevice, st));
-  if (nq) {
-    SIVO_CUDA(cudaMemcpyAsync(d_xyr, xyr, 3 * sizeof(float) * nq, cudaMemcpyHostToDevice, st));
-    SIVO_CUDA(cudaMemcpyAsync(d_lv, levels, 2 * sizeof(int) * nq, cudaMemcpyHostToDevice, st));
-  }
+  const long long count = n;
+  const long long* d_count = hc.upload(&count, 1);
+  const float* d_xyr = hc.upload(xyr, 3 * static_cast<size_t>(nq));
+  const int* d_lv = hc.upload(levels, 2 * static_cast<size_t>(nq));
+  int* d_off = hc.take<int>(nq + 1);
+  int* d_idx = hc.take<int>(std::max(idx_cap, 0));
+  const TrackBufs b = carve(hc.take<uint8_t>(scratch_bytes(n, 0)), n, 0);
   k_track_grid<<<1, kGridThreads, 0, st>>>(p, d_kps, d_desc, nullptr, d_count, n, d_ur, b);
   SIVO_CUDA(cudaGetLastError());
   std::vector<int> len(std::max(nq, 1));
   if (nq) {
     k_area_lists<<<ceil_div(nq * 32, 128), 128, 0, st>>>(p, b, d_xyr, d_lv, nq, nullptr, d_off);
     SIVO_CUDA(cudaGetLastError());
-    SIVO_CUDA(cudaMemcpyAsync(len.data(), d_off, nq * sizeof(int), cudaMemcpyDeviceToHost, st));
+    hc.download(len.data(), d_off, nq);
   }
-  SIVO_CUDA(cudaStreamSynchronize(st));
+  hc.sync();
   offsets[0] = 0;
   for (int q = 0; q < nq; ++q) offsets[q + 1] = offsets[q] + len[q];
   if (offsets[nq] > idx_cap) fail(SIVO_ERANGE, "features_in_area: %d candidates, room for %d", offsets[nq], idx_cap);
@@ -638,8 +620,8 @@ void features_in_area(const Orb& left, const sivo_keypoint* kps, int n, const si
   SIVO_CUDA(cudaMemcpyAsync(d_off, offsets, (nq + 1) * sizeof(int), cudaMemcpyHostToDevice, st));
   k_area_lists<<<ceil_div(nq * 32, 128), 128, 0, st>>>(p, b, d_xyr, d_lv, nq, d_off, d_idx);
   SIVO_CUDA(cudaGetLastError());
-  SIVO_CUDA(cudaMemcpyAsync(idx, d_idx, offsets[nq] * sizeof(int), cudaMemcpyDeviceToHost, st));
-  SIVO_CUDA(cudaStreamSynchronize(st));
+  hc.download(idx, d_idx, offsets[nq]);
+  hc.sync();
 }
 
 }  // namespace sivo

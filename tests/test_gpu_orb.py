@@ -170,6 +170,30 @@ def test_hamming_best2_equals_the_sequential_loop():
     assert (got[:5] == np.array([-1, 256, -1, 256, -1])).all()
 
 
+def test_hamming_best2_on_a_fresh_thread_small_large_small():
+    """The host-call staging is per thread, so a new thread starts with none.  The first call is small; the second needs several
+    times what the first left behind, so it gets more device memory while its earlier buffers are in use; the third runs on what
+    the second's pieces were merged into.  Each result equals the sequential loop."""
+    from sivo_b200.orb import hamming_best2
+    rng = np.random.default_rng(12)
+    cases = []
+    for nq, nt, max_len in ((20, 50, 8), (3000, 40000, 20), (20, 50, 8)):
+        train = rng.integers(0, 256, size=(nt, 32), dtype=np.uint8)
+        query = train[rng.integers(0, nt, nq)] ^ rng.integers(0, 256, size=(nq, 32), dtype=np.uint8) * (rng.random((nq, 32)) < 0.1)
+        level = rng.integers(0, 8, nt).astype(np.int32)
+        lens = rng.integers(0, max_len, nq)
+        off = np.concatenate([[0], np.cumsum(lens)]).astype(np.int32)
+        cand = rng.integers(0, nt, off[-1]).astype(np.int32)
+        cases.append((query, train, off, cand, level))
+    got = []
+    t = threading.Thread(target=lambda: got.extend(hamming_best2(*c) for c in cases))
+    t.start()
+    t.join()
+    assert len(got) == len(cases)
+    for c, g in zip(cases, got):
+        assert np.array_equal(g, O.hamming_best2(*c))
+
+
 def gpu_tree(xs, ys, rs, min_x, max_x, min_y, max_y, tgt):
     import ctypes as C
     from sivo_b200 import _lib as L
