@@ -26,6 +26,9 @@
 //    tap row between the next block's MMA commits, so they drain under the tensor core's work.
 //  * Constants (bias, BN, classifier weights) are kernel parameters: the epilogue reads them from the constant bank and
 //    leaves the shared-memory data path to the MMA operand reads.
+//  * The Cin = 64, 7x7 layers with 64-wide half output tiles (Basic's conv1 .. conv_decode2) run on k_conv_tn instead: the
+//    same producers and rings with the GEMM transposed -- the weights as M, all 128 pixels of a row as N -- and an
+//    epilogue staged through shared memory.
 //  * The 64 -> 16 float-logits layers (K = 3, 7) run on k_conv_stack instead: tap rows stacked along N, resident weights.
 //    Fed by a max-unpool (Basic's composed classifier), it unpools the pooled tensor as it loads its halo rows.
 #include <cuda.h>
@@ -437,8 +440,21 @@ __device__ __forceinline__ void epilogue_stage(const TcParams& p, const TcConsts
   }
 }
 
-// Issues the stores of staged chunk i (a compile-time index after unrolling): one 16-byte store, or four for unpool,
-// where each channel's value goes to the 2x2 position its mask byte names and zeros to the other three.
+// The max-unpool scatter of 8 channels (16 bytes `v`) of pixel (y, x): each channel's value goes to the 2x2 position of the
+// 2H x 2W output its mask byte (of `m`) names, zeros to the other three.
+__device__ __forceinline__ void unpool_store8(const TcParams& p, int img, int y, int x, int c, uint4 v, uint2 m) {
+  __half* const ob = static_cast<__half*>(p.out) + ((static_cast<size_t>(img) * 2 * p.H + 2 * y) * (2 * p.W) + 2 * x) * p.cout_total + c;
+  const size_t row_step = static_cast<size_t>(2 * p.W) * p.cout_total;
+#pragma unroll
+  for (int pos = 0; pos < 4; ++pos) {
+    const uint32_t lo = __vcmpeq4(m.x, 0x01010101u * pos), hi = __vcmpeq4(m.y, 0x01010101u * pos);  // 0xFF per matching byte
+    const uint4 o = make_uint4(v.x & __byte_perm(lo, 0u, 0x1100), v.y & __byte_perm(lo, 0u, 0x3322),
+                               v.z & __byte_perm(hi, 0u, 0x1100), v.w & __byte_perm(hi, 0u, 0x3322));
+    *reinterpret_cast<uint4*>(ob + (pos >> 1) * row_step + (pos & 1) * p.cout_total) = o;
+  }
+}
+
+// Issues the stores of staged chunk i (a compile-time index after unrolling): one 16-byte store, or four for unpool.
 template <int N>
 __device__ __forceinline__ void epilogue_flush(const TcParams& p, const EpiStage<N>& e, int i, int x_m0, int n0, int q) {
   const int r = i / (2 * (N / 32)), h = (i / (N / 32)) & 1, J = i % (N / 32);
@@ -450,15 +466,7 @@ __device__ __forceinline__ void epilogue_flush(const TcParams& p, const EpiStage
   const int c = n0 + 8 * (4 * J + q);
   const uint4 v = e.v[i];
   if (p.unpool_mask) {
-    __half* const ob = static_cast<__half*>(p.out) + ((static_cast<size_t>(img) * 2 * p.H + 2 * y) * (2 * p.W) + 2 * x) * p.cout_total + c;
-    const size_t row_step = static_cast<size_t>(2 * p.W) * p.cout_total;
-#pragma unroll
-    for (int pos = 0; pos < 4; ++pos) {
-      const uint32_t lo = __vcmpeq4(e.m[i].x, 0x01010101u * pos), hi = __vcmpeq4(e.m[i].y, 0x01010101u * pos);  // 0xFF per matching byte
-      const uint4 o = make_uint4(v.x & __byte_perm(lo, 0u, 0x1100), v.y & __byte_perm(lo, 0u, 0x3322),
-                                 v.z & __byte_perm(hi, 0u, 0x1100), v.w & __byte_perm(hi, 0u, 0x3322));
-      *reinterpret_cast<uint4*>(ob + (pos >> 1) * row_step + (pos & 1) * p.cout_total) = o;
-    }
+    unpool_store8(p, img, y, x, c, v, e.m[i]);
   } else {
     *reinterpret_cast<uint4*>(static_cast<__half*>(p.out) + ((static_cast<size_t>(img) * p.H + y) * p.W + x) * p.cout_total + c) = v;
   }
@@ -477,54 +485,55 @@ __device__ __forceinline__ void epilogue_flush(const TcParams& p, const EpiStage
 //               A operand of tap (kh, kw) is an unshifted, fully populated tile.  3x the halo traffic, which these small layers
 //               have to spare; weights arrive in (kw, kh) order.
 // SPLIT: split-operand fp32 mode (see TcParams::split / seg_rows); N <= 64 so that the segment sums fit in registers.
-template <int K, bool ROLL, int KW, bool PK2, int N, bool SPLIT>
-__global__ void __launch_bounds__(kTcThreads, 1)
-k_conv_tc(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const __grid_constant__ TcParams p,
-          const __grid_constant__ TcConsts cst) {
-  static_assert(!PK2 || (!ROLL && KW == K), "image-pair tiles use the chunked kernel");
-  static_assert(!SPLIT || (!ROLL && N <= 64), "split mode: chunked kernel, segment sums in registers");
-  constexpr int RK = kRows + K - 1;                  // halo rows one row block reads (per chunk)
+//
+// TcCta: what k_conv_tc and k_conv_tn share -- the CTA's shared-memory carve-up (halo ring, weight ring, `stage_bytes` for the
+// consumers' epilogue staging, mbarriers), its place in the (strip, row block, cout tile, image) grid, and warpgroup 0's
+// producers that fill the two rings.
+template <int K, bool ROLL, int KW, bool PK2, int N>
+struct TcCta {
+  static constexpr int RK = kRows + K - 1;           // halo rows one row block reads (per chunk)
   // rows are released as soon as their last tap row retired; !ROLL double-buffers chunks where that fits (K = 7: RK + 2)
-  constexpr int kSlots = ROLL ? RK : (K == 7 ? RK + 2 : 2 * RK);
-  constexpr int kPad = (K - 1) / 2, kPadW = (KW - 1) / 2;
-  constexpr int F = N / 2;                           // accumulator registers per thread per output row
-  constexpr int b_bytes = N * 128;
-  constexpr int b_stride = (b_bytes + 1023) & ~1023;
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-  uint8_t* a_slots = smem;
-  uint8_t* b_stages = smem + kSlots * kSlotBytes;
-  const int kBStages = p.b_stages;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(b_stages + kBStages * b_stride);
-  uint64_t* a_full = bars;                       // [kSlots]
-  uint64_t* a_empty = a_full + kSlots;           // [kSlots]
-  uint64_t* b_full = a_empty + kSlots;           // [kBStages]
-  uint64_t* b_empty = b_full + kBStages;         // [kBStages]
+  static constexpr int kSlots = ROLL ? RK : (K == 7 ? RK + 2 : 2 * RK);
+  static constexpr int kPad = (K - 1) / 2, kPadW = (KW - 1) / 2;
+  static constexpr int b_bytes = N * 128;
+  static constexpr int b_stride = (b_bytes + 1023) & ~1023;
+  static constexpr int UPC = PK2 ? KW * RK : RK;     // halo units per (row block, chunk)
+  uint8_t *a_slots, *b_stages, *stage;
+  uint64_t *a_full, *a_empty, *b_full, *b_empty;   // [kSlots], [kSlots], [kBStages], [kBStages]
+  int kBStages, n0, img, x0, NC, npairs, y_base, n_units;
 
-  const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int strip = blockIdx.x % p.strips, rowblk = blockIdx.x / p.strips;
-  constexpr int UPC = PK2 ? KW * RK : RK;          // halo units per (row block, chunk)
-  const int n0 = blockIdx.y * N;
-  const int img = PK2 ? 2 * blockIdx.z : blockIdx.z;
-  const int x0 = strip * 128;
-  const int NC = ROLL ? 1 : p.chunks;
-  const int total_pairs = (p.H + kRows - 1) / kRows;
-  const int pair0 = rowblk * p.pairs_per_cta;
-  const int npairs = min(p.pairs_per_cta, total_pairs - pair0);
-  const int y_base = pair0 * kRows;              // first output row of this CTA
-  const int n_units = ROLL ? npairs * kRows + K - 1 : npairs * NC * UPC;
+  __device__ __forceinline__ TcCta(const TcParams& p, uint8_t* smem, int stage_bytes) {
+    a_slots = smem;
+    b_stages = smem + kSlots * kSlotBytes;
+    kBStages = p.b_stages;
+    stage = b_stages + kBStages * b_stride;
+    a_full = reinterpret_cast<uint64_t*>(stage + stage_bytes);
+    a_empty = a_full + kSlots;
+    b_full = a_empty + kSlots;
+    b_empty = b_full + kBStages;
+    const int strip = blockIdx.x % p.strips, rowblk = blockIdx.x / p.strips;
+    n0 = blockIdx.y * N;
+    img = PK2 ? 2 * blockIdx.z : blockIdx.z;
+    x0 = strip * 128;
+    NC = ROLL ? 1 : p.chunks;
+    const int total_pairs = (p.H + kRows - 1) / kRows;
+    const int pair0 = rowblk * p.pairs_per_cta;
+    npairs = min(p.pairs_per_cta, total_pairs - pair0);
+    y_base = pair0 * kRows;                          // first output row of this CTA
+    n_units = ROLL ? npairs * kRows + K - 1 : npairs * NC * UPC;
+  }
 
-  if (threadIdx.x == 0) {
+  __device__ __forceinline__ void init_barriers() const {
     for (int i = 0; i < kSlots; ++i) { mbar_init(a_full + i, 1); mbar_init(a_empty + i, kEmptyArrivals); }
     for (int i = 0; i < kBStages; ++i) { mbar_init(b_full + i, 1); mbar_init(b_empty + i, kEmptyArrivals); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
-  __syncthreads();
 
-  if (wg == 0) {
-    // 384 threads start with 168 registers each; the producers need few, the consumers (2 rows x N/2 accumulators, the
-    // split sums, the epilogue's packed outputs) many: 128 x 40 + 256 x 232 = 64 512 <= 65 536
+  // Warpgroup 0: warp 0 streams the halo rows, warp 1 the weight tiles; the other producer threads have nothing to do.
+  __device__ __forceinline__ void produce(const CUtensorMap& map_a, const CUtensorMap& map_b, const TcParams& p, int warp, int lane) const {
+    // 384 threads start with 168 registers each; the producers need few, the consumers (the accumulators, the split sums,
+    // the epilogue's packed outputs) many: 128 x 40 + 256 x 232 = 64 512 <= 65 536
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
     if (warp == 0 && lane == 0) {
       // ===== halo-row producer =====
@@ -571,8 +580,34 @@ k_conv_tc(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUt
             }
         }
     }
+  }
+};
+
+__device__ __forceinline__ uint8_t* tc_smem_base() {
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  return reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
+}
+
+template <int K, bool ROLL, int KW, bool PK2, int N, bool SPLIT>
+__global__ void __launch_bounds__(kTcThreads, 1)
+k_conv_tc(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const __grid_constant__ TcParams p,
+          const __grid_constant__ TcConsts cst) {
+  static_assert(!PK2 || (!ROLL && KW == K), "image-pair tiles use the chunked kernel");
+  static_assert(!SPLIT || (!ROLL && N <= 64), "split mode: chunked kernel, segment sums in registers");
+  using Cta = TcCta<K, ROLL, KW, PK2, N>;
+  constexpr int RK = Cta::RK, kSlots = Cta::kSlots, b_stride = Cta::b_stride;
+  constexpr int F = N / 2;                           // accumulator registers per thread per output row
+  const Cta cta(p, tc_smem_base(), 0);
+  const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (threadIdx.x == 0) cta.init_barriers();
+  __syncthreads();
+  if (wg == 0) {
+    cta.produce(map_a, map_b, p, warp, lane);
     return;
   }
+  const int kBStages = cta.kBStages, n0 = cta.n0, img = cta.img, x0 = cta.x0, NC = cta.NC, npairs = cta.npairs;
+  const int y_base = cta.y_base, n_units = cta.n_units;
+  uint64_t *const a_full = cta.a_full, *const a_empty = cta.a_empty, *const b_full = cta.b_full, *const b_empty = cta.b_empty;
 
   asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
   // ===== consumers: warpgroup g = wg - 1 owns tile rows (pixels) [64 g, 64 g + 64) =====
@@ -581,7 +616,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUt
   const int img_c = PK2 ? img + g : img;
   const int x_m0 = (PK2 ? 0 : x0 + 64 * g) + m0;
   // PK2: the second image's 64-pixel box sits 64 rows into the slot; otherwise pixel 64 g of the halo row is 64 g rows in
-  const uint32_t a_base = smem_u32(a_slots) + static_cast<uint32_t>(g * 64 * 128), b_base = smem_u32(b_stages);
+  const uint32_t a_base = smem_u32(cta.a_slots) + static_cast<uint32_t>(g * 64 * 128), b_base = smem_u32(cta.b_stages);
   const bool releaser = lane == 0;
   const int q = lane & 3;
   // N = 64 store / dropout / unpool epilogues are deferred: block j's outputs are staged in registers, and their stores go
@@ -706,6 +741,218 @@ k_conv_tc(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUt
   } else {
     walk(std::false_type{});
   }
+}
+
+// k_conv_tn: the Cin = 64 -> 64-wide half convolutions of k_conv_tc<K, true, KW, false, 64> with the GEMM transposed
+// (run for K = 7, see tc_is_tn).
+// There, each consumer's m64n64k16 reads a 2 KB pixel tile and a 2 KB weight tile for 64 K multiply-adds: 0.0625 B of
+// shared-memory operand reads per MAC.  Here D^T[64 cout x 128 px] = W[64 cout x 16 cin] * X^T[16 cin x 128 px] is ONE
+// m64n128k16 per (output row, tap, K step): 2 KB of weights + 4 KB of pixels, 0.047 B per MAC.  No layout changes: the
+// weight stage [cout][cin] is a K-major A tile as it is, and a halo row [px][64 cin] a K-major B tile with N = 128 pixels,
+// shifted by kw pixels through its start address (the swizzle phase follows the absolute address, see make_desc).
+//  * Producers, rings and row-block walk: TcCta<K, true, KW, false, 64>, as k_conv_tc.
+//  * Consumer g computes output row y0 + g of every block: 128 pixels x 64 couts, 64 fp32 accumulators per thread
+//    (d[4 j + 2 h + e] = cout 16 warp + lane / 4 + 8 h, pixel 8 j + 2 (lane % 4) + e).  Per output element the adds run in
+//    k_conv_tc's order -- tap row, tap column, K step, onto a zeroed accumulator -- so the results are the same bits.
+//  * Epilogue through shared memory: bias / BN / ReLU -> half, then stmatrix .trans into a [2 rows][128 px][64 ch] staging
+//    tile in SWIZZLE_128B chunk order (one 16-byte chunk = 8 channels of a pixel).  Once both rows are there (named barrier
+//    over the two consumers) the stores go out in 16-byte units (pixel, 8 channels), one slice per tap row of the next
+//    block right after its first MMA group is committed, the last block's at the end: a store, dropout (keep bits drawn
+//    once per pixel), the max-unpool scatter, or 2x2 max-pool + argmax over four staged pixels.  A second barrier before
+//    the next staging keeps the single tile safe.
+constexpr int kTnStageBytes = kRows * 128 * 128;  // [kRows][128 px][64 ch] half
+constexpr int kTnUnits = kRows * 128 * 8 / 256;   // 16-byte store units per consumer thread per block (2x2 pool: 2)
+
+__device__ __forceinline__ void stmatrix_x4_trans(uint32_t addr, const uint32_t (&r)[4]) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r[0]), "r"(r[1]), "r"(r[2]),
+               "r"(r[3])
+               : "memory");
+}
+__device__ __forceinline__ uint4 lds128(uint32_t addr) {
+  uint4 v;
+  asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
+  return v;
+}
+__device__ __forceinline__ void consumers_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }  // warpgroups 1 and 2
+// staged chunk c (channels 8 c .. 8 c + 7 of the tile) of pixel px, output row r of the block
+__device__ __forceinline__ uint32_t tn_chunk(uint32_t s_base, int r, int px, int c) {
+  return s_base + static_cast<uint32_t>(r * (128 * 128) + px * 128 + ((c ^ (px & 7)) << 4));
+}
+// dropout on two staged halves: y = x * keep * scale (exact); `kb` holds the keep bits of the chunk's 8 channels
+__device__ __forceinline__ uint32_t drop_word(uint32_t w, uint32_t kb, int k, float scale) {
+  __half2 hv = *reinterpret_cast<const __half2*>(&w);
+  hv = __hmul2(hv, __floats2half2_rn((kb >> (2 * k)) & 1u ? scale : 0.f, (kb >> (2 * k + 1)) & 1u ? scale : 0.f));
+  return *reinterpret_cast<const uint32_t*>(&hv);
+}
+
+template <int F>
+__device__ __forceinline__ void fence_acc(float (&d)[F]) {
+#pragma unroll
+  for (int i = 0; i < F; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+template <int K, int KW>
+__global__ void __launch_bounds__(kTcThreads, 1)
+k_conv_tn(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const __grid_constant__ TcParams p,
+          const __grid_constant__ TcConsts cst) {
+  using Cta = TcCta<K, true, KW, false, 64>;
+  constexpr int kSlots = Cta::kSlots, b_stride = Cta::b_stride;
+  static_assert(K >= kRows, "a block's own halo rows are released by its tap rows kh < kRows");
+  const Cta cta(p, tc_smem_base(), kTnStageBytes);
+  const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (threadIdx.x == 0) cta.init_barriers();
+  __syncthreads();
+  if (wg == 0) {
+    cta.produce(map_a, map_b, p, warp, lane);
+    return;
+  }
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+  const int g = wg - 1;             // output row y0 + g of every block
+  const int t = threadIdx.x - 128;  // consumer thread
+  const int n0 = cta.n0, img = cta.img, x0 = cta.x0, kBStages = cta.kBStages;
+  const uint32_t a_base = smem_u32(cta.a_slots), b_base = smem_u32(cta.b_stages), s_base = smem_u32(cta.stage);
+  const bool releaser = lane == 0;
+  const int c_lo = n0 + 16 * (warp & 3) + (lane >> 2);  // this thread's couts (rows of D^T): c_lo, c_lo + 8
+
+  // The staged block: its first row, and per store unit i of this thread -- chunk t % 8 of pixel t / 8 + 32 (i % 4) of
+  // row i / 4 (pool: pooled pixel t / 8 + 32 i) -- the unpool mask bytes.  Lane l draws the dropout keep bits of the
+  // pixel of unit l / 4 of lane 8 (l % 4) (two words: the tile's 64 channels) and shuffles them to its owners.
+  int ys = 0;
+  bool pending = false;
+  uint2 mk[kTnUnits] = {};
+  uint32_t keep[2] = {0xFFFFFFFFu, 0xFFFFFFFFu};
+  const int c = t & 7;
+  auto flush_store = [&](int i) {
+    const int px = (t >> 3) + 32 * (i & 3), y = ys + (i >> 2), x = x0 + px;
+    uint4 v = lds128(tn_chunk(s_base, i >> 2, px, c));
+    if (p.has_drop) {
+      const int src = 4 * i + (lane >> 3);
+      const uint32_t k0 = __shfl_sync(0xffffffffu, keep[0], src), k1 = __shfl_sync(0xffffffffu, keep[1], src);
+      const uint32_t kb = ((c >> 2) ? k1 : k0) >> (8 * (c & 3));
+      v = make_uint4(drop_word(v.x, kb, 0, p.drop_scale), drop_word(v.y, kb, 1, p.drop_scale), drop_word(v.z, kb, 2, p.drop_scale),
+                     drop_word(v.w, kb, 3, p.drop_scale));
+    }
+    if (!(y < p.H && x < p.W)) return;
+    if (p.unpool_mask) unpool_store8(p, img, y, x, n0 + 8 * c, v, mk[i]);
+    else *reinterpret_cast<uint4*>(static_cast<__half*>(p.out) + ((static_cast<size_t>(img) * p.H + y) * p.W + x) * p.cout_total + n0 + 8 * c) = v;
+  };
+  auto flush_pool = [&](int i) {  // window in scan order: (y, x), (y, x+1), (y+1, x), (y+1, x+1); strict '>', first maximum wins
+    const int pp = (t >> 3) + 32 * i, x = x0 + 2 * pp;
+    const uint4 a = lds128(tn_chunk(s_base, 0, 2 * pp, c)), b = lds128(tn_chunk(s_base, 0, 2 * pp + 1, c));
+    const uint4 cc = lds128(tn_chunk(s_base, 1, 2 * pp, c)), d = lds128(tn_chunk(s_base, 1, 2 * pp + 1, c));
+    const uint32_t av[4] = {a.x, a.y, a.z, a.w}, bv[4] = {b.x, b.y, b.z, b.w}, cv[4] = {cc.x, cc.y, cc.z, cc.w}, dv[4] = {d.x, d.y, d.z, d.w};
+    uint32_t best[4], arg[4];
+#pragma unroll
+    for (int w = 0; w < 4; ++w) {  // two channels per word
+      best[w] = av[w];
+      arg[w] = 0;
+      const uint32_t cand[3] = {bv[w], cv[w], dv[w]};
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        const uint32_t sel = __hgt2_mask(*reinterpret_cast<const __half2*>(&cand[k]), *reinterpret_cast<const __half2*>(&best[w]));
+        best[w] = (best[w] & ~sel) | (cand[k] & sel);
+        const uint32_t selb = __byte_perm(sel, 0u, 0x4420);  // the two half masks as two byte masks (bytes 0 and 1)
+        arg[w] = (arg[w] & ~selb) | ((0x0101u * static_cast<uint32_t>(k + 1)) & selb);
+      }
+    }
+    if (ys + 1 < p.H && x + 1 < p.W) {
+      const size_t o = ((static_cast<size_t>(img) * (p.H >> 1) + (ys >> 1)) * (p.W >> 1) + (x >> 1)) * p.cout_total + n0 + 8 * c;
+      *reinterpret_cast<uint4*>(p.pool_out + o) = make_uint4(best[0], best[1], best[2], best[3]);
+      *reinterpret_cast<uint2*>(p.pool_mask + o) = make_uint2(arg[0] | (arg[1] << 16), arg[2] | (arg[3] << 16));
+    }
+  };
+  // the staged block's units that go out during tap row kh: every unit during the K tap rows
+  auto flush_slice = [&](int kh) {
+    if (p.has_drop && kh == 0) {
+      const int i = lane >> 2, px = (t >> 5) * 4 + (lane & 3) + 32 * (i & 3), y = ys + (i >> 2), x = x0 + px;
+      uint32_t bits[4];
+      dropout_bits128_nl(p.seed, *p.frame, p.drop_nl + img, static_cast<uint32_t>(y * p.W + x), n0 >> 7, bits);
+      keep[0] = (n0 & 64) ? bits[2] : bits[0];
+      keep[1] = (n0 & 64) ? bits[3] : bits[1];
+    }
+#pragma unroll
+    for (int i = 0; i < kTnUnits; ++i) {
+      if (p.pool_out) {
+        if (i < 2 && (i * K) / 2 == kh) flush_pool(i);
+      } else if ((i * K) / kTnUnits == kh) {
+        flush_store(i);
+      }
+    }
+  };
+
+  float acc[64];
+  int st = 0;
+  uint32_t b_phase = 0;
+  int waited = 0;  // halo units whose TMA has been observed
+  for (int j = 0; j < cta.npairs; ++j) {
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    const int base_u = j * kRows;
+    for (int kh = 0; kh < K; ++kh) {
+      while (waited <= base_u + kh + kRows - 1 && waited < cta.n_units) {
+        mbar_wait(cta.a_full + waited % kSlots, (waited / kSlots) & 1);
+        ++waited;
+      }
+      const uint32_t x_row = a_base + ((base_u + g + kh) % kSlots) * kSlotBytes;
+      int prev_st = -1;
+#pragma unroll
+      for (int kw = 0; kw < KW; ++kw) {
+        mbar_wait(cta.b_full + st, b_phase);
+        const uint32_t w_addr = b_base + st * b_stride;
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wgmma(acc, make_desc(w_addr + 32 * k), make_desc(x_row + kw * 128 + 32 * k));
+        wgmma_commit();
+        if (kw == 0 && pending) flush_slice(kh);
+        // keep one group in flight: the previous one has retired, so its weight stage goes back to the producer
+        wgmma_wait<1>();
+        if (prev_st >= 0 && releaser) mbar_arrive(cta.b_empty + prev_st);
+        prev_st = st;
+        if (++st == kBStages) { st = 0; b_phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      fence_acc(acc);
+      if (releaser) {
+        mbar_arrive(cta.b_empty + prev_st);
+        // k_conv_tc's release rule holds: consumer 1 reads halo row base_u + kh at tap row kh - 1, consumer 0 at tap row kh --
+        // one tap row earlier, never later -- so once both have passed tap row kh neither reads it again in this block, and
+        // rows >= kRows are the next block's (released by its tap rows)
+        if (kh < kRows) mbar_arrive(cta.a_empty + (base_u + kh) % kSlots);
+      }
+    }
+    consumers_sync();  // both consumers have flushed the previous block out of the staging tile
+    {
+      // lane l addresses row l % 8 of matrix l / 8 = (h, j) = (l / 8 % 2, 2 jp + l / 16): pixel 8 j + l % 8, chunk 2 warp + h
+      const int rr = lane & 7, h = (lane >> 3) & 1;
+      const uint32_t addr = s_base + static_cast<uint32_t>(g * (128 * 128) + (8 * (lane >> 4) + rr) * 128 + (((2 * (warp & 3) + h) ^ rr) << 4));
+#pragma unroll
+      for (int jp = 0; jp < 8; ++jp) {
+        uint32_t r4[4];
+#pragma unroll
+        for (int m = 0; m < 4; ++m) {
+          const int mh = m & 1, mj = 2 * jp + (m >> 1);
+          const __half2 hv = __floats2half2_rn(affine(p, cst, acc[4 * mj + 2 * mh], c_lo + 8 * mh),
+                                               affine(p, cst, acc[4 * mj + 2 * mh + 1], c_lo + 8 * mh));
+          r4[m] = *reinterpret_cast<const uint32_t*>(&hv);
+        }
+        stmatrix_x4_trans(addr + jp * 16 * 128, r4);
+      }
+    }
+    consumers_sync();  // both rows staged
+    ys = cta.y_base + j * kRows;
+    pending = true;
+    if (p.unpool_mask) {  // the mask loads are in flight under the next block's first MMAs
+#pragma unroll
+      for (int i = 0; i < kTnUnits; ++i) {
+        const int y = ys + (i >> 2), x = x0 + (t >> 3) + 32 * (i & 3);
+        mk[i] = make_uint2(0u, 0u);
+        if (y < p.H && x < p.W)
+          mk[i] = __ldg(reinterpret_cast<const uint2*>(p.unpool_mask + ((static_cast<size_t>(img % p.mask_n) * p.H + y) * p.W + x) * p.cout_total + n0 + 8 * c));
+      }
+    }
+  }
+  if (pending)
+    for (int kh = 0; kh < K; ++kh) flush_slice(kh);
 }
 
 // k_conv_stack's shared memory: the resident weights (per kw the tap rows kh = 0 .. K-1, 0 .. K-2 of [16 cout][64 cin] half:
@@ -1004,6 +1251,7 @@ struct ConvTcPlan {
   int k;
   int kw;             // filter width the kernel walks (== k, or 1 for a window-folded layer)
   bool roll;
+  bool tn = false;    // k_conv_tn: Cin = 64 -> 64-wide half tiles, K = 3 / 7, every epilogue but the two-step classifier
   bool pk2 = false;   // two images per 128-pixel M tile (layers at most 64 pixels wide, chunked 3x3 kernel)
   bool stack = false; // k_conv_stack: 64 -> 16 float logits, K = 3 / 7
   double rows_ratio = 1.0;  // k_conv_stack: input rows it runs the MMAs of / output rows (the warm-up rows of every run)
@@ -1027,14 +1275,17 @@ void conv_tc_dispatch(const ConvTcPlan& plan, cudaStream_t s, bool configure) {
   if (plan.p.split) {
     if (plan.p.n_tile == 16) { if (K == 7) go(k_conv_tc<7, false, 7, false, 16, true>); else if (K == 3) go(k_conv_tc<3, false, 3, false, 16, true>); else go(k_conv_tc<1, false, 1, false, 16, true>); }
     else { if (K == 7) go(k_conv_tc<7, false, 7, false, 64, true>); else if (K == 3) go(k_conv_tc<3, false, 3, false, 64, true>); else go(k_conv_tc<1, false, 1, false, 64, true>); }
-  } else if (plan.kw == 1 && K > 1) {  // window-folded first layer (K x 1), 64-wide tiles
-    if (K == 7) go(k_conv_tc<7, true, 1, false, 64, false>); else go(k_conv_tc<3, true, 1, false, 64, false>);
-  } else if (plan.pk2) {
-    if (plan.p.n_tile == 64) go(k_conv_tc<3, false, 3, true, 64, false>); else go(k_conv_tc<3, false, 3, true, 128, false>);
   } else if (plan.stack) {  // 64 -> 16 float logits, K = 3 / 7
     if (K == 7) { if (plan.p.unpool_in) go(k_conv_stack<7, true>); else go(k_conv_stack<7>); }
     else go(k_conv_stack<3>);
+  } else if (plan.tn) {  // Cin = 64 -> 64-wide half tiles, K = 7; KW = 1: window-folded first layer
+    if (plan.kw == 7) go(k_conv_tn<7, 7>); else go(k_conv_tn<7, 1>);
+  } else if (plan.kw == 1 && K == 3) {  // window-folded 3x3 first layer (3 x 1), 64-wide tiles
+    go(k_conv_tc<3, true, 1, false, 64, false>);
+  } else if (plan.pk2) {
+    if (plan.p.n_tile == 64) go(k_conv_tc<3, false, 3, true, 64, false>); else go(k_conv_tc<3, false, 3, true, 128, false>);
   } else if (plan.roll) {
+    // 64-wide K = 7 tiles get here only with the two-step classifier epilogue (conv_tc_set_classifier)
     if (K == 7) { if (plan.p.n_tile == 64) go(k_conv_tc<7, true, 7, false, 64, false>); else go(k_conv_tc<7, true, 7, false, 128, false>); }
     else if (K == 3) { if (plan.p.n_tile == 64) go(k_conv_tc<3, true, 3, false, 64, false>); else go(k_conv_tc<3, true, 3, false, 128, false>); }
     else by_n(k_conv_tc<1, true, 1, false, 16, false>, k_conv_tc<1, true, 1, false, 64, false>, k_conv_tc<1, true, 1, false, 128, false>);
@@ -1055,23 +1306,34 @@ int num_sms() {
 // frees up, so the extractors' short dependent kernels -- highest stream priority notwithstanding -- each wait for a
 // whole CTA lifetime; this cap trades the two (unit: 2-row blocks).
 constexpr int kTcMaxPpc = 48;
-size_t tc_smem_bytes(int K, bool roll, int n_tile, int stages) {
+// tn: k_conv_tn, whose epilogue staging tile follows the weight ring
+size_t tc_smem_bytes(int K, bool roll, int n_tile, int stages, bool tn) {
   const int rk = kRows + K - 1;
-  const int slots = roll ? rk : (K == 7 ? rk + 2 : 2 * rk);  // k_conv_tc's kSlots
+  const int slots = roll ? rk : (K == 7 ? rk + 2 : 2 * rk);  // TcCta::kSlots
   const int b_stride = (n_tile * 128 + 1023) & ~1023;
-  return 1024 + static_cast<size_t>(slots) * kSlotBytes + static_cast<size_t>(stages) * b_stride + (2 * slots + 2 * stages) * 8;
+  return 1024 + static_cast<size_t>(slots) * kSlotBytes + static_cast<size_t>(stages) * b_stride + (tn ? kTnStageBytes : 0) +
+         (2 * slots + 2 * stages) * 8;
 }
-int tc_stages(int K, bool roll, int n_tile) {  // deepest weight ring that fits (0 = configuration does not fit)
+int tc_stages(int K, bool roll, int n_tile, bool tn) {  // deepest weight ring that fits (0 = configuration does not fit)
   for (int st = kMaxBStages; st >= 3; --st)
-    if (tc_smem_bytes(K, roll, n_tile, st) <= 227 * 1024) return st;
+    if (tc_smem_bytes(K, roll, n_tile, st, tn) <= 227 * 1024) return st;
   return 0;
 }
+// k_conv_tn runs every Cin = 64, K = 7 layer with 64-wide half output tiles (the two-step classifier epilogue is moved
+// back to k_conv_tc by conv_tc_set_classifier).  The K = 3 layers stay on k_conv_tc: on k_conv_tn Standard's conv1_2_D
+// (352 x 1024, T = 12) took 0.75 ms in one session and 1.77 ms in another, against k_conv_tc's steady 1.35 ms (H100 80GB
+// HBM3, 700 W).
+bool tc_is_tn(int K, bool roll, int n_tile, bool out_f32) { return roll && n_tile == 64 && K == 7 && !out_f32; }
 int tc_pick_n(const Op& op, const TensorView& out, bool roll) {
   if (out.dt == DType::F32 && out.cs <= 16) return 16;  // the float logits layer
   if (op.split || op.fold_kw) return 64;                // split: the segment sums must fit in registers next to the accumulators
   int n = (op.cout_p % 128 == 0) ? 128 : 64;
-  if (!tc_stages(op.k, roll, n)) n = 64;
+  if (!tc_stages(op.k, roll, n, false)) n = 64;
   return n;
+}
+int tc_stages_for(const Op& op, const TensorView& out, bool roll) {
+  const int n = tc_pick_n(op, out, roll);
+  return tc_stages(op.k, roll, n, tc_is_tn(op.k, roll, n, out.dt == DType::F32));
 }
 // row blocks per CTA: minimise (waves over the SMs) x (blocks per CTA + ~1 block of prologue / halo overhead)
 int tc_blocks_per_cta(long columns, int total_pairs, double overhead) {
@@ -1122,12 +1384,12 @@ bool conv_tc_supported(const Op& op, const TensorView& in, const TensorView& out
   if (op.cout_p > kMaxCout) return false;
   if (op.fold_kw) {
     if (in.cs != 8 || op.cin_p != 64 || (op.k != 3 && op.k != 7) || out.dt != DType::F16 || op.cout % 64 || out.cs != op.cout) return false;
-    return tc_stages(op.k, true, tc_pick_n(op, out, true)) > 0;
+    return tc_stages_for(op, out, true) > 0;
   }
   if (op.split) {  // `in` = the [hi Cin | lo Cin] half planes of the float input
     if (op.cin % 64 || in.cs != 2 * op.cin || out.dt != DType::F32) return false;
     if (!((out.cs == op.cout && op.cout % 64 == 0) || (out.cs == 16 && op.cout <= 16))) return false;
-    return tc_stages(op.k, false, tc_pick_n(op, out, false)) > 0;
+    return tc_stages_for(op, out, false) > 0;
   }
   if (in.cs % 64 || op.cin != in.cs) return false;
   if (out.dt == DType::F16) {
@@ -1136,7 +1398,7 @@ bool conv_tc_supported(const Op& op, const TensorView& in, const TensorView& out
     if (out.cs != 16 || op.cout > 16) return false;  // float logits, 16-channel pixels
   }
   const bool roll = in.cs == 64;
-  return tc_stages(op.k, roll, tc_pick_n(op, out, roll)) > 0;
+  return tc_stages_for(op, out, roll) > 0;
 }
 
 std::shared_ptr<ConvTcPlan> conv_tc_plan(const Op& op, const TensorView& in, const TensorView& out, const void* w_tc) {
@@ -1205,8 +1467,9 @@ std::shared_ptr<ConvTcPlan> conv_tc_plan(const Op& op, const TensorView& in, con
   p.pool_out = nullptr; p.pool_mask = nullptr;
   p.has_cls = 0; p.cls_out = nullptr;
   plan->grid = dim3(p.strips * ceil_div(total_pairs, p.pairs_per_cta), cout_tiles, n_z);
-  p.b_stages = tc_stages(K, roll, n_tile);
-  plan->smem = tc_smem_bytes(K, roll, n_tile, p.b_stages);
+  plan->tn = tc_is_tn(K, roll, n_tile, p.out_f32 != 0);
+  p.b_stages = tc_stages(K, roll, n_tile, plan->tn);
+  plan->smem = tc_smem_bytes(K, roll, n_tile, p.b_stages, plan->tn);
   plan->k = K;
   plan->kw = KW;
   plan->roll = roll;
@@ -1276,7 +1539,8 @@ void conv_tc_set_pool(ConvTcPlan& plan, void* pooled, uint8_t* mask) {
 }
 
 bool conv_tc_can_fuse_classifier(const ConvTcPlan& plan) {
-  return plan.roll && plan.p.n_tile == 64 && plan.p.cout_total == 64 && !plan.p.out_f32 && !plan.p.unpool_mask && !plan.p.has_drop && !plan.p.pool_out;
+  return plan.roll && plan.kw == plan.k && plan.p.n_tile == 64 && plan.p.cout_total == 64 && !plan.p.out_f32 && !plan.p.unpool_mask &&
+         !plan.p.has_drop && !plan.p.pool_out;
 }
 
 void conv_tc_set_classifier(ConvTcPlan& plan, const float* w_cin_by_cout, int stride, const float* bias, int n_bias, float* logits) {
@@ -1285,6 +1549,11 @@ void conv_tc_set_classifier(ConvTcPlan& plan, const float* w_cin_by_cout, int st
   for (int j = 0; j < 16; ++j) plan.cst.cls_b[j] = j < n_bias ? bias[j] : 0.f;
   plan.p.has_cls = 1;
   plan.p.cls_out = logits;
+  // the two-step classifier epilogue is k_conv_tc's
+  plan.tn = false;
+  plan.p.b_stages = tc_stages(plan.k, true, 64, false);
+  plan.smem = tc_smem_bytes(plan.k, true, 64, plan.p.b_stages, false);
+  conv_tc_dispatch(plan, nullptr, true);
 }
 
 bool conv_tc_can_compose_classifier(const ConvTcPlan& plan) {
