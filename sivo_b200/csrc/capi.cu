@@ -776,11 +776,11 @@ int sivo_dbg_conv(int device, int engine, int precision, const float* in, int n,
       vs.p = op.a_split.p;
       op.tc = conv_tc_plan(op, vs, vo, op.w_tc.p);
       launch_split_hilo(vi, op.a_split.p, nullptr);
-      conv_tc_launch(*op.tc, op, nullptr);
+      conv_tc_launch(*op.tc, nullptr);
     } else if (engine == SIVO_ENGINE_TCGEN05) {
       if (dt != DType::F16 || !conv_tc_supported(op, vi, vo)) fail(SIVO_EINVAL, "conv: shape not supported by the tcgen05 engine");
       op.tc = conv_tc_plan(op, vi, vo, op.w_tc.p);
-      conv_tc_launch(*op.tc, op, nullptr);
+      conv_tc_launch(*op.tc, nullptr);
     } else {
       ConvParams p;
       p.in = vi; p.out = vo;
@@ -818,7 +818,7 @@ int sivo_dbg_conv_unpooled(int device, const float* pooled, const int* mask, int
     if (!conv_tc_supported(op, vu, vo)) fail(SIVO_EINVAL, "conv_unpooled: shape not supported by the tensor-core kernel");
     op.tc = conv_tc_plan(op, vu, vo, op.w_tc.p);
     conv_tc_set_unpool_input(*op.tc, vp.p, bm.as<uint8_t>(), mask_n, h, w);
-    conv_tc_launch(*op.tc, op, nullptr);
+    conv_tc_launch(*op.tc, nullptr);
     SIVO_CUDA(cudaDeviceSynchronize());
     download_nchw(vo, out);
     SIVO_CUDA(cudaDeviceSynchronize());

@@ -224,13 +224,41 @@ __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_grou
 template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 // Ties the accumulator registers to the preceding wait: the compiler must not move their reads (or the zeroing of a
-// fresh segment) across it.
-template <int R, int F>
-__device__ __forceinline__ void fence_acc(float (&d)[R][F]) {
+// fresh segment) across it.  Takes a register array of any rank.
+template <typename T, int F>
+__device__ __forceinline__ void fence_acc(T (&d)[F]) {
 #pragma unroll
-  for (int r = 0; r < R; ++r)
+  for (int i = 0; i < F; ++i) {
+    if constexpr (std::is_array_v<T>) fence_acc(d[i]);
+    else asm volatile("" : "+f"(d[i])::"memory");
+  }
+}
+
+// One of four words by a run-time index: selects, not a dynamically indexed (= local-memory) array.
+__device__ __forceinline__ uint32_t pick4(const uint32_t (&a)[4], int i) { return i == 0 ? a[0] : i == 1 ? a[1] : i == 2 ? a[2] : a[3]; }
+
+// Dropout on two channels' half values in one word: y = x * keep * scale (exact), keep = bits `bit`, `bit` + 1 of `keep`.
+__device__ __forceinline__ uint32_t drop_word(uint32_t w, uint32_t keep, int bit, float scale) {
+  __half2 hv = *reinterpret_cast<const __half2*>(&w);
+  hv = __hmul2(hv, __floats2half2_rn((keep >> bit) & 1u ? scale : 0.f, (keep >> (bit + 1)) & 1u ? scale : 0.f));
+  return *reinterpret_cast<const uint32_t*>(&hv);
+}
+
+// 2x2 max-pool of two channels' half values per word over a window in scan order: a = (y, x), b = (y, x+1), c = (y+1, x),
+// d = (y+1, x+1).  Strict '>' per half (false on NaN, like __hgt), so the first maximum wins; `arg` gets its position
+// (0 .. 3) in bytes 0 and 1.
+__device__ __forceinline__ uint32_t pool2x2(uint32_t a, uint32_t b, uint32_t c, uint32_t d, uint32_t& arg) {
+  uint32_t best = a;
+  arg = 0;
+  const uint32_t cand[3] = {b, c, d};
 #pragma unroll
-    for (int i = 0; i < F; ++i) asm volatile("" : "+f"(d[r][i])::"memory");
+  for (int k = 0; k < 3; ++k) {
+    const uint32_t sel = __hgt2_mask(*reinterpret_cast<const __half2*>(&cand[k]), *reinterpret_cast<const __half2*>(&best));  // 0xFFFF where the candidate wins
+    best = (best & ~sel) | (cand[k] & sel);
+    const uint32_t selb = __byte_perm(sel, 0u, 0x4420);  // the two half masks as two byte masks (bytes 0 and 1)
+    arg = (arg & ~selb) | ((0x0101u * static_cast<uint32_t>(k + 1)) & selb);
+  }
+  return best;
 }
 
 __device__ __forceinline__ float affine(const TcParams& p, const TcConsts& cst, float v, int c) {
@@ -279,17 +307,8 @@ __device__ __forceinline__ void epilogue_block(const TcParams& p, const TcConsts
         const __half2 hc = __floats2half2_rn(affine(p, cst, acc[1][4 * j + 2 * h], n0 + c), affine(p, cst, acc[1][4 * j + 2 * h + 1], n0 + c + 1));
         const uint32_t a = *reinterpret_cast<const uint32_t*>(&ha), cc = *reinterpret_cast<const uint32_t*>(&hc);
         const uint32_t b = __shfl_xor_sync(0xffffffffu, a, 4), d = __shfl_xor_sync(0xffffffffu, cc, 4);
-        // window in scan order: a = (y, x), b = (y, x+1), c = (y+1, x), d = (y+1, x+1); two channels per register
-        uint32_t best = a, arg = 0;
-        const uint32_t cand[3] = {b, cc, d};
-#pragma unroll
-        for (int k = 0; k < 3; ++k) {
-          // strict '>' per half (false on NaN, like __hgt): 0xFFFF where the candidate wins
-          const uint32_t sel = __hgt2_mask(*reinterpret_cast<const __half2*>(&cand[k]), *reinterpret_cast<const __half2*>(&best));
-          best = (best & ~sel) | (cand[k] & sel);
-          const uint32_t selb = __byte_perm(sel, 0u, 0x4420);  // the two half masks as two byte masks (bytes 0 and 1)
-          arg = (arg & ~selb) | ((0x0101u * static_cast<uint32_t>(k + 1)) & selb);
-        }
+        uint32_t arg;
+        const uint32_t best = pool2x2(a, b, cc, d, arg);
         if (writer) {
           *reinterpret_cast<uint32_t*>(p.pool_out + o + c) = best;
           *reinterpret_cast<uint16_t*>(p.pool_mask + o + c) = static_cast<uint16_t>(arg);
@@ -346,14 +365,9 @@ __device__ __forceinline__ void epilogue_block(const TcParams& p, const TcConsts
 #pragma unroll
       for (int j = 0; j < N / 8; ++j) {
         const int c = n0 + 8 * j + 2 * q;
-        __half2 hv = __floats2half2_rn(affine(p, cst, acc[r][4 * j + 2 * h], c), affine(p, cst, acc[r][4 * j + 2 * h + 1], c + 1));
-        if (p.has_drop) {  // y = x * keep * 2 on the stored half value (exact)
-          const int wsel = (c >> 5) & 3;  // selects, not a dynamically indexed (= local-memory) array
-          const uint32_t keep = wsel == 0 ? bits[0] : wsel == 1 ? bits[1] : wsel == 2 ? bits[2] : bits[3];
-          const int bit = c & 31;
-          hv = __hmul2(hv, __floats2half2_rn((keep >> bit) & 1u ? p.drop_scale : 0.f, (keep >> (bit + 1)) & 1u ? p.drop_scale : 0.f));
-        }
-        const uint32_t w = *reinterpret_cast<const uint32_t*>(&hv);
+        const __half2 hv = __floats2half2_rn(affine(p, cst, acc[r][4 * j + 2 * h], c), affine(p, cst, acc[r][4 * j + 2 * h + 1], c + 1));
+        uint32_t w = *reinterpret_cast<const uint32_t*>(&hv);
+        if (p.has_drop) w = drop_word(w, pick4(bits, (c >> 5) & 3), c & 31, p.drop_scale);
         if (!inside) continue;
         if (p.unpool_mask) {
           // the value goes to the 2x2 position its mask byte names, zeros to the other three
@@ -387,12 +401,11 @@ struct EpiStage {
 // 4 x 4 word transpose within a quad: lane q holds w[k] = channels 8 k + 2 q, +1 of a 32-channel group and gets back
 // channels 8 q .. 8 q + 7 (lane q' sends w[q' ^ x] across xor distance x, which is the word lane q' ^ x keeps).
 __device__ __forceinline__ uint4 quad_transpose(const uint32_t (&w)[4], int q) {
-  auto pick = [](const uint32_t (&a)[4], int i) { return i == 0 ? a[0] : i == 1 ? a[1] : i == 2 ? a[2] : a[3]; };
   uint32_t r[4];  // r[x] = word q of column q ^ x
-  r[0] = pick(w, q);
+  r[0] = pick4(w, q);
 #pragma unroll
-  for (int x = 1; x < 4; ++x) r[x] = __shfl_xor_sync(0xffffffffu, pick(w, q ^ x), x);
-  return make_uint4(pick(r, q), pick(r, q ^ 1), pick(r, q ^ 2), pick(r, q ^ 3));
+  for (int x = 1; x < 4; ++x) r[x] = __shfl_xor_sync(0xffffffffu, pick4(w, q ^ x), x);
+  return make_uint4(pick4(r, q), pick4(r, q ^ 1), pick4(r, q ^ 2), pick4(r, q ^ 3));
 }
 
 // Converts one row block's accumulators into its staged outputs with the arithmetic of epilogue_block (bias / BN /
@@ -417,14 +430,9 @@ __device__ __forceinline__ void epilogue_stage(const TcParams& p, const TcConsts
 #pragma unroll
       for (int j = 0; j < N / 8; ++j) {
         const int c = n0 + 8 * j + 2 * q;
-        __half2 hv = __floats2half2_rn(affine(p, cst, acc[r][4 * j + 2 * h], c), affine(p, cst, acc[r][4 * j + 2 * h + 1], c + 1));
-        if (p.has_drop) {
-          const int wsel = (c >> 5) & 3;
-          const uint32_t keep = wsel == 0 ? bits[0] : wsel == 1 ? bits[1] : wsel == 2 ? bits[2] : bits[3];
-          const int bit = c & 31;
-          hv = __hmul2(hv, __floats2half2_rn((keep >> bit) & 1u ? p.drop_scale : 0.f, (keep >> (bit + 1)) & 1u ? p.drop_scale : 0.f));
-        }
+        const __half2 hv = __floats2half2_rn(affine(p, cst, acc[r][4 * j + 2 * h], c), affine(p, cst, acc[r][4 * j + 2 * h + 1], c + 1));
         w[j] = *reinterpret_cast<const uint32_t*>(&hv);
+        if (p.has_drop) w[j] = drop_word(w[j], pick4(bits, (c >> 5) & 3), c & 31, p.drop_scale);
       }
       const size_t mask_pix = (static_cast<size_t>(img % p.mask_n) * p.H + y) * p.W + x;
 #pragma unroll
@@ -486,17 +494,33 @@ __device__ __forceinline__ void epilogue_flush(const TcParams& p, const EpiStage
 //               have to spare; weights arrive in (kw, kh) order.
 // SPLIT: split-operand fp32 mode (see TcParams::split / seg_rows); N <= 64 so that the segment sums fit in registers.
 //
-// TcCta: what k_conv_tc and k_conv_tn share -- the CTA's shared-memory carve-up (halo ring, weight ring, `stage_bytes` for the
-// consumers' epilogue staging, mbarriers), its place in the (strip, row block, cout tile, image) grid, and warpgroup 0's
-// producers that fill the two rings.
+// TcCta's shared memory, in this order: the halo ring (tc_slots rows of kSlotBytes), the weight ring (`stages` tiles of
+// N couts x 64 cin half, each 1 KB aligned), `stage_bytes` for the consumers' epilogue staging, then the full / empty
+// mbarriers of both rings; the leading 1 KB aligns the dynamic shared-memory base.
+__host__ __device__ constexpr int tc_slots(int K, bool roll) {
+  // rows are released as soon as their last tap row retired; !ROLL double-buffers chunks where that fits (K = 7: RK + 2)
+  return roll ? kRows + K - 1 : (K == 7 ? kRows + K + 1 : 2 * (kRows + K - 1));
+}
+__host__ __device__ constexpr int tc_b_stride(int n) { return (n * 128 + 1023) & ~1023; }
+__host__ __device__ constexpr int tc_smem_bytes(int K, bool roll, int n, int stages, int stage_bytes) {
+  return 1024 + tc_slots(K, roll) * kSlotBytes + stages * tc_b_stride(n) + stage_bytes + (2 * tc_slots(K, roll) + 2 * stages) * 8;
+}
+// the deepest weight ring that fits (0: none of at least 3 stages does)
+__host__ __device__ constexpr int tc_stages(int K, bool roll, int n, int stage_bytes) {
+  for (int st = kMaxBStages; st >= 3; --st)
+    if (tc_smem_bytes(K, roll, n, st, stage_bytes) <= 227 * 1024) return st;
+  return 0;
+}
+
+// TcCta: what k_conv_tc and k_conv_tn share -- the CTA's shared-memory carve-up (see tc_smem_bytes), its place in the
+// (strip, row block, cout tile, image) grid, and warpgroup 0's producers that fill the two rings.
 template <int K, bool ROLL, int KW, bool PK2, int N>
 struct TcCta {
   static constexpr int RK = kRows + K - 1;           // halo rows one row block reads (per chunk)
-  // rows are released as soon as their last tap row retired; !ROLL double-buffers chunks where that fits (K = 7: RK + 2)
-  static constexpr int kSlots = ROLL ? RK : (K == 7 ? RK + 2 : 2 * RK);
+  static constexpr int kSlots = tc_slots(K, ROLL);
   static constexpr int kPad = (K - 1) / 2, kPadW = (KW - 1) / 2;
   static constexpr int b_bytes = N * 128;
-  static constexpr int b_stride = (b_bytes + 1023) & ~1023;
+  static constexpr int b_stride = tc_b_stride(N);
   static constexpr int UPC = PK2 ? KW * RK : RK;     // halo units per (row block, chunk)
   uint8_t *a_slots, *b_stages, *stage;
   uint64_t *a_full, *a_empty, *b_full, *b_empty;   // [kSlots], [kSlots], [kBStages], [kBStages]
@@ -595,6 +619,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUt
   static_assert(!PK2 || (!ROLL && KW == K), "image-pair tiles use the chunked kernel");
   static_assert(!SPLIT || (!ROLL && N <= 64), "split mode: chunked kernel, segment sums in registers");
   using Cta = TcCta<K, ROLL, KW, PK2, N>;
+  static_assert(tc_stages(K, ROLL, N, 0) > 0, "halo ring + 3 weight stages must fit in shared memory");
   constexpr int RK = Cta::RK, kSlots = Cta::kSlots, b_stride = Cta::b_stride;
   constexpr int F = N / 2;                           // accumulator registers per thread per output row
   const Cta cta(p, tc_smem_base(), 0);
@@ -744,7 +769,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUt
 }
 
 // k_conv_tn: the Cin = 64 -> 64-wide half convolutions of k_conv_tc<K, true, KW, false, 64> with the GEMM transposed
-// (run for K = 7, see tc_is_tn).
+// (run for K = 7, see tc_choose_kernel).
 // There, each consumer's m64n64k16 reads a 2 KB pixel tile and a 2 KB weight tile for 64 K multiply-adds: 0.0625 B of
 // shared-memory operand reads per MAC.  Here D^T[64 cout x 128 px] = W[64 cout x 16 cin] * X^T[16 cin x 128 px] is ONE
 // m64n128k16 per (output row, tap, K step): 2 KB of weights + 4 KB of pixels, 0.047 B per MAC.  No layout changes: the
@@ -778,19 +803,6 @@ __device__ __forceinline__ void consumers_sync() { asm volatile("bar.sync 1, 256
 __device__ __forceinline__ uint32_t tn_chunk(uint32_t s_base, int r, int px, int c) {
   return s_base + static_cast<uint32_t>(r * (128 * 128) + px * 128 + ((c ^ (px & 7)) << 4));
 }
-// dropout on two staged halves: y = x * keep * scale (exact); `kb` holds the keep bits of the chunk's 8 channels
-__device__ __forceinline__ uint32_t drop_word(uint32_t w, uint32_t kb, int k, float scale) {
-  __half2 hv = *reinterpret_cast<const __half2*>(&w);
-  hv = __hmul2(hv, __floats2half2_rn((kb >> (2 * k)) & 1u ? scale : 0.f, (kb >> (2 * k + 1)) & 1u ? scale : 0.f));
-  return *reinterpret_cast<const uint32_t*>(&hv);
-}
-
-template <int F>
-__device__ __forceinline__ void fence_acc(float (&d)[F]) {
-#pragma unroll
-  for (int i = 0; i < F; ++i) asm volatile("" : "+f"(d[i])::"memory");
-}
-
 template <int K, int KW>
 __global__ void __launch_bounds__(kTcThreads, 1)
 k_conv_tn(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const __grid_constant__ TcParams p,
@@ -798,6 +810,7 @@ k_conv_tn(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUt
   using Cta = TcCta<K, true, KW, false, 64>;
   constexpr int kSlots = Cta::kSlots, b_stride = Cta::b_stride;
   static_assert(K >= kRows, "a block's own halo rows are released by its tap rows kh < kRows");
+  static_assert(tc_stages(K, true, 64, kTnStageBytes) > 0, "halo ring + staging tile + 3 weight stages must fit in shared memory");
   const Cta cta(p, tc_smem_base(), kTnStageBytes);
   const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) cta.init_barriers();
@@ -828,33 +841,22 @@ k_conv_tn(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUt
     if (p.has_drop) {
       const int src = 4 * i + (lane >> 3);
       const uint32_t k0 = __shfl_sync(0xffffffffu, keep[0], src), k1 = __shfl_sync(0xffffffffu, keep[1], src);
-      const uint32_t kb = ((c >> 2) ? k1 : k0) >> (8 * (c & 3));
-      v = make_uint4(drop_word(v.x, kb, 0, p.drop_scale), drop_word(v.y, kb, 1, p.drop_scale), drop_word(v.z, kb, 2, p.drop_scale),
-                     drop_word(v.w, kb, 3, p.drop_scale));
+      const uint32_t kb = ((c >> 2) ? k1 : k0) >> (8 * (c & 3));  // the keep bits of the chunk's 8 channels
+      v = make_uint4(drop_word(v.x, kb, 0, p.drop_scale), drop_word(v.y, kb, 2, p.drop_scale), drop_word(v.z, kb, 4, p.drop_scale),
+                     drop_word(v.w, kb, 6, p.drop_scale));
     }
     if (!(y < p.H && x < p.W)) return;
     if (p.unpool_mask) unpool_store8(p, img, y, x, n0 + 8 * c, v, mk[i]);
     else *reinterpret_cast<uint4*>(static_cast<__half*>(p.out) + ((static_cast<size_t>(img) * p.H + y) * p.W + x) * p.cout_total + n0 + 8 * c) = v;
   };
-  auto flush_pool = [&](int i) {  // window in scan order: (y, x), (y, x+1), (y+1, x), (y+1, x+1); strict '>', first maximum wins
+  auto flush_pool = [&](int i) {  // the window's four staged pixels, in scan order
     const int pp = (t >> 3) + 32 * i, x = x0 + 2 * pp;
     const uint4 a = lds128(tn_chunk(s_base, 0, 2 * pp, c)), b = lds128(tn_chunk(s_base, 0, 2 * pp + 1, c));
     const uint4 cc = lds128(tn_chunk(s_base, 1, 2 * pp, c)), d = lds128(tn_chunk(s_base, 1, 2 * pp + 1, c));
     const uint32_t av[4] = {a.x, a.y, a.z, a.w}, bv[4] = {b.x, b.y, b.z, b.w}, cv[4] = {cc.x, cc.y, cc.z, cc.w}, dv[4] = {d.x, d.y, d.z, d.w};
     uint32_t best[4], arg[4];
 #pragma unroll
-    for (int w = 0; w < 4; ++w) {  // two channels per word
-      best[w] = av[w];
-      arg[w] = 0;
-      const uint32_t cand[3] = {bv[w], cv[w], dv[w]};
-#pragma unroll
-      for (int k = 0; k < 3; ++k) {
-        const uint32_t sel = __hgt2_mask(*reinterpret_cast<const __half2*>(&cand[k]), *reinterpret_cast<const __half2*>(&best[w]));
-        best[w] = (best[w] & ~sel) | (cand[k] & sel);
-        const uint32_t selb = __byte_perm(sel, 0u, 0x4420);  // the two half masks as two byte masks (bytes 0 and 1)
-        arg[w] = (arg[w] & ~selb) | ((0x0101u * static_cast<uint32_t>(k + 1)) & selb);
-      }
-    }
+    for (int w = 0; w < 4; ++w) best[w] = pool2x2(av[w], bv[w], cv[w], dv[w], arg[w]);
     if (ys + 1 < p.H && x + 1 < p.W) {
       const size_t o = ((static_cast<size_t>(img) * (p.H >> 1) + (ys >> 1)) * (p.W >> 1) + (x >> 1)) * p.cout_total + n0 + 8 * c;
       *reinterpret_cast<uint4*>(p.pool_out + o) = make_uint4(best[0], best[1], best[2], best[3]);
@@ -1240,6 +1242,9 @@ void encode(CUtensorMap* m, void* base, int rank, const cuuint64_t* dims, const 
   if (r != CUDA_SUCCESS) fail(SIVO_ECUDA, "cuTensorMapEncodeTiled failed with %d", static_cast<int>(r));
 }
 
+// every convolution kernel's signature
+using TcKernel = void (*)(CUtensorMap, CUtensorMap, TcParams, TcConsts);
+
 }  // namespace
 
 struct ConvTcPlan {
@@ -1250,50 +1255,66 @@ struct ConvTcPlan {
   size_t smem;
   int k;
   int kw;             // filter width the kernel walks (== k, or 1 for a window-folded layer)
-  bool roll;
-  bool tn = false;    // k_conv_tn: Cin = 64 -> 64-wide half tiles, K = 3 / 7, every epilogue but the two-step classifier
-  bool pk2 = false;   // two images per 128-pixel M tile (layers at most 64 pixels wide, chunked 3x3 kernel)
-  bool stack = false; // k_conv_stack: 64 -> 16 float logits, K = 3 / 7
+  TcKernel kern = nullptr;  // set by tc_choose_kernel
   double rows_ratio = 1.0;  // k_conv_stack: input rows it runs the MMAs of / output rows (the warm-up rows of every run)
   DevBuf w_own;       // weights the plan owns (the composed classifier)
 };
 
 namespace {
-// one place that names every instantiation: configure == true sets the dynamic shared-memory limit, else launches
-void conv_tc_dispatch(const ConvTcPlan& plan, cudaStream_t s, bool configure) {
-  auto go = [&](auto kern) {
-    // the limit is per kernel function, not per launch: always raise it to the full 227 KB so that plans of different
-    // sizes that share an instantiation cannot lower it for each other
-    if (configure) SIVO_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    else kern<<<plan.grid, kTcThreads, plan.smem, s>>>(plan.map_a, plan.map_b, plan.p, plan.cst);
-  };
+// one 64-channel input chunk: the halo rows persist in the ring while a CTA walks down its strip (ROLL)
+bool tc_roll(const TcParams& p) { return p.chunks == 1 && !p.split; }
+// k_conv_stack: the 64 -> 16 float-logits layers, K = 3 / 7
+bool tc_stacked(const ConvTcPlan& plan) { return tc_roll(plan.p) && plan.p.n_tile == 16 && plan.k > 1; }
+// two images per 128-pixel M tile (PK2): chunked 3x3 layers at most 64 pixels wide
+bool tc_pk2(const ConvTcPlan& plan) {
+  const TcParams& p = plan.p;
+  return !tc_roll(p) && !p.split && plan.k == 3 && p.W <= 64 && p.N_batch >= 2 && p.n_tile != 16;
+}
+
+// The one place that names every instantiation: picks the kernel for the plan's shape and epilogue state, sizes its
+// shared memory (and weight ring) to match and raises the kernel's dynamic shared-memory limit.  Called again whenever
+// a fusion changes that state.
+void tc_choose_kernel(ConvTcPlan& plan) {
+  TcParams& p = plan.p;
+  const int K = plan.k, n = p.n_tile;
+  const bool roll = tc_roll(p);
+  // k_conv_tn runs every Cin = 64, K = 7 layer with 64-wide half output tiles but the two-step classifier epilogue.  The
+  // K = 3 layers stay on k_conv_tc: on k_conv_tn Standard's conv1_2_D (352 x 1024, T = 12) took 0.75 ms in one session and
+  // 1.77 ms in another, against k_conv_tc's steady 1.35 ms (H100 80GB HBM3, 700 W).
+  const bool tn = roll && n == 64 && K == 7 && !p.out_f32 && !p.has_cls;
   // per (K, ROLL, KW, PK2): the three tile widths
-  auto by_n = [&](auto k16, auto k64, auto k128) {
-    if (plan.p.n_tile == 16) go(k16); else if (plan.p.n_tile == 64) go(k64); else go(k128);
-  };
-  const int K = plan.k;
-  if (plan.p.split) {
-    if (plan.p.n_tile == 16) { if (K == 7) go(k_conv_tc<7, false, 7, false, 16, true>); else if (K == 3) go(k_conv_tc<3, false, 3, false, 16, true>); else go(k_conv_tc<1, false, 1, false, 16, true>); }
-    else { if (K == 7) go(k_conv_tc<7, false, 7, false, 64, true>); else if (K == 3) go(k_conv_tc<3, false, 3, false, 64, true>); else go(k_conv_tc<1, false, 1, false, 64, true>); }
-  } else if (plan.stack) {  // 64 -> 16 float logits, K = 3 / 7
-    if (K == 7) { if (plan.p.unpool_in) go(k_conv_stack<7, true>); else go(k_conv_stack<7>); }
-    else go(k_conv_stack<3>);
-  } else if (plan.tn) {  // Cin = 64 -> 64-wide half tiles, K = 7; KW = 1: window-folded first layer
-    if (plan.kw == 7) go(k_conv_tn<7, 7>); else go(k_conv_tn<7, 1>);
-  } else if (plan.kw == 1 && K == 3) {  // window-folded 3x3 first layer (3 x 1), 64-wide tiles
-    go(k_conv_tc<3, true, 1, false, 64, false>);
-  } else if (plan.pk2) {
-    if (plan.p.n_tile == 64) go(k_conv_tc<3, false, 3, true, 64, false>); else go(k_conv_tc<3, false, 3, true, 128, false>);
-  } else if (plan.roll) {
-    // 64-wide K = 7 tiles get here only with the two-step classifier epilogue (conv_tc_set_classifier)
-    if (K == 7) { if (plan.p.n_tile == 64) go(k_conv_tc<7, true, 7, false, 64, false>); else go(k_conv_tc<7, true, 7, false, 128, false>); }
-    else if (K == 3) { if (plan.p.n_tile == 64) go(k_conv_tc<3, true, 3, false, 64, false>); else go(k_conv_tc<3, true, 3, false, 128, false>); }
-    else by_n(k_conv_tc<1, true, 1, false, 16, false>, k_conv_tc<1, true, 1, false, 64, false>, k_conv_tc<1, true, 1, false, 128, false>);
+  auto by_n = [n](TcKernel k16, TcKernel k64, TcKernel k128) { return n == 16 ? k16 : n == 64 ? k64 : k128; };
+  if (tc_stacked(plan)) {
+    plan.kern = K == 3 ? k_conv_stack<3> : p.unpool_in ? k_conv_stack<7, true> : k_conv_stack<7>;
+    plan.smem = stack_smem_bytes(K);
   } else {
-    if (K == 7) by_n(k_conv_tc<7, false, 7, false, 16, false>, k_conv_tc<7, false, 7, false, 64, false>, k_conv_tc<7, false, 7, false, 128, false>);
-    else if (K == 3) by_n(k_conv_tc<3, false, 3, false, 16, false>, k_conv_tc<3, false, 3, false, 64, false>, k_conv_tc<3, false, 3, false, 128, false>);
-    else by_n(k_conv_tc<1, false, 1, false, 16, false>, k_conv_tc<1, false, 1, false, 64, false>, k_conv_tc<1, false, 1, false, 128, false>);
+    if (p.split) {
+      if (n == 16) plan.kern = K == 7 ? k_conv_tc<7, false, 7, false, 16, true> : K == 3 ? k_conv_tc<3, false, 3, false, 16, true> : k_conv_tc<1, false, 1, false, 16, true>;
+      else plan.kern = K == 7 ? k_conv_tc<7, false, 7, false, 64, true> : K == 3 ? k_conv_tc<3, false, 3, false, 64, true> : k_conv_tc<1, false, 1, false, 64, true>;
+    } else if (tn) {  // KW = 1: window-folded first layer
+      plan.kern = plan.kw == 7 ? k_conv_tn<7, 7> : k_conv_tn<7, 1>;
+    } else if (plan.kw == 1 && K == 3) {  // window-folded 3x3 first layer (3 x 1), 64-wide tiles
+      plan.kern = k_conv_tc<3, true, 1, false, 64, false>;
+    } else if (tc_pk2(plan)) {
+      plan.kern = n == 64 ? k_conv_tc<3, false, 3, true, 64, false> : k_conv_tc<3, false, 3, true, 128, false>;
+    } else if (roll) {
+      // 64-wide K = 7 tiles get here only with the two-step classifier epilogue (conv_tc_set_classifier)
+      if (K == 7) plan.kern = n == 64 ? k_conv_tc<7, true, 7, false, 64, false> : k_conv_tc<7, true, 7, false, 128, false>;
+      else if (K == 3) plan.kern = n == 64 ? k_conv_tc<3, true, 3, false, 64, false> : k_conv_tc<3, true, 3, false, 128, false>;
+      else plan.kern = by_n(k_conv_tc<1, true, 1, false, 16, false>, k_conv_tc<1, true, 1, false, 64, false>, k_conv_tc<1, true, 1, false, 128, false>);
+    } else {
+      if (K == 7) plan.kern = by_n(k_conv_tc<7, false, 7, false, 16, false>, k_conv_tc<7, false, 7, false, 64, false>, k_conv_tc<7, false, 7, false, 128, false>);
+      else if (K == 3) plan.kern = by_n(k_conv_tc<3, false, 3, false, 16, false>, k_conv_tc<3, false, 3, false, 64, false>, k_conv_tc<3, false, 3, false, 128, false>);
+      else plan.kern = by_n(k_conv_tc<1, false, 1, false, 16, false>, k_conv_tc<1, false, 1, false, 64, false>, k_conv_tc<1, false, 1, false, 128, false>);
+    }
+    // every kernel above fits at least 3 weight stages (static_assert in k_conv_tc / k_conv_tn)
+    const int stage_bytes = tn ? kTnStageBytes : 0;
+    p.b_stages = tc_stages(K, roll, n, stage_bytes);
+    plan.smem = tc_smem_bytes(K, roll, n, p.b_stages, stage_bytes);
   }
+  // the limit is per kernel function, not per launch: always raise it to the full 227 KB so that plans of different
+  // sizes that share an instantiation cannot lower it for each other
+  SIVO_CUDA(cudaFuncSetAttribute(plan.kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
 }
 
 int num_sms() {
@@ -1306,34 +1327,10 @@ int num_sms() {
 // frees up, so the extractors' short dependent kernels -- highest stream priority notwithstanding -- each wait for a
 // whole CTA lifetime; this cap trades the two (unit: 2-row blocks).
 constexpr int kTcMaxPpc = 48;
-// tn: k_conv_tn, whose epilogue staging tile follows the weight ring
-size_t tc_smem_bytes(int K, bool roll, int n_tile, int stages, bool tn) {
-  const int rk = kRows + K - 1;
-  const int slots = roll ? rk : (K == 7 ? rk + 2 : 2 * rk);  // TcCta::kSlots
-  const int b_stride = (n_tile * 128 + 1023) & ~1023;
-  return 1024 + static_cast<size_t>(slots) * kSlotBytes + static_cast<size_t>(stages) * b_stride + (tn ? kTnStageBytes : 0) +
-         (2 * slots + 2 * stages) * 8;
-}
-int tc_stages(int K, bool roll, int n_tile, bool tn) {  // deepest weight ring that fits (0 = configuration does not fit)
-  for (int st = kMaxBStages; st >= 3; --st)
-    if (tc_smem_bytes(K, roll, n_tile, st, tn) <= 227 * 1024) return st;
-  return 0;
-}
-// k_conv_tn runs every Cin = 64, K = 7 layer with 64-wide half output tiles (the two-step classifier epilogue is moved
-// back to k_conv_tc by conv_tc_set_classifier).  The K = 3 layers stay on k_conv_tc: on k_conv_tn Standard's conv1_2_D
-// (352 x 1024, T = 12) took 0.75 ms in one session and 1.77 ms in another, against k_conv_tc's steady 1.35 ms (H100 80GB
-// HBM3, 700 W).
-bool tc_is_tn(int K, bool roll, int n_tile, bool out_f32) { return roll && n_tile == 64 && K == 7 && !out_f32; }
-int tc_pick_n(const Op& op, const TensorView& out, bool roll) {
+int tc_pick_n(const Op& op, const TensorView& out) {
   if (out.dt == DType::F32 && out.cs <= 16) return 16;  // the float logits layer
   if (op.split || op.fold_kw) return 64;                // split: the segment sums must fit in registers next to the accumulators
-  int n = (op.cout_p % 128 == 0) ? 128 : 64;
-  if (!tc_stages(op.k, roll, n, false)) n = 64;
-  return n;
-}
-int tc_stages_for(const Op& op, const TensorView& out, bool roll) {
-  const int n = tc_pick_n(op, out, roll);
-  return tc_stages(op.k, roll, n, tc_is_tn(op.k, roll, n, out.dt == DType::F32));
+  return (op.cout_p % 128 == 0) ? 128 : 64;
 }
 // row blocks per CTA: minimise (waves over the SMs) x (blocks per CTA + ~1 block of prologue / halo overhead)
 int tc_blocks_per_cta(long columns, int total_pairs, double overhead) {
@@ -1373,8 +1370,6 @@ void plan_stack(ConvTcPlan& plan, void* w, int cout_rows) {
   }
   plan.rows_ratio = static_cast<double>(rows + (K - 1) * runs) / static_cast<double>(rows);
   plan.grid = dim3(static_cast<unsigned>(ctas), 1, 1);
-  plan.smem = stack_smem_bytes(K);
-  plan.stack = true;
 }
 }  // namespace
 
@@ -1383,30 +1378,32 @@ bool conv_tc_supported(const Op& op, const TensorView& in, const TensorView& out
   if (op.k != 1 && op.k != 3 && op.k != 7) return false;
   if (op.cout_p > kMaxCout) return false;
   if (op.fold_kw) {
-    if (in.cs != 8 || op.cin_p != 64 || (op.k != 3 && op.k != 7) || out.dt != DType::F16 || op.cout % 64 || out.cs != op.cout) return false;
-    return tc_stages_for(op, out, true) > 0;
+    return in.cs == 8 && op.cin_p == 64 && (op.k == 3 || op.k == 7) && out.dt == DType::F16 && op.cout % 64 == 0 && out.cs == op.cout;
   }
   if (op.split) {  // `in` = the [hi Cin | lo Cin] half planes of the float input
     if (op.cin % 64 || in.cs != 2 * op.cin || out.dt != DType::F32) return false;
-    if (!((out.cs == op.cout && op.cout % 64 == 0) || (out.cs == 16 && op.cout <= 16))) return false;
-    return tc_stages_for(op, out, false) > 0;
+    return (out.cs == op.cout && op.cout % 64 == 0) || (out.cs == 16 && op.cout <= 16);
   }
   if (in.cs % 64 || op.cin != in.cs) return false;
-  if (out.dt == DType::F16) {
-    if (op.cout % 64 || out.cs != op.cout) return false;
-  } else {
-    if (out.cs != 16 || op.cout > 16) return false;  // float logits, 16-channel pixels
-  }
-  const bool roll = in.cs == 64;
-  return tc_stages_for(op, out, roll) > 0;
+  if (out.dt == DType::F16) return op.cout % 64 == 0 && out.cs == op.cout;
+  return out.cs == 16 && op.cout <= 16;  // float logits, 16-channel pixels
 }
 
 std::shared_ptr<ConvTcPlan> conv_tc_plan(const Op& op, const TensorView& in, const TensorView& out, const void* w_tc) {
   auto plan = std::make_shared<ConvTcPlan>();
   const int K = op.k;
   const int KW = op.fold_kw ? 1 : K;
-  const bool roll = (in.cs == 64 || op.fold_kw) && !op.split;
-  const int n_tile = tc_pick_n(op, out, roll);
+  const int n_tile = tc_pick_n(op, out);
+  plan->k = K;
+  plan->kw = KW;
+  TcParams& p = plan->p;
+  p.H = in.h; p.W = op.fold_kw ? in.w - 8 : in.w; p.N_batch = in.n;
+  p.cout_total = out.cs;
+  p.n_tile = n_tile;
+  p.chunks = op.fold_kw ? 1 : in.cs / 64;
+  p.out_f32 = out.dt == DType::F32 ? (n_tile == 16 ? 1 : 2) : 0;
+  p.split = op.split ? 1 : 0;
+  const bool roll = tc_roll(p), pk2 = tc_pk2(*plan);
   if (op.fold_kw) {
     // window-folded input: `in` is the zero-padded 8-channel image [N][H][W + 8][8] half (3 zero pixels left, 5 right);
     // "pixel" x of the operand is the 128-byte window of 8 pixels x 8 channels starting at padded pixel x, i.e. image
@@ -1423,8 +1420,7 @@ std::shared_ptr<ConvTcPlan> conv_tc_plan(const Op& op, const TensorView& in, con
                           static_cast<cuuint64_t>(in.n)};
     cuuint64_t strides[3] = {static_cast<cuuint64_t>(in.cs) * 2, static_cast<cuuint64_t>(in.w) * in.cs * 2,
                              static_cast<cuuint64_t>(in.h) * in.w * in.cs * 2};
-    plan->pk2 = !roll && !op.split && K == 3 && in.w <= 64 && in.n >= 2 && n_tile != 16;
-    cuuint32_t box[4] = {64, static_cast<cuuint32_t>(plan->pk2 ? 64 : 128 + K - 1), 1, 1};
+    cuuint32_t box[4] = {64, static_cast<cuuint32_t>(pk2 ? 64 : 128 + K - 1), 1, 1};
     encode(&plan->map_a, in.p, 4, dims, strides, box);
   }
   {  // weights: [tap][cout_p][cin_p] half, dims (cin, cout, tap)
@@ -1434,20 +1430,13 @@ std::shared_ptr<ConvTcPlan> conv_tc_plan(const Op& op, const TensorView& in, con
     cuuint32_t box[3] = {64, static_cast<cuuint32_t>(n_tile), 1};
     encode(&plan->map_b, const_cast<void*>(w_tc), 3, dims, strides, box);
   }
-  TcParams& p = plan->p;
-  p.H = in.h; p.W = op.fold_kw ? in.w - 8 : in.w; p.N_batch = in.n;
-  p.cout_total = out.cs;
-  p.n_tile = n_tile;
-  p.chunks = op.fold_kw ? 1 : in.cs / 64;
-  p.out_f32 = out.dt == DType::F32 ? (n_tile == 16 ? 1 : 2) : 0;
-  p.split = op.split ? 1 : 0;
   p.cin_real = op.cin;
   p.acc_scale = op.split ? op.acc_scale : 1.f;
   p.seg_rows = 1;  // a segment per (chunk, tap row): 7x7 56 / 28 accumulate steps, 3x3 24 / 12, 1x1 8 / 4
   p.rz_comp = 0.216f * 1.1920929e-7f;  // x 2^-23
   p.strips = ceil_div(p.W, 128);
   const int cout_tiles = p.out_f32 == 1 ? 1 : op.cout_p / n_tile;
-  const int n_z = plan->pk2 ? ceil_div(in.n, 2) : in.n;  // PK2: an image pair per tile
+  const int n_z = pk2 ? ceil_div(in.n, 2) : in.n;  // PK2: an image pair per tile
   const int columns = p.strips * n_z * cout_tiles;
   const int total_pairs = ceil_div(in.h, kRows);
   p.pairs_per_cta = tc_blocks_per_cta(columns, total_pairs, roll ? (K - 1.0) / kRows * 0.5 + 0.5 : 0.3);
@@ -1467,14 +1456,8 @@ std::shared_ptr<ConvTcPlan> conv_tc_plan(const Op& op, const TensorView& in, con
   p.pool_out = nullptr; p.pool_mask = nullptr;
   p.has_cls = 0; p.cls_out = nullptr;
   plan->grid = dim3(p.strips * ceil_div(total_pairs, p.pairs_per_cta), cout_tiles, n_z);
-  plan->tn = tc_is_tn(K, roll, n_tile, p.out_f32 != 0);
-  p.b_stages = tc_stages(K, roll, n_tile, plan->tn);
-  plan->smem = tc_smem_bytes(K, roll, n_tile, p.b_stages, plan->tn);
-  plan->k = K;
-  plan->kw = KW;
-  plan->roll = roll;
-  if (roll && n_tile == 16 && K > 1) plan_stack(*plan, const_cast<void*>(w_tc), op.cout_p);
-  conv_tc_dispatch(*plan, nullptr, true);
+  if (tc_stacked(*plan)) plan_stack(*plan, const_cast<void*>(w_tc), op.cout_p);
+  tc_choose_kernel(*plan);
   return plan;
 }
 
@@ -1496,13 +1479,13 @@ void conv_tc_set_unpool(ConvTcPlan& plan, const uint8_t* mask, int mask_n, void*
 }
 
 void conv_tc_set_unpool_input(ConvTcPlan& plan, const void* pooled, const uint8_t* mask, int mask_n, int h, int w) {
-  if (!plan.stack || plan.k != 7 || 2 * h != plan.p.H || 2 * w != plan.p.W || !pooled || !mask || mask_n < 1)
+  if (!tc_stacked(plan) || plan.k != 7 || 2 * h != plan.p.H || 2 * w != plan.p.W || !pooled || !mask || mask_n < 1)
     fail(SIVO_EINVAL, "conv_tc_set_unpool_input: needs a 7x7 float-logits plan over the %d x %d unpooled input (got %d x %d pooled)",
          plan.p.H, plan.p.W, h, w);
   plan.p.unpool_in = static_cast<const __half*>(pooled);
   plan.p.unpool_mask = mask;
   plan.p.mask_n = mask_n;
-  conv_tc_dispatch(plan, nullptr, true);
+  tc_choose_kernel(plan);
 }
 
 std::vector<__half> conv_tc_split_weights(const float* W, int cout, int cin, int K, int cout_p, int cin_p, float* acc_scale) {
@@ -1539,7 +1522,7 @@ void conv_tc_set_pool(ConvTcPlan& plan, void* pooled, uint8_t* mask) {
 }
 
 bool conv_tc_can_fuse_classifier(const ConvTcPlan& plan) {
-  return plan.roll && plan.kw == plan.k && plan.p.n_tile == 64 && plan.p.cout_total == 64 && !plan.p.out_f32 && !plan.p.unpool_mask &&
+  return tc_roll(plan.p) && plan.kw == plan.k && plan.p.n_tile == 64 && plan.p.cout_total == 64 && !plan.p.out_f32 && !plan.p.unpool_mask &&
          !plan.p.has_drop && !plan.p.pool_out;
 }
 
@@ -1549,15 +1532,11 @@ void conv_tc_set_classifier(ConvTcPlan& plan, const float* w_cin_by_cout, int st
   for (int j = 0; j < 16; ++j) plan.cst.cls_b[j] = j < n_bias ? bias[j] : 0.f;
   plan.p.has_cls = 1;
   plan.p.cls_out = logits;
-  // the two-step classifier epilogue is k_conv_tc's
-  plan.tn = false;
-  plan.p.b_stages = tc_stages(plan.k, true, 64, false);
-  plan.smem = tc_smem_bytes(plan.k, true, 64, plan.p.b_stages, false);
-  conv_tc_dispatch(plan, nullptr, true);
+  tc_choose_kernel(plan);  // the two-step classifier epilogue is k_conv_tc's
 }
 
 bool conv_tc_can_compose_classifier(const ConvTcPlan& plan) {
-  return plan.roll && plan.k == 7 && plan.kw == 7 && plan.p.n_tile == 64 && !plan.p.out_f32 && !plan.p.unpool_mask &&
+  return tc_roll(plan.p) && plan.k == 7 && plan.kw == 7 && plan.p.n_tile == 64 && !plan.p.out_f32 && !plan.p.unpool_mask &&
          !plan.p.has_drop && !plan.p.pool_out && !plan.p.has_cls && !plan.p.relu && !plan.p.has_bn && plan.p.cout_total == 64;
 }
 
@@ -1588,14 +1567,13 @@ void conv_tc_set_composed_classifier(ConvTcPlan& plan, const Op& conv, const flo
   plan.p.cout_total = 16;
   plan.p.out = logits;
   plan_stack(plan, plan.w_own.p, 16);
-  conv_tc_dispatch(plan, nullptr, true);
+  tc_choose_kernel(plan);
 }
 
 double conv_tc_rows_ratio(const ConvTcPlan& plan) { return plan.rows_ratio; }
 
-void conv_tc_launch(const ConvTcPlan& plan, const Op& op, cudaStream_t s) {
-  (void)op;
-  conv_tc_dispatch(plan, s, false);
+void conv_tc_launch(const ConvTcPlan& plan, cudaStream_t s) {
+  plan.kern<<<plan.grid, kTcThreads, plan.smem, s>>>(plan.map_a, plan.map_b, plan.p, plan.cst);
   SIVO_CUDA(cudaGetLastError());
 }
 

@@ -463,7 +463,7 @@ void SegNet::enqueue(const uint8_t* bgr_dev, uint8_t* classes_dev, double* conf_
             launch_split_hilo(tensors_[op.in]->v, op.a_split.p, s);
             ++launches;
           }
-          conv_tc_launch(*op.tc, op, s);
+          conv_tc_launch(*op.tc, s);
         } else {
           ConvParams p;
           p.in = tensors_[op.in]->v;

@@ -163,7 +163,7 @@ class SegNet {
 // conv_tc.cu -- wgmma implicit-GEMM convolution
 bool conv_tc_supported(const Op& op, const TensorView& in, const TensorView& out);
 std::shared_ptr<ConvTcPlan> conv_tc_plan(const Op& op, const TensorView& in, const TensorView& out, const void* w_tc);
-void conv_tc_launch(const ConvTcPlan& plan, const Op& op, cudaStream_t s);
+void conv_tc_launch(const ConvTcPlan& plan, cudaStream_t s);
 // input rows whose MMAs the plan's kernel runs per output row: > 1 for the tap-row-stacked float-logits kernel (warm-up rows)
 double conv_tc_rows_ratio(const ConvTcPlan& plan);
 // fuses the sampling Dropout that follows the convolution in place into its epilogue
