@@ -615,42 +615,6 @@ void download_nchw(TensorView v, float* dst) {
   launch_act_to_nchw(v, tmp.as<float>(), nullptr);
   SIVO_CUDA(cudaMemcpy(dst, tmp.p, count * sizeof(float), cudaMemcpyDeviceToHost));
 }
-// the convolution op of the conv test hooks, weights through the same preparation the executor uses
-Op dbg_conv_op(DType dt, int cin, int cs_in, const float* weight, const float* bias, const float* bn_scale, const float* bn_shift,
-               int cout, int k, int pad, int relu) {
-  Op op;
-  op.kind = Op::Conv;
-  op.layer = "dbg_conv";
-  op.k = k; op.pad = pad; op.cin = cin; op.cout = cout; op.cin_p = cs_in; op.cout_p = (cout + 63) / 64 * 64;
-  op.relu = relu != 0;
-  auto th = [&](float x) { return dt == DType::F16 ? __half2float(__float2half_rn(x)) : x; };
-  std::vector<float> ws(static_cast<size_t>(k) * k * op.cin_p * op.cout_p, 0.f);
-  std::vector<__half> wt(static_cast<size_t>(k) * k * op.cout_p * op.cin_p, __float2half_rn(0.f));
-  for (int co = 0; co < cout; ++co)
-    for (int ci = 0; ci < cin; ++ci)
-      for (int t = 0; t < k * k; ++t) {
-        float v = weight[(static_cast<size_t>(co) * cin + ci) * k * k + t];
-        ws[(static_cast<size_t>(t) * op.cin_p + ci) * op.cout_p + co] = th(v);
-        wt[(static_cast<size_t>(t) * op.cout_p + co) * op.cin_p + ci] = __float2half_rn(v);
-      }
-  std::vector<float> b(op.cout_p, 0.f), sc(op.cout_p, 1.f), sh(op.cout_p, 0.f);
-  if (bias) std::copy(bias, bias + cout, b.begin());
-  if (bn_scale) std::copy(bn_scale, bn_scale + cout, sc.begin());
-  if (bn_shift) std::copy(bn_shift, bn_shift + cout, sh.begin());
-  op.h_bias = b; op.h_bn_scale = sc; op.h_bn_shift = sh;
-  op.w_simt.alloc(ws.size() * 4);
-  op.w_tc.alloc(wt.size() * 2);
-  op.bias.alloc(b.size() * 4);
-  op.bn_scale.alloc(sc.size() * 4);
-  op.bn_shift.alloc(sh.size() * 4);
-  SIVO_CUDA(cudaMemcpy(op.w_simt.p, ws.data(), ws.size() * 4, cudaMemcpyHostToDevice));
-  SIVO_CUDA(cudaMemcpy(op.w_tc.p, wt.data(), wt.size() * 2, cudaMemcpyHostToDevice));
-  SIVO_CUDA(cudaMemcpy(op.bias.p, b.data(), b.size() * 4, cudaMemcpyHostToDevice));
-  SIVO_CUDA(cudaMemcpy(op.bn_scale.p, sc.data(), sc.size() * 4, cudaMemcpyHostToDevice));
-  SIVO_CUDA(cudaMemcpy(op.bn_shift.p, sh.data(), sh.size() * 4, cudaMemcpyHostToDevice));
-  op.has_bn = bn_scale != nullptr;
-  return op;
-}
 }  // namespace
 
 int sivo_dbg_pool(int device, const float* in, int n, int c, int h, int w, float* out, int* mask) {
@@ -761,36 +725,21 @@ int sivo_dbg_conv(int device, int engine, int precision, const float* in, int n,
     DType odt = (cout % 8) ? DType::F32 : dt;
     TensorView vo = make_view(bo, n, cout, h, w, cs_out, odt);
     upload_nchw(in, vi);
-    Op op = dbg_conv_op(dt, cin, cs_in, weight, bias, bn_scale, bn_shift, cout, k, pad, relu);
-    // tensors for the tc plan live in a scratch vector; run on the default stream
+    Op op;  // the network's convolution op, prepared and launched as SegNet does
+    op.kind = Op::Conv;
+    op.layer = "dbg_conv";
+    op.k = k; op.pad = pad; op.cin = cin; op.cout = cout; op.cin_p = cs_in; op.cout_p = (cout + 63) / 64 * 64;
+    op.relu = relu != 0;
     if (engine == SIVO_ENGINE_TCGEN05 && dt == DType::F32) {  // split-operand fp32 mode
-      TensorView vs = vi;
-      vs.dt = DType::F16;
-      vs.cs = 2 * vi.cs;
-      op.split = true;
-      if (cin % 64 || !conv_tc_supported(op, vs, vo)) fail(SIVO_EINVAL, "conv: shape not supported by the split-operand tcgen05 mode");
-      std::vector<__half> wsplit = conv_tc_split_weights(weight, cout, cin, k, op.cout_p, op.cin_p, &op.acc_scale);
-      op.w_tc.alloc(wsplit.size() * 2);
-      SIVO_CUDA(cudaMemcpy(op.w_tc.p, wsplit.data(), wsplit.size() * 2, cudaMemcpyHostToDevice));
-      op.a_split.alloc(vs.elems() * 2);
-      vs.p = op.a_split.p;
-      op.tc = conv_tc_plan(op, vs, vo, op.w_tc.p);
-      launch_split_hilo(vi, op.a_split.p, nullptr);
-      conv_tc_launch(*op.tc, nullptr);
+      op.split = op.use_tc = true;
+      if (cin % 64 || !conv_tc_supported(op, split_view(vi), vo))
+        fail(SIVO_EINVAL, "conv: shape not supported by the split-operand tcgen05 mode");
     } else if (engine == SIVO_ENGINE_TCGEN05) {
+      op.use_tc = true;
       if (dt != DType::F16 || !conv_tc_supported(op, vi, vo)) fail(SIVO_EINVAL, "conv: shape not supported by the tcgen05 engine");
-      op.tc = conv_tc_plan(op, vi, vo, op.w_tc.p);
-      conv_tc_launch(*op.tc, nullptr);
-    } else {
-      ConvParams p;
-      p.in = vi; p.out = vo;
-      p.w_simt = op.w_simt.as<float>();
-      p.bias = op.bias.as<float>();
-      p.bn_scale = op.has_bn ? op.bn_scale.as<float>() : nullptr;
-      p.bn_shift = op.has_bn ? op.bn_shift.as<float>() : nullptr;
-      p.k = k; p.pad = pad; p.cin_p = op.cin_p; p.cout_p = op.cout_p; p.relu = op.relu; p.slope = 0.f;
-      launch_conv_simt(p, nullptr);
     }
+    prepare_conv(op, dt, weight, bias, bn_scale, bn_shift, vi, vo);
+    launch_conv(op, vi, vo, nullptr);
     SIVO_CUDA(cudaDeviceSynchronize());
     download_nchw(vo, out);
     SIVO_CUDA(cudaDeviceSynchronize());
@@ -811,14 +760,18 @@ int sivo_dbg_conv_unpooled(int device, const float* pooled, const int* mask, int
     upload_nchw(pooled, vp);
     SIVO_CUDA(cudaMemcpy(bmi.p, mask, mask_cnt * sizeof(int), cudaMemcpyHostToDevice));
     launch_mask_from_nchw(bmi.as<int>(), mask_n, 64, h, w, bm.as<uint8_t>(), nullptr);
-    Op op = dbg_conv_op(DType::F16, 64, 64, weight, bias, bn_scale, bn_shift, cout, k, (k - 1) / 2, 0);
+    Op op;
+    op.kind = Op::Conv;
+    op.layer = "dbg_conv_unpooled";
+    op.k = k; op.pad = (k - 1) / 2; op.cin = op.cin_p = 64; op.cout = cout; op.cout_p = 64;
+    op.use_tc = true;
     TensorView vu = vp;  // the unpooled input's shape: the plan is made for it, and then reads the pooled tensor instead
     vu.h = 2 * h;
     vu.w = 2 * w;
     if (!conv_tc_supported(op, vu, vo)) fail(SIVO_EINVAL, "conv_unpooled: shape not supported by the tensor-core kernel");
-    op.tc = conv_tc_plan(op, vu, vo, op.w_tc.p);
+    prepare_conv(op, DType::F16, weight, bias, bn_scale, bn_shift, vu, vo);
     conv_tc_set_unpool_input(*op.tc, vp.p, bm.as<uint8_t>(), mask_n, h, w);
-    conv_tc_launch(*op.tc, nullptr);
+    launch_conv(op, vu, vo, nullptr);
     SIVO_CUDA(cudaDeviceSynchronize());
     download_nchw(vo, out);
     SIVO_CUDA(cudaDeviceSynchronize());

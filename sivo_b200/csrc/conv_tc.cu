@@ -19,13 +19,13 @@
 //  * 384 threads = three warpgroups.  Warpgroup 0 produces (warp 0: halo rows, warp 1: weights; setmaxnreg 40);
 //    warpgroups 1 and 2 consume (setmaxnreg 232): consumer g owns pixels [64 g, 64 g + 64) of the tile, issues the
 //    m64nNk16 wgmma of both rows of the block into register accumulators, and runs the epilogue on them -- bias / BN
-//    affine / ReLU -> half, then store | dropout | max-unpool scatter | 2x2 max-pool + argmax | 1x1 classifier -> float
-//    logits.  Both consumers read every weight stage, so they reach a block's epilogue together and no MMA is issued
-//    while it runs.  The 64-wide store / dropout / unpool epilogues are therefore deferred: a block's outputs are
-//    converted and staged in registers (16 B per lane after a quad transpose), and their stores are issued one slice per
-//    tap row between the next block's MMA commits, so they drain under the tensor core's work.
-//  * Constants (bias, BN, classifier weights) are kernel parameters: the epilogue reads them from the constant bank and
-//    leaves the shared-memory data path to the MMA operand reads.
+//    affine / ReLU -> half, then store | dropout | max-unpool scatter | 2x2 max-pool + argmax, or -> float logits.  Both
+//    consumers read every weight stage, so they reach a block's epilogue together and no MMA is issued while it runs.
+//    The 64-wide store / dropout / unpool epilogues are therefore deferred: a block's outputs are converted and staged in
+//    registers (16 B per lane after a quad transpose), and their stores are issued one slice per tap row between the next
+//    block's MMA commits, so they drain under the tensor core's work.
+//  * Constants (bias, BN) are kernel parameters: the epilogue reads them from the constant bank and leaves the
+//    shared-memory data path to the MMA operand reads.
 //  * The Cin = 64, 7x7 layers with 64-wide half output tiles (Basic's conv1 .. conv_decode2) run on k_conv_tn instead: the
 //    same producers and rings with the GEMM transposed -- the weights as M, all 128 pixels of a row as N -- and an
 //    epilogue staged through shared memory.
@@ -92,10 +92,6 @@ struct TcParams {
   // written (pooling_layer.cpp:140-187: scan (0,0),(0,1),(1,0),(1,1), strict '>', so the first maximum wins)
   __half* pool_out;        // [N][H/2][W/2][cout_total]
   uint8_t* pool_mask;      // same shape
-  // 1x1 classifier fused into the epilogue (the layer feeding Softmax): logits[j] = cls_b[j] + sum_c half(out[c]) * cls_w[c][j];
-  // the 64-channel output itself is then never written
-  int has_cls;
-  float* cls_out;          // [N][H][W][16]
   // k_conv_stack<K, true>: the input is the max-unpool of this pooled tensor [N][H/2][W/2][64] by unpool_mask (same shape,
   // batch mask_n), expanded as the halo rows are loaded; the 2H x 2W unpooled tensor is never stored
   const __half* unpool_in;
@@ -105,8 +101,6 @@ struct TcParams {
 constexpr int kMaxCout = 512;
 struct TcConsts {
   float bias[kMaxCout], bn_scale[kMaxCout], bn_shift[kMaxCout];
-  float cls_w[64 * 16];    // fused classifier: [cin][16] float (half-rounded values), j >= classes zero
-  float cls_b[16];
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
@@ -269,22 +263,6 @@ __device__ __forceinline__ float affine(const TcParams& p, const TcConsts& cst, 
   return t;
 }
 
-// Fused 1x1 classifier, one quad lane's share: partial logits over its 16 channels (8 j + 2 Q + e) of pixel h.
-template <int Q>
-__device__ __forceinline__ void cls_partial(const TcParams& p, const TcConsts& cst, const float (&a)[32], int h, float (&l)[16]) {
-#pragma unroll
-  for (int jj = 0; jj < 16; ++jj) l[jj] = 0.f;
-#pragma unroll
-  for (int j = 0; j < 8; ++j)
-#pragma unroll
-    for (int e = 0; e < 2; ++e) {
-      const int c = 8 * j + 2 * Q + e;
-      const float hv = __half2float(__float2half_rn(affine(p, cst, a[4 * j + 2 * h + e], c)));
-#pragma unroll
-      for (int jj = 0; jj < 16; ++jj) l[jj] = fmaf(hv, cst.cls_w[c * 16 + jj], l[jj]);
-    }
-}
-
 // Epilogue of one row block for one consumer thread.  The thread holds, per output row r, pixels m0 and m0 + 8 of its
 // consumer's 64 (h = 0, 1) and channels 8 j + 2 q + e (q = lane % 4) of each: acc[r][4 j + 2 h + e].  `x_m0` = image column
 // of pixel m0, `y0` = first row of the block, `n0` = first output channel of the CTA's tile.  Called by all 32 lanes
@@ -321,29 +299,6 @@ __device__ __forceinline__ void epilogue_block(const TcParams& p, const TcConsts
   for (int r = 0; r < kRows; ++r) {
     const int y = y0 + r;
     const bool row_ok = y < p.H && img_ok;
-    if constexpr (N == 64) if (p.has_cls) {  // conv (+bias) -> half rounding (as the unfused path stores it) -> 1x1 classifier -> float logits
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        float l[16];
-        switch (q) {  // one copy per quad lane, so that the classifier weights are compile-time constant-bank operands
-          case 0: cls_partial<0>(p, cst, acc[r], h, l); break;
-          case 1: cls_partial<1>(p, cst, acc[r], h, l); break;
-          case 2: cls_partial<2>(p, cst, acc[r], h, l); break;
-          default: cls_partial<3>(p, cst, acc[r], h, l); break;
-        }
-#pragma unroll
-        for (int jj = 0; jj < 16; ++jj) {  // the four lanes of a pixel hold a quarter of its channels each
-          l[jj] += __shfl_xor_sync(0xffffffffu, l[jj], 1);
-          l[jj] += __shfl_xor_sync(0xffffffffu, l[jj], 2);
-          l[jj] = __fadd_rn(l[jj], cst.cls_b[jj]);
-        }
-        const int x = x_m0 + 8 * h;
-        const float4 v = q == 0 ? make_float4(l[0], l[1], l[2], l[3]) : q == 1 ? make_float4(l[4], l[5], l[6], l[7])
-                       : q == 2 ? make_float4(l[8], l[9], l[10], l[11]) : make_float4(l[12], l[13], l[14], l[15]);
-        if (row_ok && x < p.W) *reinterpret_cast<float4*>(p.cls_out + ((static_cast<size_t>(img) * p.H + y) * p.W + x) * 16 + 4 * q) = v;
-      }
-      continue;
-    }
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int x = x_m0 + 8 * h;
@@ -647,7 +602,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUt
   // N = 64 store / dropout / unpool epilogues are deferred: block j's outputs are staged in registers, and their stores go
   // out one slice per tap row of block j + 1, right after that tap row's first MMA group is committed, so they drain while
   // the tensor core works (the last block's are flushed at the end).  The walk is instantiated once per epilogue kind so
-  // that the staged registers are not live next to the immediate epilogues (pool, classifier), which would then spill.
+  // that the staged registers are not live next to the immediate pool epilogue, which would then spill.
   constexpr bool kDefer = N == 64 && !SPLIT;
   auto walk = [&](auto defer_tag) {
     constexpr bool D = decltype(defer_tag)::value;
@@ -761,7 +716,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUt
     }
   };
   if constexpr (kDefer) {
-    if (!p.pool_out && !p.has_cls && !p.out_f32) walk(std::true_type{});
+    if (!p.pool_out && !p.out_f32) walk(std::true_type{});
     else walk(std::false_type{});
   } else {
     walk(std::false_type{});
@@ -1278,10 +1233,10 @@ void tc_choose_kernel(ConvTcPlan& plan) {
   TcParams& p = plan.p;
   const int K = plan.k, n = p.n_tile;
   const bool roll = tc_roll(p);
-  // k_conv_tn runs every Cin = 64, K = 7 layer with 64-wide half output tiles but the two-step classifier epilogue.  The
-  // K = 3 layers stay on k_conv_tc: on k_conv_tn Standard's conv1_2_D (352 x 1024, T = 12) took 0.75 ms in one session and
-  // 1.77 ms in another, against k_conv_tc's steady 1.35 ms (H100 80GB HBM3, 700 W).
-  const bool tn = roll && n == 64 && K == 7 && !p.out_f32 && !p.has_cls;
+  // k_conv_tn runs every Cin = 64, K = 7 layer with 64-wide half output tiles.  The K = 3 layers stay on k_conv_tc: on
+  // k_conv_tn Standard's conv1_2_D (352 x 1024, T = 12) took 0.75 ms in one session and 1.77 ms in another, against
+  // k_conv_tc's steady 1.35 ms (H100 80GB HBM3, 700 W).
+  const bool tn = roll && n == 64 && K == 7 && !p.out_f32;
   // per (K, ROLL, KW, PK2): the three tile widths
   auto by_n = [n](TcKernel k16, TcKernel k64, TcKernel k128) { return n == 16 ? k16 : n == 64 ? k64 : k128; };
   if (tc_stacked(plan)) {
@@ -1298,8 +1253,7 @@ void tc_choose_kernel(ConvTcPlan& plan) {
     } else if (tc_pk2(plan)) {
       plan.kern = n == 64 ? k_conv_tc<3, false, 3, true, 64, false> : k_conv_tc<3, false, 3, true, 128, false>;
     } else if (roll) {
-      // 64-wide K = 7 tiles get here only with the two-step classifier epilogue (conv_tc_set_classifier)
-      if (K == 7) plan.kern = n == 64 ? k_conv_tc<7, true, 7, false, 64, false> : k_conv_tc<7, true, 7, false, 128, false>;
+      if (K == 7) plan.kern = k_conv_tc<7, true, 7, false, 128, false>;  // 64-wide K = 7 tiles run on k_conv_tn
       else if (K == 3) plan.kern = n == 64 ? k_conv_tc<3, true, 3, false, 64, false> : k_conv_tc<3, true, 3, false, 128, false>;
       else plan.kern = by_n(k_conv_tc<1, true, 1, false, 16, false>, k_conv_tc<1, true, 1, false, 64, false>, k_conv_tc<1, true, 1, false, 128, false>);
     } else {
@@ -1454,7 +1408,6 @@ std::shared_ptr<ConvTcPlan> conv_tc_plan(const Op& op, const TensorView& in, con
   p.has_drop = 0; p.seed = 0; p.frame = nullptr; p.drop_nl = 0; p.drop_scale = 2.f;
   p.unpool_mask = nullptr; p.mask_n = 1; p.unpool_in = nullptr;
   p.pool_out = nullptr; p.pool_mask = nullptr;
-  p.has_cls = 0; p.cls_out = nullptr;
   plan->grid = dim3(p.strips * ceil_div(total_pairs, p.pairs_per_cta), cout_tiles, n_z);
   if (tc_stacked(*plan)) plan_stack(*plan, const_cast<void*>(w_tc), op.cout_p);
   tc_choose_kernel(*plan);
@@ -1513,7 +1466,7 @@ std::vector<__half> conv_tc_split_weights(const float* W, int cout, int cin, int
 }
 
 bool conv_tc_can_fuse_pool(const ConvTcPlan& plan) {
-  return !plan.p.out_f32 && !plan.p.unpool_mask && !plan.p.has_drop && !plan.p.has_cls && (plan.p.H % 2) == 0 && (plan.p.W % 2) == 0;
+  return !plan.p.out_f32 && !plan.p.unpool_mask && !plan.p.has_drop && (plan.p.H % 2) == 0 && (plan.p.W % 2) == 0;
 }
 
 void conv_tc_set_pool(ConvTcPlan& plan, void* pooled, uint8_t* mask) {
@@ -1521,23 +1474,9 @@ void conv_tc_set_pool(ConvTcPlan& plan, void* pooled, uint8_t* mask) {
   plan.p.pool_mask = mask;
 }
 
-bool conv_tc_can_fuse_classifier(const ConvTcPlan& plan) {
-  return tc_roll(plan.p) && plan.kw == plan.k && plan.p.n_tile == 64 && plan.p.cout_total == 64 && !plan.p.out_f32 && !plan.p.unpool_mask &&
-         !plan.p.has_drop && !plan.p.pool_out;
-}
-
-void conv_tc_set_classifier(ConvTcPlan& plan, const float* w_cin_by_cout, int stride, const float* bias, int n_bias, float* logits) {
-  for (int c = 0; c < 64; ++c)
-    for (int j = 0; j < 16; ++j) plan.cst.cls_w[c * 16 + j] = j < stride ? w_cin_by_cout[static_cast<size_t>(c) * stride + j] : 0.f;
-  for (int j = 0; j < 16; ++j) plan.cst.cls_b[j] = j < n_bias ? bias[j] : 0.f;
-  plan.p.has_cls = 1;
-  plan.p.cls_out = logits;
-  tc_choose_kernel(plan);  // the two-step classifier epilogue is k_conv_tc's
-}
-
 bool conv_tc_can_compose_classifier(const ConvTcPlan& plan) {
   return tc_roll(plan.p) && plan.k == 7 && plan.kw == 7 && plan.p.n_tile == 64 && !plan.p.out_f32 && !plan.p.unpool_mask &&
-         !plan.p.has_drop && !plan.p.pool_out && !plan.p.has_cls && !plan.p.relu && !plan.p.has_bn && plan.p.cout_total == 64;
+         !plan.p.has_drop && !plan.p.pool_out && !plan.p.relu && !plan.p.has_bn && plan.p.cout_total == 64;
 }
 
 void conv_tc_set_composed_classifier(ConvTcPlan& plan, const Op& conv, const float* wc, const float* bc, int n_cls, float* logits) {
@@ -1560,7 +1499,7 @@ void conv_tc_set_composed_classifier(ConvTcPlan& plan, const Op& conv, const flo
   SIVO_CUDA(cudaMemcpy(plan.w_own.p, w.data(), w.size() * sizeof(__half), cudaMemcpyHostToDevice));
   std::memset(&plan.cst, 0, sizeof(TcConsts));
   for (int o = 0; o < n_cls; ++o) {
-    double acc = bc[o];
+    double acc = bc ? bc[o] : 0.0;
     for (int c = 0; c < 64; ++c) acc += static_cast<double>(wc[o * 64 + c]) * conv.h_bias[c];
     plan.cst.bias[o] = static_cast<float>(acc);
   }

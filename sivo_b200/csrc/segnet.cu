@@ -7,7 +7,6 @@
 
 #include <algorithm>
 #include <cmath>
-#include <cstdlib>
 #include <cstring>
 
 namespace sivo {
@@ -15,6 +14,11 @@ namespace sivo {
 namespace {
 int round_up(int a, int b) { return (a + b - 1) / b * b; }
 float through_half(float x) { return __half2float(__float2half_rn(x)); }
+template <typename T>
+void upload(DevBuf& buf, const std::vector<T>& v) {
+  buf.alloc(v.size() * sizeof(T));
+  SIVO_CUDA(cudaMemcpy(buf.p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
+}
 }  // namespace
 
 int SegNet::add_tensor(const std::string& name, int n, int c, int h, int w, int cs, DType dt, bool mask) {
@@ -31,7 +35,15 @@ int SegNet::add_tensor(const std::string& name, int n, int c, int h, int w, int 
   return id;
 }
 
-void SegNet::prepare_conv(Op& op, const std::vector<Blob>& cb, const std::vector<Blob>* bn) {
+TensorView split_view(TensorView v) {
+  v.p = nullptr;
+  v.dt = DType::F16;
+  v.cs *= 2;
+  return v;
+}
+
+void prepare_conv(Op& op, DType act, const float* W, const float* bias, const float* bn_scale, const float* bn_shift,
+                  const TensorView& in, const TensorView& out) {
   const int K = op.k, cin = op.fold_kw ? 3 : op.cin, cout = op.cout;
   const int taps = op.fold_kw ? K : K * K;
   auto slot = [&](int t, int ci, int& tap, int& cidx) {
@@ -40,26 +52,23 @@ void SegNet::prepare_conv(Op& op, const std::vector<Blob>& cb, const std::vector
     if (op.fold_kw) { tap = t / K; cidx = (t % K + 3 - (K - 1) / 2) * 8 + ci; }
     else { tap = t; cidx = ci; }
   };
-  if (cb.empty() || cb[0].shape.size() != 4 || cb[0].shape[0] != cout || cb[0].shape[1] != cin || cb[0].shape[2] != K ||
-      cb[0].shape[3] != K)
-    fail(SIVO_EFORMAT, "layer '%s': weight blob shape does not match (%d,%d,%d,%d) (net.cpp:750-785 would CHECK-fail)",
-         op.layer.c_str(), cout, cin, K, K);
-  const bool half = act_ == DType::F16;
-  const float* W = cb[0].data.data();
-  std::vector<float> ws(static_cast<size_t>(taps) * op.cin_p * op.cout_p, 0.f);
-  for (int co = 0; co < cout; ++co)
-    for (int ci = 0; ci < cin; ++ci)
-      for (int t = 0; t < K * K; ++t) {
-        float v = W[(static_cast<size_t>(co) * cin + ci) * K * K + t];
-        int tap, cidx;
-        slot(t, ci, tap, cidx);
-        ws[(static_cast<size_t>(tap) * op.cin_p + cidx) * op.cout_p + co] = half ? through_half(v) : v;
-      }
-  op.h_w = ws;
   op.h_w_raw.assign(W, W + static_cast<size_t>(cout) * cin * K * K);
-  op.w_simt.alloc(ws.size() * sizeof(float));
-  SIVO_CUDA(cudaMemcpy(op.w_simt.p, ws.data(), ws.size() * sizeof(float), cudaMemcpyHostToDevice));
-  if (half) {  // tensor-core layout: [tap][cout_p][cin_p] half, K(=cin)-major rows
+  op.h_bias.assign(op.cout_p, 0.f);
+  if (bias) std::copy(bias, bias + cout, op.h_bias.begin());
+  op.has_bn = bn_scale != nullptr;
+  if (op.has_bn) {
+    op.h_bn_scale.assign(op.cout_p, 1.f);
+    op.h_bn_shift.assign(op.cout_p, 0.f);
+    std::copy(bn_scale, bn_scale + cout, op.h_bn_scale.begin());
+    if (bn_shift) std::copy(bn_shift, bn_shift + cout, op.h_bn_shift.begin());
+  }
+  if (op.split) {
+    upload(op.w_tc, conv_tc_split_weights(W, cout, cin, K, op.cout_p, op.cin_p, &op.acc_scale));
+    TensorView planes = split_view(in);
+    op.a_split.alloc(planes.bytes());
+    planes.p = op.a_split.p;
+    op.tc = conv_tc_plan(op, planes, out, op.w_tc.p);
+  } else if (op.use_tc) {  // [tap][cout_p][cin_p] half, K(=cin)-major rows
     std::vector<__half> wt(static_cast<size_t>(taps) * op.cout_p * op.cin_p, __float2half_rn(0.f));
     for (int co = 0; co < cout; ++co)
       for (int ci = 0; ci < cin; ++ci)
@@ -69,37 +78,43 @@ void SegNet::prepare_conv(Op& op, const std::vector<Blob>& cb, const std::vector
           wt[(static_cast<size_t>(tap) * op.cout_p + co) * op.cin_p + cidx] =
               __float2half_rn(W[(static_cast<size_t>(co) * cin + ci) * K * K + t]);
         }
-    op.w_tc.alloc(wt.size() * sizeof(__half));
-    SIVO_CUDA(cudaMemcpy(op.w_tc.p, wt.data(), wt.size() * sizeof(__half), cudaMemcpyHostToDevice));
+    upload(op.w_tc, wt);
+    op.tc = conv_tc_plan(op, in, out, op.w_tc.p);
+  } else {  // [tap][cin_p][cout_p] float, through half for fp16 activations
+    std::vector<float> ws(static_cast<size_t>(taps) * op.cin_p * op.cout_p, 0.f);
+    for (int co = 0; co < cout; ++co)
+      for (int ci = 0; ci < cin; ++ci)
+        for (int t = 0; t < K * K; ++t) {
+          float v = W[(static_cast<size_t>(co) * cin + ci) * K * K + t];
+          int tap, cidx;
+          slot(t, ci, tap, cidx);
+          ws[(static_cast<size_t>(tap) * op.cin_p + cidx) * op.cout_p + co] = act == DType::F16 ? through_half(v) : v;
+        }
+    upload(op.w_simt, ws);
+    upload(op.bias, op.h_bias);
+    if (op.has_bn) {
+      upload(op.bn_scale, op.h_bn_scale);
+      upload(op.bn_shift, op.h_bn_shift);
+    }
   }
-  if (op.split) {
-    if (taps != K * K) fail(SIVO_EINVAL, "layer '%s': split-operand mode does not take window-folded first layers", op.layer.c_str());
-    std::vector<__half> wt = conv_tc_split_weights(W, cout, cin, K, op.cout_p, op.cin_p, &op.acc_scale);
-    op.w_tc.alloc(wt.size() * sizeof(__half));
-    SIVO_CUDA(cudaMemcpy(op.w_tc.p, wt.data(), wt.size() * sizeof(__half), cudaMemcpyHostToDevice));
+}
+
+void launch_conv(const Op& op, const TensorView& in, const TensorView& out, cudaStream_t s) {
+  if (op.use_tc) {
+    if (op.split) launch_split_hilo(in, op.a_split.p, s);  // the float input as [hi | lo] half planes
+    conv_tc_launch(*op.tc, s);
+    return;
   }
-  std::vector<float> b(op.cout_p, 0.f);
-  if (cb.size() > 1) {
-    if (static_cast<int>(cb[1].count()) != cout) fail(SIVO_EFORMAT, "layer '%s': bias blob size mismatch", op.layer.c_str());
-    std::copy(cb[1].data.begin(), cb[1].data.end(), b.begin());
-  }
-  op.h_bias = b;
-  op.bias.alloc(b.size() * sizeof(float));
-  SIVO_CUDA(cudaMemcpy(op.bias.p, b.data(), b.size() * sizeof(float), cudaMemcpyHostToDevice));
-  if (bn) {
-    if (bn->size() < 2 || static_cast<int>((*bn)[0].count()) != cout || static_cast<int>((*bn)[1].count()) != cout)
-      fail(SIVO_EFORMAT, "BN after '%s': expected scale and shift blobs of %d channels", op.layer.c_str(), cout);
-    std::vector<float> sc(op.cout_p, 1.f), sh(op.cout_p, 0.f);
-    std::copy((*bn)[0].data.begin(), (*bn)[0].data.end(), sc.begin());
-    std::copy((*bn)[1].data.begin(), (*bn)[1].data.end(), sh.begin());
-    op.h_bn_scale = sc;
-    op.h_bn_shift = sh;
-    op.bn_scale.alloc(sc.size() * sizeof(float));
-    op.bn_shift.alloc(sh.size() * sizeof(float));
-    SIVO_CUDA(cudaMemcpy(op.bn_scale.p, sc.data(), sc.size() * sizeof(float), cudaMemcpyHostToDevice));
-    SIVO_CUDA(cudaMemcpy(op.bn_shift.p, sh.data(), sh.size() * sizeof(float), cudaMemcpyHostToDevice));
-    op.has_bn = true;
-  }
+  ConvParams p;
+  p.in = in;
+  p.out = out;
+  p.w_simt = op.w_simt.as<float>();
+  p.bias = op.bias.as<float>();
+  p.bn_scale = op.has_bn ? op.bn_scale.as<float>() : nullptr;
+  p.bn_shift = op.has_bn ? op.bn_shift.as<float>() : nullptr;
+  p.k = op.k; p.pad = op.pad; p.cin_p = op.cin_p; p.cout_p = op.cout_p;
+  p.relu = op.relu; p.slope = op.slope;
+  launch_conv_simt(p, s);
 }
 
 void SegNet::build(const NetSpec& net, const WeightMap& weights) {
@@ -203,82 +218,71 @@ void SegNet::build(const NetSpec& net, const WeightMap& weights) {
         op.out = add_tensor(ly.tops[0], iv.n, op.cout, iv.h, iv.w, cs, logits ? DType::F32 : act_);
         auto it = weights.find(ly.name);
         if (it == weights.end()) fail(SIVO_EFORMAT, "caffemodel has no blobs for layer '%s'", ly.name.c_str());
-        // fp32 activations on the tensor-core engine: split-operand mode (three half MMAs per tap, fp32 accumulation)
-        TensorView split_in = civ;
-        if (act_ == DType::F32 && opt_.engine != SIVO_ENGINE_SIMT && !op.fold_kw && civ.cs % 64 == 0 && civ.c == civ.cs) {
-          split_in.dt = DType::F16;
-          split_in.cs = 2 * civ.cs;
-          op.split = true;
-          if (!conv_tc_supported(op, split_in, tensors_[op.out]->v)) op.split = false;
-        }
-        prepare_conv(op, it->second, bn);
+        const std::vector<Blob>& cb = it->second;
+        const int wcin = op.fold_kw ? 3 : op.cin;
+        if (cb.empty() || cb[0].shape.size() != 4 || cb[0].shape[0] != op.cout || cb[0].shape[1] != wcin || cb[0].shape[2] != op.k ||
+            cb[0].shape[3] != op.k)
+          fail(SIVO_EFORMAT, "layer '%s': weight blob shape does not match (%d,%d,%d,%d) (net.cpp:750-785 would CHECK-fail)",
+               op.layer.c_str(), op.cout, wcin, op.k, op.k);
+        if (cb.size() > 1 && static_cast<int>(cb[1].count()) != op.cout)
+          fail(SIVO_EFORMAT, "layer '%s': bias blob size mismatch", op.layer.c_str());
+        if (bn && (bn->size() < 2 || static_cast<int>((*bn)[0].count()) != op.cout || static_cast<int>((*bn)[1].count()) != op.cout))
+          fail(SIVO_EFORMAT, "BN after '%s': expected scale and shift blobs of %d channels", op.layer.c_str(), op.cout);
+        const float* w = cb[0].data.data();
+        const float* bias = cb.size() > 1 ? cb[1].data.data() : nullptr;
         op.flops = 2.0 * iv.c * ly.kernel * ly.kernel * op.cout * iv.h * iv.w * iv.n;  // algorithmic, whatever the mapping
-        op.flops_exec = op.split ? 3.0 * op.flops : op.flops;
         flops_dedup += op.flops;
         flops_naive += op.flops / iv.n * ns_;
         if (logits && !opt_.keep_blobs && op.k == 1 && op.cin == 64 && op.cout <= 16 && !op.relu && !bn && !ops_.empty() &&
-            ops_.back().kind == Op::Conv && ops_.back().use_tc && ops_.back().out == in && conv_tc_can_fuse_classifier(*ops_.back().tc)) {
-          // 1x1 classifier straight after a tensor-core convolution: computed in that convolution's epilogue from the
-          // half-rounded activations, so the 64-channel tensor is never written or re-read
-          // No non-linearity sits between the two layers (Basic), so logits = (Wc W) * x + (Wc b + bc): ONE 64 -> 16 convolution
-          // with weights composed in double and rounded to half once -- a quarter of the multiply-adds, and closer to the
-          // reference's fp32 arithmetic than the two-step half path (the 64-channel activation is never rounded to half;
-          // tests/test_gpu_parity.py, tools/compose_classifier_study.py).  Default; SIVO_B200_COMPOSE=0 keeps the two-step form.
-          const char* compose = std::getenv("SIVO_B200_COMPOSE");
+            ops_.back().kind == Op::Conv && ops_.back().use_tc && ops_.back().out == in && conv_tc_can_compose_classifier(*ops_.back().tc)) {
+          // 1x1 classifier straight after a tensor-core convolution with no non-linearity between them (Basic): logits =
+          // (Wc W) * x + (Wc b + bc), ONE 64 -> 16 convolution with weights composed in double and rounded to half once --
+          // a quarter of the multiply-adds, the 64-channel tensor is never written or re-read, and closer to the reference's
+          // fp32 arithmetic than the two layers in half (the 64-channel activation is never rounded to half;
+          // tests/test_gpu_parity.py, tools/compose_classifier_study.py).  The classifier's own weights are never uploaded.
           Op& conv = ops_.back();
-          if (!(compose && compose[0] == '0') && !conv.relu && !conv.has_bn && conv_tc_can_compose_classifier(*conv.tc)) {
-            conv_tc_set_composed_classifier(*conv.tc, conv, op.h_w_raw.data(), op.h_bias.data(), op.cout,
-                                            static_cast<float*>(tensors_[op.out]->v.p));
-            // the 16-wide composed layer, warm-up rows included
-            conv.flops_exec = 2.0 * conv.cin * conv.k * conv.k * 16 * iv.h * iv.w * iv.n * conv_tc_rows_ratio(*conv.tc);
-            conv.layer += "*" + ly.name;  // '*': composed, not merely fused
-            Op* up = ops_.size() >= 2 ? &ops_[ops_.size() - 2] : nullptr;
-            if (up && up->kind == Op::Conv && up->use_tc && up->out2 == conv.in) {
-              // the input is scattered by the previous convolution's fused unpool (Basic: conv_decode2 -> upsample1), three
-              // quarters zeros: take that fusion back.  The previous convolution stores its own pooled-resolution output, and
-              // the composed kernel unpools it as it loads its halo rows.  The unpooled tensor is derived, never written.
-              Tensor& pooled = *tensors_[up->out];
-              Tensor& unpooled = *tensors_[conv.in];
-              const Tensor& mask = *tensors_[up->in2];
-              conv_tc_set_unpool(*up->tc, nullptr, 1, pooled.v.p);
-              pooled.elided = false;
-              conv_tc_set_unpool_input(*conv.tc, pooled.v.p, mask.buf.as<uint8_t>(), mask.v.n, pooled.v.h, pooled.v.w);
-              unpooled.derived_from = up->out;
-              unpooled.derived_mask = up->in2;
-              unpooled.buf.release();
-              unpooled.v.p = nullptr;
-              const size_t plus = up->layer.rfind('+');  // the unpool is the last layer fused into it
-              conv.layer = up->layer.substr(plus + 1) + "+" + conv.layer;
-              up->layer.erase(plus);
-              up->in2 = up->out2 = -1;
-            }
-          } else {
-            conv_tc_set_classifier(*conv.tc, op.h_w.data(), op.cout_p, op.h_bias.data(), std::min(16, op.cout_p),
-                                   static_cast<float*>(tensors_[op.out]->v.p));
-            conv.flops_exec += op.flops;
-            conv.layer += "+" + ly.name;
+          conv_tc_set_composed_classifier(*conv.tc, conv, w, bias, op.cout, static_cast<float*>(tensors_[op.out]->v.p));
+          // the 16-wide composed layer, warm-up rows included
+          conv.flops_exec = 2.0 * conv.cin * conv.k * conv.k * 16 * iv.h * iv.w * iv.n * conv_tc_rows_ratio(*conv.tc);
+          conv.layer += "*" + ly.name;  // '*': composed, not merely fused
+          Op* up = ops_.size() >= 2 ? &ops_[ops_.size() - 2] : nullptr;
+          if (up && up->kind == Op::Conv && up->use_tc && up->out2 == conv.in) {
+            // the input is scattered by the previous convolution's fused unpool (Basic: conv_decode2 -> upsample1), three
+            // quarters zeros: take that fusion back.  The previous convolution stores its own pooled-resolution output, and
+            // the composed kernel unpools it as it loads its halo rows.  The unpooled tensor is derived, never written.
+            Tensor& pooled = *tensors_[up->out];
+            Tensor& unpooled = *tensors_[conv.in];
+            const Tensor& mask = *tensors_[up->in2];
+            conv_tc_set_unpool(*up->tc, nullptr, 1, pooled.v.p);
+            pooled.elided = false;
+            conv_tc_set_unpool_input(*conv.tc, pooled.v.p, mask.buf.as<uint8_t>(), mask.v.n, pooled.v.h, pooled.v.w);
+            unpooled.derived_from = up->out;
+            unpooled.derived_mask = up->in2;
+            unpooled.buf.release();
+            unpooled.v.p = nullptr;
+            const size_t plus = up->layer.rfind('+');  // the unpool is the last layer fused into it
+            conv.layer = up->layer.substr(plus + 1) + "+" + conv.layer;
+            up->layer.erase(plus);
+            up->in2 = up->out2 = -1;
           }
           conv.flops += op.flops;  // algorithmic: the reference runs both layers
           tensors_[in]->elided = true;
-          fused_.push_back(std::move(op));
           li = lj - 1;
           break;
         }
-        if (op.split) {
-          op.a_split.alloc(split_in.elems() * sizeof(__half));
-          split_in.p = op.a_split.p;
-          op.tc = conv_tc_plan(op, split_in, tensors_[op.out]->v, op.w_tc.p);
-          op.use_tc = true;
-        } else if (opt_.engine != SIVO_ENGINE_SIMT && act_ == DType::F16 &&
-            conv_tc_supported(op, civ, tensors_[op.out]->v)) {
-          op.tc = conv_tc_plan(op, civ, tensors_[op.out]->v, op.w_tc.p);
-          op.flops_exec *= conv_tc_rows_ratio(*op.tc);
-          op.use_tc = true;
-        } else if (op.fold_kw) {
-          fail(SIVO_EINVAL, "layer '%s': window-folded first layer is not supported by the tensor-core kernel", ly.name.c_str());
-        } else if (opt_.engine == SIVO_ENGINE_TCGEN05 && op.cin_p % 64 == 0 && (!logits || act_ == DType::F32)) {
-          fail(SIVO_EINVAL, "layer '%s': tcgen05 engine requested but the shape is not supported", ly.name.c_str());
+        const TensorView& ov = tensors_[op.out]->v;
+        // fp32 activations on the tensor-core engine: split-operand mode (three half MMAs per tap, fp32 accumulation)
+        if (act_ == DType::F32 && opt_.engine != SIVO_ENGINE_SIMT && !op.fold_kw && civ.cs % 64 == 0 && civ.c == civ.cs) {
+          op.split = true;
+          if (!conv_tc_supported(op, split_view(civ), ov)) op.split = false;
         }
+        op.use_tc = op.split || (opt_.engine != SIVO_ENGINE_SIMT && act_ == DType::F16 && conv_tc_supported(op, civ, ov));
+        if (!op.use_tc && op.fold_kw)
+          fail(SIVO_EINVAL, "layer '%s': window-folded first layer is not supported by the tensor-core kernel", ly.name.c_str());
+        if (!op.use_tc && opt_.engine == SIVO_ENGINE_TCGEN05 && op.cin_p % 64 == 0 && (!logits || act_ == DType::F32))
+          fail(SIVO_EINVAL, "layer '%s': tcgen05 engine requested but the shape is not supported", ly.name.c_str());
+        prepare_conv(op, act_, w, bias, bn ? (*bn)[0].data.data() : nullptr, bn ? (*bn)[1].data.data() : nullptr, civ, ov);
+        op.flops_exec = op.split ? 3.0 * op.flops : op.flops * (op.use_tc ? conv_tc_rows_ratio(*op.tc) : 1.0);
         ops_.push_back(std::move(op));
         li = lj - 1;
         break;
@@ -457,27 +461,10 @@ void SegNet::enqueue(const uint8_t* bgr_dev, uint8_t* classes_dev, double* conf_
       case Op::LRN:
         launch_lrn(tensors_[op.in]->v, tensors_[op.out]->v, op.lrn_size, op.lrn_alpha, op.lrn_beta, op.lrn_k, s);
         break;
-      case Op::Conv: {
-        if (op.use_tc) {
-          if (op.split) {  // the float input as [hi | lo] half planes
-            launch_split_hilo(tensors_[op.in]->v, op.a_split.p, s);
-            ++launches;
-          }
-          conv_tc_launch(*op.tc, s);
-        } else {
-          ConvParams p;
-          p.in = tensors_[op.in]->v;
-          p.out = tensors_[op.out]->v;
-          p.w_simt = op.w_simt.as<float>();
-          p.bias = op.bias.as<float>();
-          p.bn_scale = op.has_bn ? op.bn_scale.as<float>() : nullptr;
-          p.bn_shift = op.has_bn ? op.bn_shift.as<float>() : nullptr;
-          p.k = op.k; p.pad = op.pad; p.cin_p = op.cin_p; p.cout_p = op.cout_p;
-          p.relu = op.relu; p.slope = op.slope;
-          launch_conv_simt(p, s);
-        }
+      case Op::Conv:
+        if (op.split) ++launches;  // the hi / lo pass
+        launch_conv(op, tensors_[op.in]->v, tensors_[op.out]->v, s);
         break;
-      }
       case Op::Pool:
         launch_pool(tensors_[op.in]->v, tensors_[op.out]->v, tensors_[op.out2]->buf.as<uint8_t>(), s);
         break;

@@ -38,11 +38,12 @@ struct Op {
   // Conv
   int k = 0, pad = 0, cin = 0, cout = 0, cin_p = 0, cout_p = 0;
   std::vector<float> h_w_raw;  // the caffemodel's (cout, cin, k, k) floats, unrounded (the composed classifier's input)
-  std::vector<float> h_bias, h_bn_scale, h_bn_shift, h_w;  // host copies (the tensor-core kernels take them as kernel parameters)
+  std::vector<float> h_bias, h_bn_scale, h_bn_shift;  // [cout_p] host copies (the tensor-core kernels take them as kernel parameters)
   int fold_kw = 0;  // > 0: KxK conv over 3 channels run as a Kx1 conv over the window-folded padded input (conv_tc.cu)
   bool relu = false, has_bn = false;
   float slope = 0.f;
-  DevBuf w_simt, w_tc, bias, bn_scale, bn_shift;
+  DevBuf w_simt, bias, bn_scale, bn_shift;  // the SIMT kernel's weights [tap][cin_p][cout_p] float and constants
+  DevBuf w_tc;                              // the tensor-core kernels' weights [tap][cout_p][cin_p] half
   // split-operand fp32 mode (precision fp32 on the tensor-core engine): x = hi + lo and w * 2^s = hi + lo in half, and
   // x * w ~= (x_hi w_hi + x_hi w_lo + x_lo w_hi) * 2^-s accumulated in fp32 -- three MMAs per tap, ~2^-22 relative per product.
   // w_tc holds [tap][cout_p][3 cin_p] = per 64-channel chunk [W_hi | W_lo | W_hi]; a_split the [hi Cin | lo Cin] planes of the input.
@@ -112,7 +113,6 @@ class SegNet {
  private:
   int add_tensor(const std::string& name, int n, int c, int h, int w, int cs, DType dt, bool mask = false);
   void build(const NetSpec& net, const WeightMap& weights);
-  void prepare_conv(Op& op, const std::vector<Blob>& conv_blobs, const std::vector<Blob>* bn_blobs);
   void enqueue(const uint8_t* bgr_dev, uint8_t* classes_dev, double* conf_dev, double* ent_dev, cudaStream_t s, bool timed);
   // one frame of the op list (graph replay or plain launches) with the per-frame arguments `fa`, ending as reduce_ says
   void launch_frame(FrameArgs fa, cudaStream_t s);
@@ -129,7 +129,6 @@ class SegNet {
   std::vector<std::unique_ptr<Tensor>> tensors_;
   std::map<std::string, int> by_name_;
   std::vector<Op> ops_;
-  std::vector<Op> fused_;  // ops folded into a neighbour's epilogue; kept alive for their weight buffers
   cudaStream_t stream_ = nullptr;
   DevBuf d_bgr_, d_classes_, d_conf_, d_ent_, d_frame_;
   PinnedBuf h_in_, h_classes_, h_conf_, h_ent_;
@@ -160,6 +159,18 @@ class SegNet {
   float* rec_ent32_ = nullptr;
 };
 
+// Packs convolution `op`'s weights (`w`: the caffemodel's (cout, cin, k, k) floats; `bias`, `bn_scale`, `bn_shift`: cout
+// floats or NULL, no BN without a scale) into the one layout its path reads and uploads them.  The caller has set the
+// shape fields and chosen the path (op.split, op.use_tc); a tensor-core op also gets its plan from `in` to `out` (split:
+// the float input, whose half planes a_split it allocates).  `act`: the activation type (fp16 rounds the SIMT weights
+// through half).
+void prepare_conv(Op& op, DType act, const float* w, const float* bias, const float* bn_scale, const float* bn_shift,
+                  const TensorView& in, const TensorView& out);
+// one run of convolution `op` from `in` to `out` on `s`: the split-operand mode's hi / lo pass and the plan, or the SIMT kernel
+void launch_conv(const Op& op, const TensorView& in, const TensorView& out, cudaStream_t s);
+// the [hi Cin | lo Cin] half planes of float tensor `v` that a split-operand convolution reads (p unset)
+TensorView split_view(TensorView v);
+
 // conv_tc.cu -- wgmma implicit-GEMM convolution
 bool conv_tc_supported(const Op& op, const TensorView& in, const TensorView& out);
 std::shared_ptr<ConvTcPlan> conv_tc_plan(const Op& op, const TensorView& in, const TensorView& out, const void* w_tc);
@@ -178,15 +189,11 @@ void conv_tc_set_unpool_input(ConvTcPlan& plan, const void* pooled, const uint8_
 // fuses the 2x2/2 max pool (+ argmax mask) that consumes the convolution's output into its epilogue
 bool conv_tc_can_fuse_pool(const ConvTcPlan& plan);
 void conv_tc_set_pool(ConvTcPlan& plan, void* pooled, uint8_t* mask);
-// fuses a following 1x1 convolution to <= 16 float logits (the layer feeding Softmax) into the epilogue
-bool conv_tc_can_fuse_classifier(const ConvTcPlan& plan);
 // host-side weight layout of the split-operand fp32 mode: [tap][cout_p][3 cin_p] half + the accumulator scale 2^-s
 std::vector<__half> conv_tc_split_weights(const float* w_cout_cin_k_k, int cout, int cin, int K, int cout_p, int cin_p, float* acc_scale);
-// The composed classifier (default; SIVO_B200_COMPOSE=0 keeps the two-step form): conv (64 -> 64, 7x7, no BN / ReLU) followed by
-// the 1x1 classifier run as ONE 64 -> 16 convolution with composed weights; logits come straight from the accumulators.
-// wc = [n_cls][64], bc = [n_cls] (host).
+// The composed classifier: conv (64 -> 64, 7x7, no BN / ReLU) followed by the 1x1 classifier run as ONE 64 -> 16 convolution
+// with composed weights; logits come straight from the accumulators.  wc = [n_cls][64], bc = [n_cls] or NULL (host).
 bool conv_tc_can_compose_classifier(const ConvTcPlan& plan);
 void conv_tc_set_composed_classifier(ConvTcPlan& plan, const Op& conv, const float* wc, const float* bc, int n_cls, float* logits);
-void conv_tc_set_classifier(ConvTcPlan& plan, const float* w_cin_by_cout, int stride, const float* bias, int n_bias, float* logits);  // host pointers
 
 }  // namespace sivo

@@ -35,10 +35,7 @@ def _exposed(seg, names):
     return out
 
 
-def _check_fused_equals_unfused(net, proto, model, img, T, monkeypatch, must_have=""):
-    # the two-step classifier fused into conv_decode1's epilogue sums its products in another fp32 order than the 1x1 kernel,
-    # and the composed one rounds differently again: the maps are compared within that, the blobs bit for bit
-    monkeypatch.setenv("SIVO_B200_COMPOSE", "0")
+def _check_fused_equals_unfused(net, proto, model, img, T, must_have="", composed=False):
     names = sorted({t for ly in net.layers for t in ly.tops})
     seg_u, (c0, f0, e0) = _run(proto, model, img, True, T)
     unfused = _exposed(seg_u, names)
@@ -50,24 +47,34 @@ def _check_fused_equals_unfused(net, proto, model, img, T, monkeypatch, must_hav
     for n in common:
         assert fused[n].shape == unfused[n].shape, n
         assert np.array_equal(fused[n], unfused[n]), (n, float(np.abs(fused[n] - unfused[n]).max()))
-    assert (c0 != c1).mean() < 1e-3
-    assert np.abs(e0 - e1).max() < 1e-4 and np.abs(f0 - f1).max() < 1e-4
+    if composed:
+        # the composed classifier never rounds the 64-channel activation to half (its composed weights are), so its maps
+        # differ from the two layers' at the half-rounding level
+        assert not np.array_equal(e0, e1), "the composed kernel did not engage"
+        assert (c0 != c1).mean() < 2e-3
+        assert np.abs(e0 - e1).max() < 2e-2 and np.median(np.abs(e0 - e1)) < 1e-3
+        assert np.abs(f0 - f1).max() < 1e-2
+    else:
+        assert (c0 != c1).mean() < 1e-3
+        assert np.abs(e0 - e1).max() < 1e-4 and np.abs(f0 - f1).max() < 1e-4
 
 
 # (H, W): 48 x 272 -- partial strips at every level (272, 136, 68, 34 px) and 3 row blocks at H / 8; 80 x 320 -- 5 row
 # blocks at H / 8, a 32-px last strip at H / 2; 352 x 464 -- tall layers, whose CTAs walk many row blocks (and the last
 # CTA of a column fewer), with a partial strip everywhere
 @pytest.mark.parametrize("H,W", [(48, 272), (80, 320), (352, 464)])
-def test_basic_fused_blobs_equal_unfused(model_dir, monkeypatch, H, W):
+def test_basic_composed_build_blobs_equal_unfused(model_dir, H, W):
+    # the default build composes conv_decode1 and the classifier, and its composed kernel unpools conv_decode2's output on
+    # load: conv_decode2 and the derived upsample1 are compared bit for bit too
     net, _, proto, model = make_model(model_dir, "basic", T=2, H=H, W=W, seed=0)
-    _check_fused_equals_unfused(net, proto, model, _image(H, W), 2, monkeypatch, must_have="upsample")
+    _check_fused_equals_unfused(net, proto, model, _image(H, W), 2, must_have="upsample", composed=True)
 
 
-def test_standard_fused_blobs_equal_unfused(model_dir, monkeypatch):
+def test_standard_fused_blobs_equal_unfused(model_dir):
     # Standard's widths: 128-wide tiles (N = 128, immediate epilogue), chunked Cin > 64 layers and image-pair tiles (conv5 at
     # 4 x 8) next to the 64-wide deferred ones
     net, _, proto, model = make_model(model_dir, "standard", T=2, H=64, W=128, seed=0)
-    _check_fused_equals_unfused(net, proto, model, _image(64, 128), 2, monkeypatch)
+    _check_fused_equals_unfused(net, proto, model, _image(64, 128), 2)
 
 
 def test_default_build_is_deterministic(model_dir):

@@ -1,6 +1,7 @@
 """CPU study: how does composing conv_decode1 with the 1x1 classifier
-(logits = (Wc W) * x + Wc b + bc, half weights, fp32 accumulation) compare with today's two-step fp16 path, both measured
-against the same two convolutions evaluated in float64 on the same (half-rounded) input?  Oracle only; no GPU."""
+(logits = (Wc W) * x + Wc b + bc, half weights, fp32 accumulation) compare with running the two layers in fp16 (the unfused
+op list), both measured against the same two convolutions evaluated in float64 on the same (half-rounded) input?  Oracle
+only; no GPU."""
 import os
 import sys
 
@@ -35,7 +36,7 @@ def h(t):  # round to IEEE half, back to float64
 
 conv = torch.nn.functional.conv2d
 truth = conv(conv(x, Wd, bd, padding=3), Wc, bc)                      # float64, unrounded weights: the reference's arithmetic
-two_step = conv(h(conv(x, h(Wd), bd, padding=3)), h(Wc), bc)          # today's path: half weights, activation rounded to half
+two_step = conv(h(conv(x, h(Wd), bd, padding=3)), h(Wc), bc)          # the two layers: half weights, activation rounded to half
 Wcomp = torch.einsum("oc,cikl->oikl", Wc[:, :, 0, 0], Wd)             # composed 15 x 64 x 7 x 7 weights (float64)
 bcomp = Wc[:, :, 0, 0] @ bd + bc
 composed = conv(x, h(Wcomp), bcomp, padding=3)
