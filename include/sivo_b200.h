@@ -476,6 +476,96 @@ int sivo_dbg_pose_system(const sivo_orb_t* left, const sivo_keypoint* kps, const
                          float fy, float cx, float cy, float mbf, const double* pose7, int robust_stereo, const uint8_t* level1,
                          double* err, double* chi2, double* rho, double* jac, double* H, double* b, double* chi);
 
+/* ---- a keyframe's new map points: LocalMapping::CreateNewMapPoints (LocalMapping.cc:198-472) with ORBmatcher::
+ * SearchForTriangulation (ORBmatcher.cc:631-785, ORBmatcher(0.6, false): no orientation check), CheckDistEpipolarLine
+ * (:137-159), ComputeF12 (LocalMapping.cc:639-654) and SIVO's CheckSemantics (:474-545), stereo only -------------------------
+ * Every operation is the IEEE float / double operation as written (no contracted multiply-add).  oracle/mapping_oracle.py restates
+ * the rule and lists every reference fact kept; in short:
+ *   walk      current-keyframe key j (no map point on entry) visits the neighbours in order and stops at its first created point.
+ *             A neighbour with (float) norm(Ow2 - Ow1) < mb is skipped.  Key results do not depend on one another: the reference
+ *             never sets vbMatched2, so one neighbour key may be matched (and get points) from several current keys.
+ *   match     candidates: the neighbour's keys with node == node[j] >= 0 and no map point on entry (node -1: not in mFeatVec);
+ *             Hamming distance <= TH_LOW (50); if both keys are mono, (ex - x2)^2 + (ey - y2)^2 < 100 scale[octave2] rejects (the
+ *             scale factor, not squared); CheckDistEpipolarLine in float with den == 0 rejecting and dsqr < 3.84 sigma2 in double.
+ *             The best is the smallest distance, the LATER candidate on ties (the reference's `dist > bestDist` skip).
+ *   checks    in the reference's order: parallax (cos(2 atan2(mb / 2, depth)) as the float overloads, the second keyframe's only in
+ *             the `else if`), w == 0, z1 <= 0, z2 <= 0, the reprojection errors (5.991 / 7.8 sigma2 in double; the neighbour's
+ *             stereo error with the current keyframe's mbf), scale consistency (1.5f scale_factor).
+ *   SVD       the triangulation's right singular vector is a documented rule, not cv::SVD's float Jacobi: one-sided Jacobi in
+ *             double on A's columns (pairs (0,1) (0,2) (0,3) (1,2) (1,3) (2,3), a pair rotated only while |gamma| > 2^-52
+ *             sqrt(alpha beta), at most 30 sweeps, stop after a sweep without a rotation), the column of least norm (first on
+ *             ties); rounded to float, w == 0 rejects, x = v[0..2] / v[3] in float.
+ *   semantic  current key: depth > 0, class <= max_static_class, (double) confidence >= (float) th_confidence, and not
+ *             MI - H < (float) th_entropy_reduction, with MI of the triangulated WORLD point, sigma2[octave] and sigma_cw (a NaN
+ *             reduction passes).  Neighbour key: its class.  Created iff the two classes are equal and not 255 (VOID).
+ * A key whose octave is outside the extractor's levels never takes part (the reference would index out of its tables). */
+typedef struct sivo_keyframe_keys {        /* one keyframe's semantic keys, sivo_orb_capacity(left) entries per array */
+  const sivo_keypoint* kps;                /* mvKeysSemantic */
+  const uint8_t* desc;                     /* mDescriptorsSemantic, 32 bytes per key */
+  const float* u_right;                    /* mvRight (< 0: mono) */
+  const float* depth;                      /* mvDepth */
+  const uint8_t* kp_class;                 /* mClasses, mConfidence, mEntropy at ((int) y, (int) x) */
+  const double* kp_conf;
+  const double* kp_entropy;
+  const int32_t* node;                     /* the key's mFeatVec node (DBoW2, levelsup 4); -1 for none */
+  const uint8_t* has_point;                /* GetMapPoint(i) != NULL on entry */
+  const long long* count;                  /* int64 number of keys */
+  float Rcw[9], tcw[3], Ow[3];             /* GetRotation (row-major), GetTranslation, GetCameraCenter (host values) */
+} sivo_keyframe_keys;
+
+typedef struct sivo_mapping_params {       /* the keyframes' shared camera and SIVO's thresholds */
+  float fx, fy, cx, cy, invfx, invfy, mb, mbf;
+  double sigma_cw[36];                     /* the current keyframe's mSigmacw, row-major 6 x 6 */
+  int32_t max_static_class;                /* Classes::TERRAIN = 8 in the reference */
+  float th_confidence, th_entropy_reduction;  /* mThConfidence, mThEntropyReduction */
+  int32_t reserved;
+} sivo_mapping_params;
+
+/* KeyFrame's copy of the Frame's semantic keys: for j < *n_keep_device (clamped to the capacity), with k = keep_idx_device[j] (j
+ * when NULL), out_kps[j] = kps[k], out_desc[32 j ..] = desc[32 k ..], out_u_right[j] = u_right[j], out_depth[j] = depth[j],
+ * out_class / out_conf / out_entropy[j] = kp_class / kp_conf / kp_entropy[k]; *out_count = the clamped count (-1 for a negative
+ * count, which writes nothing else).  A key index outside the capacity gives octave -1 (the key never takes part).  Outputs hold
+ * sivo_orb_capacity(left) keys and belong to the caller, so the next sivo_orb_enqueue_device does not overwrite them.  Runs on
+ * `stream` (NULL = the left extractor's stream) with no waits and no host synchronisation; the inputs must be ordered before it
+ * on that stream, as for the other Frame-tail calls.  SIVO_EINVAL for NULL handles, inputs or outputs. */
+int sivo_keyframe_gather_device(const sivo_orb_t* left, const sivo_keypoint* kps_device, const uint8_t* desc_device,
+                                const int* keep_idx_device, const long long* n_keep_device, const float* u_right_device,
+                                const float* depth_device, const uint8_t* kp_class_device, const double* kp_conf_device,
+                                const double* kp_entropy_device, sivo_keypoint* out_kps, uint8_t* out_desc, float* out_u_right,
+                                float* out_depth, uint8_t* out_class, double* out_conf, double* out_entropy, long long* out_count,
+                                void* stream);
+/* CreateNewMapPoints of keyframe kf1 against neighbours[0 .. n_neighbours) (GetBestCovisibilityKeyFrames order, at most 32) on
+ * device buffers.  Outputs, each may be NULL, for current keys j < kf1's count (sivo_orb_capacity(left) room):
+ * created_nb_device[j] = the neighbour whose pair created j's point, or -1; created_idx_device[j] = that neighbour's key;
+ * world_device[3 j ..] = the point (NaN when none); created_list_device[2 e ..] = (neighbour, key j) of the e-th point created, in
+ * the reference's order (neighbour-major, j ascending: mlpRecentAddedMapPoints); *n_created_device (int64) its length.  Counts are
+ * clamped to the capacity; a negative count (the -1 of sivo_segnet_semantic_keys_device) in any keyframe writes only
+ * *n_created_device = -1.  Runs on `stream` (NULL = the left extractor's stream) with no waits and no host synchronisation.  Its
+ * scratch is allocated and freed on `stream` (stream-ordered), never on the extractor, and it reads only the extractor's scale
+ * tables: LocalMapping's thread may run it concurrently with Tracking's calls on the same extractor.  SIVO_EINVAL for NULL
+ * handles or inputs, n_neighbours outside [0, 32]. */
+int sivo_create_map_points_device(const sivo_orb_t* left, const sivo_keyframe_keys* kf1, const sivo_keyframe_keys* neighbours,
+                                  int n_neighbours, const sivo_mapping_params* params, int* created_nb_device,
+                                  int* created_idx_device, float* world_device, int* created_list_device, long long* n_created_device,
+                                  void* stream);
+/* Host form: every sivo_keyframe_keys pointer (count included) is a host array of its own count's keys; outputs per current key
+ * (n1 = kf1's count) and created_list 2 n1 ints, *n_created.  It stages the inputs, runs the device form's kernels and
+ * synchronises. */
+int sivo_create_map_points(const sivo_orb_t* left, const sivo_keyframe_keys* kf1, const sivo_keyframe_keys* neighbours, int n_neighbours,
+                           const sivo_mapping_params* params, int* created_nb, int* created_idx, float* world, int* created_list,
+                           long long* n_created);
+/* Test hook: the host form, every key searched (the production path skips a key whose depth, class or confidence already
+ * rules it out), plus per (neighbour i, key j) at [i n1 + j]: match = SearchForTriangulation's vMatchedPairs partner or -1;
+ * stage = where the reference's loop ends for the pair (SIVO_MAP_STAGE_*); reduction = MI - H (NaN unless computed). */
+enum {
+  SIVO_MAP_STAGE_HAS_POINT = 0, SIVO_MAP_STAGE_BASELINE, SIVO_MAP_STAGE_NO_MATCH, SIVO_MAP_STAGE_PARALLAX, SIVO_MAP_STAGE_W_ZERO,
+  SIVO_MAP_STAGE_Z1, SIVO_MAP_STAGE_Z2, SIVO_MAP_STAGE_REPROJ1, SIVO_MAP_STAGE_REPROJ2, SIVO_MAP_STAGE_SCALE,
+  SIVO_MAP_STAGE_SEMANTIC, SIVO_MAP_STAGE_CREATED
+};
+int sivo_dbg_create_map_points(const sivo_orb_t* left, const sivo_keyframe_keys* kf1, const sivo_keyframe_keys* neighbours,
+                               int n_neighbours, const sivo_mapping_params* params, int* match, int* stage, double* reduction,
+                               int* created_nb, int* created_idx, float* world, int* created_list, long long* n_created);
+
 /* Best / second-best match over per-query candidate lists -- the inner loop of ORBmatcher::SearchByProjection
  * (ORBmatcher.cc:79-113), its last-frame / keyframe variants (:1278-, :1420-), SearchForTriangulation (:631-) and
  * SearchBySim3 (next row 4).  Query i's candidates are cand_idx[cand_offsets[i] .. cand_offsets[i+1]) (indices into the

@@ -593,6 +593,54 @@ int sivo_dbg_pose_system(const sivo_orb_t* left, const sivo_keypoint* kps, const
   });
 }
 
+// ---------------------------------------------------------------------------------------- keyframe map points
+int sivo_keyframe_gather_device(const sivo_orb_t* left, const sivo_keypoint* kps_device, const uint8_t* desc_device,
+                                const int* keep_idx_device, const long long* n_keep_device, const float* u_right_device,
+                                const float* depth_device, const uint8_t* kp_class_device, const double* kp_conf_device,
+                                const double* kp_entropy_device, sivo_keypoint* out_kps, uint8_t* out_desc, float* out_u_right,
+                                float* out_depth, uint8_t* out_class, double* out_conf, double* out_entropy, long long* out_count,
+                                void* stream) {
+  return guarded([&] {
+    if (!left || !kps_device || !desc_device || !n_keep_device || !u_right_device || !depth_device || !kp_class_device || !kp_conf_device ||
+        !kp_entropy_device || !out_kps || !out_desc || !out_u_right || !out_depth || !out_class || !out_conf || !out_entropy || !out_count)
+      fail(SIVO_EINVAL, "keyframe_gather: null argument");
+    keyframe_gather_device(*left->impl, kps_device, desc_device, keep_idx_device, n_keep_device, u_right_device, depth_device, kp_class_device,
+                           kp_conf_device, kp_entropy_device, out_kps, out_desc, out_u_right, out_depth, out_class, out_conf, out_entropy,
+                           out_count, static_cast<cudaStream_t>(stream));
+  });
+}
+
+int sivo_create_map_points_device(const sivo_orb_t* left, const sivo_keyframe_keys* kf1, const sivo_keyframe_keys* neighbours,
+                                  int n_neighbours, const sivo_mapping_params* params, int* created_nb_device,
+                                  int* created_idx_device, float* world_device, int* created_list_device, long long* n_created_device,
+                                  void* stream) {
+  return guarded([&] {
+    if (!left || !kf1 || !params) fail(SIVO_EINVAL, "create_map_points: null argument");
+    create_map_points_device(*left->impl, *kf1, neighbours, n_neighbours, *params, created_nb_device, created_idx_device, world_device,
+                             created_list_device, n_created_device, static_cast<cudaStream_t>(stream));
+  });
+}
+
+int sivo_create_map_points(const sivo_orb_t* left, const sivo_keyframe_keys* kf1, const sivo_keyframe_keys* neighbours, int n_neighbours,
+                           const sivo_mapping_params* params, int* created_nb, int* created_idx, float* world, int* created_list,
+                           long long* n_created) {
+  return guarded([&] {
+    if (!left || !kf1 || !params) fail(SIVO_EINVAL, "create_map_points: null argument");
+    create_map_points_host(*left->impl, *kf1, neighbours, n_neighbours, *params, nullptr, nullptr, nullptr, created_nb, created_idx, world,
+                           created_list, n_created);
+  });
+}
+
+int sivo_dbg_create_map_points(const sivo_orb_t* left, const sivo_keyframe_keys* kf1, const sivo_keyframe_keys* neighbours,
+                               int n_neighbours, const sivo_mapping_params* params, int* match, int* stage, double* reduction,
+                               int* created_nb, int* created_idx, float* world, int* created_list, long long* n_created) {
+  return guarded([&] {
+    if (!left || !kf1 || !params || !match || !stage || !reduction) fail(SIVO_EINVAL, "create_map_points: null argument");
+    create_map_points_host(*left->impl, *kf1, neighbours, n_neighbours, *params, match, stage, reduction, created_nb, created_idx, world,
+                           created_list, n_created);
+  });
+}
+
 // ---------------------------------------------------------------------------------------- layer test hooks
 namespace {
 TensorView make_view(DevBuf& buf, int n, int c, int h, int w, int cs, DType dt) {

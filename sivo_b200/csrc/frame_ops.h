@@ -56,4 +56,16 @@ void pose_system(const Orb& left, const sivo_keypoint* kps, const float* u_right
                  float cy, float mbf, const double* pose7, int robust_stereo, const uint8_t* level1, double* err, double* chi2, double* rho,
                  double* jac, double* H, double* b, double* chi);
 
+// ---- mapping.cu
+void keyframe_gather_device(const Orb& left, const sivo_keypoint* kps, const uint8_t* desc, const int* keep_idx, const long long* n_keep,
+                            const float* u_right, const float* depth, const uint8_t* cls, const double* conf, const double* ent,
+                            sivo_keypoint* o_kps, uint8_t* o_desc, float* o_ur, float* o_depth, uint8_t* o_cls, double* o_conf,
+                            double* o_ent, long long* o_count, cudaStream_t s);
+void create_map_points_device(const Orb& left, const sivo_keyframe_keys& kf1, const sivo_keyframe_keys* nbs, int n_nb,
+                              const sivo_mapping_params& prm, int* created_nb, int* created_idx, float* world, int* created_list,
+                              long long* n_created, cudaStream_t s);
+void create_map_points_host(const Orb& left, const sivo_keyframe_keys& kf1, const sivo_keyframe_keys* nbs, int n_nb,
+                            const sivo_mapping_params& prm, int* dbg_match, int* dbg_stage, double* dbg_red, int* created_nb,
+                            int* created_idx, float* world, int* created_list, long long* n_created);
+
 }  // namespace sivo

@@ -8,6 +8,7 @@
 #include "compact.cuh"
 #include "frame_ops.h"
 #include "host_call.h"
+#include "info_mi.cuh"
 
 namespace sivo {
 
@@ -25,59 +26,6 @@ namespace {
 constexpr int kInfoThreads = 128;
 constexpr int kInfoShared = 81 * kInfoThreads * static_cast<int>(sizeof(double));  // one 9 x 9 matrix per thread
 constexpr int kCompactThreads = 512;
-
-// det by LU with partial pivoting of the n x n row-major matrix a[(r * n + c) * stride] (overwritten).  The pivot is the first
-// row with the largest |a| in the column (a NaN never displaces it); a zero pivot column is skipped.  The result is the product
-// of the diagonal in order, times the permutation sign.
-__device__ double det_lu(double* a, int n, int stride) {
-#define A(r, c) a[((r) * n + (c)) * stride]
-  bool neg = false;
-  for (int c = 0; c < n; ++c) {
-    int p = c;
-    double best = fabs(A(c, c));
-    for (int r = c + 1; r < n; ++r) {
-      const double v = fabs(A(r, c));
-      if (v > best) { best = v; p = r; }
-    }
-    if (best == 0.0) continue;
-    if (p != c) {
-      for (int j = c; j < n; ++j) { const double t = A(c, j); A(c, j) = A(p, j); A(p, j) = t; }
-      neg = !neg;
-    }
-    const double piv = A(c, c);
-    for (int r = c + 1; r < n; ++r) {
-      const double l = A(r, c) / piv;
-      for (int j = c + 1; j < n; ++j) A(r, j) = A(r, j) - l * A(c, j);
-    }
-  }
-  double d = A(0, 0);
-  for (int i = 1; i < n; ++i) d = d * A(i, i);
-  return neg ? d * -1.0 : d;
-#undef A
-}
-
-// computeStereoJacobianPose (sivo_helpers.cpp:64-88), each expression left to right as written; zero when Z == 0
-__device__ __forceinline__ void stereo_jacobian_pose(double fx, double fy, double bl, double X, double Y, double Z, double J[3][6]) {
-  for (int r = 0; r < 3; ++r)
-    for (int c = 0; c < 6; ++c) J[r][c] = 0.0;
-  if (Z == 0.0) return;
-  const double ZZ = Z * Z, Xb = X - bl;
-  J[0][0] = fx / Z;
-  J[0][2] = -fx * X / ZZ;
-  J[0][3] = -fx * X * Y / ZZ;
-  J[0][4] = fx * (1.0 + X * X / ZZ);
-  J[0][5] = -fx * Y / Z;
-  J[1][1] = fy / Z;
-  J[1][2] = -fy * Y / ZZ;
-  J[1][3] = -fy * (1.0 + Y * Y / ZZ);
-  J[1][4] = fy * X * Y / ZZ;
-  J[1][5] = fy * X / Z;
-  J[2][0] = fx / Z;
-  J[2][2] = -fx * Xb / ZZ;
-  J[2][3] = -fx * Xb * Y / ZZ;
-  J[2][4] = fx * (1.0 + X * Xb / ZZ);
-  J[2][5] = -fx * Y / Z;
-}
 
 // One thread per semantic key j < min(*count, cap): the decision goes to flags[j] (1 = selected), the optional outputs to
 // world[3 j ..], reduction[j] and the three determinants.  The working 9 x 9 matrix lives in dynamic shared memory as
@@ -115,53 +63,10 @@ __global__ void __launch_bounds__(kInfoThreads) k_info_select(const InfoParams p
   for (int r = 0; r < 3; ++r) w[r] = p.rwc[3 * r] * xc[0] + p.rwc[3 * r + 1] * xc[1] + p.rwc[3 * r + 2] * xc[2] + p.ow[r];
   if (world) { world[3 * j] = w[0]; world[3 * j + 1] = w[1]; world[3 * j + 2] = w[2]; }
 
-  double J[3][6];
-  stereo_jacobian_pose(p.fx, p.fy, p.mb, w[0], w[1], w[2], J);
   const double s2 = p.sigma2[kp.octave];
-  double* ws = ws_all + threadIdx.x;  // element e of this thread's matrix: ws[e * kInfoThreads]
-  // det S, by the same LU as det M
-  for (int e = 0; e < 36; ++e) ws[e * kInfoThreads] = p.sigma[e];
-  const double det_s = det_lu(ws, 6, kInfoThreads);
-  // M = [[S, S J^T], [J S, (J S) J^T + R]]
-#define M(r, c) ws[((r) * 9 + (c)) * kInfoThreads]
-#pragma unroll
-  for (int r = 0; r < 6; ++r)
-#pragma unroll
-    for (int c = 0; c < 6; ++c) M(r, c) = p.sigma[r * 6 + c];
-#pragma unroll
-  for (int i = 0; i < 6; ++i)
-#pragma unroll
-    for (int r = 0; r < 3; ++r) {
-      double s = p.sigma[i * 6] * J[r][0];
-#pragma unroll
-      for (int q = 1; q < 6; ++q) s = s + p.sigma[i * 6 + q] * J[r][q];
-      M(i, 6 + r) = s;
-    }
-#pragma unroll
-  for (int r = 0; r < 3; ++r)
-#pragma unroll
-    for (int c = 0; c < 6; ++c) {
-      double s = J[r][0] * p.sigma[c];
-#pragma unroll
-      for (int q = 1; q < 6; ++q) s = s + J[r][q] * p.sigma[q * 6 + c];
-      M(6 + r, c) = s;
-    }
-  double m33[3][3];
-#pragma unroll
-  for (int r = 0; r < 3; ++r)
-#pragma unroll
-    for (int c = 0; c < 3; ++c) {
-      double s = M(6 + r, 0) * J[c][0];
-#pragma unroll
-      for (int q = 1; q < 6; ++q) s = s + M(6 + r, q) * J[c][q];
-      m33[r][c] = s + (r == c ? s2 : 0.0);
-      M(6 + r, 6 + c) = m33[r][c];
-    }
-#undef M
-  const double det_m33 = m33[0][0] * (m33[1][1] * m33[2][2] - m33[1][2] * m33[2][1]) -
-                         m33[0][1] * (m33[1][0] * m33[2][2] - m33[1][2] * m33[2][0]) +
-                         m33[0][2] * (m33[1][0] * m33[2][1] - m33[1][1] * m33[2][0]);
-  const double det_m = det_lu(ws, 9, kInfoThreads);
+  // the working 9 x 9 matrix: element e of this thread's at ws_all[e * kInfoThreads + threadIdx.x]
+  const StereoMiTerms t = stereo_mi_terms(p.sigma, p.fx, p.fy, p.mb, w[0], w[1], w[2], s2, ws_all + threadIdx.x, kInfoThreads);
+  const double det_s = t.det_state, det_m33 = t.det_meas, det_m = t.det_joint;
   const double mi = 0.5 * log2(det_s * det_m33 / det_m);
   const double red = mi - entropy[k];
   if (reduction) reduction[j] = red;

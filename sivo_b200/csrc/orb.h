@@ -113,6 +113,7 @@ class Orb {
   int device() const { return device_; }
   bool has_run() const { return rows_ > 0; }
   int nlevels() const { return nlevels_; }
+  float scale_factor() const { return scale_factor_; }
   void candidates(int level, int* xs, int* ys, int* resp, int cap, int* n) const;
   // Fully asynchronous form (needs the device quad tree): enqueues the whole extractor on this handle's stream and returns.
   // Results stay on the device: kps_dev (>= capacity() records), desc_dev (capacity() x 32 bytes), *count_dev (int64).
