@@ -3,6 +3,7 @@
 // concurrently from two threads as Frame.cc:126-129 does.
 #pragma once
 #include <algorithm>
+#include <chrono>
 #include <condition_variable>
 #include <cstdlib>
 #include <functional>
@@ -55,12 +56,6 @@ struct OrbTreeParams {
   int min_b;                    // EDGE_THRESHOLD - 3: level coordinate of candidate (0, 0)
 };
 
-struct OrbSelected {  // one retained keypoint, level coordinates
-  short x, y;
-  short level;
-  short pad;
-};
-
 // ---- kernels (orb_kernels.cu)
 void orb_launch_pyramid(const uint8_t* gray, int rows, int cols, size_t gray_pitch, uint8_t* pyr, const OrbLevelTable& t,
                         cudaStream_t s);
@@ -71,16 +66,13 @@ void orb_launch_compact(const OrbLevelTable& t, const OrbCell* cells, int ncells
                         const uint32_t* cell_items, int* cell_offset, int* level_offsets, uint32_t* cand, int cand_cap,
                         cudaStream_t s);
 void orb_launch_blur(const uint8_t* pyr, uint8_t* blur, const OrbLevelTable& t, cudaStream_t s);
-void orb_launch_describe(const uint8_t* pyr, const uint8_t* blur, const OrbLevelTable& t, const OrbSelected* sel, int n,
-                         const int* umax, float* angles, uint8_t* desc, cudaStream_t s);
-// the same for a keypoint count that lives on the device (<= cap): angles go straight into the keypoint records
-// Device-tree form: per-level selections (sel_packed[l * kTreeSelCap + i], level_count[l]) -> level-major keypoint records
-// (ComputeKeyPointsOctTree :824-835 + the final scaling of operator() :1071-1078, angle from IC_Angle) and descriptors;
-// *n_out (and *n_out_i64 if given) = the keypoint count, bit 30 of *error if it exceeds cap.
+// Either quad tree's per-level selections (packed candidates sel_packed[l * stride + i], i < level_count[l]; the count lives on
+// the device) -> level-major keypoint records (ComputeKeyPointsOctTree :824-835 + the final scaling of operator() :1071-1078,
+// angle from IC_Angle) and descriptors; *n_out (and *n_out_i64 if given) = the keypoint count, bit 30 of *error if it exceeds cap.
 void orb_launch_describe_dev(const uint8_t* pyr, const uint8_t* blur, const OrbLevelTable& t, const uint32_t* sel_packed,
-                             const int* level_count, const OrbTreeParams& prm, int cap, const int* umax, sivo_keypoint* kps,
-                             uint8_t* desc, int* n_out, long long* n_out_i64, int* error, cudaStream_t s);
-// DistributeOctTree on the device, one block per level (orb_tree.cu), then the level-major keypoint records
+                             const int* level_count, int stride, const OrbTreeParams& prm, int cap, const int* umax,
+                             sivo_keypoint* kps, uint8_t* desc, int* n_out, long long* n_out_i64, int* error, cudaStream_t s);
+// DistributeOctTree on the device, one block per level (orb_tree.cu): the selection describe reads, at stride kTreeSelCap
 void orb_launch_distribute(const uint32_t* cand, const int* level_off, const uint32_t* cell_items, const int* cell_count,
                            const OrbTreeParams& prm, int nlevels, uint32_t* sel_packed, int* level_count, int* error, cudaStream_t s);
 void orb_tree_configure();  // raises k_distribute's dynamic shared-memory limit on the current device
@@ -147,10 +139,15 @@ class Orb {
   void enqueue_compact(cudaStream_t s);
   bool compacted_ = false;
   void enqueue_tree_and_describe(sivo_keypoint* kps_dev, uint8_t* desc_dev, long long* count_dev, cudaStream_t s);
+  void enqueue_describe(int stride, sivo_keypoint* kps_dev, uint8_t* desc_dev, long long* count_dev, cudaStream_t s);
+  void enqueue_results_readback(cudaStream_t s);  // count and error word, keypoint records, descriptors -> h_n_err_, h_kps_, h_desc_
+  void run_host_tree(std::chrono::steady_clock::time_point start);
   bool device_tree_ = true;
   OrbTreeParams tree_prm_{};
+  // the per-level selection k_describe reads, from either quad tree: level l's packed candidates at d_sel_packed_[l * stride ...],
+  // its count at d_level_count_[l]; h_sel_packed_ stages the host tree's counts (kOrbMaxLevels ints), then its words
   DevBuf d_sel_packed_, d_level_count_, d_n_err_, d_kps_;
-  PinnedBuf h_n_err_, h_kps_;
+  PinnedBuf h_sel_packed_, h_n_err_, h_kps_;
   cudaEvent_t ev_wait_ = nullptr, ev_wait2_ = nullptr, ev_pyr_ = nullptr;
   cudaStream_t copy_stream_ = nullptr;
   int nfeatures_, nlevels_, ini_th_, min_th_, device_;
@@ -162,8 +159,8 @@ class Orb {
   cudaStream_t stream_ = nullptr;
   cudaEvent_t ev_[4] = {nullptr, nullptr, nullptr, nullptr};
   DevBuf d_gray_, d_pyr_, d_blur_, d_cells_, d_cell_count_, d_cell_items_, d_cell_offset_, d_level_off_, d_cand_,
-      d_sel_, d_umax_, d_angles_, d_desc_, d_scales_, d_stereo_sad_, d_info_flags_;
-  PinnedBuf h_gray_, h_cand_, h_level_off_, h_sel_, h_angles_, h_desc_, h_pyr_;
+      d_umax_, d_desc_, d_scales_, d_stereo_sad_, d_info_flags_;
+  PinnedBuf h_gray_, h_cand_, h_level_off_, h_desc_, h_pyr_;
   void* d_track_ = nullptr;  // cudaMallocAsync'd by track_scratch()
   size_t track_bytes_ = 0;
   size_t pyr_bytes_ = 0, flat_bytes_ = 0;

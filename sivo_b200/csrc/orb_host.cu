@@ -1,6 +1,7 @@
-// Host side of the ORB operator: constructor tables, the per-level cell grid, the quad-tree keypoint
-// distribution (order dependent and tiny -- stays on the host), and the two-phase device schedule
-//   [pyramid, cells, compact, blur] -> candidates D2H -> quad tree -> selection H2D -> [angle+rBRIEF] -> D2H.
+// Host side of the ORB operator: constructor tables, the per-level cell grid, the host quad tree (the fallback for levels beyond
+// the device tree's caps), and the device schedule
+//   device tree: [pyramid, cells, blur, quad tree, angle+rBRIEF] -> D2H
+//   host tree:   [pyramid, cells, compact, blur] -> candidates D2H -> quad tree -> selection H2D -> [angle+rBRIEF] -> D2H.
 #include <algorithm>
 #include <chrono>
 #include <cmath>
@@ -306,14 +307,20 @@ Orb::Orb(int nfeatures, float scale_factor, int nlevels, int ini_th, int min_th,
     SIVO_CUDA(cudaStreamCreateWithPriority(&stream_, cudaStreamNonBlocking, hi));
   }
   for (auto& e : ev_) SIVO_CUDA(cudaEventCreate(&e));
+  SIVO_CUDA(cudaEventCreateWithFlags(&ev_pyr_, cudaEventDisableTiming));
   d_umax_.alloc(sizeof(tab_.umax));
   SIVO_CUDA(cudaMemcpy(d_umax_.p, tab_.umax, sizeof(tab_.umax), cudaMemcpyHostToDevice));
   sel_cap_ = nfeatures + 4 * nlevels + 64;
-  d_sel_.alloc(sel_cap_ * sizeof(OrbSelected));
-  d_angles_.alloc(sel_cap_ * sizeof(float));
+  // one level of the selection holds up to kTreeSelCap keypoints from the device tree and, short of the capacity error, up to
+  // capacity() from the host tree
+  d_sel_packed_.alloc(static_cast<size_t>(nlevels) * std::max(kTreeSelCap, sel_cap_) * sizeof(uint32_t));
+  d_level_count_.alloc(kOrbMaxLevels * sizeof(int));
+  h_sel_packed_.ensure((kOrbMaxLevels + static_cast<size_t>(nlevels) * sel_cap_) * sizeof(uint32_t));
+  d_n_err_.alloc(2 * sizeof(int));
+  h_n_err_.ensure(2 * sizeof(int));
+  d_kps_.alloc(static_cast<size_t>(sel_cap_) * sizeof(sivo_keypoint));
+  h_kps_.ensure(static_cast<size_t>(sel_cap_) * sizeof(sivo_keypoint));
   d_desc_.alloc(static_cast<size_t>(sel_cap_) * 32);
-  h_sel_.ensure(sel_cap_ * sizeof(OrbSelected));
-  h_angles_.ensure(sel_cap_ * sizeof(float));
   h_desc_.ensure(static_cast<size_t>(sel_cap_) * 32);
   d_stereo_sad_.alloc(sel_cap_ * sizeof(int));
   d_info_flags_.alloc(sel_cap_);
@@ -329,17 +336,7 @@ Orb::Orb(int nfeatures, float scale_factor, int nlevels, int ini_th, int min_th,
     const char* e = std::getenv("SIVO_B200_ORB_DEVICE_TREE");
     device_tree_ = !(e && e[0] == '0');
     for (int l = 0; l < nlevels; ++l) if (tab_.per_level[l] + 8 > kTreeSelCap) device_tree_ = false;
-    if (device_tree_) {
-      orb_tree_configure();
-      d_sel_packed_.alloc(static_cast<size_t>(kOrbMaxLevels) * kTreeSelCap * sizeof(uint32_t));
-      d_level_count_.alloc(kOrbMaxLevels * sizeof(int));
-      d_n_err_.alloc(2 * sizeof(int));
-      d_kps_.alloc(static_cast<size_t>(sel_cap_) * sizeof(sivo_keypoint));
-      h_n_err_.ensure(2 * sizeof(int));
-      h_kps_.ensure(static_cast<size_t>(sel_cap_) * sizeof(sivo_keypoint));
-      SIVO_CUDA(cudaEventCreateWithFlags(&ev_wait_, cudaEventDisableTiming));
-      SIVO_CUDA(cudaEventCreateWithFlags(&ev_pyr_, cudaEventDisableTiming));
-    }
+    if (device_tree_) orb_tree_configure();
   }
   d_level_off_.alloc((kOrbMaxLevels + 1) * sizeof(int));
   h_level_off_.ensure((kOrbMaxLevels + 1) * sizeof(int));
@@ -468,24 +465,55 @@ void Orb::run(const uint8_t* gray, int rows, int cols, size_t stride, sivo_keypo
     SIVO_CUDA(cudaEventRecord(ev_[0], s));
   }
   enqueue_front(src, src_pitch, s);
+  // the 1.6 MB pyramid read-back (the public mvImagePyramid) leaves on a second stream as soon as the level images exist, under
+  // FAST, the quad tree and describe
   bool pyr_direct = pyr_out != nullptr;
-  if (pyr_out)
+  if (pyr_out) {
     for (int l = 0; l < nlevels_; ++l) pyr_direct = pyr_direct && pyr_out[l] && is_pinned_host(pyr_out[l]);
-  auto enqueue_pyramid_readback = [&](cudaStream_t s) {
-    if (pyr_out && pyr_direct) {  // page-locked level buffers (mvImagePyramid storage): strided copies straight into them
+    if (!copy_stream_) SIVO_CUDA(cudaStreamCreateWithFlags(&copy_stream_, cudaStreamNonBlocking));
+    SIVO_CUDA(cudaStreamWaitEvent(copy_stream_, ev_pyr_, 0));
+    if (pyr_direct) {  // page-locked level buffers (mvImagePyramid storage): strided copies straight into them
       for (int l = 0; l < nlevels_; ++l) {
         const OrbLevel& lv = lt_.lv[l];
         const size_t dst_stride = pyr_strides ? pyr_strides[l] : static_cast<size_t>(lv.w + 2 * kEdge);
         if (dst_stride < static_cast<size_t>(lv.w + 2 * kEdge)) fail(SIVO_EINVAL, "pyramid stride %zu too small for level %d", dst_stride, l);
         SIVO_CUDA(cudaMemcpy2DAsync(pyr_out[l], dst_stride, d_pyr_.as<uint8_t>() + lv.img_off, lv.pitch, lv.w + 2 * kEdge,
-                                    lv.h + 2 * kEdge, cudaMemcpyDeviceToHost, s));
+                                    lv.h + 2 * kEdge, cudaMemcpyDeviceToHost, copy_stream_));
       }
-    } else if (pyr_out) {
-      SIVO_CUDA(cudaMemcpyAsync(h_pyr_.p, d_pyr_.p, pyr_bytes_, cudaMemcpyDeviceToHost, s));
+    } else {
+      SIVO_CUDA(cudaMemcpyAsync(h_pyr_.p, d_pyr_.p, pyr_bytes_, cudaMemcpyDeviceToHost, copy_stream_));
     }
-  };
-  auto copy_out_pyramid = [&] {
-    if (!(pyr_out && !pyr_direct)) return;
+  }
+  const int* n_err = h_n_err_.as<int>();
+  bool host_tree = !device_tree_;
+  launches = nlevels_ + 1;  // the pyramid levels and k_cells
+  if (device_tree_) {
+    // ---- device quad tree: one asynchronous chain, one synchronisation at the end
+    SIVO_CUDA(cudaEventRecord(ev_[1], s));
+    enqueue_tree_and_describe(d_kps_.as<sivo_keypoint>(), d_desc_.as<uint8_t>(), nullptr, s);
+    enqueue_results_readback(s);
+    launches += 3;  // blur, distribute, describe
+    SIVO_CUDA(cudaStreamSynchronize(s));
+    // bits 0-15: a level exceeded the device tree's caps, so the host tree takes the call (the candidates are still on the device)
+    host_tree = (n_err[1] & 0xFFFF) != 0;
+    if (!host_tree) {
+      float a = 0, b2 = 0;
+      SIVO_CUDA(cudaEventElapsedTime(&a, ev_[0], ev_[1]));
+      SIVO_CUDA(cudaEventElapsedTime(&b2, ev_[1], ev_[3]));
+      device_ms = a + b2;
+      tree_ms = 0.f;
+      last_off_.clear();  // candidates() fetches them from the device on demand
+    }
+  }
+  if (host_tree) run_host_tree(w0);
+  if (pyr_out) SIVO_CUDA(cudaStreamSynchronize(copy_stream_));
+  if (n_err[1] & (1 << 30)) fail(SIVO_ERANGE, "ORBextractor: more keypoints than the workspace holds (%d)", sel_cap_);
+  const int total = n_err[0];
+  if (n) *n = total;
+  if (total > cap) fail(SIVO_ERANGE, "ORBextractor: %d keypoints but the caller's buffers hold %d", total, cap);
+  if (kps && total) memcpy(kps, h_kps_.p, static_cast<size_t>(total) * sizeof(sivo_keypoint));
+  if (desc && total) memcpy(desc, h_desc_.p, static_cast<size_t>(total) * 32);
+  if (pyr_out && !pyr_direct) {
     for (int l = 0; l < nlevels_; ++l) {
       if (!pyr_out[l]) continue;
       const OrbLevel& lv = lt_.lv[l];
@@ -495,54 +523,19 @@ void Orb::run(const uint8_t* gray, int rows, int cols, size_t stride, sivo_keypo
       for (int y = 0; y < lv.h + 2 * kEdge; ++y)
         memcpy(pyr_out[l] + static_cast<size_t>(y) * dst_stride, srcl + static_cast<size_t>(y) * lv.pitch, lv.w + 2 * kEdge);
     }
-  };
-  bool pyramid_enqueued = false;
-  if (device_tree_) {
-    // ---- device quad tree: one asynchronous chain, one synchronisation at the end; the 1.6 MB pyramid read-back (the public
-    // mvImagePyramid) leaves on a second stream as soon as the level images exist, under FAST / tree / describe
-    if (pyr_out) {
-      if (!copy_stream_) {
-        SIVO_CUDA(cudaStreamCreateWithFlags(&copy_stream_, cudaStreamNonBlocking));
-      }
-      SIVO_CUDA(cudaStreamWaitEvent(copy_stream_, ev_pyr_, 0));
-      enqueue_pyramid_readback(copy_stream_);
-      pyramid_enqueued = true;
-    }
-    SIVO_CUDA(cudaEventRecord(ev_[1], s));
-    enqueue_tree_and_describe(d_kps_.as<sivo_keypoint>(), d_desc_.as<uint8_t>(), nullptr, s);
-    SIVO_CUDA(cudaEventRecord(ev_[2], s));
-    SIVO_CUDA(cudaMemcpyAsync(h_n_err_.p, d_n_err_.p, 2 * sizeof(int), cudaMemcpyDeviceToHost, s));
-    SIVO_CUDA(cudaMemcpyAsync(h_kps_.p, d_kps_.p, static_cast<size_t>(sel_cap_) * sizeof(sivo_keypoint), cudaMemcpyDeviceToHost, s));
-    SIVO_CUDA(cudaMemcpyAsync(h_desc_.p, d_desc_.p, static_cast<size_t>(sel_cap_) * 32, cudaMemcpyDeviceToHost, s));
-    SIVO_CUDA(cudaEventRecord(ev_[3], s));
-    launches = nlevels_ + 4;
-    SIVO_CUDA(cudaStreamSynchronize(s));
-    if (pyramid_enqueued) SIVO_CUDA(cudaStreamSynchronize(copy_stream_));
-    const int total = h_n_err_.as<int>()[0], err = h_n_err_.as<int>()[1];
-    if (!err) {
-      float a = 0, b2 = 0;
-      SIVO_CUDA(cudaEventElapsedTime(&a, ev_[0], ev_[1]));
-      SIVO_CUDA(cudaEventElapsedTime(&b2, ev_[1], ev_[3]));
-      device_ms = a + b2;
-      tree_ms = 0.f;
-      last_off_.clear();  // candidates() fetches them from the device on demand
-      if (n) *n = total;
-      if (total > cap) fail(SIVO_ERANGE, "ORBextractor: %d keypoints but the caller's buffers hold %d", total, cap);
-      if (kps && total) memcpy(kps, h_kps_.p, static_cast<size_t>(total) * sizeof(sivo_keypoint));
-      if (desc && total) memcpy(desc, h_desc_.p, static_cast<size_t>(total) * 32);
-      copy_out_pyramid();
-      return;
-    }
-    // a level exceeded the device tree's caps: take the host path below (the candidates are still on the device)
   }
+}
+
+// ---- host quad tree: candidates down, orb_distribute per level on the pool, the selection up, the describe pass
+void Orb::run_host_tree(std::chrono::steady_clock::time_point w0) {
+  cudaStream_t s = stream_;
   enqueue_compact(s);
   SIVO_CUDA(cudaMemcpyAsync(h_level_off_.p, d_level_off_.p, (nlevels_ + 1) * sizeof(int), cudaMemcpyDeviceToHost, s));
   SIVO_CUDA(cudaMemcpyAsync(h_cand_.p, d_cand_.p, static_cast<size_t>(cand_cap_) * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
   SIVO_CUDA(cudaEventRecord(ev_[1], s));
-  // the blur and the pyramid read-back overlap the host quad tree
-  orb_launch_blur(d_pyr_.as<uint8_t>(), d_blur_.as<uint8_t>(), lt_, s);
-  if (!pyramid_enqueued) enqueue_pyramid_readback(s);
-  launches = nlevels_ + 6;
+  // the blur overlaps the host quad tree (the device tree's chain, if it ran, has blurred already)
+  if (!device_tree_) orb_launch_blur(d_pyr_.as<uint8_t>(), d_blur_.as<uint8_t>(), lt_, s);
+  launches += device_tree_ ? 3 : 4;  // compact's two, describe, and the blur if it has not run
   static const bool trace = [] { const char* e = std::getenv("SIVO_B200_ORB_TRACE"); return e && e[0] == '1'; }();
   const auto w1 = std::chrono::steady_clock::now();
   SIVO_CUDA(cudaEventSynchronize(ev_[1]));
@@ -552,9 +545,6 @@ void Orb::run(const uint8_t* gray, int rows, int cols, size_t stride, sivo_keypo
   const uint32_t* cand = h_cand_.as<uint32_t>();
   if (loff[nlevels_] > cand_cap_) fail(SIVO_ERANGE, "ORBextractor: %d FAST candidates exceed the workspace (%d)", loff[nlevels_], cand_cap_);
   auto t0 = std::chrono::steady_clock::now();
-  std::vector<sivo_keypoint> out;
-  out.reserve(nfeatures_ + 4 * nlevels_);
-  OrbSelected* sel = h_sel_.as<OrbSelected>();
   last_off_.assign(loff, loff + nlevels_ + 1);
   last_cand_.assign(cand, cand + loff[nlevels_]);
   const int min_b = kEdge - 3;
@@ -596,37 +586,24 @@ void Orb::run(const uint8_t* gray, int rows, int cols, size_t stride, sivo_keypo
     if (pool_) pool_->run(share); else share(0);
     if (!worker_error.empty()) fail(SIVO_EINVAL, "ORBextractor: quad tree failed: %s", worker_error.c_str());
   }
+  // the selection in the device tree's form: kept index k of level l is candidate loff[l] + k, whose packed word is the entry;
+  // a level longer than capacity() means more keypoints than that in all, which k_describe reports without reading the words
+  int stride = 0;
+  for (int l = 0; l < nlevels_; ++l) stride = std::max(stride, static_cast<int>(lkeep_[l].size()));
+  stride = std::min(stride, sel_cap_);
+  int* count = h_sel_packed_.as<int>();
+  uint32_t* sel = h_sel_packed_.as<uint32_t>() + kOrbMaxLevels;
   for (int l = 0; l < nlevels_; ++l) {
-    const std::vector<float>&xs = lxs_[l], &ys = lys_[l], &rs = lrs_[l];
-    const std::vector<int>& keep = lkeep_[l];
-    const int scaled_patch = static_cast<int>(31 * tab_.scale[l]);  // PATCH_SIZE * mvScaleFactor[level] (:828)
-    for (int k : keep) {
-      sivo_keypoint kp;
-      kp.x = xs[k] + min_b;
-      kp.y = ys[k] + min_b;
-      kp.size = static_cast<float>(scaled_patch);
-      kp.angle = -1.f;
-      kp.response = rs[k];
-      kp.octave = l;
-      kp.class_id = -1;
-      if (static_cast<int>(out.size()) >= sel_cap_) fail(SIVO_ERANGE, "ORBextractor: more keypoints than the workspace holds");
-      OrbSelected& sk = sel[out.size()];
-      sk.x = static_cast<short>(kp.x); sk.y = static_cast<short>(kp.y); sk.level = static_cast<short>(l); sk.pad = 0;
-      out.push_back(kp);
-    }
+    count[l] = static_cast<int>(lkeep_[l].size());
+    for (int k = 0; k < std::min(count[l], stride); ++k) sel[l * stride + k] = cand[loff[l] + lkeep_[l][k]];
   }
   tree_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
-  const int total = static_cast<int>(out.size());
   SIVO_CUDA(cudaEventRecord(ev_[2], s));
-  if (total) {
-    SIVO_CUDA(cudaMemcpyAsync(d_sel_.p, sel, total * sizeof(OrbSelected), cudaMemcpyHostToDevice, s));
-    orb_launch_describe(d_pyr_.as<uint8_t>(), d_blur_.as<uint8_t>(), lt_, d_sel_.as<OrbSelected>(), total, d_umax_.as<int>(),
-                        d_angles_.as<float>(), d_desc_.as<uint8_t>(), s);
-    SIVO_CUDA(cudaMemcpyAsync(h_angles_.p, d_angles_.p, total * sizeof(float), cudaMemcpyDeviceToHost, s));
-    SIVO_CUDA(cudaMemcpyAsync(h_desc_.p, d_desc_.p, static_cast<size_t>(total) * 32, cudaMemcpyDeviceToHost, s));
-    ++launches;
-  }
-  SIVO_CUDA(cudaEventRecord(ev_[3], s));
+  SIVO_CUDA(cudaMemcpyAsync(d_level_count_.p, count, nlevels_ * sizeof(int), cudaMemcpyHostToDevice, s));
+  SIVO_CUDA(cudaMemcpyAsync(d_sel_packed_.p, sel, static_cast<size_t>(nlevels_) * stride * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+  SIVO_CUDA(cudaMemsetAsync(d_n_err_.p, 0, 2 * sizeof(int), s));
+  enqueue_describe(stride, d_kps_.as<sivo_keypoint>(), d_desc_.as<uint8_t>(), nullptr, s);
+  enqueue_results_readback(s);
   const auto w3 = std::chrono::steady_clock::now();
   SIVO_CUDA(cudaStreamSynchronize(s));
   if (trace) {
@@ -638,28 +615,12 @@ void Orb::run(const uint8_t* gray, int rows, int cols, size_t stride, sivo_keypo
   SIVO_CUDA(cudaEventElapsedTime(&a, ev_[0], ev_[1]));
   SIVO_CUDA(cudaEventElapsedTime(&b2, ev_[2], ev_[3]));
   device_ms = a + b2;
-  if (n) *n = total;
-  if (total > cap) fail(SIVO_ERANGE, "ORBextractor: %d keypoints but the caller's buffers hold %d", total, cap);
-  const float* ang = h_angles_.as<float>();
-  for (int i = 0; i < total; ++i) {
-    sivo_keypoint kp = out[i];
-    kp.angle = ang[i];
-    if (kp.octave != 0) {  // keypoint->pt *= scale (:1071-1078)
-      float sc = tab_.scale[kp.octave];
-      kp.x *= sc;
-      kp.y *= sc;
-    }
-    if (kps) kps[i] = kp;
-  }
-  if (desc && total) memcpy(desc, h_desc_.p, static_cast<size_t>(total) * 32);
-  if (pyramid_enqueued && copy_stream_) SIVO_CUDA(cudaStreamSynchronize(copy_stream_));
-  copy_out_pyramid();
 }
 
 void Orb::enqueue_front(const uint8_t* src, size_t src_pitch, cudaStream_t s) {
   const int ncells = static_cast<int>(cells_.size());
   orb_launch_pyramid(src, rows_, cols_, src_pitch, d_pyr_.as<uint8_t>(), lt_, s);
-  if (ev_pyr_) SIVO_CUDA(cudaEventRecord(ev_pyr_, s));  // the level images are final: their read-back can start on the copy stream
+  SIVO_CUDA(cudaEventRecord(ev_pyr_, s));  // the level images are final: their read-back can start on the copy stream
   orb_launch_cells(d_pyr_.as<uint8_t>(), lt_, d_cells_.as<OrbCell>(), ncells, ini_th_, min_th_, d_cell_count_.as<int>(),
                    d_cell_items_.as<uint32_t>(), s);
   compacted_ = false;  // the device tree reads the cell lists directly; the host path and the test hook compact on demand
@@ -678,8 +639,20 @@ void Orb::enqueue_tree_and_describe(sivo_keypoint* kps_dev, uint8_t* desc_dev, l
   orb_launch_blur(d_pyr_.as<uint8_t>(), d_blur_.as<uint8_t>(), lt_, s);
   orb_launch_distribute(nullptr, nullptr, d_cell_items_.as<uint32_t>(), d_cell_count_.as<int>(), tree_prm_, nlevels_,
                         d_sel_packed_.as<uint32_t>(), d_level_count_.as<int>(), n_dev + 1, s);
-  orb_launch_describe_dev(d_pyr_.as<uint8_t>(), d_blur_.as<uint8_t>(), lt_, d_sel_packed_.as<uint32_t>(), d_level_count_.as<int>(), tree_prm_,
-                          sel_cap_, d_umax_.as<int>(), kps_dev, desc_dev, n_dev, count_dev, n_dev + 1, s);
+  enqueue_describe(kTreeSelCap, kps_dev, desc_dev, count_dev, s);
+}
+
+void Orb::enqueue_describe(int stride, sivo_keypoint* kps_dev, uint8_t* desc_dev, long long* count_dev, cudaStream_t s) {
+  int* n_dev = d_n_err_.as<int>();
+  orb_launch_describe_dev(d_pyr_.as<uint8_t>(), d_blur_.as<uint8_t>(), lt_, d_sel_packed_.as<uint32_t>(), d_level_count_.as<int>(), stride,
+                          tree_prm_, sel_cap_, d_umax_.as<int>(), kps_dev, desc_dev, n_dev, count_dev, n_dev + 1, s);
+}
+
+void Orb::enqueue_results_readback(cudaStream_t s) {
+  SIVO_CUDA(cudaMemcpyAsync(h_n_err_.p, d_n_err_.p, 2 * sizeof(int), cudaMemcpyDeviceToHost, s));
+  SIVO_CUDA(cudaMemcpyAsync(h_kps_.p, d_kps_.p, static_cast<size_t>(sel_cap_) * sizeof(sivo_keypoint), cudaMemcpyDeviceToHost, s));
+  SIVO_CUDA(cudaMemcpyAsync(h_desc_.p, d_desc_.p, static_cast<size_t>(sel_cap_) * 32, cudaMemcpyDeviceToHost, s));
+  SIVO_CUDA(cudaEventRecord(ev_[3], s));
 }
 
 void Orb::enqueue_device(const uint8_t* gray_dev, int rows, int cols, size_t pitch, sivo_keypoint* kps_dev, uint8_t* desc_dev,

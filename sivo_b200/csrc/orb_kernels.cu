@@ -303,47 +303,37 @@ __device__ __forceinline__ float fast_atan2_deg(float y, float x) {
 }
 
 // ---- one warp per keypoint: IC_Angle (ORBextractor.cc:75-100) then computeOrbDescriptor (:104-150).
-// Device-tree form (sel_packed != nullptr): the per-level selections of k_distribute are concatenated level-major on the fly --
-// every warp derives the level offsets from the eight counts -- and the finished keypoint record is written here
-// (ComputeKeyPointsOctTree :824-835, operator() :1071-1078), so no separate pass builds the OrbSelected list.
-__global__ void k_describe(const uint8_t* __restrict__ pyr, const uint8_t* __restrict__ blur, OrbLevelTable t,
-                           const OrbSelected* __restrict__ sel, int n, const int* __restrict__ umax,
-                           float* __restrict__ angles, uint8_t* __restrict__ desc, const uint32_t* __restrict__ sel_packed,
-                           const int* __restrict__ level_count, OrbTreeParams prm, sivo_keypoint* __restrict__ kps,
-                           int* __restrict__ n_out, long long* __restrict__ n_out_i64, int* __restrict__ out_error) {
+// The per-level selections (either quad tree's) are concatenated level-major on the fly -- every warp derives the level
+// offsets from the counts -- and the finished keypoint record is written here (ComputeKeyPointsOctTree :824-835,
+// operator() :1071-1078).  Bounded to 32 registers (16 blocks of 128 fill an SM), which it fits without spilling.
+__global__ void __launch_bounds__(128, 16)
+k_describe(const uint8_t* __restrict__ pyr, const uint8_t* __restrict__ blur, OrbLevelTable t, int n, const int* __restrict__ umax,
+           uint8_t* __restrict__ desc, const uint32_t* __restrict__ sel_packed, const int* __restrict__ level_count, int stride,
+           OrbTreeParams prm, sivo_keypoint* __restrict__ kps, int* __restrict__ n_out, long long* __restrict__ n_out_i64,
+           int* __restrict__ out_error) {
   int wid = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  OrbSelected kp;
-  uint32_t packed = 0;
-  if (sel_packed) {
-    int off = 0, lvl = -1, idx = 0;
-    for (int l = 0; l < t.nlevels; ++l) {
-      const int c = level_count[l];
-      if (lvl < 0 && wid < off + c) { lvl = l; idx = wid - off; }
-      off += c;
-    }
-    const bool too_many = off > n;  // n = capacity of the output buffers
-    if (blockIdx.x == 0 && threadIdx.x == 0) {
-      if (too_many) atomicOr(out_error, 1 << 30);
-      *n_out = too_many ? 0 : off;
-      if (n_out_i64) *n_out_i64 = too_many ? 0 : off;
-    }
-    if (too_many || lvl < 0) return;
-    packed = sel_packed[lvl * kTreeSelCap + idx];
-    kp.x = static_cast<short>(static_cast<int>(packed & 0xFFF) + prm.min_b);
-    kp.y = static_cast<short>(static_cast<int>((packed >> 12) & 0xFFF) + prm.min_b);
-    kp.level = static_cast<short>(lvl);
-    kp.pad = 0;
-  } else {
-    if (wid >= n) return;
-    kp = sel[wid];
+  int off = 0, level = -1, i = 0;  // this warp's keypoint: the i-th of `level`
+  for (int l = 0; l < t.nlevels; ++l) {
+    const int c = level_count[l];
+    if (level < 0 && wid < off + c) { level = l; i = wid - off; }
+    off += c;
   }
-  const OrbLevel lv = t.lv[kp.level];
+  const bool too_many = off > n;  // n = capacity of the output buffers
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    if (too_many) atomicOr(out_error, 1 << 30);
+    *n_out = too_many ? 0 : off;
+    if (n_out_i64) *n_out_i64 = too_many ? 0 : off;
+  }
+  if (too_many || level < 0) return;
+  const uint32_t packed = sel_packed[level * stride + i];
+  const int kx = static_cast<int>(packed & 0xFFF) + prm.min_b, ky = static_cast<int>((packed >> 12) & 0xFFF) + prm.min_b;
+  const OrbLevel lv = t.lv[level];
   // intensity centroid over the radius-15 disc: lane = row v + 15
   int m10 = 0, m01 = 0;
   if (lane < 2 * kHalfPatch + 1) {
     int v = lane - kHalfPatch;
     int d = umax[abs(v)];
-    const uint8_t* row = pyr + lv.img_off + static_cast<size_t>(kp.y + v + kEdge) * lv.pitch + kp.x + kEdge;
+    const uint8_t* row = pyr + lv.img_off + static_cast<size_t>(ky + v + kEdge) * lv.pitch + kx + kEdge;
     int sum = 0;
     for (int u = -d; u <= d; ++u) {
       int val = row[u];
@@ -359,20 +349,16 @@ __global__ void k_describe(const uint8_t* __restrict__ pyr, const uint8_t* __res
   }
   const float angle = fast_atan2_deg(static_cast<float>(m01), static_cast<float>(m10));
   if (lane == 0) {
-    if (sel_packed) {
-      sivo_keypoint o;
-      o.x = static_cast<float>(kp.x);
-      o.y = static_cast<float>(kp.y);
-      if (kp.level != 0) { o.x = __fmul_rn(o.x, prm.scale[kp.level]); o.y = __fmul_rn(o.y, prm.scale[kp.level]); }
-      o.size = prm.size[kp.level];
-      o.angle = angle;
-      o.response = static_cast<float>(packed >> 24);
-      o.octave = kp.level;
-      o.class_id = -1;
-      kps[wid] = o;
-    } else {
-      angles[wid] = angle;
-    }
+    sivo_keypoint o;
+    o.x = static_cast<float>(kx);
+    o.y = static_cast<float>(ky);
+    if (level != 0) { o.x = __fmul_rn(o.x, prm.scale[level]); o.y = __fmul_rn(o.y, prm.scale[level]); }
+    o.size = prm.size[level];
+    o.angle = angle;
+    o.response = static_cast<float>(packed >> 24);
+    o.octave = level;
+    o.class_id = -1;
+    kps[wid] = o;
   }
   // rotated BRIEF: lane = descriptor byte
   const float factor_pi = static_cast<float>(3.141592653589793238462643383279502884 / 180.f);
@@ -391,7 +377,7 @@ __global__ void k_describe(const uint8_t* __restrict__ pyr, const uint8_t* __res
       float px = static_cast<float>(pt[2 * q]), py = static_cast<float>(pt[2 * q + 1]);
       int ry = __float2int_rn(__fadd_rn(__fmul_rn(px, b), __fmul_rn(py, a)));
       int rx = __float2int_rn(__fsub_rn(__fmul_rn(px, a), __fmul_rn(py, b)));
-      int idx = (kp.y + ry) * lv.w + kp.x + rx;  // flat index into the continuous clone, as the reference computes it
+      int idx = (ky + ry) * lv.w + kx + rx;  // flat index into the continuous clone, as the reference computes it
       tv[q] = (idx >= 0 && idx < npx) ? img[idx] : 0;
     }
     val |= (tv[0] < tv[1]) << k;
@@ -438,18 +424,11 @@ void orb_launch_blur(const uint8_t* pyr, uint8_t* blur, const OrbLevelTable& t, 
   SIVO_CUDA(cudaGetLastError());
 }
 
-void orb_launch_describe(const uint8_t* pyr, const uint8_t* blur, const OrbLevelTable& t, const OrbSelected* sel, int n,
-                         const int* umax, float* angles, uint8_t* desc, cudaStream_t s) {
-  if (n == 0) return;
-  k_describe<<<ceil_div(n * 32, 128), 128, 0, s>>>(pyr, blur, t, sel, n, umax, angles, desc, nullptr, nullptr, OrbTreeParams{}, nullptr, nullptr, nullptr, nullptr);
-  SIVO_CUDA(cudaGetLastError());
-}
-
 void orb_launch_describe_dev(const uint8_t* pyr, const uint8_t* blur, const OrbLevelTable& t, const uint32_t* sel_packed,
-                             const int* level_count, const OrbTreeParams& prm, int cap, const int* umax, sivo_keypoint* kps,
-                             uint8_t* desc, int* n_out, long long* n_out_i64, int* error, cudaStream_t s) {
+                             const int* level_count, int stride, const OrbTreeParams& prm, int cap, const int* umax,
+                             sivo_keypoint* kps, uint8_t* desc, int* n_out, long long* n_out_i64, int* error, cudaStream_t s) {
   if (cap == 0) return;
-  k_describe<<<ceil_div(cap * 32, 128), 128, 0, s>>>(pyr, blur, t, nullptr, cap, umax, nullptr, desc, sel_packed, level_count, prm, kps, n_out,
+  k_describe<<<ceil_div(cap * 32, 128), 128, 0, s>>>(pyr, blur, t, cap, umax, desc, sel_packed, level_count, stride, prm, kps, n_out,
                                                      n_out_i64, error);
   SIVO_CUDA(cudaGetLastError());
 }

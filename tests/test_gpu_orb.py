@@ -250,6 +250,19 @@ def test_device_and_host_quad_tree_give_the_same_extraction(monkeypatch, kitti_g
             assert ka.tobytes() == kb.tobytes() and np.array_equal(da, db)
 
 
+def test_host_tree_level_larger_than_the_device_tree_selection(kitti_gray_crop):
+    """nfeatures = 5000 asks for 1086 keypoints at level 0, more than one level of the device tree's selection holds (1024), so
+    the host tree takes every call; it keeps 1087 at level 0, which the describe pass reads at a stride wider than the device
+    tree's."""
+    ext = ORBextractor(5000, 1.2, 8, 20, 7)
+    assert not ext.has_device_tree()
+    kps, desc = ext(kitti_gray_crop, None)
+    r = O.extract(kitti_gray_crop, O.ExtractorParams(5000))
+    assert (kps["octave"] == 0).sum() == 1087
+    assert np.array_equal(kp_matrix(kps), r.keypoints.astype(np.float32))
+    assert np.array_equal(desc, r.descriptors)
+
+
 def test_asynchronous_device_form_writes_the_same_record(kitti_gray_crop):
     """sivo_orb_enqueue_device: gray image, keypoints, descriptors and count all stay on the device (what the multi-GPU record
     path uses); the results equal the synchronous operator's."""
