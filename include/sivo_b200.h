@@ -566,6 +566,111 @@ int sivo_dbg_create_map_points(const sivo_orb_t* left, const sivo_keyframe_keys*
                                int n_neighbours, const sivo_mapping_params* params, int* match, int* stage, double* reduction,
                                int* created_nb, int* created_idx, float* world, int* created_list, long long* n_created);
 
+/* ---- the DBoW2 vocabulary: TemplatedVocabulary<FORB::TDescriptor, FORB>::loadFromTextFile (DBoW2 TemplatedVocabulary.h:1338-1420)
+ * ---------------------------------------------------------------------------------------------------------------------------------
+ * Text form: line 1 is `k L scoring weighting`; every further line is one node, id = its line number (the root is 0 and has no
+ * line): `parent isLeaf d0 .. d31 weight`.  A descriptor byte is (unsigned char) of its integer token (FORB::fromString); the
+ * weight is a double; tokens after the weight are ignored; leaves (isLeaf > 0) get word ids in id order; a node's children keep
+ * id order, which decides ties in the descent.  Refused with SIVO_EFORMAT:
+ *   header    where the reference returns false: k < 0 || k > 20 || L < 1 || L > 10 || scoring outside [0, 5] || weighting outside
+ *             [0, 3]; also fewer than four integer tokens.
+ *   node      a parent that is not an earlier node, a parent that is a leaf, fewer than 34 integer tokens before the weight or no
+ *             weight (a truncated final line included), a non-leaf node without children (the reference would index its empty child
+ *             list), an empty tree.
+ *   blank     trailing whitespace-only lines add no node (the reference's eof loop would append a phantom child of the root with an
+ *             indeterminate descriptor); a blank line followed by a further node is refused (the reference would shift every later
+ *             id).
+ * Enum values are DBoW2's: weighting TF_IDF 0, TF 1, IDF 2, BINARY 3; scoring L1_NORM 0, L2_NORM 1, CHI_SQUARE 2, KL 3,
+ * BHATTACHARYYA 4, DOT_PRODUCT 5.  The device copy holds 32 descriptor bytes, a child offset, a child id and a word id per node and
+ * a double per word (about 56 MB for ORBvoc).  A vocabulary is read-only once created: any number of threads may use it at once. */
+typedef struct sivo_vocabulary sivo_vocabulary_t;
+enum { SIVO_WEIGHTING_TF_IDF = 0, SIVO_WEIGHTING_TF = 1, SIVO_WEIGHTING_IDF = 2, SIVO_WEIGHTING_BINARY = 3 };
+enum { SIVO_SCORING_L1_NORM = 0, SIVO_SCORING_L2_NORM = 1, SIVO_SCORING_CHI_SQUARE = 2, SIVO_SCORING_KL = 3,
+       SIVO_SCORING_BHATTACHARYYA = 4, SIVO_SCORING_DOT_PRODUCT = 5 };
+/* Loads a text vocabulary onto `device`.  SIVO_ENOENT if the file cannot be read, SIVO_EFORMAT as above. */
+int sivo_vocabulary_load_text(const char* path, int device, sivo_vocabulary_t** out);
+/* The same tree as arrays of n_nodes entries indexed by node id, the root at 0 (its entries are ignored): parent, is_leaf (nonzero:
+ * leaf), desc (32 bytes per node), weight.  The text loader is a parser in front of this call; the same rules apply. */
+int sivo_vocabulary_create(int device, int k, int L, int scoring, int weighting, const int32_t* parent, const uint8_t* is_leaf,
+                           const uint8_t* desc, const double* weight, int n_nodes, sivo_vocabulary_t** out);
+/* n_nodes counts the root; any output may be NULL. */
+int sivo_vocabulary_info(const sivo_vocabulary_t* voc, int* k, int* L, int* scoring, int* weighting, int* n_nodes, int* n_words);
+void sivo_vocabulary_destroy(sivo_vocabulary_t* voc);
+/* Test hook: the text parser and the checks without a device.  header[4] = k, L, scoring, weighting; *n_nodes (root included);
+ * the arrays as sivo_vocabulary_create takes them (the root's entries: parent -1, not a leaf, zero descriptor and weight), written
+ * only when capacity >= *n_nodes (each may be NULL); SIVO_ERANGE with *n_nodes set when capacity is smaller. */
+int sivo_dbg_vocabulary_parse(const char* path, int* header, int* n_nodes, int32_t* parent, uint8_t* is_leaf, uint8_t* desc,
+                              double* weight, int capacity);
+
+/* ---- Frame::ComputeBoW / KeyFrame::ComputeBoW: TemplatedVocabulary::transform(features, v, fv, levelsup) (TemplatedVocabulary.h:
+ * 1127-1195) and the per-feature descent (:1218-1259) over a frame's semantic descriptors --------------------------------------
+ * Every operation is the IEEE double operation as written (no contracted multiply-add).  oracle/bow_oracle.py restates the rules:
+ *   descent   from the root, each level takes the child with the smallest Hamming distance, compared with a strict `<` in child
+ *             order (the first child wins ties), until a node without children (a leaf).  The node recorded is the one reached at
+ *             level nid_level = L - levelsup; the root (0) when nid_level <= 0; the leaf itself when the path ends above
+ *             nid_level (the reference leaves nid uninitialised there: in practice the previous feature's node).
+ *   keys      a key enters the BowVector and the FeatureVector only when its word's weight w > 0 (stopped words have w = 0).
+ *   BowVec    TF / TF_IDF: the double sum of w per word in feature order (addWeight); IDF / BINARY: w (addIfNotExist).  Scoring
+ *             DOT_PRODUCT needs no normalisation: TF / TF_IDF weights are divided by the number of words, IDF / BINARY kept.
+ *             Otherwise BowVector::normalize: L1 = the sum of |w| in ascending word order (L1_NORM, CHI_SQUARE, KL, BHATTACHARYYA),
+ *             L2 = sqrt of the sum of w * w in that order (L2_NORM); each weight divided by the norm only if it is > 0.
+ * Semantic key j < *n_keep_device is extractor key keep_idx_device[j] (j when NULL) of desc_device.  Outputs, each may be NULL:
+ * node_device[j] = the key's mFeatVec node or -1 when the key is in no FeatureVector entry (sivo_keyframe_keys.node's convention);
+ * word_device[j] = its BowVector word or -1 likewise (both sivo_orb_capacity(left) room); bow_word_device / bow_weight_device =
+ * mBowVec as ascending word ids and double weights (capacity room), *bow_len_device (int64) its length.  The count is clamped to
+ * the capacity; a negative count (the -1 of sivo_segnet_semantic_keys_device) writes only *bow_len_device = -1.  A key index
+ * outside the capacity gives node and word -1.  The same call computes KeyFrame::ComputeBoW on sivo_keyframe_gather_device's copy
+ * (keep_idx NULL).  Runs on `stream` (NULL = the left extractor's stream) with no waits and no host synchronisation; its scratch
+ * is allocated and freed on `stream` (stream-ordered) and it reads only the vocabulary and its inputs, so LocalMapping's thread may
+ * run it concurrently with Tracking's calls on the same extractor.  SIVO_EINVAL for NULL handles or inputs, levelsup < 0, or a
+ * vocabulary on another device; SIVO_ERANGE for an extractor capacity above 16,384 keys (the BowVector is sorted in shared memory). */
+int sivo_compute_bow_device(const sivo_vocabulary_t* voc, const sivo_orb_t* left, const uint8_t* desc_device, const int* keep_idx_device,
+                            const long long* n_keep_device, int levelsup, int* node_device, int* word_device, int* bow_word_device,
+                            double* bow_weight_device, long long* bow_len_device, void* stream);
+/* Host form: n host descriptors (n x 32); node / word (n), bow_word / bow_weight (n room), *bow_len, any may be NULL.  It stages
+ * the descriptors on the vocabulary's device, runs the device form's kernels and synchronises.  SIVO_EINVAL as above and for
+ * n < 0; SIVO_ERANGE for n > 16,384. */
+int sivo_compute_bow(const sivo_vocabulary_t* voc, const uint8_t* desc, int n, int levelsup, int* node, int* word, int* bow_word,
+                     double* bow_weight, int* bow_len);
+
+/* ---- ORBmatcher::SearchByBoW(KeyFrame*, Frame&, vpMapPointMatches) (ORBmatcher.cc:161-284), batched over keyframes: Tracking::
+ * TrackReferenceKeyFrame (ratio 0.7, orientation check; Tracking.cc:597-639) and Relocalization's candidates (0.75;
+ * Tracking.cc:1237-1286) ---------------------------------------------------------------------------------------------------------
+ * Every operation is the IEEE float operation as written.  oracle/bow_oracle.py restates the rules:
+ *   walk      nodes present in both FeatureVectors, ascending id; within a node the keyframe's keys in ascending index, only those
+ *             with a point (kf_point >= 0); candidates are the frame's keys of that node, ascending index, not yet matched by this
+ *             call (vpMapPointMatches starts empty per call).  Best and second-best folded with strict `<` (:209-226); accepted iff
+ *             bestDist <= TH_LOW (50) and (float) bestDist < nnratio * (float) bestDist2 (a second best of 256 counts); the accepted
+ *             key claims its frame key.
+ *   rotation  with check_orientation: rot = kf angle - frame angle, + 360 if negative; bin = roundf(rot * (1.f / 30)), 30 -> 0 (bins
+ *             0..12 only, the reference's factor); ComputeThreeMaxima with its 0.1f * max1 rule; every match in another bin is
+ *             nulled and the count decremented.
+ *   angles    the projection searches' angle rule: key angles finite and in [0, 360].  The host form returns SIVO_ERANGE for any
+ *             other frame or keyframe key angle; the device form puts such a frame key in no node and does not search such a
+ *             keyframe key.
+ * Claims involve only frame keys of one node and each frame key is in one node, so the device runs one warp per (keyframe, common
+ * node), walking that node's keyframe keys in order with lanes over the candidates; the histogram is applied after the walk.
+ * Frame: semantic key j < *n_keep_device is extractor key keep_idx_device[j] (j when NULL) of kps_device / desc_device, node_device[j]
+ * its node (sivo_compute_bow_device's output).  Keyframe k: keyframes[k].kps / desc / node / count (device, sivo_orb_capacity(left)
+ * keys; the other members are not read) and kf_point_device[k][i] = the index of GetMapPointMatches()[i] in the caller's
+ * sivo_map_point array, -1 for NULL or isBad().  Outputs: match_device[k cap + j] (cap = sivo_orb_capacity(left)) = the point
+ * keyframe k's search gave frame key j, or -1 (so sivo_pose_gather_device takes match_device + k cap); n_matches_device[k] (int64)
+ * = the function's return.  Counts are clamped to the capacity; a negative count in the frame or in keyframe k writes only
+ * n_matches_device[k] = -1 for every affected k.  Runs on `stream` (NULL = the left extractor's stream) with no waits and no host
+ * synchronisation; its scratch is allocated and freed on `stream` (stream-ordered), never on the extractor.  SIVO_EINVAL for NULL
+ * handles, inputs or outputs, n_kf < 0, or nnratio not finite; SIVO_ERANGE for a capacity above 16,384 keys. */
+int sivo_search_by_bow_device(const sivo_orb_t* left, const sivo_keypoint* kps_device, const uint8_t* desc_device,
+                              const int* keep_idx_device, const long long* n_keep_device, const int* node_device,
+                              const sivo_keyframe_keys* keyframes, const int* const* kf_point_device, int n_kf, float nnratio,
+                              int check_orientation, int* match_device, long long* n_matches_device, void* stream);
+/* Host form: n frame keys gathered per semantic key (mvKeysSemantic, mDescriptorsSemantic, node); keyframes[k]'s kps / desc / node
+ * and kf_point[k] host arrays of *keyframes[k].count keys (a negative count: n_matches[k] = -1); match (n_kf x n, row k at k n)
+ * and n_matches (n_kf).  It stages the inputs, runs the device form's kernels and synchronises.  SIVO_EINVAL as above and for
+ * n < 0; SIVO_ERANGE for an angle that breaks the angle rule and for n above 16,384. */
+int sivo_search_by_bow(const sivo_orb_t* left, const sivo_keypoint* kps, const uint8_t* desc, const int* node, int n,
+                       const sivo_keyframe_keys* keyframes, const int* const* kf_point, int n_kf, float nnratio, int check_orientation,
+                       int* match, long long* n_matches);
+
 /* Best / second-best match over per-query candidate lists -- the inner loop of ORBmatcher::SearchByProjection
  * (ORBmatcher.cc:79-113), its last-frame / keyframe variants (:1278-, :1420-), SearchForTriangulation (:631-) and
  * SearchBySim3 (next row 4).  Query i's candidates are cand_idx[cand_offsets[i] .. cand_offsets[i+1]) (indices into the

@@ -6,3 +6,4 @@ from .info import InfoCamera, info_select, info_select_device, make_camera  # no
 from .track import (MAP_POINT_DTYPE, TrackFrame, make_frame, map_points, search_last_frame, search_last_frame_device,  # noqa: F401
                     search_local_points, search_local_points_device)
 from .pose import PoseResult, pose_gather_device, pose_optimize, pose_optimize_device  # noqa: F401
+from .bow import Vocabulary, compute_bow, compute_bow_device, search_by_bow, search_by_bow_device  # noqa: F401

@@ -81,6 +81,14 @@ def lib() -> C.CDLL:
         _lib.sivo_create_map_points_device.argtypes = [vp, vp, vp, i32, vp, vp, vp, vp, vp, vp, vp]
         _lib.sivo_create_map_points.argtypes = [vp, vp, vp, i32, vp, vp, vp, vp, vp, vp]
         _lib.sivo_dbg_create_map_points.argtypes = [vp, vp, vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+        _lib.sivo_vocabulary_destroy.restype = None
+        _lib.sivo_vocabulary_load_text.argtypes = [C.c_char_p, i32, vp]
+        _lib.sivo_vocabulary_create.argtypes = [i32, i32, i32, i32, i32, vp, vp, vp, vp, i32, vp]
+        _lib.sivo_dbg_vocabulary_parse.argtypes = [C.c_char_p, vp, vp, vp, vp, vp, vp, i32]
+        _lib.sivo_compute_bow_device.argtypes = [vp, vp, vp, vp, vp, i32, vp, vp, vp, vp, vp, vp]
+        _lib.sivo_compute_bow.argtypes = [vp, vp, i32, i32, vp, vp, vp, vp, vp]
+        _lib.sivo_search_by_bow_device.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, i32, f32, i32, vp, vp, vp]
+        _lib.sivo_search_by_bow.argtypes = [vp, vp, vp, vp, i32, vp, vp, i32, f32, i32, vp, vp]
         _lib.sivo_dbg_conv_unpooled.argtypes = [i32, vp, vp, i32, i32, i32, i32, vp, vp, vp, vp, i32, i32, vp]
     return _lib
 

@@ -9,6 +9,7 @@
 
 #include "frame_ops.h"
 #include "segnet.h"
+#include "vocabulary.h"
 
 namespace sivo {
 namespace {
@@ -21,6 +22,7 @@ using namespace sivo;
 
 struct sivo_segnet { SegNet* impl; };
 struct sivo_orb { Orb* impl; };
+struct sivo_vocabulary { Vocabulary* impl; };
 
 extern "C" {
 
@@ -638,6 +640,105 @@ int sivo_dbg_create_map_points(const sivo_orb_t* left, const sivo_keyframe_keys*
     if (!left || !kf1 || !params || !match || !stage || !reduction) fail(SIVO_EINVAL, "create_map_points: null argument");
     create_map_points_host(*left->impl, *kf1, neighbours, n_neighbours, *params, match, stage, reduction, created_nb, created_idx, world,
                            created_list, n_created);
+  });
+}
+
+// ---------------------------------------------------------------------------------------- vocabulary and bag of words
+int sivo_vocabulary_load_text(const char* path, int device, sivo_vocabulary_t** out) {
+  return guarded([&] {
+    if (!path || !out) fail(SIVO_EINVAL, "vocabulary_load_text: null argument");
+    *out = nullptr;
+    VocTree t;
+    parse_vocabulary_text(path, t);
+    auto* v = new Vocabulary(device, t.k, t.L, t.scoring, t.weighting, t.parent.data(), t.is_leaf.data(), t.desc.data(), t.weight.data(),
+                             static_cast<int>(t.parent.size()));
+    *out = new sivo_vocabulary{v};
+  });
+}
+
+int sivo_vocabulary_create(int device, int k, int L, int scoring, int weighting, const int32_t* parent, const uint8_t* is_leaf,
+                           const uint8_t* desc, const double* weight, int n_nodes, sivo_vocabulary_t** out) {
+  return guarded([&] {
+    if (!out || (n_nodes > 0 && (!parent || !is_leaf || !desc || !weight))) fail(SIVO_EINVAL, "vocabulary_create: null argument");
+    *out = nullptr;
+    auto* v = new Vocabulary(device, k, L, scoring, weighting, parent, is_leaf, desc, weight, n_nodes);
+    *out = new sivo_vocabulary{v};
+  });
+}
+
+int sivo_vocabulary_info(const sivo_vocabulary_t* voc, int* k, int* L, int* scoring, int* weighting, int* n_nodes, int* n_words) {
+  return guarded([&] {
+    if (!voc) fail(SIVO_EINVAL, "null handle");
+    const Vocabulary& v = *voc->impl;
+    if (k) *k = v.k;
+    if (L) *L = v.L;
+    if (scoring) *scoring = v.scoring;
+    if (weighting) *weighting = v.weighting;
+    if (n_nodes) *n_nodes = v.n_nodes;
+    if (n_words) *n_words = v.n_words;
+  });
+}
+
+void sivo_vocabulary_destroy(sivo_vocabulary_t* voc) {
+  if (!voc) return;
+  cudaSetDevice(voc->impl->device);
+  delete voc->impl;
+  delete voc;
+}
+
+int sivo_dbg_vocabulary_parse(const char* path, int* header, int* n_nodes, int32_t* parent, uint8_t* is_leaf, uint8_t* desc,
+                              double* weight, int capacity) {
+  return guarded([&] {
+    if (!path || !header || !n_nodes) fail(SIVO_EINVAL, "vocabulary_parse: null argument");
+    VocTree t;
+    parse_vocabulary_text(path, t);
+    const int n = static_cast<int>(t.parent.size());
+    header[0] = t.k; header[1] = t.L; header[2] = t.scoring; header[3] = t.weighting;
+    *n_nodes = n;
+    if (capacity < n) fail(SIVO_ERANGE, "vocabulary_parse: %d nodes, room for %d", n, capacity);
+    if (parent) std::copy(t.parent.begin(), t.parent.end(), parent);
+    if (is_leaf) std::copy(t.is_leaf.begin(), t.is_leaf.end(), is_leaf);
+    if (desc) std::copy(t.desc.begin(), t.desc.end(), desc);
+    if (weight) std::copy(t.weight.begin(), t.weight.end(), weight);
+  });
+}
+
+int sivo_compute_bow_device(const sivo_vocabulary_t* voc, const sivo_orb_t* left, const uint8_t* desc_device, const int* keep_idx_device,
+                            const long long* n_keep_device, int levelsup, int* node_device, int* word_device, int* bow_word_device,
+                            double* bow_weight_device, long long* bow_len_device, void* stream) {
+  return guarded([&] {
+    if (!voc || !left || !desc_device || !n_keep_device) fail(SIVO_EINVAL, "compute_bow: null argument");
+    compute_bow_device(*voc->impl, *left->impl, desc_device, keep_idx_device, n_keep_device, levelsup, node_device, word_device,
+                       bow_word_device, bow_weight_device, bow_len_device, static_cast<cudaStream_t>(stream));
+  });
+}
+
+int sivo_compute_bow(const sivo_vocabulary_t* voc, const uint8_t* desc, int n, int levelsup, int* node, int* word, int* bow_word,
+                     double* bow_weight, int* bow_len) {
+  return guarded([&] {
+    if (!voc) fail(SIVO_EINVAL, "compute_bow: null handle");
+    compute_bow_host(*voc->impl, desc, n, levelsup, node, word, bow_word, bow_weight, bow_len);
+  });
+}
+
+int sivo_search_by_bow_device(const sivo_orb_t* left, const sivo_keypoint* kps_device, const uint8_t* desc_device,
+                              const int* keep_idx_device, const long long* n_keep_device, const int* node_device,
+                              const sivo_keyframe_keys* keyframes, const int* const* kf_point_device, int n_kf, float nnratio,
+                              int check_orientation, int* match_device, long long* n_matches_device, void* stream) {
+  return guarded([&] {
+    if (!left || !kps_device || !desc_device || !n_keep_device || !node_device || !match_device || !n_matches_device)
+      fail(SIVO_EINVAL, "search_by_bow: null argument");
+    search_by_bow_device(*left->impl, kps_device, desc_device, keep_idx_device, n_keep_device, node_device, keyframes, kf_point_device, n_kf,
+                         nnratio, check_orientation, match_device, n_matches_device, static_cast<cudaStream_t>(stream));
+  });
+}
+
+int sivo_search_by_bow(const sivo_orb_t* left, const sivo_keypoint* kps, const uint8_t* desc, const int* node, int n,
+                       const sivo_keyframe_keys* keyframes, const int* const* kf_point, int n_kf, float nnratio, int check_orientation,
+                       int* match, long long* n_matches) {
+  return guarded([&] {
+    if (!left) fail(SIVO_EINVAL, "search_by_bow: null handle");
+    search_by_bow_host(*left->impl, kps, desc, node, n, keyframes, kf_point, n_kf, nnratio, check_orientation, match, n_matches);
   });
 }
 

@@ -31,4 +31,19 @@ __device__ __forceinline__ void best2_fold_warp(Best2& b, int d, int idx, int lv
   }
 }
 
+// ORBmatcher::ComputeThreeMaxima (ORBmatcher.cc:1545-1577) over the rotation histogram's bin sizes, shared by the last-frame search
+// (track.cu) and SearchByBoW (bow.cu): keep[0..2] = ind1, ind2, ind3 (-1: none).
+__device__ __forceinline__ void three_maxima(const int* counts, int n, int* keep) {
+  int max1 = 0, max2 = 0, max3 = 0, ind1 = -1, ind2 = -1, ind3 = -1;
+  for (int i = 0; i < n; ++i) {
+    const int s = counts[i];
+    if (s > max1) { max3 = max2; max2 = max1; max1 = s; ind3 = ind2; ind2 = ind1; ind1 = i; }
+    else if (s > max2) { max3 = max2; max2 = s; ind3 = ind2; ind2 = i; }
+    else if (s > max3) { max3 = s; ind3 = i; }
+  }
+  if (max2 < 0.1f * static_cast<float>(max1)) { ind2 = -1; ind3 = -1; }
+  else if (max3 < 0.1f * static_cast<float>(max1)) ind3 = -1;
+  keep[0] = ind1; keep[1] = ind2; keep[2] = ind3;
+}
+
 }  // namespace sivo

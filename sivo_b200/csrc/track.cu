@@ -390,18 +390,7 @@ __global__ void __launch_bounds__(32) k_track_ordered(const TrackParams p, const
   if (p.last_frame) {
     __syncwarp();
     __shared__ int keep_bin[3];
-    if (lane == 0) {  // ComputeThreeMaxima (ORBmatcher.cc:1545-1577)
-      int max1 = 0, max2 = 0, max3 = 0, ind1 = -1, ind2 = -1, ind3 = -1;
-      for (int i = 0; i < kHisto; ++i) {
-        const int s = hist_count[i];
-        if (s > max1) { max3 = max2; max2 = max1; max1 = s; ind3 = ind2; ind2 = ind1; ind1 = i; }
-        else if (s > max2) { max3 = max2; max2 = s; ind3 = ind2; ind2 = i; }
-        else if (s > max3) { max3 = s; ind3 = i; }
-      }
-      if (max2 < 0.1f * static_cast<float>(max1)) { ind2 = -1; ind3 = -1; }
-      else if (max3 < 0.1f * static_cast<float>(max1)) ind3 = -1;
-      keep_bin[0] = ind1; keep_bin[1] = ind2; keep_bin[2] = ind3;
-    }
+    if (lane == 0) three_maxima(hist_count, kHisto, keep_bin);
     __syncwarp();
     int culled = 0;
     for (int e = lane; e < n_hist; e += 32) {
