@@ -147,7 +147,8 @@ int sivo_segnet_blob(sivo_segnet_t* h, const char* name, float* out, size_t cap,
  * do later (Tracking.cc:487,538; LocalMapping.cc:483-485), evaluated on the device-resident maps of the last
  * sivo_segnet_run / _run_device -- so a caller that only needs per-keypoint values can pass NULL maps to sivo_segnet_run
  * and skip the 6.1 MB read-back.  For keypoint i: (row, col) = ((int) y, (int) x); kp_class/kp_conf/kp_entropy[i] = the map
- * values there (class 255, 0, 0 and never kept if outside the maps -- the reference would read out of bounds).
+ * values there (class 255, 0, 0 and never kept if outside the maps, or if x or y is not finite -- the reference would read out of
+ * bounds or convert a NaN to int; the test is made in float, before the conversion).
  * keep_idx[0..*n_keep) = indices with class <= max_static_class (Classes::TERRAIN = 8 in the reference), ascending, i.e. the
  * order mvKeysSemantic / mDescriptorsSemantic are built in.  Any output pointer may be NULL. */
 int sivo_segnet_semantic_keys(sivo_segnet_t* h, const sivo_keypoint* kps, int n, int max_static_class, uint8_t* kp_class,
@@ -235,16 +236,29 @@ int sivo_dbg_orb_distribute_device(int device, const int* xs, const int* ys, con
 /* ---- stereo Hamming stage (next-row 1) -------------------------------------------------------- */
 /* For each left keypoint: best right candidate in its row band (rows vL +- 2*scale[octave]), octave
  * within +-1, uR in [uL - max_d, uL - min_d], minimal DescriptorDistance; best_idx = -1 if none.
- * Mirrors Frame.cc:452-533 up to (not including) the SAD refinement. */
+ * Mirrors Frame.cc:452-533 up to (not including) the SAD refinement.  A left key with a non-finite x or y, or with (int) y outside
+ * [0, rows), has no candidate; a right key with a non-finite x or y is never a candidate (sivo_stereo_match's rule).
+ * SIVO_EINVAL for n_right >= 2^20 (the search packs the right index into 20 bits). */
 int sivo_stereo_hamming(int device, const sivo_keypoint* left, const uint8_t* desc_left, int n_left,
                         const sivo_keypoint* right, const uint8_t* desc_right, int n_right,
                         const float* scale_factors, int nlevels, int rows, float min_d, float max_d,
                         int* best_idx, int* best_dist);
 
+/* Test hook: the median-based outlier cut of sivo_stereo_match alone.  sad[i] < 0 marks key i unmatched; with m matched keys the
+ * median is the SAD of rank m / 2 in ascending order, and every matched key with (float) sad >= 1.5f * 1.4f * median gets
+ * u[i] = z[i] = -1 (u and z are read and written in place, n entries each). */
+int sivo_dbg_stereo_median_cut(int device, const int* sad, int n, float* u, float* z);
+
 /* The whole of Frame::ComputeStereoMatches (Frame.cc:444-629): Hamming search, 11x11 SAD slide (+-5 px) on the keypoint's
  * pyramid level, parabola sub-pixel fit, disparity gate [0, mbf/mb), median-based outlier cut.  Uses the device-resident
  * pyramids of the last sivo_orb_run of `left` / `right` (so mvImagePyramid need not travel to the host for it).
- * u_right / depth: n_left floats each = mvRight / mvDepth (-1 where unmatched). */
+ * u_right / depth: n_left floats each = mvRight / mvDepth (-1 where unmatched).
+ * Rule where the reference throws or is undefined (it changes nothing for keys an extractor produces): a left key stays unmatched,
+ * and no SAD of it enters the median, if its x or y is not finite, if (int) y is outside [0, rows), if its 11 x 11 window at its
+ * octave leaves that level's image (rows sv_l +- 5, columns su_l +- 5), or if the right slide does (rows sv_l +- 5, columns
+ * su_r0 - 10 .. su_r0 + 10); a right key with a non-finite x or y is never a candidate.  Every test is made in float, before any
+ * conversion to int; the reference's own endu >= cols test stays as written.  SIVO_EINVAL, before anything is launched or
+ * written, if the two extractors' last runs have different level tables (image size or scale factor), and for n_right >= 2^20. */
 int sivo_stereo_match(const sivo_orb_t* left, const sivo_orb_t* right, const sivo_keypoint* kp_left, const uint8_t* desc_left,
                       int n_left, const sivo_keypoint* kp_right, const uint8_t* desc_right, int n_right, float mb, float mbf,
                       float* u_right, float* depth);
@@ -260,7 +274,8 @@ int sivo_stereo_match(const sivo_orb_t* left, const sivo_orb_t* right, const siv
  * call reads both pyramids and writes the left extractor's SAD scratch, so the next sivo_orb_enqueue_device on either extractor
  * must be ordered after it (sivo_orb_wait_for_stream(extractor, stream)), and calls that share a left extractor must be ordered
  * among themselves.  No host synchronisation.  SIVO_EINVAL for NULL handles or buffers (keep_idx_device may be NULL), extractors
- * that have not run, extractors on different devices or with different nlevels, and mb / mbf <= 0. */
+ * that have not run, extractors on different devices, with different nlevels or different level tables, mb / mbf <= 0, and a right
+ * extractor whose sivo_orb_capacity is >= 2^20; nothing is enqueued then.  Keys follow sivo_stereo_match's rule. */
 int sivo_stereo_match_device(sivo_orb_t* left, sivo_orb_t* right, const sivo_keypoint* kp_left_device, const uint8_t* desc_left_device,
                              const int* keep_idx_device, const long long* n_left_device, const sivo_keypoint* kp_right_device,
                              const uint8_t* desc_right_device, const long long* n_right_device, float mb, float mbf,

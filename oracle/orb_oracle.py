@@ -523,104 +523,210 @@ def descriptor_distance(a: np.ndarray, b: np.ndarray) -> int:
     return int(np.unpackbits(np.bitwise_xor(a, b)).sum())
 
 
-def compute_stereo_matches(kl, dl, kr, dr, pyr_l, pyr_r, scale, inv_scale, mb, mbf):
+_POP8 = np.array([bin(v).count("1") for v in range(256)], np.int64)
+
+# where a left key's search ended (compute_stereo_matches' trace): the reference's own exits, in the order it takes them, and
+# the rule's (RULE_STAGES), which the reference cannot reach without throwing or indexing out of range
+STAGES = ("nonfinite", "no_row", "no_candidate", "hamming", "slide_ref", "slide", "left_window", "binc_edge", "delta",
+          "disparity", "matched", "cut")
+RULE_STAGES = ("nonfinite", "no_row", "slide", "left_window")
+# the wants of oracle/stereo_scene.py that name a group of stages
+STAGE_GROUPS = {"no_match": ("no_candidate", "hamming"),
+                "past_hamming": STAGES[STAGES.index("slide_ref"):],
+                "past_slide": STAGES[STAGES.index("binc_edge"):]}
+
+
+def round_half_away(v) -> np.float32:
+    """std::round / roundf on a float: half away from zero.  Exact through float64 (every float32 + 0.5 is exact there)."""
+    v = float(np.float32(v))
+    return np.float32(math.copysign(math.floor(abs(v) + 0.5), v))
+
+
+def window_sad(img_l, img_r, cy, cxl, cxr) -> int:
+    """L1 distance of the two 11 x 11 windows centred at (cy, cxl) / (cy, cxr), each minus its centre pixel (Frame.cc:546-576)."""
+    a = img_l[cy - 5:cy + 6, cxl - 5:cxl + 6].astype(np.int64)
+    b = img_r[cy - 5:cy + 6, cxr - 5:cxr + 6].astype(np.int64)
+    return int(np.abs((a - a[5, 5]) - (b - b[5, 5])).sum())
+
+
+def median_cut(sad):
+    """The median-based outlier cut (Frame.cc:617-628) over per-key SAD distances (< 0 = unmatched): the median is the SAD of
+    rank m / 2 of the m matched keys in ascending order, th = 1.5f * 1.4f * median in float, and every matched key with
+    (float) sad >= th is cut.  Returns the bool mask of cut keys."""
+    sad = np.asarray(sad, np.int64)
+    matched = sad >= 0
+    if not matched.any():
+        return np.zeros(len(sad), bool)
+    median = np.float32(np.sort(sad[matched])[int(matched.sum()) // 2])
+    th = np.float32(np.float32(np.float32(1.5) * np.float32(1.4)) * median)
+    return matched & (sad.astype(np.float32) >= th)
+
+
+class _RightSearch:
+    """The row-band Hamming search of Frame.cc:486-533 over right keys (x, y, octave) and descriptors dr."""
+
+    def __init__(self, kr, dr, scale):
+        f32 = np.float32
+        self.x = np.asarray(kr["x"], f32)
+        self.o = np.asarray(kr["octave"], np.int64)
+        y = np.asarray(kr["y"], f32)
+        nlv = len(scale)
+        self.ok = np.isfinite(self.x) & np.isfinite(y) & (self.o >= 0) & (self.o < nlv)
+        band = (f32(2.0) * np.asarray(scale, f32)[np.clip(self.o, 0, nlv - 1)]).astype(f32)
+        with np.errstate(invalid="ignore", over="ignore"):
+            self.lo = np.floor((y - band).astype(f32))
+            self.hi = np.ceil((y + band).astype(f32))
+        self.dr = np.asarray(dr, np.uint8).reshape(-1, 32)
+
+    def best(self, ul, vl, lv, dl, min_d, max_d):
+        """(best distance, its right index) of a left key with a row, i.e. finite x and y in (-1, rows): the smallest distance
+        below TH_HIGH = 100 and the lowest index among equals, or (100, 0) if no candidate is below 100; (100, -1) if the row
+        holds no right key or maxU < 0 (the reference's two early exits)."""
+        f32 = np.float32
+        row = f32(int(vl))
+        min_u, max_u = f32(ul - max_d), f32(ul - min_d)
+        with np.errstate(invalid="ignore"):
+            cand = self.ok & (row >= self.lo) & (row <= self.hi)
+        if not cand.any() or max_u < 0:
+            return 100, -1
+        with np.errstate(invalid="ignore"):
+            cand &= (self.o >= lv - 1) & (self.o <= lv + 1) & (self.x >= min_u) & (self.x <= max_u)
+        idx = np.nonzero(cand)[0]
+        if len(idx):
+            d = _POP8[np.bitwise_xor(self.dr[idx], np.asarray(dl, np.uint8))].sum(axis=1)
+            k = int(np.argmin(d))  # first of the smallest: the reference's strict '<' walking iR upwards
+            if d[k] < 100:
+                return int(d[k]), int(idx[k])
+        return 100, 0
+
+
+def stereo_hamming(kl, dl, kr, dr, scale, rows, min_d, max_d):
+    """sivo_stereo_hamming: per left key the best right index (-1 if none below 100) and its distance (100 if none), with the
+    rule of compute_stereo_matches for non-finite keys and rows outside [0, rows)."""
+    f32 = np.float32
+    search = _RightSearch(kr, dr, scale)
+    idx = np.full(len(kl), -1, np.int32)
+    dist = np.full(len(kl), 100, np.int32)
+    for il in range(len(kl)):
+        ul, vl = f32(kl["x"][il]), f32(kl["y"][il])
+        if not (np.isfinite(ul) and vl > -1 and vl < rows):
+            continue
+        d, i = search.best(ul, vl, int(kl["octave"][il]), dl[il], f32(min_d), f32(max_d))
+        dist[il] = d
+        idx[il] = i if d < 100 else -1
+    return idx, dist
+
+
+def compute_stereo_matches(kl, dl, kr, dr, pyr_l, pyr_r, scale, inv_scale, mb, mbf, trace=None):
     """Frame::ComputeStereoMatches (src/orbslam/Frame.cc:444-629) restated: row table, Hamming search with the octave
     and disparity gates, 11x11 SAD slide on the keypoint's pyramid level, parabola fit, median-based outlier cut.
     kl / kr: structured keypoint arrays (x, y, octave), dl / dr: [N, 32] u8, pyr_*: bordered level buffers.
-    Returns (mvRight, mvDepth) float32 arrays."""
+    Returns (mvRight, mvDepth) float32 arrays.
+
+    Rule where the reference throws or is undefined (the product's, header comment of sivo_stereo_match): a left key stays
+    unmatched if its x or y is not finite, if int(y) is outside [0, rows), if its 11 x 11 window at its octave leaves that level's
+    image, or if the right slide (columns su_r0 - 10 .. su_r0 + 10, rows sv_l +- 5) does; a right key with a non-finite x or y is
+    never a candidate.  Every test is made in float before any conversion to int.  A right key's row band is tested per left key
+    (row in [floor(y - 2 s), ceil(y + 2 s)]), which is the reference's row table without its out-of-range rows.
+
+    trace: a list that receives, per left key, a dict with the stage where its search ended (STAGES), the SAD vector, binc,
+    delta and disparity as far as they were computed."""
     f32 = np.float32
     n_l = len(kl)
     u_right = np.full(n_l, -1.0, f32)
     depth = np.full(n_l, -1.0, f32)
+    sad = np.full(n_l, -1, np.int64)
     rows = pyr_l[0].shape[0] - 2 * EDGE_THRESHOLD
-    table = [[] for _ in range(rows)]
-    for i in range(len(kr)):
-        r = f32(2.0) * scale[kr["octave"][i]]
-        lo, hi = int(np.floor(f32(kr["y"][i] - r))), int(np.ceil(f32(kr["y"][i] + r)))
-        for y in range(lo, hi + 1):
-            table[y].append(i)
+    search = _RightSearch(kr, dr, scale)
     th_orb = (100 + 50) // 2
     min_d, max_d = f32(0), f32(f32(mbf) / f32(mb))
-    cand = []
-
-    def c_round(v):
-        return f32(np.floor(v + f32(0.5))) if v >= 0 else f32(-np.floor(-v + f32(0.5)))
+    levels = [p[EDGE_THRESHOLD:-EDGE_THRESHOLD, EDGE_THRESHOLD:-EDGE_THRESHOLD] for p in pyr_l]
+    levels_r = [p[EDGE_THRESHOLD:-EDGE_THRESHOLD, EDGE_THRESHOLD:-EDGE_THRESHOLD] for p in pyr_r]
     for il in range(n_l):
+        t = {"stage": None, "sad": None, "binc": None, "delta": None, "disp": None}
+        if trace is not None:
+            trace.append(t)
         ul, vl, lv = f32(kl["x"][il]), f32(kl["y"][il]), int(kl["octave"][il])
-        cands = table[int(vl)]
-        if not cands:
+        if not (np.isfinite(ul) and np.isfinite(vl)):
+            t["stage"] = "nonfinite"
             continue
-        min_u, max_u = f32(ul - max_d), f32(ul - min_d)
-        if max_u < 0:
+        if not (vl > -1 and vl < rows):
+            t["stage"] = "no_row"
             continue
-        best, best_i = 100, 0
-        for j in cands:
-            if kr["octave"][j] < lv - 1 or kr["octave"][j] > lv + 1:
-                continue
-            if min_u <= kr["x"][j] <= max_u:
-                d = descriptor_distance(dl[il], dr[j])
-                if d < best:
-                    best, best_i = d, j
+        best, best_i = search.best(ul, vl, lv, dl[il], min_d, max_d)
+        t["best"], t["best_i"] = best, best_i
+        if best_i < 0:
+            t["stage"] = "no_candidate"
+            continue
         if best >= th_orb:
+            t["stage"] = "hamming"
             continue
         sf = inv_scale[lv]
-        su_l, sv_l, su_r0 = c_round(f32(ul * sf)), c_round(f32(vl * sf)), c_round(f32(kr["x"][best_i] * sf))
-        img_l = pyr_l[lv][EDGE_THRESHOLD:-EDGE_THRESHOLD, EDGE_THRESHOLD:-EDGE_THRESHOLD].astype(np.int64)
-        img_r = pyr_r[lv][EDGE_THRESHOLD:-EDGE_THRESHOLD, EDGE_THRESHOLD:-EDGE_THRESHOLD].astype(np.int64)
-        w = 5
-        cy, cxl, cxr = int(sv_l), int(su_l), int(su_r0)
+        su_l, sv_l, su_r0 = (round_half_away(f32(v * sf)) for v in (ul, vl, f32(kr["x"][best_i])))
+        img_l, img_r = levels[lv], levels_r[lv]
+        (h, w), hr = img_l.shape, img_r.shape[0]
         if su_r0 + 5 - 5 < 0 or su_r0 + 5 + 5 + 1 >= img_r.shape[1]:
+            t["stage"] = "slide_ref"
             continue
-        il_win = img_l[cy - w:cy + w + 1, cxl - w:cxl + w + 1]
-        il_win = il_win - il_win[w, w]
-        dists = []
-        for inc in range(-5, 6):
-            ir_win = img_r[cy - w:cy + w + 1, cxr + inc - w:cxr + inc + w + 1]
-            ir_win = ir_win - ir_win[w, w]
-            dists.append(int(np.abs(il_win - ir_win).sum()))
-        bd, binc = 2 ** 31 - 1, 0
-        for k, d in enumerate(dists):
-            if d < bd:
-                bd, binc = d, k - 5
+        if not (su_r0 >= 10 and 5 <= sv_l <= hr - 6):
+            t["stage"] = "slide"
+            continue
+        if not (5 <= su_l <= w - 6 and 5 <= sv_l <= h - 6):
+            t["stage"] = "left_window"
+            continue
+        cy, cxl, cxr = int(sv_l), int(su_l), int(su_r0)
+        dists = [window_sad(img_l, img_r, cy, cxl, cxr + inc) for inc in range(-5, 6)]
+        binc = int(np.argmin(dists)) - 5  # first minimum
+        t["sad"], t["binc"] = dists, binc
         if binc in (-5, 5):
+            t["stage"] = "binc_edge"
             continue
         d1, d2, d3 = f32(dists[binc + 4]), f32(dists[binc + 5]), f32(dists[binc + 6])
         with np.errstate(divide="ignore", invalid="ignore"):
             delta = f32(f32(d1 - d3) / f32(f32(2.0) * f32(f32(d1 + d3) - f32(f32(2.0) * d2))))
+        t["delta"] = delta
         if delta < -1 or delta > 1 or np.isnan(delta):
+            t["stage"] = "delta"
             continue
         best_u = f32(scale[lv] * f32(f32(su_r0 + f32(binc)) + delta))
         disp = f32(ul - best_u)
-        if min_d <= disp < max_d:
-            if disp <= 0:
-                disp = f32(0.01)
-                best_u = f32(float(ul) - 0.01)
-            depth[il] = f32(f32(mbf) / disp)
-            u_right[il] = best_u
-            cand.append((bd, il))
-    if cand:
-        cand.sort()
-        median = f32(cand[len(cand) // 2][0])
-        th = f32(1.5) * f32(1.4) * median
-        for d, il in reversed(cand):
-            if f32(d) < th:
-                break
-            u_right[il] = -1
-            depth[il] = -1
+        t["disp"] = disp
+        if not (min_d <= disp < max_d):
+            t["stage"] = "disparity"
+            continue
+        if disp <= 0:
+            disp = f32(0.01)
+            best_u = f32(float(ul) - 0.01)
+        depth[il] = f32(f32(mbf) / disp)
+        u_right[il] = best_u
+        sad[il] = dists[binc + 5]
+        t["stage"] = "matched"
+    cut = median_cut(sad)
+    u_right[cut] = -1
+    depth[cut] = -1
+    if trace is not None:
+        for il in np.nonzero(cut)[0]:
+            trace[il]["stage"] = "cut"
     return u_right, depth
 
 
 def select_semantic_keys(kps_xy, classes, confidence=None, entropy=None, max_static_class=8):
     """Frame::SelectSemanticKeys (Frame.cc:177-203): col = int(pt.x), row = int(pt.y) (C++ truncation), keep the keypoint
     iff mClasses(row, col) <= Classes::TERRAIN (= 8, bayesian_segnet.hpp:67-83), in keypoint order.  Also returns the per-keypoint
-    reads of the maps (what Tracking.cc:487,538 / LocalMapping.cc:483-485 look up later).  kps_xy: [n, 2] float32 (x, y)."""
-    kps_xy = np.asarray(kps_xy, np.float32)
-    col = np.trunc(kps_xy[:, 0]).astype(np.int64)
-    row = np.trunc(kps_xy[:, 1]).astype(np.int64)
-    cls = classes[row, col]
-    keep = np.nonzero(cls <= max_static_class)[0].astype(np.int32)
-    conf = confidence[row, col] if confidence is not None else None
-    ent = entropy[row, col] if entropy is not None else None
+    reads of the maps (what Tracking.cc:487,538 / LocalMapping.cc:483-485 look up later).  kps_xy: [n, 2] float32 (x, y).
+    Rule where the reference reads out of bounds or converts a NaN to int: a key whose x or y is not finite, or whose (col, row)
+    is outside the maps, gets class 255, confidence 0 and entropy 0 and is never kept (tested in float, before the conversion)."""
+    kps_xy = np.asarray(kps_xy, np.float32).reshape(-1, 2)
+    H, W = classes.shape
+    x, y = kps_xy[:, 0], kps_xy[:, 1]
+    with np.errstate(invalid="ignore"):
+        ok = (x > -1) & (x < W) & (y > -1) & (y < H)
+    col = np.where(ok, np.trunc(np.where(ok, x, 0)), 0).astype(np.int64)
+    row = np.where(ok, np.trunc(np.where(ok, y, 0)), 0).astype(np.int64)
+    cls = np.where(ok, classes[row, col], 255).astype(classes.dtype)
+    keep = np.nonzero((cls != 255) & (cls <= max_static_class))[0].astype(np.int32)
+    conf = np.where(ok, confidence[row, col], 0.0) if confidence is not None else None
+    ent = np.where(ok, entropy[row, col], 0.0) if entropy is not None else None
     return cls, conf, ent, keep
 
 

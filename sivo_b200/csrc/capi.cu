@@ -469,6 +469,13 @@ int sivo_stereo_match_device(sivo_orb_t* left, sivo_orb_t* right, const sivo_key
   });
 }
 
+int sivo_dbg_stereo_median_cut(int device, const int* sad, int n, float* u, float* z) {
+  return guarded([&] {
+    if (n > 0 && (!sad || !u || !z)) fail(SIVO_EINVAL, "null argument");
+    stereo_median_cut(device, sad, n, u, z);
+  });
+}
+
 // ---------------------------------------------------------------------------------------- information selection
 int sivo_info_select(const sivo_orb_t* left, const sivo_keypoint* kps, const float* depth, const double* entropy, int n,
                      const sivo_info_camera* cam, double threshold, float* world, double* reduction, int* selected, int* n_selected) {

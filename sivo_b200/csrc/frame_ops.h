@@ -18,6 +18,7 @@ void stereo_match(const Orb& left, const Orb& right, const sivo_keypoint* kl, co
 void stereo_match_device(Orb& left, Orb& right, const sivo_keypoint* kl, const uint8_t* dl, const int* keep_idx, const long long* n_left,
                          const sivo_keypoint* kr, const uint8_t* dr, const long long* n_right, float mb, float mbf, float* u_right,
                          float* depth, cudaStream_t s);
+void stereo_median_cut(int device, const int* sad, int n, float* u, float* z);
 
 // ---- info.cu
 void info_select(const Orb& left, const sivo_keypoint* kps, const float* depth, const double* entropy, int n, const sivo_info_camera& cam,

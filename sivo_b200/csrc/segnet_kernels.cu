@@ -733,9 +733,10 @@ __global__ void __launch_bounds__(kSemThreads) k_semantic_keys(const sivo_keypoi
     const int i = c0 + tid;
     bool keep = false;
     if (i < n) {
-      const int col = static_cast<int>(kps[i].x), row = static_cast<int>(kps[i].y);  // static_cast<int>(pt.x / pt.y): truncation
-      const bool ok = col >= 0 && col < W && row >= 0 && row < H;
-      const size_t o = ok ? static_cast<size_t>(row) * W + col : 0;
+      // (int) x in [0, W) <=> x in (-1, W), tested in float before the conversion so that NaN and +-inf are outside the maps
+      const float x = kps[i].x, y = kps[i].y;
+      const bool ok = x > -1.f && x < static_cast<float>(W) && y > -1.f && y < static_cast<float>(H);
+      const size_t o = ok ? static_cast<size_t>(static_cast<int>(y)) * W + static_cast<int>(x) : 0;  // truncation, as int(pt.x / pt.y)
       const uint8_t c = ok ? classes[o] : static_cast<uint8_t>(255);
       if (out_class) out_class[i] = c;
       if (out_conf) out_conf[i] = ok ? conf[o] : 0.0;

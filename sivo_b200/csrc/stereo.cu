@@ -13,21 +13,23 @@ constexpr int kThHigh = 100;  // ORBmatcher::TH_HIGH (ORBmatcher.cc:37)
 
 // The row-band Hamming search of left keypoint L (descriptor a) over right keypoints [0, nr), warp-wide: every lane calls it with
 // the same L and gets the warp's packed best (dist << 20 | idx), or (kThHigh << 20 | 0xFFFFF) if no candidate is below kThHigh.
-// Right keypoints whose octave is outside [0, nlevels) are skipped.
+// Right keypoints whose octave is outside [0, nlevels) are skipped.  Where the reference is undefined (a NaN or out-of-range row
+// index into vRowIndices) the rule is: a left key with a non-finite x or y, or with (int) y outside [0, rows), has no candidate,
+// and a right key with a non-finite x or y is no candidate.  Every test is made in float, before any conversion to int.
 __device__ __forceinline__ unsigned stereo_best_right(const sivo_keypoint L, const ulonglong4 a, const sivo_keypoint* __restrict__ kr,
                                                       const uint8_t* __restrict__ dr, int nr, const float* __restrict__ scale, int nlevels,
                                                       int rows, float min_d, float max_d, int lane) {
-  const int row = static_cast<int>(L.y);
   const float min_u = __fsub_rn(L.x, max_d), max_u = __fsub_rn(L.x, min_d);
   unsigned best = (static_cast<unsigned>(kThHigh) << 20) | 0xFFFFFu;  // dist:12 | idx:20
-  if (max_u >= 0.f && row >= 0 && row < rows) {
+  // (int) y in [0, rows) <=> y in (-1, rows) for finite y; NaN fails both compares
+  if (isfinite(L.x) && L.y > -1.f && L.y < static_cast<float>(rows) && max_u >= 0.f) {
+    const float row = static_cast<float>(static_cast<int>(L.y));
     for (int i = lane; i < nr; i += 32) {
       const sivo_keypoint R = kr[i];
       if (static_cast<unsigned>(R.octave) >= static_cast<unsigned>(nlevels)) continue;
+      if (!isfinite(R.x) || !isfinite(R.y)) continue;
       const float band = __fmul_rn(2.0f, scale[R.octave]);
-      const int maxr = static_cast<int>(ceilf(__fadd_rn(R.y, band)));
-      const int minr = static_cast<int>(floorf(__fsub_rn(R.y, band)));
-      if (row < minr || row > maxr) continue;
+      if (row < floorf(__fsub_rn(R.y, band)) || row > ceilf(__fadd_rn(R.y, band))) continue;
       if (R.octave < L.octave - 1 || R.octave > L.octave + 1) continue;
       if (!(R.x >= min_u && R.x <= max_u)) continue;
       const ulonglong4 b = *reinterpret_cast<const ulonglong4*>(dr + static_cast<size_t>(i) * 32);
@@ -59,7 +61,11 @@ __global__ void k_stereo_hamming(const sivo_keypoint* __restrict__ kl, const uin
 // above, then the 11x11 SAD slide over +-5 px on the keypoint's pyramid level (windows are centred-intensity
 // differences of u8 pixels, so every L1 distance is an exact integer), parabola sub-pixel fit, disparity gate.
 // The median-based outlier cut (:617-628) needs all matches: k_stereo_median_cut does it over the SAD distances.
-__device__ __forceinline__ float c_roundf(float v) { return v >= 0.f ? floorf(__fadd_rn(v, 0.5f)) : -floorf(__fadd_rn(-v, 0.5f)); }
+// `round` of the reference is std::round on a float: roundf, half away from zero.
+// Where the reference's rowRange / colRange would throw, the rule is: a key stays unmatched (no SAD enters the median) if its
+// 11 x 11 window at its octave (rows sv_l +- 5, columns su_l +- 5) or the right slide (rows sv_l +- 5, columns su_r0 - 10 ..
+// su_r0 + 10) leaves that level's image.  The reference's own test (iniu < 0 || endu >= cols) stays as written, one column
+// stricter on the right than the slide needs.  The tests are made on the rounded floats, before any conversion to int.
 
 // The per-keypoint body; every lane of the warp calls it with the same left keypoint L and descriptor row.
 __device__ __forceinline__ void stereo_match_key(const sivo_keypoint L, const uint8_t* __restrict__ dl_key, const sivo_keypoint* __restrict__ kr,
@@ -78,12 +84,13 @@ __device__ __forceinline__ void stereo_match_key(const sivo_keypoint L, const ui
     const int ir = best & 0xFFFFFu;
     const int oct = L.octave;
     const float sf = inv_scale[oct];
-    const float su_l = c_roundf(__fmul_rn(L.x, sf)), sv_l = c_roundf(__fmul_rn(L.y, sf)), su_r0 = c_roundf(__fmul_rn(kr[ir].x, sf));
+    const float su_l = roundf(__fmul_rn(L.x, sf)), sv_l = roundf(__fmul_rn(L.y, sf)), su_r0 = roundf(__fmul_rn(kr[ir].x, sf));
     const OrbLevel ll = lt_l.lv[oct], lr = lt_r.lv[oct];
     const float iniu = su_r0 + 5.f - 5.f, endu = su_r0 + 5.f + 5.f + 1.f;
-    const int cx_l = static_cast<int>(su_l), cy = static_cast<int>(sv_l), cx_r = static_cast<int>(su_r0);
-    if (!(iniu < 0.f || endu >= static_cast<float>(lr.w)) && cx_l - 5 >= -kEdge && cx_l + 5 < ll.w + kEdge && cy - 5 >= -kEdge &&
-        cy + 5 < ll.h + kEdge) {
+    const bool slide_in = su_r0 >= 10.f && sv_l >= 5.f && sv_l <= static_cast<float>(lr.h - 6);
+    const bool left_in = su_l >= 5.f && su_l <= static_cast<float>(ll.w - 6) && sv_l >= 5.f && sv_l <= static_cast<float>(ll.h - 6);
+    if (!(iniu < 0.f || endu >= static_cast<float>(lr.w)) && slide_in && left_in) {
+      const int cx_l = static_cast<int>(su_l), cy = static_cast<int>(sv_l), cx_r = static_cast<int>(su_r0);
       const uint8_t* pl = pyr_l + ll.img_off + static_cast<size_t>(cy + kEdge) * ll.pitch + cx_l + kEdge;
       const uint8_t* pr = pyr_r + lr.img_off + static_cast<size_t>(cy + kEdge) * lr.pitch + cx_r + kEdge;
       const int lc = pl[0];
@@ -248,6 +255,17 @@ void launch_stereo(const Orb& left, const Orb& right, const sivo_keypoint* kl, c
   SIVO_CUDA(cudaGetLastError());
 }
 
+// The SAD windows of both images are read at the left key's octave with one set of rounded coordinates: the two extractors' last
+// runs must have the same level tables (same image size and scale factor), or the right reads would leave its pyramid.
+void check_extractors(const Orb& left, const Orb& right) {
+  if (!left.has_run() || !right.has_run()) fail(SIVO_EINVAL, "stereo: run both extractors first");
+  if (left.device() != right.device() || left.nlevels() != right.nlevels()) fail(SIVO_EINVAL, "stereo: extractors differ");
+  for (int l = 0; l < left.nlevels(); ++l)
+    if (left.levels().lv[l].w != right.levels().lv[l].w || left.levels().lv[l].h != right.levels().lv[l].h)
+      fail(SIVO_EINVAL, "stereo: level %d is %d x %d on the left and %d x %d on the right", l, left.levels().lv[l].w,
+           left.levels().lv[l].h, right.levels().lv[l].w, right.levels().lv[l].h);
+}
+
 void check_octaves(const sivo_keypoint* left, int nl, const sivo_keypoint* right, int nr, int nlevels) {
   for (int i = 0; i < nl; ++i) if (left[i].octave < 0 || left[i].octave >= nlevels) fail(SIVO_EINVAL, "stereo: left octave out of range");
   for (int i = 0; i < nr; ++i) if (right[i].octave < 0 || right[i].octave >= nlevels) fail(SIVO_EINVAL, "stereo: right octave out of range");
@@ -346,8 +364,7 @@ namespace sivo {
 // ComputeStereoMatches end to end; `left` / `right` are the extractors whose last runs produced the keypoints.
 void stereo_match(const Orb& left, const Orb& right, const sivo_keypoint* kl, const uint8_t* dl, int nl, const sivo_keypoint* kr,
                   const uint8_t* dr, int nr, float mb, float mbf, float* u_right, float* depth) {
-  if (!left.has_run() || !right.has_run()) fail(SIVO_EINVAL, "stereo: run both extractors first");
-  if (left.device() != right.device() || left.nlevels() != right.nlevels()) fail(SIVO_EINVAL, "stereo: extractors differ");
+  check_extractors(left, right);
   if (nl < 0 || nr < 0 || nr >= (1 << 20) || !(mb > 0.f) || !(mbf > 0.f)) fail(SIVO_EINVAL, "stereo: bad arguments");
   for (int i = 0; i < nl; ++i) { u_right[i] = -1.f; depth[i] = -1.f; }
   if (nl == 0 || nr == 0) return;
@@ -378,14 +395,33 @@ void stereo_match(const Orb& left, const Orb& right, const sivo_keypoint* kl, co
 void stereo_match_device(Orb& left, Orb& right, const sivo_keypoint* kl, const uint8_t* dl, const int* keep_idx, const long long* n_left,
                          const sivo_keypoint* kr, const uint8_t* dr, const long long* n_right, float mb, float mbf, float* u_right,
                          float* depth, cudaStream_t s) {
-  if (!left.has_run() || !right.has_run()) fail(SIVO_EINVAL, "stereo: run both extractors first");
-  if (left.device() != right.device() || left.nlevels() != right.nlevels()) fail(SIVO_EINVAL, "stereo: extractors differ");
+  check_extractors(left, right);
   if (!(mb > 0.f) || !(mbf > 0.f)) fail(SIVO_EINVAL, "stereo: bad arguments");
+  // the Hamming search packs a right index into 20 bits
+  if (right.capacity() >= (1 << 20)) fail(SIVO_EINVAL, "stereo: right extractor capacity %d needs more than 20 index bits", right.capacity());
   SIVO_CUDA(cudaSetDevice(left.device()));
   if (!s) s = left.stream();
   left.stream_wait(s);
   right.stream_wait(s);
   launch_stereo(left, right, kl, dl, keep_idx, n_left, left.capacity(), kr, dr, n_right, right.capacity(), mb, mbf, u_right, depth,
                 left.stereo_sad(), s);
+}
+
+// Test hook: k_stereo_median_cut alone over n SAD distances (negative = unmatched), cutting u / z in place.
+void stereo_median_cut(int device, const int* sad, int n, float* u, float* z) {
+  if (n < 0) fail(SIVO_EINVAL, "stereo_median_cut: n = %d", n);
+  if (n == 0) return;
+  HostCall& hc = host_call();
+  hc.begin(device);
+  const long long count = n;
+  const long long* d_n = hc.upload(&count, 1);
+  const int* d_s = hc.upload(sad, n);
+  float* d_u = hc.upload(u, n);
+  float* d_z = hc.upload(z, n);
+  k_stereo_median_cut<<<1, kCutThreads, 0, hc.stream>>>(d_n, n, d_s, d_u, d_z);
+  SIVO_CUDA(cudaGetLastError());
+  hc.download(u, d_u, n);
+  hc.download(z, d_z, n);
+  hc.sync();
 }
 }  // namespace sivo

@@ -214,6 +214,17 @@ def stereo_match_device(left: ORBextractor, right: ORBextractor, kp_left_ptr: in
                                              desc_right_ptr, n_right_ptr, mb, mbf, u_right_ptr, depth_ptr, stream or None))
 
 
+def stereo_median_cut(sad, u, z, device: int = 0):
+    """Test hook: the median-based outlier cut of stereo_match alone (sivo_dbg_stereo_median_cut) over int SAD distances (< 0 =
+    unmatched).  Returns copies of u and z with the cut keys set to -1."""
+    s = np.ascontiguousarray(sad, np.int32)
+    u = np.array(u, np.float32)
+    z = np.array(z, np.float32)
+    L.check(L.lib().sivo_dbg_stereo_median_cut(device, s.ctypes.data_as(C.c_void_p), len(s), u.ctypes.data_as(C.c_void_p),
+                                               z.ctypes.data_as(C.c_void_p)))
+    return u, z
+
+
 def hamming_best2(query_desc, train_desc, cand_offsets, cand_idx, train_level=None, device: int = 0) -> np.ndarray:
     """Inner loop of ORBmatcher::SearchByProjection & co (ORBmatcher.cc:79-113) for all queries at once.
     Returns int32 [n_query, 5] = (bestIdx, bestDist, bestLevel, bestDist2, bestLevel2)."""
