@@ -686,6 +686,87 @@ int sivo_search_by_bow(const sivo_orb_t* left, const sivo_keypoint* kps, const u
                        const sivo_keyframe_keys* keyframes, const int* const* kf_point, int n_kf, float nnratio, int check_orientation,
                        int* match, long long* n_matches);
 
+/* ---- Tracking::Relocalization's pose hypotheses: PnPsolver (PnPsolver.cc) with SetRansacParameters(0.99, 10, 300, 4, 0.5, 5.991),
+ * batched over the candidate keyframes ------------------------------------------------------------------------------------------
+ * Every operation is the IEEE float / double operation as written (no contracted multiply-add).  oracle/pnp_oracle.py restates
+ * the rule and the reference facts kept; in short:
+ *   setup     candidate k's correspondences are the semantic keys j < *n_keep_device in order with 0 <= match[k cap + j] <
+ *             n_points (cap = sivo_orb_capacity(left)), a key index inside the capacity and an octave inside the extractor's
+ *             levels: mvP2D = the key's (x, y), mvP3Dw = the point's pos, maxError = sigma2[octave] * 5.991f.  N = their number;
+ *             minInliers = max((int)(N * 0.5f), 10); epsilon = max(0.5f, (float) minInliers / N); maxIts = 1 when minInliers ==
+ *             N, else max(1, min(ceil(log(1 - 0.99) / log(1 - e^3)), 300)) in double with e^3 = (e * e) * e (a NaN or infinite
+ *             quotient counts as INT_MIN, so maxIts = 1).  maxIts <= 35 always.
+ *   iterate   iterate(n): no pose and no_more at once when N < minInliers.  Otherwise hypotheses g = mnIterations,
+ *             mnIterations + 1, ... while mnIterations < maxIts || (this call's count) < n; a hypothesis whose inlier count is
+ *             >= minInliers replaces the best set only with a strictly greater count, then Refine runs on the BEST set so far and
+ *             returns its pose iff its count > minInliers.  After the loop, mnIterations >= maxIts gives no_more and, when the
+ *             best count >= minInliers, the best pose.
+ *   draws     hypothesis g's minimal set: Philox4x32-10 (philox.cuh) with ctr = (g, kf_id[k], frame_id lo, frame_id hi), key =
+ *             (seed lo, seed hi); draw i (0..3) = int((double) word_i / 2^32 * (N - i)), then the reference's swap-remove.  This
+ *             replaces the reference's global rand() stream; every hypothesis is independent of the others.
+ *   EPnP      compute_pose (PnPsolver.cc:482-531) in double as written, with every decomposition the documented one-sided Jacobi
+ *             rule (jacobi.cuh: pairs in row-major order, rotate while |gamma| > 2^-52 sqrt(alpha beta), at most 30 sweeps;
+ *             columns by descending squared norm, ties in column order).  cvSVD's D = the column norms, V = the rotated
+ *             identity, U's column = B's column / its norm.  cvSolve / cvInvert(CV_SVD) keep singular value j iff sigma_j >
+ *             2^-51 * sum(sigma) (OpenCV's SVBkSb threshold): x = sum_j V_j ((B_j . b) / sigma_j^2).  gauss_newton's x starts
+ *             at 0 and qr_solve's early return keeps it.  Sums over correspondences run in correspondence order (Refine's MtM: below).
+ *   departs   from cv::SVD: singular vector signs are Jacobi's; a zero singular value of ABt (coplanar or collinear sets) gives a
+ *             NaN column of U (0 / 0) where cv::SVD completes a basis, so the hypothesis' pose is NaN and it has no inliers.
+ *   inliers   CheckInliers (:318-347): Xc, Yc, invZc rounded to float from double expressions, ue / ve in double, distX / distY
+ *             rounded to float, error2 < maxError in float.  Poses are Rcw | tcw rounded to float.
+ *   Refine    the same compute_pose over the best set's correspondences, one block per candidate: alphas across threads, MtM in a
+ *             fixed tree (thread t of 256 sums correspondences t, t + 256, ... in order; xor shuffles 16 .. 1 in each warp; the 8
+ *             warp totals folded by halves), every other sum in correspondence order in one thread.  The reference sums MtM in row
+ *             order; the two agree to rounding.
+ *   cost      EPnP's decompositions run in one thread per hypothesis and per Refine; k_pnp_hyp and k_pnp_decide use 255 registers
+ *             and spill a few hundred bytes (the 12 x 12 and 6 x K working arrays).
+ * Handle: one PnPsolver per candidate, kept across calls (mnIterations, the best count, set and pose).  The extractor must outlive
+ * the handle.  Calls on one handle must be ordered on one stream. */
+typedef struct sivo_pnp sivo_pnp_t;
+/* max_candidates in [1, 256]; SIVO_EINVAL otherwise.  Enqueues nothing: the candidates' state is written by setup. */
+int sivo_pnp_create(const sivo_orb_t* left, int max_candidates, uint64_t seed, sivo_pnp_t** out);
+void sivo_pnp_destroy(sivo_pnp_t* h);
+/* Builds n_kf PnPsolvers (n_kf <= max_candidates) from sivo_search_by_bow_device's outputs as they are: match_device (n_kf rows of
+ * cap ints), n_matches_device (n_kf int64).  Frame keys as for the other Frame-tail calls (keep_idx_device NULL = identity);
+ * points_device the map points the rows index.  kf_id (host, n_kf) and frame_id select the draws.  A negative frame count or
+ * n_matches_device[k] makes candidate k return no_more with no pose.  Resets every candidate's state.  Runs on `stream` (NULL = the
+ * left extractor's stream) with no host synchronisation; the inputs may be reused once it has run.  SIVO_EINVAL for NULL handles
+ * or inputs, n_kf outside [0, max_candidates], n_points < 0 or a camera parameter not finite. */
+int sivo_pnp_setup_device(sivo_pnp_t* h, const sivo_keypoint* kps_device, const int* keep_idx_device, const long long* n_keep_device,
+                          const int* match_device, const long long* n_matches_device, const sivo_map_point* points_device,
+                          int n_points, const uint32_t* kf_id, int n_kf, uint64_t frame_id, float fx, float fy, float cx, float cy,
+                          void* stream);
+/* iterate(n_iterations) on every candidate k of the last setup with active[k] != 0 (host array; the others are neither run nor
+ * written).  Per active k: Tcw_device[12 k ..] (3 x 4 row-major, usable as sivo_pose_optimize_device's Tcw_in) when
+ * has_pose_device[k]; no_more_device[k]; n_inliers_device[k]; inlier_match_device[k cap + j] = match[k cap + j] for the
+ * inliers, -1 for every other j < cap (the row that becomes mvpMapPoints).  Scratch is allocated and freed on `stream`
+ * (stream-ordered), never on the extractor.  SIVO_EINVAL for NULL handles or outputs. */
+int sivo_pnp_iterate_device(sivo_pnp_t* h, int n_iterations, const uint8_t* active, float* Tcw_device, int* has_pose_device,
+                            int* no_more_device, int* inlier_match_device, int* n_inliers_device, void* stream);
+/* Test hooks.  sivo_dbg_pnp_state synchronises the device, then per candidate of the last setup: out[7 k ..] = N, minInliers,
+ * maxIts, mnIterations, best count, the best set's Refine has failed, dead (a negative count); eps[k] = epsilon (may be NULL). */
+int sivo_dbg_pnp_state(const sivo_pnp_t* h, int* out, float* eps);
+typedef struct sivo_pnp_pose_debug {
+  double cws[12];                          /* control points, 4 x 3 */
+  double d[12], ut[144];                   /* MtM's singular values (descending); Ut: row r = V's column for d[r] */
+  double l_6x10[60], rho[6];
+  double betas[12];                        /* approximations 1, 2, 3 after gauss_newton, 4 each */
+  double Rs[27], ts[9], rep_errors[3];     /* compute_R_and_t of each */
+  double R[9], t[3];                       /* the chosen one */
+  int32_t best, reserved;                  /* 1, 2 or 3 */
+} sivo_pnp_pose_debug;
+/* Refine's kernel path (block_pose: the gather, compute_pose with MtM in its tree order, CheckInliers) on n >= 1 host
+ * correspondences, all selected: p3d n x 3, p2d n x 2, max_err n (floats).  Outputs alphas (4 n, may be NULL), mask ((n + 31) / 32
+ * words, may be NULL), *n_inliers (may be NULL) and *dbg. */
+int sivo_dbg_pnp_compute_pose(int device, const float* p3d, const float* p2d, const float* max_err, int n, float fx, float fy, float cx,
+                              float cy, double* alphas, uint32_t* mask, int* n_inliers, sivo_pnp_pose_debug* dbg);
+/* k_pnp_hyp itself for candidate k of the last setup, hypotheses first .. first + n_hyp - 1, without touching the state (it
+ * synchronises the device): draws[4 h ..], Rt[12 h ..] (R row-major, then t, doubles), counts[h] (-1 when the candidate has no
+ * hypotheses: dead or N < minInliers), masks[h words ..] (words = (sivo_orb_capacity + 31) / 32). */
+int sivo_dbg_pnp_hypotheses(sivo_pnp_t* h, int k, int first, int n_hyp, int* draws, double* Rt, int* counts, uint32_t* masks);
+/* The minimal sets of hypotheses first .. first + n_hyp - 1 among N >= 4 correspondences: out[4 h ..]. */
+int sivo_dbg_pnp_draws(int device, uint64_t seed, uint32_t kf_id, uint64_t frame_id, int first, int n_hyp, int N, int* out);
+
 /* Best / second-best match over per-query candidate lists -- the inner loop of ORBmatcher::SearchByProjection
  * (ORBmatcher.cc:79-113), its last-frame / keyframe variants (:1278-, :1420-), SearchForTriangulation (:631-) and
  * SearchBySim3 (next row 4).  Query i's candidates are cand_idx[cand_offsets[i] .. cand_offsets[i+1]) (indices into the

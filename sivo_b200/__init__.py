@@ -7,3 +7,4 @@ from .track import (MAP_POINT_DTYPE, TrackFrame, make_frame, map_points, search_
                     search_local_points, search_local_points_device)
 from .pose import PoseResult, pose_gather_device, pose_optimize, pose_optimize_device  # noqa: F401
 from .bow import Vocabulary, compute_bow, compute_bow_device, search_by_bow, search_by_bow_device  # noqa: F401
+from .reloc import PnpSolver  # noqa: F401

@@ -89,6 +89,15 @@ def lib() -> C.CDLL:
         _lib.sivo_compute_bow.argtypes = [vp, vp, i32, i32, vp, vp, vp, vp, vp]
         _lib.sivo_search_by_bow_device.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, i32, f32, i32, vp, vp, vp]
         _lib.sivo_search_by_bow.argtypes = [vp, vp, vp, vp, i32, vp, vp, i32, f32, i32, vp, vp]
+        _lib.sivo_pnp_destroy.restype = None
+        _lib.sivo_pnp_create.argtypes = [vp, i32, C.c_uint64, vp]
+        _lib.sivo_pnp_setup_device.argtypes = [vp, vp, vp, vp, vp, vp, vp, i32, vp, i32, C.c_uint64, f32, f32, f32, f32, vp]
+        _lib.sivo_pnp_iterate_device.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, vp]
+        _lib.sivo_dbg_pnp_state.argtypes = [vp, vp, vp]
+        d64 = C.c_double
+        _lib.sivo_dbg_pnp_compute_pose.argtypes = [i32, vp, vp, vp, i32, f32, f32, f32, f32, vp, vp, vp, vp]
+        _lib.sivo_dbg_pnp_hypotheses.argtypes = [vp, i32, i32, i32, vp, vp, vp, vp]
+        _lib.sivo_dbg_pnp_draws.argtypes = [i32, C.c_uint64, C.c_uint32, C.c_uint64, i32, i32, i32, vp]
         _lib.sivo_dbg_conv_unpooled.argtypes = [i32, vp, vp, i32, i32, i32, i32, vp, vp, vp, vp, i32, i32, vp]
     return _lib
 

@@ -23,6 +23,7 @@ using namespace sivo;
 struct sivo_segnet { SegNet* impl; };
 struct sivo_orb { Orb* impl; };
 struct sivo_vocabulary { Vocabulary* impl; };
+struct sivo_pnp { Pnp* impl; };
 
 extern "C" {
 
@@ -648,6 +649,67 @@ int sivo_dbg_create_map_points(const sivo_orb_t* left, const sivo_keyframe_keys*
     create_map_points_host(*left->impl, *kf1, neighbours, n_neighbours, *params, match, stage, reduction, created_nb, created_idx, world,
                            created_list, n_created);
   });
+}
+
+// ---------------------------------------------------------------------------------------- relocalisation PnP RANSAC
+int sivo_pnp_create(const sivo_orb_t* left, int max_candidates, uint64_t seed, sivo_pnp_t** out) {
+  return guarded([&] {
+    if (!left || !out) fail(SIVO_EINVAL, "pnp_create: null argument");
+    *out = nullptr;
+    Pnp* impl = pnp_create(*left->impl, max_candidates, seed);
+    *out = new sivo_pnp{impl};
+  });
+}
+
+void sivo_pnp_destroy(sivo_pnp_t* h) {
+  if (!h) return;
+  pnp_destroy(h->impl);
+  delete h;
+}
+
+int sivo_pnp_setup_device(sivo_pnp_t* h, const sivo_keypoint* kps_device, const int* keep_idx_device, const long long* n_keep_device,
+                          const int* match_device, const long long* n_matches_device, const sivo_map_point* points_device,
+                          int n_points, const uint32_t* kf_id, int n_kf, uint64_t frame_id, float fx, float fy, float cx, float cy,
+                          void* stream) {
+  return guarded([&] {
+    if (!h || !kps_device || !n_keep_device || (n_kf > 0 && (!match_device || !n_matches_device)) || (n_points > 0 && !points_device))
+      fail(SIVO_EINVAL, "pnp_setup: null argument");
+    pnp_setup_device(*h->impl, kps_device, keep_idx_device, n_keep_device, match_device, n_matches_device, points_device, n_points, kf_id,
+                     n_kf, frame_id, fx, fy, cx, cy, static_cast<cudaStream_t>(stream));
+  });
+}
+
+int sivo_pnp_iterate_device(sivo_pnp_t* h, int n_iterations, const uint8_t* active, float* Tcw_device, int* has_pose_device,
+                            int* no_more_device, int* inlier_match_device, int* n_inliers_device, void* stream) {
+  return guarded([&] {
+    if (!h || !Tcw_device || !has_pose_device || !no_more_device || !inlier_match_device || !n_inliers_device)
+      fail(SIVO_EINVAL, "pnp_iterate: null argument");
+    pnp_iterate_device(*h->impl, n_iterations, active, Tcw_device, has_pose_device, no_more_device, inlier_match_device, n_inliers_device,
+                       static_cast<cudaStream_t>(stream));
+  });
+}
+
+int sivo_dbg_pnp_state(const sivo_pnp_t* h, int* out, float* eps) {
+  return guarded([&] {
+    if (!h || !out) fail(SIVO_EINVAL, "pnp_state: null argument");
+    pnp_state(*h->impl, out, eps);
+  });
+}
+
+int sivo_dbg_pnp_compute_pose(int device, const float* p3d, const float* p2d, const float* max_err, int n, float fx, float fy, float cx,
+                              float cy, double* alphas, uint32_t* mask, int* n_inliers, sivo_pnp_pose_debug* dbg) {
+  return guarded([&] { pnp_compute_pose_debug(device, p3d, p2d, max_err, n, fx, fy, cx, cy, alphas, mask, n_inliers, dbg); });
+}
+
+int sivo_dbg_pnp_hypotheses(sivo_pnp_t* h, int k, int first, int n_hyp, int* draws, double* Rt, int* counts, uint32_t* masks) {
+  return guarded([&] {
+    if (!h || !draws || !Rt || !counts || !masks) fail(SIVO_EINVAL, "pnp_hypotheses: null argument");
+    pnp_hypotheses(*h->impl, k, first, n_hyp, draws, Rt, counts, masks);
+  });
+}
+
+int sivo_dbg_pnp_draws(int device, uint64_t seed, uint32_t kf_id, uint64_t frame_id, int first, int n_hyp, int N, int* out) {
+  return guarded([&] { pnp_draws(device, seed, kf_id, frame_id, first, n_hyp, N, out); });
 }
 
 // ---------------------------------------------------------------------------------------- vocabulary and bag of words

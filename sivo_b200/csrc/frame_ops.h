@@ -69,4 +69,20 @@ void create_map_points_host(const Orb& left, const sivo_keyframe_keys& kf1, cons
                             const sivo_mapping_params& prm, int* dbg_match, int* dbg_stage, double* dbg_red, int* created_nb,
                             int* created_idx, float* world, int* created_list, long long* n_created);
 
+// ---- pnp.cu
+constexpr int kPnpMaxCandidates = 256;
+struct Pnp;
+Pnp* pnp_create(const Orb& left, int max_candidates, uint64_t seed);
+void pnp_destroy(Pnp* h);
+void pnp_setup_device(Pnp& h, const sivo_keypoint* kps, const int* keep_idx, const long long* n_keep, const int* match,
+                      const long long* n_matches, const sivo_map_point* points, int n_points, const uint32_t* kf_id, int n_kf,
+                      uint64_t frame_id, float fx, float fy, float cx, float cy, cudaStream_t s);
+void pnp_iterate_device(Pnp& h, int n_iterations, const uint8_t* active, float* Tcw, int* has_pose, int* no_more, int* inlier_match,
+                        int* n_inliers, cudaStream_t s);
+void pnp_state(const Pnp& h, int* out, float* eps);
+void pnp_compute_pose_debug(int device, const float* p3d, const float* p2d, const float* max_err, int n, float fx, float fy, float cx,
+                            float cy, double* alphas, uint32_t* mask, int* n_inliers, sivo_pnp_pose_debug* dbg);
+void pnp_hypotheses(Pnp& h, int k, int first, int n_hyp, int* draws, double* Rt, int* counts, uint32_t* masks);
+void pnp_draws(int device, uint64_t seed, uint32_t kf_id, uint64_t frame_id, int first, int n_hyp, int N, int* out);
+
 }  // namespace sivo

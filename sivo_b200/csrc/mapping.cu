@@ -16,6 +16,7 @@
 #include "frame_ops.h"
 #include "host_call.h"
 #include "info_mi.cuh"
+#include "jacobi.cuh"
 
 namespace sivo {
 namespace {
@@ -23,7 +24,6 @@ constexpr int kMaxNeighbours = 32;
 constexpr int kThLow = 50;  // ORBmatcher::TH_LOW
 constexpr int kMapThreads = 128, kMapWarps = kMapThreads / 32;
 constexpr int kListThreads = 1024;
-constexpr int kMaxSweeps = 30;
 constexpr int kVoid = 255;  // Classes::VOID
 enum { kHasPoint = 0, kBaseline, kNoMatch, kParallax, kWZero, kZ1, kZ2, kReproj1, kReproj2, kScale, kSemantic, kCreated };
 
@@ -96,43 +96,14 @@ __device__ __forceinline__ float cos_parallax_stereo(float mb, float depth) {
   return static_cast<float>(cos(static_cast<double>(2.f * a)));
 }
 
-// The triangulation's right singular vector (the documented rule): one-sided Jacobi on A's columns in double.
+// The triangulation's right singular vector (the documented rule, jacobi.cuh): the rotated identity's column of least norm.
 __device__ void svd_null_vector(double a[4][4], double out[4]) {
   double v[4][4];
 #pragma unroll
   for (int r = 0; r < 4; ++r)
 #pragma unroll
     for (int c = 0; c < 4; ++c) v[r][c] = r == c ? 1.0 : 0.0;
-  for (int sweep = 0; sweep < kMaxSweeps; ++sweep) {
-    bool rotated = false;
-#pragma unroll
-    for (int p = 0; p < 3; ++p)
-#pragma unroll
-      for (int q = p + 1; q < 4; ++q) {
-        double alpha = 0.0, beta = 0.0, gamma = 0.0;
-#pragma unroll
-        for (int r = 0; r < 4; ++r) {
-          alpha = alpha + a[r][p] * a[r][p];
-          beta = beta + a[r][q] * a[r][q];
-          gamma = gamma + a[r][p] * a[r][q];
-        }
-        if (!(fabs(gamma) > 0x1p-52 * sqrt(alpha * beta))) continue;
-        const double zeta = (beta - alpha) / (2.0 * gamma);
-        const double t = (zeta >= 0.0 ? 1.0 : -1.0) / (fabs(zeta) + sqrt(1.0 + zeta * zeta));
-        const double c = 1.0 / sqrt(1.0 + t * t), s = c * t;
-#pragma unroll
-        for (int r = 0; r < 4; ++r) {
-          const double ap = a[r][p], aq = a[r][q];
-          a[r][p] = c * ap - s * aq;
-          a[r][q] = s * ap + c * aq;
-          const double vp = v[r][p], vq = v[r][q];
-          v[r][p] = c * vp - s * vq;
-          v[r][q] = s * vp + c * vq;
-        }
-        rotated = true;
-      }
-    if (!rotated) break;
-  }
+  jacobi_sweeps<4, 4>(a, v);
   int best = 0;
   double best_n = 0.0;
 #pragma unroll
