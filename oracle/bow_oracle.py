@@ -40,6 +40,7 @@ import math
 
 import numpy as np
 
+from oracle.orb_oracle import descriptor_distance
 from oracle.track_oracle import F32, HISTO_LENGTH, angle_ok, compute_three_maxima, round_half_away
 
 TH_LOW = 50
@@ -240,10 +241,6 @@ def bow_arrays(bow: dict):
 
 
 # ------------------------------------------------------------------------------------------------------------------ SearchByBoW
-def descriptor_distance(a, b) -> int:
-    return int(np.unpackbits(np.bitwise_xor(np.asarray(a, np.uint8), np.asarray(b, np.uint8))).sum())
-
-
 def feature_vector(node, angles) -> dict:
     """{node: [key indices ascending]} of the keys with node >= 0 whose angle obeys the angle rule."""
     fv = {}

@@ -48,6 +48,7 @@ from dataclasses import dataclass, field
 import numpy as np
 
 from oracle.info_oracle import stereo_covariance, stereo_jacobian_pose, det3_cofactor, det_lu
+from oracle.orb_oracle import descriptor_distance
 
 F32, F64 = np.float32, np.float64
 TH_LOW = 50
@@ -249,10 +250,6 @@ def check_dist_epipolar_line(kp1, kp2, F, sigma2) -> bool:
     return float(dsqr) < 3.84 * float(F32(sigma2[kp2["octave"]]))
 
 
-def hamming(a, b) -> int:
-    return int(np.unpackbits(np.bitwise_xor(a, b)).sum())
-
-
 def search_key(kf1: KeyFrame, j, kf2: KeyFrame, F, ex, ey, scale, sigma2, groups) -> int:
     """SearchForTriangulation's loop for current key j: the matched neighbour key or -1."""
     nl = len(scale)
@@ -263,7 +260,7 @@ def search_key(kf1: KeyFrame, j, kf2: KeyFrame, F, ex, ey, scale, sigma2, groups
         kp2 = kf2.kps[i2]
         if not 0 <= kp2["octave"] < nl:
             continue
-        d = hamming(kf1.desc[j], kf2.desc[i2])
+        d = descriptor_distance(kf1.desc[j], kf2.desc[i2])
         if d > TH_LOW or d > best_d:
             continue
         if not stereo1 and not F32(kf2.u_right[i2]) >= 0:

@@ -518,9 +518,9 @@ def extract(image: np.ndarray, params: ExtractorParams = ExtractorParams()) -> O
 
 
 # ---------------------------------------------------------------------------------- Hamming
-def descriptor_distance(a: np.ndarray, b: np.ndarray) -> int:
-    """ORBmatcher::DescriptorDistance (src/orbslam/ORBmatcher.cc:1582-1596): popcount of a XOR b."""
-    return int(np.unpackbits(np.bitwise_xor(a, b)).sum())
+def descriptor_distance(a, b) -> int:
+    """ORBmatcher::DescriptorDistance (src/orbslam/ORBmatcher.cc:1582-1596): popcount of a XOR b (32-byte descriptors)."""
+    return int(np.unpackbits(np.bitwise_xor(np.asarray(a, np.uint8), np.asarray(b, np.uint8))).sum())
 
 
 _POP8 = np.array([bin(v).count("1") for v in range(256)], np.int64)

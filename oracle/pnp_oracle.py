@@ -44,6 +44,7 @@ from dataclasses import dataclass, field
 import numpy as np
 
 from oracle.philox import philox4x32_10
+from oracle.pose_oracle import tree_sum
 
 F32 = np.float32
 MAX_SWEEPS = 30
@@ -252,7 +253,7 @@ def _sqrt(x):
 
 def mtm_tree(M, a, b):
     """MtM[a][b] in Refine's device order: thread t of 256 sums correspondences t, t + 256, ... (rows 2i then 2i + 1), xor
-    shuffles 16 .. 1 within each warp of 32, then the 8 warp totals folded by halves."""
+    shuffles 16 .. 1 within each warp of 32, then the 8 warp totals folded by halves (pose_oracle.tree_sum)."""
     M = np.asarray(M, np.float64)
     n = len(M) // 2
     P1, P2 = M[0::2, a] * M[0::2, b], M[1::2, a] * M[1::2, b]
@@ -263,13 +264,7 @@ def mtm_tree(M, a, b):
         ok = i < n
         s[ok] = s[ok] + P1[i[ok]]
         s[ok] = s[ok] + P2[i[ok]]
-    s = s.reshape(8, 32)
-    lane = np.arange(32)
-    for off in (16, 8, 4, 2, 1):
-        s = s + s[:, lane ^ off]
-    w = s[:, 0]
-    q = [w[i] + w[i + 4] for i in range(4)]
-    return float((q[0] + q[2]) + (q[1] + q[3]))
+    return float(tree_sum(s))
 
 
 def compute_pose(pws, us, fu, fv, uc, vc, la=None, tree=False) -> PoseDebug:

@@ -340,6 +340,23 @@ def edge_terms(E: Edges, ev: EdgeEval) -> np.ndarray:
     return out
 
 
+def tree_sum(acc):
+    """The device's fixed reduction tree over per-thread sums acc (THREADS, ...) of a THREADS-thread block: xor shuffles
+    16 .. 1 within each warp (lane 0's sum adds the halves, w[i] + w[i + s] for s = 16 .. 1), then the warp totals folded as
+    w[i] + w[i + s] for s = 4, 2, 1."""
+    w = np.asarray(acc, F64).reshape(THREADS // WARP, WARP, *np.shape(acc)[1:])
+    s = WARP // 2
+    while s:
+        w = w[:, :s] + w[:, s:2 * s]
+        s //= 2
+    t = w[:, 0]
+    s = THREADS // WARP // 2
+    while s:
+        t = t[:s] + t[s:2 * s]
+        s //= 2
+    return t[0]
+
+
 def reduce_edges(v, order: str) -> np.ndarray:
     """Sum the rows of v (n, m) in the given order (rows in key order; rows of edges left out must be zero)."""
     v = np.asarray(v, F64)
@@ -356,17 +373,7 @@ def reduce_edges(v, order: str) -> np.ndarray:
     acc = np.zeros((THREADS, m), F64)
     for k in range(0, n_pad, THREADS):
         acc = acc + p[k:k + THREADS]
-    w = acc.reshape(THREADS // WARP, WARP, m)
-    s = WARP // 2
-    while s:
-        w = w[:, :s] + w[:, s:2 * s]
-        s //= 2
-    t = w[:, 0]
-    s = THREADS // WARP // 2
-    while s:
-        t = t[:s] + t[s:2 * s]
-        s //= 2
-    return t[0]
+    return tree_sum(acc)
 
 
 @dataclass

@@ -26,6 +26,8 @@ from dataclasses import dataclass
 
 import numpy as np
 
+from oracle.orb_oracle import descriptor_distance
+
 F32, F64 = np.float32, np.float64
 COLS, ROWS = 64, 48  # FRAME_GRID_COLS / FRAME_GRID_ROWS
 TH_HIGH = 100
@@ -194,10 +196,6 @@ def is_in_frustum(mp, f: Frame, log_scale, nlevels, viewing_cos_limit=0.5):
         if level is None:
             return None
         return u, v, u - f.mbf * invz, level, view_cos
-
-
-def descriptor_distance(a, b) -> int:
-    return int(np.unpackbits(np.bitwise_xor(np.asarray(a, np.uint8), np.asarray(b, np.uint8))).sum())
 
 
 # ---------------------------------------------------------------------------------------------------------- the searches

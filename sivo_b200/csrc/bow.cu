@@ -16,6 +16,7 @@
 #include <cmath>
 #include <mutex>
 
+#include "block_ops.cuh"
 #include "host_call.h"
 #include "match_fold.cuh"
 #include "vocabulary.h"
@@ -29,18 +30,6 @@ constexpr int kWarpThreads = 256, kWarps = kWarpThreads / 32;
 constexpr int kBlockThreads = 1024;
 constexpr int kChunk = 64;           // keyframes per launch (their table travels as a kernel parameter)
 constexpr unsigned long long kNone = ~0ull;
-
-__device__ __forceinline__ int clamp_count(long long n, int cap) {
-  return n < 0 ? -1 : static_cast<int>(min(n, static_cast<long long>(cap)));
-}
-
-__device__ __forceinline__ int hamming(uint4 a0, uint4 a1, uint4 b0, uint4 b1) {
-  return __popc(a0.x ^ b0.x) + __popc(a0.y ^ b0.y) + __popc(a0.z ^ b0.z) + __popc(a0.w ^ b0.w) + __popc(a1.x ^ b1.x) +
-         __popc(a1.y ^ b1.y) + __popc(a1.z ^ b1.z) + __popc(a1.w ^ b1.w);
-}
-
-// the projection searches' angle rule (track.cu)
-__device__ __forceinline__ bool angle_ok(float a) { return a >= 0.f && a <= 360.f; }
 
 int pow2_at_least(int n) {
   int p = 1;
@@ -83,7 +72,7 @@ __global__ void __launch_bounds__(kWarpThreads) k_bow_descend(const VocView v, c
       unsigned long long best = kNone;
       for (int c = b + lane; c < e; c += 32) {
         const int ch = v.children[c];
-        const int d = hamming(q0, q1, v.desc[2 * ch], v.desc[2 * ch + 1]);
+        const int d = descriptor_distance(q0, q1, v.desc[2 * ch], v.desc[2 * ch + 1]);
         best = min(best, (static_cast<unsigned long long>(d) << 32) | static_cast<unsigned>(c - b));
       }
 #pragma unroll
@@ -111,7 +100,7 @@ __global__ void __launch_bounds__(kBlockThreads) k_bow_vector(const VocView v, c
   unsigned* s = reinterpret_cast<unsigned*>(val + cap);
   __shared__ int warp_count[kBlockThreads / 32];
   __shared__ double norm_s;
-  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  const int tid = threadIdx.x;
   const int n = clamp_count(*n_keep, cap);
   if (n < 0) {
     if (tid == 0 && bow_len) *bow_len = -1;
@@ -126,16 +115,10 @@ __global__ void __launch_bounds__(kBlockThreads) k_bow_vector(const VocView v, c
   for (int c0 = 0; c0 < n; c0 += kBlockThreads) {
     const int i = c0 + tid;
     const bool start = i < n && s[i] != 0xffffffffu && (i == 0 || s[i - 1] != s[i]);
-    const unsigned bal = __ballot_sync(0xffffffffu, start);
-    if (lane == 0) warp_count[wid] = __popc(bal);
-    __syncthreads();
-    int before = 0, total = 0;
-    for (int w = 0; w < kBlockThreads / 32; ++w) {
-      before += w < wid ? warp_count[w] : 0;
-      total += warp_count[w];
-    }
+    int total;
+    const int rank = block_rank<kBlockThreads>(start, warp_count, &total);
     if (start) {
-      const int pos = m + before + __popc(bal & ((1u << lane) - 1u));
+      const int pos = m + rank;
       int e = i + 1;
       while (e < n && s[e] == s[i]) ++e;
       const double w = v.word_weight[s[i]];
@@ -265,7 +248,7 @@ __global__ void __launch_bounds__(kWarpThreads) k_sbb_walk(const SbbFrame f, con
           j = static_cast<int>(sorted[g] & 0xffffffffu);
           if (row[j] < 0) {
             const int fk = frame_key(f, j);
-            d = hamming(q0, q1, f.desc[2 * fk], f.desc[2 * fk + 1]);
+            d = descriptor_distance(q0, q1, f.desc[2 * fk], f.desc[2 * fk + 1]);
           }
         }
         best2_fold_warp(b, d, j, 0, min(32, e - g0));
@@ -394,8 +377,7 @@ void compute_bow_device(const Vocabulary& voc, const Orb& left, const uint8_t* d
   if (voc.device != left.device()) fail(SIVO_EINVAL, "compute_bow: the vocabulary is on device %d, the extractor on %d", voc.device, left.device());
   const int cap = left.capacity();
   check_cap(cap, "compute_bow");
-  SIVO_CUDA(cudaSetDevice(left.device()));
-  if (!s) s = left.stream();
+  s = left.enter(s);
   // stream-ordered scratch of this call: LocalMapping runs it concurrently with Tracking's calls on the same extractor
   int* scratch = nullptr;
   if (!word) SIVO_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&scratch), static_cast<size_t>(std::max(cap, 1)) * sizeof(int), s));
@@ -446,8 +428,7 @@ void search_by_bow_device(const Orb& left, const sivo_keypoint* kps, const uint8
     if (!kfs[k].kps || !kfs[k].desc || !kfs[k].node || !kf_point[k]) fail(SIVO_EINVAL, "search_by_bow: null array in keyframe %d", k);
     t[k] = SbbKf{kfs[k].kps, reinterpret_cast<const uint4*>(kfs[k].desc), kfs[k].node, kf_point[k], kfs[k].count, cap};
   }
-  SIVO_CUDA(cudaSetDevice(left.device()));
-  if (!s) s = left.stream();
+  s = left.enter(s);
   const SbbFrame f{kps, reinterpret_cast<const uint4*>(desc), keep_idx, n_keep, node, cap, nnratio, check ? 1 : 0};
   // stream-ordered scratch of this call: the frame's sorted keys and one rotation bin per (keyframe, frame key)
   const size_t sort_bytes = static_cast<size_t>(std::max(cap, 1)) * sizeof(unsigned long long);
@@ -471,7 +452,7 @@ void search_by_bow_host(const Orb& left, const sivo_keypoint* kps, const uint8_t
   if (n_kf > 0 && n > 0 && !match) fail(SIVO_EINVAL, "search_by_bow: null match");
   check_cap(n, "search_by_bow");
   for (int j = 0; j < n; ++j)
-    if (!(kps[j].angle >= 0.f && kps[j].angle <= 360.f)) fail(SIVO_ERANGE, "search_by_bow: frame key %d angle %g outside [0, 360]", j, kps[j].angle);
+    if (!angle_ok(kps[j].angle)) fail(SIVO_ERANGE, "search_by_bow: frame key %d angle %g outside [0, 360]", j, kps[j].angle);
   HostCall& hc = host_call();
   hc.begin(left.device());
   std::vector<SbbKf> t(n_kf);
@@ -481,7 +462,7 @@ void search_by_bow_host(const Orb& left, const sivo_keypoint* kps, const uint8_t
     if (c > kMaxKeys) fail(SIVO_ERANGE, "search_by_bow: keyframe %d has %lld keys, at most %d", k, c, kMaxKeys);
     if (m > 0 && (!kfs[k].kps || !kfs[k].desc || !kfs[k].node || !kf_point[k])) fail(SIVO_EINVAL, "search_by_bow: null array in keyframe %d", k);
     for (int i = 0; i < m; ++i)
-      if (!(kfs[k].kps[i].angle >= 0.f && kfs[k].kps[i].angle <= 360.f))
+      if (!angle_ok(kfs[k].kps[i].angle))
         fail(SIVO_ERANGE, "search_by_bow: keyframe %d key %d angle %g outside [0, 360]", k, i, kfs[k].kps[i].angle);
     t[k] = SbbKf{hc.upload(kfs[k].kps, m), reinterpret_cast<const uint4*>(hc.upload(kfs[k].desc, 32 * static_cast<size_t>(m))),
                  hc.upload(kfs[k].node, m), hc.upload(kf_point[k], m), hc.upload(kfs[k].count, 1), m};

@@ -5,7 +5,7 @@
 // (the divisions and log2 keep the math library's own sequences).
 #include <cmath>
 
-#include "compact.cuh"
+#include "block_ops.cuh"
 #include "frame_ops.h"
 #include "host_call.h"
 #include "info_mi.cuh"
@@ -79,17 +79,15 @@ __global__ void __launch_bounds__(kCompactThreads) k_info_compact(const long lon
                                                                  const uint8_t* __restrict__ flags, int* __restrict__ selected,
                                                                  long long* __restrict__ n_selected) {
   __shared__ int warp_kept[kCompactThreads / 32];
-  const long long n64 = *count;
-  if (n64 < 0) {
+  const int n = clamp_count(*count, cap);
+  if (n < 0) {
     if (threadIdx.x == 0 && n_selected) *n_selected = -1;
     return;
   }
-  const int n = static_cast<int>(min(n64, static_cast<long long>(cap)));
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   int base = 0;
   for (int c0 = 0; c0 < n; c0 += kCompactThreads) {
-    const int i = c0 + tid;
-    base = compact_chunk<kCompactThreads>(i < n && flags[i], i, base, lane, warp, warp_kept, selected);
+    const int i = c0 + threadIdx.x;
+    base = compact_chunk<kCompactThreads>(i < n && flags[i], i, base, warp_kept, selected);
   }
   if (threadIdx.x == 0 && n_selected) *n_selected = base;
 }
@@ -173,8 +171,7 @@ void info_terms(const Orb& left, const sivo_keypoint* kps, const float* depth, i
 void info_select_device(const Orb& left, const sivo_keypoint* kps, const double* kp_entropy, const int* keep_idx, const long long* n_keep,
                         const float* depth, const sivo_info_camera& cam, double threshold, float* world, double* reduction, int* selected,
                         long long* n_selected, cudaStream_t s) {
-  SIVO_CUDA(cudaSetDevice(left.device()));
-  if (!s) s = left.stream();
+  s = left.enter(s);
   launch_info_select(make_params(left, cam, threshold), kps, kp_entropy, keep_idx, n_keep, left.capacity(), depth, world, reduction,
                      left.info_flags(), selected, n_selected, nullptr, nullptr, nullptr, s);
 }

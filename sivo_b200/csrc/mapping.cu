@@ -12,11 +12,12 @@
 //   k_map_list       one block: the created points neighbour-major, key ascending (mlpRecentAddedMapPoints' order).
 #include <cmath>
 
-#include "compact.cuh"
+#include "block_ops.cuh"
 #include "frame_ops.h"
 #include "host_call.h"
 #include "info_mi.cuh"
 #include "jacobi.cuh"
+#include "match_fold.cuh"
 
 namespace sivo {
 namespace {
@@ -57,10 +58,6 @@ struct MapParams {
   int n_nb, nlevels, cap, stride, max_class, full;
 };
 
-__device__ __forceinline__ int clamp_count(long long n, int cap) {
-  return n < 0 ? -1 : static_cast<int>(min(n, static_cast<long long>(cap)));
-}
-
 // any keyframe's count negative (every lane of the warp gets the same answer)
 __device__ __forceinline__ bool any_negative(const MapParams& p, int lane) {
   const bool neg = (lane < p.n_nb && *p.nb[lane].kf.count < 0) || (lane == 0 && *p.kf1.count < 0);
@@ -82,11 +79,6 @@ __device__ __forceinline__ double dot3(const float* a, const float* b) {
 #pragma unroll
   for (int i = 0; i < 3; ++i) s = s + static_cast<double>(a[i]) * static_cast<double>(b[i]);
   return s;
-}
-
-__device__ __forceinline__ int hamming(uint4 a0, uint4 a1, uint4 b0, uint4 b1) {
-  return __popc(a0.x ^ b0.x) + __popc(a0.y ^ b0.y) + __popc(a0.z ^ b0.z) + __popc(a0.w ^ b0.w) + __popc(a1.x ^ b1.x) +
-         __popc(a1.y ^ b1.y) + __popc(a1.z ^ b1.z) + __popc(a1.w ^ b1.w);
 }
 
 // cos(2 * atan2(mb / 2, depth)) with the float overloads, as the correctly rounded float functions (within an ulp of glibc's)
@@ -209,7 +201,7 @@ __global__ void __launch_bounds__(kMapThreads) k_map_create(const __grid_constan
         if (!cand) continue;
         const sivo_keypoint kp2 = k2.kps[i2];
         if (kp2.octave < 0 || kp2.octave >= p.nlevels) continue;
-        const int d = hamming(q0, q1, k2.desc[2 * i2], k2.desc[2 * i2 + 1]);
+        const int d = descriptor_distance(q0, q1, k2.desc[2 * i2], k2.desc[2 * i2 + 1]);
         if (d > bd) continue;
         if (!stereo1 && !(k2.ur[i2] >= 0.f)) {
           const float dex = nb.ex - kp2.x, dey = nb.ey - kp2.y;
@@ -316,8 +308,8 @@ __global__ void __launch_bounds__(kMapThreads) k_map_create(const __grid_constan
 __global__ void __launch_bounds__(kListThreads) k_map_list(const __grid_constant__ MapParams p, const int* __restrict__ made_nb,
                                                            int* __restrict__ keys, int* __restrict__ list, long long* __restrict__ n_created) {
   __shared__ int warp_kept[kListThreads / 32];
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  if (any_negative(p, lane)) {
+  const int tid = threadIdx.x;
+  if (any_negative(p, tid & 31)) {
     if (tid == 0 && n_created) *n_created = -1;
     return;
   }
@@ -326,7 +318,7 @@ __global__ void __launch_bounds__(kListThreads) k_map_list(const __grid_constant
   for (int i = 0; i < p.n_nb; ++i)
     for (int c0 = 0; c0 < n1; c0 += kListThreads) {
       const int j = c0 + tid;
-      base = compact_chunk<kListThreads>(j < n1 && made_nb[j] == i, j, base, lane, warp, warp_kept, keys);
+      base = compact_chunk<kListThreads>(j < n1 && made_nb[j] == i, j, base, warp_kept, keys);
     }
   if (list)
     for (int e = tid; e < base; e += kListThreads) {
@@ -500,8 +492,7 @@ void create_map_points_device(const Orb& left, const sivo_keyframe_keys& kf1, co
   for (int i = 0; i < n_nb; ++i) check_keys(nbs[i], true);
   const int cap = left.capacity();
   const MapParams p = make_params(left, kf1, nbs, n_nb, prm, cap, cap, false);
-  SIVO_CUDA(cudaSetDevice(left.device()));
-  if (!s) s = left.stream();
+  s = left.enter(s);
   // stream-ordered scratch of this call: LocalMapping runs it concurrently with Tracking's calls on the same extractor
   int* scratch = nullptr;
   SIVO_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&scratch), 2 * static_cast<size_t>(std::max(cap, 1)) * sizeof(int), s));
@@ -581,8 +572,7 @@ void keyframe_gather_device(const Orb& left, const sivo_keypoint* kps, const uin
                             const float* u_right, const float* depth, const uint8_t* cls, const double* conf, const double* ent,
                             sivo_keypoint* o_kps, uint8_t* o_desc, float* o_ur, float* o_depth, uint8_t* o_cls, double* o_conf,
                             double* o_ent, long long* o_count, cudaStream_t s) {
-  SIVO_CUDA(cudaSetDevice(left.device()));
-  if (!s) s = left.stream();
+  s = left.enter(s);
   const int cap = left.capacity();
   k_kf_gather<<<ceil_div(std::max(cap, 1), 256), 256, 0, s>>>(kps, reinterpret_cast<const uint4*>(desc), keep_idx, n_keep, cap, u_right, depth,
                                                               cls, conf, ent, o_kps, reinterpret_cast<uint4*>(o_desc), o_ur, o_depth, o_cls,

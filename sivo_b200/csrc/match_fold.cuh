@@ -1,3 +1,5 @@
+// The ORBmatcher rules shared by the matching kernels (stereo.cu, track.cu, bow.cu, mapping.cu).
+//
 // The best / second-best fold of ORBmatcher's candidate loops (SearchByProjection, ORBmatcher.cc:79-113 and :1352-1376), shared
 // by k_hamming_best2 (stereo.cu) and the projection searches (track.cu):
 //   for idx in candidates (in order): dist = DescriptorDistance(q, train[idx]);
@@ -7,6 +9,17 @@
 #include <cuda_runtime.h>
 
 namespace sivo {
+
+// ORBmatcher::DescriptorDistance (ORBmatcher.cc:1582-1596): the popcount of the XOR of two 256-bit descriptors (a0 a1, b0 b1)
+__device__ __forceinline__ int descriptor_distance(uint4 a0, uint4 a1, uint4 b0, uint4 b1) {
+  return __popc(a0.x ^ b0.x) + __popc(a0.y ^ b0.y) + __popc(a0.z ^ b0.z) + __popc(a0.w ^ b0.w) + __popc(a1.x ^ b1.x) +
+         __popc(a1.y ^ b1.y) + __popc(a1.z ^ b1.z) + __popc(a1.w ^ b1.w);
+}
+
+// The angle rule of the rotation histogram's searches: a key or point angle takes part only if it is finite and in [0, 360].
+// With both angles in range, rot is in [0, 360] and the rotation bin in 0..12, inside the 30-bin histogram; a NaN or infinite
+// angle, or one off by more than 360, would index outside it.
+__host__ __device__ __forceinline__ bool angle_ok(float a) { return a >= 0.f && a <= 360.f; }
 
 struct Best2 {
   int dist = 256, level = -1, idx = -1;    // bestDist, bestLevel, bestIdx

@@ -120,6 +120,12 @@ class Orb {
   int capacity() const { return sel_cap_; }
   bool device_tree() const { return device_tree_; }
   cudaStream_t stream() const { return stream_; }
+  // The start of a device-form call on this extractor's outputs: makes its device current and returns the stream to enqueue on,
+  // `s`, or stream() when `s` is NULL.
+  cudaStream_t enter(cudaStream_t s) const {
+    SIVO_CUDA(cudaSetDevice(device_));
+    return s ? s : stream_;
+  }
   // device copies of tables().scale / inv_scale, and capacity() ints of scratch for the device stereo form's SAD distances
   // (a frame's stereo call on this handle as the left extractor is ordered before its next enqueue_device, like the pyramid)
   const float* dev_scale() const { return d_scales_.as<float>(); }

@@ -3,6 +3,7 @@
 // per-cell threshold / 3x3 NMS / ordered compaction, 7x7 sigma-2 fixed-point blur, IC angle, rBRIEF.
 // Everything here is latency/launch bound on the GPU (~8 MB touched per image), so the design goal is few
 // launches over all 8 levels at once rather than bandwidth tricks.
+#include "block_ops.cuh"
 #include "orb.h"
 
 namespace sivo {
@@ -106,23 +107,6 @@ __device__ __forceinline__ int fast_score_at(const uint8_t* __restrict__ pyr, co
 constexpr int kCellThreads = 256;
 constexpr int kCellMaxDim = 62;  // interior side bound: wCell = ceil(width / floor(width/30)) <= 59
 
-__device__ int block_exclusive_scan(int flag, int* s_warp, int& total) {
-  unsigned b = __ballot_sync(0xffffffffu, flag);
-  int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  int within = __popc(b & ((1u << lane) - 1));
-  if (lane == 0) s_warp[wid] = __popc(b);
-  __syncthreads();
-  int base = 0, tot = 0;
-  for (int w = 0; w < kCellThreads / 32; ++w) {
-    int c = s_warp[w];
-    if (w < wid) base += c;
-    tot += c;
-  }
-  __syncthreads();
-  total = tot;
-  return base + within;
-}
-
 // The cell computes its own FAST scores from the pyramid (cell interiors tile the level without overlap, so no pixel is
 // scored twice and no score map is written and read back)
 __global__ void __launch_bounds__(kCellThreads) k_cells(const uint8_t* __restrict__ pyr, OrbLevelTable t,
@@ -191,7 +175,8 @@ __global__ void __launch_bounds__(kCellThreads) k_cells(const uint8_t* __restric
       }
     }
     int total;
-    int pos = written + block_exclusive_scan(flag, s_warp, total);
+    int pos = written + block_rank<kCellThreads>(flag, s_warp, &total);
+    __syncthreads();  // s_warp is rewritten by the next chunk
     if (flag && pos < kCellCap)
       out[pos] = static_cast<uint32_t>(relx + x) | (static_cast<uint32_t>(rely + y) << 12) | (static_cast<uint32_t>(v) << 24);
     written += total;

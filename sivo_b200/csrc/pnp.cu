@@ -13,6 +13,7 @@
 //                 not fit in registers, so k_pnp_hyp and k_pnp_decide use 255 registers with a few hundred bytes of spills.
 #include <cmath>
 
+#include "block_ops.cuh"
 #include "frame_ops.h"
 #include "host_call.h"
 #include "jacobi.cuh"
@@ -460,22 +461,6 @@ struct SetupParams {
   uint32_t kf_id[kPnpMaxCandidates];
 };
 
-// block-wide exclusive prefix of `flag` (blockDim.x threads, a multiple of 32); returns the block total
-__device__ __forceinline__ int block_scan(bool flag, int* pos, int* warp_tot) {
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  const unsigned b = __ballot_sync(0xffffffffu, flag);
-  __syncthreads();
-  if (lane == 0) warp_tot[w] = __popc(b);
-  __syncthreads();
-  int before = 0, total = 0;
-  for (int i = 0; i < nw; ++i) {
-    if (i < w) before += warp_tot[i];
-    total += warp_tot[i];
-  }
-  *pos = before + __popc(b & ((1u << lane) - 1u));
-  return total;
-}
-
 __global__ void __launch_bounds__(256) k_pnp_setup(const __grid_constant__ SetupParams p) {
   __shared__ int warp_tot[8];
   const int kf = blockIdx.x, cap = p.a.cap;
@@ -497,8 +482,9 @@ __global__ void __launch_bounds__(256) k_pnp_setup(const __grid_constant__ Setup
         valid = oct >= 0 && oct < p.nlevels;
       }
     }
-    int pos;
-    const int tot = block_scan(valid, &pos, warp_tot);
+    int tot;
+    __syncthreads();  // the previous chunk has read warp_tot
+    const int pos = block_rank<256>(valid, warp_tot, &tot);
     if (valid) {
       const size_t o = base + count + pos;
       const sivo_keypoint kp = p.kps[kidx];
@@ -625,7 +611,7 @@ __device__ void mtm_tree(const double* alphas, const double* us, int n, const Ca
         s = s + m_entry(a, u, v, k, 0, r) * m_entry(a, u, v, k, 0, c);
         s = s + m_entry(a, u, v, k, 1, r) * m_entry(a, u, v, k, 1, c);
       }
-      for (int off = 16; off > 0; off >>= 1) s = s + __shfl_xor_sync(0xffffffffu, s, off);
+      s = warp_tree_sum(s);
       if (lane == 0) sh.part[w][e] = s;
     }
   __syncthreads();
@@ -634,9 +620,9 @@ __device__ void mtm_tree(const double* alphas, const double* us, int n, const Ca
     int r = 0, c = t;
     while (c >= 12 - r) { c -= 12 - r; ++r; }
     c += r;
-    double q[4];
-    for (int i = 0; i < 4; ++i) q[i] = sh.part[i][t] + sh.part[i + 4][t];
-    const double v = (q[0] + q[2]) + (q[1] + q[3]);
+    double q[kDecideWarps];
+    for (int i = 0; i < kDecideWarps; ++i) q[i] = sh.part[i][t];
+    const double v = fold_warp_totals<kDecideWarps>(q);
     sh.mtm[r][c] = v;
     sh.mtm[c][r] = v;
   }
@@ -654,8 +640,9 @@ __device__ int block_pose(const PnpArrays& a, size_t base, int N, const uint32_t
   for (int i0 = 0; i0 < N; i0 += blockDim.x) {
     const int i = i0 + threadIdx.x;
     const bool in = i < N && ((sel[i >> 5] >> (i & 31)) & 1u);
-    int pos;
-    const int tot = block_scan(in, &pos, sh.warp_tot);
+    int tot;
+    __syncthreads();  // the previous chunk has read sh.warp_tot
+    const int pos = block_rank<kDecideThreads>(in, sh.warp_tot, &tot);
     if (in) {
       const size_t o = base + i;
       const int d = count + pos;
@@ -824,8 +811,7 @@ void pnp_setup_device(Pnp& h, const sivo_keypoint* kps, const int* keep_idx, con
   if (n_kf > 0 && !kf_id) fail(SIVO_EINVAL, "pnp_setup: null kf_id");
   if (!(std::isfinite(fx) && std::isfinite(fy) && std::isfinite(cx) && std::isfinite(cy)))
     fail(SIVO_EINVAL, "pnp_setup: camera parameters not finite");
-  SIVO_CUDA(cudaSetDevice(h.device));
-  if (!s) s = h.left->stream();
+  s = h.left->enter(s);
   h.n_kf = n_kf;
   h.frame_id = frame_id;
   h.cam = Cam{fx, fy, cx, cy};
@@ -851,8 +837,7 @@ void pnp_setup_device(Pnp& h, const sivo_keypoint* kps, const int* keep_idx, con
 void pnp_iterate_device(Pnp& h, int n_iterations, const uint8_t* active, float* Tcw, int* has_pose, int* no_more, int* inlier_match,
                         int* n_inliers, cudaStream_t s) {
   if (h.n_kf > 0 && !active) fail(SIVO_EINVAL, "pnp_iterate: null active");
-  SIVO_CUDA(cudaSetDevice(h.device));
-  if (!s) s = h.left->stream();
+  s = h.left->enter(s);
   IterParams p{};
   for (int k = 0; k < h.n_kf; ++k)
     if (active[k]) p.act[p.n_act++] = k;

@@ -13,6 +13,7 @@
 #include <cfloat>
 #include <cmath>
 
+#include "block_ops.cuh"
 #include "frame_ops.h"
 #include "host_call.h"
 
@@ -36,11 +37,6 @@ struct PoseEdge {  // one edge, in semantic-key order (80 bytes)
 struct DPose { double q[4], t[3]; };  // SE3Quat: q = (x, y, z, w)
 
 size_t edges_bytes(int cap) { return static_cast<size_t>(std::max(cap, 1)) * sizeof(PoseEdge); }
-
-__device__ __forceinline__ int clamp_count(const long long* n_keep, int cap) {
-  const long long n = *n_keep;
-  return n < 0 ? -1 : static_cast<int>(min(n, static_cast<long long>(cap)));
-}
 
 // ---- SE3Quat and Eigen 3's quaternion formulas
 __device__ void normalize_rotation(double* q) {
@@ -238,15 +234,13 @@ __device__ __forceinline__ void add_terms(const PoseEdge& E, const EdgeEval& o, 
   acc[27] = acc[27] + o.rho0;
 }
 
-// The fixed reduction tree: per-thread sums (above), xor shuffles within each warp (16, 8, 4, 2, 1), then the 8 warp totals
-// folded as w[i] + w[i + s] for s = 4, 2, 1.  out[q] is valid after the call (it ends with __syncthreads).
+// The fixed reduction tree (block_ops.cuh) over the per-thread sums (above).  out[q] is valid after the call (it ends with
+// __syncthreads).
 template <int M>
 __device__ void pose_reduce(double (&v)[M], double (*sh)[kTerms], double* out) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 #pragma unroll
-  for (int s = 16; s; s >>= 1)
-#pragma unroll
-    for (int q = 0; q < M; ++q) v[q] = v[q] + __shfl_xor_sync(0xffffffffu, v[q], s);
+  for (int q = 0; q < M; ++q) v[q] = warp_tree_sum(v[q]);
   if (lane == 0)
 #pragma unroll
     for (int q = 0; q < M; ++q) sh[warp][q] = v[q];
@@ -254,9 +248,7 @@ __device__ void pose_reduce(double (&v)[M], double (*sh)[kTerms], double* out) {
   if (threadIdx.x < M) {
     double w[kWarps];
     for (int i = 0; i < kWarps; ++i) w[i] = sh[i][threadIdx.x];
-    for (int s = kWarps / 2; s; s >>= 1)
-      for (int i = 0; i < s; ++i) w[i] = w[i] + w[i + s];
-    out[threadIdx.x] = w[0];
+    out[threadIdx.x] = fold_warp_totals<kWarps>(w);
   }
   __syncthreads();
 }
@@ -334,6 +326,8 @@ __device__ int build_edges(const PoseParams& p, const sivo_keypoint* __restrict_
         }
       }
     }
+    // block_rank (block_ops.cuh) written out with `warp` computed once, outside the loop: on block_rank, which computes it per
+    // chunk, k_pose_optimize needs two more registers
     const unsigned m = __ballot_sync(0xffffffffu, ok);
     if (lane == 0) warp_count[warp] = __popc(m);
     __syncthreads();
@@ -434,7 +428,7 @@ __global__ void __launch_bounds__(kThreads, 1)
   uint8_t* outlier = outlier_all ? outlier_all + static_cast<size_t>(prob) * cap : nullptr;
   sivo_pose_result* res = results + prob;
   const int tid = threadIdx.x;
-  const int n = clamp_count(n_keep + prob, cap);
+  const int n = clamp_count(n_keep[prob], cap);
   if (n < 0) {
     if (tid == 0) res->n_good = -1;
     return;
@@ -609,7 +603,7 @@ __global__ void __launch_bounds__(kThreads, 1)
 
 __global__ void k_pose_gather(const int* __restrict__ match, const long long* __restrict__ n_keep, int cap,
                               const sivo_map_point* __restrict__ pts, int n_points, float* __restrict__ xw) {
-  const int n = clamp_count(n_keep, cap);
+  const int n = clamp_count(*n_keep, cap);
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= n) return;
   const int m = match[j];
@@ -647,8 +641,7 @@ void pose_optimize_device(const Orb& left, const sivo_keypoint* kps, const int* 
                           const float* xw, float fx, float fy, float cx, float cy, float mbf, const float* Tcw_in,
                           sivo_pose_result* result, uint8_t* outlier, cudaStream_t s) {
   const PoseParams p = make_params(left, fx, fy, cx, cy, mbf);
-  SIVO_CUDA(cudaSetDevice(left.device()));
-  if (!s) s = left.stream();
+  s = left.enter(s);
   const int cap = left.capacity();
   PoseEdge* edges = reinterpret_cast<PoseEdge*>(const_cast<Orb&>(left).track_scratch(edges_bytes(cap), s));
   launch_optimize(p, kps, keep_idx, n_keep, cap, u_right, xw, Tcw_in, edges, result, outlier, s);
@@ -657,8 +650,7 @@ void pose_optimize_device(const Orb& left, const sivo_keypoint* kps, const int* 
 void pose_gather_device(const Orb& left, const int* match, const long long* n_keep, const sivo_map_point* pts, int n_points, float* xw,
                         cudaStream_t s) {
   if (n_points < 0) fail(SIVO_EINVAL, "pose_gather: n_points = %d", n_points);
-  SIVO_CUDA(cudaSetDevice(left.device()));
-  if (!s) s = left.stream();
+  s = left.enter(s);
   const int cap = left.capacity();
   k_pose_gather<<<ceil_div(std::max(cap, 1), kThreads), kThreads, 0, s>>>(match, n_keep, cap, pts, n_points, xw);
   SIVO_CUDA(cudaGetLastError());

@@ -4,7 +4,7 @@
 #include <cuda_fp16.h>
 
 #include "common.h"
-#include "compact.cuh"
+#include "block_ops.cuh"
 #include "philox.cuh"
 #include "segnet_kernels.h"
 
@@ -727,7 +727,7 @@ __global__ void __launch_bounds__(kSemThreads) k_semantic_keys(const sivo_keypoi
     return;
   }
   const int n = static_cast<int>(n64);
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int tid = threadIdx.x;
   int base = 0;  // kept keys in the chunks before this one (the same value in every thread)
   for (int c0 = 0; c0 < n; c0 += kSemThreads) {
     const int i = c0 + tid;
@@ -743,7 +743,7 @@ __global__ void __launch_bounds__(kSemThreads) k_semantic_keys(const sivo_keypoi
       if (out_ent) out_ent[i] = ok ? ent[o] : 0.0;
       keep = c != 255 && static_cast<int>(c) <= max_static_class;  // `detection <= Classes::TERRAIN` (Frame.cc:190)
     }
-    base = compact_chunk<kSemThreads>(keep, i, base, lane, warp, warp_kept, keep_idx);
+    base = compact_chunk<kSemThreads>(keep, i, base, warp_kept, keep_idx);
   }
   if (tid == 0 && n_keep) *n_keep = base;
 }

@@ -399,8 +399,7 @@ void stereo_match_device(Orb& left, Orb& right, const sivo_keypoint* kl, const u
   if (!(mb > 0.f) || !(mbf > 0.f)) fail(SIVO_EINVAL, "stereo: bad arguments");
   // the Hamming search packs a right index into 20 bits
   if (right.capacity() >= (1 << 20)) fail(SIVO_EINVAL, "stereo: right extractor capacity %d needs more than 20 index bits", right.capacity());
-  SIVO_CUDA(cudaSetDevice(left.device()));
-  if (!s) s = left.stream();
+  s = left.enter(s);
   left.stream_wait(s);
   right.stream_wait(s);
   launch_stereo(left, right, kl, dl, keep_idx, n_left, left.capacity(), kr, dr, n_right, right.capacity(), mb, mbf, u_right, depth,

@@ -16,6 +16,7 @@
 //                      last-frame search then runs the rotation histogram and ComputeThreeMaxima.
 #include <cmath>
 
+#include "block_ops.cuh"
 #include "frame_ops.h"
 #include "host_call.h"
 #include "match_fold.cuh"
@@ -87,16 +88,6 @@ TrackBufs carve(uint8_t* base, int cap, int np) {
   return b;
 }
 
-// The angle rule: a key or point angle takes part only if it is finite and in [0, 360].  With both angles in range, rot is in
-// [0, 360] and the rotation bin in 0..12, inside hist_count; a NaN or infinite angle, or one off by more than 360, would index
-// outside it.
-__host__ __device__ __forceinline__ bool angle_ok(float a) { return a >= 0.f && a <= 360.f; }
-
-__device__ __forceinline__ int clamp_count(const long long* n_keep, int cap) {
-  const long long n = *n_keep;
-  return n < 0 ? -1 : static_cast<int>(min(n, static_cast<long long>(cap)));
-}
-
 // ---- grid
 __global__ void __launch_bounds__(kGridThreads, 1) k_track_grid(const TrackParams p, const sivo_keypoint* __restrict__ kps,
                                                                 const uint8_t* __restrict__ desc, const int* __restrict__ keep_idx,
@@ -104,7 +95,7 @@ __global__ void __launch_bounds__(kGridThreads, 1) k_track_grid(const TrackParam
                                                                 const float* __restrict__ u_right, TrackBufs b) {
   __shared__ int cnt[kCells];
   __shared__ int warp_sum[kGridThreads / 32];
-  const int n = clamp_count(n_keep, cap);
+  const int n = clamp_count(*n_keep, cap);
   if (n < 0) return;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   for (int c = tid; c < kCells; c += kGridThreads) cnt[c] = 0;
@@ -221,8 +212,7 @@ __device__ __forceinline__ Best2 search_window(const TrackParams& p, const Track
       const TrackKey k = b.keys[j];
       if (!(k.ur > 0.f && fabsf(w.xr - k.ur) > w.rad)) {
         const uint4 t0 = b.desc[2 * j], t1 = b.desc[2 * j + 1];
-        d = __popc(q0.x ^ t0.x) + __popc(q0.y ^ t0.y) + __popc(q0.z ^ t0.z) + __popc(q0.w ^ t0.w) + __popc(q1.x ^ t1.x) +
-            __popc(q1.y ^ t1.y) + __popc(q1.z ^ t1.z) + __popc(q1.w ^ t1.w);
+        d = descriptor_distance(q0, q1, t0, t1);
         lvl = k.octave;
       }
     }
@@ -326,7 +316,7 @@ __global__ void __launch_bounds__(32) k_track_ordered(const TrackParams p, const
   __shared__ int hist_count[kHisto];
   uint8_t* blocked = reinterpret_cast<uint8_t*>(owner + cap);
   const int lane = threadIdx.x;
-  const int n = clamp_count(n_keep, cap);
+  const int n = clamp_count(*n_keep, cap);
   if (n < 0) {
     if (lane == 0 && n_matches) *n_matches = -1;
     return;
@@ -527,8 +517,7 @@ void search_device(const Orb& left, bool last, const sivo_keypoint* kps, const u
   p.nnratio = nnratio;
   p.last_frame = last;
   if (last) last_frame_direction(p, f, Rlw, tlw);
-  SIVO_CUDA(cudaSetDevice(left.device()));
-  if (!s) s = left.stream();
+  s = left.enter(s);
   const int cap = left.capacity();
   const TrackBufs b = carve(const_cast<Orb&>(left).track_scratch(scratch_bytes(cap, n_points), s), cap, n_points);
   launch_search(p, kps, desc, keep_idx, n_keep, cap, u_right, blocked, pts, n_points, b, in_view, match, n_matches, s);
