@@ -35,37 +35,12 @@ def run_host(left, kf1, nbs, debug=True, **kw):
     return create_map_points(left, host_kf(kf1), [host_kf(k) for k in nbs], params(**kw), debug=debug)
 
 
-def compare(got, want, th_red=TH_RED, max_exempt=5):
-    """Bit-identical, except that a (neighbour, key) decision may differ where the oracle's reduction lies within 1e-12 of the
-    threshold (log2) or a decision reading cos(2 atan2(...)) is within 2 float ulps of flipping; such a key is left out of every
-    comparison from that pair on, and the number of such keys must stay small.  Returns the number of exempt keys."""
-    red_g, red_w = got["reduction"], want["reduction"]
-    with np.errstate(invalid="ignore"):
-        near = (np.abs(red_w - np.float64(np.float32(th_red))) < 1e-12) | (want["parallax_ulps"] <= 2)
-    exempt_key = near.any(axis=0)
-    assert exempt_key.sum() <= max_exempt
-    ok = ~exempt_key
-    both = ~np.isnan(red_w[:, ok])
-    assert np.array_equal(np.isnan(red_g[:, ok]), ~both)
-    np.testing.assert_allclose(red_g[:, ok][both], red_w[:, ok][both], rtol=0, atol=1e-12)
-    np.testing.assert_array_equal(got["stage"][:, ok], want["stage"][:, ok])
-    np.testing.assert_array_equal(got["match"][:, ok], want["match"][:, ok])
-    np.testing.assert_array_equal(got["created_nb"][ok], want["created_nb"][ok])
-    np.testing.assert_array_equal(got["created_idx"][ok], want["created_idx"][ok])
-    np.testing.assert_array_equal(got["world"][ok].view(np.uint32), want["world"][ok].view(np.uint32))
-    keep = lambda lst: lst[ok[lst[:, 1]]] if len(lst) else lst
-    np.testing.assert_array_equal(keep(got["created"]), keep(want["created"]))
-    if not exempt_key.any():
-        assert got["n_created"] == len(want["created"])
-    return int(exempt_key.sum())
-
-
 @pytest.mark.parametrize("n_nb", [1, 3, 10])
 def test_scene_matches_oracle(left, n_nb):
     kf1, nbs = S.make_scene(2000, n_nb, seed=n_nb)
     want = S.oracle_run(kf1, nbs, TH_CONF, TH_RED, MAX_CLASS)
     got = run_host(left, kf1, nbs)
-    compare(got, want)
+    S.compare(got, want)
     assert want["stage"].max() == MO.CREATED and len(want["created"]) > 100
     # the production path (no per-key search for keys its criteria rule out) creates the same points
     prod = run_host(left, kf1, nbs, debug=False)
@@ -80,7 +55,7 @@ def test_baseline_and_points_on_entry(left):
     kf1.has_point[:50] = 1
     want = S.oracle_run(kf1, nbs)
     got = run_host(left, kf1, nbs)
-    compare(got, want)
+    S.compare(got, want)
     assert (got["stage"][1] == MO.BASELINE).all()
     assert (got["stage"][0, :50] == MO.HAS_POINT).all()
     made0 = np.flatnonzero(got["stage"][0] == MO.CREATED)
@@ -92,7 +67,7 @@ def test_thresholds_move_decisions(left):
     for th_conf, th_red in ((0.0, -1e9), (1.5, 0.0), (0.5, float("inf"))):
         want = MO.create_new_map_points(kf1, nbs, S.camera(), S.TABLES.scale, S.TABLES.sigma2, np.float32(1.2), S.sigma_cw(), MAX_CLASS,
                                         th_conf, th_red)
-        compare(run_host(left, kf1, nbs, th_conf=th_conf, th_red=th_red), want, th_red)
+        S.compare(run_host(left, kf1, nbs, th_conf=th_conf, th_red=th_red), want, th_red)
 
 
 def test_nan_reduction_passes(left):
@@ -101,7 +76,7 @@ def test_nan_reduction_passes(left):
     kf1.kp_entropy[::2] = np.nan
     want = S.oracle_run(kf1, nbs)
     got = run_host(left, kf1, nbs)
-    compare(got, want)
+    S.compare(got, want)
     made = got["created_nb"] >= 0
     assert made.any() and np.all(np.isnan(kf1.kp_entropy[made]))
 
@@ -115,7 +90,7 @@ def test_empty_and_negative_counts(left):
                     Rcw=kf1.Rcw, tcw=kf1.tcw)
     assert run_host(left, e, nbs)["n_created"] == 0
     r = run_host(left, kf1, [e] + nbs[1:])
-    compare(r, S.oracle_run(kf1, [e] + nbs[1:]))
+    S.compare(r, S.oracle_run(kf1, [e] + nbs[1:]))
     neg = create_map_points(left, host_kf(kf1), [host_kf(nbs[0], count=-1)], params())
     assert neg["n_created"] == -1
 
@@ -282,7 +257,7 @@ def test_geometric_threshold_at_its_flip(left, name):
     got, want = _run_device_dbg_equal(left, kf1, [kf2], 0.5, -1e9)
     st = want["stage"][0]
     assert (st[1] == reject) != (st[2] == reject) and (st[0] == st[1]) and (st[2] == st[3])
-    assert compare(got, want, -1e9, max_exempt=0) == 0
+    assert S.compare(got, want, -1e9, max_exempt=0) == 0
 
 
 def test_confidence_at_its_threshold(left):
@@ -292,7 +267,7 @@ def test_confidence_at_its_threshold(left):
     kf1.kp_conf[:] = [np.nextafter(eq, 0), eq, np.nextafter(eq, 1), float(np.nextafter(th, np.float32(0))), float(np.nextafter(th, np.float32(1)))]
     got, want = _run_device_dbg_equal(left, kf1, [kf2], th_conf=float(th), th_red=-1e9)
     assert list(want["stage"][0]) == [MO.SEMANTIC, MO.CREATED, MO.CREATED, MO.SEMANTIC, MO.CREATED]
-    assert compare(got, want, -1e9, max_exempt=0) == 0
+    assert S.compare(got, want, -1e9, max_exempt=0) == 0
 
 
 def test_entropy_reduction_at_its_threshold(left):
@@ -306,7 +281,7 @@ def test_entropy_reduction_at_its_threshold(left):
     red = want["reduction"][0]
     assert (red < float(th)).any() and (red >= float(th)).any()
     assert want["stage"][0, 5] == MO.SEMANTIC and want["stage"][0, 6] == MO.CREATED
-    assert compare(got, want, float(th), max_exempt=5) <= 5  # the keys within 1e-12 of the threshold are the log2 exemption
+    assert S.compare(got, want, float(th), max_exempt=5) <= 5  # the keys within 1e-12 of the threshold are the log2 exemption
 
 
 def test_ties_take_the_later_candidate_and_duplicates_match_twice(left):
@@ -317,7 +292,7 @@ def test_ties_take_the_later_candidate_and_duplicates_match_twice(left):
     got, want = _run_device_dbg_equal(left, kf1, [kf2], th_red=-1e9)
     assert (want["match"][0] == 2).all()  # equal distances: the later candidate; every current key matches neighbour key 2
     assert (want["stage"][0] == MO.CREATED).all()
-    assert compare(got, want, -1e9, max_exempt=0) == 0
+    assert S.compare(got, want, -1e9, max_exempt=0) == 0
 
 
 def test_epipole_gate_and_the_second_keyframes_stereo_branch(left):
@@ -335,12 +310,12 @@ def test_epipole_gate_and_the_second_keyframes_stereo_branch(left):
         kf1.kps["y"][i] = np.float32(S.CY)
     got, want = _run_device_dbg_equal(left, kf1, [kf2], th_red=-1e9)
     assert list(want["match"][0]) == [-1, 1, 2]  # inside the gate; outside it; inside only a squared-scale gate
-    assert compare(got, want, -1e9, max_exempt=0) == 0
+    assert S.compare(got, want, -1e9, max_exempt=0) == 0
     k1, k2 = S.pair_scene([S.P0] * 2, stereo1=False, stereo2=True, o2=3)
     got, want = _run_device_dbg_equal(left, k1, [k2], th_red=-1e9)
     assert (want["stage"][0] == MO.CREATED).all()
     assert np.array_equal(want["world"][0], MO.unproject(k2, 0, S.camera()))
-    assert compare(got, want, -1e9, max_exempt=0) == 0
+    assert S.compare(got, want, -1e9, max_exempt=0) == 0
 
 
 BOUNDARY = {}

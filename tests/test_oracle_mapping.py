@@ -1,5 +1,6 @@
 """CPU: oracle/mapping_oracle.py -- its cv::Mat forms pinned against cv2, the triangulation rule against cv2.SVDecomp and a float64
 SVD, and hand-built cases for the reference facts it keeps."""
+import copy
 import math
 
 import cv2
@@ -199,3 +200,50 @@ def test_nan_reduction_passes():
     r = S.oracle_run(kf1, nbs)
     made = r["stage"] == MO.CREATED
     assert made.any() and np.isnan(r["reduction"][made]).all()
+
+
+@pytest.fixture(scope="module")
+def constructed():
+    return [(sc, sc.run()) for sc in S.constructed_scenes()]
+
+
+def test_constructed_pairs_end_where_they_say(constructed):
+    for sc, r in constructed:
+        for k, st in sc.want.items():
+            assert r["stage"][k] == st, (sc.name, k, int(r["stage"][k]), st)
+        for k, m in sc.match.items():
+            assert r["match"][k] == m, (sc.name, k, int(r["match"][k]), m)
+        if sc.flip is not None:  # one ulp apart, pairs 1 and 2 fall on either side of the flip
+            st = r["stage"][0]
+            assert (st[1] == sc.flip) != (st[2] == sc.flip) and st[0] == st[1] and st[2] == st[3], (sc.name, st)
+
+
+def test_constructed_scenes_reach_every_stage(constructed):
+    """Every stage of the rule is reached by some constructed pair, none named unreachable: W_ZERO needs a pose that is not a
+    rotation (the `w_zero` scene) and dist == 0 a camera centre that is not -Rcw^T tcw (`dist_zero`); with true poses neither
+    can happen (the reasons are in oracle/mapping_scene.py)."""
+    reached = {int(s) for _, r in constructed for s in np.unique(r["stage"])}
+    assert reached == set(range(MO.CREATED + 1))
+    by = {sc.name: (sc, r) for sc, r in constructed}
+    # dist_zero's SCALE is the dist1 == 0 branch: with the current keyframe's centre put back, the same pair creates the point
+    # that the scene's centre sits on
+    sc, _ = by["dist_zero"]
+    kf1 = copy.copy(sc.kf1)
+    kf1.Ow = np.zeros(3, F32)  # the current keyframe of a pair scene sits at the origin
+    back = S.oracle_run(kf1, sc.nbs, sc.th_conf, sc.th_red)
+    assert back["stage"][0, 0] == MO.CREATED and np.array_equal(back["world"][0], sc.kf1.Ow)
+    # the epipole gate at octave 0 sits on distex^2 == 100 exactly
+    sc, _ = by["epipole_o0"]
+    assert (F32(S.CX) - sc.nbs[0].kps["x"][1]) ** 2 == F32(100)
+    # the 4-level 1.5x extractor: ratioFactor 2.25, a key at octave nlevels (4) left out
+    sc, r = by["four_levels"]
+    assert F32(1.5) * F32(sc.ext.scale_factor) == F32(2.25) and sc.ext.nlevels == 4
+
+
+def test_stereo_min_keeps_the_rays_cosine_over_a_nan_stereo_cosine():
+    """std::min(cosParallaxStereo1, cosParallaxStereo2) is (b < a) ? b : a: a NaN stereo cosine of the neighbour key gives
+    cosParallaxRays + 1, so a mono current key against a stereo neighbour key at depth NaN triangulates its rays."""
+    k1, k2 = S.pair_scene([S.P0], stereo1=False, stereo2=True, o2=3)
+    k2.depth[0] = np.nan
+    st, x3, _, _ = MO.triangulate_pair(k1, 0, k2, 0, S.camera(), S.TABLES.scale, S.TABLES.sigma2, F32(1.2), S.sigma_cw(), 8, 0.5, -1e9)
+    assert st == MO.CREATED and np.isfinite(x3).all()
