@@ -20,7 +20,10 @@
  * across the boundary; sivo_last_error() returns a thread-local message for the last failure on the
  * calling thread.  Pointers are plain host pointers unless the name says `_device`.  Handles are
  * independent: two sivo_orb_t may be driven concurrently from two threads (Frame.cc:126-129); one handle
- * must not be used from two threads at once.
+ * must not be used from two threads at once.  A `_device` call's scratch is its own: allocated and freed on its `stream`
+ * (stream-ordered, no host synchronisation), never on an extractor.  So calls on different streams share only the buffers they
+ * are given, and a call's inputs (e.g. the keypoints the next sivo_orb_enqueue_device into the same buffers rewrites) must not be
+ * rewritten until it has run.
  */
 #ifndef SIVO_B200_H_
 #define SIVO_B200_H_
@@ -271,9 +274,8 @@ int sivo_stereo_match(const sivo_orb_t* left, const sivo_orb_t* right, const siv
  * octave is outside [0, nlevels) are left unmatched.
  * Ordering: the call makes `stream` (NULL = the left extractor's stream) wait for everything enqueued so far on both extractors'
  * streams, so no manual wait is needed after sivo_orb_enqueue_device; keep_idx / n_keep must be ordered before it on `stream`.  The
- * call reads both pyramids and writes the left extractor's SAD scratch, so the next sivo_orb_enqueue_device on either extractor
- * must be ordered after it (sivo_orb_wait_for_stream(extractor, stream)), and calls that share a left extractor must be ordered
- * among themselves.  No host synchronisation.  SIVO_EINVAL for NULL handles or buffers (keep_idx_device may be NULL), extractors
+ * call reads both pyramids, so the next sivo_orb_enqueue_device on either extractor must be ordered after it
+ * (sivo_orb_wait_for_stream(extractor, stream)).  No host synchronisation.  SIVO_EINVAL for NULL handles or buffers (keep_idx_device may be NULL), extractors
  * that have not run, extractors on different devices, with different nlevels or different level tables, mb / mbf <= 0, and a right
  * extractor whose sivo_orb_capacity is >= 2^20; nothing is enqueued then.  Keys follow sivo_stereo_match's rule. */
 int sivo_stereo_match_device(sivo_orb_t* left, sivo_orb_t* right, const sivo_keypoint* kp_left_device, const uint8_t* desc_left_device,
@@ -316,9 +318,8 @@ int sivo_info_select(const sivo_orb_t* left, const sivo_keypoint* kps, const flo
  * *n_keep_device (int64) is read on the device and clamped to the capacity; a negative count (the -1 of
  * sivo_segnet_semantic_keys_device) writes nothing except *n_selected_device = -1.  A key index outside the capacity is invalid.
  * Ordering: runs on `stream` (NULL = the left extractor's stream) with no host synchronisation and no waits of its own, so every
- * input must be ordered before it on `stream` (on the Frame tail's stream they are).  The per-key decisions go to scratch on the
- * left extractor, so calls that share a left extractor must be ordered among themselves, and its next sivo_orb_enqueue_device
- * must be ordered after this call (sivo_orb_wait_for_stream(left, stream) after it). */
+ * input must be ordered before it on `stream` (on the Frame tail's stream they are), and the next sivo_orb_enqueue_device into
+ * kps_device after it (sivo_orb_wait_for_stream(left, stream)). */
 int sivo_info_select_device(const sivo_orb_t* left, const sivo_keypoint* kps_device, const double* kp_entropy_device,
                             const int* keep_idx_device, const long long* n_keep_device, const float* depth_device,
                             const sivo_info_camera* cam, double threshold, float* world_device, double* reduction_device,
@@ -393,8 +394,7 @@ typedef struct sivo_map_point {            /* 80 bytes, one per map point */
  * sivo_orb_capacity(left)) = the point this call gave key j, or -1; *n_matches_device (int64) = SearchByProjection's return.
  * *n_keep_device is clamped to the capacity; a negative count writes only *n_matches_device = -1.  A key index outside the
  * capacity is in no cell.  Runs on `stream` (NULL = the left extractor's stream) with no waits of its own and no host
- * synchronisation.  Scratch lives on the left extractor: calls sharing it must be ordered among themselves and before its next
- * sivo_orb_enqueue_device.  SIVO_EINVAL for NULL handles or inputs, n_points < 0, th <= 0, nnratio not finite, or max <= min in
+ * synchronisation.  SIVO_EINVAL for NULL handles or inputs, n_points < 0, th <= 0, nnratio not finite, or max <= min in
  * the bounds. */
 int sivo_search_local_points_device(const sivo_orb_t* left, const sivo_keypoint* kps_device, const uint8_t* desc_device,
                                     const int* keep_idx_device, const long long* n_keep_device, const float* u_right_device,
@@ -466,9 +466,7 @@ typedef struct sivo_pose_result {
  * the reference leaves mvbOutlier as the caller had it, so the buffer is the call's whole output.  A key index outside the capacity, or a key with an octave outside the extractor's levels, has no edge.  The count is
  * clamped to the capacity; a negative count (the -1 of sivo_segnet_semantic_keys_device) writes only result_device->n_good =
  * -1.  One block runs the whole optimisation.  Runs on `stream` (NULL = the left extractor's stream) with no waits of its own
- * and no host synchronisation; the edges live in the left extractor's projection-search scratch, so calls sharing it (both
- * searches included) must be ordered among themselves and before its next sivo_orb_enqueue_device.  SIVO_EINVAL for NULL
- * handles or inputs, or fx, fy, mbf not finite and positive, cx, cy not finite. */
+ * and no host synchronisation.  SIVO_EINVAL for NULL handles or inputs, or fx, fy, mbf not finite and positive, cx, cy not finite. */
 int sivo_pose_optimize_device(const sivo_orb_t* left, const sivo_keypoint* kps_device, const int* keep_idx_device,
                               const long long* n_keep_device, const float* u_right_device, const float* xw_device, float fx, float fy,
                               float cx, float cy, float mbf, const float* Tcw_in_device, sivo_pose_result* result_device,
@@ -555,9 +553,8 @@ int sivo_keyframe_gather_device(const sivo_orb_t* left, const sivo_keypoint* kps
  * world_device[3 j ..] = the point (NaN when none); created_list_device[2 e ..] = (neighbour, key j) of the e-th point created, in
  * the reference's order (neighbour-major, j ascending: mlpRecentAddedMapPoints); *n_created_device (int64) its length.  Counts are
  * clamped to the capacity; a negative count (the -1 of sivo_segnet_semantic_keys_device) in any keyframe writes only
- * *n_created_device = -1.  Runs on `stream` (NULL = the left extractor's stream) with no waits and no host synchronisation.  Its
- * scratch is allocated and freed on `stream` (stream-ordered), never on the extractor, and it reads only the extractor's scale
- * tables: LocalMapping's thread may run it concurrently with Tracking's calls on the same extractor.  SIVO_EINVAL for NULL
+ * *n_created_device = -1.  Runs on `stream` (NULL = the left extractor's stream) with no waits and no host synchronisation.  It
+ * reads only the extractor's scale tables: LocalMapping's thread may run it concurrently with Tracking's calls on the same extractor.  SIVO_EINVAL for NULL
  * handles or inputs, n_neighbours outside [0, 32]. */
 int sivo_create_map_points_device(const sivo_orb_t* left, const sivo_keyframe_keys* kf1, const sivo_keyframe_keys* neighbours,
                                   int n_neighbours, const sivo_mapping_params* params, int* created_nb_device,
@@ -635,9 +632,8 @@ int sivo_dbg_vocabulary_parse(const char* path, int* header, int* n_nodes, int32
  * mBowVec as ascending word ids and double weights (capacity room), *bow_len_device (int64) its length.  The count is clamped to
  * the capacity; a negative count (the -1 of sivo_segnet_semantic_keys_device) writes only *bow_len_device = -1.  A key index
  * outside the capacity gives node and word -1.  The same call computes KeyFrame::ComputeBoW on sivo_keyframe_gather_device's copy
- * (keep_idx NULL).  Runs on `stream` (NULL = the left extractor's stream) with no waits and no host synchronisation; its scratch
- * is allocated and freed on `stream` (stream-ordered) and it reads only the vocabulary and its inputs, so LocalMapping's thread may
- * run it concurrently with Tracking's calls on the same extractor.  SIVO_EINVAL for NULL handles or inputs, levelsup < 0, or a
+ * (keep_idx NULL).  Runs on `stream` (NULL = the left extractor's stream) with no waits and no host synchronisation; it reads
+ * only the vocabulary and its inputs, so LocalMapping's thread may run it concurrently with Tracking's calls on the same extractor.  SIVO_EINVAL for NULL handles or inputs, levelsup < 0, or a
  * vocabulary on another device; SIVO_ERANGE for an extractor capacity above 16,384 keys (the BowVector is sorted in shared memory). */
 int sivo_compute_bow_device(const sivo_vocabulary_t* voc, const sivo_orb_t* left, const uint8_t* desc_device, const int* keep_idx_device,
                             const long long* n_keep_device, int levelsup, int* node_device, int* word_device, int* bow_word_device,
@@ -672,8 +668,7 @@ int sivo_compute_bow(const sivo_vocabulary_t* voc, const uint8_t* desc, int n, i
  * keyframe k's search gave frame key j, or -1 (so sivo_pose_gather_device takes match_device + k cap); n_matches_device[k] (int64)
  * = the function's return.  Counts are clamped to the capacity; a negative count in the frame or in keyframe k writes only
  * n_matches_device[k] = -1 for every affected k.  Runs on `stream` (NULL = the left extractor's stream) with no waits and no host
- * synchronisation; its scratch is allocated and freed on `stream` (stream-ordered), never on the extractor.  SIVO_EINVAL for NULL
- * handles, inputs or outputs, n_kf < 0, or nnratio not finite; SIVO_ERANGE for a capacity above 16,384 keys. */
+ * synchronisation.  SIVO_EINVAL for NULL handles, inputs or outputs, n_kf < 0, or nnratio not finite; SIVO_ERANGE for a capacity above 16,384 keys. */
 int sivo_search_by_bow_device(const sivo_orb_t* left, const sivo_keypoint* kps_device, const uint8_t* desc_device,
                               const int* keep_idx_device, const long long* n_keep_device, const int* node_device,
                               const sivo_keyframe_keys* keyframes, const int* const* kf_point_device, int n_kf, float nnratio,
@@ -739,8 +734,7 @@ int sivo_pnp_setup_device(sivo_pnp_t* h, const sivo_keypoint* kps_device, const 
 /* iterate(n_iterations) on every candidate k of the last setup with active[k] != 0 (host array; the others are neither run nor
  * written).  Per active k: Tcw_device[12 k ..] (3 x 4 row-major, usable as sivo_pose_optimize_device's Tcw_in) when
  * has_pose_device[k]; no_more_device[k]; n_inliers_device[k]; inlier_match_device[k cap + j] = match[k cap + j] for the
- * inliers, -1 for every other j < cap (the row that becomes mvpMapPoints).  Scratch is allocated and freed on `stream`
- * (stream-ordered), never on the extractor.  SIVO_EINVAL for NULL handles or outputs. */
+ * inliers, -1 for every other j < cap (the row that becomes mvpMapPoints).  SIVO_EINVAL for NULL handles or outputs. */
 int sivo_pnp_iterate_device(sivo_pnp_t* h, int n_iterations, const uint8_t* active, float* Tcw_device, int* has_pose_device,
                             int* no_more_device, int* inlier_match_device, int* n_inliers_device, void* stream);
 /* Test hooks.  sivo_dbg_pnp_state synchronises the device, then per candidate of the last setup: out[7 k ..] = N, minInliers,

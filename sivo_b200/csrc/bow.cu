@@ -19,6 +19,7 @@
 #include "block_ops.cuh"
 #include "host_call.h"
 #include "match_fold.cuh"
+#include "stream_scratch.h"
 #include "vocabulary.h"
 
 namespace sivo {
@@ -378,16 +379,9 @@ void compute_bow_device(const Vocabulary& voc, const Orb& left, const uint8_t* d
   const int cap = left.capacity();
   check_cap(cap, "compute_bow");
   s = left.enter(s);
-  // stream-ordered scratch of this call: LocalMapping runs it concurrently with Tracking's calls on the same extractor
-  int* scratch = nullptr;
-  if (!word) SIVO_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&scratch), static_cast<size_t>(std::max(cap, 1)) * sizeof(int), s));
-  try {
-    launch_bow(voc, desc, keep_idx, n_keep, cap, levelsup, node, word ? word : scratch, bow_word, bow_weight, bow_len, s);
-  } catch (...) {
-    if (scratch) cudaFreeAsync(scratch, s);
-    throw;
-  }
-  if (scratch) SIVO_CUDA(cudaFreeAsync(scratch, s));
+  const size_t c = std::max(cap, 1);
+  StreamScratch sc(word ? 0 : StreamScratch::bytes<int>(c), s);
+  launch_bow(voc, desc, keep_idx, n_keep, cap, levelsup, node, word ? word : sc.take<int>(c), bow_word, bow_weight, bow_len, s);
 }
 
 void compute_bow_host(const Vocabulary& voc, const uint8_t* desc, int n, int levelsup, int* node, int* word, int* bow_word,
@@ -430,17 +424,11 @@ void search_by_bow_device(const Orb& left, const sivo_keypoint* kps, const uint8
   }
   s = left.enter(s);
   const SbbFrame f{kps, reinterpret_cast<const uint4*>(desc), keep_idx, n_keep, node, cap, nnratio, check ? 1 : 0};
-  // stream-ordered scratch of this call: the frame's sorted keys and one rotation bin per (keyframe, frame key)
-  const size_t sort_bytes = static_cast<size_t>(std::max(cap, 1)) * sizeof(unsigned long long);
-  uint8_t* scratch = nullptr;
-  SIVO_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&scratch), sort_bytes + static_cast<size_t>(n_kf) * cap + 16, s));
-  try {
-    launch_sbb(f, t.data(), n_kf, reinterpret_cast<unsigned long long*>(scratch), scratch + sort_bytes, match, n_matches, s);
-  } catch (...) {
-    cudaFreeAsync(scratch, s);
-    throw;
-  }
-  SIVO_CUDA(cudaFreeAsync(scratch, s));
+  // the frame's sorted keys and one rotation bin per (keyframe, frame key)
+  const size_t c = std::max(cap, 1), n_bins = static_cast<size_t>(n_kf) * cap;
+  StreamScratch sc(StreamScratch::bytes<unsigned long long>(c) + n_bins, s);
+  unsigned long long* sorted = sc.take<unsigned long long>(c);
+  launch_sbb(f, t.data(), n_kf, sorted, sc.take<uint8_t>(n_bins), match, n_matches, s);
 }
 
 void search_by_bow_host(const Orb& left, const sivo_keypoint* kps, const uint8_t* desc, const int* node, int n,

@@ -9,6 +9,7 @@
 #include "frame_ops.h"
 #include "host_call.h"
 #include "info_mi.cuh"
+#include "stream_scratch.h"
 
 namespace sivo {
 
@@ -172,8 +173,9 @@ void info_select_device(const Orb& left, const sivo_keypoint* kps, const double*
                         const float* depth, const sivo_info_camera& cam, double threshold, float* world, double* reduction, int* selected,
                         long long* n_selected, cudaStream_t s) {
   s = left.enter(s);
+  StreamScratch sc(StreamScratch::bytes<uint8_t>(left.capacity()), s);
   launch_info_select(make_params(left, cam, threshold), kps, kp_entropy, keep_idx, n_keep, left.capacity(), depth, world, reduction,
-                     left.info_flags(), selected, n_selected, nullptr, nullptr, nullptr, s);
+                     sc.take<uint8_t>(left.capacity()), selected, n_selected, nullptr, nullptr, nullptr, s);
 }
 
 }  // namespace sivo

@@ -18,6 +18,7 @@
 #include "info_mi.cuh"
 #include "jacobi.cuh"
 #include "match_fold.cuh"
+#include "stream_scratch.h"
 
 namespace sivo {
 namespace {
@@ -493,17 +494,10 @@ void create_map_points_device(const Orb& left, const sivo_keyframe_keys& kf1, co
   const int cap = left.capacity();
   const MapParams p = make_params(left, kf1, nbs, n_nb, prm, cap, cap, false);
   s = left.enter(s);
-  // stream-ordered scratch of this call: LocalMapping runs it concurrently with Tracking's calls on the same extractor
-  int* scratch = nullptr;
-  SIVO_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&scratch), 2 * static_cast<size_t>(std::max(cap, 1)) * sizeof(int), s));
-  int* made = created_nb ? created_nb : scratch;
-  try {
-    launch_create(p, made, created_idx, world, scratch + std::max(cap, 1), created_list, n_created, nullptr, nullptr, nullptr, s);
-  } catch (...) {
-    cudaFreeAsync(scratch, s);
-    throw;
-  }
-  SIVO_CUDA(cudaFreeAsync(scratch, s));
+  const size_t c = std::max(cap, 1);
+  StreamScratch sc(2 * StreamScratch::bytes<int>(c), s);
+  int* made = sc.take<int>(c);
+  launch_create(p, created_nb ? created_nb : made, created_idx, world, sc.take<int>(c), created_list, n_created, nullptr, nullptr, nullptr, s);
 }
 
 // The host form and the test hook: stage every keyframe's keys, run the kernels, download.

@@ -126,16 +126,9 @@ class Orb {
     SIVO_CUDA(cudaSetDevice(device_));
     return s ? s : stream_;
   }
-  // device copies of tables().scale / inv_scale, and capacity() ints of scratch for the device stereo form's SAD distances
-  // (a frame's stereo call on this handle as the left extractor is ordered before its next enqueue_device, like the pyramid)
+  // device copies of tables().scale / inv_scale
   const float* dev_scale() const { return d_scales_.as<float>(); }
   const float* dev_inv_scale() const { return d_scales_.as<float>() + nlevels_; }
-  int* stereo_sad() const { return d_stereo_sad_.as<int>(); }
-  // capacity() bytes of scratch for the device information selection's per-key decisions (ordered like stereo_sad())
-  uint8_t* info_flags() const { return d_info_flags_.as<uint8_t>(); }
-  // at least `bytes` of scratch for the device projection searches (track.cu), ordered like stereo_sad(); it grows by a
-  // stream-ordered reallocation on `s`, so no call synchronises the host
-  uint8_t* track_scratch(size_t bytes, cudaStream_t s);
   float device_ms = 0, tree_ms = 0;
   int launches = 0;
 
@@ -165,10 +158,8 @@ class Orb {
   cudaStream_t stream_ = nullptr;
   cudaEvent_t ev_[4] = {nullptr, nullptr, nullptr, nullptr};
   DevBuf d_gray_, d_pyr_, d_blur_, d_cells_, d_cell_count_, d_cell_items_, d_cell_offset_, d_level_off_, d_cand_,
-      d_umax_, d_desc_, d_scales_, d_stereo_sad_, d_info_flags_;
+      d_umax_, d_desc_, d_scales_;
   PinnedBuf h_gray_, h_cand_, h_level_off_, h_desc_, h_pyr_;
-  void* d_track_ = nullptr;  // cudaMallocAsync'd by track_scratch()
-  size_t track_bytes_ = 0;
   size_t pyr_bytes_ = 0, flat_bytes_ = 0;
   int cand_cap_ = 0, sel_cap_ = 0;
   mutable std::vector<uint32_t> last_cand_;  // last call's packed candidates (x | y << 12 | resp << 24), all levels (test hook)

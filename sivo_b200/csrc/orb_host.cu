@@ -322,8 +322,6 @@ Orb::Orb(int nfeatures, float scale_factor, int nlevels, int ini_th, int min_th,
   h_kps_.ensure(static_cast<size_t>(sel_cap_) * sizeof(sivo_keypoint));
   d_desc_.alloc(static_cast<size_t>(sel_cap_) * 32);
   h_desc_.ensure(static_cast<size_t>(sel_cap_) * 32);
-  d_stereo_sad_.alloc(sel_cap_ * sizeof(int));
-  d_info_flags_.alloc(sel_cap_);
   {
     std::vector<float> sc(tab_.scale);
     sc.insert(sc.end(), tab_.inv_scale.begin(), tab_.inv_scale.end());
@@ -350,7 +348,6 @@ Orb::~Orb() {
   if (copy_stream_) cudaStreamDestroy(copy_stream_);
   if (ev_wait2_) cudaEventDestroy(ev_wait2_);
   if (stream_) cudaStreamDestroy(stream_);
-  if (d_track_) cudaFree(d_track_);
 }
 
 void Orb::level_size(int rows, int cols, int level, int* w, int* h) const {

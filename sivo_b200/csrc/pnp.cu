@@ -18,6 +18,7 @@
 #include "host_call.h"
 #include "jacobi.cuh"
 #include "philox.cuh"
+#include "stream_scratch.h"
 
 namespace sivo {
 namespace {
@@ -855,25 +856,18 @@ void pnp_iterate_device(Pnp& h, int n_iterations, const uint8_t* active, float* 
   p.inlier_match = inlier_match;
   p.n_inliers = n_inliers;
   const size_t cap = std::max(h.cap, 1), words = std::max(h.words, 1), hyps = static_cast<size_t>(p.n_act) * p.H;
-  const size_t b_cnt = (hyps * sizeof(int) + 255) & ~size_t(255), b_tcw = (hyps * 12 * sizeof(float) + 255) & ~size_t(255);
-  const size_t b_mask = (hyps * words * sizeof(uint32_t) + 255) & ~size_t(255);
-  const size_t b_work = p.n_act * cap * 12 * sizeof(double), b_rmask = p.n_act * words * sizeof(uint32_t);
-  // stream-ordered scratch of this call, never on the extractor
-  uint8_t* scratch = nullptr;
-  SIVO_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&scratch), b_cnt + b_tcw + b_mask + b_work + b_rmask, s));
-  p.h_cnt = reinterpret_cast<int*>(scratch);
-  p.h_tcw = reinterpret_cast<float*>(scratch + b_cnt);
-  p.h_mask = reinterpret_cast<uint32_t*>(scratch + b_cnt + b_tcw);
-  p.r_work = reinterpret_cast<double*>(scratch + b_cnt + b_tcw + b_mask);
-  p.r_mask = reinterpret_cast<uint32_t*>(scratch + b_cnt + b_tcw + b_mask + b_work);
+  const size_t n_cnt = hyps, n_tcw = hyps * 12, n_mask = hyps * words, n_work = p.n_act * cap * 12, n_rmask = p.n_act * words;
+  StreamScratch sc(StreamScratch::bytes<int>(n_cnt) + StreamScratch::bytes<float>(n_tcw) + StreamScratch::bytes<uint32_t>(n_mask) +
+                   StreamScratch::bytes<double>(n_work) + StreamScratch::bytes<uint32_t>(n_rmask), s);
+  p.h_cnt = sc.take<int>(n_cnt);
+  p.h_tcw = sc.take<float>(n_tcw);
+  p.h_mask = sc.take<uint32_t>(n_mask);
+  p.r_work = sc.take<double>(n_work);
+  p.r_mask = sc.take<uint32_t>(n_rmask);
   k_pnp_hyp<<<dim3((p.H + kHypWarps - 1) / kHypWarps, p.n_act), kHypThreads, 0, s>>>(p);
-  cudaError_t e = cudaGetLastError();
-  if (e == cudaSuccess) {
-    k_pnp_decide<<<p.n_act, kDecideThreads, 0, s>>>(p);
-    e = cudaGetLastError();
-  }
-  cudaFreeAsync(scratch, s);
-  if (e != cudaSuccess) fail(SIVO_ECUDA, "pnp_iterate: launch failed: %s", cudaGetErrorString(e));
+  SIVO_CUDA(cudaGetLastError());
+  k_pnp_decide<<<p.n_act, kDecideThreads, 0, s>>>(p);
+  SIVO_CUDA(cudaGetLastError());
 }
 
 void pnp_state(const Pnp& h, int* out, float* eps) {

@@ -16,6 +16,7 @@
 #include "block_ops.cuh"
 #include "frame_ops.h"
 #include "host_call.h"
+#include "stream_scratch.h"
 
 namespace sivo {
 namespace {
@@ -643,8 +644,8 @@ void pose_optimize_device(const Orb& left, const sivo_keypoint* kps, const int* 
   const PoseParams p = make_params(left, fx, fy, cx, cy, mbf);
   s = left.enter(s);
   const int cap = left.capacity();
-  PoseEdge* edges = reinterpret_cast<PoseEdge*>(const_cast<Orb&>(left).track_scratch(edges_bytes(cap), s));
-  launch_optimize(p, kps, keep_idx, n_keep, cap, u_right, xw, Tcw_in, edges, result, outlier, s);
+  StreamScratch sc(edges_bytes(cap), s);
+  launch_optimize(p, kps, keep_idx, n_keep, cap, u_right, xw, Tcw_in, sc.take<PoseEdge>(std::max(cap, 1)), result, outlier, s);
 }
 
 void pose_gather_device(const Orb& left, const int* match, const long long* n_keep, const sivo_map_point* pts, int n_points, float* xw,

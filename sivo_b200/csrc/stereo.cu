@@ -6,6 +6,7 @@
 #include "frame_ops.h"
 #include "host_call.h"
 #include "match_fold.cuh"
+#include "stream_scratch.h"
 
 namespace sivo {
 namespace {
@@ -380,9 +381,7 @@ void stereo_match(const Orb& left, const Orb& right, const sivo_keypoint* kl, co
   float* d_u = hc.take<float>(nl);
   float* d_z = hc.take<float>(nl);
   int* d_s = hc.take<int>(nl);
-  // the pyramids were written on the two extractors' own streams; their synchronous run() has returned, so they are complete.
-  // The SAD distances go to this call's workspace: the left extractor's scratch holds capacity() entries and belongs to its
-  // device-form calls, which are not ordered with this one.
+  // the pyramids were written on the two extractors' own streams; their synchronous run() has returned, so they are complete
   launch_stereo(left, right, d_kl, d_dl, nullptr, d_n, nl, d_kr, d_dr, d_n + 1, nr, mb, mbf, d_u, d_z, d_s, hc.stream);
   hc.download(u_right, d_u, nl);
   hc.download(depth, d_z, nl);
@@ -391,7 +390,7 @@ void stereo_match(const Orb& left, const Orb& right, const sivo_keypoint* kl, co
 
 // ComputeStereoMatches on device-resident keypoints, descriptors and counts, enqueued on `s` (NULL: the left extractor's stream)
 // without a host synchronisation.  `s` first waits for everything enqueued so far on both extractors' streams (their pyramids
-// are read).  The SAD distances go to the left extractor's scratch.
+// are read).  The SAD distances go to the call's own stream-ordered scratch.
 void stereo_match_device(Orb& left, Orb& right, const sivo_keypoint* kl, const uint8_t* dl, const int* keep_idx, const long long* n_left,
                          const sivo_keypoint* kr, const uint8_t* dr, const long long* n_right, float mb, float mbf, float* u_right,
                          float* depth, cudaStream_t s) {
@@ -402,8 +401,9 @@ void stereo_match_device(Orb& left, Orb& right, const sivo_keypoint* kl, const u
   s = left.enter(s);
   left.stream_wait(s);
   right.stream_wait(s);
+  StreamScratch sc(StreamScratch::bytes<int>(left.capacity()), s);
   launch_stereo(left, right, kl, dl, keep_idx, n_left, left.capacity(), kr, dr, n_right, right.capacity(), mb, mbf, u_right, depth,
-                left.stereo_sad(), s);
+                sc.take<int>(left.capacity()), s);
 }
 
 // Test hook: k_stereo_median_cut alone over n SAD distances (negative = unmatched), cutting u / z in place.

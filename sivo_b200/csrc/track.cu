@@ -20,6 +20,7 @@
 #include "frame_ops.h"
 #include "host_call.h"
 #include "match_fold.cuh"
+#include "stream_scratch.h"
 
 namespace sivo {
 namespace {
@@ -51,7 +52,7 @@ struct TrackWin {  // one point's projection and window
   int lmin, lmax, in_view, pad;
 };
 
-struct TrackBufs {  // scratch of one call, carved from one allocation
+struct TrackBufs {  // scratch of one call, taken in order by carve()
   int* cell_start;  // kCells + 1
   int* cell_keys;   // cap
   int* cell_of;     // cap
@@ -63,29 +64,19 @@ struct TrackBufs {  // scratch of one call, carved from one allocation
   int* hist;        // n_points
 };
 
-size_t align256(size_t b) { return (b + 255) & ~static_cast<size_t>(255); }
-
 size_t scratch_bytes(int cap, int np) {
   const size_t c = std::max(cap, 1), p = std::max(np, 1);
-  return align256((kCells + 1) * sizeof(int)) + 2 * align256(c * sizeof(int)) + align256(c * sizeof(TrackKey)) + align256(c * 32) +
-         align256(c * sizeof(float)) + align256(p * sizeof(TrackWin)) + align256(p * sizeof(Best2)) + align256(p * sizeof(int));
+  return StreamScratch::bytes<int>(kCells + 1) + 2 * StreamScratch::bytes<int>(c) + StreamScratch::bytes<TrackKey>(c) +
+         StreamScratch::bytes<uint4>(2 * c) + StreamScratch::bytes<float>(c) + StreamScratch::bytes<TrackWin>(p) +
+         StreamScratch::bytes<Best2>(p) + StreamScratch::bytes<int>(p);
 }
 
-TrackBufs carve(uint8_t* base, int cap, int np) {
+// takes the buffers, in order, from a HostCall or a StreamScratch of scratch_bytes(cap, np)
+template <class Scratch> TrackBufs carve(Scratch& a, int cap, int np) {
   const size_t c = std::max(cap, 1), p = std::max(np, 1);
-  TrackBufs b;
-  size_t off = 0;
-  auto take = [&](size_t bytes) { uint8_t* q = base + off; off += align256(bytes); return q; };
-  b.cell_start = reinterpret_cast<int*>(take((kCells + 1) * sizeof(int)));
-  b.cell_keys = reinterpret_cast<int*>(take(c * sizeof(int)));
-  b.cell_of = reinterpret_cast<int*>(take(c * sizeof(int)));
-  b.keys = reinterpret_cast<TrackKey*>(take(c * sizeof(TrackKey)));
-  b.desc = reinterpret_cast<uint4*>(take(c * 32));
-  b.angle = reinterpret_cast<float*>(take(c * sizeof(float)));
-  b.win = reinterpret_cast<TrackWin*>(take(p * sizeof(TrackWin)));
-  b.fold = reinterpret_cast<Best2*>(take(p * sizeof(Best2)));
-  b.hist = reinterpret_cast<int*>(take(p * sizeof(int)));
-  return b;
+  return {a.template take<int>(kCells + 1), a.template take<int>(c),     a.template take<int>(c),
+          a.template take<TrackKey>(c),     a.template take<uint4>(2 * c), a.template take<float>(c),
+          a.template take<TrackWin>(p),     a.template take<Best2>(p),     a.template take<int>(p)};
 }
 
 // ---- grid
@@ -497,7 +488,7 @@ void search_host(const Orb& left, bool last, const sivo_keypoint* kps, const uin
   uint8_t* d_view = hc.take<uint8_t>(n_points);
   int* d_match = hc.take<int>(n);
   long long* d_nm = hc.take<long long>(1);
-  const TrackBufs b = carve(hc.take<uint8_t>(scratch_bytes(n, n_points)), n, n_points);
+  const TrackBufs b = carve(hc, n, n_points);
   launch_search(p, d_kps, d_desc, nullptr, d_count, n, d_ur, d_blocked, d_pts, n_points, b, d_view, d_match, d_nm, hc.stream);
   long long nm = 0;
   hc.download(in_view, d_view, n_points);
@@ -519,21 +510,11 @@ void search_device(const Orb& left, bool last, const sivo_keypoint* kps, const u
   if (last) last_frame_direction(p, f, Rlw, tlw);
   s = left.enter(s);
   const int cap = left.capacity();
-  const TrackBufs b = carve(const_cast<Orb&>(left).track_scratch(scratch_bytes(cap, n_points), s), cap, n_points);
+  StreamScratch sc(scratch_bytes(cap, n_points), s);
+  const TrackBufs b = carve(sc, cap, n_points);
   launch_search(p, kps, desc, keep_idx, n_keep, cap, u_right, blocked, pts, n_points, b, in_view, match, n_matches, s);
 }
 }  // namespace
-
-uint8_t* Orb::track_scratch(size_t bytes, cudaStream_t s) {
-  if (track_bytes_ < bytes) {
-    if (d_track_) SIVO_CUDA(cudaFreeAsync(d_track_, s));
-    d_track_ = nullptr;
-    track_bytes_ = 0;
-    SIVO_CUDA(cudaMallocAsync(&d_track_, bytes + bytes / 2, s));
-    track_bytes_ = bytes + bytes / 2;
-  }
-  return static_cast<uint8_t*>(d_track_);
-}
 
 void search_local_points(const Orb& left, const sivo_keypoint* kps, const uint8_t* desc, const float* u_right, const uint8_t* blocked, int n,
                          const sivo_map_point* pts, int n_points, const sivo_track_frame& f, float th, float nnratio, uint8_t* in_view,
@@ -581,7 +562,7 @@ void features_in_area(const Orb& left, const sivo_keypoint* kps, int n, const si
   const int* d_lv = hc.upload(levels, 2 * static_cast<size_t>(nq));
   int* d_off = hc.take<int>(nq + 1);
   int* d_idx = hc.take<int>(std::max(idx_cap, 0));
-  const TrackBufs b = carve(hc.take<uint8_t>(scratch_bytes(n, 0)), n, 0);
+  const TrackBufs b = carve(hc, n, 0);
   k_track_grid<<<1, kGridThreads, 0, st>>>(p, d_kps, d_desc, nullptr, d_count, n, d_ur, b);
   SIVO_CUDA(cudaGetLastError());
   std::vector<int> len(std::max(nq, 1));

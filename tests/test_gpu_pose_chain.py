@@ -2,8 +2,7 @@
 semantic keys -> stereo -> last-frame search -> gather -> pose -> (the host reads the result) -> local-map search at that pose ->
 gather -> pose -> (the host reads the result) -> information selection with its Rwc, Ow and Sigma -- each stage checked against
 oracle/track_oracle.py, oracle/pose_oracle.py and oracle/info_oracle.py on the stage's own inputs (the KITTI fixture crop and two
-synthetic frames).  The pose calls share the left extractor's search scratch with both searches and run before the next frame's
-enqueue_device."""
+synthetic frames).  The searches and pose calls read the frame's keys, so they run before the next frame's enqueue_device."""
 import numpy as np
 import pytest
 import torch
@@ -133,7 +132,7 @@ def test_three_frames_in_flight_through_both_optimisations(seg, ext, kitti_bgr):
     torch.cuda.synchronize()
 
     # the chain: front end, last-frame search, gather, pose for the three frames in flight; each frame's enqueue_device waits for
-    # the previous frame's search and optimisation, which share the left extractor's scratch
+    # the previous frame's search and optimisation
     for i, b in enumerate(bufs):
         front_end(i, b)
         c, kl = cases[i], b["kl"]
