@@ -489,6 +489,39 @@ int sivo_dbg_pose_system(const sivo_orb_t* left, const sivo_keypoint* kps, const
                          float fy, float cx, float cy, float mbf, const double* pose7, int robust_stereo, const uint8_t* level1,
                          double* err, double* chi2, double* rho, double* jac, double* H, double* b, double* chi);
 
+/* Test hook: sivo_pose_optimize run by the traced instantiation of its kernel, which also records the optimisation as thread 0
+ * runs it.  Per trial (after its lambda update): kind SIVO_POSE_TRACE_TRIAL, round, iteration, trial (qmax before the increment),
+ * ok2 (the factorisation succeeded), accepted, current (currentChi before the update), temp (DBL_MAX after a failed
+ * factorisation), lam / ni before and after, rho, x (the solver's buffer used) and the trial pose q, t.  Before it, one record
+ * per transcendental call, in call order, with its argument and result: the theta >= 1e-5 branch of oplus calls sin(theta),
+ * cos(theta) and pow(theta, 3) (arg = theta); an accepted trial calls pow(2 rho - 1, 3) (arg = 2 rho - 1).  Per round run, after
+ * its classification: SIVO_POSE_TRACE_ROUND with n_active (the round's level-0 edges), n_bad and robust_stereo (the round's
+ * stereo kernels).  At most SIVO_POSE_TRACE_MAX records (4 rounds x 10 iterations x 10 trials of at most 5, plus 4).  Writes
+ * the first trace_cap records to trace (may be NULL when trace_cap is 0) and returns the number recorded, or a negative error
+ * code as sivo_pose_optimize; outlier may be NULL. */
+#define SIVO_POSE_TRACE_TRIAL 0
+#define SIVO_POSE_TRACE_ROUND 1
+#define SIVO_POSE_TRACE_SIN 2
+#define SIVO_POSE_TRACE_COS 3
+#define SIVO_POSE_TRACE_POW_THETA 4
+#define SIVO_POSE_TRACE_POW_RHO 5
+#define SIVO_POSE_TRACE_MAX (4 + 4 * 10 * 10 * 5)
+typedef struct sivo_pose_trace_rec {
+  int32_t kind, round, iteration, trial;
+  int32_t ok2, accepted, n_active, n_bad, robust_stereo, reserved;
+  double current, temp, lam_before, ni_before, lam_after, ni_after, rho;
+  double x[6], q[4], t[3];
+  double arg, value;
+} sivo_pose_trace_rec;
+int sivo_dbg_pose_trace(const sivo_orb_t* left, const sivo_keypoint* kps, const float* u_right, const float* xw, int n, float fx,
+                        float fy, float cx, float cy, float mbf, const float* Tcw_in, sivo_pose_result* result, uint8_t* outlier,
+                        sivo_pose_trace_rec* trace, int trace_cap);
+/* Test hook: the kernel's own SE3Quat functions on n >= 1 host entries, one thread each on `device`.  Entry i: se3[7 i ..] =
+ * to_se3quat(T[12 i ..]) as (qx, qy, qz, qw, tx, ty, tz); up[7 i ..] = oplus(d[6 i ..], that pose) as a trial step computes it;
+ * tv[4 i ..] = (theta, sin theta, cos theta, pow(theta, 3)) of that oplus (the last three NaN on the theta < 1e-5 branch);
+ * res[i] = the result's pose fields as the kernel writes them from that estimate (sigma and counts unwritten). */
+int sivo_dbg_pose_se3(int device, int n, const float* T, const double* d, double* se3, double* up, double* tv, sivo_pose_result* res);
+
 /* ---- a keyframe's new map points: LocalMapping::CreateNewMapPoints (LocalMapping.cc:198-472) with ORBmatcher::
  * SearchForTriangulation (ORBmatcher.cc:631-785, ORBmatcher(0.6, false): no orientation check), CheckDistEpipolarLine
  * (:137-159), ComputeF12 (LocalMapping.cc:639-654) and SIVO's CheckSemantics (:474-545), stereo only -------------------------

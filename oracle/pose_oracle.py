@@ -52,6 +52,12 @@ Unpinned (the order of operations of code that is not built here): CHOLMOD's AMD
 (natural order here); Eigen's quaternion-from-matrix, quaternion product, cross product, q * v and toRotationMatrix operation
 orders, its 3-term sums and its product kernels (Eigen 3's scalar formulas here); sin / cos / pow.
 
+Replay: se3_exp's sin(theta), cos(theta), pow(theta, 3) and the lambda update's pow(2 rho - 1, 3) come from a Transcendentals
+source, Python's math by default.  pose_optimization(..., replay=calls) takes them from calls instead, in call order, each after
+asserting that the argument computed here has the bits of the one recorded; with the device's own values (sivo_dbg_pose_trace)
+every other operation is restated, so the whole optimisation is comparable bit for bit.  The log it returns holds one record per
+transcendental call, per trial and per round, with sivo_pose_trace_rec's field names.
+
 Reductions over edges, `order`:
   "sequential"  s = 0; s = s + v_e in key order (g2o).
   "device"      the kernel's fixed tree: 256 threads, thread t sums the edges t, t + 256, t + 512, ... in order from 0; each warp
@@ -179,7 +185,46 @@ def _mat3(a, b):
     return np.array([[(a[i, 0] * b[0, j] + a[i, 1] * b[1, j]) + a[i, 2] * b[2, j] for j in range(3)] for i in range(3)], F64)
 
 
-def se3_exp(delta) -> Pose:
+def _same_bits(a, b) -> bool:
+    a, b = float(a), float(b)
+    return (a != a and b != b) or np.float64(a).view(np.int64) == np.float64(b).view(np.int64)
+
+
+TRANSCENDENTAL_KINDS = ("sin", "cos", "pow_theta", "pow_rho")
+
+
+class Transcendentals:
+    """The source of sin(theta), cos(theta), pow(theta, 3) ("pow_theta") and pow(2 rho - 1, 3) ("pow_rho"): Python's math, or
+    `replay`, a sequence of {"kind", "arg", "value"} taken in call order (other kinds skipped) after checking the kind and the
+    argument's bits.  Every call is appended to `log` (when given) with the current `where` (round, iteration, trial)."""
+
+    def __init__(self, replay=None, log=None):
+        self.calls = None if replay is None else [c for c in replay if c["kind"] in TRANSCENDENTAL_KINDS]
+        self.used = 0
+        self.log = log
+        self.where = (0, 0, 0)
+
+    def __call__(self, kind, arg):
+        arg = float(arg)
+        if self.calls is None:
+            value = math.sin(arg) if kind == "sin" else math.cos(arg) if kind == "cos" else math.pow(arg, 3)
+        else:
+            assert self.used < len(self.calls), f"replay: no recorded value left for {kind}({arg!r})"
+            c = self.calls[self.used]
+            assert c["kind"] == kind and _same_bits(c["arg"], arg), \
+                f"replay call {self.used}: {kind}({arg.hex()}) here, {c['kind']}({float(c['arg']).hex()}) recorded"
+            value = float(c["value"])
+            self.used += 1
+        if self.log is not None:
+            r, it, q = self.where
+            self.log.append({"kind": kind, "round": r, "iteration": it, "trial": q, "arg": arg, "value": value})
+        return value
+
+
+MATH = Transcendentals()
+
+
+def se3_exp(delta, tx: Transcendentals = MATH) -> Pose:
     """SE3Quat::exp(update): update = [omega, upsilon]."""
     d = [float(v) for v in delta]
     omega, upsilon = d[:3], d[3:]
@@ -191,16 +236,16 @@ def se3_exp(delta) -> Pose:
         V = R
     else:
         O2 = _mat3(O, O)
-        s, c = math.sin(theta), math.cos(theta)
+        s, c = tx("sin", theta), tx("cos", theta)
         R = (I3 + (s / theta) * O) + ((1 - c) / (theta * theta)) * O2
-        V = (I3 + ((1 - c) / (theta * theta)) * O) + ((theta - s) / math.pow(theta, 3)) * O2
+        V = (I3 + ((1 - c) / (theta * theta)) * O) + ((theta - s) / tx("pow_theta", theta)) * O2
     t = np.array([(V[i, 0] * upsilon[0] + V[i, 1] * upsilon[1]) + V[i, 2] * upsilon[2] for i in range(3)], F64)
     return Pose(normalize_rotation(quat_from_matrix(R)), t)
 
 
-def oplus(delta, T: Pose) -> Pose:
+def oplus(delta, T: Pose, tx: Transcendentals = MATH) -> Pose:
     """VertexSE3Expmap::oplusImpl: exp(delta) * T (SE3Quat::operator*)."""
-    E = se3_exp(delta)
+    E = se3_exp(delta, tx)
     return Pose(normalize_rotation(quat_mul(E.q, T.q)), E.t + transform(E.q, T.t))
 
 
@@ -473,8 +518,10 @@ class Optimized:
     log: list                 # (iteration, trial, accepted, currentChi, tempChi, lambda, trial pose)
 
 
-def optimize(E: Edges, T0: Pose, cam: Camera, robust, active, order: str, state: LMState, iterations=ITERATIONS) -> Optimized:
-    """SparseOptimizer::optimize(iterations) with OptimizationAlgorithmLevenberg over the active edges, from T0."""
+def optimize(E: Edges, T0: Pose, cam: Camera, robust, active, order: str, state: LMState, iterations=ITERATIONS,
+             tx: Transcendentals = MATH, trace=None, round_=0) -> Optimized:
+    """SparseOptimizer::optimize(iterations) with OptimizationAlgorithmLevenberg over the active edges, from T0.  tx: the
+    transcendentals' source; trace: a list that receives one record per trial (sivo_pose_trace_rec's fields)."""
     T = T0
     chi2 = np.full(len(E), np.nan)
     log = []
@@ -499,7 +546,9 @@ def optimize(E: Edges, T0: Pose, cam: Camera, robust, active, order: str, state:
             L = cholesky(A)
             if L is not None:
                 state.x = cholesky_solve(L, S.b)
-            trial = oplus(state.x, T)
+            tx.where = (round_, it, qmax)
+            lam0, ni0, current0 = lam, ni, current
+            trial = oplus(state.x, T, tx)
             temp, ev = robust_chi(E, trial, cam, robust, active, order)
             chi2 = np.where(active, ev.chi2, chi2)
             if L is None:
@@ -510,8 +559,9 @@ def optimize(E: Edges, T0: Pose, cam: Camera, robust, active, order: str, state:
                 scale += state.x[j] * (lam * state.x[j] + S.b[j])
             scale += 1e-3
             rho /= scale
-            if rho > 0 and math.isfinite(temp):
-                alpha = 1.0 - math.pow(2 * rho - 1, 3)
+            accepted = rho > 0 and math.isfinite(temp)
+            if accepted:
+                alpha = 1.0 - tx("pow_rho", 2 * rho - 1)
                 alpha = 2.0 / 3.0 if 2.0 / 3.0 < alpha else alpha
                 lam *= alpha if 1.0 / 3.0 < alpha else 1.0 / 3.0
                 ni = 2.0
@@ -522,8 +572,13 @@ def optimize(E: Edges, T0: Pose, cam: Camera, robust, active, order: str, state:
                 lam *= ni
                 ni *= 2
                 log.append((it, qmax, False, current, temp, lam, trial))
-                if not math.isfinite(lam):
-                    break
+            if trace is not None:
+                trace.append({"kind": "trial", "round": round_, "iteration": it, "trial": qmax, "ok2": int(L is not None),
+                              "accepted": int(accepted), "current": current0, "temp": float(temp), "lam_before": lam0,
+                              "ni_before": ni0, "lam_after": lam, "ni_after": ni, "rho": rho, "x": state.x.copy(),
+                              "q": trial.q.copy(), "t": trial.t.copy()})
+            if not accepted and not math.isfinite(lam):
+                break
             qmax += 1
             if not (rho < 0 and qmax < MAX_TRIALS):
                 break
@@ -563,9 +618,21 @@ def _result(Tcw, T: Pose, n_keys, E, outlier, sigma, valid, n_bad, n_good, round
                   sigma if valid else np.zeros((6, 6), F64), bool(valid), len(E), n_bad, n_good, rounds, out, chi2, E, logs)
 
 
-def pose_optimization(kps, u_right, xw, Tcw, inv_sigma2, cam: Camera, order: str = "sequential") -> Result:
+def pose_optimization(kps, u_right, xw, Tcw, inv_sigma2, cam: Camera, order: str = "sequential", replay=None, log=False):
     """Optimizer::PoseOptimization for the semantic keys kps (mvKeysSemantic), mvRight, the matched points' positions (NaN x: no
-    map point) and the frame's pose (float 3 x 4 or 4 x 4)."""
+    map point) and the frame's pose (float 3 x 4 or 4 x 4).  Returns the Result; with `replay` (the recorded transcendental
+    calls, see Transcendentals) or `log`, (Result, log): the transcendental, trial and round records in the device's order."""
+    if replay is None and not log:
+        return _pose_optimization(kps, u_right, xw, Tcw, inv_sigma2, cam, order, MATH, None)
+    trace = []
+    tx = Transcendentals(replay, trace)
+    r = _pose_optimization(kps, u_right, xw, Tcw, inv_sigma2, cam, order, tx, trace)
+    if replay is not None:
+        assert tx.used == len(tx.calls), f"replay: {len(tx.calls) - tx.used} recorded calls left over"
+    return r, trace
+
+
+def _pose_optimization(kps, u_right, xw, Tcw, inv_sigma2, cam, order, tx, trace) -> Result:
     E = make_edges(kps, u_right, xw, inv_sigma2)
     n_keys = len(np.asarray(u_right))
     T_in = to_se3quat(Tcw)
@@ -583,7 +650,7 @@ def pose_optimization(kps, u_right, xw, Tcw, inv_sigma2, cam: Camera, order: str
         chi2 = np.full(len(E), np.nan)
         log = []
         if active.any():
-            o = optimize(E, T_in, cam, robust, active, order, state)
+            o = optimize(E, T_in, cam, robust, active, order, state, tx=tx, trace=trace, round_=r)
             T, H, chi2, log = o.pose, o.H, o.chi2, o.log
         logs.append({"robust": robust.copy(), "active": active.copy(), "lm": log, "pose": T})
         redo = E.stereo & outlier
@@ -593,6 +660,8 @@ def pose_optimization(kps, u_right, xw, Tcw, inv_sigma2, cam: Camera, order: str
             bad = E.stereo & ~(chi2.astype(F32) <= CHI2_STEREO)
         outlier = bad
         n_bad = int(bad.sum())
+        if trace is not None:
+            trace.append({"kind": "round", "round": r, "n_active": int(active.sum()), "n_bad": n_bad, "robust_stereo": int(r < 3)})
         chi2_last = np.where(E.stereo, chi2, np.nan)
         if r == 2:
             robust = ~E.stereo

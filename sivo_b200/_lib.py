@@ -77,6 +77,8 @@ def lib() -> C.CDLL:
         _lib.sivo_pose_gather_device.argtypes = [vp, vp, vp, vp, i32, vp, vp]
         _lib.sivo_pose_optimize.argtypes = [vp, vp, vp, vp, i32, f32, f32, f32, f32, f32, vp, vp, vp]
         _lib.sivo_dbg_pose_system.argtypes = [vp, vp, vp, vp, i32, f32, f32, f32, f32, f32, vp, i32, vp, vp, vp, vp, vp, vp, vp, vp]
+        _lib.sivo_dbg_pose_trace.argtypes = [vp, vp, vp, vp, i32, f32, f32, f32, f32, f32, vp, vp, vp, vp, i32]
+        _lib.sivo_dbg_pose_se3.argtypes = [i32, i32, vp, vp, vp, vp, vp, vp]
         _lib.sivo_keyframe_gather_device.argtypes = [vp] * 19
         _lib.sivo_create_map_points_device.argtypes = [vp, vp, vp, i32, vp, vp, vp, vp, vp, vp, vp]
         _lib.sivo_create_map_points.argtypes = [vp, vp, vp, i32, vp, vp, vp, vp, vp, vp]

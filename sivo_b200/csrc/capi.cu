@@ -603,6 +603,21 @@ int sivo_dbg_pose_system(const sivo_orb_t* left, const sivo_keypoint* kps, const
   });
 }
 
+int sivo_dbg_pose_trace(const sivo_orb_t* left, const sivo_keypoint* kps, const float* u_right, const float* xw, int n, float fx,
+                        float fy, float cx, float cy, float mbf, const float* Tcw_in, sivo_pose_result* result, uint8_t* outlier,
+                        sivo_pose_trace_rec* trace, int trace_cap) {
+  int n_rec = 0;
+  const int rc = guarded([&] {
+    if (!left || !Tcw_in || !result || n < 0 || (n && (!kps || !u_right || !xw))) fail(SIVO_EINVAL, "pose_trace: null argument or n < 0");
+    n_rec = pose_trace(*left->impl, kps, u_right, xw, n, fx, fy, cx, cy, mbf, Tcw_in, result, outlier, trace, trace_cap);
+  });
+  return rc ? rc : n_rec;
+}
+
+int sivo_dbg_pose_se3(int device, int n, const float* T, const double* d, double* se3, double* up, double* tv, sivo_pose_result* res) {
+  return guarded([&] { pose_se3(device, n, T, d, se3, up, tv, res); });
+}
+
 // ---------------------------------------------------------------------------------------- keyframe map points
 int sivo_keyframe_gather_device(const sivo_orb_t* left, const sivo_keypoint* kps_device, const uint8_t* desc_device,
                                 const int* keep_idx_device, const long long* n_keep_device, const float* u_right_device,

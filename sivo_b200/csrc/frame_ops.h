@@ -53,6 +53,10 @@ void pose_gather_device(const Orb& left, const int* match, const long long* n_ke
                         cudaStream_t s);
 void pose_optimize(const Orb& left, const sivo_keypoint* kps, const float* u_right, const float* xw, int n, float fx, float fy, float cx,
                    float cy, float mbf, const float* Tcw_in, sivo_pose_result* result, uint8_t* outlier);
+int pose_trace(const Orb& left, const sivo_keypoint* kps, const float* u_right, const float* xw, int n, float fx, float fy, float cx,
+               float cy, float mbf, const float* Tcw_in, sivo_pose_result* result, uint8_t* outlier, sivo_pose_trace_rec* trace,
+               int trace_cap);
+void pose_se3(int device, int n, const float* T, const double* d, double* se3, double* up, double* tv, sivo_pose_result* res);
 void pose_system(const Orb& left, const sivo_keypoint* kps, const float* u_right, const float* xw, int n, float fx, float fy, float cx,
                  float cy, float mbf, const double* pose7, int robust_stereo, const uint8_t* level1, double* err, double* chi2, double* rho,
                  double* jac, double* H, double* b, double* chi);

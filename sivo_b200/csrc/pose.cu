@@ -111,8 +111,10 @@ __device__ __forceinline__ void mat3(const double (&a)[3][3], const double (&b)[
     for (int j = 0; j < 3; ++j) c[i][j] = (a[i][0] * b[0][j] + a[i][1] * b[1][j]) + a[i][2] * b[2][j];
 }
 
-// VertexSE3Expmap::oplusImpl: SE3Quat::exp(d) * T
-__device__ void oplus(const double* d, const DPose& T, DPose& out) {
+// VertexSE3Expmap::oplusImpl: SE3Quat::exp(d) * T.  kTrace: tv = (theta, sin theta, cos theta, pow(theta, 3)), the last three
+// written only when the theta >= 1e-5 branch calls them.
+template <bool kTrace = false>
+__device__ void oplus(const double* d, const DPose& T, DPose& out, double* tv = nullptr) {
   const double theta = sqrt((d[0] * d[0] + d[1] * d[1]) + d[2] * d[2]);
   const double O[3][3] = {{0.0, -d[2], d[1]}, {d[2], 0.0, -d[0]}, {-d[1], d[0], 0.0}};
   double O2[3][3], R[3][3], V[3][3];
@@ -123,6 +125,7 @@ __device__ void oplus(const double* d, const DPose& T, DPose& out) {
   } else {
     const double s = sin(theta), c = cos(theta);
     const double a = s / theta, b = (1 - c) / (theta * theta), e = (theta - s) / pow(theta, 3.0);
+    if constexpr (kTrace) { tv[1] = s; tv[2] = c; tv[3] = pow(theta, 3.0); }  // pow is a pure function: the value e used
     for (int i = 0; i < 3; ++i)
       for (int j = 0; j < 3; ++j) {
         const double id = i == j ? 1.0 : 0.0;
@@ -130,6 +133,7 @@ __device__ void oplus(const double* d, const DPose& T, DPose& out) {
         V[i][j] = (id + b * O[i][j]) + e * O2[i][j];
       }
   }
+  if constexpr (kTrace) tv[0] = theta;
   double eq[4], et[3];
   quat_from_matrix(R, eq);
   normalize_rotation(eq);
@@ -412,12 +416,47 @@ __device__ void write_pose(const float* T, const DPose& P, sivo_pose_result* r) 
   }
 }
 
+// Converter::toCvMat of the estimate: toRotationMatrix and t rounded to float, then write_pose
+__device__ void write_estimate(const DPose& P, sivo_pose_result* r) {
+  double R[3][3];
+  rotation_matrix(P.q, R);
+  float T[12];
+  for (int i = 0; i < 3; ++i) {
+    for (int j = 0; j < 3; ++j) T[4 * i + j] = static_cast<float>(R[i][j]);
+    T[4 * i + 3] = static_cast<float>(P.t[i]);
+  }
+  write_pose(T, P, r);
+}
+
+// Thread 0's record stream of the traced kernel (sivo_dbg_pose_trace): records past the caller's capacity are counted, not written.
+struct Tracer {
+  sivo_pose_trace_rec* rec;
+  int cap, n;
+  __device__ sivo_pose_trace_rec* add(int kind, int round, int it, int trial) {
+    sivo_pose_trace_rec* r = n < cap ? rec + n : nullptr;
+    ++n;
+    if (r) {
+      *r = sivo_pose_trace_rec{};
+      r->kind = kind; r->round = round; r->iteration = it; r->trial = trial;
+    }
+    return r;
+  }
+  __device__ void call(int kind, int round, int it, int trial, double arg, double value) {
+    if (sivo_pose_trace_rec* r = add(kind, round, it, trial)) { r->arg = arg; r->value = value; }
+  }
+};
+
+// kTrace (sivo_dbg_pose_trace): thread 0 also appends its records to trace (trace_cap of them) and writes their count to
+// *trace_count; the production instantiation ignores the three.
+template <bool kTrace>
 __global__ void __launch_bounds__(kThreads, 1)
     k_pose_optimize(const PoseParams p, const sivo_keypoint* __restrict__ kps, const int* __restrict__ keep_idx,
                     const long long* __restrict__ n_keep, int cap, const float* __restrict__ u_right, const float* __restrict__ xw,
                     const float* Tcw_in, PoseEdge* __restrict__ edges_all, sivo_pose_result* results,
-                    uint8_t* __restrict__ outlier_all) {
+                    uint8_t* __restrict__ outlier_all, sivo_pose_trace_rec* trace, int trace_cap, int* trace_count) {
   __shared__ PoseShared s;
+  Tracer tr{trace, trace_cap, 0};
+  double lam0 = 0.0, ni0 = 0.0, cur0 = 0.0;
   // Tcw_in may be the Tcw of *results (an in-place update): it is read into shared memory before anything is written to results.
   // problem blockIdx.x: its keys, points and outputs at stride cap (a batch of problems is a grid size away)
   const int prob = blockIdx.x;
@@ -483,7 +522,19 @@ __global__ void __launch_bounds__(kThreads, 1)
           for (int j = 0; j < 6; ++j) A[j][j] = A[j][j] + s.lam;
           s.ok2 = cholesky6(A, L);
           if (s.ok2) cholesky6_solve(L, s.b, s.x);  // a failed factorisation leaves x as it was
-          oplus(s.x, s.cur, s.trial);
+          if constexpr (kTrace) {
+            double tv[4];
+            oplus<true>(s.x, s.cur, s.trial, tv);
+            if (!(tv[0] < 0.00001)) {
+              tr.call(SIVO_POSE_TRACE_SIN, round, it, qmax, tv[0], tv[1]);
+              tr.call(SIVO_POSE_TRACE_COS, round, it, qmax, tv[0], tv[2]);
+              tr.call(SIVO_POSE_TRACE_POW_THETA, round, it, qmax, tv[0], tv[3]);
+            }
+            lam0 = s.lam;
+            ni0 = s.ni;
+          } else {
+            oplus(s.x, s.cur, s.trial);
+          }
         }
         __syncthreads();
         const double temp_computed = error_pass(p, edges, ne, robust_stereo, s);
@@ -494,8 +545,10 @@ __global__ void __launch_bounds__(kThreads, 1)
           scale += 1e-3;
           rho /= scale;
           s.go = 1;
+          if constexpr (kTrace) cur0 = s.current;
           if (rho > 0 && isfinite(temp)) {
             double alpha = 1. - pow((2 * rho - 1), 3.0);
+            if constexpr (kTrace) tr.call(SIVO_POSE_TRACE_POW_RHO, round, it, qmax, 2 * rho - 1, pow((2 * rho - 1), 3.0));
             alpha = (2. / 3.) < alpha ? (2. / 3.) : alpha;
             s.lam *= (1. / 3.) < alpha ? alpha : (1. / 3.);
             s.ni = 2;
@@ -507,6 +560,16 @@ __global__ void __launch_bounds__(kThreads, 1)
             if (!isfinite(s.lam)) s.go = 0;
           }
           s.rho = rho;
+          if constexpr (kTrace) {
+            if (sivo_pose_trace_rec* r = tr.add(SIVO_POSE_TRACE_TRIAL, round, it, qmax)) {
+              r->ok2 = s.ok2; r->accepted = rho > 0 && isfinite(temp);
+              r->current = cur0; r->temp = temp; r->rho = rho;
+              r->lam_before = lam0; r->ni_before = ni0; r->lam_after = s.lam; r->ni_after = s.ni;
+              for (int j = 0; j < 6; ++j) r->x[j] = s.x[j];
+              for (int j = 0; j < 4; ++j) r->q[j] = s.trial.q[j];
+              for (int j = 0; j < 3; ++j) r->t[j] = s.trial.t[j];
+            }
+          }
         }
         __syncthreads();
         if (!s.go) break;
@@ -537,6 +600,11 @@ __global__ void __launch_bounds__(kThreads, 1)
       __syncthreads();
       if (tid == 0) n_bad = s.n_bad;  // only thread 0 reads it: it alone resets it for the next round
     }
+    if constexpr (kTrace)
+      if (tid == 0)
+        if (sivo_pose_trace_rec* r = tr.add(SIVO_POSE_TRACE_ROUND, round, -1, -1)) {
+          r->n_active = s.n_active; r->n_bad = n_bad; r->robust_stereo = robust_stereo;
+        }
     if (round == 2) robust_stereo = false;
     rounds = round + 1;
     if (ne < 10) break;
@@ -546,16 +614,10 @@ __global__ void __launch_bounds__(kThreads, 1)
     const bool valid = have_h && cholesky6(s.H, L);
     if (valid) marginal6(L, res->sigma_cw);
     else for (int i = 0; i < 36; ++i) res->sigma_cw[i] = 0.0;
-    double R[3][3];
-    rotation_matrix(s.cur.q, R);
-    float T[12];
-    for (int r = 0; r < 3; ++r) {
-      for (int c = 0; c < 3; ++c) T[4 * r + c] = static_cast<float>(R[r][c]);
-      T[4 * r + 3] = static_cast<float>(s.cur.t[r]);
-    }
-    write_pose(T, s.cur, res);
+    write_estimate(s.cur, res);
     res->sigma_valid = valid; res->n_initial = ne; res->n_bad = n_bad; res->n_good = ne - n_bad; res->rounds_run = rounds;
     res->reserved = 0;
+    if constexpr (kTrace) *trace_count = tr.n;
   }
   if (outlier)
     for (int e = tid; e < ne; e += kThreads) outlier[edges[e].key] = static_cast<uint8_t>(edges[e].outlier);
@@ -602,6 +664,25 @@ __global__ void __launch_bounds__(kThreads, 1)
   }
 }
 
+// test hook: per entry i, P = to_se3quat(T[i]), then oplus(d[i], P) as the trial step computes it, and its write_estimate
+__global__ void k_pose_se3(int n, const float* __restrict__ T, const double* __restrict__ d, double* __restrict__ se3, double* __restrict__ up,
+                           double* __restrict__ tv, sivo_pose_result* __restrict__ res) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  float Ti[12];
+  for (int k = 0; k < 12; ++k) Ti[k] = T[12 * i + k];
+  double di[6];
+  for (int k = 0; k < 6; ++k) di[k] = d[6 * i + k];
+  DPose P, U;
+  to_se3quat(Ti, P);
+  const double nan = __longlong_as_double(0x7ff8000000000000ll);
+  double t[4] = {nan, nan, nan, nan};
+  oplus<true>(di, P, U, t);
+  for (int k = 0; k < 4; ++k) { se3[7 * i + k] = P.q[k]; up[7 * i + k] = U.q[k]; tv[4 * i + k] = t[k]; }
+  for (int k = 0; k < 3; ++k) { se3[7 * i + 4 + k] = P.t[k]; up[7 * i + 4 + k] = U.t[k]; }
+  write_estimate(U, res + i);
+}
+
 __global__ void k_pose_gather(const int* __restrict__ match, const long long* __restrict__ n_keep, int cap,
                               const sivo_map_point* __restrict__ pts, int n_points, float* __restrict__ xw) {
   const int n = clamp_count(*n_keep, cap);
@@ -626,7 +707,8 @@ PoseParams make_params(const Orb& left, float fx, float fy, float cx, float cy, 
 void launch_optimize(const PoseParams& p, const sivo_keypoint* kps, const int* keep_idx, const long long* n_keep, int cap,
                      const float* u_right, const float* xw, const float* Tcw_in, PoseEdge* edges, sivo_pose_result* result,
                      uint8_t* outlier, cudaStream_t s) {
-  k_pose_optimize<<<1, kThreads, 0, s>>>(p, kps, keep_idx, n_keep, cap, u_right, xw, Tcw_in, edges, result, outlier);
+  k_pose_optimize<false><<<1, kThreads, 0, s>>>(p, kps, keep_idx, n_keep, cap, u_right, xw, Tcw_in, edges, result, outlier, nullptr, 0,
+                                                nullptr);
   SIVO_CUDA(cudaGetLastError());
 }
 
@@ -677,6 +759,59 @@ void pose_optimize(const Orb& left, const sivo_keypoint* kps, const float* u_rig
   launch_optimize(p, d_kps, nullptr, d_count, n, d_ur, d_xw, d_T, d_edges, d_res, d_out, hc.stream);
   hc.download(result, d_res, 1);
   hc.download(outlier, d_out, n);
+  hc.sync();
+}
+
+int pose_trace(const Orb& left, const sivo_keypoint* kps, const float* u_right, const float* xw, int n, float fx, float fy, float cx,
+               float cy, float mbf, const float* Tcw_in, sivo_pose_result* result, uint8_t* outlier, sivo_pose_trace_rec* trace,
+               int trace_cap) {
+  if (n < 0 || trace_cap < 0 || (trace_cap && !trace)) fail(SIVO_EINVAL, "pose_trace: n = %d, trace_cap = %d", n, trace_cap);
+  const PoseParams p = make_params(left, fx, fy, cx, cy, mbf);
+  check_octaves("pose_trace", kps, xw, n, p.nlevels);
+  HostCall& hc = host_call();
+  hc.begin(left.device());
+  const sivo_keypoint* d_kps = hc.upload(kps, n);
+  const float* d_ur = hc.upload(u_right, n);
+  const float* d_xw = hc.upload(xw, 3 * static_cast<size_t>(n));
+  const float* d_T = hc.upload(Tcw_in, 12);
+  const long long count = n;
+  const long long* d_count = hc.upload(&count, 1);
+  const int zero = 0;
+  int* d_nrec = hc.upload(&zero, 1);
+  sivo_pose_result* d_res = hc.take<sivo_pose_result>(1);
+  uint8_t* d_out = hc.take<uint8_t>(n);
+  sivo_pose_trace_rec* d_tr = hc.take<sivo_pose_trace_rec>(std::max(trace_cap, 1));
+  PoseEdge* d_edges = reinterpret_cast<PoseEdge*>(hc.take<uint8_t>(edges_bytes(n)));
+  k_pose_optimize<true><<<1, kThreads, 0, hc.stream>>>(p, d_kps, nullptr, d_count, n, d_ur, d_xw, d_T, d_edges, d_res, d_out, d_tr,
+                                                       trace_cap, d_nrec);
+  SIVO_CUDA(cudaGetLastError());
+  int n_rec = 0;
+  hc.download(result, d_res, 1);
+  if (outlier) hc.download(outlier, d_out, n);
+  hc.download(&n_rec, d_nrec, 1);
+  hc.sync();
+  if (trace_cap) {
+    hc.download(trace, d_tr, std::min(n_rec, trace_cap));
+    hc.sync();
+  }
+  return n_rec;
+}
+
+void pose_se3(int device, int n, const float* T, const double* d, double* se3, double* up, double* tv, sivo_pose_result* res) {
+  if (n < 1 || !T || !d || !se3 || !up || !tv || !res) fail(SIVO_EINVAL, "pose_se3: null argument or n < 1");
+  HostCall& hc = host_call();
+  hc.begin(device);
+  const float* d_T = hc.upload(T, 12 * static_cast<size_t>(n));
+  const double* d_d = hc.upload(d, 6 * static_cast<size_t>(n));
+  double* d_out = hc.take<double>(18 * static_cast<size_t>(n));
+  sivo_pose_result* d_res = hc.take<sivo_pose_result>(n);
+  k_pose_se3<<<ceil_div(n, kThreads), kThreads, 0, hc.stream>>>(n, d_T, d_d, d_out, d_out + 7 * static_cast<size_t>(n),
+                                                               d_out + 14 * static_cast<size_t>(n), d_res);
+  SIVO_CUDA(cudaGetLastError());
+  hc.download(se3, d_out, 7 * static_cast<size_t>(n));
+  hc.download(up, d_out + 7 * static_cast<size_t>(n), 7 * static_cast<size_t>(n));
+  hc.download(tv, d_out + 14 * static_cast<size_t>(n), 4 * static_cast<size_t>(n));
+  hc.download(res, d_res, n);
   hc.sync();
 }
 

@@ -109,3 +109,42 @@ def pose_system(left: ORBextractor, kps, u_right, xw, pose7, fx, fy, cx, cy, mbf
                                          C.byref(chi)))
     out["chi"] = chi.value
     return out
+
+
+# sivo_pose_trace_rec and its kinds (include/sivo_b200.h)
+TRACE_TRIAL, TRACE_ROUND, TRACE_SIN, TRACE_COS, TRACE_POW_THETA, TRACE_POW_RHO = range(6)
+TRACE_MAX = 4 + 4 * 10 * 10 * 5
+TRACE_DTYPE = np.dtype([(k, "<i4") for k in ("kind", "round", "iteration", "trial", "ok2", "accepted", "n_active", "n_bad",
+                                             "robust_stereo", "reserved")]
+                       + [(k, "<f8") for k in ("current", "temp", "lam_before", "ni_before", "lam_after", "ni_after", "rho")]
+                       + [("x", "<f8", 6), ("q", "<f8", 4), ("t", "<f8", 3), ("arg", "<f8"), ("value", "<f8")])
+assert TRACE_DTYPE.itemsize == 216
+
+
+def pose_trace(left: ORBextractor, kps, u_right, xw, Tcw, fx, fy, cx, cy, mbf):
+    """Test hook: pose_optimize run by the traced kernel.  Returns (PoseResult, outlier bool per key, the TRACE_DTYPE records:
+    per trial its transcendental calls then its state, per round its counts)."""
+    k, u, x = _host_keys(kps, u_right, xw)
+    T = np.ascontiguousarray(np.asarray(Tcw, np.float32).reshape(-1, 4)[:3]).reshape(12)
+    res = PoseResult()
+    out = np.zeros(max(len(k), 1), np.uint8)
+    rec = np.zeros(TRACE_MAX, TRACE_DTYPE)
+    n = L.check(L.lib().sivo_dbg_pose_trace(left._h, _p(k), _p(u), _p(x), len(k), fx, fy, cx, cy, mbf, _p(T), C.byref(res), _p(out),
+                                            _p(rec), TRACE_MAX))
+    if n > TRACE_MAX:
+        raise RuntimeError(f"pose_trace: {n} records, more than the bound {TRACE_MAX}")
+    return res, out[:len(k)].astype(bool), rec[:n]
+
+
+def pose_se3(T, d, device: int = 0):
+    """Test hook: the kernel's to_se3quat, oplus and result rounding on n entries (T (n, 12) float, d (n, 6) double).  Returns
+    (se3 (n, 7), up (n, 7), tv (n, 4): theta, sin, cos, pow(theta, 3) or NaN, results: a PoseResult array of n)."""
+    T = np.ascontiguousarray(T, np.float32).reshape(-1, 12)
+    d = np.ascontiguousarray(d, np.float64).reshape(-1, 6)
+    n = len(T)
+    if len(d) != n:
+        raise ValueError("T and d need one row per entry")
+    se3, up, tv = np.empty((n, 7)), np.empty((n, 7)), np.empty((n, 4))
+    res = (PoseResult * n)()
+    L.check(L.lib().sivo_dbg_pose_se3(device, n, _p(T), _p(d), _p(se3), _p(up), _p(tv), res))
+    return se3, up, tv, res

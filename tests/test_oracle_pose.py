@@ -260,3 +260,77 @@ def test_the_two_reduction_orders_agree():
         assert np.abs(a.H - b.H).max() <= 1e-12 * np.abs(a.H).max()
         assert np.abs(a.b - b.b).max() <= 1e-12 * np.abs(a.b).max() and abs(a.chi - b.chi) <= 1e-12 * a.chi
         assert np.array_equal(a.ev.chi2, b.ev.chi2, equal_nan=True)
+
+
+# ---------------------------------------------------------------------------------------------------------- constructed scenes
+from oracle import pose_scene as PS  # noqa: E402
+from scipy.spatial.transform import Rotation  # noqa: E402
+
+_SCENES = {s.name: s for s in PS.constructed_scenes()}
+
+
+def _run(s):
+    return P.pose_optimization(s.kps, s.ur, s.X, s.Tin, PS.INV_SIGMA2, s.camera(), order="device", log=True)
+
+
+@pytest.mark.parametrize("name", [n for n, s in _SCENES.items() if s.paths])
+def test_constructed_scene_reaches_its_paths(name):
+    s = _SCENES[name]
+    r, log = _run(s)
+    assert s.paths <= PS.paths_reached(s, r, log)
+
+
+def test_constructed_scenes_cover_every_path():
+    """Together the scenes reach every path of PATHS.  Not in PATHS because no float input reaches it through a mirrored pair
+    or a robust edge: (float) chi2 at the double halfway above 7.815f, chi2 one ulp below delta^2 (see pose_scene.chi2_targets)
+    and a lambda that turns non-finite (see pose_scene.overflow_scenes)."""
+    got = set()
+    for s in _SCENES.values():
+        r, log = _run(s)
+        got |= PS.paths_reached(s, r, log)
+    assert set(PS.PATHS) <= got, set(PS.PATHS) - got
+
+
+def test_fixed_points_keep_the_input_bits():
+    for name in ("fixed_mono", "fixed_stereo", "fixed_mixed", "pair_chi2_7815f"):
+        s = _SCENES[name]
+        r, log = _run(s)
+        assert np.array_equal(r.Tcw, s.Tin) and np.array_equal(r.q, [0, 0, 0, 1]) and np.array_equal(r.t, [0, 0, 0])
+        trials = [e for e in log if e["kind"] == "trial"]
+        assert len(trials) == 4 and all(e["rho"] == 0 and not e["accepted"] and (e["x"] == 0).all() for e in trials)
+
+
+def test_pairs_hit_their_chi2_bits():
+    for name, target in PS.chi2_targets().items():
+        where, stereo, e = PS.pair_errors(name)
+        assert PS.chi2_of(e, 1.0, stereo) == target, name
+        s = _SCENES["pair_" + name]
+        E = P.make_edges(s.kps, s.ur, s.X, PS.INV_SIGMA2)
+        c = P.evaluate(E, P.to_se3quat(s.Tin), s.camera(), np.ones(len(E), bool)).chi2
+        assert c[-1] == target and c[-2] == target and (c[:-2] == 0).all(), name
+    t = float(P.CHI2_STEREO)
+    assert int(np.float32(t).view(np.int32)) & 1  # odd mantissa: the halfway double rounds up to the next float
+    assert np.float32((t + PS.f32_next(t)) / 2) == np.float32(PS.f32_next(t))
+
+
+def _sweep_matrices():
+    out = []
+    for ax in ((1, 0, 0), (0, 1, 0), (0, 0, 1), (1, 1, 1), (0.3, -1, 0.2)):
+        for ang in np.linspace(0, np.pi, 61):
+            out.append(PS.axis_rotation(ax, ang).astype(np.float32).astype(np.float64))
+    return out + [m for m in PS._rot_special().values()]
+
+
+def test_quat_from_matrix_against_scipy():
+    for m in _sweep_matrices():
+        q = P.normalize_rotation(P.quat_from_matrix(m))
+        ref = Rotation.from_matrix(m).as_quat()  # (x, y, z, w), scalar last
+        assert min(np.abs(q - ref).max(), np.abs(q + ref).max()) <= 1e-6
+
+
+def test_to_se3quat_reproduces_the_float_matrix():
+    """The float matrix is a rotation to about 1e-7 per entry, so the quaternion's matrix reproduces it to 4e-7."""
+    for m in _sweep_matrices():
+        T = np.concatenate([m, np.ones((3, 1))], 1).astype(np.float32)
+        R = P.rotation_matrix(P.to_se3quat(T).q)
+        assert np.abs(R - m).max() <= 4e-7
