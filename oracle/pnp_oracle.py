@@ -170,6 +170,12 @@ class PoseDebug:
     best: int = 1
     R: list = None
     t: list = None
+    # which branches the run took (for the scene tests; no value depends on them): per approximation 1..3 the sign of x[0]
+    # (and of x[1] for 2, 3), solve_for_sign's pcs flip and the det < 0 flip; qr_solve's early returns over all Gauss-Newton runs
+    signs: dict = field(default_factory=dict)
+    pcs_flip: list = field(default_factory=lambda: [False] * 4)
+    det_flip: list = field(default_factory=lambda: [False] * 4)
+    qr_early: int = 0
 
 
 def _dot(a, b):
@@ -226,7 +232,7 @@ def qr_solve(A, b):
     return X
 
 
-def _gauss_newton(L, rho, betas):
+def _gauss_newton(L, rho, betas, dbg=None):
     x = [0.0] * 4
     for _ in range(5):
         A, b = [], []
@@ -243,6 +249,8 @@ def _gauss_newton(L, rho, betas):
         X = qr_solve(A, b)
         if X is not None:
             x = X
+        elif dbg is not None:
+            dbg.qr_early += 1
         for i in range(4):
             betas[i] = betas[i] + x[i]
 
@@ -358,6 +366,7 @@ def compute_pose(pws, us, fu, fv, uc, vc, la=None, tree=False) -> PoseDebug:
         B[0] = _sqrt(b4[0])
         B[1], B[2], B[3] = _div(b4[1], B[0]), _div(b4[2], B[0]), _div(b4[3], B[0])
     dbg.betas[1] = B
+    dbg.signs[1] = (b4[0] < 0,)
     b3 = la.solve([[r[0], r[1], r[2]] for r in L], rho)
     B = [0.0] * 4
     if b3[0] < 0:
@@ -369,6 +378,7 @@ def compute_pose(pws, us, fu, fv, uc, vc, la=None, tree=False) -> PoseDebug:
     if b3[1] < 0:
         B[0] = -B[0]
     dbg.betas[2] = B
+    dbg.signs[2] = (b3[0] < 0, b3[1] < 0)
     b5 = la.solve([[r[0], r[1], r[2], r[3], r[4]] for r in L], rho)
     B = [0.0] * 4
     if b5[0] < 0:
@@ -381,9 +391,12 @@ def compute_pose(pws, us, fu, fv, uc, vc, la=None, tree=False) -> PoseDebug:
         B[0] = -B[0]
     B[2] = _div(b5[3], B[0])
     dbg.betas[3] = B
+    dbg.signs[3] = (b5[0] < 0, b5[1] < 0)
     for k in (1, 2, 3):
-        _gauss_newton(L, rho, dbg.betas[k])
-        dbg.Rs[k], dbg.ts[k], dbg.rep_errors[k] = _compute_R_and_t(ut, dbg.betas[k], alphas, pws, us, n, fu, fv, uc, vc, la)
+        _gauss_newton(L, rho, dbg.betas[k], dbg)
+        flips = []
+        dbg.Rs[k], dbg.ts[k], dbg.rep_errors[k] = _compute_R_and_t(ut, dbg.betas[k], alphas, pws, us, n, fu, fv, uc, vc, la, flips)
+        dbg.pcs_flip[k], dbg.det_flip[k] = flips
     N = 1
     if dbg.rep_errors[2] < dbg.rep_errors[1]:
         N = 2
@@ -393,7 +406,7 @@ def compute_pose(pws, us, fu, fv, uc, vc, la=None, tree=False) -> PoseDebug:
     return dbg
 
 
-def _compute_R_and_t(ut, betas, alphas, pws, us, n, fu, fv, uc, vc, la):
+def _compute_R_and_t(ut, betas, alphas, pws, us, n, fu, fv, uc, vc, la, flips=None):
     ccs = [[0.0] * 3 for _ in range(4)]
     for i in range(4):
         v = ut[12 * (11 - i):12 * (12 - i)]
@@ -404,7 +417,8 @@ def _compute_R_and_t(ut, betas, alphas, pws, us, n, fu, fv, uc, vc, la):
     for i in range(n):
         a = alphas[i]
         pcs.append([a[0] * ccs[0][j] + a[1] * ccs[1][j] + a[2] * ccs[2][j] + a[3] * ccs[3][j] for j in range(3)])
-    if pcs[0][2] < 0.0:
+    pcs_flip = pcs[0][2] < 0.0
+    if pcs_flip:
         pcs = [[-x for x in p] for p in pcs]
     # estimate_R_and_t
     pc0, pw0 = [0.0] * 3, [0.0] * 3
@@ -426,6 +440,8 @@ def _compute_R_and_t(ut, betas, alphas, pws, us, n, fu, fv, uc, vc, la):
            - R[0][2] * R[1][1] * R[2][0] - R[0][1] * R[1][0] * R[2][2] - R[0][0] * R[1][2] * R[2][1])
     if det < 0:
         R[2] = [-x for x in R[2]]
+    if flips is not None:
+        flips += [pcs_flip, det < 0]
     t = [pc0[i] - _dot(R[i], pw0) for i in range(3)]
     # reprojection_error
     s2 = 0.0
@@ -544,7 +560,7 @@ class IterResult:
 class Solver:
     """PnPsolver for one candidate: correspondences p2d (N x 2 float32), p3d (N x 3 float32), sigma2 (N float32)."""
 
-    def __init__(self, p2d, p3d, sigma2, fx, fy, cx, cy, seed, kf_id, frame_id, dead=False):
+    def __init__(self, p2d, p3d, sigma2, fx, fy, cx, cy, seed, kf_id, frame_id, dead=False, log=False):
         self.p2d = np.asarray(p2d, F32).reshape(-1, 2)
         self.p3d = np.asarray(p3d, F32).reshape(-1, 3)
         self.N = len(self.p2d)
@@ -554,6 +570,13 @@ class Solver:
         self.min_inl, self.eps, self.max_its = ransac_parameters(self.N)
         self.iterations, self.best, self.best_mask, self.best_tcw = 0, 0, np.zeros(self.N, bool), None
         self.cache = {}
+        # the device's refine_failed: Refine of the current best set has failed, so it fails again (Refine is a function of the
+        # set); the device skips it until a hypothesis improves the best count
+        self.refine_failed = False
+        # log=True: one entry per hypothesis (call, g, count, kind = below / improve / tie / worse, refine = ok / failed / skipped /
+        # None, refine_count) and one per call (kind "call"); read by oracle/pnp_scene.paths_reached
+        self.log = [] if log else None
+        self.calls = 0
 
     def hypothesis(self, g):
         """-> (draw indices, PoseDebug, mask, count) of hypothesis g, memoised."""
@@ -575,6 +598,18 @@ class Solver:
         return cnt > self.min_inl, tcw_of(dbg.R, dbg.t), mask, cnt
 
     def iterate(self, n_iterations: int) -> IterResult:
+        res = self._iterate(n_iterations)
+        if self.log is not None:
+            self.log.append(dict(kind="call", call=self.calls, n=n_iterations, ran=res.hypotheses, pose=res.Tcw is not None,
+                                 no_more=res.no_more, n_inliers=res.n_inliers, end=self.iterations))
+        self.calls += 1
+        return res
+
+    def _note(self, **e):
+        if self.log is not None:
+            self.log.append(dict(call=self.calls, **e))
+
+    def _iterate(self, n_iterations: int) -> IterResult:
         empty = np.zeros(self.N, bool)
         if self.dead or self.N < self.min_inl:
             return IterResult(None, True, empty, 0, 0)
@@ -584,17 +619,33 @@ class Solver:
             cur += 1
             self.iterations += 1
             _, dbg, mask, cnt = self.hypothesis(g)
-            if cnt >= self.min_inl:
-                if cnt > self.best:
-                    self.best, self.best_mask, self.best_tcw = cnt, mask, tcw_of(dbg.R, dbg.t)
-                ok, T, rmask, rcnt = self.refine()
-                if ok:
-                    return IterResult(T, False, rmask, rcnt, cur)
+            if cnt < self.min_inl:
+                self._note(kind="below", g=g, count=cnt, refine=None, last=False)
+                continue
+            kind = "improve" if cnt > self.best else "tie" if cnt == self.best else "worse"
+            if cnt > self.best:
+                self.best, self.best_mask, self.best_tcw = cnt, mask, tcw_of(dbg.R, dbg.t)
+                self.refine_failed = False
+            elif kind == "tie" and np.array_equal(mask, self.best_mask):
+                kind = "tie_same"
+            skipped = self.refine_failed  # the reference runs Refine again on the same set; the device skips it
+            ok, T, rmask, rcnt = self.refine()
+            self._note(kind=kind, g=g, count=cnt, refine="skipped" if skipped else "ok" if ok else "failed", refine_count=rcnt,
+                       refine_n=self.best, last=False)
+            if ok:
+                self._mark_last(cur, n_iterations)
+                return IterResult(T, False, rmask, rcnt, cur)
+            self.refine_failed = True
         if self.iterations >= self.max_its:
             if self.best >= self.min_inl:
                 return IterResult(self.best_tcw, True, self.best_mask, self.best, cur)
             return IterResult(None, True, empty, 0, cur)
         return IterResult(None, False, empty, 0, cur)
+
+    def _mark_last(self, cur, n_iterations):
+        """The entry just logged returned a pose on the last hypothesis the call would have run."""
+        if self.log is not None:
+            self.log[-1]["last"] = cur == max(self.max_its - (self.iterations - cur), n_iterations, 0)
 
 
 def correspondences(kps, match_row, n_keep, points_pos, sigma2_table, keep_idx=None, cap=None):

@@ -260,3 +260,90 @@ def test_no_more_with_and_without_a_best_pose():
     s = synthetic_solver(9, 0.0, 4)
     r = s.iterate(5)
     assert r.no_more and r.Tcw is None and r.hypotheses == 0
+
+
+# ---------------------------------------------------------------------------------------------------------- constructed scenes
+def test_constructed_scenes_reach_their_paths_and_together_every_path():
+    """oracle/pnp_scene.py: each scene reaches the paths it names, its embedding gives the setup exactly its correspondences,
+    and together the scenes reach every path of PATHS except those UNREACHED lists."""
+    from oracle import pnp_scene as S
+    cap = S.capacity()
+    reached = set()
+    for sc in S.constructed_scenes():
+        s, res, _ = S.run(sc)
+        got = S.paths_reached(sc, s, cap=cap)
+        assert sc.paths <= got, (sc.name, sc.paths - got)
+        reached |= got
+        for nlevels in (8, 4):
+            if nlevels == 4 and sc.N > 600:
+                continue
+            fr = S.embed(sc, cap, nlevels, np.random.default_rng(0))
+            p2, p3, s2, key = S.frame_correspondences(fr, cap, S.SIGMA2)
+            if nlevels == 8:
+                assert np.array_equal(p2, sc.p2d) and np.array_equal(p3, sc.p3d) and np.array_equal(s2, S.SIGMA2[sc.octave])
+            reached |= fr.paths
+    missing = set(S.PATHS) - reached
+    assert missing == set(S.UNREACHED), missing
+    print(f"{len(reached & set(S.PATHS))} of {len(S.PATHS)} paths reached")
+
+
+def test_searched_scenes_are_the_first_that_reach_their_paths():
+    """SEARCHED records, per family, the first kf_id whose run takes the named paths."""
+    from oracle import pnp_scene as S
+    for name, kf in S.SEARCHED.items():
+        assert S.find_searched(name, 1, kf) == kf, name
+
+
+def test_the_log_is_additive():
+    """The per-hypothesis log changes no result: a logged and an unlogged solver agree call by call."""
+    for seed in range(4):
+        a, b = synthetic_solver(40, 0.4, seed), synthetic_solver(40, 0.4, seed, log=True)
+        for n in (5, 1, 0, 36, 5):
+            ra, rb = a.iterate(n), b.iterate(n)
+            assert (ra.no_more, ra.n_inliers, ra.hypotheses) == (rb.no_more, rb.n_inliers, rb.hypotheses)
+            assert np.array_equal(ra.inliers, rb.inliers) and ((ra.Tcw is None and rb.Tcw is None) or np.array_equal(ra.Tcw, rb.Tcw))
+        assert len(b.log) >= 5
+
+
+# ---------------------------------------------------------------------------------------------------------- 50-digit bounds
+def test_jacobi_rule_within_its_bounds_against_50_digits():
+    """oracle/pnp_bounds.py on generated matrices: 600 12 x 12 spectra (spread, a clustered near-null four, rank 8, repeated
+    eigenvalues, noise-free MtM) and 2400 6 x K solves (K = 3, 4, 5, column scales over 1e-3 .. 1e3, consistent and with a
+    residual).  Each error, as a ratio to its first-order bound, stays below C."""
+    from oracle import pnp_bounds as B
+    rng = np.random.default_rng(2024)
+    worst = {"eigen": 0.0, "span": 0.0, "solve": 0.0}
+    for i in range(600):
+        A = B.spectrum_matrix(rng, ("spread", "cluster", "null4", "equal", "mtm")[i % 5])
+        sig, V, _ = P.svd(A.tolist())
+        e, sp, _ = B.eigen_ratios(sig, [V[j][r] for r in range(12) for j in range(12)], A)
+        worst["eigen"], worst["span"] = max(worst["eigen"], e), max(worst["span"], sp)
+    skipped = 0
+    for i in range(2400):
+        K = 3 + i % 3
+        A = rng.normal(size=(6, K)) * 10.0 ** rng.uniform(-3, 3, K)
+        if i % 7 == 0:
+            A[:, -1] = A[:, 0] + 10.0 ** rng.uniform(-12, -6) * np.abs(A).max() * rng.normal(size=6)  # nearly dependent
+        b = A @ rng.normal(size=K) + (rng.normal(size=6) * 10.0 ** rng.uniform(-6, 0) if i % 2 else 0.0)
+        r = B.solve_ratio(A, b)
+        if r is None:
+            skipped += 1
+            continue
+        worst["solve"] = max(worst["solve"], r)
+    print("largest ratio to the bound:", {k: round(v, 2) for k, v in worst.items()}, f"({skipped} solves below the threshold)")
+    assert max(worst.values()) <= B.C and skipped < 2400 // 14
+
+
+def test_compute_pose_within_its_bounds_across_conditioning():
+    """The oracle's compute_pose (the device's, bit for bit) on noise-free scenes from 5 m to 300 m depth, spread 1 m to 1 cm,
+    thickness 1 m to 1 mm: every decomposition within its bound; the pose error against the true pose is printed."""
+    from oracle import pnp_bounds as B
+    worst = [0.0, 0.0, 0.0]
+    for D, s, h in B.CONDITIONING:
+        X, us, R, t = B.conditioned_scene(D, s, h, n=20)
+        d = P.compute_pose(X.astype(np.float64).tolist(), us.astype(np.float64).tolist(), *(float(np.float32(c)) for c in F), tree=True)
+        r = B.check_pose_debug(d.alphas, us, d, F)
+        worst = [max(a, b) for a, b in zip(worst, r)]
+        print(f"depth {D:5.0f} m spread {s:5.2f} m thickness {h:6.3f} m: pose error R {B.pose_error(d.R, d.t, R, t)[0]:.1e} "
+              f"t {B.pose_error(d.R, d.t, R, t)[1]:.1e}; ratios {[round(x, 2) for x in r]}")
+    assert max(worst) <= B.C, worst
