@@ -47,6 +47,40 @@ TH_LOW = 50
 TF_IDF, TF, IDF, BINARY = range(4)
 L1_NORM, L2_NORM, CHI_SQUARE, KL, BHATTACHARYYA, DOT_PRODUCT = range(6)
 
+# The paths the optional `trace` of Tree.descend, transform and search_by_bow records (oracle/bow_scene.py builds cases for each).
+DESCENT_PATHS = (
+    "tie_first_child",    # a later child at the best distance: the first keeps it
+    "tie_across_stride",  # the winner at child position < 32, a tied child at >= 32 (the warp's second lane stride)
+    "best_past_stride",   # the winner at child position >= 32
+    "leaf_above_nid",     # the path ends at a leaf above nid_level: the leaf is the node
+    "nid_root",           # levelsup >= L: the node is the root
+)
+TRANSFORM_PATHS = (
+    "stopped_word",            # w > 0 fails: 0, negative, -0.0 or NaN
+    "tf_repeat",               # TF / TF_IDF: a further feature on a word already in the vector
+    "tf_divide",               # DOT_PRODUCT with TF / TF_IDF: each weight / the number of words
+    "norm_zero",               # a non-empty vector whose norm is 0 (subnormal squares): nothing is divided
+    "norm_inf",                # the norm overflows to inf (or sums an inf weight): finite weights become 0, inf / inf NaN
+    "empty_vector_with_keys",  # keys, but every one on a stopped word
+)
+SEARCH_PATHS = (
+    "node_frame_only", "node_kf_only",   # a node in one FeatureVector only
+    "kf_key_no_point",                   # a keyframe key without a point is not searched
+    "candidate_claimed",                 # a frame key matched earlier in the call is skipped
+    "best_tie", "second_tie",            # a later candidate at the best / second distance
+    "th_low_50_accept", "th_low_51_reject",
+    "ratio_equal_reject",                # bestDist == nnratio * bestDist2 in float
+    "ratio_ulp_accept",                  # nnratio * bestDist2 one float above bestDist
+    "single_candidate",                  # accepted with bestDist2 = 256
+    "rot_wrap", "rot_zero",              # rot < 0 then + 360; rot exactly 0 (not wrapped)
+    "bin_half_up",                       # rot * (1 / 30) exactly k + 0.5: rounded up
+    "bin_12",                            # rot = 360
+    "bin_30_to_0",                       # the reference's 30 -> 0 rule
+    "three_maxima_0", "three_maxima_1", "three_maxima_2", "three_maxima_3",  # bins kept
+    "tenth_rule_equal", "tenth_rule_cull",  # max2 / max3 at exactly 0.1f * max1 (kept) and below it (culled)
+    "no_orientation",
+)
+
 
 class FormatError(ValueError):
     pass
@@ -162,27 +196,40 @@ class Tree:
         self.word_weight = np.asarray(t["weight"], np.float64)[leaves]
         self.n_words = len(leaves)
 
-    def descend(self, d, levelsup):
-        """transform(feature, word_id, weight, &nid, levelsup) -> (word, weight, nid)."""
+    def descend(self, d, levelsup, trace=None):
+        """transform(feature, word_id, weight, &nid, levelsup) -> (word, weight, nid).  trace: a set that receives the names of
+        the descent paths taken (DESCENT_PATHS)."""
         d = np.asarray(d, np.uint8)
         nid_level = self.L - levelsup
         nid = 0 if nid_level <= 0 else None
+        if trace is not None and nid_level <= 0:
+            trace.add("nid_root")
         final, level = 0, 0
         while True:
             level += 1
             nodes = self.children[final]
             dist = np.unpackbits(np.bitwise_xor(self.desc[nodes], d), axis=1).sum(axis=1)
             final = nodes[0]
-            best = float(dist[0])
-            for c, dc in zip(nodes[1:], dist[1:]):
+            best, pos = float(dist[0]), 0
+            for p, (c, dc) in enumerate(zip(nodes[1:], dist[1:]), 1):
                 if float(dc) < best:
-                    best, final = float(dc), c
+                    best, final, pos = float(dc), c, p
+            if trace is not None:
+                tied = [p for p in range(pos + 1, len(nodes)) if float(dist[p]) == best]
+                if tied:
+                    trace.add("tie_first_child")
+                if pos < 32 and any(p >= 32 for p in tied):
+                    trace.add("tie_across_stride")
+                if pos >= 32:
+                    trace.add("best_past_stride")
             if level == nid_level:
                 nid = final
             if not self.children[final]:
                 break
         if nid is None:
             nid = final  # a leaf above nid_level: the leaf itself
+            if trace is not None:
+                trace.add("leaf_above_nid")
         w = int(self.word[final])
         return w, float(self.word_weight[w]), int(nid)
 
@@ -194,7 +241,7 @@ def must_normalize(scoring):
     return True, ("L2" if scoring == L2_NORM else "L1")
 
 
-def normalize(bow: dict, norm: str):
+def normalize(bow: dict, norm: str, trace=None):
     """BowVector::normalize over a dict walked in ascending word order."""
     s = 0.0
     if norm == "L1":
@@ -204,34 +251,48 @@ def normalize(bow: dict, norm: str):
         for w in sorted(bow):
             s += bow[w] * bow[w]
         s = math.sqrt(s)
+    if trace is not None and bow:
+        if s == 0.0:
+            trace.add("norm_zero")  # every square underflowed: nothing is divided
+        elif s == math.inf:
+            trace.add("norm_inf")   # finite weights become 0, an infinite one NaN
     if s > 0.0:
         for w in sorted(bow):
             bow[w] /= s
 
 
-def transform(tree: Tree, descs, levelsup):
+def transform(tree: Tree, descs, levelsup, trace=None):
     """transform(features, v, fv, levelsup) -> (bow {word: weight}, fv {node: [feature indices]}, node per key, word per key);
-    node / word -1 for a key in neither vector."""
+    node / word -1 for a key in neither vector.  trace: a set that receives the names of the paths taken (DESCENT_PATHS and
+    TRANSFORM_PATHS)."""
     must, norm = must_normalize(tree.scoring)
     bow, fv = {}, {}
     n = len(descs)
     node, word = np.full(n, -1, np.int32), np.full(n, -1, np.int32)
     tf = tree.weighting in (TF, TF_IDF)
     for i in range(n):
-        w_id, w, nid = tree.descend(descs[i], levelsup)
+        w_id, w, nid = tree.descend(descs[i], levelsup, trace)
         if w > 0:
             if tf:
+                if trace is not None and w_id in bow:
+                    trace.add("tf_repeat")
                 bow[w_id] = bow[w_id] + w if w_id in bow else w
             elif w_id not in bow:
                 bow[w_id] = w
             fv.setdefault(nid, []).append(i)
             node[i], word[i] = nid, w_id
+        elif trace is not None:
+            trace.add("stopped_word")  # w = 0, negative, -0.0 or NaN
+    if trace is not None and n and not bow:
+        trace.add("empty_vector_with_keys")
     if tf and bow and not must:
+        if trace is not None:
+            trace.add("tf_divide")
         nd = float(len(bow))
         for w_id in bow:
             bow[w_id] /= nd
     if must:
-        normalize(bow, norm)
+        normalize(bow, norm, trace)
     return bow, fv, node, word
 
 
@@ -250,19 +311,63 @@ def feature_vector(node, angles) -> dict:
     return fv
 
 
-def rotation_bin(kf_angle, f_angle) -> int:
+def rotation_bin(kf_angle, f_angle, trace=None) -> int:
     rot = F32(kf_angle) - F32(f_angle)
     if rot < F32(0):
         rot = rot + F32(360)
-    b = int(round_half_away(rot * (F32(1) / F32(HISTO_LENGTH))))
+        if trace is not None:
+            trace.add("rot_wrap")
+    q = rot * (F32(1) / F32(HISTO_LENGTH))
+    b = int(round_half_away(q))
+    if trace is not None:
+        if rot == F32(0):
+            trace.add("rot_zero")
+        if q == F32(math.floor(q)) + F32(0.5):
+            trace.add("bin_half_up")
+        if rot == F32(360):
+            trace.add("bin_12")
+        if b == HISTO_LENGTH:
+            trace.add("bin_30_to_0")
     return 0 if b == HISTO_LENGTH else b
 
 
-def search_by_bow(f_kps, f_desc, f_node, kf_kps, kf_desc, kf_node, kf_point, nnratio, check_orientation):
-    """SearchByBoW(pKF, F, vpMapPointMatches) as the literal loop -> (match int32 per frame key: the point index or -1, nmatches)."""
+def _trace_accept(trace, best1, best2, nnratio, accept):
+    bound = nnratio * F32(best2)
+    if best2 == 256 and accept:
+        trace.add("single_candidate")
+    if best1 == TH_LOW and accept:
+        trace.add("th_low_50_accept")
+    if best1 == TH_LOW + 1 and F32(best1) < bound:
+        trace.add("th_low_51_reject")  # the ratio test alone would accept
+    if best1 <= TH_LOW and F32(best1) == bound:
+        trace.add("ratio_equal_reject")
+    if accept and bound == np.nextafter(F32(best1), F32(np.inf)):
+        trace.add("ratio_ulp_accept")
+
+
+def _trace_maxima(trace, counts, keep):
+    top = sorted(counts, reverse=True)[:3]  # ComputeThreeMaxima's max1, max2, max3
+    trace.add(f"three_maxima_{sum(i >= 0 for i in keep)}")
+    tenth = F32(0.1) * F32(top[0])
+    if any(0 < m and F32(m) == tenth for m in top[1:]):
+        trace.add("tenth_rule_equal")
+    if any(0 < m and F32(m) < tenth for m in top[1:]):
+        trace.add("tenth_rule_cull")
+
+
+def search_by_bow(f_kps, f_desc, f_node, kf_kps, kf_desc, kf_node, kf_point, nnratio, check_orientation, trace=None):
+    """SearchByBoW(pKF, F, vpMapPointMatches) as the literal loop -> (match int32 per frame key: the point index or -1, nmatches).
+    trace: a set that receives the names of the paths taken (SEARCH_PATHS)."""
     fv_f = feature_vector(f_node, f_kps["angle"])
     fv_kf = feature_vector(kf_node, kf_kps["angle"])
     kf_keys, f_keys = sorted(fv_kf), sorted(fv_f)
+    if trace is not None:
+        if set(f_keys) - set(kf_keys):
+            trace.add("node_frame_only")
+        if set(kf_keys) - set(f_keys):
+            trace.add("node_kf_only")
+        if not check_orientation:
+            trace.add("no_orientation")
     n = len(f_kps)
     match = np.full(n, -1, np.int32)
     nnratio = F32(nnratio)
@@ -274,20 +379,32 @@ def search_by_bow(f_kps, f_desc, f_node, kf_kps, kf_desc, kf_node, kf_point, nnr
             for i_kf in fv_kf[kf_keys[a]]:
                 p = int(kf_point[i_kf])
                 if p < 0:
+                    if trace is not None:
+                        trace.add("kf_key_no_point")
                     continue
                 best1, best_idx, best2 = 256, -1, 256
                 for i_f in fv_f[f_keys[b]]:
                     if match[i_f] >= 0:
+                        if trace is not None:
+                            trace.add("candidate_claimed")
                         continue
                     d = descriptor_distance(kf_desc[i_kf], f_desc[i_f])
+                    if trace is not None and d < 256:
+                        if d == best1:
+                            trace.add("best_tie")    # the earlier candidate stays best
+                        elif d == best2:
+                            trace.add("second_tie")  # changes nothing
                     if d < best1:
                         best2, best1, best_idx = best1, d, i_f
                     elif d < best2:
                         best2 = d
-                if best1 <= TH_LOW and F32(best1) < nnratio * F32(best2):
+                accept = best1 <= TH_LOW and F32(best1) < nnratio * F32(best2)
+                if trace is not None:
+                    _trace_accept(trace, best1, best2, nnratio, accept)
+                if accept:
                     match[best_idx] = p
                     if check_orientation:
-                        rot_hist[rotation_bin(kf_kps["angle"][i_kf], f_kps["angle"][best_idx])].append(best_idx)
+                        rot_hist[rotation_bin(kf_kps["angle"][i_kf], f_kps["angle"][best_idx], trace)].append(best_idx)
                     nmatches += 1
             a += 1
             b += 1
@@ -296,7 +413,10 @@ def search_by_bow(f_kps, f_desc, f_node, kf_kps, kf_desc, kf_node, kf_point, nnr
         else:
             b = bisect.bisect_left(f_keys, kf_keys[a])
     if check_orientation:
-        keep = compute_three_maxima([len(h) for h in rot_hist])
+        counts = [len(h) for h in rot_hist]
+        keep = compute_three_maxima(counts)
+        if trace is not None:
+            _trace_maxima(trace, counts, keep)
         for i in range(HISTO_LENGTH):
             if i in keep:
                 continue

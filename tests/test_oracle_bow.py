@@ -206,3 +206,67 @@ def test_rotation_bin_half_rounds_away():
     assert B.rotation_bin(np.float32(15), np.float32(0)) == 1
     assert B.rotation_bin(np.float32(0), np.float32(15)) == 12
     assert B.rotation_bin(np.float32(360), np.float32(0)) == 12
+
+
+# ---------------------------------------------------------------------------------------------------------- constructed cases
+TRANSFORM_CASES = S.transform_cases()
+SEARCH_CASES = S.search_cases()
+
+
+@pytest.mark.parametrize("case", TRANSFORM_CASES, ids=lambda c: c.name)
+def test_transform_case_reaches_its_paths(case):
+    got = S.transform_paths(case)
+    assert case.paths <= got, sorted(case.paths - got)
+    assert got <= set(S.PATHS), sorted(got - set(S.PATHS))
+    # the trace changes nothing
+    tree = B.Tree(case.tree)
+    plain = B.transform(tree, case.desc, case.levelsup)
+    traced = B.transform(tree, case.desc, case.levelsup, trace=set())
+    w0, v0 = B.bow_arrays(plain[0])
+    w1, v1 = B.bow_arrays(traced[0])
+    np.testing.assert_array_equal(w0, w1)
+    np.testing.assert_array_equal(v0.view(np.uint64), v1.view(np.uint64))
+    np.testing.assert_array_equal(plain[2], traced[2])
+
+
+@pytest.mark.parametrize("case", SEARCH_CASES, ids=lambda c: c.name)
+def test_search_case_reaches_its_paths(case):
+    got = S.search_paths(case)
+    assert case.paths <= got, sorted(case.paths - got)
+    assert got <= set(S.PATHS), sorted(got - set(S.PATHS))
+    f = case.frame
+    for kf in S._live(case):
+        args = (f["kps"], f["desc"], f["node"], kf["kps"], kf["desc"], kf["node"], kf["point"], case.ratio, case.check)
+        m0, n0 = B.search_by_bow(*args)
+        m1, n1 = B.search_by_bow(*args, trace=set())
+        np.testing.assert_array_equal(m0, m1)
+        assert n0 == n1
+
+
+def test_the_cases_reach_every_path():
+    reached = set()
+    for c in TRANSFORM_CASES:
+        reached |= S.transform_paths(c)
+    for c in SEARCH_CASES:
+        reached |= S.search_paths(c)
+    assert len(set(S.PATHS)) == len(S.PATHS)
+    assert set(S.PATHS) - reached == set(S.UNREACHED), sorted(set(S.PATHS) - reached)
+
+
+def test_the_unreached_bin_needs_an_angle_outside_the_rule():
+    # every float rot the rule allows: [0, 360] after the wrap; the largest gives bin 12
+    assert B.rotation_bin(np.float32(360), np.float32(0)) == 12
+    assert B.rotation_bin(np.float32(0), np.float32(np.nextafter(np.float32(0), np.float32(1)))) == 12
+    t = set()
+    assert B.rotation_bin(np.float32(900), np.float32(0), t) == 0 and "bin_30_to_0" in t  # 900 breaks the angle rule
+
+
+def test_the_fuzz_cases_agree_with_the_per_node_form():
+    for seed in range(0, 200, 5):
+        c = S.fuzz_case(seed)
+        for kf in S._live(c):
+            m, nm = B.search_by_bow(c.frame["kps"], c.frame["desc"], c.frame["node"], kf["kps"], kf["desc"], kf["node"], kf["point"],
+                                    c.ratio, c.check)
+            m2, nm2 = _search_by_node(c.frame, kf, c.ratio, c.check)
+            np.testing.assert_array_equal(m, m2)
+            assert nm == nm2
