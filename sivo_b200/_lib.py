@@ -22,11 +22,6 @@ class SivoError(RuntimeError):
         self.code = code
 
 
-class Keypoint(C.Structure):
-    _fields_ = [("x", C.c_float), ("y", C.c_float), ("size", C.c_float), ("angle", C.c_float),
-                ("response", C.c_float), ("octave", C.c_int32), ("class_id", C.c_int32)]
-
-
 class SegnetOptions(C.Structure):
     _fields_ = [("device", C.c_int32), ("T", C.c_int32), ("seed", C.c_uint64), ("precision", C.c_int32),
                 ("engine", C.c_int32), ("keep_blobs", C.c_int32), ("reserved", C.c_int32)]
@@ -48,59 +43,77 @@ def build(verbose: bool = False) -> str:
     return LIB_PATH
 
 
+# Every C type in the header's prototypes: the scalars by name, `const char*` as a string, every other pointer (handles, struct
+# and array pointers, `T**`, `T* const*`, the `char*` a string buffer is passed for) as an address.  A type outside these tables
+# fails the load, so no declared function is ever called untyped.
+_SCALARS = {"int": C.c_int32, "int32_t": C.c_int32, "uint32_t": C.c_uint32, "uint64_t": C.c_uint64, "size_t": C.c_size_t,
+            "float": C.c_float, "double": C.c_double}
+_RETURNS = {"int": C.c_int, "void": None, "const char*": C.c_char_p}
+
+
+def _type(t: str) -> str:
+    return re.sub(r" ?\* ?", "*", " ".join(t.split()))
+
+
+def _param(decl: str, name: str):
+    t = _type(re.sub(r"\b[A-Za-z_]\w*\s*$", "", decl))  # drop the parameter's name
+    if "*" in t:
+        return C.c_char_p if t == "const char*" else C.c_void_p
+    if t.removeprefix("const ") not in _SCALARS:
+        raise ValueError(f"{name}: parameter {decl.strip()!r} has no ctypes type")
+    return _SCALARS[t.removeprefix("const ")]
+
+
+def prototypes(text: str = None) -> dict:
+    """{name: (restype, argtypes)} of every sivo_* function declared in `text` (default: include/sivo_b200.h).  Raises
+    ValueError, naming the function, for a type outside the mapping."""
+    if text is None:
+        with open(HEADER) as f:
+            text = f.read()
+    text = re.sub(r"/\*.*?\*/", "", text, flags=re.S)
+    text = re.sub(r"^\s*#.*$", "", text, flags=re.M)
+    out = {}
+    for stmt in re.split(r"[;{}]", text):
+        m = re.fullmatch(r"\s*(.*?)\b(sivo_[a-z0-9_]+)\s*\((.*)\)\s*", stmt, flags=re.S)
+        if m is None:
+            continue
+        ret, name, params = _type(m[1]), m[2], m[3]
+        if ret not in _RETURNS:
+            raise ValueError(f"{name}: return type {ret!r} has no ctypes type")
+        params = [] if _type(params) in ("", "void") else params.split(",")
+        out[name] = (_RETURNS[ret], [_param(p, name) for p in params])
+    return out
+
+
+def declared_symbols() -> list:
+    """Every function name declared in include/sivo_b200.h."""
+    return sorted(prototypes())
+
+
+def ptr(a):
+    """The address of numpy array `a` for a pointer parameter (None: NULL).  The returned object keeps `a` alive."""
+    return None if a is None else a.ctypes.data_as(C.c_void_p)
+
+
 _lib = None
 
 
 def lib() -> C.CDLL:
+    """The library, every declared function typed from the header (argtypes / restype) before first use."""
     global _lib
     if _lib is None:
         if not os.path.exists(LIB_PATH):
             raise ImportError(f"{LIB_PATH} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` "
                               "(there is no CPU fallback)")
-        _lib = C.CDLL(LIB_PATH)
-        _lib.sivo_last_error.restype = C.c_char_p
-        _lib.sivo_version.restype = C.c_char_p
-        _lib.sivo_segnet_destroy.restype = None
-        _lib.sivo_orb_destroy.restype = None
-        vp, i32, f32 = C.c_void_p, C.c_int, C.c_float
-        _lib.sivo_segnet_semantic_keys_device.argtypes = [vp, vp, vp, i32, i32, vp, vp, vp, vp, vp, vp]
-        _lib.sivo_stereo_match_device.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, f32, f32, vp, vp, vp]
-        _lib.sivo_info_select.argtypes = [vp, vp, vp, vp, i32, vp, C.c_double, vp, vp, vp, vp]
-        _lib.sivo_info_select_device.argtypes = [vp, vp, vp, vp, vp, vp, vp, C.c_double, vp, vp, vp, vp, vp]
-        _lib.sivo_dbg_info_terms.argtypes = [vp, vp, vp, i32, vp, vp, vp, vp, vp]
-        _lib.sivo_search_local_points_device.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, i32, vp, f32, f32, vp, vp, vp, vp]
-        _lib.sivo_search_last_frame_device.argtypes = [vp, vp, vp, vp, vp, vp, vp, i32, vp, vp, vp, f32, vp, vp, vp]
-        _lib.sivo_search_local_points.argtypes = [vp, vp, vp, vp, vp, i32, vp, i32, vp, f32, f32, vp, vp, vp]
-        _lib.sivo_search_last_frame.argtypes = [vp, vp, vp, vp, i32, vp, i32, vp, vp, vp, f32, vp, vp]
-        _lib.sivo_dbg_features_in_area.argtypes = [vp, vp, i32, f32, f32, f32, f32, vp, vp, i32, vp, vp, i32]
-        _lib.sivo_pose_optimize_device.argtypes = [vp, vp, vp, vp, vp, vp, f32, f32, f32, f32, f32, vp, vp, vp, vp]
-        _lib.sivo_pose_gather_device.argtypes = [vp, vp, vp, vp, i32, vp, vp]
-        _lib.sivo_pose_optimize.argtypes = [vp, vp, vp, vp, i32, f32, f32, f32, f32, f32, vp, vp, vp]
-        _lib.sivo_dbg_pose_system.argtypes = [vp, vp, vp, vp, i32, f32, f32, f32, f32, f32, vp, i32, vp, vp, vp, vp, vp, vp, vp, vp]
-        _lib.sivo_dbg_pose_trace.argtypes = [vp, vp, vp, vp, i32, f32, f32, f32, f32, f32, vp, vp, vp, vp, i32]
-        _lib.sivo_dbg_pose_se3.argtypes = [i32, i32, vp, vp, vp, vp, vp, vp]
-        _lib.sivo_keyframe_gather_device.argtypes = [vp] * 19
-        _lib.sivo_create_map_points_device.argtypes = [vp, vp, vp, i32, vp, vp, vp, vp, vp, vp, vp]
-        _lib.sivo_create_map_points.argtypes = [vp, vp, vp, i32, vp, vp, vp, vp, vp, vp]
-        _lib.sivo_dbg_create_map_points.argtypes = [vp, vp, vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
-        _lib.sivo_vocabulary_destroy.restype = None
-        _lib.sivo_vocabulary_load_text.argtypes = [C.c_char_p, i32, vp]
-        _lib.sivo_vocabulary_create.argtypes = [i32, i32, i32, i32, i32, vp, vp, vp, vp, i32, vp]
-        _lib.sivo_dbg_vocabulary_parse.argtypes = [C.c_char_p, vp, vp, vp, vp, vp, vp, i32]
-        _lib.sivo_compute_bow_device.argtypes = [vp, vp, vp, vp, vp, i32, vp, vp, vp, vp, vp, vp]
-        _lib.sivo_compute_bow.argtypes = [vp, vp, i32, i32, vp, vp, vp, vp, vp]
-        _lib.sivo_search_by_bow_device.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, i32, f32, i32, vp, vp, vp]
-        _lib.sivo_search_by_bow.argtypes = [vp, vp, vp, vp, i32, vp, vp, i32, f32, i32, vp, vp]
-        _lib.sivo_pnp_destroy.restype = None
-        _lib.sivo_pnp_create.argtypes = [vp, i32, C.c_uint64, vp]
-        _lib.sivo_pnp_setup_device.argtypes = [vp, vp, vp, vp, vp, vp, vp, i32, vp, i32, C.c_uint64, f32, f32, f32, f32, vp]
-        _lib.sivo_pnp_iterate_device.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, vp]
-        _lib.sivo_dbg_pnp_state.argtypes = [vp, vp, vp]
-        d64 = C.c_double
-        _lib.sivo_dbg_pnp_compute_pose.argtypes = [i32, vp, vp, vp, i32, f32, f32, f32, f32, vp, vp, vp, vp]
-        _lib.sivo_dbg_pnp_hypotheses.argtypes = [vp, i32, i32, i32, vp, vp, vp, vp]
-        _lib.sivo_dbg_pnp_draws.argtypes = [i32, C.c_uint64, C.c_uint32, C.c_uint64, i32, i32, i32, vp]
-        _lib.sivo_dbg_conv_unpooled.argtypes = [i32, vp, vp, i32, i32, i32, i32, vp, vp, vp, vp, i32, i32, vp]
+        dll = C.CDLL(LIB_PATH)
+        protos = prototypes()
+        missing = [s for s in sorted(protos) if not hasattr(dll, s)]
+        if missing:
+            raise RuntimeError(f"{LIB_PATH} does not export {missing}")
+        for name, (restype, argtypes) in protos.items():
+            fn = getattr(dll, name)
+            fn.restype, fn.argtypes = restype, argtypes
+        _lib = dll
     return _lib
 
 
@@ -108,10 +121,3 @@ def check(rc: int) -> int:
     if rc < 0:
         raise SivoError(rc, lib().sivo_last_error().decode(errors="replace"))
     return rc
-
-
-def declared_symbols() -> list:
-    """Every function name declared in include/sivo_b200.h (for the export test)."""
-    text = open(HEADER).read()
-    text = re.sub(r"/\*.*?\*/", "", text, flags=re.S)
-    return sorted(set(re.findall(r"\b(sivo_[a-z0-9_]+)\s*\(", text)))

@@ -15,10 +15,6 @@ WEIGHTINGS = ("TF_IDF", "TF", "IDF", "BINARY")
 SCORINGS = ("L1_NORM", "L2_NORM", "CHI_SQUARE", "KL", "BHATTACHARYYA", "DOT_PRODUCT")
 
 
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p)
-
-
 class Vocabulary:
     """A vocabulary on one device (read-only: any thread may use it)."""
 
@@ -42,7 +38,8 @@ class Vocabulary:
         if not (len(par) == len(leaf) == len(d) == len(w)):
             raise ValueError("every node array needs one entry per node")
         h = C.c_void_p()
-        L.check(L.lib().sivo_vocabulary_create(device, k, L_, scoring, weighting, _p(par), _p(leaf), _p(d), _p(w), len(par), C.byref(h)))
+        L.check(L.lib().sivo_vocabulary_create(device, k, L_, scoring, weighting, L.ptr(par), L.ptr(leaf), L.ptr(d), L.ptr(w),
+                                               len(par), C.byref(h)))
         return cls(h, device)
 
     def info(self) -> dict:
@@ -67,12 +64,13 @@ def parse_text(path: str) -> dict:
     weight); raises SivoError (SIVO_EFORMAT / SIVO_ENOENT) as the loader would."""
     hdr = np.zeros(4, np.int32)
     n = C.c_int(0)
-    rc = L.lib().sivo_dbg_vocabulary_parse(str(path).encode(), _p(hdr), C.byref(n), None, None, None, None, 0)
+    rc = L.lib().sivo_dbg_vocabulary_parse(str(path).encode(), L.ptr(hdr), C.byref(n), None, None, None, None, 0)
     if rc != L.ERANGE:
         L.check(rc)
     par, leaf = np.empty(n.value, np.int32), np.empty(n.value, np.uint8)
     desc, w = np.empty((n.value, 32), np.uint8), np.empty(n.value, np.float64)
-    L.check(L.lib().sivo_dbg_vocabulary_parse(str(path).encode(), _p(hdr), C.byref(n), _p(par), _p(leaf), _p(desc), _p(w), n.value))
+    L.check(L.lib().sivo_dbg_vocabulary_parse(str(path).encode(), L.ptr(hdr), C.byref(n), L.ptr(par), L.ptr(leaf), L.ptr(desc),
+                                              L.ptr(w), n.value))
     return dict(k=int(hdr[0]), L=int(hdr[1]), scoring=int(hdr[2]), weighting=int(hdr[3]), parent=par, is_leaf=leaf, desc=desc, weight=w)
 
 
@@ -84,7 +82,7 @@ def compute_bow(voc: Vocabulary, desc, levelsup: int = 4) -> dict:
     node, word = np.empty(max(n, 1), np.int32), np.empty(max(n, 1), np.int32)
     bw, bwt = np.empty(max(n, 1), np.int32), np.empty(max(n, 1), np.float64)
     m = C.c_int(0)
-    L.check(L.lib().sivo_compute_bow(voc._h, _p(d), n, levelsup, _p(node), _p(word), _p(bw), _p(bwt), C.byref(m)))
+    L.check(L.lib().sivo_compute_bow(voc._h, L.ptr(d), n, levelsup, L.ptr(node), L.ptr(word), L.ptr(bw), L.ptr(bwt), C.byref(m)))
     return dict(node=node[:n].copy(), word=word[:n].copy(), bow_words=bw[:m.value].copy(), bow_weights=bwt[:m.value].copy())
 
 
@@ -93,9 +91,8 @@ def compute_bow_device(voc: Vocabulary, left: ORBextractor, desc_ptr: int, keep_
                        stream: int = 0):
     """sivo_compute_bow_device on device pointers (0: not wanted / identity keep_idx); outputs of left.capacity() keys.  Enqueued
     on `stream` (0 = the left extractor's stream) with no waits and no host synchronisation."""
-    L.check(L.lib().sivo_compute_bow_device(voc._h, left._h, desc_ptr, keep_idx_ptr or None, n_keep_ptr, levelsup, node_ptr or None,
-                                            word_ptr or None, bow_word_ptr or None, bow_weight_ptr or None, bow_len_ptr or None,
-                                            stream or None))
+    L.check(L.lib().sivo_compute_bow_device(voc._h, left._h, desc_ptr, keep_idx_ptr, n_keep_ptr, levelsup, node_ptr, word_ptr,
+                                            bow_word_ptr, bow_weight_ptr, bow_len_ptr, stream))
 
 
 def keyframe_keys(kps_ptr: int, desc_ptr: int, node_ptr: int, count_ptr: int) -> KeyframeKeys:
@@ -134,8 +131,8 @@ def search_by_bow(left: ORBextractor, kps, desc, node, keyframes, nnratio: float
     nk = len(keys)
     match = np.full((max(nk, 1), max(n, 1)), -1, np.int32)
     nm = np.zeros(max(nk, 1), np.int64)
-    L.check(L.lib().sivo_search_by_bow(left._h, _p(k), _p(d), _p(nd), n, arr, pts, nk, nnratio, int(bool(check_orientation)),
-                                       _p(match), _p(nm)))
+    L.check(L.lib().sivo_search_by_bow(left._h, L.ptr(k), L.ptr(d), L.ptr(nd), n, arr, pts, nk, nnratio, int(bool(check_orientation)),
+                                       L.ptr(match), L.ptr(nm)))
     return match[:nk, :n].copy(), nm[:nk].copy()
 
 
@@ -144,6 +141,5 @@ def search_by_bow_device(left: ORBextractor, kps_ptr: int, desc_ptr: int, keep_i
     """sivo_search_by_bow_device: keyframes = KeyframeKeys with device pointers (keyframe_keys()), kf_point_ptrs one device int
     array per keyframe; match_ptr holds len(keyframes) rows of left.capacity() ints, n_matches_ptr one int64 per keyframe."""
     arr, pts = _kf_table(list(keyframes), list(kf_point_ptrs))
-    L.check(L.lib().sivo_search_by_bow_device(left._h, kps_ptr, desc_ptr, keep_idx_ptr or None, n_keep_ptr, node_ptr, arr, pts,
-                                              len(keyframes), nnratio, int(bool(check_orientation)), match_ptr, n_matches_ptr,
-                                              stream or None))
+    L.check(L.lib().sivo_search_by_bow_device(left._h, kps_ptr, desc_ptr, keep_idx_ptr, n_keep_ptr, node_ptr, arr, pts, len(keyframes),
+                                              nnratio, int(bool(check_orientation)), match_ptr, n_matches_ptr, stream))

@@ -24,10 +24,6 @@ def make_camera(fx, fy, cx, cy, mb, Rwc, Ow, sigma_cw) -> InfoCamera:
     return cam
 
 
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p)
-
-
 def info_select(left: ORBextractor, kps, depth, entropy, camera: InfoCamera, threshold: float):
     """Host form: kps / depth / entropy gathered per semantic key (mvKeysSemantic, mvDepth, mEntropy at the key).
     Returns (world (n, 3) float32, reduction float64, selected int32 ascending)."""
@@ -41,8 +37,8 @@ def info_select(left: ORBextractor, kps, depth, entropy, camera: InfoCamera, thr
     red = np.empty(n, np.float64)
     sel = np.empty(max(n, 1), np.int32)
     ns = C.c_int(0)
-    L.check(L.lib().sivo_info_select(left._h, _p(k), _p(z), _p(h), n, C.byref(camera), threshold, _p(world), _p(red), _p(sel),
-                                     C.byref(ns)))
+    L.check(L.lib().sivo_info_select(left._h, L.ptr(k), L.ptr(z), L.ptr(h), n, C.byref(camera), threshold, L.ptr(world), L.ptr(red),
+                                     L.ptr(sel), C.byref(ns)))
     return world, red, sel[:ns.value].copy()
 
 
@@ -52,9 +48,8 @@ def info_select_device(left: ORBextractor, kps_ptr: int, kp_entropy_ptr: int, ke
     """info_select on device buffers (sivo_info_select_device): semantic key j is extractor key keep_idx[j] (keep_idx_ptr 0: key j)
     for j < the int64 count at n_keep_ptr; outputs of left.capacity() keys (any pointer may be 0), *n_selected int64.  Runs on
     `stream` (0 = the left extractor's stream) without waits of its own and without a host synchronisation."""
-    L.check(L.lib().sivo_info_select_device(left._h, kps_ptr, kp_entropy_ptr, keep_idx_ptr or None, n_keep_ptr, depth_ptr, C.byref(camera),
-                                            threshold, world_ptr or None, reduction_ptr or None, selected_ptr or None,
-                                            n_selected_ptr or None, stream or None))
+    L.check(L.lib().sivo_info_select_device(left._h, kps_ptr, kp_entropy_ptr, keep_idx_ptr, n_keep_ptr, depth_ptr, C.byref(camera),
+                                            threshold, world_ptr, reduction_ptr, selected_ptr, n_selected_ptr, stream))
 
 
 def info_terms(left: ORBextractor, kps, depth, camera: InfoCamera):
@@ -64,5 +59,5 @@ def info_terms(left: ORBextractor, kps, depth, camera: InfoCamera):
     n = len(k)
     world = np.empty((n, 3), np.float32)
     dets = [np.empty(n, np.float64) for _ in range(3)]
-    L.check(L.lib().sivo_dbg_info_terms(left._h, _p(k), _p(z), n, C.byref(camera), _p(world), *(_p(d) for d in dets)))
+    L.check(L.lib().sivo_dbg_info_terms(left._h, L.ptr(k), L.ptr(z), n, C.byref(camera), L.ptr(world), *(L.ptr(d) for d in dets)))
     return (world, *dets)

@@ -72,10 +72,6 @@ def _nb_array(neighbours):
     return arr
 
 
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p)
-
-
 def create_map_points(left: ORBextractor, kf1: HostKeyframe, neighbours, params: MappingParams, debug=False):
     """Host form (debug: the test hook, every key searched).  Returns a dict: created_nb, created_idx, world (n1, 3), created
     (m, 2) pairs (neighbour, key), n_created; with debug also match / stage / reduction (n_neighbours, n1)."""
@@ -86,11 +82,11 @@ def create_map_points(left: ORBextractor, kf1: HostKeyframe, neighbours, params:
     nc = C.c_longlong(0)
     nbs = _nb_array([k.keys for k in neighbours])
     common = (left._h, C.byref(kf1.keys), nbs, nn, C.byref(params))
-    tail = (_p(out["created_nb"]), _p(out["created_idx"]), _p(out["world"]), _p(out["created"]), C.byref(nc))
+    tail = (L.ptr(out["created_nb"]), L.ptr(out["created_idx"]), L.ptr(out["world"]), L.ptr(out["created"]), C.byref(nc))
     if debug:
         for k, dt in (("match", np.int32), ("stage", np.int32), ("reduction", np.float64)):
             out[k] = np.empty((nn, n1), dt)
-        L.check(L.lib().sivo_dbg_create_map_points(*common, _p(out["match"]), _p(out["stage"]), _p(out["reduction"]), *tail))
+        L.check(L.lib().sivo_dbg_create_map_points(*common, L.ptr(out["match"]), L.ptr(out["stage"]), L.ptr(out["reduction"]), *tail))
     else:
         L.check(L.lib().sivo_create_map_points(*common, *tail))
     out["n_created"] = nc.value
@@ -104,8 +100,7 @@ def create_map_points_device(left: ORBextractor, kf1: KeyframeKeys, neighbours, 
     """sivo_create_map_points_device: kf1 / neighbours hold device pointers; outputs of left.capacity() keys (0: not wanted).
     Enqueued on `stream` (0 = the left extractor's stream) with no waits and no host synchronisation."""
     L.check(L.lib().sivo_create_map_points_device(left._h, C.byref(kf1), _nb_array(neighbours), len(neighbours), C.byref(params),
-                                                  created_nb_ptr or None, created_idx_ptr or None, world_ptr or None,
-                                                  created_list_ptr or None, n_created_ptr or None, stream or None))
+                                                  created_nb_ptr, created_idx_ptr, world_ptr, created_list_ptr, n_created_ptr, stream))
 
 
 def keyframe_gather_device(left: ORBextractor, kps_ptr, desc_ptr, keep_idx_ptr, n_keep_ptr, u_right_ptr, depth_ptr, class_ptr, conf_ptr,
@@ -114,5 +109,5 @@ def keyframe_gather_device(left: ORBextractor, kps_ptr, desc_ptr, keep_idx_ptr, 
     count] (torch tensors or raw pointers of left.capacity() keys)."""
     ptr = [int(out[k].data_ptr()) if hasattr(out[k], "data_ptr") else int(out[k])
            for k in ("kps", "desc", "u_right", "depth", "kp_class", "kp_conf", "kp_entropy", "count")]
-    L.check(L.lib().sivo_keyframe_gather_device(left._h, kps_ptr, desc_ptr, keep_idx_ptr or None, n_keep_ptr, u_right_ptr, depth_ptr,
-                                                class_ptr, conf_ptr, entropy_ptr, *ptr, stream or None))
+    L.check(L.lib().sivo_keyframe_gather_device(left._h, kps_ptr, desc_ptr, keep_idx_ptr, n_keep_ptr, u_right_ptr, depth_ptr,
+                                                class_ptr, conf_ptr, entropy_ptr, *ptr, stream))

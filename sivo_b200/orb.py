@@ -17,16 +17,14 @@ KP_DTYPE = np.dtype([("x", "<f4"), ("y", "<f4"), ("size", "<f4"), ("angle", "<f4
 class ORBextractor:
     def __init__(self, nfeatures: int, scaleFactor: float, nlevels: int, iniThFAST: int, minThFAST: int, device: int = 0):
         self._h = C.c_void_p()
-        L.check(L.lib().sivo_orb_create(nfeatures, C.c_float(scaleFactor), nlevels, iniThFAST, minThFAST, device,
-                                        C.byref(self._h)))
+        L.check(L.lib().sivo_orb_create(nfeatures, scaleFactor, nlevels, iniThFAST, minThFAST, device, C.byref(self._h)))
         self.nfeatures, self.nlevels = nfeatures, nlevels
         self._scale = np.empty(nlevels, np.float32)
         self._inv = np.empty(nlevels, np.float32)
         self._s2 = np.empty(nlevels, np.float32)
         self._is2 = np.empty(nlevels, np.float32)
         self._per = np.empty(nlevels, np.int32)
-        L.check(L.lib().sivo_orb_tables(self._h, *(a.ctypes.data_as(C.c_void_p) for a in
-                                                   (self._scale, self._inv, self._s2, self._is2, self._per))))
+        L.check(L.lib().sivo_orb_tables(self._h, *(L.ptr(a) for a in (self._scale, self._inv, self._s2, self._is2, self._per))))
         self.mvImagePyramid: List[np.ndarray] = []
         self._scale_factor = scaleFactor
 
@@ -90,8 +88,7 @@ class ORBextractor:
         else:
             self._bordered = []
             self.mvImagePyramid = []
-        L.check(L.lib().sivo_orb_run(self._h, image.ctypes.data_as(C.c_void_p), rows, cols, C.c_size_t(image.strides[0]),
-                                     kps.ctypes.data_as(C.c_void_p), cap, C.byref(n), desc.ctypes.data_as(C.c_void_p),
+        L.check(L.lib().sivo_orb_run(self._h, L.ptr(image), rows, cols, image.strides[0], L.ptr(kps), cap, C.byref(n), L.ptr(desc),
                                      ptrs, strides))
         return kps[:n.value], desc[:n.value]
 
@@ -112,9 +109,7 @@ class ORBextractor:
         kps = np.empty(cap, KP_DTYPE)
         desc = np.empty((cap, 32), np.uint8)
         n = C.c_int(0)
-        L.check(L.lib().sivo_orb_run_device_input(self._h, C.c_void_p(gray_ptr), rows, cols, C.c_size_t(pitch),
-                                                  kps.ctypes.data_as(C.c_void_p), cap, C.byref(n),
-                                                  desc.ctypes.data_as(C.c_void_p)))
+        L.check(L.lib().sivo_orb_run_device_input(self._h, gray_ptr, rows, cols, pitch, L.ptr(kps), cap, C.byref(n), L.ptr(desc)))
         return kps[:n.value], desc[:n.value]
 
     def has_device_tree(self) -> bool:
@@ -131,17 +126,16 @@ class ORBextractor:
     def enqueue_device(self, gray_ptr: int, rows: int, cols: int, pitch: int, kps_ptr: int, desc_ptr: int, count_ptr: int):
         """Asynchronous operator on device-resident buffers (sivo_orb_enqueue_device): returns after the launches are enqueued on
         the handle's stream; kps / desc / count (int64) stay on the device."""
-        L.check(L.lib().sivo_orb_enqueue_device(self._h, C.c_void_p(gray_ptr), rows, cols, C.c_size_t(pitch), C.c_void_p(kps_ptr),
-                                                C.c_void_p(desc_ptr), C.c_void_p(count_ptr)))
+        L.check(L.lib().sivo_orb_enqueue_device(self._h, gray_ptr, rows, cols, pitch, kps_ptr, desc_ptr, count_ptr))
 
     def stream_wait(self, consumer_stream: int):
-        L.check(L.lib().sivo_orb_stream_wait(self._h, C.c_void_p(consumer_stream)))
+        L.check(L.lib().sivo_orb_stream_wait(self._h, consumer_stream))
 
     def wait_for_stream(self, producer_stream: int):
-        L.check(L.lib().sivo_orb_wait_for_stream(self._h, C.c_void_p(producer_stream)))
+        L.check(L.lib().sivo_orb_wait_for_stream(self._h, producer_stream))
 
     def wait_event(self, cuda_event: int):
-        L.check(L.lib().sivo_orb_wait_event(self._h, C.c_void_p(cuda_event)))
+        L.check(L.lib().sivo_orb_wait_event(self._h, cuda_event))
 
     def device_status(self) -> int:
         m = C.c_int()
@@ -152,8 +146,7 @@ class ORBextractor:
         n = C.c_int()
         cap = 1 << 16
         xs, ys, rs = (np.empty(cap, np.int32) for _ in range(3))
-        L.check(L.lib().sivo_orb_candidates(self._h, level, xs.ctypes.data_as(C.c_void_p), ys.ctypes.data_as(C.c_void_p),
-                                            rs.ctypes.data_as(C.c_void_p), cap, C.byref(n)))
+        L.check(L.lib().sivo_orb_candidates(self._h, level, L.ptr(xs), L.ptr(ys), L.ptr(rs), cap, C.byref(n)))
         return xs[:n.value].copy(), ys[:n.value].copy(), rs[:n.value].copy()
 
     def last_timing(self):
@@ -168,9 +161,8 @@ def distribute_octtree(xs, ys, resp, min_x, max_x, min_y, max_y, n_target) -> np
     ys = np.ascontiguousarray(ys, np.float32)
     resp = np.ascontiguousarray(resp, np.float32)
     keep = np.empty(max(len(xs), 1), np.int32)
-    n = L.check(L.lib().sivo_orb_distribute(xs.ctypes.data_as(C.c_void_p), ys.ctypes.data_as(C.c_void_p),
-                                            resp.ctypes.data_as(C.c_void_p), len(xs), min_x, max_x, min_y, max_y, n_target,
-                                            keep.ctypes.data_as(C.c_void_p), len(keep)))
+    n = L.check(L.lib().sivo_orb_distribute(L.ptr(xs), L.ptr(ys), L.ptr(resp), len(xs), min_x, max_x, min_y, max_y, n_target,
+                                            L.ptr(keep), len(keep)))
     return keep[:n].copy()
 
 
@@ -182,10 +174,8 @@ def stereo_hamming(kp_left, desc_left, kp_right, desc_right, scale_factors, rows
     sf = np.ascontiguousarray(scale_factors, np.float32)
     idx = np.empty(len(kl), np.int32)
     dist = np.empty(len(kl), np.int32)
-    L.check(L.lib().sivo_stereo_hamming(device, kl.ctypes.data_as(C.c_void_p), dl.ctypes.data_as(C.c_void_p), len(kl),
-                                        kr.ctypes.data_as(C.c_void_p), dr.ctypes.data_as(C.c_void_p), len(kr),
-                                        sf.ctypes.data_as(C.c_void_p), len(sf), rows, C.c_float(min_d), C.c_float(max_d),
-                                        idx.ctypes.data_as(C.c_void_p), dist.ctypes.data_as(C.c_void_p)))
+    L.check(L.lib().sivo_stereo_hamming(device, L.ptr(kl), L.ptr(dl), len(kl), L.ptr(kr), L.ptr(dr), len(kr), L.ptr(sf), len(sf), rows,
+                                        min_d, max_d, L.ptr(idx), L.ptr(dist)))
     return idx, dist
 
 
@@ -197,9 +187,8 @@ def stereo_match(left: ORBextractor, right: ORBextractor, kp_left, desc_left, kp
     dr = np.ascontiguousarray(desc_right, np.uint8)
     u = np.empty(len(kl), np.float32)
     z = np.empty(len(kl), np.float32)
-    L.check(L.lib().sivo_stereo_match(left._h, right._h, kl.ctypes.data_as(C.c_void_p), dl.ctypes.data_as(C.c_void_p), len(kl),
-                                      kr.ctypes.data_as(C.c_void_p), dr.ctypes.data_as(C.c_void_p), len(kr), C.c_float(mb),
-                                      C.c_float(mbf), u.ctypes.data_as(C.c_void_p), z.ctypes.data_as(C.c_void_p)))
+    L.check(L.lib().sivo_stereo_match(left._h, right._h, L.ptr(kl), L.ptr(dl), len(kl), L.ptr(kr), L.ptr(dr), len(kr), mb, mbf,
+                                      L.ptr(u), L.ptr(z)))
     return u, z
 
 
@@ -210,8 +199,8 @@ def stereo_match_device(left: ORBextractor, right: ORBextractor, kp_left_ptr: in
     keypoint j) for j < the int64 count at n_left_ptr; float32 outputs of left.capacity() entries.  `stream` (0 = the left
     extractor's stream) first waits for both extractors' work; the next enqueue_device on either must be ordered after this call
     (wait_for_stream).  No host synchronisation."""
-    L.check(L.lib().sivo_stereo_match_device(left._h, right._h, kp_left_ptr, desc_left_ptr, keep_idx_ptr or None, n_left_ptr, kp_right_ptr,
-                                             desc_right_ptr, n_right_ptr, mb, mbf, u_right_ptr, depth_ptr, stream or None))
+    L.check(L.lib().sivo_stereo_match_device(left._h, right._h, kp_left_ptr, desc_left_ptr, keep_idx_ptr, n_left_ptr, kp_right_ptr,
+                                             desc_right_ptr, n_right_ptr, mb, mbf, u_right_ptr, depth_ptr, stream))
 
 
 def stereo_median_cut(sad, u, z, device: int = 0):
@@ -220,8 +209,7 @@ def stereo_median_cut(sad, u, z, device: int = 0):
     s = np.ascontiguousarray(sad, np.int32)
     u = np.array(u, np.float32)
     z = np.array(z, np.float32)
-    L.check(L.lib().sivo_dbg_stereo_median_cut(device, s.ctypes.data_as(C.c_void_p), len(s), u.ctypes.data_as(C.c_void_p),
-                                               z.ctypes.data_as(C.c_void_p)))
+    L.check(L.lib().sivo_dbg_stereo_median_cut(device, L.ptr(s), len(s), L.ptr(u), L.ptr(z)))
     return u, z
 
 
@@ -236,7 +224,5 @@ def hamming_best2(query_desc, train_desc, cand_offsets, cand_idx, train_level=No
         raise ValueError("cand_offsets must have n_query + 1 entries")
     lvl = None if train_level is None else np.ascontiguousarray(train_level, np.int32)
     out = np.empty((len(q), 5), np.int32)
-    L.check(L.lib().sivo_hamming_best2(device, q.ctypes.data_as(C.c_void_p), len(q), t.ctypes.data_as(C.c_void_p), len(t),
-                                       off.ctypes.data_as(C.c_void_p), idx.ctypes.data_as(C.c_void_p),
-                                       None if lvl is None else lvl.ctypes.data_as(C.c_void_p), out.ctypes.data_as(C.c_void_p)))
+    L.check(L.lib().sivo_hamming_best2(device, L.ptr(q), len(q), L.ptr(t), len(t), L.ptr(off), L.ptr(idx), L.ptr(lvl), L.ptr(out)))
     return out

@@ -33,9 +33,6 @@ class PoseResult(C.Structure):
         return np.array(self.sigma_cw, np.float64).reshape(6, 6)
 
 
-assert C.sizeof(PoseResult) == 512
-
-
 def frame_from_result(res: PoseResult, fx, fy, cx, cy, mbf, bounds) -> TrackFrame:
     """The sivo_track_frame of the optimised pose (Rcw, tcw and Ow copied from the result)."""
     f = make_frame(fx, fy, cx, cy, mbf, bounds, np.array(res.Rcw, np.float32), np.array(res.tcw, np.float32))
@@ -49,10 +46,6 @@ def camera_from_result(res: PoseResult, fx, fy, cx, cy, mb, prior_sigma) -> Info
     S = res.sigma() if res.sigma_valid else np.asarray(prior_sigma, np.float64)
     cam = make_camera(fx, fy, cx, cy, mb, np.array(res.Rwc, np.float32), np.array(res.Ow, np.float32), S)
     return cam
-
-
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p)
 
 
 def _host_keys(kps, u_right, xw):
@@ -71,7 +64,8 @@ def pose_optimize(left: ORBextractor, kps, u_right, xw, Tcw, fx, fy, cx, cy, mbf
     T = np.ascontiguousarray(np.asarray(Tcw, np.float32).reshape(-1, 4)[:3]).reshape(12)
     res = PoseResult()
     out = np.zeros(max(len(k), 1), np.uint8)
-    L.check(L.lib().sivo_pose_optimize(left._h, _p(k), _p(u), _p(x), len(k), fx, fy, cx, cy, mbf, _p(T), C.byref(res), _p(out)))
+    L.check(L.lib().sivo_pose_optimize(left._h, L.ptr(k), L.ptr(u), L.ptr(x), len(k), fx, fy, cx, cy, mbf, L.ptr(T), C.byref(res),
+                                       L.ptr(out)))
     return res, out[:len(k)].astype(bool)
 
 
@@ -80,13 +74,13 @@ def pose_optimize_device(left: ORBextractor, kps_ptr: int, keep_idx_ptr: int, n_
     """sivo_pose_optimize_device on device pointers (keep_idx_ptr / outlier_ptr may be 0); result_ptr points to a device
     sivo_pose_result (512 bytes).  Runs on `stream` (0 = the left extractor's) without waits of its own and without a host
     synchronisation."""
-    L.check(L.lib().sivo_pose_optimize_device(left._h, kps_ptr, keep_idx_ptr or None, n_keep_ptr, u_right_ptr, xw_ptr, fx, fy, cx, cy,
-                                              mbf, Tcw_in_ptr, result_ptr, outlier_ptr or None, stream or None))
+    L.check(L.lib().sivo_pose_optimize_device(left._h, kps_ptr, keep_idx_ptr, n_keep_ptr, u_right_ptr, xw_ptr, fx, fy, cx, cy, mbf,
+                                              Tcw_in_ptr, result_ptr, outlier_ptr, stream))
 
 
 def pose_gather_device(left: ORBextractor, match_ptr: int, n_keep_ptr: int, points_ptr: int, n_points: int, xw_ptr: int, stream: int = 0):
     """sivo_pose_gather_device: xw[j] = points[match[j]].pos for the keys with a match, other entries untouched."""
-    L.check(L.lib().sivo_pose_gather_device(left._h, match_ptr, n_keep_ptr, points_ptr or None, n_points, xw_ptr, stream or None))
+    L.check(L.lib().sivo_pose_gather_device(left._h, match_ptr, n_keep_ptr, points_ptr, n_points, xw_ptr, stream))
 
 
 def result_from_bytes(b) -> PoseResult:
@@ -104,9 +98,9 @@ def pose_system(left: ORBextractor, kps, u_right, xw, pose7, fx, fy, cx, cy, mbf
     out = {"err": np.empty((n, 3)), "chi2": np.empty(n), "rho": np.empty((n, 2)), "jac": np.empty((n, 3, 6)), "H": np.empty((6, 6)),
            "b": np.empty(6)}
     chi = C.c_double(0)
-    L.check(L.lib().sivo_dbg_pose_system(left._h, _p(k), _p(u), _p(x), n, fx, fy, cx, cy, mbf, _p(p7), int(bool(robust_stereo)),
-                                         None if l1 is None else _p(l1), *(_p(out[key]) for key in ("err", "chi2", "rho", "jac", "H", "b")),
-                                         C.byref(chi)))
+    L.check(L.lib().sivo_dbg_pose_system(left._h, L.ptr(k), L.ptr(u), L.ptr(x), n, fx, fy, cx, cy, mbf, L.ptr(p7),
+                                         int(bool(robust_stereo)), L.ptr(l1),
+                                         *(L.ptr(out[key]) for key in ("err", "chi2", "rho", "jac", "H", "b")), C.byref(chi)))
     out["chi"] = chi.value
     return out
 
@@ -118,7 +112,6 @@ TRACE_DTYPE = np.dtype([(k, "<i4") for k in ("kind", "round", "iteration", "tria
                                              "robust_stereo", "reserved")]
                        + [(k, "<f8") for k in ("current", "temp", "lam_before", "ni_before", "lam_after", "ni_after", "rho")]
                        + [("x", "<f8", 6), ("q", "<f8", 4), ("t", "<f8", 3), ("arg", "<f8"), ("value", "<f8")])
-assert TRACE_DTYPE.itemsize == 216
 
 
 def pose_trace(left: ORBextractor, kps, u_right, xw, Tcw, fx, fy, cx, cy, mbf):
@@ -129,8 +122,8 @@ def pose_trace(left: ORBextractor, kps, u_right, xw, Tcw, fx, fy, cx, cy, mbf):
     res = PoseResult()
     out = np.zeros(max(len(k), 1), np.uint8)
     rec = np.zeros(TRACE_MAX, TRACE_DTYPE)
-    n = L.check(L.lib().sivo_dbg_pose_trace(left._h, _p(k), _p(u), _p(x), len(k), fx, fy, cx, cy, mbf, _p(T), C.byref(res), _p(out),
-                                            _p(rec), TRACE_MAX))
+    n = L.check(L.lib().sivo_dbg_pose_trace(left._h, L.ptr(k), L.ptr(u), L.ptr(x), len(k), fx, fy, cx, cy, mbf, L.ptr(T), C.byref(res),
+                                            L.ptr(out), L.ptr(rec), TRACE_MAX))
     if n > TRACE_MAX:
         raise RuntimeError(f"pose_trace: {n} records, more than the bound {TRACE_MAX}")
     return res, out[:len(k)].astype(bool), rec[:n]
@@ -146,5 +139,5 @@ def pose_se3(T, d, device: int = 0):
         raise ValueError("T and d need one row per entry")
     se3, up, tv = np.empty((n, 7)), np.empty((n, 7)), np.empty((n, 4))
     res = (PoseResult * n)()
-    L.check(L.lib().sivo_dbg_pose_se3(device, n, _p(T), _p(d), _p(se3), _p(up), _p(tv), res))
+    L.check(L.lib().sivo_dbg_pose_se3(device, n, L.ptr(T), L.ptr(d), L.ptr(se3), L.ptr(up), L.ptr(tv), res))
     return se3, up, tv, res

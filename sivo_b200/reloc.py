@@ -25,7 +25,7 @@ class PnpSolver:
     def __init__(self, left: ORBextractor, max_candidates: int, seed: int = 0):
         self._h = C.c_void_p()
         self.left = left
-        L.check(L.lib().sivo_pnp_create(left._h, max_candidates, C.c_uint64(seed), C.byref(self._h)))
+        L.check(L.lib().sivo_pnp_create(left._h, max_candidates, seed, C.byref(self._h)))
         self.n_kf = 0
 
     def setup_device(self, kps_ptr: int, keep_idx_ptr: int, n_keep_ptr: int, match_ptr: int, n_matches_ptr: int, points_ptr: int,
@@ -33,9 +33,8 @@ class PnpSolver:
         """sivo_pnp_setup_device on device pointers (keep_idx 0: identity); kf_ids one id per candidate (host)."""
         ids = np.ascontiguousarray(kf_ids, np.uint32)
         self.n_kf = len(ids)
-        L.check(L.lib().sivo_pnp_setup_device(self._h, kps_ptr, keep_idx_ptr or None, n_keep_ptr, match_ptr or None, n_matches_ptr or None,
-                                              points_ptr or None, n_points, ids.ctypes.data_as(C.c_void_p), len(ids),
-                                              C.c_uint64(frame_id), fx, fy, cx, cy, stream or None))
+        L.check(L.lib().sivo_pnp_setup_device(self._h, kps_ptr, keep_idx_ptr, n_keep_ptr, match_ptr, n_matches_ptr, points_ptr,
+                                              n_points, L.ptr(ids), len(ids), frame_id, fx, fy, cx, cy, stream))
 
     def iterate_device(self, n_iterations: int, active, Tcw_ptr: int, has_pose_ptr: int, no_more_ptr: int, inlier_match_ptr: int,
                        n_inliers_ptr: int, stream: int = 0):
@@ -43,14 +42,14 @@ class PnpSolver:
         act = np.ascontiguousarray(active, np.uint8)
         if len(act) != self.n_kf:
             raise ValueError("active needs one entry per candidate of the last setup")
-        L.check(L.lib().sivo_pnp_iterate_device(self._h, n_iterations, act.ctypes.data_as(C.c_void_p), Tcw_ptr, has_pose_ptr, no_more_ptr,
-                                                inlier_match_ptr, n_inliers_ptr, stream or None))
+        L.check(L.lib().sivo_pnp_iterate_device(self._h, n_iterations, L.ptr(act), Tcw_ptr, has_pose_ptr, no_more_ptr,
+                                                inlier_match_ptr, n_inliers_ptr, stream))
 
     def state(self) -> dict:
         """Test hook: per candidate N, min_inliers, max_its, iterations, best, refine_failed, dead and eps (synchronises the device)."""
         out = np.zeros((max(self.n_kf, 1), 7), np.int32)
         eps = np.zeros(max(self.n_kf, 1), np.float32)
-        L.check(L.lib().sivo_dbg_pnp_state(self._h, out.ctypes.data_as(C.c_void_p), eps.ctypes.data_as(C.c_void_p)))
+        L.check(L.lib().sivo_dbg_pnp_state(self._h, L.ptr(out), L.ptr(eps)))
         names = ("N", "min_inliers", "max_its", "iterations", "best", "refine_failed", "dead")
         d = {k: out[:self.n_kf, i].copy() for i, k in enumerate(names)}
         d["eps"] = eps[:self.n_kf].copy()
@@ -64,8 +63,7 @@ class PnpSolver:
         rt = np.zeros((n_hyp, 12), np.float64)
         cnt = np.zeros(n_hyp, np.int32)
         masks = np.zeros((n_hyp, max(words, 1)), np.uint32)
-        L.check(L.lib().sivo_dbg_pnp_hypotheses(self._h, k, first, n_hyp, dr.ctypes.data_as(C.c_void_p), rt.ctypes.data_as(C.c_void_p),
-                                                cnt.ctypes.data_as(C.c_void_p), masks.ctypes.data_as(C.c_void_p)))
+        L.check(L.lib().sivo_dbg_pnp_hypotheses(self._h, k, first, n_hyp, L.ptr(dr), L.ptr(rt), L.ptr(cnt), L.ptr(masks)))
         bits = np.unpackbits(masks.view(np.uint8), axis=1, bitorder="little").astype(bool)
         return dict(draws=dr, R=rt[:, :9].reshape(-1, 3, 3), t=rt[:, 9:], counts=cnt, masks=bits)
 
@@ -94,9 +92,8 @@ def compute_pose(p3d, p2d, max_err, fx, fy, cx, cy, device: int = 0):
     mask = np.zeros(max((n + 31) // 32, 1), np.uint32)
     cnt = C.c_int(0)
     dbg = PoseDebug()
-    L.check(L.lib().sivo_dbg_pnp_compute_pose(device, p.ctypes.data_as(C.c_void_p), u.ctypes.data_as(C.c_void_p),
-                                              e.ctypes.data_as(C.c_void_p), n, fx, fy, cx, cy, alphas.ctypes.data_as(C.c_void_p),
-                                              mask.ctypes.data_as(C.c_void_p), C.byref(cnt), C.byref(dbg)))
+    L.check(L.lib().sivo_dbg_pnp_compute_pose(device, L.ptr(p), L.ptr(u), L.ptr(e), n, fx, fy, cx, cy, L.ptr(alphas), L.ptr(mask),
+                                              C.byref(cnt), C.byref(dbg)))
     bits = np.unpackbits(mask.view(np.uint8), bitorder="little")[:n].astype(bool)
     return alphas[:n], bits, cnt.value, dbg
 
@@ -104,6 +101,5 @@ def compute_pose(p3d, p2d, max_err, fx, fy, cx, cy, device: int = 0):
 def draws(seed: int, kf_id: int, frame_id: int, first: int, n_hyp: int, N: int, device: int = 0) -> np.ndarray:
     """Test hook: the minimal sets of hypotheses first .. first + n_hyp - 1 -> (n_hyp, 4) int32."""
     out = np.zeros((max(n_hyp, 1), 4), np.int32)
-    L.check(L.lib().sivo_dbg_pnp_draws(device, C.c_uint64(seed), C.c_uint32(kf_id), C.c_uint64(frame_id), first, n_hyp, N,
-                                       out.ctypes.data_as(C.c_void_p)))
+    L.check(L.lib().sivo_dbg_pnp_draws(device, seed, kf_id, frame_id, first, n_hyp, N, L.ptr(out)))
     return out[:n_hyp]

@@ -51,8 +51,8 @@ class BayesianSegNet:
                                                C.byref(self._h))
         else:
             begin, count = samples
-            rc = L.lib().sivo_segnet_create_shard(params.model_file.encode(), params.weights_file.encode(), C.byref(opt),
-                                                  int(begin), int(count), C.byref(self._h))
+            rc = L.lib().sivo_segnet_create_shard(params.model_file.encode(), params.weights_file.encode(), C.byref(opt), begin, count,
+                                                  C.byref(self._h))
         if rc == L.EINVAL:  # the reference throws std::invalid_argument (bayesian_segnet.cpp:66,68,82,86)
             raise ValueError(L.lib().sivo_last_error().decode())
         L.check(rc)
@@ -75,10 +75,10 @@ class BayesianSegNet:
         return (self.width, self.height)  # cv::Size(width, height)
 
     def set_frame(self, frame: int):
-        L.check(L.lib().sivo_segnet_set_frame(self._h, C.c_uint64(frame)))
+        L.check(L.lib().sivo_segnet_set_frame(self._h, frame))
 
     def set_profiling(self, on: bool):
-        L.check(L.lib().sivo_segnet_set_profiling(self._h, int(on)))
+        L.check(L.lib().sivo_segnet_set_profiling(self._h, on))
 
     def segmentImage(self, image: np.ndarray, out=None):
         """image: HxWx3 u8 BGR.  Returns (classes u8 [H,W], confidence f64 [H,W], entropy f64 [H,W]).
@@ -97,9 +97,8 @@ class BayesianSegNet:
             classes = np.empty((self.height, self.width), np.uint8)
             conf = np.empty((self.height, self.width), np.float64)
             ent = np.empty((self.height, self.width), np.float64)
-        L.check(L.lib().sivo_segnet_run(self._h, image.ctypes.data_as(C.c_void_p), image.shape[0], image.shape[1],
-                                        C.c_size_t(image.strides[0]), classes.ctypes.data_as(C.c_void_p),
-                                        conf.ctypes.data_as(C.c_void_p), ent.ctypes.data_as(C.c_void_p)))
+        L.check(L.lib().sivo_segnet_run(self._h, L.ptr(image), image.shape[0], image.shape[1], image.strides[0], L.ptr(classes),
+                                        L.ptr(conf), L.ptr(ent)))
         return classes, conf, ent
 
     def segment_on_device(self, image: np.ndarray):
@@ -108,8 +107,7 @@ class BayesianSegNet:
             raise ValueError("segmentImage expects an HxWx3 uint8 BGR image")
         if image.strides[2] != 1 or image.strides[1] != 3:
             image = np.ascontiguousarray(image)
-        L.check(L.lib().sivo_segnet_run(self._h, image.ctypes.data_as(C.c_void_p), image.shape[0], image.shape[1],
-                                        C.c_size_t(image.strides[0]), None, None, None))
+        L.check(L.lib().sivo_segnet_run(self._h, L.ptr(image), image.shape[0], image.shape[1], image.strides[0], None, None, None))
 
     def semantic_keys(self, kps: np.ndarray, max_static_class: int = 8):
         """Frame::SelectSemanticKeys (Frame.cc:177-203) + per-keypoint map reads on the device-resident result of the last
@@ -124,9 +122,8 @@ class BayesianSegNet:
         ent = np.empty(n, np.float64)
         keep = np.empty(max(n, 1), np.int32)
         m = C.c_int(0)
-        L.check(L.lib().sivo_segnet_semantic_keys(self._h, kps.ctypes.data_as(C.c_void_p), n, int(max_static_class),
-                                                  cls.ctypes.data_as(C.c_void_p), conf.ctypes.data_as(C.c_void_p),
-                                                  ent.ctypes.data_as(C.c_void_p), keep.ctypes.data_as(C.c_void_p), C.byref(m)))
+        L.check(L.lib().sivo_segnet_semantic_keys(self._h, L.ptr(kps), n, max_static_class, L.ptr(cls), L.ptr(conf), L.ptr(ent),
+                                                  L.ptr(keep), C.byref(m)))
         return cls, conf, ent, keep[:m.value].copy()
 
     def semantic_keys_device(self, kps_ptr: int, count_ptr: int, cap: int, max_static_class: int = 8, class_ptr: int = 0,
@@ -135,35 +132,30 @@ class BayesianSegNet:
         their int64 count (e.g. what ORBextractor.enqueue_device wrote), cap the capacity of the output buffers (u8 classes,
         float64 confidence / entropy, int32 keep indices; 0 = not wanted).  *n_keep_ptr (int64) receives the kept count, or -1
         if the count exceeds cap.  Enqueued on `stream` (0 = the stream of the last run) without a host synchronisation."""
-        L.check(L.lib().sivo_segnet_semantic_keys_device(self._h, kps_ptr, count_ptr, int(cap), int(max_static_class), class_ptr or None,
-                                                         conf_ptr or None, ent_ptr or None, keep_ptr or None, n_keep_ptr or None,
-                                                         stream or None))
+        L.check(L.lib().sivo_segnet_semantic_keys_device(self._h, kps_ptr, count_ptr, cap, max_static_class, class_ptr, conf_ptr,
+                                                         ent_ptr, keep_ptr, n_keep_ptr, stream))
 
     def run_device(self, bgr_ptr: int, classes_ptr: int, conf_ptr: int, ent_ptr: int, stream: int = 0):
-        L.check(L.lib().sivo_segnet_run_device(self._h, C.c_void_p(bgr_ptr), C.c_void_p(classes_ptr), C.c_void_p(conf_ptr),
-                                               C.c_void_p(ent_ptr), C.c_void_p(stream)))
+        L.check(L.lib().sivo_segnet_run_device(self._h, bgr_ptr, classes_ptr, conf_ptr, ent_ptr, stream))
 
     def set_record_outputs(self, classes_ptr: int = 0, conf32_ptr: int = 0, ent32_ptr: int = 0):
         """segmentImage additionally leaves classes + f32 maps at these device addresses (a packed multi-GPU record); 0s: off."""
-        L.check(L.lib().sivo_segnet_set_record_outputs(self._h, C.c_void_p(classes_ptr), C.c_void_p(conf32_ptr), C.c_void_p(ent32_ptr)))
+        L.check(L.lib().sivo_segnet_set_record_outputs(self._h, classes_ptr, conf32_ptr, ent32_ptr))
 
     def run_device_maps(self, bgr_ptr: int, classes_ptr: int, conf_ptr: int, ent_ptr: int, conf32_ptr: int, ent32_ptr: int, stream: int = 0):
         """run_device plus single-precision copies of the two maps (the packed multi-GPU record's layout); any pointer may be 0."""
-        L.check(L.lib().sivo_segnet_run_device_maps(self._h, C.c_void_p(bgr_ptr), C.c_void_p(classes_ptr), C.c_void_p(conf_ptr),
-                                                    C.c_void_p(ent_ptr), C.c_void_p(conf32_ptr), C.c_void_p(ent32_ptr), C.c_void_p(stream)))
+        L.check(L.lib().sivo_segnet_run_device_maps(self._h, bgr_ptr, classes_ptr, conf_ptr, ent_ptr, conf32_ptr, ent32_ptr, stream))
 
     def run_partial(self, bgr_ptr: int, sum_ptr: int, stream: int = 0):
         """Latency mode: this handle's samples of the frame at bgr_ptr (device, height x width x 3 u8); sum_ptr (device,
         height*width x 16 float64) receives their sum of per-sample softmax.  Advances the frame counter like run_device."""
-        L.check(L.lib().sivo_segnet_run_partial_device(self._h, C.c_void_p(bgr_ptr), C.c_void_p(sum_ptr), C.c_void_p(stream)))
+        L.check(L.lib().sivo_segnet_run_partial_device(self._h, bgr_ptr, sum_ptr, stream))
 
     def finalize(self, sum_ptr: int, classes_ptr: int, conf_ptr: int, ent_ptr: int, conf32_ptr: int = 0, ent32_ptr: int = 0,
                  stream: int = 0):
         """Latency mode: the maps of run_device_maps from sum_ptr = the sum over ALL T samples (e.g. reduced over the ranks'
         run_partial sums); any output pointer may be 0."""
-        L.check(L.lib().sivo_segnet_finalize_device(self._h, C.c_void_p(sum_ptr), C.c_void_p(classes_ptr), C.c_void_p(conf_ptr),
-                                                    C.c_void_p(ent_ptr), C.c_void_p(conf32_ptr), C.c_void_p(ent32_ptr),
-                                                    C.c_void_p(stream)))
+        L.check(L.lib().sivo_segnet_finalize_device(self._h, sum_ptr, classes_ptr, conf_ptr, ent_ptr, conf32_ptr, ent32_ptr, stream))
 
     def computeVariance(self, classes: np.ndarray) -> np.ndarray:
         """bayesian_segnet.cpp:205-260 after segmentImage / segment_on_device: float64 [H, W], per pixel the sample variance
@@ -172,29 +164,27 @@ class BayesianSegNet:
         if classes.dtype != np.uint8 or classes.shape != (self.height, self.width):
             raise ValueError(f"computeVariance expects a {self.height}x{self.width} uint8 class map")
         var = np.empty((self.height, self.width), np.float64)
-        L.check(L.lib().sivo_segnet_variance(self._h, classes.ctypes.data_as(C.c_void_p), var.ctypes.data_as(C.c_void_p)))
+        L.check(L.lib().sivo_segnet_variance(self._h, L.ptr(classes), L.ptr(var)))
         return var
 
     def variance_device(self, classes_ptr: int, var_ptr: int, stream: int = 0):
         """computeVariance on device buffers (height*width u8 in, float64 out), ordered on `stream` after the run it reads."""
-        L.check(L.lib().sivo_segnet_variance_device(self._h, C.c_void_p(classes_ptr), C.c_void_p(var_ptr), C.c_void_p(stream)))
+        L.check(L.lib().sivo_segnet_variance_device(self._h, classes_ptr, var_ptr, stream))
 
     def variance_partial(self, classes_ptr: int, moments_ptr: int, stream: int = 0):
         """Latency mode: moments_ptr (device, height*width x 2 float64) receives (sum p, sum p^2) of the given class over this
         shard's samples of its last run_partial."""
-        L.check(L.lib().sivo_segnet_variance_partial_device(self._h, C.c_void_p(classes_ptr), C.c_void_p(moments_ptr),
-                                                            C.c_void_p(stream)))
+        L.check(L.lib().sivo_segnet_variance_partial_device(self._h, classes_ptr, moments_ptr, stream))
 
     def variance_finalize(self, moments_ptr: int, var_ptr: int, stream: int = 0):
         """Latency mode: the variance map from the moments summed over ALL T samples of the frame."""
-        L.check(L.lib().sivo_segnet_variance_finalize_device(self._h, C.c_void_p(moments_ptr), C.c_void_p(var_ptr), C.c_void_p(stream)))
+        L.check(L.lib().sivo_segnet_variance_finalize_device(self._h, moments_ptr, var_ptr, stream))
 
     def blob(self, name: str) -> np.ndarray:
         n, c, h, w = C.c_int(), C.c_int(), C.c_int(), C.c_int()
-        L.check(L.lib().sivo_segnet_blob(self._h, name.encode(), None, C.c_size_t(0), C.byref(n), C.byref(c), C.byref(h), C.byref(w)))
+        L.check(L.lib().sivo_segnet_blob(self._h, name.encode(), None, 0, C.byref(n), C.byref(c), C.byref(h), C.byref(w)))
         out = np.empty((n.value, c.value, h.value, w.value), np.float32)
-        L.check(L.lib().sivo_segnet_blob(self._h, name.encode(), out.ctypes.data_as(C.c_void_p), C.c_size_t(out.size),
-                                         None, None, None, None))
+        L.check(L.lib().sivo_segnet_blob(self._h, name.encode(), L.ptr(out), out.size, None, None, None, None))
         return out
 
     def op_flops_executed(self):

@@ -15,7 +15,6 @@ from .orb import KP_DTYPE, ORBextractor
 MAP_POINT_DTYPE = np.dtype([("desc", np.uint8, 32), ("pos", np.float32, 3), ("normal", np.float32, 3), ("min_distance", np.float32),
                             ("max_distance", np.float32), ("observed", np.int32), ("octave", np.int32), ("angle", np.float32),
                             ("reserved", np.int32)])
-assert MAP_POINT_DTYPE.itemsize == 80
 
 
 class TrackFrame(C.Structure):
@@ -56,10 +55,6 @@ def map_points(desc, pos, normal, min_distance, max_distance, observed=1, octave
     return pts
 
 
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p)
-
-
 def _keys(kps, desc, u_right):
     k = np.ascontiguousarray(kps, KP_DTYPE)
     d = np.ascontiguousarray(desc, np.uint8).reshape(-1, 32)
@@ -80,8 +75,8 @@ def search_local_points(left: ORBextractor, kps, desc, u_right, points, frame: T
     view = np.empty(max(len(pts), 1), np.uint8)
     match = np.empty(max(len(k), 1), np.int32)
     nm = C.c_int(0)
-    L.check(L.lib().sivo_search_local_points(left._h, _p(k), _p(d), _p(u), None if b is None else _p(b), len(k), _p(pts), len(pts),
-                                             C.byref(frame), th, nnratio, _p(view), _p(match), C.byref(nm)))
+    L.check(L.lib().sivo_search_local_points(left._h, L.ptr(k), L.ptr(d), L.ptr(u), L.ptr(b), len(k), L.ptr(pts), len(pts),
+                                             C.byref(frame), th, nnratio, L.ptr(view), L.ptr(match), C.byref(nm)))
     return view[:len(pts)].astype(bool), match[:len(k)].copy(), nm.value
 
 
@@ -93,8 +88,8 @@ def search_last_frame(left: ORBextractor, kps, desc, u_right, points, frame: Tra
     t = np.ascontiguousarray(tlw, np.float32).reshape(3)
     match = np.empty(max(len(k), 1), np.int32)
     nm = C.c_int(0)
-    L.check(L.lib().sivo_search_last_frame(left._h, _p(k), _p(d), _p(u), len(k), _p(pts), len(pts), C.byref(frame), _p(R), _p(t), th,
-                                           _p(match), C.byref(nm)))
+    L.check(L.lib().sivo_search_last_frame(left._h, L.ptr(k), L.ptr(d), L.ptr(u), len(k), L.ptr(pts), len(pts), C.byref(frame),
+                                           L.ptr(R), L.ptr(t), th, L.ptr(match), C.byref(nm)))
     return match[:len(k)].copy(), nm.value
 
 
@@ -103,9 +98,9 @@ def search_local_points_device(left: ORBextractor, kps_ptr: int, desc_ptr: int, 
                                in_view_ptr: int, match_ptr: int, n_matches_ptr: int, stream: int = 0):
     """sivo_search_local_points_device on device pointers (0 for an optional one).  Runs on `stream` (0 = the left extractor's)
     without waits of its own and without a host synchronisation."""
-    L.check(L.lib().sivo_search_local_points_device(left._h, kps_ptr, desc_ptr, keep_idx_ptr or None, n_keep_ptr, u_right_ptr,
-                                                    blocked_ptr or None, points_ptr or None, n_points, C.byref(frame), th, nnratio,
-                                                    in_view_ptr or None, match_ptr or None, n_matches_ptr or None, stream or None))
+    L.check(L.lib().sivo_search_local_points_device(left._h, kps_ptr, desc_ptr, keep_idx_ptr, n_keep_ptr, u_right_ptr, blocked_ptr,
+                                                    points_ptr, n_points, C.byref(frame), th, nnratio, in_view_ptr, match_ptr,
+                                                    n_matches_ptr, stream))
 
 
 def search_last_frame_device(left: ORBextractor, kps_ptr: int, desc_ptr: int, keep_idx_ptr: int, n_keep_ptr: int, u_right_ptr: int,
@@ -114,9 +109,8 @@ def search_last_frame_device(left: ORBextractor, kps_ptr: int, desc_ptr: int, ke
     """sivo_search_last_frame_device on device pointers; Rlw / tlw are host arrays."""
     R = np.ascontiguousarray(Rlw, np.float32).reshape(9)
     t = np.ascontiguousarray(tlw, np.float32).reshape(3)
-    L.check(L.lib().sivo_search_last_frame_device(left._h, kps_ptr, desc_ptr, keep_idx_ptr or None, n_keep_ptr, u_right_ptr,
-                                                  points_ptr or None, n_points, C.byref(frame), _p(R), _p(t), th, match_ptr or None,
-                                                  n_matches_ptr or None, stream or None))
+    L.check(L.lib().sivo_search_last_frame_device(left._h, kps_ptr, desc_ptr, keep_idx_ptr, n_keep_ptr, u_right_ptr, points_ptr,
+                                                  n_points, C.byref(frame), L.ptr(R), L.ptr(t), th, match_ptr, n_matches_ptr, stream))
 
 
 def features_in_area(left: ORBextractor, kps, bounds, queries):
@@ -130,8 +124,8 @@ def features_in_area(left: ORBextractor, kps, bounds, queries):
     cap = 1 << 16
     while True:
         idx = np.empty(cap, np.int32)
-        rc = L.lib().sivo_dbg_features_in_area(left._h, _p(k), len(k), *(C.c_float(np.float32(v)) for v in bounds), _p(xyr), _p(lv),
-                                               len(q), _p(off), _p(idx), cap)
+        rc = L.lib().sivo_dbg_features_in_area(left._h, L.ptr(k), len(k), *bounds, L.ptr(xyr), L.ptr(lv), len(q), L.ptr(off),
+                                               L.ptr(idx), cap)
         if rc == L.ERANGE and off[-1] > cap:
             cap = int(off[-1])
             continue

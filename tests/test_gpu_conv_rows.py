@@ -2,8 +2,6 @@
 a single output row, an odd height (the second row of the last row block lies outside the image) with a last 128-pixel
 strip one pixel wide, images narrower than half a strip, and more than one 64-channel cout tile.  Every output is held to
 the per-element float64 interval of oracle/conv_bounds.py."""
-import ctypes as C
-
 import numpy as np
 import pytest
 
@@ -11,10 +9,6 @@ from oracle import conv_bounds as B
 from sivo_b200 import _lib as L
 
 pytestmark = pytest.mark.gpu
-
-
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p)
 
 
 @pytest.mark.parametrize("k,cout,n,h,w", [
@@ -32,8 +26,8 @@ def test_conv_rows_within_float64_bounds(k, cout, n, h, w):
     sc = (1 + rng.normal(0, 0.1, size=cout)).astype(np.float32)
     sh = rng.normal(0, 0.1, size=cout).astype(np.float32)
     out = np.full((n, cout, h, w), np.nan, np.float32)
-    L.check(L.lib().sivo_dbg_conv(0, L.ENGINE_TCGEN05, L.PRECISION_FP16, _p(x), n, cin, h, w, _p(wt), _p(b), _p(sc), _p(sh), cout,
-                                  k, (k - 1) // 2, 1, _p(out)))
+    L.check(L.lib().sivo_dbg_conv(0, L.ENGINE_TCGEN05, L.PRECISION_FP16, L.ptr(x), n, cin, h, w, L.ptr(wt), L.ptr(b), L.ptr(sc),
+                                  L.ptr(sh), cout, k, (k - 1) // 2, 1, L.ptr(out)))
     cb = B.ConvBound(x, wt, k // 2, B.gamma_tc(k, cin), b, sc, sh, relu=True)
     lo, hi = cb.half_interval()
     bad = B.outside(out, lo, hi)

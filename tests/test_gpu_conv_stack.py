@@ -1,7 +1,5 @@
 """-m gpu: the tap-row-stacked float-logits convolution (k_conv_stack: Cin = 64 -> at most 16 float channels, 3x3 / 7x7),
 called through the C-ABI test hook, against torch fp32 on identical half-rounded operands."""
-import ctypes as C
-
 import numpy as np
 import pytest
 import torch
@@ -11,10 +9,6 @@ from sivo_b200 import _lib as L
 from test_gpu_layers import interval_violations
 
 pytestmark = pytest.mark.gpu
-
-
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p)
 
 
 def _layer(k, n, h, w, seed):
@@ -30,8 +24,8 @@ def _layer(k, n, h, w, seed):
 def _run(k, x, wt, b, sc, sh):
     n, _, h, w = x.shape
     out = np.empty((n, 15, h, w), np.float32)
-    L.check(L.lib().sivo_dbg_conv(0, L.ENGINE_TCGEN05, L.PRECISION_FP16, _p(np.ascontiguousarray(x)), n, 64, h, w, _p(wt), _p(b),
-                                  _p(sc), _p(sh), 15, k, (k - 1) // 2, 1, _p(out)))
+    L.check(L.lib().sivo_dbg_conv(0, L.ENGINE_TCGEN05, L.PRECISION_FP16, L.ptr(np.ascontiguousarray(x)), n, 64, h, w, L.ptr(wt),
+                                  L.ptr(b), L.ptr(sc), L.ptr(sh), 15, k, (k - 1) // 2, 1, L.ptr(out)))
     return out
 
 

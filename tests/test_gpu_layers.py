@@ -13,10 +13,6 @@ from sivo_b200 import _lib as L
 pytestmark = pytest.mark.gpu
 
 
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p)
-
-
 def interval_violations(x, wt, b, sc, sh, out, gamma, relu=True, half=True, abs_per_input=0.0):
     """Outputs outside the float64 interval of oracle/conv_bounds.py, over the whole output tensor."""
     k = wt.shape[-1]
@@ -34,7 +30,7 @@ def gpu_pool(x):
     n, c, h, w = x.shape
     out = np.empty((n, c, h // 2, w // 2), np.float32)
     mask = np.empty((n, c, h // 2, w // 2), np.int32)
-    L.check(L.lib().sivo_dbg_pool(0, _p(x), n, c, h, w, _p(out), _p(mask)))
+    L.check(L.lib().sivo_dbg_pool(0, L.ptr(x), n, c, h, w, L.ptr(out), L.ptr(mask)))
     return out, mask
 
 
@@ -54,14 +50,14 @@ def test_upsample_kat_and_round_trip():
     m[0, :] = [[0, 3], [8, 15]]   # one index per 2x2 block (test_upsample_layer.cpp:58-105 uses [2 5 / 12 14])
     m[0, 0] = [[1, 2], [12, 14]]
     out = np.empty((1, 8, 4, 4), np.float32)
-    L.check(L.lib().sivo_dbg_unpool(0, _p(x), _p(m), 1, 8, 2, 2, _p(out)))
+    L.check(L.lib().sivo_dbg_unpool(0, L.ptr(x), L.ptr(m), 1, 8, 2, 2, L.ptr(out)))
     ref = S.unpool(torch.from_numpy(x), torch.from_numpy(m.astype(np.int64))).numpy()
     assert np.array_equal(out, ref)
     rng = np.random.default_rng(1)
     y = rng.normal(size=(2, 8, 8, 12)).astype(np.float32)
     v, mk = gpu_pool(y)
     up = np.empty_like(y)
-    L.check(L.lib().sivo_dbg_unpool(0, _p(v), _p(mk), 2, 8, 4, 6, _p(up)))
+    L.check(L.lib().sivo_dbg_unpool(0, L.ptr(v), L.ptr(mk), 2, 8, 4, 6, L.ptr(up)))
     nz = up != 0
     assert nz.sum() == v.size and np.array_equal(up[nz], y[nz])
 
@@ -70,7 +66,8 @@ def test_lrn_matches_oracle():
     rng = np.random.default_rng(2)
     x = rng.uniform(0, 255, size=(1, 3, 16, 24)).astype(np.float32)
     out = np.empty_like(x)
-    L.check(L.lib().sivo_dbg_lrn(0, _p(x), 1, 3, 16, 24, 5, C.c_float(9.99999974738e-05), C.c_float(0.75), C.c_float(1.0), _p(out)))
+    L.check(L.lib().sivo_dbg_lrn(0, L.ptr(x), 1, 3, 16, 24, 5, C.c_float(9.99999974738e-05), C.c_float(0.75), C.c_float(1.0),
+                                 L.ptr(out)))
     ref = S.lrn_across(torch.from_numpy(x), 5, 9.99999974738e-05, 0.75, 1.0).numpy()
     assert np.allclose(out, ref, rtol=2e-6, atol=1e-5)  # test_lrn_layer.cpp uses 1e-5
 
@@ -78,7 +75,7 @@ def test_lrn_matches_oracle():
 def test_dropout_bits_equal_oracle():
     T, Cc, H, W = 3, 192, 5, 7
     keep = np.empty((T, Cc, H, W), np.uint8)
-    L.check(L.lib().sivo_dbg_dropout_mask(0, C.c_uint64(0xDEADBEEF12345678), C.c_uint64(41), 5, T, Cc, H, W, _p(keep)))
+    L.check(L.lib().sivo_dbg_dropout_mask(0, C.c_uint64(0xDEADBEEF12345678), C.c_uint64(41), 5, T, Cc, H, W, L.ptr(keep)))
     ref = philox.dropout_keep(0xDEADBEEF12345678, 41, 5, T, Cc, H, W)
     assert np.array_equal(keep.astype(bool), ref)
 
@@ -92,7 +89,7 @@ def test_mc_reduce_matches_oracle_and_first_max():
     cls = np.empty((H, W), np.uint8)
     conf = np.empty((H, W), np.float64)
     ent = np.empty((H, W), np.float64)
-    L.check(L.lib().sivo_dbg_mc_reduce(0, _p(logits), T, 15, H, W, _p(cls), _p(conf), _p(ent)))
+    L.check(L.lib().sivo_dbg_mc_reduce(0, L.ptr(logits), T, 15, H, W, L.ptr(cls), L.ptr(conf), L.ptr(ent)))
     rc, rf, re = S.mc_reduce(S.softmax_channels(torch.from_numpy(logits)).numpy())
     assert np.array_equal(cls, rc)
     assert cls[0, 0] == 0 and cls[0, 1] == 3 and ent[0, 1] == 0.0
@@ -118,7 +115,7 @@ def test_mc_reduce_sweep_within_float64_bounds(T, Cn):
     cls = np.empty((H, W), np.uint8)
     conf = np.empty((H, W), np.float64)
     ent = np.empty((H, W), np.float64)
-    L.check(L.lib().sivo_dbg_mc_reduce(0, _p(logits), T, Cn, H, W, _p(cls), _p(conf), _p(ent)))
+    L.check(L.lib().sivo_dbg_mc_reduce(0, L.ptr(logits), T, Cn, H, W, L.ptr(cls), L.ptr(conf), L.ptr(ent)))
     rc, rf, re = S.mc_reduce(S.softmax_channels(torch.from_numpy(logits)).numpy())
     bc, bconf, bent, conf_b, ent_b, margin = B.map_bounds(logits)
     print(f"mc reduce T={T} C={Cn}: |d conf| {np.abs(conf - bconf).max():.2e} (bound {conf_b.max():.2e}), "
@@ -145,8 +142,8 @@ def test_conv_simt_matches_oracle(k, cin, cout, prec):
     sc = (1 + rng.normal(0, 0.1, size=cout)).astype(np.float32)
     sh = rng.normal(0, 0.1, size=cout).astype(np.float32)
     out = np.empty((n, cout, h, w), np.float32)
-    L.check(L.lib().sivo_dbg_conv(0, L.ENGINE_SIMT, L.PRECISION_FP32 if prec == "fp32" else L.PRECISION_FP16, _p(x), n, cin, h, w,
-                                  _p(wt), _p(b), _p(sc), _p(sh), cout, k, (k - 1) // 2, 1, _p(out)))
+    L.check(L.lib().sivo_dbg_conv(0, L.ENGINE_SIMT, L.PRECISION_FP32 if prec == "fp32" else L.PRECISION_FP16, L.ptr(x), n, cin, h, w,
+                                  L.ptr(wt), L.ptr(b), L.ptr(sc), L.ptr(sh), cout, k, (k - 1) // 2, 1, L.ptr(out)))
     xt, wtt = torch.from_numpy(x), torch.from_numpy(wt)
     if prec == "fp16":
         xt, wtt = xt.half().float(), wtt.half().float()
@@ -181,8 +178,8 @@ def test_conv_tcgen05_matches_oracle(k, cin, cout, n, h, w):
     sc = (1 + rng.normal(0, 0.1, size=cout)).astype(np.float32)
     sh = rng.normal(0, 0.1, size=cout).astype(np.float32)
     out = np.empty((n, cout, h, w), np.float32)
-    L.check(L.lib().sivo_dbg_conv(0, L.ENGINE_TCGEN05, L.PRECISION_FP16, _p(x), n, cin, h, w, _p(wt), _p(b), _p(sc), _p(sh), cout,
-                                  k, (k - 1) // 2, 1, _p(out)))
+    L.check(L.lib().sivo_dbg_conv(0, L.ENGINE_TCGEN05, L.PRECISION_FP16, L.ptr(x), n, cin, h, w, L.ptr(wt), L.ptr(b), L.ptr(sc),
+                                  L.ptr(sh), cout, k, (k - 1) // 2, 1, L.ptr(out)))
     xt, wtt = torch.from_numpy(x).half().float(), torch.from_numpy(wt).half().float()
     ref = F.conv2d(xt, wtt, None, padding=(k - 1) // 2) + torch.from_numpy(b).view(1, -1, 1, 1)
     ref = torch.relu(ref * torch.from_numpy(sc).view(1, -1, 1, 1) + torch.from_numpy(sh).view(1, -1, 1, 1))
@@ -207,8 +204,8 @@ def test_conv_tcgen05_split_operand_mode_is_fp32_grade(k, cin, cout, n, h, w):
     sc = (1 + rng.normal(0, 0.1, size=cout)).astype(np.float32)
     sh = rng.normal(0, 0.1, size=cout).astype(np.float32)
     out = np.empty((n, cout, h, w), np.float32)
-    L.check(L.lib().sivo_dbg_conv(0, L.ENGINE_TCGEN05, L.PRECISION_FP32, _p(x), n, cin, h, w, _p(wt), _p(b), _p(sc), _p(sh), cout,
-                                  k, (k - 1) // 2, 1, _p(out)))
+    L.check(L.lib().sivo_dbg_conv(0, L.ENGINE_TCGEN05, L.PRECISION_FP32, L.ptr(x), n, cin, h, w, L.ptr(wt), L.ptr(b), L.ptr(sc),
+                                  L.ptr(sh), cout, k, (k - 1) // 2, 1, L.ptr(out)))
     xd, wd = torch.from_numpy(x).double(), torch.from_numpy(wt).double()
     ref = F.conv2d(xd, wd, None, padding=(k - 1) // 2) + torch.from_numpy(b).double().view(1, -1, 1, 1)
     ref = torch.relu(ref * torch.from_numpy(sc).double().view(1, -1, 1, 1) + torch.from_numpy(sh).double().view(1, -1, 1, 1)).numpy()

@@ -2,8 +2,6 @@
 upsample1 -> conv_decode1 x classifier).  The unpool is an exact select and the accumulation order is that of the plain
 kernel, so it must equal the unpool kernel followed by the convolution bit for bit, and the default network build, which
 runs it, must expose the same conv_decode2 and upsample1 blobs as the unfused keep_blobs build."""
-import ctypes as C
-
 import numpy as np
 import pytest
 
@@ -18,10 +16,6 @@ from sivo_b200 import _lib as L
 from sivo_b200.synth import stereo_frame
 
 pytestmark = pytest.mark.gpu
-
-
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p)
 
 
 def _case(n, mask_n, h, w, seed):
@@ -42,8 +36,8 @@ def _case(n, mask_n, h, w, seed):
 def _fused(x, mask, wt, b, sc, sh):
     n, _, h, w = x.shape
     out = np.empty((n, 15, 2 * h, 2 * w), np.float32)
-    L.check(L.lib().sivo_dbg_conv_unpooled(0, _p(np.ascontiguousarray(x)), _p(np.ascontiguousarray(mask)), n, mask.shape[0], h, w,
-                                           _p(wt), _p(b), _p(sc), _p(sh), 15, 7, _p(out)))
+    L.check(L.lib().sivo_dbg_conv_unpooled(0, L.ptr(np.ascontiguousarray(x)), L.ptr(np.ascontiguousarray(mask)), n, mask.shape[0], h,
+                                           w, L.ptr(wt), L.ptr(b), L.ptr(sc), L.ptr(sh), 15, 7, L.ptr(out)))
     return out
 
 
@@ -51,10 +45,10 @@ def _two_kernels(x, mask, wt, b, sc, sh):
     n, _, h, w = x.shape
     full_mask = np.ascontiguousarray(mask[np.arange(n) % mask.shape[0]])
     up = np.empty((n, 64, 2 * h, 2 * w), np.float32)
-    L.check(L.lib().sivo_dbg_unpool(0, _p(np.ascontiguousarray(x)), _p(full_mask), n, 64, h, w, _p(up)))
+    L.check(L.lib().sivo_dbg_unpool(0, L.ptr(np.ascontiguousarray(x)), L.ptr(full_mask), n, 64, h, w, L.ptr(up)))
     out = np.empty((n, 15, 2 * h, 2 * w), np.float32)
-    L.check(L.lib().sivo_dbg_conv(0, L.ENGINE_TCGEN05, L.PRECISION_FP16, _p(up), n, 64, 2 * h, 2 * w, _p(wt), _p(b), _p(sc), _p(sh),
-                                  15, 7, 3, 0, _p(out)))
+    L.check(L.lib().sivo_dbg_conv(0, L.ENGINE_TCGEN05, L.PRECISION_FP16, L.ptr(up), n, 64, 2 * h, 2 * w, L.ptr(wt), L.ptr(b),
+                                  L.ptr(sc), L.ptr(sh), 15, 7, 3, 0, L.ptr(out)))
     return out
 
 
