@@ -205,8 +205,10 @@ int sivo_orb_run_device_input(sivo_orb_t* h, const uint8_t* gray_device, int row
 /* Fully asynchronous operator for device-resident pipelines (frame sharding across GPUs, CUDA-graph style callers): enqueues
  * pyramid -> FAST -> cells -> device quad tree -> blur -> rBRIEF on the handle's own stream and returns without synchronising.
  * kps_device needs room for sivo_orb_capacity(h) records, desc32_device for 32 bytes each; *count_device (int64) receives the
- * keypoint count.  sivo_orb_stream_wait makes another stream wait for the enqueued work; sivo_orb_device_status (synchronises)
- * returns a non-zero level mask if a level exceeded the device tree's capacity (use sivo_orb_run for such inputs). */
+ * keypoint count, or -1 if a pyramid level exceeded the device tree's capacity (more than 8,192 FAST candidates, more than 16
+ * initial quad-tree nodes, or more nodes than its shared memory holds): the records are then not valid, and the device forms of the
+ * Frame tail that read the count write their own -1 and nothing else.  sivo_orb_stream_wait makes another stream wait for the
+ * enqueued work; sivo_orb_device_status (synchronises) returns the mask of those levels (sivo_orb_run extracts such inputs). */
 int sivo_orb_enqueue_device(sivo_orb_t* h, const uint8_t* gray_device, int rows, int cols, size_t pitch, sivo_keypoint* kps_device,
                             uint8_t* desc32_device, long long* count_device);
 int sivo_orb_stream_wait(sivo_orb_t* h, void* consumer_cuda_stream);

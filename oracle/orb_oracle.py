@@ -406,6 +406,10 @@ def level_cells(lw: int, lh: int):
     height = np.float32(max_by - min_by)
     n_cols = int(width / np.float32(30))
     n_rows = int(height / np.float32(30))
+    if n_cols == 0 or n_rows == 0:
+        # a detection region under 30 px: the reference's cell loops run zero times (its wCell / hCell are ceil(x / 0)), so the
+        # level has no cells and keeps no keypoints
+        return [], (min_bx, min_by, max_bx, max_by)
     w_cell = int(math.ceil(width / np.float32(n_cols)))
     h_cell = int(math.ceil(height / np.float32(n_rows)))
     cells = []

@@ -69,6 +69,7 @@ void orb_launch_blur(const uint8_t* pyr, uint8_t* blur, const OrbLevelTable& t, 
 // Either quad tree's per-level selections (packed candidates sel_packed[l * stride + i], i < level_count[l]; the count lives on
 // the device) -> level-major keypoint records (ComputeKeyPointsOctTree :824-835 + the final scaling of operator() :1071-1078,
 // angle from IC_Angle) and descriptors; *n_out (and *n_out_i64 if given) = the keypoint count, bit 30 of *error if it exceeds cap.
+// *n_out_i64 = -1 instead if a level bit (0-15) of *error is set on entry: the device tree left that level out.
 void orb_launch_describe_dev(const uint8_t* pyr, const uint8_t* blur, const OrbLevelTable& t, const uint32_t* sel_packed,
                              const int* level_count, int stride, const OrbTreeParams& prm, int cap, const int* umax,
                              sivo_keypoint* kps, uint8_t* desc, int* n_out, long long* n_out_i64, int* error, cudaStream_t s);
@@ -115,7 +116,7 @@ class Orb {
   void stream_wait(cudaStream_t consumer);
   void wait_for_stream(cudaStream_t producer);
   void wait_event(cudaEvent_t e);
-  // bit l set: level l of the last enqueue_device() did not fit the device tree (the results are then not valid)
+  // bit l set: level l of the last enqueue_device() did not fit the device tree (the results are then not valid, and its count -1)
   int device_tree_status();
   int capacity() const { return sel_cap_; }
   bool device_tree() const { return device_tree_; }

@@ -360,6 +360,7 @@ void Orb::level_size(int rows, int cols, int level, int* w, int* h) const {
 
 void Orb::ensure(int rows, int cols) {
   if (rows == rows_ && cols == cols_) return;
+  rows_ = cols_ = 0;  // until the tables below are complete: a refused size must not leave them half rebuilt under the old one
   lt_.nlevels = nlevels_;
   cells_.clear();
   size_t img_off = 0, flat_off = 0;
@@ -393,9 +394,11 @@ void Orb::ensure(int rows, int cols) {
     }
     const float width = static_cast<float>(max_bx - min_bx), height = static_cast<float>(max_by - min_by);
     const int n_cols = static_cast<int>(width / 30.f), n_rows = static_cast<int>(height / 30.f);
-    const int w_cell = static_cast<int>(std::ceil(width / n_cols)), h_cell = static_cast<int>(std::ceil(height / n_rows));
     lv.cell_begin = static_cast<int>(cells_.size());
-    for (int i = 0; i < n_rows; ++i) {
+    // a FAST region under 30 px has no cells (the reference's loops run zero times; its wCell / hCell, ceil(x / 0), are never used)
+    const int w_cell = n_cols ? static_cast<int>(std::ceil(width / n_cols)) : 0;
+    const int h_cell = n_rows ? static_cast<int>(std::ceil(height / n_rows)) : 0;
+    for (int i = 0; i < n_rows && n_cols; ++i) {
       const int ini_y = min_by + i * h_cell;
       int max_y = ini_y + h_cell + 6;
       if (ini_y >= max_by - 3) continue;
@@ -428,7 +431,9 @@ void Orb::ensure(int rows, int cols) {
   d_cell_count_.alloc(std::max<size_t>(1, ncells) * sizeof(int));
   d_cell_offset_.alloc((static_cast<size_t>(ncells) + 1) * sizeof(int));
   d_cell_items_.alloc(std::max<size_t>(1, ncells) * kCellCap * sizeof(uint32_t));
-  cand_cap_ = std::max(32768, nfeatures_ * 16);
+  // the compacted candidates are the cell lists back to back, so they never outgrow them; run_host_tree copies only the words a
+  // call produced
+  cand_cap_ = std::max(1, ncells) * kCellCap;
   d_cand_.alloc(static_cast<size_t>(cand_cap_) * sizeof(uint32_t));
   h_cand_.ensure(static_cast<size_t>(cand_cap_) * sizeof(uint32_t));
   rows_ = rows;
@@ -527,8 +532,11 @@ void Orb::run(const uint8_t* gray, int rows, int cols, size_t stride, sivo_keypo
 void Orb::run_host_tree(std::chrono::steady_clock::time_point w0) {
   cudaStream_t s = stream_;
   enqueue_compact(s);
+  // the level offsets first: the candidates' copy then moves the words this call produced, not the whole workspace
   SIVO_CUDA(cudaMemcpyAsync(h_level_off_.p, d_level_off_.p, (nlevels_ + 1) * sizeof(int), cudaMemcpyDeviceToHost, s));
-  SIVO_CUDA(cudaMemcpyAsync(h_cand_.p, d_cand_.p, static_cast<size_t>(cand_cap_) * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+  SIVO_CUDA(cudaStreamSynchronize(s));
+  const int* loff = h_level_off_.as<int>();
+  SIVO_CUDA(cudaMemcpyAsync(h_cand_.p, d_cand_.p, static_cast<size_t>(loff[nlevels_]) * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
   SIVO_CUDA(cudaEventRecord(ev_[1], s));
   // the blur overlaps the host quad tree (the device tree's chain, if it ran, has blurred already)
   if (!device_tree_) orb_launch_blur(d_pyr_.as<uint8_t>(), d_blur_.as<uint8_t>(), lt_, s);
@@ -538,9 +546,7 @@ void Orb::run_host_tree(std::chrono::steady_clock::time_point w0) {
   SIVO_CUDA(cudaEventSynchronize(ev_[1]));
   const auto w2 = std::chrono::steady_clock::now();
 
-  const int* loff = h_level_off_.as<int>();
   const uint32_t* cand = h_cand_.as<uint32_t>();
-  if (loff[nlevels_] > cand_cap_) fail(SIVO_ERANGE, "ORBextractor: %d FAST candidates exceed the workspace (%d)", loff[nlevels_], cand_cap_);
   auto t0 = std::chrono::steady_clock::now();
   last_off_.assign(loff, loff + nlevels_ + 1);
   last_cand_.assign(cand, cand + loff[nlevels_]);

@@ -305,9 +305,12 @@ k_describe(const uint8_t* __restrict__ pyr, const uint8_t* __restrict__ blur, Or
   }
   const bool too_many = off > n;  // n = capacity of the output buffers
   if (blockIdx.x == 0 && threadIdx.x == 0) {
+    // bits 0-15: k_distribute could not hold those levels and left them empty, so the selection is truncated.  The synchronous
+    // form redoes the call on the host tree; a device-resident consumer sees it as the -1 count the Frame-tail kernels skip on
+    const bool truncated = (*out_error & 0xFFFF) != 0;
     if (too_many) atomicOr(out_error, 1 << 30);
     *n_out = too_many ? 0 : off;
-    if (n_out_i64) *n_out_i64 = too_many ? 0 : off;
+    if (n_out_i64) *n_out_i64 = truncated ? -1 : too_many ? 0 : off;
   }
   if (too_many || level < 0) return;
   const uint32_t packed = sel_packed[level * stride + i];

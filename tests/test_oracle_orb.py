@@ -1,12 +1,14 @@
 """Pins the ORB oracle (numpy restatement of OpenCV's algorithms) to the operational oracle cv2, bit for
 bit, and to the committed golden fixtures.  The reference holds no ORB vectors (SURVEY 4); parity with an
 OpenCV-3.x build of it is therefore 'unpinned' and the cv2 version is recorded here."""
+import functools
 import os
 
 import numpy as np
 import pytest
 
 from oracle import orb_oracle as O
+from oracle import orb_scene as S
 
 cv2 = pytest.importorskip("cv2")
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
@@ -62,10 +64,9 @@ def test_fast_cells_bit_exact(kitti_gray_crop):
     assert total > 1000
 
 
-def _cv2_pipeline(gray, nfeatures=2000):
+def _cv2_pipeline(gray, p=O.ExtractorParams()):
     """ORBextractor::operator() composed from cv2 primitives exactly as the reference composes OpenCV
     (ORBextractor.cc:752-847,1019-1122); the quad tree is the oracle's."""
-    p = O.ExtractorParams(nfeatures)
     t = O.Tables(p)
     pattern = O.load_pattern()
     h, w = gray.shape
@@ -87,6 +88,8 @@ def _cv2_pipeline(gray, nfeatures=2000):
                 cx.append(q.pt[0] + x0 - mbx)
                 cy.append(q.pt[1] + y0 - mby)
                 cr.append(q.response)
+        if not cx:
+            continue
         sel = O.distribute_octtree(np.array(cx), np.array(cy), np.array(cr, np.float32), mbx, Mbx, mby, Mby, t.per_level[lvl])
         bordered = cv2.copyMakeBorder(im, 19, 19, 19, 19, cv2.BORDER_REFLECT_101)
         blur = cv2.GaussianBlur(im.copy(), (7, 7), 2, 2, borderType=cv2.BORDER_REFLECT_101)
@@ -97,7 +100,7 @@ def _cv2_pipeline(gray, nfeatures=2000):
             sc = t.scale[lvl]
             fx, fy = (np.float32(x), np.float32(y)) if lvl == 0 else (np.float32(np.float32(x) * sc), np.float32(np.float32(y) * sc))
             kps.append([fx, fy, np.float32(int(np.float32(31) * sc)), ang, cr[s], lvl, -1])
-    return np.array(kps, np.float32), np.array(descs, np.uint8)
+    return np.array(kps, np.float32).reshape(-1, 7), np.array(descs, np.uint8).reshape(-1, 32)
 
 
 def test_pipeline_matches_cv2_composition(kitti_gray_crop):
@@ -106,6 +109,76 @@ def test_pipeline_matches_cv2_composition(kitti_gray_crop):
     assert np.array_equal(r.keypoints.astype(np.float32), kp)
     assert np.array_equal(r.descriptors, desc)
     assert len(kp) >= 2000
+
+
+@pytest.fixture(scope="module")
+def scene(kitti_bgr):
+    """name -> (image, parameters, oracle result, oracle level stats) of oracle/orb_scene.py's cases, each computed once."""
+    from sivo_b200.synth import bgr_to_gray
+    gray = bgr_to_gray(kitti_bgr)
+
+    @functools.lru_cache(maxsize=None)
+    def get(name):
+        build, p = S.CASES[name]
+        img = build(gray)
+        r = O.extract(img, p)
+        return img, p, r, S.level_stats(r, img.shape, p)
+    return get
+
+
+# every image at its own parameters, and the parameter sets that change what cv2 computes (thresholds, pyramid) on both images
+CV2_CASES = [n for n in S.CASES if not n.startswith(("crop_", "dense_"))] + [
+    f"{img}_{k}" for img in ("crop", "dense") for k in ("th12_7", "pyr1.5x5", "pyr1.1x12")]
+
+
+@pytest.mark.parametrize("name", CV2_CASES)
+def test_scene_matches_cv2_composition(scene, name):
+    img, p, r, _ = scene(name)
+    kp, desc = _cv2_pipeline(img, p)
+    assert np.array_equal(r.keypoints.astype(np.float32), kp)
+    assert np.array_equal(r.descriptors, desc)
+    assert len(kp) > 0
+
+
+def test_level_without_cells():
+    """A level whose FAST region is under 30 px in either direction has no cells (the reference's cell loops run zero times)."""
+    assert O.level_cells(61, 200)[0] == [] and O.level_cells(200, 61)[0] == []
+    assert len(O.level_cells(62, 62)[0]) == 1
+
+
+def test_scenes_reach_what_they_were_built_for(scene):
+    st = lambda name: scene(name)[3]
+    # the density ladder: level 0 on either side of the device tree's key cap, then pure noise with levels 0-2 above it
+    over = lambda name: {l for l, s in enumerate(st(name)) if s["candidates"] > S.TREE_KEY_CAP}
+    assert over("ladder_below") == set() and over("ladder_above") == {0} and over("ladder_full") == {0, 1, 2}
+    below, above = st("ladder_below")[0]["candidates"], st("ladder_above")[0]["candidates"]
+    assert S.TREE_KEY_CAP - 200 < below <= S.TREE_KEY_CAP < above < S.TREE_KEY_CAP + 200
+    assert sum(s["candidates"] for s in st("ladder_full")) > 70000
+    # the densest cell holds the whole 27 x 27 lattice, below kCellCap
+    assert st("densest_cell")[0]["cell_max"] == 27 * 27 <= S.CELL_CAP and st("densest_cell")[0]["cells"] == 1
+    assert all(s["cell_max"] <= S.CELL_CAP for n in S.CASES for s in st(n))
+    # binary noise ties: level 0 holds few distinct responses
+    assert len(np.unique(scene("binary")[2].candidates[0][2])) < 20
+    ch = st("checkerboard")
+    assert ch[0]["candidates"] == 0 and ch[1]["candidates"] > 1000 and ch[2]["candidates"] > 1000
+    # the smallest 8-level image: its coarsest level is 45 px high (one row less: 44) and, under 30 px of FAST region, has no cells
+    img, p, _, _ = scene("smallest_8_levels")
+    t = O.Tables(p)
+    assert O.level_sizes(img.shape[1], img.shape[0], t)[-1][1] == 45
+    assert O.level_sizes(img.shape[1], img.shape[0] - 1, t)[-1][1] == 44
+    assert st("smallest_8_levels")[-1]["cells"] == 0
+    img, p, _, _ = scene("narrow_level")
+    assert 45 <= O.level_sizes(img.shape[1], img.shape[0], O.Tables(p))[-1][0] < 62 and st("narrow_level")[-1]["cells"] == 0
+    img = scene("portrait")[0]
+    assert int(np.float32(img.shape[1] - 32) / np.float32(img.shape[0] - 32) + np.float32(0.5)) == 0  # n_ini 0, clamped to 1
+    assert scene("wide_4058")[0].shape[1] == S.MAX_PACKED_WIDTH and min(s["n_ini"] for s in st("wide_4058")) > 16
+    # the min_th fallback: at level 0 some cells keep iniThFAST corners and more retry at minThFAST
+    img, p, _, _ = scene("min_th_fallback")
+    score = O.fast_score_map(img)
+    cells, _ = O.level_cells(img.shape[1], img.shape[0])
+    at_ini = [len(O.cell_keypoints(score, *c, p.ini_th)[0]) > 0 for c in cells]
+    at_min = [not a and len(O.cell_keypoints(score, *c, p.min_th)[0]) > 0 for c, a in zip(cells, at_ini)]
+    assert sum(at_ini) > 100 and sum(at_min) > 100
 
 
 @pytest.mark.parametrize("name,nf", [("orb_kitti_2000", 2000), ("orb_kitti_1000", 1000)])
