@@ -6,12 +6,12 @@ import numpy as np
 import pytest
 import torch
 
+from frame_support import extractors, upload
 from oracle import bow_oracle as B
 from oracle import bow_scene as S
 from sivo_b200 import _lib as L
 from sivo_b200.bow import Vocabulary, compute_bow, compute_bow_device, keyframe_keys, search_by_bow, search_by_bow_device
 from sivo_b200.orb import KP_DTYPE
-from test_gpu_frame_tail import extractors
 
 pytestmark = pytest.mark.gpu
 
@@ -37,21 +37,15 @@ def frames():
     return [("kitti", S.fixture_descriptors())] + [(f"synth{s}", S.synthetic_descriptors(s, 1800)) for s in (1, 2, 3)]
 
 
-def _dev(a):
-    t = torch.from_numpy(np.ascontiguousarray(a)).cuda()
-    torch.cuda.synchronize()
-    return t
-
-
 def device_bow(voc, el, desc, levelsup, keep=None, count=None):
     """Runs the device form on a capacity-sized copy; returns the per-key and BowVector outputs on the host."""
     cap = el.capacity()
     n = len(desc)
     buf = np.zeros((cap, 32), np.uint8)
     buf[:min(n, cap)] = desc[:cap]
-    d = _dev(buf)
-    nk = _dev(np.array([n if count is None else count], np.int64))
-    kp = _dev(np.asarray(keep, np.int32)) if keep is not None else None
+    d = upload(buf)
+    nk = upload(np.array([n if count is None else count], np.int64))
+    kp = upload(np.asarray(keep, np.int32)) if keep is not None else None
     out = dict(node=torch.full((cap,), -7, dtype=torch.int32, device="cuda"), word=torch.full((cap,), -7, dtype=torch.int32, device="cuda"),
                bw=torch.full((cap,), -7, dtype=torch.int32, device="cuda"), bwt=torch.full((cap,), 7.0, dtype=torch.float64, device="cuda"),
                len=torch.full((1,), -7, dtype=torch.int64, device="cuda"))
@@ -168,14 +162,14 @@ def device_search(el, f, kfs, ratio, check, counts=None):
         a = np.ascontiguousarray(a)
         out = np.full((cap,) + a.shape[1:], fill, dt) if a.dtype.names is None else np.zeros(cap, a.dtype)
         out[:len(a)] = a
-        return _dev(out.view(np.uint8).reshape(-1) if a.dtype.names else out)
+        return upload(out)
 
-    hold = [pad(f["kps"], KP_DTYPE), pad(f["desc"], np.uint8), pad(f["node"], np.int32, -1), _dev(np.array([len(f["kps"])], np.int64))]
+    hold = [pad(f["kps"], KP_DTYPE), pad(f["desc"], np.uint8), pad(f["node"], np.int32, -1), upload(np.array([len(f["kps"])], np.int64))]
     keys, pts = [], []
     for i, kf in enumerate(kfs):
         c = len(kf["kps"]) if counts is None else counts[i]
         a = [pad(kf["kps"], KP_DTYPE), pad(kf["desc"], np.uint8), pad(kf["node"], np.int32, -1), pad(kf["point"], np.int32, -1),
-             _dev(np.array([c], np.int64))]
+             upload(np.array([c], np.int64))]
         hold += a
         keys.append(keyframe_keys(a[0].data_ptr(), a[1].data_ptr(), a[2].data_ptr(), a[4].data_ptr()))
         pts.append(a[3].data_ptr())

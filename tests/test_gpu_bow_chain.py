@@ -7,21 +7,20 @@ import numpy as np
 import pytest
 import torch
 
+from frame_support import CX, CY, FX, MB, MBF, check_pose, extractors, frame_inputs, ptr, seg, upload  # noqa: F401
 from oracle import bow_oracle as B
 from oracle import bow_scene as S
 from oracle import pose_oracle as P
 from oracle import track_oracle as T
+from oracle.mapping_scene import rotation
 from sivo_b200 import map_points, pose_gather_device, pose_optimize_device
 from sivo_b200.bow import Vocabulary, compute_bow_device, keyframe_keys, search_by_bow_device
+from sivo_b200.frame import DeviceFrame
 from sivo_b200.mapping import keyframe_gather_device
 from sivo_b200.orb import KP_DTYPE
 from sivo_b200.pose import result_from_bytes
-from test_gpu_frame_tail import BASELINES, DeviceKeys, SemanticOut, StereoOut, extractors, ptr, seg  # noqa: F401
-from test_gpu_info_select import rotation
-from test_gpu_pose_chain import CX, CY, FX, check_pose, dev, frame_inputs
 
 pytestmark = pytest.mark.gpu
-MB, MBF = BASELINES["kitti"]
 LEVELSUP = 4
 
 
@@ -32,7 +31,7 @@ def test_track_reference_keyframe_chain(seg, kitti_bgr):
     el, er = extractors(2000)
     cap = el.capacity()
     inputs = frame_inputs(kitti_bgr)
-    d_in = [[torch.from_numpy(x).cuda() for x in f] for f in inputs]
+    d_in = [[upload(x) for x in f] for f in inputs]
     s_track, s_map = torch.cuda.Stream(), torch.cuda.Stream()
     s = s_track.cuda_stream
     H, W = inputs[0][1].shape
@@ -42,9 +41,7 @@ def test_track_reference_keyframe_chain(seg, kitti_bgr):
 
     bufs = []
     for _ in inputs:
-        b = {"cls": torch.empty(H * W, dtype=torch.uint8, device="cuda"), "conf": torch.empty(H * W, dtype=torch.float64, device="cuda"),
-             "ent": torch.empty(H * W, dtype=torch.float64, device="cuda"), "kl": DeviceKeys(el), "kr": DeviceKeys(er)}
-        b["sem"], b["st"] = SemanticOut(cap), StereoOut(cap)
+        b = {"f": DeviceFrame(el, er, H, W)}
         b["kf"] = dict(kps=torch.zeros(cap * 28, dtype=torch.uint8, device="cuda"), desc=torch.zeros(cap * 32, dtype=torch.uint8, device="cuda"),
                        u_right=torch.zeros(cap, device="cuda"), depth=torch.zeros(cap, device="cuda"),
                        kp_class=torch.zeros(cap, dtype=torch.uint8, device="cuda"), kp_conf=torch.zeros(cap, dtype=torch.float64, device="cuda"),
@@ -63,16 +60,9 @@ def test_track_reference_keyframe_chain(seg, kitti_bgr):
     torch.cuda.synchronize()
 
     def front_end(i, b):
-        bgr, gl, gr = d_in[i]
         seg.set_frame(700 + i)
-        seg.run_device_maps(ptr(bgr), ptr(b["cls"]), ptr(b["conf"]), ptr(b["ent"]), 0, 0, s)
-        el.wait_for_stream(s)
-        er.wait_for_stream(s)
-        b["kl"].enqueue(el, gl)
-        b["kr"].enqueue(er, gr)
-        el.stream_wait(s)
-        b["sem"].run(seg, b["kl"], 8, s)
-        b["st"].run(el, er, b["kl"], b["kr"], MB, MBF, s, keep=b["sem"].keep, n_left=b["sem"].n)
+        b["f"].extract(seg, *d_in[i], s)
+        b["f"].tail(seg, MB, MBF, s)
 
     def kf_bow(b, stream):
         compute_bow_device(voc, el, ptr(b["kf"]["desc"]), 0, ptr(b["kf"]["count"]), LEVELSUP, ptr(b["node_kf"]), 0, ptr(b["bw_kf"]), 0,
@@ -81,9 +71,8 @@ def test_track_reference_keyframe_chain(seg, kitti_bgr):
     # an earlier pass makes each frame's reference keyframe: the gather on Tracking's stream, its BoW on LocalMapping's stream
     for i, b in enumerate(bufs):
         front_end(i, b)
-        sem, st, kl = b["sem"], b["st"], b["kl"]
-        keyframe_gather_device(el, ptr(kl.kps), ptr(kl.desc), ptr(sem.keep), ptr(sem.n), ptr(st.u), ptr(st.z), ptr(sem.cls), ptr(sem.conf),
-                               ptr(sem.ent), b["kf"], s)
+        f = b["f"]
+        keyframe_gather_device(el, f.kps, f.desc, f.keep, f.n_keep, f.u_right, f.depth, f.kp_class, f.kp_conf, f.kp_entropy, b["kf"], s)
         b["ev"].record(s_track)
         s_map.wait_event(b["ev"])
         kf_bow(b, s_map)
@@ -106,23 +95,23 @@ def test_track_reference_keyframe_chain(seg, kitti_bgr):
         _, _, node_kf, _ = B.transform(tree, desc, LEVELSUP)
         assert np.array_equal(b["node_kf"].cpu().numpy()[:n], node_kf) and n > 100
         b["point"] = torch.from_numpy(np.concatenate([point, np.full(cap - n, -1, np.int32)])).cuda()
-        b["pts"] = dev(pts)
+        b["pts"] = upload(pts)
         b["T0"].copy_(torch.from_numpy(Tpred.reshape(-1)))
         cases.append(dict(kps=kps, desc=desc, node=node_kf, point=point, pts=pts, Tpred=Tpred))
     torch.cuda.synchronize()
 
     def track(i, b):
         front_end(i, b)
-        sem, kl = b["sem"], b["kl"]
-        compute_bow_device(voc, el, ptr(kl.desc), ptr(sem.keep), ptr(sem.n), LEVELSUP, ptr(b["node_f"]), ptr(b["word_f"]), ptr(b["bw_f"]),
-                           ptr(b["bwt_f"]), ptr(b["len_f"]), s)
+        f = b["f"]
+        compute_bow_device(voc, el, f.desc, f.keep, f.n_keep, LEVELSUP, ptr(b["node_f"]), ptr(b["word_f"]), ptr(b["bw_f"]), ptr(b["bwt_f"]),
+                           ptr(b["len_f"]), s)
         ref = keyframe_keys(ptr(b["kf"]["kps"]), ptr(b["kf"]["desc"]), ptr(b["node_kf"]), ptr(b["kf"]["count"]))
-        search_by_bow_device(el, ptr(kl.kps), ptr(kl.desc), ptr(sem.keep), ptr(sem.n), ptr(b["node_f"]), [ref], [ptr(b["point"])], 0.7, True,
-                             ptr(b["match"]), ptr(b["nm"]), s)
+        search_by_bow_device(el, f.kps, f.desc, f.keep, f.n_keep, ptr(b["node_f"]), [ref], [ptr(b["point"])], 0.7, True, ptr(b["match"]),
+                             ptr(b["nm"]), s)
         b["xw"].fill_(float("nan"))
-        pose_gather_device(el, ptr(b["match"]), ptr(sem.n), ptr(b["pts"]), len(cases[i]["pts"]), ptr(b["xw"]), s)
-        pose_optimize_device(el, ptr(kl.kps), ptr(sem.keep), ptr(sem.n), ptr(b["st"].u), ptr(b["xw"]), FX, FX, CX, CY, MBF, ptr(b["T0"]),
-                             ptr(b["r"]), ptr(b["o"]), s)
+        pose_gather_device(el, ptr(b["match"]), f.n_keep, ptr(b["pts"]), len(cases[i]["pts"]), ptr(b["xw"]), s)
+        pose_optimize_device(el, f.kps, f.keep, f.n_keep, f.u_right, ptr(b["xw"]), FX, FX, CX, CY, MBF, ptr(b["T0"]), ptr(b["r"]),
+                             ptr(b["o"]), s)
 
     with torch.cuda.stream(s_track):
         for i, b in enumerate(bufs):
@@ -131,10 +120,9 @@ def test_track_reference_keyframe_chain(seg, kitti_bgr):
 
     for i, b in enumerate(bufs):
         c = cases[i]
-        n, keep = b["sem"].host()
-        kps_all, desc_all = b["kl"].host()[:2]
+        n, keep, ur, _ = b["f"].host()
+        kps_all, desc_all = b["f"].left.host()
         kps, desc = kps_all[keep], desc_all[keep]
-        ur = b["st"].host(n)[0]
         bow, _, node, word = B.transform(tree, desc, LEVELSUP)
         words, vals = B.bow_arrays(bow)
         assert np.array_equal(b["node_f"].cpu().numpy()[:n], node) and np.array_equal(b["word_f"].cpu().numpy()[:n], word)

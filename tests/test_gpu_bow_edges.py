@@ -12,6 +12,7 @@ import numpy as np
 import pytest
 import torch
 
+from frame_support import upload
 from oracle import bow_oracle as B
 from oracle import bow_scene as S
 from sivo_b200 import _lib as L
@@ -41,11 +42,6 @@ def vocabulary(tree):
         _VOC[id(tree)] = (tree, Vocabulary.from_arrays(tree["k"], tree["L"], tree["scoring"], tree["weighting"], tree["parent"],
                                                        tree["is_leaf"], tree["desc"], tree["weight"]))
     return _VOC[id(tree)][1]
-
-
-def dev(a):
-    a = np.ascontiguousarray(a)
-    return torch.from_numpy(a.view(np.uint8).reshape(-1).copy() if a.dtype.names else a.copy()).cuda()
 
 
 def case_rng(name):
@@ -112,7 +108,7 @@ def gathered(keep, count, cap):
 def device_bow(voc, el, slot_desc, keep, count, levelsup, want=(True,) * 5):
     """sivo_compute_bow_device with every output at capacity + SLACK (sentinels -7 / 7.0) or NULL where want is False."""
     cap = el.capacity()
-    t = [dev(slot_desc), dev(keep), dev(np.array([count], np.int64))]
+    t = [upload(slot_desc), upload(keep), upload(np.array([count], np.int64))]
     out = dict(node=torch.full((cap + SLACK,), -7, dtype=torch.int32, device="cuda"),
                word=torch.full((cap + SLACK,), -7, dtype=torch.int32, device="cuda"),
                bw=torch.full((cap + SLACK,), -7, dtype=torch.int32, device="cuda"),
@@ -252,11 +248,11 @@ def device_search(el, fr, kfs, counts, ratio, check, frame_count=None):
     """sivo_search_by_bow_device with n_kf rows of cap + SLACK sentinel (-7) entries and n_kf + 1 counts."""
     cap = el.capacity()
     n_kf = len(kfs)
-    hold = [dev(fr.kps), dev(fr.desc), dev(fr.keep), dev(np.array([fr.n_keep if frame_count is None else frame_count], np.int64)),
-            dev(fr.node)]
+    hold = [upload(fr.kps), upload(fr.desc), upload(fr.keep), upload(np.array([fr.n_keep if frame_count is None else frame_count], np.int64)),
+            upload(fr.node)]
     keys, pts = [], []
     for kf, c in zip(kfs, counts):
-        a = [dev(kf["kps"]), dev(kf["desc"]), dev(kf["node"]), dev(kf["point"]), dev(np.array([c], np.int64))]
+        a = [upload(kf["kps"]), upload(kf["desc"]), upload(kf["node"]), upload(kf["point"]), upload(np.array([c], np.int64))]
         hold += a
         keys.append(keyframe_keys(a[0].data_ptr(), a[1].data_ptr(), a[2].data_ptr(), a[4].data_ptr()))
         pts.append(a[3].data_ptr())
@@ -357,7 +353,7 @@ def test_capacity_limits():
     voc = vocabulary(case.tree)
     cap = over.capacity()
     slot_desc, keep, n_keep = transform_setup(case.desc, cap, case_rng("over"), True)
-    t = [dev(slot_desc), dev(keep), dev(np.array([n_keep], np.int64))]
+    t = [upload(slot_desc), upload(keep), upload(np.array([n_keep], np.int64))]
     outs = [torch.full((cap,), -7, dtype=torch.int32, device="cuda") for _ in range(3)] + \
         [torch.full((cap,), 7.0, dtype=torch.float64, device="cuda"), torch.full((1,), -7, dtype=torch.int64, device="cuda")]
     with pytest.raises(L.SivoError) as e:
@@ -367,9 +363,9 @@ def test_capacity_limits():
     assert all((o == (7.0 if o.dtype == torch.float64 else -7)).all() for o in outs)
     sc = SEARCH["decisions_070"]
     fr = DeviceFrame(sc.frame, cap, case_rng("over2"))
-    hold = [dev(fr.kps), dev(fr.desc), dev(fr.keep), dev(np.array([fr.n_keep], np.int64)), dev(fr.node)]
+    hold = [upload(fr.kps), upload(fr.desc), upload(fr.keep), upload(np.array([fr.n_keep], np.int64)), upload(fr.node)]
     pk = pad_keyframe(sc.kfs[0], cap)
-    a = [dev(pk["kps"]), dev(pk["desc"]), dev(pk["node"]), dev(pk["point"]), dev(np.array([len(sc.kfs[0]["kps"])], np.int64))]
+    a = [upload(pk["kps"]), upload(pk["desc"]), upload(pk["node"]), upload(pk["point"]), upload(np.array([len(sc.kfs[0]["kps"])], np.int64))]
     match = torch.full((cap,), -7, dtype=torch.int32, device="cuda")
     nm = torch.full((1,), -7, dtype=torch.int64, device="cuda")
     with pytest.raises(L.SivoError) as e:

@@ -1,110 +1,32 @@
 """-m gpu: the device forms of the Frame tail -- SelectSemanticKeys (sivo_segnet_semantic_keys_device) and ComputeStereoMatches
 (sivo_stereo_match_device) -- on the extractors' device outputs, against the host forms, the oracle, and an asynchronous
 SegNet -> extractors -> semantic keys -> stereo chain with one host synchronisation."""
-import os
-
 import numpy as np
 import pytest
 import torch
 
+from frame_support import BASELINES, H, W, crop, extractors, ptr, seg, seg_paths, synth, upload  # noqa: F401
 from oracle import orb_oracle as O
 from sivo_b200 import KP_DTYPE, BayesianSegNet, BayesianSegNetParams, ORBextractor, stereo_match, stereo_match_device
 from sivo_b200 import _lib as L
-from sivo_b200.synth import bgr_to_gray, stereo_frame
+from sivo_b200.frame import DeviceFrame, FrameKeys
+from sivo_b200.synth import bgr_to_gray
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-H, W, Y0, X0 = 352, 1024, 11, 109  # the network's input: the centre crop (109, 11) of a 1242x375 frame
-KITTI_MBF = 386.1448  # Camera.bf of config/kitti/KITTI00-02.yaml; mb = bf / fx
-BASELINES = {"kitti": (KITTI_MBF / 718.856, KITTI_MBF), "wide": (0.8, 400.0)}
+
+def semantic_keys(seg, f, max_static_class, stream, cap=None):
+    """sivo_segnet_semantic_keys_device from f's left keys into f's five outputs."""
+    seg.semantic_keys_device(f.kps, f.count, f.left.cap if cap is None else cap, max_static_class, f.kp_class, f.kp_conf, f.kp_entropy,
+                             f.keep, f.n_keep, stream)
 
 
-@pytest.fixture(scope="module")
-def seg(model_dir):
-    """The shipped Basic topology at T=2 with the calibrated synthetic weights (the file other GPU tests write)."""
-    from sivo_b200.caffemodel import shipped_scales, write_synth_model
-    from sivo_b200.prototxt import load_net
-    proto = os.path.join(ROOT, "configs", "bayesian_segnet_basic.prototxt")
-    model = os.path.join(str(model_dir), "basic_full.caffemodel")
-    if not os.path.exists(model):
-        write_synth_model(load_net(open(proto).read(), T=2), model, 0, shipped_scales("basic"))
-    return BayesianSegNet(BayesianSegNetParams(proto, model), seed=7, T=2, precision="fp16", engine="auto")
-
-
-def crop(img):
-    return np.ascontiguousarray(img[Y0:Y0 + H, X0:X0 + W])
-
-
-def synth(seed):
-    left, right = stereo_frame(seed)
-    return crop(left), crop(bgr_to_gray(left)), crop(bgr_to_gray(right))
-
-
-def ptr(t):
-    return t.data_ptr()
-
-
-def to_dev(a):
-    """A device copy that is complete before anything else is enqueued (the library's streams do not wait for torch's)."""
-    t = torch.from_numpy(np.ascontiguousarray(a)).cuda()
-    torch.cuda.synchronize()
-    return t
-
-
-class DeviceKeys:
-    """The buffers sivo_orb_enqueue_device fills for one extractor: capacity() records, descriptors and an int64 count."""
-
-    def __init__(self, ext):
-        self.cap = ext.capacity()
-        self.kps = torch.zeros(self.cap * 28, dtype=torch.uint8, device="cuda")
-        self.desc = torch.zeros(self.cap * 32, dtype=torch.uint8, device="cuda")
-        self.cnt = torch.zeros(1, dtype=torch.int64, device="cuda")
-        torch.cuda.synchronize()
-
-    def enqueue(self, ext, gray_dev):
-        ext.enqueue_device(ptr(gray_dev), H, W, W, ptr(self.kps), ptr(self.desc), ptr(self.cnt))
-
-    def host(self):
-        n = int(self.cnt.cpu()[0])
-        return self.kps.cpu().numpy()[:n * 28].view(KP_DTYPE).copy(), self.desc.cpu().numpy()[:n * 32].reshape(n, 32).copy()
-
-
-class SemanticOut:
-    def __init__(self, cap):
-        self.cls = torch.full((cap,), 77, dtype=torch.uint8, device="cuda")
-        self.conf = torch.full((cap,), 7.0, dtype=torch.float64, device="cuda")
-        self.ent = torch.full((cap,), 7.0, dtype=torch.float64, device="cuda")
-        self.keep = torch.full((cap,), -7, dtype=torch.int32, device="cuda")
-        self.n = torch.full((1,), -7, dtype=torch.int64, device="cuda")
-        torch.cuda.synchronize()
-
-    def run(self, seg, dk, max_static_class, stream, cap=None):
-        seg.semantic_keys_device(ptr(dk.kps), ptr(dk.cnt), dk.cap if cap is None else cap, max_static_class, ptr(self.cls),
-                                 ptr(self.conf), ptr(self.ent), ptr(self.keep), ptr(self.n), stream)
-
-    def host(self):
-        n = int(self.n.cpu()[0])
-        return n, self.keep.cpu().numpy()[:max(n, 0)].copy()
-
-
-class StereoOut:
-    def __init__(self, cap):
-        self.u = torch.full((cap,), 7.0, dtype=torch.float32, device="cuda")
-        self.z = torch.full((cap,), 7.0, dtype=torch.float32, device="cuda")
-        torch.cuda.synchronize()
-
-    def run(self, el, er, dl_keys, dr_keys, mb, mbf, stream, keep=None, n_left=None):
-        stereo_match_device(el, er, ptr(dl_keys.kps), ptr(dl_keys.desc), 0 if keep is None else ptr(keep),
-                            ptr(dl_keys.cnt if n_left is None else n_left), ptr(dr_keys.kps), ptr(dr_keys.desc), ptr(dr_keys.cnt), mb, mbf,
-                            ptr(self.u), ptr(self.z), stream)
-
-    def host(self, n):
-        return self.u.cpu().numpy()[:n].copy(), self.z.cpu().numpy()[:n].copy()
-
-
-def extractors(nf, nlevels=8):
-    return ORBextractor(nf, 1.2, nlevels, 20, 7), ORBextractor(nf, 1.2, nlevels, 20, 7)
+def stereo(f, mb, mbf, stream, keep=0, n_left=None, right=None):
+    """sivo_stereo_match_device from f's left keys (keep_idx `keep`, count `n_left`: all of them by default) against the right
+    keys `right` (f's by default) into f's u_right / depth."""
+    r = f.right if right is None else right
+    stereo_match_device(f.el, f.er, f.kps, f.desc, keep, f.count if n_left is None else n_left, ptr(r.kps), ptr(r.desc), ptr(r.count), mb,
+                        mbf, f.u_right, f.depth, stream)
 
 
 # ---------------------------------------------------------------------------------------------------------- semantic keys
@@ -113,25 +35,25 @@ def test_semantic_keys_device_equals_the_host_form(seg, kitti_bgr, frame):
     bgr, gray = (crop(kitti_bgr), crop(bgr_to_gray(kitti_bgr))) if frame == "kitti" else synth(frame)[:2]
     seg.set_frame(5)
     seg.segment_on_device(bgr)
-    ext = ORBextractor(2000, 1.2, 8, 20, 7)
-    dk = DeviceKeys(ext)
+    el, er = extractors(2000)
+    f = DeviceFrame(el, er, H, W)
     stream = torch.cuda.Stream()
-    dk.enqueue(ext, to_dev(gray))
-    ext.stream_wait(stream.cuda_stream)
+    f.left.enqueue(el, upload(gray), H, W, W)
+    el.stream_wait(stream.cuda_stream)
     stream.synchronize()
-    kps, _ = dk.host()
+    kps, _ = f.left.host()
     assert len(kps) > 500
     for msc in (-1, 8, 14):
-        out = SemanticOut(dk.cap)
-        out.run(seg, dk, msc, stream.cuda_stream)
+        f.reset()
+        semantic_keys(seg, f, msc, stream.cuda_stream)
         stream.synchronize()
         cls, conf, ent, keep = seg.semantic_keys(kps, msc)
         n = len(kps)
-        n_keep, got_keep = out.host()
+        n_keep, got_keep = f.host()[:2]
         assert n_keep == len(keep) and np.array_equal(got_keep, keep), msc
-        assert np.array_equal(out.cls.cpu().numpy()[:n], cls)
-        assert out.conf.cpu().numpy()[:n].tobytes() == conf.tobytes() and out.ent.cpu().numpy()[:n].tobytes() == ent.tobytes()
-        assert (out.keep.cpu().numpy()[n_keep:] == -7).all() and (out.cls.cpu().numpy()[n:] == 77).all()
+        assert np.array_equal(f.out["kp_class"].cpu().numpy()[:n], cls)
+        assert f.out["kp_conf"].cpu().numpy()[:n].tobytes() == conf.tobytes() and f.out["kp_entropy"].cpu().numpy()[:n].tobytes() == ent.tobytes()
+        assert (f.out["keep_idx"].cpu().numpy()[n_keep:] == -7).all() and (f.out["kp_class"].cpu().numpy()[n:] == 77).all()
     assert 0 < len(seg.semantic_keys(kps, 8)[3]) < len(kps)
 
 
@@ -145,35 +67,33 @@ def test_semantic_keys_device_out_of_map_keys_count_above_cap_and_null_outputs(s
     kps["y"] = rng.uniform(-20, H + 20, len(kps)).astype(np.float32)
     kps["x"][:3] = (-0.5, 1e9, W - 0.25)  # -0.5 truncates to column 0, as int(pt.x) does
     cap = 1024
-    dk = type("K", (), {})()
-    dk.cap = cap
-    dk.kps = torch.zeros(cap * 28, dtype=torch.uint8, device="cuda")
-    dk.kps[:len(kps) * 28] = torch.from_numpy(kps.view(np.uint8))
-    dk.cnt = torch.tensor([len(kps)], dtype=torch.int64, device="cuda")
+    f = DeviceFrame(*extractors(1000), H, W)  # buffers of at least cap entries
+    assert f.left.cap >= cap
+    f.left.kps[:len(kps) * 28] = torch.from_numpy(kps.view(np.uint8))
+    f.left.count.fill_(len(kps))
     torch.cuda.synchronize()
     stream = torch.cuda.Stream()
-    out = SemanticOut(cap)
-    out.run(seg, dk, 14, stream.cuda_stream)
+    semantic_keys(seg, f, 14, stream.cuda_stream, cap)
     stream.synchronize()
     cls, conf, ent, keep = seg.semantic_keys(kps, 14)
     assert (cls == 255).sum() > 10
-    assert np.array_equal(out.cls.cpu().numpy()[:len(kps)], cls) and np.array_equal(out.host()[1], keep)
-    assert out.conf.cpu().numpy()[:len(kps)].tobytes() == conf.tobytes()
+    assert np.array_equal(f.out["kp_class"].cpu().numpy()[:len(kps)], cls) and np.array_equal(f.host()[1], keep)
+    assert f.out["kp_conf"].cpu().numpy()[:len(kps)].tobytes() == conf.tobytes()
     # only the count and the keep list wanted
-    only = SemanticOut(cap)
-    L.check(L.lib().sivo_segnet_semantic_keys_device(seg._h, ptr(dk.kps), ptr(dk.cnt), cap, 14, None, None, None, ptr(only.keep),
-                                                     ptr(only.n), stream.cuda_stream))
+    f.reset()
+    L.check(L.lib().sivo_segnet_semantic_keys_device(seg._h, f.kps, f.count, cap, 14, None, None, None, f.keep, f.n_keep,
+                                                     stream.cuda_stream))
     stream.synchronize()
-    assert np.array_equal(only.host()[1], keep) and (only.cls.cpu().numpy() == 77).all()
+    assert np.array_equal(f.host()[1], keep) and (f.out["kp_class"].cpu().numpy() == 77).all()
     # zero keys, and a count above the buffers' capacity: n_keep = -1 and nothing else written
     for count, want in ((0, 0), (cap + 1, -1)):
-        dk.cnt.fill_(count)
-        torch.cuda.synchronize()
-        o = SemanticOut(cap)
-        o.run(seg, dk, 14, stream.cuda_stream)
+        f.left.count.fill_(count)
+        f.reset()
+        semantic_keys(seg, f, 14, stream.cuda_stream, cap)
         stream.synchronize()
-        assert int(o.n.cpu()[0]) == want
-        assert (o.cls.cpu().numpy() == 77).all() and (o.keep.cpu().numpy() == -7).all() and (o.conf.cpu().numpy() == 7.0).all()
+        assert int(f.out["n_keep"].cpu()[0]) == want
+        assert ((f.out["kp_class"].cpu().numpy() == 77).all() and (f.out["keep_idx"].cpu().numpy() == -7).all()
+                and (f.out["kp_conf"].cpu().numpy() == 7.0).all())
 
 
 def test_semantic_keys_host_form_reads_maps_still_in_flight(seg):
@@ -181,7 +101,7 @@ def test_semantic_keys_host_form_reads_maps_still_in_flight(seg):
     (bgr_a, _, _), (bgr_b, gray_b, _) = synth(20), synth(21)
     kps, _ = ORBextractor(2000, 1.2, 8, 20, 7)(gray_b, None)
     maps = [torch.empty(H * W, dtype=t, device="cuda") for t in (torch.uint8, torch.float64, torch.float64)]
-    d_a, d_b = to_dev(bgr_a), to_dev(bgr_b)
+    d_a, d_b = upload(bgr_a), upload(bgr_b)
     side = torch.cuda.Stream()
 
     def run(d_bgr, frame):
@@ -217,30 +137,29 @@ def test_stereo_device_equals_the_host_form_and_the_oracle(nf, baseline, with_ke
     el, er = extractors(nf)
     kl, dl = el(gl, None)  # synchronous runs: the host pyramids for the oracle, the keypoints for the host form
     kr, dr = er(gr, None)
-    dkl, dkr = DeviceKeys(el), DeviceKeys(er)
-    dkl.enqueue(el, to_dev(gl))
-    dkr.enqueue(er, to_dev(gr))
+    f = DeviceFrame(el, er, H, W)
+    f.left.enqueue(el, upload(gl), H, W, W)
+    f.right.enqueue(er, upload(gr), H, W, W)
     stream = torch.cuda.Stream()
-    out = StereoOut(dkl.cap)
     if with_keep:
         keep = np.sort(np.random.default_rng(nf).choice(len(kl), len(kl) * 2 // 3, replace=False)).astype(np.int32)
         d_keep = torch.from_numpy(keep).cuda()
         d_n = torch.tensor([len(keep)], dtype=torch.int64, device="cuda")
         torch.cuda.synchronize()
-        out.run(el, er, dkl, dkr, mb, mbf, stream.cuda_stream, keep=d_keep, n_left=d_n)
+        stereo(f, mb, mbf, stream.cuda_stream, keep=ptr(d_keep), n_left=ptr(d_n))
     else:
         keep = np.arange(len(kl), dtype=np.int32)
-        out.run(el, er, dkl, dkr, mb, mbf, stream.cuda_stream)
+        stereo(f, mb, mbf, stream.cuda_stream)
     stream.synchronize()
-    assert np.array_equal(dkl.host()[0].view(np.uint8), kl.view(np.uint8))
-    u, z = out.host(len(keep))
+    assert np.array_equal(f.left.host()[0].view(np.uint8), kl.view(np.uint8))
+    u, z = (f.out[k].cpu().numpy()[:len(keep)] for k in ("u_right", "depth"))
     hu, hz = stereo_match(el, er, kl[keep], dl[keep], kr, dr, mb, mbf)
     assert u.tobytes() == hu.tobytes() and z.tobytes() == hz.tobytes()
     ru, rz = O.compute_stereo_matches(kl[keep], dl[keep], kr, dr, el._bordered, er._bordered, el.GetScaleFactors(),
                                       el.GetInverseScaleFactors(), mb, mbf)
     assert u.tobytes() == ru.tobytes() and z.tobytes() == rz.tobytes()
     assert (u >= 0).sum() > 50
-    assert (out.u.cpu().numpy()[len(keep):] == 7.0).all()
+    assert (f.out["u_right"].cpu().numpy()[len(keep):] == 7.0).all()
 
 
 def test_stereo_device_edge_cases():
@@ -249,54 +168,50 @@ def test_stereo_device_edge_cases():
     el, er = extractors(1000)
     kl, dl = el(gl, None)
     kr, dr = er(gr, None)
-    dkl, dkr = DeviceKeys(el), DeviceKeys(er)
-    dkl.enqueue(el, to_dev(gl))
-    dkr.enqueue(er, to_dev(gr))
+    f = DeviceFrame(el, er, H, W)
+    f.left.enqueue(el, upload(gl), H, W, W)
+    f.right.enqueue(er, upload(gr), H, W, W)
     torch.cuda.synchronize()  # the copies below read the extractors' outputs on torch's stream
     stream = torch.cuda.Stream()
     s = stream.cuda_stream
     zero = torch.zeros(1, dtype=torch.int64, device="cuda")
-    keep = torch.arange(dkl.cap, dtype=torch.int32, device="cuda")
+    keep = torch.arange(f.left.cap, dtype=torch.int32, device="cuda")
+    u_out, z_out = f.out["u_right"], f.out["depth"]
     # zero left keypoints, zero kept keys, a negative count (count above capacity upstream): nothing written
-    for kw in ({"n_left": zero}, {"keep": keep, "n_left": zero}, {"keep": keep, "n_left": torch.full((1,), -1, dtype=torch.int64, device="cuda")}):
-        out = StereoOut(dkl.cap)
-        out.run(el, er, dkl, dkr, mb, mbf, s, **kw)
+    for kw in ({"n_left": ptr(zero)}, {"keep": ptr(keep), "n_left": ptr(zero)},
+               {"keep": ptr(keep), "n_left": ptr(torch.full((1,), -1, dtype=torch.int64, device="cuda"))}):
+        f.reset()
+        stereo(f, mb, mbf, s, **kw)
         stream.synchronize()
-        assert (out.u.cpu().numpy() == 7.0).all() and (out.z.cpu().numpy() == 7.0).all()
+        assert (u_out.cpu().numpy() == 7.0).all() and (z_out.cpu().numpy() == 7.0).all()
     # zero right keypoints: every left keypoint unmatched
     n = len(kl)
-    out = StereoOut(dkl.cap)
-    stereo_match_device(el, er, ptr(dkl.kps), ptr(dkl.desc), 0, ptr(dkl.cnt), ptr(dkr.kps), ptr(dkr.desc), ptr(zero), mb, mbf,
-                        ptr(out.u), ptr(out.z), s)
+    f.reset()
+    stereo_match_device(el, er, f.kps, f.desc, 0, f.count, ptr(f.right.kps), ptr(f.right.desc), ptr(zero), mb, mbf, f.u_right, f.depth, s)
     stream.synchronize()
-    u, z = out.host(n)
-    assert (u == -1).all() and (z == -1).all() and (out.u.cpu().numpy()[n:] == 7.0).all()
+    u, z = u_out.cpu().numpy()[:n], z_out.cpu().numpy()[:n]
+    assert (u == -1).all() and (z == -1).all() and (u_out.cpu().numpy()[n:] == 7.0).all()
     # no match surviving: every right keypoint moved right of every left one, i.e. outside the disparity window [0, mbf / mb)
     moved_kr = kr.copy()
     moved_kr["x"] += np.float32(5000)
-    moved = DeviceKeys(er)
+    moved = FrameKeys(er)
     moved.kps[:len(kr) * 28] = torch.from_numpy(moved_kr.view(np.uint8))
-    moved.desc.copy_(dkr.desc)
-    moved.cnt.copy_(dkr.cnt)
-    torch.cuda.synchronize()
-    out = StereoOut(dkl.cap)
-    out.run(el, er, dkl, moved, mb, mbf, s)
+    moved.desc.copy_(f.right.desc)
+    moved.count.copy_(f.right.count)
+    f.reset()
+    stereo(f, mb, mbf, s, right=moved)
     stream.synchronize()
-    u, z = out.host(n)
+    u, z = u_out.cpu().numpy()[:n], z_out.cpu().numpy()[:n]
     hu, hz = stereo_match(el, er, kl, dl, moved_kr, dr, mb, mbf)
     assert (u == -1).all() and (z == -1).all() and np.array_equal(u, hu) and np.array_equal(z, hz)
     # left keypoints with an octave outside [0, nlevels) stay unmatched; the others keep their results
     bad = kl.copy()
     bad["octave"][::3] = 99
-    bad_dev = DeviceKeys(el)
-    bad_dev.kps[:n * 28] = torch.from_numpy(bad.view(np.uint8))
-    bad_dev.desc.copy_(dkl.desc)
-    bad_dev.cnt.copy_(dkl.cnt)
-    torch.cuda.synchronize()
-    out = StereoOut(dkl.cap)
-    out.run(el, er, bad_dev, dkr, mb, mbf, s)
+    f.left.kps[:n * 28] = torch.from_numpy(bad.view(np.uint8))
+    f.reset()
+    stereo(f, mb, mbf, s)
     stream.synchronize()
-    u, z = out.host(n)
+    u, z = u_out.cpu().numpy()[:n], z_out.cpu().numpy()[:n]
     assert (u[::3] == -1).all() and (z[::3] == -1).all()
     # an unmatched key does not enter the median, so the others get what the host form gives for them alone
     sel = np.setdiff1d(np.arange(n), np.arange(0, n, 3)).astype(np.int32)
@@ -324,16 +239,14 @@ def test_error_codes(seg, model_dir):
     lib = L.lib()
     mb, mbf = BASELINES["kitti"]
     el, er = extractors(500)
-    dkl, dkr = DeviceKeys(el), DeviceKeys(er)
-    out = StereoOut(dkl.cap)
-    sem = SemanticOut(dkl.cap)
-    args = lambda: [ptr(dkl.kps), ptr(dkl.desc), None, ptr(dkl.cnt), ptr(dkr.kps), ptr(dkr.desc), ptr(dkr.cnt), mb, mbf, ptr(out.u), ptr(out.z), None]
+    f = DeviceFrame(el, er, H, W)
+    args = lambda: [f.kps, f.desc, None, f.count, ptr(f.right.kps), ptr(f.right.desc), ptr(f.right.count), mb, mbf, f.u_right, f.depth, None]
     # extractors that have not run
     assert lib.sivo_stereo_match_device(el._h, er._h, *args()) == L.EINVAL
     _, gl, gr = synth(0)
-    dkl.enqueue(el, to_dev(gl))
+    f.left.enqueue(el, upload(gl), H, W, W)
     assert lib.sivo_stereo_match_device(el._h, er._h, *args()) == L.EINVAL
-    dkr.enqueue(er, to_dev(gr))
+    f.right.enqueue(er, upload(gr), H, W, W)
     assert lib.sivo_stereo_match_device(el._h, er._h, *args()) == L.OK
     # NULL handles and buffers (keep_idx may be NULL)
     assert lib.sivo_stereo_match_device(None, er._h, *args()) == L.EINVAL
@@ -353,7 +266,7 @@ def test_error_codes(seg, model_dir):
     assert "differ" in lib.sivo_last_error().decode()
     torch.cuda.synchronize()
     # semantic keys: NULL handle, keypoints or count, negative cap, and a handle that has not run
-    sargs = lambda: [ptr(dkl.kps), ptr(dkl.cnt), dkl.cap, 8, ptr(sem.cls), ptr(sem.conf), ptr(sem.ent), ptr(sem.keep), ptr(sem.n), None]
+    sargs = lambda: [f.kps, f.count, f.left.cap, 8, f.kp_class, f.kp_conf, f.kp_entropy, f.keep, f.n_keep, None]
     seg.segment_on_device(synth(0)[0])
     assert lib.sivo_segnet_semantic_keys_device(seg._h, *sargs()) == L.OK
     assert lib.sivo_segnet_semantic_keys_device(None, *sargs()) == L.EINVAL
@@ -369,10 +282,6 @@ def test_error_codes(seg, model_dir):
     torch.cuda.synchronize()
 
 
-def seg_paths(model_dir):
-    return os.path.join(ROOT, "configs", "bayesian_segnet_basic.prototxt"), os.path.join(str(model_dir), "basic_full.caffemodel")
-
-
 # ---------------------------------------------------------------------------------------------------------- asynchronous chain
 def test_stereo_waits_for_the_extractors_itself():
     """Stereo enqueued straight after enqueue_device on another stream, with no manual wait: the call orders itself."""
@@ -382,19 +291,18 @@ def test_stereo_waits_for_the_extractors_itself():
     kl, dl = el(gl, None)
     kr, dr = er(gr, None)
     hu, hz = stereo_match(el, er, kl, dl, kr, dr, mb, mbf)
-    d_gl, d_gr = to_dev(gl), to_dev(gr)
+    d_gl, d_gr = upload(gl), upload(gr)
     _, gl2, gr2 = synth(5)  # a different frame first, so that stale pyramids / keypoints would show
     el(gl2, None)
     er(gr2, None)
-    dkl, dkr = DeviceKeys(el), DeviceKeys(er)
+    f = DeviceFrame(el, er, H, W)
     stream = torch.cuda.Stream()
-    out = StereoOut(dkl.cap)
-    dkl.enqueue(el, d_gl)
-    dkr.enqueue(er, d_gr)
-    out.run(el, er, dkl, dkr, mb, mbf, stream.cuda_stream)
+    f.left.enqueue(el, d_gl, H, W, W)
+    f.right.enqueue(er, d_gr, H, W, W)
+    stereo(f, mb, mbf, stream.cuda_stream)
     stream.synchronize()
-    u, z = out.host(len(kl))
-    assert int(dkl.cnt.cpu()[0]) == len(kl)
+    u, z = (f.out[k].cpu().numpy()[:len(kl)] for k in ("u_right", "depth"))
+    assert int(f.left.count.cpu()[0]) == len(kl)
     assert u.tobytes() == hu.tobytes() and z.tobytes() == hz.tobytes()
 
 
@@ -408,55 +316,39 @@ def test_three_frames_in_flight_equal_the_host_call_path(seg):
     mb, mbf = BASELINES["kitti"]
     frames = _chain_frames()
     el, er = extractors(2000)
-    hw = H * W
-    d_in = [[torch.from_numpy(x).cuda() for x in f] for f in frames]
-    bufs = []
-    for _ in frames:
-        b = {"cls": torch.empty(hw, dtype=torch.uint8, device="cuda"), "conf": torch.empty(hw, dtype=torch.float64, device="cuda"),
-             "ent": torch.empty(hw, dtype=torch.float64, device="cuda"), "kl": DeviceKeys(el), "kr": DeviceKeys(er)}
-        b["sem"], b["st"] = SemanticOut(b["kl"].cap), StereoOut(b["kl"].cap)
-        bufs.append(b)
+    d_in = [[upload(x) for x in f] for f in frames]
+    bufs = [DeviceFrame(el, er, H, W) for _ in frames]
     stream = torch.cuda.Stream()
     s = stream.cuda_stream
-    torch.cuda.synchronize()
 
     def chain(tail=True):
-        for i, b in enumerate(bufs):
-            bgr, gl, gr = d_in[i]
+        for i, f in enumerate(bufs):
             seg.set_frame(100 + i)
-            seg.run_device_maps(ptr(bgr), ptr(b["cls"]), ptr(b["conf"]), ptr(b["ent"]), 0, 0, s)
-            el.wait_for_stream(s)  # the previous frame's stereo has read the pyramids this enqueue overwrites
-            er.wait_for_stream(s)
-            b["kl"].enqueue(el, gl)
-            b["kr"].enqueue(er, gr)
-            el.stream_wait(s)  # semantic keys read the left keypoints
+            f.extract(seg, *d_in[i], s)
             if tail:
-                b["sem"].run(seg, b["kl"], 8, s)
-                b["st"].run(el, er, b["kl"], b["kr"], mb, mbf, s, keep=b["sem"].keep, n_left=b["sem"].n)
+                f.tail(seg, mb, mbf, s)
             else:
                 er.stream_wait(s)
 
     chain()  # first use of the stream: the network's graph is captured here
     stream.synchronize()
-    for b in bufs:
-        for k in ("cls", "conf", "ent"):
-            b[k].fill_(0)
-        b["sem"].keep.fill_(-7)
-        b["st"].u.fill_(7.0)
-    torch.cuda.synchronize()
+    for f in bufs:
+        for m in f.maps:
+            m.fill_(0)
+        f.reset()
     chain()
     stream.synchronize()  # the one host synchronisation of the chain
-    got = [{"maps": [b[k].cpu().numpy() for k in ("cls", "conf", "ent")], "kl": b["kl"].host(), "kr": b["kr"].host(),
-            "sem": b["sem"].host(), "sem_vals": (b["sem"].cls.cpu().numpy(), b["sem"].conf.cpu().numpy()),
-            "st": (b["st"].u.cpu().numpy(), b["st"].z.cpu().numpy())} for b in bufs]
+    got = [{"maps": [m.cpu().numpy() for m in f.maps], "kl": f.left.host(), "kr": f.right.host(), "sem": f.host()[:2],
+            "sem_vals": (f.out["kp_class"].cpu().numpy(), f.out["kp_conf"].cpu().numpy()),
+            "st": (f.out["u_right"].cpu().numpy(), f.out["depth"].cpu().numpy())} for f in bufs]
     # without the tail the network and extractor outputs are the same bits
     chain(tail=False)
     stream.synchronize()
-    for b, g in zip(bufs, got):
-        for k, m in zip(("cls", "conf", "ent"), g["maps"]):
-            assert b[k].cpu().numpy().tobytes() == m.tobytes()
-        for side in ("kl", "kr"):
-            kp, de = b[side].host()
+    for f, g in zip(bufs, got):
+        for m, want in zip(f.maps, g["maps"]):
+            assert m.cpu().numpy().tobytes() == want.tobytes()
+        for side, keys in (("kl", f.left), ("kr", f.right)):
+            kp, de = keys.host()
             assert kp.tobytes() == g[side][0].tobytes() and np.array_equal(de, g[side][1])
     # the host-call path, frame by frame
     for i, (bgr, gl, gr) in enumerate(frames):

@@ -4,110 +4,14 @@ import numpy as np
 import pytest
 import torch
 
+from frame_support import H, MB, MBF, POSES, SIGMAS, W, InfoOut, cameras, ext, ptr, seg, synth, tails, upload  # noqa: F401
 from oracle import info_oracle as I
 from sivo_b200 import _lib as L
-from sivo_b200 import info_select, info_select_device, make_camera, stereo_match
+from sivo_b200 import info_select, stereo_match
+from sivo_b200.frame import DeviceFrame
 from sivo_b200.info import info_terms
-from sivo_b200.synth import bgr_to_gray
-from test_gpu_frame_tail import (BASELINES, H, W, DeviceKeys, SemanticOut, StereoOut, crop, extractors, ptr, seg,  # noqa: F401
-                                 synth, to_dev)
 
 pytestmark = pytest.mark.gpu
-
-MB, MBF = BASELINES["kitti"]
-FX, CX, CY = 718.856, 607.1928 - 109, 185.2157 - 11  # KITTI00-02.yaml, principal point moved to the network's crop
-FRAMES = ["kitti", 0, 1, 2]
-
-
-def rotation(ax, ay, az):
-    cx, sx, cy, sy, cz, sz = np.cos(ax), np.sin(ax), np.cos(ay), np.sin(ay), np.cos(az), np.sin(az)
-    return (np.array([[cz, -sz, 0], [sz, cz, 0], [0, 0, 1]]) @ np.array([[cy, 0, sy], [0, 1, 0], [-sy, 0, cy]])
-            @ np.array([[1, 0, 0], [0, cx, -sx], [0, sx, cx]]))
-
-
-def sigmas():
-    motion = 1e-6 * np.eye(6)
-    for i in range(3):
-        motion = I.update_state_covariance_motion(motion, rotation(0.002 * i, 0.01, -0.003), (0.02, -0.01, 0.8 + 0.1 * i))
-    a = np.random.default_rng(11).standard_normal((6, 6))
-    spd = 1e-3 * (a @ a.T + 0.5 * np.eye(6))
-    return {"tiny": 1e-6 * np.eye(6), "motion": motion, "spd": spd}
-
-
-SIGMAS = sigmas()
-POSES = {"identity": (np.eye(3), (0.0, 0.0, 0.0)), "moved": (rotation(0.03, -0.25, 0.08), (3.5, -0.7, 41.0))}
-
-
-def cameras(sigma, pose):
-    R, Ow = POSES[pose]
-    S = SIGMAS[sigma] if isinstance(sigma, str) else sigma
-    return make_camera(FX, FX, CX, CY, MB, R, Ow, S), I.Camera(FX, FX, CX, CY, MB, R, Ow, S)
-
-
-class Tail:
-    """One frame through SegNet -> two enqueue_device -> semantic keys -> stereo on the device, plus host copies of the semantic
-    keys' inputs of the selection (mvKeysSemantic, mvDepth, the entropy at each key)."""
-
-    def __init__(self, seg, el, er, bgr, gl, gr):
-        seg.set_frame(3)
-        seg.segment_on_device(bgr)
-        stream = torch.cuda.Stream()
-        s = stream.cuda_stream
-        self.dkl, self.dkr = DeviceKeys(el), DeviceKeys(er)
-        self.dkl.enqueue(el, to_dev(gl))
-        self.dkr.enqueue(er, to_dev(gr))
-        el.stream_wait(s)
-        self.sem = SemanticOut(self.dkl.cap)
-        self.sem.run(seg, self.dkl, 8, s)
-        self.st = StereoOut(self.dkl.cap)
-        self.st.run(el, er, self.dkl, self.dkr, MB, MBF, s, keep=self.sem.keep, n_left=self.sem.n)
-        self.st_all = StereoOut(self.dkl.cap)  # every extractor key, for keep_idx = NULL
-        self.st_all.run(el, er, self.dkl, self.dkr, MB, MBF, s)
-        stream.synchronize()
-        self.kps_all = self.dkl.host()[0]
-        self.n_keep, self.keep = self.sem.host()
-        self.ent_all = self.sem.ent.cpu().numpy()[:len(self.kps_all)].copy()
-        self.kps = self.kps_all[self.keep]
-        self.ent = self.ent_all[self.keep]
-        self.depth = self.st.host(self.n_keep)[1]
-        self.depth_all = self.st_all.host(len(self.kps_all))[1]
-
-
-@pytest.fixture(scope="module")
-def ext():
-    return extractors(2000)
-
-
-@pytest.fixture(scope="module")
-def tails(seg, ext, kitti_bgr):
-    out = {}
-    for f in FRAMES:
-        if f == "kitti":  # the fixture frame has no right image: the left one shifted by 12 px stands in for it
-            gl = crop(bgr_to_gray(kitti_bgr))
-            bgr, gr = crop(kitti_bgr), np.ascontiguousarray(np.roll(gl, -12, axis=1))
-        else:
-            bgr, gl, gr = synth(f)
-        out[f] = Tail(seg, ext[0], ext[1], bgr, gl, gr)
-        assert out[f].n_keep > 100 and (out[f].depth > 0).sum() > 30, (f, out[f].n_keep)
-    return out
-
-
-class InfoOut:
-    def __init__(self, cap):
-        self.world = torch.full((cap * 3,), 7.0, dtype=torch.float32, device="cuda")
-        self.red = torch.full((cap,), 7.0, dtype=torch.float64, device="cuda")
-        self.sel = torch.full((cap,), -7, dtype=torch.int32, device="cuda")
-        self.n = torch.full((1,), -7, dtype=torch.int64, device="cuda")
-        torch.cuda.synchronize()
-
-    def run(self, el, kps, ent, keep, n_keep, depth, cam, threshold, stream, null=()):
-        p = {k: (0 if k in null else ptr(getattr(self, k))) for k in ("world", "red", "sel", "n")}
-        info_select_device(el, kps, ent, keep, n_keep, depth, cam, threshold, p["world"], p["red"], p["sel"], p["n"], stream)
-
-    def host(self, n):
-        m = int(self.n.cpu()[0])
-        return (self.world.cpu().numpy()[:3 * n].reshape(n, 3).copy(), self.red.cpu().numpy()[:n].copy(),
-                self.sel.cpu().numpy()[:max(m, 0)].copy(), m)
 
 
 def same_bits(a, b):
@@ -171,8 +75,8 @@ def test_device_form_equals_the_host_form(tails, ext, sigma, pose):
     for f, t in tails.items():
         th = thresholds(info_select(el, t.kps, t.depth, t.ent, cam, 0.0)[1])[3]  # the median: some keys on either side
         hw, hr, hs = info_select(el, t.kps, t.depth, t.ent, cam, th)
-        out = InfoOut(t.dkl.cap)
-        out.run(el, ptr(t.dkl.kps), ptr(t.sem.ent), ptr(t.sem.keep), ptr(t.sem.n), ptr(t.st.z), cam, th, stream.cuda_stream)
+        out = InfoOut(t.f.left.cap)
+        out.run(el, t.f.kps, t.f.kp_entropy, t.f.keep, t.f.n_keep, t.f.depth, cam, th, stream.cuda_stream)
         stream.synchronize()
         w, r, s, m = out.host(t.n_keep)
         assert same_bits(w, hw) and same_bits(r, hr) and same_bits(s, hs) and m == len(hs), f
@@ -180,8 +84,8 @@ def test_device_form_equals_the_host_form(tails, ext, sigma, pose):
         # keep_idx NULL: semantic key j is extractor key j (depth from the stereo call without keep_idx)
         n = len(t.kps_all)
         hw, hr, hs = info_select(el, t.kps_all, t.depth_all, t.ent_all, cam, th)
-        out = InfoOut(t.dkl.cap)
-        out.run(el, ptr(t.dkl.kps), ptr(t.sem.ent), 0, ptr(t.dkl.cnt), ptr(t.st_all.z), cam, th, stream.cuda_stream)
+        out = InfoOut(t.f.left.cap)
+        out.run(el, t.f.kps, t.f.kp_entropy, 0, t.f.count, ptr(t.z_all), cam, th, stream.cuda_stream)
         stream.synchronize()
         w, r, s, m = out.host(n)
         assert same_bits(w, hw) and same_bits(r, hr) and same_bits(s, hs) and m == len(hs), f
@@ -194,13 +98,13 @@ def test_device_form_edge_cases(tails, ext):
     cam, ocam = cameras("motion", "moved")
     stream = torch.cuda.Stream()
     s = stream.cuda_stream
-    cap = t.dkl.cap
+    cap = t.f.left.cap
 
     def dev(kw=None, cam_=cam, th=0.0, null=()):
         kw = kw or {}
         out = InfoOut(cap)
-        out.run(el, ptr(kw.get("kps", t.dkl.kps)), ptr(kw.get("ent", t.sem.ent)), kw.get("keep", ptr(t.sem.keep)),
-                ptr(kw.get("n", t.sem.n)), ptr(kw.get("depth", t.st.z)), cam_, th, s, null)
+        out.run(el, t.f.kps, t.f.kp_entropy, kw.get("keep", t.f.keep), ptr(kw["n"]) if "n" in kw else t.f.n_keep,
+                ptr(kw["depth"]) if "depth" in kw else t.f.depth, cam_, th, s, null)
         stream.synchronize()
         return out
 
@@ -220,8 +124,8 @@ def test_device_form_edge_cases(tails, ext):
     torch.cuda.synchronize()
     out = dev({"keep": 0, "n": i64(cap + 1000), "depth": depth})
     w, r, sl, m = out.host(cap)
-    hw, hr, hs = info_select(el, t.dkl.kps.cpu().numpy().view(t.kps_all.dtype)[:cap], depth.cpu().numpy(),
-                             t.sem.ent.cpu().numpy()[:cap], cam, 0.0)
+    hw, hr, hs = info_select(el, t.f.left.kps.cpu().numpy().view(t.kps_all.dtype)[:cap], depth.cpu().numpy(),
+                             t.f.out["kp_entropy"].cpu().numpy()[:cap], cam, 0.0)
     assert same_bits(r, hr) and same_bits(sl, hs) and m == len(hs) and np.isnan(r[len(t.kps_all):]).all()
     # all depths -1: every key invalid, nothing selected
     out = dev({"depth": torch.full((cap,), -1.0, dtype=torch.float32, device="cuda")})
@@ -291,9 +195,9 @@ def test_error_codes(tails, ext):
     a = hargs()
     a[7:] = [None] * 4
     assert lib.sivo_info_select(*a) == L.OK
-    out = InfoOut(t.dkl.cap)
-    dargs = lambda: [el._h, ptr(t.dkl.kps), ptr(t.sem.ent), ptr(t.sem.keep), ptr(t.sem.n), ptr(t.st.z), C.byref(cam), 0.0, ptr(out.world),
-                     ptr(out.red), ptr(out.sel), ptr(out.n), None]
+    out = InfoOut(t.f.left.cap)
+    dargs = lambda: [el._h, t.f.kps, t.f.kp_entropy, t.f.keep, t.f.n_keep, t.f.depth, C.byref(cam), 0.0, ptr(out.world), ptr(out.red),
+                     ptr(out.sel), ptr(out.n), None]
     assert lib.sivo_info_select_device(*dargs()) == L.OK
     for i in (0, 1, 2, 4, 5, 6):
         a = dargs()
@@ -311,42 +215,28 @@ def test_three_frames_in_flight_with_the_selection_equal_the_host_call_path(seg,
     el, er = ext
     frames = [synth(20 + i) for i in range(3)]
     cam, _ = cameras("motion", "moved")
-    hw = H * W
-    d_in = [[torch.from_numpy(x).cuda() for x in f] for f in frames]
-    bufs = []
-    for _ in frames:
-        b = {"cls": torch.empty(hw, dtype=torch.uint8, device="cuda"), "conf": torch.empty(hw, dtype=torch.float64, device="cuda"),
-             "ent": torch.empty(hw, dtype=torch.float64, device="cuda"), "kl": DeviceKeys(el), "kr": DeviceKeys(er)}
-        b["sem"], b["st"], b["info"] = SemanticOut(b["kl"].cap), StereoOut(b["kl"].cap), InfoOut(b["kl"].cap)
-        bufs.append(b)
+    d_in = [[upload(x) for x in f] for f in frames]
+    bufs = [(DeviceFrame(el, er, H, W), InfoOut(el.capacity())) for _ in frames]
     stream = torch.cuda.Stream()
     s = stream.cuda_stream
-    torch.cuda.synchronize()
 
     def chain():
-        for i, b in enumerate(bufs):
-            bgr, gl, gr = d_in[i]
+        for i, (f, info) in enumerate(bufs):
             seg.set_frame(200 + i)
-            seg.run_device_maps(ptr(bgr), ptr(b["cls"]), ptr(b["conf"]), ptr(b["ent"]), 0, 0, s)
-            el.wait_for_stream(s)  # the previous frame's stereo and selection are done with the left extractor
-            er.wait_for_stream(s)
-            b["kl"].enqueue(el, gl)
-            b["kr"].enqueue(er, gr)
-            el.stream_wait(s)
-            b["sem"].run(seg, b["kl"], 8, s)
-            b["st"].run(el, er, b["kl"], b["kr"], MB, MBF, s, keep=b["sem"].keep, n_left=b["sem"].n)
-            b["info"].run(el, ptr(b["kl"].kps), ptr(b["sem"].ent), ptr(b["sem"].keep), ptr(b["sem"].n), ptr(b["st"].z), cam, 4.0, s)
+            f.extract(seg, *d_in[i], s)
+            f.tail(seg, MB, MBF, s)
+            info.run(el, f.kps, f.kp_entropy, f.keep, f.n_keep, f.depth, cam, 4.0, s)
 
     chain()  # first use of the stream: the network's graph is captured here
     stream.synchronize()
-    for b in bufs:
-        b["info"].sel.fill_(-7)
-        b["info"].red.fill_(7.0)
-        b["info"].n.fill_(-7)
+    for _, info in bufs:
+        info.sel.fill_(-7)
+        info.red.fill_(7.0)
+        info.n.fill_(-7)
     torch.cuda.synchronize()
     chain()
     stream.synchronize()  # the one host synchronisation of the chain
-    got = [(b["sem"].host()[0], b["info"]) for b in bufs]
+    got = [(f.host()[0], info) for f, info in bufs]
     for i, (bgr, gl, gr) in enumerate(frames):
         seg.set_frame(200 + i)
         seg.segmentImage(bgr)

@@ -6,16 +6,15 @@ import numpy as np
 import pytest
 import torch
 
+from frame_support import CX, CY, FX, MB, MBF, extractors, frame_inputs, seg, upload  # noqa: F401
 from oracle import mapping_oracle as MO
 from oracle import mapping_scene as S
+from oracle.mapping_scene import rotation
+from sivo_b200.frame import DeviceFrame
 from sivo_b200.mapping import KeyframeKeys, create_map_points_device, keyframe_gather_device, make_params, set_pose
 from sivo_b200.orb import KP_DTYPE
-from test_gpu_frame_tail import BASELINES, DeviceKeys, SemanticOut, StereoOut, extractors, ptr, seg  # noqa: F401
-from test_gpu_info_select import rotation
-from test_gpu_pose_chain import CX, CY, FX, frame_inputs
 
 pytestmark = pytest.mark.gpu
-MB, MBF = BASELINES["kitti"]
 TH_CONF, TH_RED, MAX_CLASS = 0.3, -1e9, 8
 
 
@@ -23,15 +22,13 @@ def test_chain_and_creation_beside_tracking(seg, kitti_bgr):
     el, er = extractors(2000)
     cap = el.capacity()
     inputs = frame_inputs(kitti_bgr)
-    d_in = [[torch.from_numpy(x).cuda() for x in f] for f in inputs]
+    d_in = [[upload(x) for x in f] for f in inputs]
     s_track = torch.cuda.Stream()
     s = s_track.cuda_stream
     H, W = inputs[0][1].shape
     bufs = []
     for _ in inputs:
-        b = {"cls": torch.empty(H * W, dtype=torch.uint8, device="cuda"), "conf": torch.empty(H * W, dtype=torch.float64, device="cuda"),
-             "ent": torch.empty(H * W, dtype=torch.float64, device="cuda"), "kl": DeviceKeys(el), "kr": DeviceKeys(er)}
-        b["sem"], b["st"] = SemanticOut(cap), StereoOut(cap)
+        b = {"f": DeviceFrame(el, er, H, W)}
         b["kf"] = dict(kps=torch.zeros(cap * 28, dtype=torch.uint8, device="cuda"), desc=torch.zeros(cap * 32, dtype=torch.uint8, device="cuda"),
                        u_right=torch.zeros(cap, device="cuda"), depth=torch.zeros(cap, device="cuda"),
                        kp_class=torch.zeros(cap, dtype=torch.uint8, device="cuda"), kp_conf=torch.zeros(cap, dtype=torch.float64, device="cuda"),
@@ -40,30 +37,21 @@ def test_chain_and_creation_beside_tracking(seg, kitti_bgr):
     torch.cuda.synchronize()
 
     def front_end(i, b):
-        bgr, gl, gr = d_in[i]
         seg.set_frame(600 + i)
-        seg.run_device_maps(ptr(bgr), ptr(b["cls"]), ptr(b["conf"]), ptr(b["ent"]), 0, 0, s)
-        el.wait_for_stream(s)
-        er.wait_for_stream(s)
-        b["kl"].enqueue(el, gl)
-        b["kr"].enqueue(er, gr)
-        el.stream_wait(s)
-        b["sem"].run(seg, b["kl"], 8, s)
-        b["st"].run(el, er, b["kl"], b["kr"], MB, MBF, s, keep=b["sem"].keep, n_left=b["sem"].n)
+        b["f"].extract(seg, *d_in[i], s)
+        b["f"].tail(seg, MB, MBF, s)
 
     for i, b in enumerate(bufs):
         front_end(i, b)
-        sem, st, kl = b["sem"], b["st"], b["kl"]
-        keyframe_gather_device(el, ptr(kl.kps), ptr(kl.desc), ptr(sem.keep), ptr(sem.n), ptr(st.u), ptr(st.z), ptr(sem.cls), ptr(sem.conf),
-                               ptr(sem.ent), b["kf"], s)
+        f = b["f"]
+        keyframe_gather_device(el, f.kps, f.desc, f.keep, f.n_keep, f.u_right, f.depth, f.kp_class, f.kp_conf, f.kp_entropy, b["kf"], s)
     s_track.synchronize()
 
     # the gather against the Frame tail's layout: keys, descriptors and maps by keep_idx[j], mvRight / mvDepth by j
     kfs = []
     for i, b in enumerate(bufs):
-        n, keep = b["sem"].host()
-        kps_all, desc_all = b["kl"].host()[:2]
-        ur, depth = b["st"].host(n)
+        n, keep, ur, depth = b["f"].host()
+        kps_all, desc_all = b["f"].left.host()
         g = {k: v.cpu().numpy() for k, v in b["kf"].items()}
         assert int(g["count"][0]) == n and n > 100
         gk = g["kps"].view(KP_DTYPE)[:n]
@@ -71,8 +59,8 @@ def test_chain_and_creation_beside_tracking(seg, kitti_bgr):
         assert np.array_equal(g["desc"].reshape(cap, 32)[:n], desc_all[keep])
         assert np.array_equal(g["u_right"][:n].view(np.uint32), ur.view(np.uint32))
         assert np.array_equal(g["depth"][:n].view(np.uint32), depth.view(np.uint32))
-        for k, src in (("kp_class", "cls"), ("kp_conf", "conf"), ("kp_entropy", "ent")):
-            assert np.array_equal(g[k][:n], getattr(b["sem"], src).cpu().numpy()[keep])
+        for k in ("kp_class", "kp_conf", "kp_entropy"):
+            assert np.array_equal(g[k][:n], b["f"].out[k].cpu().numpy()[keep])
         desc = g["desc"].reshape(cap, 32)[:n]
         node = (desc[:, 0] >> 3).astype(np.int32)  # a stand-in vocabulary: 32 nodes by the first descriptor byte
         b["node"] = torch.from_numpy(np.concatenate([node, np.zeros(cap - n, np.int32)])).cuda()
@@ -120,13 +108,14 @@ def test_chain_and_creation_beside_tracking(seg, kitti_bgr):
     serial = create()
     s_map.synchronize()
     # LocalMapping's creation on its own stream while Tracking runs frame 0 again on the same left extractor
-    first = {k: v.clone() for k, v in (("keep", bufs[0]["sem"].keep), ("u", bufs[0]["st"].u))}
+    first = {k: bufs[0]["f"].out[k].clone() for k in ("keep_idx", "u_right")}
     torch.cuda.synchronize()
     concurrent = create()
     front_end(0, bufs[0])
     s_map.synchronize()
     s_track.synchronize()
-    assert torch.equal(first["keep"], bufs[0]["sem"].keep) and torch.equal(first["u"].view(torch.int32), bufs[0]["st"].u.view(torch.int32))
+    out = bufs[0]["f"].out
+    assert torch.equal(first["keep_idx"], out["keep_idx"]) and torch.equal(first["u_right"].view(torch.int32), out["u_right"].view(torch.int32))
     for o in (serial, concurrent):
         r = {k: v.cpu().numpy() for k, v in o.items()}
         assert int(r["n"][0]) == len(want["created"])

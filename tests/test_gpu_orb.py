@@ -7,16 +7,12 @@ import numpy as np
 import pytest
 
 from conftest import GOLDEN
+from frame_support import kp_matrix
 from oracle import orb_oracle as O
 from sivo_b200 import ORBextractor, stereo_hamming, KP_DTYPE
 from sivo_b200.synth import bgr_to_gray, stereo_frame
 
 pytestmark = pytest.mark.gpu
-
-
-def kp_matrix(kps):
-    return np.stack([kps["x"], kps["y"], kps["size"], kps["angle"], kps["response"], kps["octave"].astype(np.float32),
-                     kps["class_id"].astype(np.float32)], axis=1)
 
 
 @pytest.mark.parametrize("name,nf", [("orb_kitti_2000", 2000), ("orb_kitti_1000", 1000)])

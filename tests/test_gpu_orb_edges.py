@@ -8,14 +8,13 @@ import numpy as np
 import pytest
 import torch
 
+from frame_support import MB, MBF, InfoOut, cameras, kp_matrix, seg, synth, upload  # noqa: F401
 from oracle import orb_oracle as O
 from oracle import orb_scene as S
 from sivo_b200 import KP_DTYPE, ORBextractor, info_select, stereo_match
 from sivo_b200 import _lib as L
+from sivo_b200.frame import DeviceFrame
 from sivo_b200.synth import bgr_to_gray
-from test_gpu_frame_tail import DeviceKeys, SemanticOut, StereoOut, seg, synth, to_dev  # noqa: F401
-from test_gpu_info_select import MB, MBF, InfoOut, cameras
-from test_gpu_orb import kp_matrix
 
 pytestmark = pytest.mark.gpu
 
@@ -45,7 +44,7 @@ def run_async(ext, img):
     """sivo_orb_enqueue_device on a device copy of img: (count, records, descriptors, status mask)."""
     rows, cols = img.shape
     cap = ext.capacity()
-    d_gray = to_dev(img)
+    d_gray = upload(img)
     d_kps = torch.zeros(cap * 28, dtype=torch.uint8, device="cuda")
     d_desc = torch.zeros(cap * 32, dtype=torch.uint8, device="cuda")
     d_cnt = torch.full((1,), -7, dtype=torch.int64, device="cuda")
@@ -138,7 +137,7 @@ def test_pitched_input_in_every_form(case):
     ext = make(p)
     k, d = ext(view, None)
     assert np.array_equal(kp_matrix(k), want_k) and np.array_equal(d, want_d)
-    d_big = to_dev(big)
+    d_big = upload(big)
     k2, d2 = ext.run_device_input(d_big.data_ptr(), rows, cols, pitch)
     assert k2.tobytes() == k.tobytes() and np.array_equal(d2, d)
     cap = ext.capacity()
@@ -157,21 +156,15 @@ def test_pitched_input_in_every_form(case):
 def _chain(seg, el, er, bgr, gl, gr, cam):
     """SegNet -> both extractors' enqueue_device -> semantic keys -> stereo -> information selection, all on the device."""
     seg.set_frame(3)
-    seg.segment_on_device(bgr)
     stream = torch.cuda.Stream()
     s = stream.cuda_stream
-    dkl, dkr = DeviceKeys(el), DeviceKeys(er)
-    dkl.enqueue(el, to_dev(gl))
-    dkr.enqueue(er, to_dev(gr))
-    el.stream_wait(s)
-    sem = SemanticOut(dkl.cap)
-    sem.run(seg, dkl, 8, s)
-    st = StereoOut(dkl.cap)
-    st.run(el, er, dkl, dkr, MB, MBF, s, keep=sem.keep, n_left=sem.n)
-    info = InfoOut(dkl.cap)
-    info.run(el, dkl.kps.data_ptr(), sem.ent.data_ptr(), sem.keep.data_ptr(), sem.n.data_ptr(), st.z.data_ptr(), cam, 0.0, s)
+    f = DeviceFrame(el, er, *gl.shape)
+    info = InfoOut(f.left.cap)
+    f.extract(seg, upload(bgr), upload(gl), upload(gr), s)
+    f.tail(seg, MB, MBF, s)
+    info.run(el, f.kps, f.kp_entropy, f.keep, f.n_keep, f.depth, cam, 0.0, s)
     stream.synchronize()
-    return dkl, sem, st, info
+    return f, info
 
 
 def test_overflow_propagates_through_the_device_frame_tail(seg):
@@ -181,25 +174,25 @@ def test_overflow_propagates_through_the_device_frame_tail(seg):
     el, er = ORBextractor(2000, 1.2, 8, 20, 7), ORBextractor(2000, 1.2, 8, 20, 7)
     gl, gr = S.noise(S.H, S.W, 1), S.noise(S.H, S.W, 2)
     bgr = np.ascontiguousarray(np.repeat(gl[:, :, None], 3, axis=2))
-    dkl, sem, st, info = _chain(seg, el, er, bgr, gl, gr, cam)
+    f, info = _chain(seg, el, er, bgr, gl, gr, cam)
     assert el.device_status() & 0b111 == 0b111 and er.device_status() & 0b111 == 0b111
-    assert int(dkl.cnt.cpu()[0]) == -1
-    assert int(sem.n.cpu()[0]) == -1 and (sem.keep.cpu().numpy() == -7).all() and (sem.cls.cpu().numpy() == 77).all()
-    assert (st.u.cpu().numpy() == 7.0).all() and (st.z.cpu().numpy() == 7.0).all()
+    assert int(f.left.count.cpu()[0]) == -1
+    out = {k: v.cpu().numpy() for k, v in f.out.items()}
+    assert int(out["n_keep"][0]) == -1 and (out["keep_idx"] == -7).all() and (out["kp_class"] == 77).all()
+    assert (out["u_right"] == 7.0).all() and (out["depth"] == 7.0).all()
     assert int(info.n.cpu()[0]) == -1 and (info.sel.cpu().numpy() == -7).all() and (info.red.cpu().numpy() == 7.0).all()
 
     bgr, gl, gr = synth(1)
-    dkl, sem, st, info = _chain(seg, el, er, bgr, gl, gr, cam)
+    f, info = _chain(seg, el, er, bgr, gl, gr, cam)
     assert el.device_status() == 0 and er.device_status() == 0
     kl, dl = ORBextractor(2000, 1.2, 8, 20, 7)(gl, None)
     kr, dr = ORBextractor(2000, 1.2, 8, 20, 7)(gr, None)
-    kps, _ = dkl.host()
+    kps, _ = f.left.host()
     assert kps.tobytes() == kl.tobytes()
-    n_keep, keep = sem.host()
+    n_keep, keep, u, z = f.host()
     assert np.array_equal(keep, seg.semantic_keys(kl, 8)[3]) and n_keep > 100
-    u, z = st.host(n_keep)
     hu, hz = stereo_match(el, er, kl[keep], dl[keep], kr, dr, MB, MBF)
     assert u.tobytes() == hu.tobytes() and z.tobytes() == hz.tobytes()
-    ent = sem.ent.cpu().numpy()[:len(kl)][keep]
+    ent = f.out["kp_entropy"].cpu().numpy()[:len(kl)][keep]
     _, _, sel = info_select(el, kl[keep], z, ent, cam, 0.0)
     assert int(info.n.cpu()[0]) == len(sel) > 0 and np.array_equal(info.sel.cpu().numpy()[:len(sel)], sel)

@@ -7,33 +7,19 @@ import numpy as np
 import pytest
 import torch
 
+from frame_support import BOUNDS, CX, CY, FX, MB, MBF, H, W, check_pose, ext, frame_inputs, ptr, seg, upload  # noqa: F401
 from oracle import info_oracle as I
 from oracle import pose_oracle as P
 from oracle import track_oracle as T
+from oracle.mapping_scene import rotation
 from sivo_b200 import (info_select, info_select_device, make_frame, map_points, pose_gather_device, pose_optimize_device, search_last_frame_device,
                        search_local_points_device)
+from sivo_b200.frame import DeviceFrame
 from sivo_b200.pose import camera_from_result, frame_from_result, result_from_bytes
-from sivo_b200.synth import bgr_to_gray
-from test_gpu_frame_tail import BASELINES, H, W, DeviceKeys, SemanticOut, StereoOut, crop, extractors, ptr, seg, synth  # noqa: F401
-from test_gpu_info_select import rotation
 
 pytestmark = pytest.mark.gpu
 
-MB, MBF = BASELINES["kitti"]
-FX, CX, CY = 718.856, 607.1928 - 109, 185.2157 - 11
-BOUNDS = (0.0, float(W), 0.0, float(H))
 TH_LAST, TH_LOCAL = 7, 1
-
-
-@pytest.fixture(scope="module")
-def ext():
-    return extractors(2000)
-
-
-def frame_inputs(kitti_bgr):
-    gl = crop(bgr_to_gray(kitti_bgr))  # the fixture frame has no right image: the left one shifted by 12 px stands in for it
-    out = [(crop(kitti_bgr), gl, np.ascontiguousarray(np.roll(gl, -12, axis=1)))]
-    return out + [synth(s) for s in (1, 2)]
 
 
 def make_map(kps, desc, depth, scale, Rcw, tcw, seed):
@@ -50,38 +36,17 @@ def make_map(kps, desc, depth, scale, Rcw, tcw, seed):
     return pts[0::2].copy(), pts[1::2].copy()
 
 
-def dev(a):
-    return torch.from_numpy(np.ascontiguousarray(a).view(np.uint8).reshape(-1).copy()).cuda()
-
-
-def check_pose(res, outl, ref):
-    assert np.abs(P.rotation_matrix(np.array(res.q)) - P.rotation_matrix(ref.q)).max() <= 1e-9
-    assert np.abs(np.array(res.t) - ref.t).max() <= 1e-9 * (np.abs(ref.t).max() + 1)
-    assert res.sigma_valid == ref.sigma_valid and res.n_initial == ref.n_initial and res.rounds_run == ref.rounds_run
-    if ref.sigma_valid:
-        assert np.linalg.norm(res.sigma() - ref.sigma) <= 1e-8 * np.linalg.norm(ref.sigma)
-    near = np.zeros(len(outl), bool)
-    with np.errstate(invalid="ignore"):
-        near[ref.edges.key] = np.abs(ref.chi2 - float(P.CHI2_STEREO)) <= 1e-6 * float(P.CHI2_STEREO)
-    assert np.array_equal(outl[~near], ref.outlier[~near])
-    if not near.any():
-        assert res.n_good == ref.n_good
-
-
 def test_three_frames_in_flight_through_both_optimisations(seg, ext, kitti_bgr):
     el, er = ext
     inputs = frame_inputs(kitti_bgr)
-    d_in = [[torch.from_numpy(x).cuda() for x in f] for f in inputs]
-    hw = H * W
+    d_in = [[upload(x) for x in f] for f in inputs]
     cap = el.capacity()
     scale = el.GetScaleFactors()
     stream = torch.cuda.Stream()
     s = stream.cuda_stream
     bufs = []
     for _ in inputs:
-        b = {"cls": torch.empty(hw, dtype=torch.uint8, device="cuda"), "conf": torch.empty(hw, dtype=torch.float64, device="cuda"),
-             "ent": torch.empty(hw, dtype=torch.float64, device="cuda"), "kl": DeviceKeys(el), "kr": DeviceKeys(er)}
-        b["sem"], b["st"] = SemanticOut(b["kl"].cap), StereoOut(b["kl"].cap)
+        b = {"f": DeviceFrame(el, er, H, W)}
         for k in ("m_last", "m_loc"):
             b[k] = torch.full((cap,), -7, dtype=torch.int32, device="cuda")
         for k in ("n_last", "n_loc", "n_sel"):
@@ -100,16 +65,9 @@ def test_three_frames_in_flight_through_both_optimisations(seg, ext, kitti_bgr):
     torch.cuda.synchronize()
 
     def front_end(i, b):
-        bgr, gl, gr = d_in[i]
         seg.set_frame(400 + i)
-        seg.run_device_maps(ptr(bgr), ptr(b["cls"]), ptr(b["conf"]), ptr(b["ent"]), 0, 0, s)
-        el.wait_for_stream(s)  # the previous frame's stereo, searches and optimisations are done with the left extractor
-        er.wait_for_stream(s)
-        b["kl"].enqueue(el, gl)
-        b["kr"].enqueue(er, gr)
-        el.stream_wait(s)
-        b["sem"].run(seg, b["kl"], 8, s)
-        b["st"].run(el, er, b["kl"], b["kr"], MB, MBF, s, keep=b["sem"].keep, n_left=b["sem"].n)
+        b["f"].extract(seg, *d_in[i], s)  # waits for the previous frame's stereo, searches and optimisations
+        b["f"].tail(seg, MB, MBF, s)
 
     # a first pass of the front end (it captures the network's graph) gives each frame's keys, from which its map is made
     for i, b in enumerate(bufs):
@@ -117,16 +75,15 @@ def test_three_frames_in_flight_through_both_optimisations(seg, ext, kitti_bgr):
     stream.synchronize()
     cases = []
     for i, b in enumerate(bufs):
-        n_keep, keep = b["sem"].host()
-        kps_all, desc_all = b["kl"].host()[:2]
+        n_keep, keep, ur, depth = b["f"].host()
+        kps_all, desc_all = b["f"].left.host()
         kps, desc = kps_all[keep], desc_all[keep]
-        ur, depth = b["st"].host(n_keep)
         R_true, t_true = rotation(0.01 * i, -0.02, 0.005), np.array([0.1 * i, -0.05, 0.3])
         last_pts, local_pts = make_map(kps, desc, depth, scale, R_true, t_true, 40 + i)
         Tpred = np.concatenate([rotation(0.001, -0.0015, 0.001) @ R_true, (t_true + [0.01, -0.005, 0.01])[:, None]], 1).astype(np.float32)
         cases.append(dict(n_keep=n_keep, keep=keep, kps=kps, desc=desc, ur=ur, depth=depth, last=last_pts, local=local_pts,
-                          Tpred=Tpred, ent=b["sem"].ent.cpu().numpy()[keep]))
-        b["d_last"], b["d_local"] = dev(last_pts), dev(local_pts)
+                          Tpred=Tpred, ent=b["f"].out["kp_entropy"].cpu().numpy()[keep]))
+        b["d_last"], b["d_local"] = upload(last_pts), upload(local_pts)
         b["T0"].copy_(torch.from_numpy(Tpred.reshape(-1)))
         assert len(last_pts) > 40 and len(local_pts) > 40
     torch.cuda.synchronize()
@@ -135,29 +92,28 @@ def test_three_frames_in_flight_through_both_optimisations(seg, ext, kitti_bgr):
     # the previous frame's search and optimisation
     for i, b in enumerate(bufs):
         front_end(i, b)
-        c, kl = cases[i], b["kl"]
+        c, f = cases[i], b["f"]
         frame = make_frame(FX, FX, CX, CY, MBF, BOUNDS, c["Tpred"][:, :3], c["Tpred"][:, 3])
-        search_last_frame_device(el, ptr(kl.kps), ptr(kl.desc), ptr(b["sem"].keep), ptr(b["sem"].n), ptr(b["st"].u), ptr(b["d_last"]),
-                                 len(c["last"]), frame, c["Tpred"][:, :3], c["Tpred"][:, 3], TH_LAST, ptr(b["m_last"]), ptr(b["n_last"]), s)
-        pose_gather_device(el, ptr(b["m_last"]), ptr(b["sem"].n), ptr(b["d_last"]), len(c["last"]), ptr(b["xw"]), s)
-        pose_optimize_device(el, ptr(kl.kps), ptr(b["sem"].keep), ptr(b["sem"].n), ptr(b["st"].u), ptr(b["xw"]), FX, FX, CX, CY, MBF,
-                             ptr(b["T0"]), ptr(b["r1"]), ptr(b["o1"]), s)
+        search_last_frame_device(el, f.kps, f.desc, f.keep, f.n_keep, f.u_right, ptr(b["d_last"]), len(c["last"]), frame, c["Tpred"][:, :3],
+                                 c["Tpred"][:, 3], TH_LAST, ptr(b["m_last"]), ptr(b["n_last"]), s)
+        pose_gather_device(el, ptr(b["m_last"]), f.n_keep, ptr(b["d_last"]), len(c["last"]), ptr(b["xw"]), s)
+        pose_optimize_device(el, f.kps, f.keep, f.n_keep, f.u_right, ptr(b["xw"]), FX, FX, CX, CY, MBF, ptr(b["T0"]), ptr(b["r1"]),
+                             ptr(b["o1"]), s)
     stream.synchronize()
     # TrackWithMotionModel discards the outliers; the local-map search then runs at the optimised pose with the kept keys blocked
     r1 = [result_from_bytes(b["r1"].cpu().numpy()) for b in bufs]
     with torch.cuda.stream(stream):
         for i, b in enumerate(bufs):
-            c, kl = cases[i], b["kl"]
+            c, f = cases[i], b["f"]
             xw = b["xw"].view(-1, 3)
             xw.masked_fill_(b["o1"].bool()[:, None], float("nan"))
             b["blocked"].copy_((~torch.isnan(xw[:, 0])).to(torch.uint8))
             frame = frame_from_result(r1[i], FX, FX, CX, CY, MBF, BOUNDS)
-            search_local_points_device(el, ptr(kl.kps), ptr(kl.desc), ptr(b["sem"].keep), ptr(b["sem"].n), ptr(b["st"].u), ptr(b["blocked"]),
-                                       ptr(b["d_local"]), len(c["local"]), frame, TH_LOCAL, 0.8, ptr(b["view"]), ptr(b["m_loc"]),
-                                       ptr(b["n_loc"]), s)
-            pose_gather_device(el, ptr(b["m_loc"]), ptr(b["sem"].n), ptr(b["d_local"]), len(c["local"]), ptr(b["xw"]), s)
-            pose_optimize_device(el, ptr(kl.kps), ptr(b["sem"].keep), ptr(b["sem"].n), ptr(b["st"].u), ptr(b["xw"]), FX, FX, CX, CY, MBF,
-                                 ptr(b["r1"]), ptr(b["r2"]), ptr(b["o2"]), s)
+            search_local_points_device(el, f.kps, f.desc, f.keep, f.n_keep, f.u_right, ptr(b["blocked"]), ptr(b["d_local"]), len(c["local"]),
+                                       frame, TH_LOCAL, 0.8, ptr(b["view"]), ptr(b["m_loc"]), ptr(b["n_loc"]), s)
+            pose_gather_device(el, ptr(b["m_loc"]), f.n_keep, ptr(b["d_local"]), len(c["local"]), ptr(b["xw"]), s)
+            pose_optimize_device(el, f.kps, f.keep, f.n_keep, f.u_right, ptr(b["xw"]), FX, FX, CX, CY, MBF, ptr(b["r1"]), ptr(b["r2"]),
+                                 ptr(b["o2"]), s)
     stream.synchronize()
     r2 = [result_from_bytes(b["r2"].cpu().numpy()) for b in bufs]
     prior = 1e-4 * np.eye(6)
@@ -172,8 +128,9 @@ def test_three_frames_in_flight_through_both_optimisations(seg, ext, kitti_bgr):
         k = len(r) // 2
         thresholds.append(0.5 * (r[k] + r[k + 1]))
         cams.append((cam, ocam))
-        info_select_device(el, ptr(b["kl"].kps), ptr(b["sem"].ent), ptr(b["sem"].keep), ptr(b["sem"].n), ptr(b["st"].z), cam,
-                           thresholds[i], ptr(b["world"]), ptr(b["red"]), ptr(b["sel"]), ptr(b["n_sel"]), s)
+        f = b["f"]
+        info_select_device(el, f.kps, f.kp_entropy, f.keep, f.n_keep, f.depth, cam, thresholds[i], ptr(b["world"]), ptr(b["red"]),
+                           ptr(b["sel"]), ptr(b["n_sel"]), s)
     stream.synchronize()
 
     n_edges = [0, 0]
@@ -182,7 +139,7 @@ def test_three_frames_in_flight_through_both_optimisations(seg, ext, kitti_bgr):
         c = cases[i]
         n = c["n_keep"]
         # the front end gave the same keys as the first pass
-        assert int(b["sem"].n.cpu()[0]) == n and np.array_equal(b["sem"].keep.cpu().numpy()[:n], c["keep"])
+        assert int(b["f"].out["n_keep"].cpu()[0]) == n and np.array_equal(b["f"].out["keep_idx"].cpu().numpy()[:n], c["keep"])
         # last-frame search
         of = T.Frame(FX, FX, CX, CY, MBF, BOUNDS, c["Tpred"][:, :3], c["Tpred"][:, 3])
         om, on = T.search_last_frame(c["kps"], c["desc"], c["ur"], c["last"], of, c["Tpred"][:, :3], c["Tpred"][:, 3], scale, TH_LAST)

@@ -9,6 +9,7 @@ import numpy as np
 import pytest
 import torch
 
+from frame_support import upload
 from oracle import orb_oracle as O
 from oracle import stereo_scene as S
 from sivo_b200 import KP_DTYPE, ORBextractor, stereo_hamming, stereo_match, stereo_match_device
@@ -22,12 +23,6 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 KITTI_MBF = 386.1448
 KITTI_MB = KITTI_MBF / 718.856
 f32 = np.float32
-
-
-def dev(a):
-    t = torch.from_numpy(np.ascontiguousarray(a).view(np.uint8).reshape(-1)).cuda()
-    torch.cuda.synchronize()
-    return t
 
 
 def dev_buf(cap, rec, fill):
@@ -54,11 +49,11 @@ def device_form(el, er, kl, dl, kr, dr, mb, mbf, keep, n_left=None, n_right=None
     bl, bdl = dev_buf(cap_l, 28, 0), dev_buf(cap_l, 32, 0)
     br, bdr = dev_buf(cap_r, 28, 0), dev_buf(cap_r, 32, 0)
     if len(kl):
-        bl[:len(kl) * 28] = dev(kl)
-        bdl[:len(kl) * 32] = dev(dl)
+        bl[:len(kl) * 28] = upload(kl)
+        bdl[:len(kl) * 32] = upload(dl)
     if len(kr):
-        br[:len(kr) * 28] = dev(kr)
-        bdr[:len(kr) * 32] = dev(dr)
+        br[:len(kr) * 28] = upload(kr)
+        bdr[:len(kr) * 32] = upload(dr)
     d_keep = torch.from_numpy(np.ascontiguousarray(keep, np.int32)).cuda()
     nl = torch.tensor([len(keep) if n_left is None else n_left], dtype=torch.int64, device="cuda")
     nr = torch.tensor([len(kr) if n_right is None else n_right], dtype=torch.int64, device="cuda")
@@ -301,7 +296,7 @@ def test_semantic_keys_of_non_finite_keys(seg):
     # the device form
     cap = 64
     buf = dev_buf(cap, 28, 0)
-    buf[:len(kps) * 28] = dev(kps)
+    buf[:len(kps) * 28] = upload(kps)
     cnt = torch.tensor([len(kps)], dtype=torch.int64, device="cuda")
     cls = torch.full((cap,), 77, dtype=torch.uint8, device="cuda")
     conf = torch.full((cap,), 7.0, dtype=torch.float64, device="cuda")

@@ -5,19 +5,16 @@ import numpy as np
 import pytest
 import torch
 
+from frame_support import BOUNDS, CX, CY, FX, MB, MBF, H, W, extractors, ptr, synth, upload
 from oracle import track_oracle as T
+from oracle.mapping_scene import rotation
 from sivo_b200 import (info_select_device, make_frame, map_points, pose_gather_device, pose_optimize_device, search_last_frame_device,
-                       search_local_points_device, stereo_match)
+                       search_local_points_device, stereo_match, stereo_match_device)
+from sivo_b200.frame import FrameKeys
 from sivo_b200.info import make_camera
 from sivo_b200.pose import result_from_bytes
-from test_gpu_frame_tail import BASELINES, H, W, DeviceKeys, StereoOut, extractors, ptr, synth, to_dev
-from test_gpu_info_select import rotation
 
 pytestmark = pytest.mark.gpu
-
-MB, MBF = BASELINES["kitti"]
-FX, CX, CY = 718.856, 607.1928 - 109, 185.2157 - 11
-BOUNDS = (0.0, float(W), 0.0, float(H))
 
 
 def problem(el, er, kl, dl, kr, dr, keep, angles, seed):
@@ -34,17 +31,17 @@ def problem(el, er, kl, dl, kr, dr, keep, angles, seed):
     cap = el.capacity()
     ent = np.zeros(cap)
     ent[:len(kl)] = rng.uniform(0, 0.5, len(kl))
-    p = dict(keep=to_dev(keep.astype(np.int32)), n=to_dev(np.array([len(keep)], np.int64)), last=pts[0::2].copy(), local=pts[1::2].copy(),
-             Tpred=Tpred, ent=to_dev(ent), cam=make_camera(FX, FX, CX, CY, MB, R.T, -R.T @ t, 1e-4 * np.eye(6)))
-    p["d_last"] = to_dev(p["last"].view(np.uint8).reshape(-1))
-    p["d_local"] = to_dev(p["local"].view(np.uint8).reshape(-1))
-    p["T0"] = to_dev(Tpred.reshape(-1))
+    p = dict(keep=upload(keep.astype(np.int32)), n=upload(np.array([len(keep)], np.int64)), last=pts[0::2].copy(), local=pts[1::2].copy(),
+             Tpred=Tpred, ent=upload(ent), cam=make_camera(FX, FX, CX, CY, MB, R.T, -R.T @ t, 1e-4 * np.eye(6)))
+    p["d_last"] = upload(p["last"])
+    p["d_local"] = upload(p["local"])
+    p["T0"] = upload(Tpred)
     p["frame"] = make_frame(FX, FX, CX, CY, MBF, BOUNDS, Tpred[:, :3], Tpred[:, 3])
     return p
 
 
 def outputs(cap, n_local):
-    o = {"st": StereoOut(cap), "world": torch.full((3 * cap,), 7.0, device="cuda"),
+    o = {"u": torch.full((cap,), 7.0, device="cuda"), "z": torch.full((cap,), 7.0, device="cuda"), "world": torch.full((3 * cap,), 7.0, device="cuda"),
          "red": torch.full((cap,), 7.0, dtype=torch.float64, device="cuda"), "view": torch.full((n_local,), 7, dtype=torch.uint8, device="cuda"),
          "xw": torch.full((3 * cap,), float("nan"), device="cuda"), "res": torch.full((512,), 0x55, dtype=torch.uint8, device="cuda"),
          "outl": torch.full((cap,), 7, dtype=torch.uint8, device="cuda")}
@@ -59,11 +56,12 @@ def outputs(cap, n_local):
 def calls(el, er, dkl, dkr, p, o, s):
     """The Frame tail's device calls on one problem, in Tracking's order, each a closure enqueuing on stream `s`."""
     keep, n = ptr(p["keep"]), ptr(p["n"])
-    u, z = ptr(o["st"].u), ptr(o["st"].z)
+    u, z = ptr(o["u"]), ptr(o["z"])
     nl, nloc = len(p["last"]), len(p["local"])
     R, t = p["Tpred"][:, :3], p["Tpred"][:, 3]
     return [
-        lambda: o["st"].run(el, er, dkl, dkr, MB, MBF, s, keep=p["keep"], n_left=p["n"]),
+        lambda: stereo_match_device(el, er, ptr(dkl.kps), ptr(dkl.desc), keep, n, ptr(dkr.kps), ptr(dkr.desc), ptr(dkr.count), MB, MBF, u, z,
+                                    s),
         lambda: info_select_device(el, ptr(dkl.kps), ptr(p["ent"]), keep, n, z, p["cam"], 0.0, ptr(o["world"]), ptr(o["red"]),
                                    ptr(o["sel"]), ptr(o["n_sel"]), s),
         lambda: search_last_frame_device(el, ptr(dkl.kps), ptr(dkl.desc), keep, n, u, ptr(p["d_last"]), nl, p["frame"], R, t, 7,
@@ -77,15 +75,15 @@ def calls(el, er, dkl, dkr, p, o, s):
 
 
 def host(o):
-    return {k: (v.u.cpu().numpy().tobytes() + v.z.cpu().numpy().tobytes() if k == "st" else v.cpu().numpy().tobytes()) for k, v in o.items()}
+    return {k: v.cpu().numpy().tobytes() for k, v in o.items()}
 
 
 def test_two_problems_on_two_streams_equal_the_calls_in_sequence():
     el, er = extractors(2000)
     _, gl, gr = synth(4)
-    dkl, dkr = DeviceKeys(el), DeviceKeys(er)
-    dkl.enqueue(el, to_dev(gl))
-    dkr.enqueue(er, to_dev(gr))
+    dkl, dkr = FrameKeys(el), FrameKeys(er)
+    dkl.enqueue(el, upload(gl), H, W, W)
+    dkr.enqueue(er, upload(gr), H, W, W)
     torch.cuda.synchronize()
     kl, dl = dkl.host()
     kr, dr = dkr.host()

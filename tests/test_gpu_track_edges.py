@@ -11,6 +11,7 @@ import numpy as np
 import pytest
 import torch
 
+from frame_support import upload
 from oracle import track_oracle as T
 from sivo_b200 import _lib as L
 from sivo_b200 import (KP_DTYPE, MAP_POINT_DTYPE, ORBextractor, make_frame, search_last_frame, search_last_frame_device,
@@ -88,10 +89,6 @@ class Scene:
         return make_frame(FX, FX, CX, CY, MBF, self.bounds, self.R, self.t), oframe(self.bounds, self.R, self.t)
 
 
-def dev_bytes(a):
-    return torch.from_numpy(np.ascontiguousarray(a).view(np.uint8).reshape(-1).copy()).cuda()
-
-
 class Searcher:
     """Runs a scene through the oracle, the host form and the device form of one extractor and asserts bit identity."""
 
@@ -123,8 +120,8 @@ class Searcher:
         blocked[np.flatnonzero(hole)] = 1
         if sc.blocked is not None:
             blocked[slot] = sc.blocked
-        bufs = [dev_bytes(a) for a in (kps, desc, keep.astype(np.int32), np.array([n + holes], np.int64), ur, blocked)]
-        pts = dev_bytes(mp_records(sc.pts)) if m else None
+        bufs = [upload(a) for a in (kps, desc, keep.astype(np.int32), np.array([n + holes], np.int64), ur, blocked)]
+        pts = upload(mp_records(sc.pts)) if m else None
         view = torch.full((max(m, 1),), 7, dtype=torch.uint8, device="cuda")
         match = torch.full((cap,), -7, dtype=torch.int32, device="cuda")
         nm = torch.full((1,), -7, dtype=torch.int64, device="cuda")

@@ -7,17 +7,17 @@ import numpy as np
 import pytest
 import torch
 
+from frame_support import BOUNDS, CX, CY, FX, MB, MBF, H, W, ext, ptr, seg, synth, tails, upload  # noqa: F401
 from oracle import track_oracle as T
+from oracle.mapping_scene import rotation
 from sivo_b200 import _lib as L
 from sivo_b200 import (MAP_POINT_DTYPE, make_frame, map_points, search_last_frame, search_last_frame_device, search_local_points,
                        search_local_points_device, stereo_match)
+from sivo_b200.frame import DeviceFrame
 from sivo_b200.track import features_in_area
-from test_gpu_frame_tail import H, W, DeviceKeys, SemanticOut, StereoOut, ptr, seg, synth  # noqa: F401
-from test_gpu_info_select import CX, CY, FX, MB, MBF, Tail, ext, rotation, tails  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
-BOUNDS = (0.0, float(W), 0.0, float(H))
 POSES = {"identity": (np.eye(3), np.zeros(3)), "moved": (rotation(0.002, 0.01, -0.003), np.array([0.02, -0.01, 0.3])),
          "forward": (np.eye(3), np.array([0.0, 0.0, -1.0])), "backward": (np.eye(3), np.array([0.0, 0.0, 1.0]))}
 
@@ -33,8 +33,8 @@ class Keys:
     def __init__(self, t):
         self.t = t
         self.kps = t.kps
-        self.desc = t.dkl.host()[1][t.keep]
-        self.ur = t.st.host(t.n_keep)[0]
+        self.desc = t.f.left.host()[1][t.keep]
+        self.ur = t.ur
         self.depth = t.depth
 
 
@@ -70,12 +70,6 @@ def keysets(tails):
     return {f: Keys(t) for f, t in tails.items()}
 
 
-def dev(a, dtype=torch.uint8):
-    x = torch.from_numpy(np.ascontiguousarray(a).view(np.uint8).reshape(-1).copy()).cuda()
-    torch.cuda.synchronize()
-    return x
-
-
 class SearchOut:
     def __init__(self, cap, n_points):
         self.view = torch.full((max(n_points, 1),), 7, dtype=torch.uint8, device="cuda")
@@ -88,20 +82,21 @@ class SearchOut:
 
 
 def run_local_device(el, t, pts_dev, n_points, frame, th, stream, n=None, keep="sem", null=(), blocked=0):
-    out = SearchOut(t.dkl.cap, n_points)
+    f = t.f
+    out = SearchOut(f.left.cap, n_points)
     p = {k: (0 if k in null else ptr(getattr(out, k))) for k in ("view", "match", "n")}
-    search_local_points_device(el, ptr(t.dkl.kps), ptr(t.dkl.desc), ptr(t.sem.keep) if keep == "sem" else 0,
-                               ptr(t.sem.n if n is None else n), ptr(t.st.u), blocked, ptr(pts_dev), n_points, frame, th, 0.8, p["view"],
-                               p["match"], p["n"], stream.cuda_stream)
+    search_local_points_device(el, f.kps, f.desc, f.keep if keep == "sem" else 0, f.n_keep if n is None else ptr(n), f.u_right, blocked,
+                               ptr(pts_dev), n_points, frame, th, 0.8, p["view"], p["match"], p["n"], stream.cuda_stream)
     stream.synchronize()
     return out
 
 
 def run_last_device(el, t, pts_dev, n_points, frame, th, stream, null=()):
-    out = SearchOut(t.dkl.cap, n_points)
+    f = t.f
+    out = SearchOut(f.left.cap, n_points)
     p = {k: (0 if k in null else ptr(getattr(out, k))) for k in ("match", "n")}
-    search_last_frame_device(el, ptr(t.dkl.kps), ptr(t.dkl.desc), ptr(t.sem.keep), ptr(t.sem.n), ptr(t.st.u), ptr(pts_dev), n_points,
-                             frame, np.eye(3), np.zeros(3), th, p["match"], p["n"], stream.cuda_stream)
+    search_last_frame_device(el, f.kps, f.desc, f.keep, f.n_keep, f.u_right, ptr(pts_dev), n_points, frame, np.eye(3), np.zeros(3), th,
+                             p["match"], p["n"], stream.cuda_stream)
     stream.synchronize()
     return out
 
@@ -146,7 +141,7 @@ def test_local_search_is_bit_identical_to_the_oracle(keysets, tails, ext, pose, 
         T.search_local_points(k.kps, k.desc, k.ur, lone, of, el.GetScaleFactors(), th, 0.8, per_point=free)
         changed += sum(a != b and a >= 0 and b >= 0 for a, b in zip(per, free))
         # the device form on the tail's buffers equals the host form
-        out = run_local_device(el, tails[f], dev(pts), len(pts), frame, th, stream)
+        out = run_local_device(el, tails[f], upload(pts), len(pts), frame, th, stream)
         dv, dm, dn = out.host(k.t.n_keep, len(pts))
         assert np.array_equal(dv.astype(bool), view) and np.array_equal(dm, match) and dn == n, f
         assert (out.match.cpu().numpy()[k.t.n_keep:] == -7).all()
@@ -163,10 +158,10 @@ def test_local_search_with_keys_blocked_on_entry(keysets, tails, ext):
     ov, om, on = T.search_local_points(k.kps, k.desc, k.ur, pts, of, el.GetScaleFactors(), 1, 0.8, blocked)
     assert np.array_equal(view, ov) and np.array_equal(match, om) and n == on > 0 and (match[blocked == 1] == -1).all()
     stream = torch.cuda.Stream()
-    b = torch.zeros(k.t.dkl.cap, dtype=torch.uint8, device="cuda")
+    b = torch.zeros(k.t.f.left.cap, dtype=torch.uint8, device="cuda")
     b[:len(blocked)] = torch.from_numpy(blocked).cuda()
     torch.cuda.synchronize()
-    out = run_local_device(el, tails[0], dev(pts), len(pts), frame, 1, stream, blocked=ptr(b))
+    out = run_local_device(el, tails[0], upload(pts), len(pts), frame, 1, stream, blocked=ptr(b))
     dv, dm, dn = out.host(k.t.n_keep, len(pts))
     assert np.array_equal(dm, match) and dn == n
 
@@ -185,7 +180,7 @@ def test_last_frame_search_is_bit_identical_to_the_oracle(keysets, tails, ext, p
         assert np.array_equal(match, om) and n == on, (f, pose)
         if pose in ("identity", "moved"):
             assert n > 50
-        out = run_last_device(el, tails[f], dev(pts), len(pts), frame, th, stream)
+        out = run_last_device(el, tails[f], upload(pts), len(pts), frame, th, stream)
         _, dm, dn = out.host(k.t.n_keep, len(pts))
         assert np.array_equal(dm, match) and dn == n, f
 
@@ -197,7 +192,7 @@ def test_edge_cases_and_error_codes(keysets, tails, ext):
     k = keysets[1]
     frame, of = frames("moved")
     pts = build_points(k, el.GetScaleFactors(), 9)
-    pd = dev(pts)
+    pd = upload(pts)
     stream = torch.cuda.Stream()
     full = run_local_device(el, t, pd, len(pts), frame, 1, stream).host(t.n_keep, len(pts))
 
@@ -225,15 +220,15 @@ def test_edge_cases_and_error_codes(keysets, tails, ext):
     out = run_last_device(el, t, pd, len(pts), frame, 7, stream, null=("match",))
     assert int(out.n.cpu()[0]) == ln and (out.match.cpu().numpy() == -7).all()
     # a count above the capacity is clamped (keep_idx NULL: key j of the extractor, every one of the capacity's records)
-    cap = t.dkl.cap
+    cap = t.f.left.cap
     u = torch.full((cap,), -1.0, dtype=torch.float32, device="cuda")
     torch.cuda.synchronize()
     out = SearchOut(cap, len(pts))
-    search_local_points_device(el, ptr(t.dkl.kps), ptr(t.dkl.desc), 0, ptr(i64(cap + 1000)), ptr(u), 0, ptr(pd), len(pts), frame, 1, 0.8,
+    search_local_points_device(el, t.f.kps, t.f.desc, 0, ptr(i64(cap + 1000)), ptr(u), 0, ptr(pd), len(pts), frame, 1, 0.8,
                                ptr(out.view), ptr(out.match), ptr(out.n), stream.cuda_stream)
     stream.synchronize()
-    kall = t.dkl.kps.cpu().numpy().view(k.kps.dtype)[:cap]
-    dall = t.dkl.desc.cpu().numpy().reshape(-1, 32)[:cap]
+    kall = t.f.left.kps.cpu().numpy().view(k.kps.dtype)[:cap]
+    dall = t.f.left.desc.cpu().numpy().reshape(-1, 32)[:cap]
     hv, hm, hn = search_local_points(el, kall, dall, np.full(cap, -1, np.float32), pts, frame, 1)
     dv, dm, dn = out.host(cap, len(pts))
     assert np.array_equal(dm, hm) and dn == hn > 0
@@ -260,8 +255,8 @@ def test_edge_cases_and_error_codes(keysets, tails, ext):
     a = largs(pts)
     a[8] = None
     assert lib.sivo_search_last_frame(*a) == L.EINVAL
-    dargs = lambda: [el._h, ptr(t.dkl.kps), ptr(t.dkl.desc), ptr(t.sem.keep), ptr(t.sem.n), ptr(t.st.u), None, ptr(pd), len(pts),
-                     C.byref(frame), 1.0, 0.8, None, None, None, None]
+    dargs = lambda: [el._h, t.f.kps, t.f.desc, t.f.keep, t.f.n_keep, t.f.u_right, None, ptr(pd), len(pts), C.byref(frame), 1.0, 0.8, None,
+                     None, None, None]
     assert lib.sivo_search_local_points_device(*dargs()) == L.OK
     for i, v in ((0, None), (1, None), (2, None), (4, None), (5, None), (7, None), (8, -1), (9, None), (10, 0.0)):
         a = dargs()
@@ -277,8 +272,7 @@ def test_three_frames_in_flight_with_both_searches_equal_the_host_call_path(seg,
     el, er = ext
     frames_in = [synth(30 + i) for i in range(3)]
     frame, _ = frames("moved")
-    hw = H * W
-    d_in = [[torch.from_numpy(x).cuda() for x in f] for f in frames_in]
+    d_in = [[upload(x) for x in f] for f in frames_in]
     rng = np.random.default_rng(4)
     pts = np.zeros(3000, MAP_POINT_DTYPE)
     z = rng.uniform(3, 40, len(pts))
@@ -288,40 +282,25 @@ def test_three_frames_in_flight_with_both_searches_equal_the_host_call_path(seg,
     pts["desc"] = rng.integers(0, 256, (len(pts), 32))
     pts["octave"] = rng.integers(0, 8, len(pts))
     pts["observed"] = 1
-    pd = dev(pts)
-    bufs = []
-    for _ in frames_in:
-        b = {"cls": torch.empty(hw, dtype=torch.uint8, device="cuda"), "conf": torch.empty(hw, dtype=torch.float64, device="cuda"),
-             "ent": torch.empty(hw, dtype=torch.float64, device="cuda"), "kl": DeviceKeys(el), "kr": DeviceKeys(er)}
-        b["sem"], b["st"] = SemanticOut(b["kl"].cap), StereoOut(b["kl"].cap)
-        b["loc"], b["last"] = SearchOut(b["kl"].cap, len(pts)), SearchOut(b["kl"].cap, len(pts))
-        bufs.append(b)
+    pd = upload(pts)
+    bufs = [(DeviceFrame(el, er, H, W), SearchOut(el.capacity(), len(pts)), SearchOut(el.capacity(), len(pts))) for _ in frames_in]
     stream = torch.cuda.Stream()
     s = stream.cuda_stream
-    torch.cuda.synchronize()
 
     def chain():
-        for i, b in enumerate(bufs):
-            bgr, gl, gr = d_in[i]
+        for i, (f, loc, last) in enumerate(bufs):
             seg.set_frame(300 + i)
-            seg.run_device_maps(ptr(bgr), ptr(b["cls"]), ptr(b["conf"]), ptr(b["ent"]), 0, 0, s)
-            el.wait_for_stream(s)  # the previous frame's stereo and searches are done with the left extractor
-            er.wait_for_stream(s)
-            b["kl"].enqueue(el, gl)
-            b["kr"].enqueue(er, gr)
-            el.stream_wait(s)
-            b["sem"].run(seg, b["kl"], 8, s)
-            b["st"].run(el, er, b["kl"], b["kr"], MB, MBF, s, keep=b["sem"].keep, n_left=b["sem"].n)
-            kl = b["kl"]
-            search_last_frame_device(el, ptr(kl.kps), ptr(kl.desc), ptr(b["sem"].keep), ptr(b["sem"].n), ptr(b["st"].u), ptr(pd), len(pts),
-                                     frame, np.eye(3), np.zeros(3), 7, ptr(b["last"].match), ptr(b["last"].n), s)
-            search_local_points_device(el, ptr(kl.kps), ptr(kl.desc), ptr(b["sem"].keep), ptr(b["sem"].n), ptr(b["st"].u), 0, ptr(pd),
-                                       len(pts), frame, 1, 0.8, ptr(b["loc"].view), ptr(b["loc"].match), ptr(b["loc"].n), s)
+            f.extract(seg, *d_in[i], s)  # waits for the previous frame's stereo and searches
+            f.tail(seg, MB, MBF, s)
+            search_last_frame_device(el, f.kps, f.desc, f.keep, f.n_keep, f.u_right, ptr(pd), len(pts), frame, np.eye(3), np.zeros(3), 7,
+                                     ptr(last.match), ptr(last.n), s)
+            search_local_points_device(el, f.kps, f.desc, f.keep, f.n_keep, f.u_right, 0, ptr(pd), len(pts), frame, 1, 0.8, ptr(loc.view),
+                                       ptr(loc.match), ptr(loc.n), s)
 
     chain()  # first use of the stream: the network's graph is captured here
     stream.synchronize()
-    for b in bufs:
-        for o in (b["loc"], b["last"]):
+    for _, loc, last in bufs:
+        for o in (loc, last):
             o.match.fill_(-7)
             o.n.fill_(-7)
     torch.cuda.synchronize()
@@ -336,9 +315,10 @@ def test_three_frames_in_flight_with_both_searches_equal_the_host_call_path(seg,
         hu, _ = stereo_match(el, er, kl[keep], dl[keep], kr, dr, MB, MBF)
         hv, hm, hn = search_local_points(el, kl[keep], dl[keep], hu, pts, frame, 1)
         lm, ln = search_last_frame(el, kl[keep], dl[keep], hu, pts, frame, np.eye(3), np.zeros(3), 7)
-        n_keep = bufs[i]["sem"].host()[0]
-        v, m, n = bufs[i]["loc"].host(n_keep, len(pts))
+        f, loc, last = bufs[i]
+        n_keep = f.host()[0]
+        v, m, n = loc.host(n_keep, len(pts))
         assert n_keep == len(keep) and np.array_equal(v.astype(bool), hv) and np.array_equal(m, hm) and n == hn
-        _, m, n = bufs[i]["last"].host(n_keep, len(pts))
+        _, m, n = last.host(n_keep, len(pts))
         assert np.array_equal(m, lm) and n == ln
         assert hv.sum() > 100

@@ -4,16 +4,9 @@ import cv2
 import numpy as np
 
 from oracle import info_oracle as I
+from oracle.mapping_scene import rotation
 
 KITTI_FX, KITTI_CX, KITTI_CY, KITTI_MBF = 718.856, 607.1928, 185.2157, 386.1448
-
-
-def rotation(ax, ay, az):
-    cx, sx, cy, sy, cz, sz = np.cos(ax), np.sin(ax), np.cos(ay), np.sin(ay), np.cos(az), np.sin(az)
-    Rx = np.array([[1, 0, 0], [0, cx, -sx], [0, sx, cx]])
-    Ry = np.array([[cy, 0, sy], [0, 1, 0], [-sy, 0, cy]])
-    Rz = np.array([[cz, -sz, 0], [sz, cz, 0], [0, 0, 1]])
-    return Rz @ Ry @ Rx
 
 
 def random_spd(rng, n, scale=1.0):

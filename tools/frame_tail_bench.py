@@ -36,7 +36,8 @@ def run(args):
     import gc
 
     import torch
-    from sivo_b200 import KP_DTYPE, BayesianSegNet, BayesianSegNetParams, ORBextractor, stereo_match, stereo_match_device
+    from sivo_b200 import BayesianSegNet, BayesianSegNetParams, ORBextractor, stereo_match
+    from sivo_b200.frame import DeviceFrame
     if not torch.cuda.is_available():
         raise SystemExit("frame_tail_bench.py needs a CUDA device (there is no CPU fallback for the product path)")
     dev = torch.device("cuda", 0)
@@ -48,19 +49,9 @@ def run(args):
         raise SystemExit("frame_tail_bench.py needs the extractors' asynchronous (device quad tree) form")
     n_frames, NBUF = 8, 3
     fr = frames(n_frames)
-    hw = NET_H * NET_W
     d_bgr = [torch.from_numpy(np.ascontiguousarray(f[0][CROP_Y:CROP_Y + NET_H, CROP_X:CROP_X + NET_W])).to(dev) for f in fr]
     d_gray = [[torch.from_numpy(f[1]).to(dev), torch.from_numpy(f[2]).to(dev)] for f in fr]
-    cap = el.capacity()
-    u8, i32, i64, f32, f64 = torch.uint8, torch.int32, torch.int64, torch.float32, torch.float64
-    d_cls, d_conf, d_ent = (torch.empty(hw, dtype=t, device=dev) for t in (u8, f64, f64))
-    kp = [[torch.zeros(cap * 28, dtype=u8, device=dev) for _ in range(2)] for _ in range(NBUF)]
-    desc = [[torch.zeros(cap * 32, dtype=u8, device=dev) for _ in range(2)] for _ in range(NBUF)]
-    cnt = [torch.zeros(2, dtype=i64, device=dev) for _ in range(NBUF)]
-    keep = [torch.empty(cap, dtype=i32, device=dev) for _ in range(NBUF)]
-    n_keep = [torch.empty(1, dtype=i64, device=dev) for _ in range(NBUF)]
-    u_r = [torch.empty(cap, dtype=f32, device=dev) for _ in range(NBUF)]
-    z_r = [torch.empty(cap, dtype=f32, device=dev) for _ in range(NBUF)]
+    F = [DeviceFrame(el, er, NET_H, NET_W) for _ in range(NBUF)]
     stream = torch.cuda.Stream(dev)  # a real stream: the library's NULL would mean its own
     s = stream.cuda_stream
     ev = [torch.cuda.Event() for _ in range(NBUF)]
@@ -69,32 +60,16 @@ def run(args):
     def step(i, tail):
         """The device step (SegNet, both extractors joined on the main stream), optionally followed by the device tail."""
         j, k = i % n_frames, i % NBUF
-        seg.run_device_maps(d_bgr[j].data_ptr(), d_cls.data_ptr(), d_conf.data_ptr(), d_ent.data_ptr(), 0, 0, s)
-        for o, side in ((el, 0), (er, 1)):
-            o.enqueue_device(d_gray[j][side].data_ptr(), NET_H, NET_W, NET_W, kp[k][side].data_ptr(), desc[k][side].data_ptr(),
-                             cnt[k][side:].data_ptr())
+        F[k].extract(seg, d_bgr[j], *d_gray[j], s)  # the extractors first wait for the previous step's tail
         if tail:
-            device_tail(k)
+            F[k].tail(seg, MB, MBF, s)
         else:
-            el.stream_wait(s)
             er.stream_wait(s)
         ev[k].record(stream)
 
-    def device_tail(k):
-        el.stream_wait(s)  # the semantic lookup reads the left keypoints; stereo orders itself after both extractors
-        seg.semantic_keys_device(kp[k][0].data_ptr(), cnt[k][0:].data_ptr(), cap, 8, 0, 0, 0, keep[k].data_ptr(), n_keep[k].data_ptr(), s)
-        stereo_match_device(el, er, kp[k][0].data_ptr(), desc[k][0].data_ptr(), keep[k].data_ptr(), n_keep[k].data_ptr(),
-                            kp[k][1].data_ptr(), desc[k][1].data_ptr(), cnt[k][1:].data_ptr(), MB, MBF, u_r[k].data_ptr(),
-                            z_r[k].data_ptr(), s)
-        el.wait_for_stream(s)  # the next enqueue_device overwrites the pyramids the tail reads
-        er.wait_for_stream(s)
-
     def host_tail(k):
-        n = cnt[k].cpu().numpy()
-        kl = kp[k][0][:n[0] * 28].cpu().numpy().view(KP_DTYPE)
-        kr = kp[k][1][:n[1] * 28].cpu().numpy().view(KP_DTYPE)
-        dl = desc[k][0][:n[0] * 32].cpu().numpy().reshape(-1, 32)
-        dr = desc[k][1][:n[1] * 32].cpu().numpy().reshape(-1, 32)
+        kl, dl = F[k].left.host()
+        kr, dr = F[k].right.host()
         sel = seg.semantic_keys(kl, 8)[3]
         return stereo_match(el, er, kl[sel], dl[sel], kr, dr, MB, MBF)
 
@@ -117,13 +92,12 @@ def run(args):
             if name == "host":
                 res[name] = host_tail(k)
             else:
-                device_tail(k)
+                F[k].tail(seg, MB, MBF, s)
                 stream.synchronize()
             if i >= args.warmup:
                 times[name].append(1e3 * (time.perf_counter() - t0))
-        m = int(n_keep[k].cpu()[0])
-        mismatches += int(u_r[k][:m].cpu().numpy().tobytes() != res["host"][0].tobytes() or
-                          z_r[k][:m].cpu().numpy().tobytes() != res["host"][1].tobytes())
+        _, _, u, z = F[k].host()
+        mismatches += int(u.tobytes() != res["host"][0].tobytes() or z.tobytes() != res["host"][1].tobytes())
     gc.enable()
 
     # (c): device-step throughput without / with the tail, alternating blocks; bounded run-ahead as in bench.py's device_step

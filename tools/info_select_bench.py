@@ -36,8 +36,8 @@ def run(args):
 
     import cv2
     import torch
-    from sivo_b200 import (KP_DTYPE, BayesianSegNet, BayesianSegNetParams, ORBextractor, info_select, info_select_device, make_camera,
-                           stereo_match_device)
+    from sivo_b200 import BayesianSegNet, BayesianSegNetParams, ORBextractor, info_select, info_select_device, make_camera
+    from sivo_b200.frame import DeviceFrame
     from sivo_b200.synth import bgr_to_gray
     if not torch.cuda.is_available():
         raise SystemExit("info_select_bench.py needs a CUDA device (there is no CPU fallback for the product path)")
@@ -48,43 +48,28 @@ def run(args):
     el, er = (ORBextractor(args.nfeatures, 1.2, 8, 20, 7) for _ in range(2))
     cam = make_camera(FX, FX, CX, CY, MB, np.eye(3), np.zeros(3), 1e-6 * np.eye(6))
     cap = el.capacity()
-    u8, i32, i64, f32, f64 = torch.uint8, torch.int32, torch.int64, torch.float32, torch.float64
     NBUF = 3
-    hw = NET_H * NET_W
-    d_cls, d_conf, d_ent = (torch.empty(hw, dtype=t, device=dev) for t in (u8, f64, f64))
-    kp = [[torch.zeros(cap * 28, dtype=u8, device=dev) for _ in range(2)] for _ in range(NBUF)]
-    desc = [[torch.zeros(cap * 32, dtype=u8, device=dev) for _ in range(2)] for _ in range(NBUF)]
-    cnt = [torch.zeros(2, dtype=i64, device=dev) for _ in range(NBUF)]
-    kp_ent = [torch.empty(cap, dtype=f64, device=dev) for _ in range(NBUF)]
-    keep = [torch.empty(cap, dtype=i32, device=dev) for _ in range(NBUF)]
-    n_keep = [torch.empty(1, dtype=i64, device=dev) for _ in range(NBUF)]
-    u_r, z_r, world = ([torch.empty(cap * m, dtype=f32, device=dev) for _ in range(NBUF)] for m in (1, 1, 3))
-    red = [torch.empty(cap, dtype=f64, device=dev) for _ in range(NBUF)]
-    sel = [torch.empty(cap, dtype=i32, device=dev) for _ in range(NBUF)]
-    n_sel = [torch.empty(1, dtype=i64, device=dev) for _ in range(NBUF)]
+    F = [DeviceFrame(el, er, NET_H, NET_W) for _ in range(NBUF)]
+    world = [torch.empty(cap * 3, dtype=torch.float32, device=dev) for _ in range(NBUF)]
+    red = [torch.empty(cap, dtype=torch.float64, device=dev) for _ in range(NBUF)]
+    sel = [torch.empty(cap, dtype=torch.int32, device=dev) for _ in range(NBUF)]
+    n_sel = [torch.empty(1, dtype=torch.int64, device=dev) for _ in range(NBUF)]
     stream = torch.cuda.Stream(dev)
     s = stream.cuda_stream
     ev = [torch.cuda.Event() for _ in range(NBUF)]
     torch.cuda.synchronize(dev)
 
     def select(k):
-        info_select_device(el, kp[k][0].data_ptr(), kp_ent[k].data_ptr(), keep[k].data_ptr(), n_keep[k].data_ptr(), z_r[k].data_ptr(), cam,
-                           THRESHOLD, world[k].data_ptr(), red[k].data_ptr(), sel[k].data_ptr(), n_sel[k].data_ptr(), s)
+        f = F[k]
+        info_select_device(el, f.kps, f.kp_entropy, f.keep, f.n_keep, f.depth, cam, THRESHOLD, world[k].data_ptr(), red[k].data_ptr(),
+                           sel[k].data_ptr(), n_sel[k].data_ptr(), s)
 
     def step(bgr, gl, gr, k, with_select):
         """SegNet, both extractors, semantic keys and stereo on the main stream, optionally followed by the selection."""
-        seg.run_device_maps(bgr.data_ptr(), d_cls.data_ptr(), d_conf.data_ptr(), d_ent.data_ptr(), 0, 0, s)
-        for o, g, side in ((el, gl, 0), (er, gr, 1)):
-            o.enqueue_device(g.data_ptr(), NET_H, NET_W, NET_W, kp[k][side].data_ptr(), desc[k][side].data_ptr(), cnt[k][side:].data_ptr())
-        el.stream_wait(s)
-        seg.semantic_keys_device(kp[k][0].data_ptr(), cnt[k][0:].data_ptr(), cap, 8, 0, 0, kp_ent[k].data_ptr(), keep[k].data_ptr(),
-                                 n_keep[k].data_ptr(), s)
-        stereo_match_device(el, er, kp[k][0].data_ptr(), desc[k][0].data_ptr(), keep[k].data_ptr(), n_keep[k].data_ptr(), kp[k][1].data_ptr(),
-                            desc[k][1].data_ptr(), cnt[k][1:].data_ptr(), MB, MBF, u_r[k].data_ptr(), z_r[k].data_ptr(), s)
+        F[k].extract(seg, bgr, gl, gr, s)  # the extractors first wait for the previous step's tail and selection
+        F[k].tail(seg, MB, MBF, s)
         if with_select:
             select(k)
-        el.wait_for_stream(s)  # the next enqueue_device overwrites what the tail reads
-        er.wait_for_stream(s)
         ev[k].record(stream)
 
     # (a) / (b) on the KITTI crop
@@ -96,9 +81,9 @@ def run(args):
     for _ in range(2):  # the first run captures the network's graph
         step(*kitti, 0, True)
     stream.synchronize()
-    m = int(n_keep[0].cpu()[0])
-    kps = kp[0][0].cpu().numpy().view(KP_DTYPE)[keep[0][:m].cpu().numpy()]
-    h_ent, h_z = kp_ent[0].cpu().numpy()[keep[0][:m].cpu().numpy()], z_r[0][:m].cpu().numpy()
+    m, kidx, _, h_z = F[0].host()
+    kps = F[0].left.host()[0][kidx]
+    h_ent = F[0].out["kp_entropy"].cpu().numpy()[kidx]
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     dev_ms, host_ms = [], []
     gc.collect()

@@ -31,16 +31,11 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 from bench import CROP_X, CROP_Y, NET_H, NET_W, frames, model_cache_dir, model_files  # noqa: E402
+from oracle.mapping_scene import rotation  # noqa: E402
 
 FX, CX, CY, MBF = 718.856, 607.1928 - CROP_X, 185.2157 - CROP_Y, 386.1448  # KITTI00-02.yaml, principal point in the crop
 MB = MBF / FX
 EDGES = (100, 500, 1000, 2000)
-
-
-def rotation(ax, ay, az):
-    cx, sx, cy, sy, cz, sz = np.cos(ax), np.sin(ax), np.cos(ay), np.sin(ay), np.cos(az), np.sin(az)
-    return (np.array([[cz, -sz, 0], [sz, cz, 0], [0, 0, 1]]) @ np.array([[cy, 0, sy], [0, 1, 0], [-sy, 0, cy]])
-            @ np.array([[1, 0, 0], [0, cx, -sx], [0, sx, cx]]))
 
 
 def synthetic_scene(n, outliers, rng):
@@ -74,7 +69,8 @@ def frame_map(kps, desc, depth, scale, rng):
 def run(args):
     import torch
     from sivo_b200 import (BayesianSegNet, BayesianSegNetParams, KP_DTYPE, ORBextractor, make_frame, pose_gather_device, pose_optimize,
-                           pose_optimize_device, search_last_frame_device, search_local_points_device, stereo_match_device)
+                           pose_optimize_device, search_last_frame_device, search_local_points_device)
+    from sivo_b200.frame import DeviceFrame
     from sivo_b200.pose import frame_from_result, result_from_bytes
     if not torch.cuda.is_available():
         raise SystemExit("pose_bench.py needs a CUDA device (there is no CPU fallback for the product path)")
@@ -138,17 +134,11 @@ def run(args):
     frame0 = make_frame(FX, FX, CX, CY, MBF, bounds, rotation(0.001, -0.0015, 0.001), (0.01, -0.005, 0.01))
     T0 = np.concatenate([np.array(frame0.Rcw, np.float32).reshape(3, 3), np.array(frame0.tcw, np.float32)[:, None]], 1)
     fr = frames(6)
-    hw = NET_H * NET_W
-    d_cls, d_conf, d_ent = (torch.empty(hw, dtype=t, device=dev) for t in (u8, f64, f64))
     B = []
     for f in fr:
         B.append({"in": [torch.from_numpy(np.ascontiguousarray(f[0][CROP_Y:CROP_Y + NET_H, CROP_X:CROP_X + NET_W])).to(dev), torch.from_numpy(f[1]).to(dev),
                          torch.from_numpy(f[2]).to(dev)],
-                  "kp": [torch.zeros(cap * 28, dtype=u8, device=dev) for _ in range(2)],
-                  "desc": [torch.zeros(cap * 32, dtype=u8, device=dev) for _ in range(2)], "cnt": torch.zeros(2, dtype=i64, device=dev),
-                  "ent": torch.empty(cap, dtype=f64, device=dev), "keep": torch.empty(cap, dtype=i32, device=dev),
-                  "n": torch.empty(1, dtype=i64, device=dev), "u": torch.empty(cap, dtype=f32, device=dev),
-                  "z": torch.empty(cap, dtype=f32, device=dev), "m1": torch.empty(cap, dtype=i32, device=dev),
+                  "f": DeviceFrame(el, er, NET_H, NET_W), "m1": torch.empty(cap, dtype=i32, device=dev),
                   "m2": torch.empty(cap, dtype=i32, device=dev), "nm": torch.empty(2, dtype=i64, device=dev),
                   "view": torch.empty(cap, dtype=u8, device=dev), "xw": torch.empty(3 * cap, dtype=f32, device=dev),
                   "T0": torch.from_numpy(T0.reshape(-1).copy()).to(dev), "r1": torch.empty(512, dtype=u8, device=dev),
@@ -157,28 +147,23 @@ def run(args):
     torch.cuda.synchronize(dev)
 
     def front(b):
-        bgr, gl, gr = b["in"]
-        seg.run_device_maps(bgr.data_ptr(), d_cls.data_ptr(), d_conf.data_ptr(), d_ent.data_ptr(), 0, 0, s)
-        for o, g, side in ((el, gl, 0), (er, gr, 1)):
-            o.enqueue_device(g.data_ptr(), NET_H, NET_W, NET_W, b["kp"][side].data_ptr(), b["desc"][side].data_ptr(), b["cnt"][side:].data_ptr())
-        el.stream_wait(s)
-        seg.semantic_keys_device(b["kp"][0].data_ptr(), b["cnt"][0:].data_ptr(), cap, 8, 0, 0, b["ent"].data_ptr(), b["keep"].data_ptr(),
-                                 b["n"].data_ptr(), s)
-        stereo_match_device(el, er, b["kp"][0].data_ptr(), b["desc"][0].data_ptr(), b["keep"].data_ptr(), b["n"].data_ptr(),
-                            b["kp"][1].data_ptr(), b["desc"][1].data_ptr(), b["cnt"][1:].data_ptr(), MB, MBF, b["u"].data_ptr(), b["z"].data_ptr(), s)
+        b["f"].extract(seg, *b["in"], s)  # the extractors first wait for the previous step's searches and optimisations
+        b["f"].tail(seg, MB, MBF, s)
 
     def last_search(b):
-        search_last_frame_device(el, b["kp"][0].data_ptr(), b["desc"][0].data_ptr(), b["keep"].data_ptr(), b["n"].data_ptr(), b["u"].data_ptr(),
-                                 b["last"].data_ptr(), b["n_last"], frame0, T0[:, :3], T0[:, 3], 7.0, b["m1"].data_ptr(), b["nm"][1:].data_ptr(), s)
+        f = b["f"]
+        search_last_frame_device(el, f.kps, f.desc, f.keep, f.n_keep, f.u_right, b["last"].data_ptr(), b["n_last"], frame0, T0[:, :3], T0[:, 3],
+                                 7.0, b["m1"].data_ptr(), b["nm"][1:].data_ptr(), s)
 
     def local_search(b, frame):
-        search_local_points_device(el, b["kp"][0].data_ptr(), b["desc"][0].data_ptr(), b["keep"].data_ptr(), b["n"].data_ptr(),
-                                   b["u"].data_ptr(), 0, b["local"].data_ptr(), b["n_local"], frame, 1.0, 0.8, b["view"].data_ptr(),
-                                   b["m2"].data_ptr(), b["nm"].data_ptr(), s)
+        f = b["f"]
+        search_local_points_device(el, f.kps, f.desc, f.keep, f.n_keep, f.u_right, 0, b["local"].data_ptr(), b["n_local"], frame, 1.0, 0.8,
+                                   b["view"].data_ptr(), b["m2"].data_ptr(), b["nm"].data_ptr(), s)
 
     def pose(b, t_in, res):
-        pose_optimize_device(el, b["kp"][0].data_ptr(), b["keep"].data_ptr(), b["n"].data_ptr(), b["u"].data_ptr(), b["xw"].data_ptr(),
-                             FX, FX, CX, CY, MBF, t_in.data_ptr(), res.data_ptr(), b["o"].data_ptr(), s)
+        f = b["f"]
+        pose_optimize_device(el, f.kps, f.keep, f.n_keep, f.u_right, b["xw"].data_ptr(), FX, FX, CX, CY, MBF, t_in.data_ptr(), res.data_ptr(),
+                             b["o"].data_ptr(), s)
 
     def step(b, with_pose):
         front(b)
@@ -186,29 +171,25 @@ def run(args):
         if with_pose:
             with torch.cuda.stream(stream):
                 b["xw"].fill_(float("nan"))
-            pose_gather_device(el, b["m1"].data_ptr(), b["n"].data_ptr(), b["last"].data_ptr(), b["n_last"], b["xw"].data_ptr(), s)
+            pose_gather_device(el, b["m1"].data_ptr(), b["f"].n_keep, b["last"].data_ptr(), b["n_last"], b["xw"].data_ptr(), s)
             pose(b, b["T0"], b["r1"])
             with torch.cuda.stream(stream):
                 b["r1_host"].copy_(b["r1"], non_blocking=True)
             stream.synchronize()  # Tracking's host read: the local-map search takes the pose as a host struct
             frame = frame_from_result(result_from_bytes(b["r1_host"].numpy()), FX, FX, CX, CY, MBF, bounds)
             local_search(b, frame)
-            pose_gather_device(el, b["m2"].data_ptr(), b["n"].data_ptr(), b["local"].data_ptr(), b["n_local"], b["xw"].data_ptr(), s)
+            pose_gather_device(el, b["m2"].data_ptr(), b["f"].n_keep, b["local"].data_ptr(), b["n_local"], b["xw"].data_ptr(), s)
             pose(b, b["r1"], b["r2"])
         else:
             local_search(b, frame0)
-        el.wait_for_stream(s)  # the next enqueue_device overwrites what the tail, the searches and the optimisations read
-        er.wait_for_stream(s)
         b["ev"].record(stream)
 
     for b in B:  # first pass: the network's graph is captured, and each frame's keys give its map
         front(b)
         stream.synchronize()
-        m = int(b["n"].cpu()[0])
-        kidx = b["keep"][:m].cpu().numpy()
-        kps = b["kp"][0].cpu().numpy().view(KP_DTYPE)[kidx]
-        desc = b["desc"][0].cpu().numpy().reshape(-1, 32)[kidx]
-        last, local = frame_map(kps, desc, b["z"][:m].cpu().numpy(), el.GetScaleFactors(), rng)
+        _, kidx, _, depth = b["f"].host()
+        kps, desc = (a[kidx] for a in b["f"].left.host())
+        last, local = frame_map(kps, desc, depth, el.GetScaleFactors(), rng)
         b["last"], b["local"] = (torch.from_numpy(p.view(np.uint8).reshape(-1).copy()).to(dev) for p in (last, local))
         b["n_last"], b["n_local"] = len(last), len(local)
     torch.cuda.synchronize(dev)

@@ -57,8 +57,9 @@ def run(args):
 
     import cv2
     import torch
-    from sivo_b200 import (BayesianSegNet, BayesianSegNetParams, KP_DTYPE, ORBextractor, make_frame, search_last_frame,
-                           search_last_frame_device, search_local_points, search_local_points_device, stereo_match_device)
+    from sivo_b200 import (BayesianSegNet, BayesianSegNetParams, ORBextractor, make_frame, search_last_frame, search_last_frame_device,
+                           search_local_points, search_local_points_device)
+    from sivo_b200.frame import DeviceFrame
     from sivo_b200.synth import bgr_to_gray
     if not torch.cuda.is_available():
         raise SystemExit("track_search_bench.py needs a CUDA device (there is no CPU fallback for the product path)")
@@ -70,47 +71,30 @@ def run(args):
     c, s_ = np.cos(0.01), np.sin(0.01)
     frame = make_frame(FX, FX, CX, CY, MBF, (0.0, float(NET_W), 0.0, float(NET_H)), [[c, 0, s_], [0, 1, 0], [-s_, 0, c]], (0.02, -0.01, 0.3))
     cap = el.capacity()
-    u8, i32, i64, f32, f64 = torch.uint8, torch.int32, torch.int64, torch.float32, torch.float64
     NBUF = 3
-    hw = NET_H * NET_W
-    d_cls, d_conf, d_ent = (torch.empty(hw, dtype=t, device=dev) for t in (u8, f64, f64))
-    kp = [[torch.zeros(cap * 28, dtype=u8, device=dev) for _ in range(2)] for _ in range(NBUF)]
-    desc = [[torch.zeros(cap * 32, dtype=u8, device=dev) for _ in range(2)] for _ in range(NBUF)]
-    cnt = [torch.zeros(2, dtype=i64, device=dev) for _ in range(NBUF)]
-    kp_ent = [torch.empty(cap, dtype=f64, device=dev) for _ in range(NBUF)]
-    keep = [torch.empty(cap, dtype=i32, device=dev) for _ in range(NBUF)]
-    n_keep = [torch.empty(1, dtype=i64, device=dev) for _ in range(NBUF)]
-    u_r, z_r = ([torch.empty(cap, dtype=f32, device=dev) for _ in range(NBUF)] for _ in range(2))
-    match = [torch.empty(cap, dtype=i32, device=dev) for _ in range(NBUF)]
-    n_m = [torch.empty(2, dtype=i64, device=dev) for _ in range(NBUF)]
-    in_view = torch.empty(max(COUNTS), dtype=u8, device=dev)
+    F = [DeviceFrame(el, er, NET_H, NET_W) for _ in range(NBUF)]
+    match = [torch.empty(cap, dtype=torch.int32, device=dev) for _ in range(NBUF)]
+    n_m = [torch.empty(2, dtype=torch.int64, device=dev) for _ in range(NBUF)]
+    in_view = torch.empty(max(COUNTS), dtype=torch.uint8, device=dev)
     stream = torch.cuda.Stream(dev)
     s = stream.cuda_stream
     ev = [torch.cuda.Event() for _ in range(NBUF)]
     torch.cuda.synchronize(dev)
 
     def searches(k, pts_dev, n_points, local=True, last=True):
+        f = F[k]
         if last:
-            search_last_frame_device(el, kp[k][0].data_ptr(), desc[k][0].data_ptr(), keep[k].data_ptr(), n_keep[k].data_ptr(), u_r[k].data_ptr(),
-                                     pts_dev.data_ptr(), n_points, frame, np.eye(3), np.zeros(3), 7.0, match[k].data_ptr(), n_m[k][1:].data_ptr(), s)
+            search_last_frame_device(el, f.kps, f.desc, f.keep, f.n_keep, f.u_right, pts_dev.data_ptr(), n_points, frame, np.eye(3), np.zeros(3),
+                                     7.0, match[k].data_ptr(), n_m[k][1:].data_ptr(), s)
         if local:
-            search_local_points_device(el, kp[k][0].data_ptr(), desc[k][0].data_ptr(), keep[k].data_ptr(), n_keep[k].data_ptr(),
-                                       u_r[k].data_ptr(), 0, pts_dev.data_ptr(), n_points, frame, 1.0, 0.8, in_view.data_ptr(),
-                                       match[k].data_ptr(), n_m[k].data_ptr(), s)
+            search_local_points_device(el, f.kps, f.desc, f.keep, f.n_keep, f.u_right, 0, pts_dev.data_ptr(), n_points, frame, 1.0, 0.8,
+                                       in_view.data_ptr(), match[k].data_ptr(), n_m[k].data_ptr(), s)
 
     def step(bgr, gl, gr, k, pts_dev=None):
-        seg.run_device_maps(bgr.data_ptr(), d_cls.data_ptr(), d_conf.data_ptr(), d_ent.data_ptr(), 0, 0, s)
-        for o, g, side in ((el, gl, 0), (er, gr, 1)):
-            o.enqueue_device(g.data_ptr(), NET_H, NET_W, NET_W, kp[k][side].data_ptr(), desc[k][side].data_ptr(), cnt[k][side:].data_ptr())
-        el.stream_wait(s)
-        seg.semantic_keys_device(kp[k][0].data_ptr(), cnt[k][0:].data_ptr(), cap, 8, 0, 0, kp_ent[k].data_ptr(), keep[k].data_ptr(),
-                                 n_keep[k].data_ptr(), s)
-        stereo_match_device(el, er, kp[k][0].data_ptr(), desc[k][0].data_ptr(), keep[k].data_ptr(), n_keep[k].data_ptr(), kp[k][1].data_ptr(),
-                            desc[k][1].data_ptr(), cnt[k][1:].data_ptr(), MB, MBF, u_r[k].data_ptr(), z_r[k].data_ptr(), s)
+        F[k].extract(seg, bgr, gl, gr, s)  # the extractors first wait for the previous step's tail and searches
+        F[k].tail(seg, MB, MBF, s)
         if pts_dev is not None:
             searches(k, pts_dev, pts_dev.numel() // 80)
-        el.wait_for_stream(s)  # the next enqueue_device overwrites what the tail and the searches read
-        er.wait_for_stream(s)
         ev[k].record(stream)
 
     # (a) / (b) on the KITTI crop
@@ -122,11 +106,8 @@ def run(args):
     for _ in range(2):  # the first run captures the network's graph
         step(*kitti, 0)
     stream.synchronize()
-    m = int(n_keep[0].cpu()[0])
-    kidx = keep[0][:m].cpu().numpy()
-    h_kps = kp[0][0].cpu().numpy().view(KP_DTYPE)[kidx]
-    h_desc = desc[0][0].cpu().numpy().reshape(-1, 32)[kidx]
-    h_ur, h_z = u_r[0][:m].cpu().numpy(), z_r[0][:m].cpu().numpy()
+    m, kidx, h_ur, h_z = F[0].host()
+    h_kps, h_desc = (a[kidx] for a in F[0].left.host())
     rng = np.random.default_rng(0)
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     med = lambda v: float(np.median(v))
