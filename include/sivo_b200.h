@@ -613,6 +613,68 @@ int sivo_dbg_create_map_points(const sivo_orb_t* left, const sivo_keyframe_keys*
                                int n_neighbours, const sivo_mapping_params* params, int* match, int* stage, double* reduction,
                                int* created_nb, int* created_idx, float* world, int* created_list, long long* n_created);
 
+/* ---- a keyframe's map points fused with its neighbours': ORBmatcher::Fuse(pKF, vpMapPoints, th) (ORBmatcher.cc:787-930) as
+ * LocalMapping::SearchInNeighbors (LocalMapping.cc:547-637) runs it, over every target keyframe at once ------------------------
+ * Every operation is the IEEE float / double operation as written (no contracted multiply-add).  oracle/fuse_oracle.py restates
+ * the rule and lists the reference facts kept; per (target k, point i):
+ *   Pc        the projection searches' gemm form with target k's pose; out (DEPTH) if Pc_z < 0.0f (z = +-0 carries on).
+ *   image     invz = 1 / Pc_z, x = Pc_x invz, u = fx x + cx (v likewise), all float; out (IMAGE) unless KeyFrame::IsInImage:
+ *             min_x <= u < max_x && min_y <= v < max_y (strict upper bounds, unlike Frame::isInFrustum; a NaN is out).
+ *             ur = u - mbf invz.
+ *   distance  PO = pos - Ow in float, dist3D as the projection searches' cv::norm; out (DISTANCE) if dist3D < 0.8f min_distance
+ *             || dist3D > 1.2f max_distance.
+ *   angle     out (ANGLE) if PO . normal (Mat::dot, double, as the projection searches) < 0.5 * dist3D in double.  A NaN dot
+ *             passes, as in the reference.
+ *   level     PredictScale(dist3D) with the projection searches' rule; a NaN quotient searches nothing (NO_CANDIDATE).  radius =
+ *             th scale[level] in float.
+ *   window    KeyFrame::GetFeaturesInArea(u, v, radius): the projection searches' grid and walk, no level filter.  An empty
+ *             window ends at NO_CANDIDATE.
+ *   keys      a key in the window is a candidate iff level - 1 <= octave <= level, 0 <= octave < nlevels (the reference would
+ *             read mvInvLevelSigma2[-1] for sivo_keyframe_gather_device's octave -1 at level 0), and e2 invSigma2[octave] in
+ *             float, compared in double, is not above 7.8 for a stereo key (u_right >= 0; e2 = (ex^2 + ey^2) + er^2) or 5.99 for
+ *             a mono one (a NaN u_right is mono; e2 = ex^2 + ey^2), with ex = u - x, ey = v - y, er = ur - u_right.
+ *   best      the first strictly smaller Hamming distance in walk order, from 256; MATCHED iff it is <= TH_LOW (50), else
+ *             ABOVE_TH_LOW.
+ *   angles    key angles follow the projection searches' angle rule: a key with another angle is in no cell (the host form
+ *             returns SIVO_ERANGE).  Extractor keys satisfy it.
+ * Fuse claims no key: a pair's decision reads only the point's position, normal, distances and descriptor and the target's keys
+ * and pose, so one warp decides each pair independently.  Replay contract: during SearchInNeighbors only a point's descriptor
+ * can change (MapPoint::Replace ends with ComputeDistinctiveDescriptors on the survivor; UpdateNormalAndDepth runs after both
+ * phases).  A caller that walks the pairs in the reference's order (phase 1: target-major, the current keyframe's points in
+ * key order; phase 2: the current keyframe against the deduplicated candidates) and
+ *   1. skips a point that is bad now or already in target k now,
+ *   2. applies match[k n_points + i] to any other point (the reference's Replace / AddObservation / AddMapPoint), and
+ *   3. searches again any point whose descriptor now differs from the one it was searched with (only the survivor of a Replace
+ *      in an earlier target, so never in phase 2), applying that result instead,
+ * reproduces the sequential loop exactly. */
+typedef struct sivo_fuse_camera {          /* the keyframes' shared members */
+  float fx, fy, cx, cy, mbf;
+  float min_x, max_x, min_y, max_y;        /* mnMinX, mnMaxX, mnMinY, mnMaxY */
+} sivo_fuse_camera;
+/* Fuse of points_device[0 .. n_points) into targets[0 .. n_targets) on device buffers.  Target k: its kps / desc / u_right /
+ * count (device, sivo_orb_capacity(left) keys, as sivo_keyframe_gather_device writes them) and its pose (Rcw, tcw, Ow); the
+ * other pointers may be NULL.  A point reads only desc, pos, normal, min_distance and max_distance.  Outputs, row k at k n_points:
+ * match_device[k n_points + i] = the key point i fuses with in target k, or -1; dist_device[...] (may be NULL) = the best
+ * distance (256 when no key passed).  Counts are clamped to the capacity; a target with a negative count gets -1 (and 256) in
+ * its whole row.  Targets go 64 to a launch.  Runs on `stream` (NULL = the left extractor's stream) with no waits of its own and
+ * no host synchronisation.  SIVO_EINVAL for NULL handles or inputs, n_targets < 0, n_points < 0, n_targets n_points > INT_MAX,
+ * th <= 0 or not finite, or max <= min in the bounds. */
+int sivo_fuse_device(const sivo_orb_t* left, const sivo_keyframe_keys* targets, int n_targets, const sivo_fuse_camera* cam,
+                     const sivo_map_point* points_device, int n_points, float th, int* match_device, int* dist_device, void* stream);
+/* Host form: every target's kps / desc / u_right / count are host arrays of its own count's keys; points, match and dist (may be
+ * NULL) on the host.  It stages the inputs, runs the device form's kernels and synchronises.  SIVO_EINVAL as above; SIVO_ERANGE
+ * for a key angle that breaks the angle rule. */
+int sivo_fuse(const sivo_orb_t* left, const sivo_keyframe_keys* targets, int n_targets, const sivo_fuse_camera* cam,
+              const sivo_map_point* points, int n_points, float th, int* match, int* dist);
+/* Test hook: the host form plus stage[k n_points + i] = where the reference's loop ends for the pair (SIVO_FUSE_STAGE_*; -1 for a
+ * target with a negative count). */
+enum {
+  SIVO_FUSE_STAGE_DEPTH = 0, SIVO_FUSE_STAGE_IMAGE, SIVO_FUSE_STAGE_DISTANCE, SIVO_FUSE_STAGE_ANGLE, SIVO_FUSE_STAGE_NO_CANDIDATE,
+  SIVO_FUSE_STAGE_ABOVE_TH_LOW, SIVO_FUSE_STAGE_MATCHED
+};
+int sivo_dbg_fuse(const sivo_orb_t* left, const sivo_keyframe_keys* targets, int n_targets, const sivo_fuse_camera* cam,
+                  const sivo_map_point* points, int n_points, float th, int* match, int* dist, int* stage);
+
 /* ---- the DBoW2 vocabulary: TemplatedVocabulary<FORB::TDescriptor, FORB>::loadFromTextFile (DBoW2 TemplatedVocabulary.h:1338-1420)
  * ---------------------------------------------------------------------------------------------------------------------------------
  * Text form: line 1 is `k L scoring weighting`; every further line is one node, id = its line number (the root is 0 and has no

@@ -666,6 +666,33 @@ int sivo_dbg_create_map_points(const sivo_orb_t* left, const sivo_keyframe_keys*
   });
 }
 
+// ---------------------------------------------------------------------------------------- keyframe Fuse
+int sivo_fuse_device(const sivo_orb_t* left, const sivo_keyframe_keys* targets, int n_targets, const sivo_fuse_camera* cam,
+                     const sivo_map_point* points_device, int n_points, float th, int* match_device, int* dist_device, void* stream) {
+  return guarded([&] {
+    if (!left || !cam || (n_points > 0 && !points_device) || (n_targets > 0 && n_points > 0 && !match_device))
+      fail(SIVO_EINVAL, "fuse: null argument");
+    fuse_device(*left->impl, targets, n_targets, *cam, points_device, n_points, th, match_device, dist_device, static_cast<cudaStream_t>(stream));
+  });
+}
+
+int sivo_fuse(const sivo_orb_t* left, const sivo_keyframe_keys* targets, int n_targets, const sivo_fuse_camera* cam,
+              const sivo_map_point* points, int n_points, float th, int* match, int* dist) {
+  return guarded([&] {
+    if (!left || !cam || (n_points > 0 && !points) || (n_targets > 0 && n_points > 0 && !match)) fail(SIVO_EINVAL, "fuse: null argument");
+    fuse_host(*left->impl, targets, n_targets, *cam, points, n_points, th, match, dist, nullptr);
+  });
+}
+
+int sivo_dbg_fuse(const sivo_orb_t* left, const sivo_keyframe_keys* targets, int n_targets, const sivo_fuse_camera* cam,
+                  const sivo_map_point* points, int n_points, float th, int* match, int* dist, int* stage) {
+  return guarded([&] {
+    if (!left || !cam || (n_points > 0 && !points) || (n_targets > 0 && n_points > 0 && (!match || !dist || !stage)))
+      fail(SIVO_EINVAL, "fuse: null argument");
+    fuse_host(*left->impl, targets, n_targets, *cam, points, n_points, th, match, dist, stage);
+  });
+}
+
 // ---------------------------------------------------------------------------------------- relocalisation PnP RANSAC
 int sivo_pnp_create(const sivo_orb_t* left, int max_candidates, uint64_t seed, sivo_pnp_t** out) {
   return guarded([&] {

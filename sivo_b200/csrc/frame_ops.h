@@ -1,5 +1,5 @@
 // The Frame-tail stages behind the C ABI (capi.cu): stereo and Hamming matching (stereo.cu), information selection (info.cu),
-// projection searches (track.cu) and pose optimisation (pose.cu).  A name ending in _device works on device-resident arrays and
+// projection searches and the keyframe Fuse (track.cu) and pose optimisation (pose.cu).  A name ending in _device works on device-resident arrays and
 // enqueues on a stream without a host synchronisation; the others take host arrays and return with the results downloaded.
 // Each function's contract is written above its definition.
 #pragma once
@@ -44,6 +44,10 @@ void search_last_frame_device(const Orb& left, const sivo_keypoint* kps, const u
                               const float* tlw, float th, int* match, long long* n_matches, cudaStream_t s);
 void features_in_area(const Orb& left, const sivo_keypoint* kps, int n, const sivo_track_frame& f, const float* xyr, const int* levels, int nq,
                       int* offsets, int* idx, int idx_cap);
+void fuse_device(const Orb& left, const sivo_keyframe_keys* targets, int n_targets, const sivo_fuse_camera& cam, const sivo_map_point* pts,
+                 int n_points, float th, int* match, int* dist, cudaStream_t s);
+void fuse_host(const Orb& left, const sivo_keyframe_keys* targets, int n_targets, const sivo_fuse_camera& cam, const sivo_map_point* pts,
+               int n_points, float th, int* match, int* dist, int* stage);
 
 // ---- pose.cu
 void pose_optimize_device(const Orb& left, const sivo_keypoint* kps, const int* keep_idx, const long long* n_keep, const float* u_right,

@@ -14,7 +14,13 @@
 //                      result depends on a removed candidate only if that candidate was its best or its second-best, so only
 //                      the points whose recorded best (local: or second) key an earlier point took are searched again.  The
 //                      last-frame search then runs the rotation histogram and ComputeThreeMaxima.
+//
+// LocalMapping::SearchInNeighbors' ORBmatcher::Fuse(pKF, vpMapPoints, th) (ORBmatcher.cc:787-930) shares the grid builder, the
+// area walk, to_camera and predict_scale: k_fuse_grid builds one grid per target keyframe (one block each), k_fuse_decide runs one
+// warp per (target, point).  Fuse claims no key, so it needs no ordered pass.
+#include <climits>
 #include <cmath>
+#include <vector>
 
 #include "block_ops.cuh"
 #include "frame_ops.h"
@@ -64,30 +70,42 @@ struct TrackBufs {  // scratch of one call, taken in order by carve()
   int* hist;        // n_points
 };
 
-size_t scratch_bytes(int cap, int np) {
-  const size_t c = std::max(cap, 1), p = std::max(np, 1);
-  return StreamScratch::bytes<int>(kCells + 1) + 2 * StreamScratch::bytes<int>(c) + StreamScratch::bytes<TrackKey>(c) +
-         StreamScratch::bytes<uint4>(2 * c) + StreamScratch::bytes<float>(c) + StreamScratch::bytes<TrackWin>(p) +
-         StreamScratch::bytes<Best2>(p) + StreamScratch::bytes<int>(p);
+// `grids` grids of cap keys each (the Fuse keeps one per target, grid_at) and the per-point arrays of np points
+size_t scratch_bytes(int cap, int np, int grids = 1) {
+  const size_t c = static_cast<size_t>(std::max(cap, 1)) * grids, p = std::max(np, 1);
+  return StreamScratch::bytes<int>(static_cast<size_t>(kCells + 1) * grids) + 2 * StreamScratch::bytes<int>(c) +
+         StreamScratch::bytes<TrackKey>(c) + StreamScratch::bytes<uint4>(2 * c) + StreamScratch::bytes<float>(c) +
+         StreamScratch::bytes<TrackWin>(p) + StreamScratch::bytes<Best2>(p) + StreamScratch::bytes<int>(p);
 }
 
-// takes the buffers, in order, from a HostCall or a StreamScratch of scratch_bytes(cap, np)
-template <class Scratch> TrackBufs carve(Scratch& a, int cap, int np) {
-  const size_t c = std::max(cap, 1), p = std::max(np, 1);
-  return {a.template take<int>(kCells + 1), a.template take<int>(c),     a.template take<int>(c),
-          a.template take<TrackKey>(c),     a.template take<uint4>(2 * c), a.template take<float>(c),
-          a.template take<TrackWin>(p),     a.template take<Best2>(p),     a.template take<int>(p)};
+// takes the buffers, in order, from a HostCall or a StreamScratch of scratch_bytes(cap, np, grids)
+template <class Scratch> TrackBufs carve(Scratch& a, int cap, int np, int grids = 1) {
+  const size_t c = static_cast<size_t>(std::max(cap, 1)) * grids, p = std::max(np, 1);
+  return {a.template take<int>(static_cast<size_t>(kCells + 1) * grids), a.template take<int>(c),
+          a.template take<int>(c),                                      a.template take<TrackKey>(c),
+          a.template take<uint4>(2 * c),                                a.template take<float>(c),
+          a.template take<TrackWin>(p),                                 a.template take<Best2>(p),
+          a.template take<int>(p)};
 }
 
-// ---- grid
-__global__ void __launch_bounds__(kGridThreads, 1) k_track_grid(const TrackParams p, const sivo_keypoint* __restrict__ kps,
-                                                                const uint8_t* __restrict__ desc, const int* __restrict__ keep_idx,
-                                                                const long long* __restrict__ n_keep, int cap,
-                                                                const float* __restrict__ u_right, TrackBufs b) {
+// grid g of a carve(.., cap, .., grids)
+__device__ __forceinline__ TrackBufs grid_at(TrackBufs b, int g, int cap) {
+  const size_t c = static_cast<size_t>(max(cap, 1)) * g;
+  b.cell_start += static_cast<size_t>(kCells + 1) * g;
+  b.cell_keys += c;
+  b.cell_of += c;
+  b.keys += c;
+  b.desc += 2 * c;
+  b.angle += c;
+  return b;
+}
+
+// ---- grid: one block of kGridThreads builds the grid of keys j < n (n >= 0, already clamped to cap)
+__device__ __forceinline__ void build_grid(const TrackParams& p, const sivo_keypoint* __restrict__ kps, const uint8_t* __restrict__ desc,
+                                           const int* __restrict__ keep_idx, int n, int cap, const float* __restrict__ u_right,
+                                           const TrackBufs& b) {
   __shared__ int cnt[kCells];
   __shared__ int warp_sum[kGridThreads / 32];
-  const int n = clamp_count(*n_keep, cap);
-  if (n < 0) return;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   for (int c = tid; c < kCells; c += kGridThreads) cnt[c] = 0;
   __syncthreads();
@@ -160,6 +178,15 @@ __global__ void __launch_bounds__(kGridThreads, 1) k_track_grid(const TrackParam
   }
 }
 
+__global__ void __launch_bounds__(kGridThreads, 1) k_track_grid(const TrackParams p, const sivo_keypoint* __restrict__ kps,
+                                                                const uint8_t* __restrict__ desc, const int* __restrict__ keep_idx,
+                                                                const long long* __restrict__ n_keep, int cap,
+                                                                const float* __restrict__ u_right, TrackBufs b) {
+  const int n = clamp_count(*n_keep, cap);
+  if (n < 0) return;
+  build_grid(p, kps, desc, keep_idx, n, cap, u_right, b);
+}
+
 // ---- GetFeaturesInArea: visits the window's candidates 32 at a time in the reference's order.  visit(ok, j, n_in_chunk) is
 // called by every lane of the warp for every chunk; lane i holds the chunk's i-th key (ok: it passes the level and position
 // filters).  Returns without visiting when an early return of Frame.cc:334-358 applies.
@@ -213,16 +240,26 @@ __device__ __forceinline__ Best2 search_window(const TrackParams& p, const Track
 }
 
 // Pc = Rcw P + tcw as cv::gemm computes it for 3 x 3 floats
-__device__ __forceinline__ void to_camera(const TrackParams& p, const float* P, float* pc) {
+__device__ __forceinline__ void to_camera(const float* rcw, const float* tcw, const float* P, float* pc) {
 #pragma unroll
-  for (int r = 0; r < 3; ++r) pc[r] = ((p.rcw[3 * r] * P[0] + p.rcw[3 * r + 1] * P[1]) + p.rcw[3 * r + 2] * P[2]) + p.tcw[r];
+  for (int r = 0; r < 3; ++r) pc[r] = ((rcw[3 * r] * P[0] + rcw[3 * r + 1] * P[1]) + rcw[3 * r + 2] * P[2]) + tcw[r];
+}
+
+// MapPoint::PredictScale(dist, F / pKF): ceil(logf(max_distance / dist) / logf(scale_factor)) clamped to [0, nlevels); -1 for a
+// NaN quotient (the reference converts it to int)
+__device__ __forceinline__ int predict_scale(const TrackParams& p, float max_distance, float dist) {
+  const float ratio = max_distance / dist;
+  const float lq = static_cast<float>(log(static_cast<double>(ratio))) / p.log_scale;
+  if (isnan(lq)) return -1;
+  const float c = ceilf(lq);
+  return c < 0.f ? 0 : (c >= static_cast<float>(p.nlevels) ? p.nlevels - 1 : static_cast<int>(c));
 }
 
 // The projection and window of one point; in_view = 0 when it is not searched.
 __device__ TrackWin project(const TrackParams& p, const sivo_map_point& mp) {
   TrackWin w{0.f, 0.f, 0.f, 0.f, 0, 0, 0, 0};
   float pc[3];
-  to_camera(p, mp.pos, pc);
+  to_camera(p.rcw, p.tcw, mp.pos, pc);
   if (!p.last_frame) {
     // Frame::isInFrustum(pMP, 0.5)
     if (pc[2] < 0.0f) return w;
@@ -244,12 +281,8 @@ __device__ TrackWin project(const TrackParams& p, const sivo_map_point& mp) {
     dot = dot + static_cast<double>(a2) * mp.normal[2];
     const float view_cos = static_cast<float>(dot / static_cast<double>(dist));
     if (isnan(view_cos) || view_cos < 0.5f) return w;
-    // MapPoint::PredictScale(dist, F)
-    const float ratio = mp.max_distance / dist;
-    const float lq = static_cast<float>(log(static_cast<double>(ratio))) / p.log_scale;
-    if (isnan(lq)) return w;
-    const float c = ceilf(lq);
-    const int level = c < 0.f ? 0 : (c >= static_cast<float>(p.nlevels) ? p.nlevels - 1 : static_cast<int>(c));
+    const int level = predict_scale(p, mp.max_distance, dist);
+    if (level < 0) return w;
     // ORBmatcher::SearchByProjection(F, vpMapPoints, th)
     float r = static_cast<double>(view_cos) > 0.998 ? 2.5f : 4.0f;
     if (p.th != 1.0f) r *= p.th;
@@ -514,6 +547,160 @@ void search_device(const Orb& left, bool last, const sivo_keypoint* kps, const u
   const TrackBufs b = carve(sc, cap, n_points);
   launch_search(p, kps, desc, keep_idx, n_keep, cap, u_right, blocked, pts, n_points, b, in_view, match, n_matches, s);
 }
+
+// ---- ORBmatcher::Fuse(pKF, vpMapPoints, th) over a chunk of targets: every target's grid in one launch (block k builds target
+// k's), then one warp per (target, point) pair.  The pair's decision depends only on the point and the target, so the pairs run
+// independently; the caller's map bookkeeping replays them in the reference's order (include/sivo_b200.h).
+constexpr int kFuseChunk = 64;  // targets per launch: their records ride in the kernel parameters
+constexpr int kFuseThreads = 128;
+constexpr int kThLow = 50;      // ORBmatcher::TH_LOW
+enum { kFuseNegative = -1, kFuseDepth = 0, kFuseImage, kFuseDistance, kFuseAngle, kFuseNoCandidate, kFuseAboveThLow, kFuseMatched };
+
+struct FuseTarget {
+  const sivo_keypoint* kps;
+  const uint8_t* desc;
+  const float* ur;
+  const long long* count;
+  float rcw[9], tcw[3], ow[3];
+};
+
+struct FuseParams {
+  TrackParams geo;  // the shared camera, bounds and scale tables (its pose is unused)
+  float inv_sigma2[kOrbMaxLevels];
+  int cap, n_targets, base, n_points;  // base: the chunk's first target
+  FuseTarget t[kFuseChunk];
+};
+
+__global__ void __launch_bounds__(kGridThreads, 1) k_fuse_grid(const __grid_constant__ FuseParams p, TrackBufs g) {
+  const FuseTarget& t = p.t[blockIdx.x];
+  const int n = clamp_count(*t.count, p.cap);
+  if (n < 0) return;
+  build_grid(p.geo, t.kps, t.desc, nullptr, n, p.cap, t.ur, grid_at(g, blockIdx.x, p.cap));
+}
+
+// One warp per pair: (blockIdx.y = target in the chunk, point).  Writes match / dist / stage at (base + k) n_points + i.
+__global__ void __launch_bounds__(kFuseThreads) k_fuse_decide(const __grid_constant__ FuseParams p, TrackBufs g,
+                                                              const sivo_map_point* __restrict__ pts, float th, int* __restrict__ match,
+                                                              int* __restrict__ dist, int* __restrict__ stage_out) {
+  const int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31, k = blockIdx.y;
+  if (i >= p.n_points) return;
+  const FuseTarget& t = p.t[k];
+  const TrackParams& c = p.geo;
+  const sivo_map_point& mp = pts[i];
+  int stage = kFuseNegative, bd = 256, bi = -1;
+  if (*t.count >= 0) {
+    float pc[3];
+    to_camera(t.rcw, t.tcw, mp.pos, pc);
+    stage = kFuseDepth;
+    if (!(pc[2] < 0.0f)) {
+      const float invz = 1 / pc[2];
+      const float x = pc[0] * invz, y = pc[1] * invz;
+      const float u = c.fx * x + c.cx, v = c.fy * y + c.cy;
+      stage = kFuseImage;
+      // KeyFrame::IsInImage: strict upper bounds; a NaN is out
+      if (u >= c.min_x && u < c.max_x && v >= c.min_y && v < c.max_y) {
+        const float ur = u - c.mbf * invz;
+        const float max_d = 1.2f * mp.max_distance, min_d = 0.8f * mp.min_distance;
+        const float a[3] = {mp.pos[0] - t.ow[0], mp.pos[1] - t.ow[1], mp.pos[2] - t.ow[2]};
+        double ss = 0.0, dot = 0.0;
+#pragma unroll
+        for (int r = 0; r < 3; ++r) ss = ss + static_cast<double>(a[r]) * a[r];
+        const float dist3 = static_cast<float>(sqrt(ss));
+#pragma unroll
+        for (int r = 0; r < 3; ++r) dot = dot + static_cast<double>(a[r]) * mp.normal[r];
+        stage = kFuseDistance;
+        if (!(dist3 < min_d || dist3 > max_d)) {
+          stage = kFuseAngle;
+          if (!(dot < 0.5 * static_cast<double>(dist3))) {
+            const int level = predict_scale(c, mp.max_distance, dist3);
+            stage = kFuseNoCandidate;  // also a NaN level quotient: nothing is searched
+            if (level >= 0) {
+              const float radius = th * c.scale[level];
+              const uint4 q0 = reinterpret_cast<const uint4*>(mp.desc)[0], q1 = reinterpret_cast<const uint4*>(mp.desc)[1];
+              const TrackBufs b = grid_at(g, k, p.cap);
+              bool any = false;
+              walk_area(c, b, u, v, radius, -1, -1, lane, [&](bool ok, int j, int) {
+                any |= __any_sync(0xffffffffu, ok);
+                unsigned key = 256u << 5 | 31u;
+                if (ok) {
+                  const TrackKey kp = b.keys[j];
+                  const int o = kp.octave;
+                  if (o >= level - 1 && o <= level && o >= 0 && o < c.nlevels) {
+                    const float ex = u - kp.x, ey = v - kp.y;
+                    bool pass;
+                    if (kp.ur >= 0.f) {
+                      const float er = ur - kp.ur;
+                      const float e2 = (ex * ex + ey * ey) + er * er;
+                      pass = !(static_cast<double>(e2 * p.inv_sigma2[o]) > 7.8);
+                    } else {
+                      const float e2 = ex * ex + ey * ey;
+                      pass = !(static_cast<double>(e2 * p.inv_sigma2[o]) > 5.99);
+                    }
+                    if (pass) key = static_cast<unsigned>(descriptor_distance(q0, q1, b.desc[2 * j], b.desc[2 * j + 1])) << 5 | lane;
+                  }
+                }
+                // the chunk's smallest distance, first in walk order on ties; a later chunk takes over only when strictly smaller
+                const unsigned m = __reduce_min_sync(0xffffffffu, key);
+                const int jm = __shfl_sync(0xffffffffu, j, m & 31u);
+                if (static_cast<int>(m >> 5) < bd) { bd = static_cast<int>(m >> 5); bi = jm; }
+              });
+              if (any) stage = bd <= kThLow ? kFuseMatched : kFuseAboveThLow;
+            }
+          }
+        }
+      }
+    }
+  }
+  if (lane == 0) {
+    const size_t e = static_cast<size_t>(p.base + k) * p.n_points + i;
+    match[e] = stage == kFuseMatched ? bi : -1;
+    if (dist) dist[e] = bd;
+    if (stage_out) stage_out[e] = stage;
+  }
+}
+
+FuseParams fuse_params(const Orb& left, const sivo_fuse_camera& cam, int cap, int n_points) {
+  sivo_track_frame f{};
+  f.fx = cam.fx; f.fy = cam.fy; f.cx = cam.cx; f.cy = cam.cy; f.mbf = cam.mbf;
+  f.min_x = cam.min_x; f.max_x = cam.max_x; f.min_y = cam.min_y; f.max_y = cam.max_y;
+  FuseParams p{};
+  p.geo = make_params(left, f);
+  for (int l = 0; l < p.geo.nlevels; ++l) p.inv_sigma2[l] = left.tables().inv_sigma2[l];
+  p.cap = cap;
+  p.n_points = n_points;
+  return p;
+}
+
+void check_fuse_args(const sivo_keyframe_keys* targets, int n_targets, int n_points, float th) {
+  if (n_targets < 0 || n_points < 0) fail(SIVO_EINVAL, "fuse: n_targets %d, n_points %d", n_targets, n_points);
+  if (static_cast<long long>(n_targets) * n_points > INT_MAX) fail(SIVO_EINVAL, "fuse: %d x %d pairs exceed INT_MAX", n_targets, n_points);
+  if (!(th > 0.f) || !std::isfinite(th)) fail(SIVO_EINVAL, "fuse: th %g", th);
+  if (n_targets > 0 && !targets) fail(SIVO_EINVAL, "fuse: null targets");
+  for (int k = 0; k < n_targets; ++k)
+    if (!targets[k].count) fail(SIVO_EINVAL, "fuse: target %d has no count", k);
+}
+
+// Runs every chunk of targets (t: device pointers) with the grids g (min(n_targets, kFuseChunk) of them).
+void launch_fuse(FuseParams& p, const FuseTarget* t, int n_targets, const TrackBufs& g, const sivo_map_point* pts, float th, int* match,
+                 int* dist, int* stage, cudaStream_t s) {
+  if (p.n_points == 0) return;
+  for (int base = 0; base < n_targets; base += kFuseChunk) {
+    p.base = base;
+    p.n_targets = std::min(kFuseChunk, n_targets - base);
+    for (int k = 0; k < p.n_targets; ++k) p.t[k] = t[base + k];
+    k_fuse_grid<<<p.n_targets, kGridThreads, 0, s>>>(p, g);
+    SIVO_CUDA(cudaGetLastError());
+    k_fuse_decide<<<dim3(ceil_div(p.n_points, kFuseThreads / 32), p.n_targets), kFuseThreads, 0, s>>>(p, g, pts, th, match, dist, stage);
+    SIVO_CUDA(cudaGetLastError());
+  }
+}
+
+FuseTarget fuse_target(const sivo_keyframe_keys& k, const sivo_keypoint* kps, const uint8_t* desc, const float* ur, const long long* count) {
+  FuseTarget t{kps, desc, ur, count, {}, {}, {}};
+  for (int i = 0; i < 9; ++i) t.rcw[i] = k.Rcw[i];
+  for (int i = 0; i < 3; ++i) { t.tcw[i] = k.tcw[i]; t.ow[i] = k.Ow[i]; }
+  return t;
+}
 }  // namespace
 
 void search_local_points(const Orb& left, const sivo_keypoint* kps, const uint8_t* desc, const float* u_right, const uint8_t* blocked, int n,
@@ -580,6 +767,62 @@ void features_in_area(const Orb& left, const sivo_keypoint* kps, int n, const si
   k_area_lists<<<ceil_div(nq * 32, 128), 128, 0, st>>>(p, b, d_xyr, d_lv, nq, d_off, d_idx);
   SIVO_CUDA(cudaGetLastError());
   hc.download(idx, d_idx, offsets[nq]);
+  hc.sync();
+}
+
+void fuse_device(const Orb& left, const sivo_keyframe_keys* targets, int n_targets, const sivo_fuse_camera& cam, const sivo_map_point* pts,
+                 int n_points, float th, int* match, int* dist, cudaStream_t s) {
+  check_fuse_args(targets, n_targets, n_points, th);
+  const int cap = left.capacity();
+  FuseParams p = fuse_params(left, cam, cap, n_points);
+  std::vector<FuseTarget> t(n_targets);
+  for (int k = 0; k < n_targets; ++k) {
+    const sivo_keyframe_keys& tk = targets[k];
+    if (!tk.kps || !tk.desc || !tk.u_right) fail(SIVO_EINVAL, "fuse: null array in target %d", k);
+    t[k] = fuse_target(tk, tk.kps, tk.desc, tk.u_right, tk.count);
+  }
+  if (!n_targets || !n_points) return;
+  s = left.enter(s);
+  const int grids = std::min(n_targets, kFuseChunk);
+  StreamScratch sc(scratch_bytes(cap, 0, grids), s);
+  const TrackBufs g = carve(sc, cap, 0, grids);
+  launch_fuse(p, t.data(), n_targets, g, pts, th, match, dist, nullptr, s);
+}
+
+// The host form and the test hook: stage every target's keys and the points, run the device form's kernels, download.
+void fuse_host(const Orb& left, const sivo_keyframe_keys* targets, int n_targets, const sivo_fuse_camera& cam, const sivo_map_point* pts,
+               int n_points, float th, int* match, int* dist, int* stage) {
+  check_fuse_args(targets, n_targets, n_points, th);
+  int cap = 0;
+  for (int k = 0; k < n_targets; ++k) {
+    const sivo_keyframe_keys& tk = targets[k];
+    const long long n = *tk.count;
+    if (n > INT_MAX) fail(SIVO_EINVAL, "fuse: target %d has %lld keys", k, n);
+    if (n > 0 && (!tk.kps || !tk.desc || !tk.u_right)) fail(SIVO_EINVAL, "fuse: null array in target %d", k);
+    for (long long j = 0; j < n; ++j)
+      if (!angle_ok(tk.kps[j].angle)) fail(SIVO_ERANGE, "fuse: target %d key %lld has angle %g outside [0, 360]", k, j, tk.kps[j].angle);
+    cap = std::max(cap, static_cast<int>(std::max(n, 0ll)));
+  }
+  FuseParams p = fuse_params(left, cam, cap, n_points);
+  if (!n_targets || !n_points) return;
+  HostCall& hc = host_call();
+  hc.begin(left.device());
+  std::vector<FuseTarget> t(n_targets);
+  for (int k = 0; k < n_targets; ++k) {
+    const sivo_keyframe_keys& tk = targets[k];
+    const size_t n = static_cast<size_t>(std::max(*tk.count, 0ll));
+    t[k] = fuse_target(tk, hc.upload(tk.kps, n), hc.upload(tk.desc, 32 * n), hc.upload(tk.u_right, n), hc.upload(tk.count, 1));
+  }
+  const sivo_map_point* d_pts = hc.upload(pts, n_points);
+  const size_t np = static_cast<size_t>(n_targets) * n_points;
+  int* d_match = hc.take<int>(np);
+  int* d_dist = hc.take<int>(np);
+  int* d_stage = stage ? hc.take<int>(np) : nullptr;
+  const TrackBufs g = carve(hc, cap, 0, std::min(n_targets, kFuseChunk));
+  launch_fuse(p, t.data(), n_targets, g, d_pts, th, d_match, d_dist, d_stage, hc.stream);
+  hc.download(match, d_match, np);
+  hc.download(dist, d_dist, np);
+  hc.download(stage, d_stage, np);
   hc.sync();
 }
 

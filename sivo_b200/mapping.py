@@ -1,6 +1,6 @@
 """A keyframe's new map points over the C-ABI: LocalMapping::CreateNewMapPoints with ORBmatcher::SearchForTriangulation and SIVO's
-CheckSemantics, and the KeyFrame's copy of a Frame's semantic keys.  The rule is spelled out in include/sivo_b200.h and
-oracle/mapping_oracle.py."""
+CheckSemantics, the KeyFrame's copy of a Frame's semantic keys, and SearchInNeighbors' ORBmatcher::Fuse over every target keyframe
+at once.  The rules are spelled out in include/sivo_b200.h, oracle/mapping_oracle.py and oracle/fuse_oracle.py."""
 from __future__ import annotations
 
 import ctypes as C
@@ -10,6 +10,7 @@ import numpy as np
 from . import _lib as L
 from .orb import KP_DTYPE, ORBextractor
 
+FUSE_STAGES = ("depth", "image", "distance", "angle", "no_candidate", "above_th_low", "matched")  # SIVO_FUSE_STAGE_*
 STAGES = ("has_point", "baseline", "no_match", "parallax", "w_zero", "z1", "z2", "reproj1", "reproj2", "scale", "semantic", "created")
 
 
@@ -111,3 +112,68 @@ def keyframe_gather_device(left: ORBextractor, kps_ptr, desc_ptr, keep_idx_ptr, 
            for k in ("kps", "desc", "u_right", "depth", "kp_class", "kp_conf", "kp_entropy", "count")]
     L.check(L.lib().sivo_keyframe_gather_device(left._h, kps_ptr, desc_ptr, keep_idx_ptr, n_keep_ptr, u_right_ptr, depth_ptr,
                                                 class_ptr, conf_ptr, entropy_ptr, *ptr, stream))
+
+
+class FuseCamera(C.Structure):
+    """sivo_fuse_camera: the keyframes' shared camera and image bounds."""
+    _fields_ = [(n, C.c_float) for n in ("fx", "fy", "cx", "cy", "mbf", "min_x", "max_x", "min_y", "max_y")]
+
+
+def make_fuse_camera(fx, fy, cx, cy, mbf, bounds) -> FuseCamera:
+    """bounds = (mnMinX, mnMaxX, mnMinY, mnMaxY)."""
+    c = FuseCamera()
+    c.fx, c.fy, c.cx, c.cy, c.mbf = (np.float32(v) for v in (fx, fy, cx, cy, mbf))
+    c.min_x, c.max_x, c.min_y, c.max_y = (np.float32(v) for v in bounds)
+    return c
+
+
+class FuseTarget:
+    """Host arrays of one Fuse target (kept alive here): its semantic keys, descriptors, mvRight and pose; count defaults to the
+    number of keys (a negative count: the target's row is all -1)."""
+
+    def __init__(self, kps, desc, u_right, Rcw, tcw, Ow, count=None):
+        self.arrays = [np.ascontiguousarray(kps, KP_DTYPE), np.ascontiguousarray(desc, np.uint8).reshape(-1, 32),
+                       np.ascontiguousarray(u_right, np.float32)]
+        n = len(self.arrays[0])
+        if any(len(a) != n for a in self.arrays):
+            raise ValueError("kps, desc and u_right need one entry per key")
+        self.n = n
+        self.count = np.array([n if count is None else count], np.int64)
+        k, d, u = (a.ctypes.data for a in self.arrays)
+        self.keys = KeyframeKeys(k, d, u, None, None, None, None, None, None, self.count.ctypes.data)
+        set_pose(self.keys, Rcw, tcw, Ow)
+
+
+def _points(points):
+    from .track import MAP_POINT_DTYPE
+    return np.ascontiguousarray(points, MAP_POINT_DTYPE)
+
+
+def fuse(left: ORBextractor, targets, cam: FuseCamera, points, th: float = 3.0, debug: bool = False):
+    """Host form of sivo_fuse (debug: sivo_dbg_fuse).  targets: FuseTarget list; points: sivo_map_point records.  Returns (match,
+    dist) as (n_targets, n_points) int32 arrays, with debug also stage (SIVO_FUSE_STAGE_*, -1 for a negative count)."""
+    pts = _points(points)
+    nt, npt = len(targets), len(pts)
+    match = np.empty((nt, npt), np.int32)
+    dist = np.empty((nt, npt), np.int32)
+    common = (left._h, _nb_array([t.keys for t in targets]), nt, C.byref(cam), L.ptr(pts), npt, th, L.ptr(match), L.ptr(dist))
+    if not debug:
+        L.check(L.lib().sivo_fuse(*common))
+        return match, dist
+    stage = np.empty((nt, npt), np.int32)
+    L.check(L.lib().sivo_dbg_fuse(*common, L.ptr(stage)))
+    return match, dist, stage
+
+
+def dbg_fuse(left: ORBextractor, targets, cam: FuseCamera, points, th: float = 3.0):
+    """The test hook sivo_dbg_fuse: (match, dist, stage)."""
+    return fuse(left, targets, cam, points, th, debug=True)
+
+
+def fuse_device(left: ORBextractor, targets, cam: FuseCamera, points_ptr: int, n_points: int, th: float, match_ptr: int, dist_ptr: int = 0,
+                stream: int = 0):
+    """sivo_fuse_device: targets are KeyframeKeys holding device pointers (kps, desc, u_right, count) and poses; points_ptr a
+    device array of n_points sivo_map_point records; match_ptr / dist_ptr device int32 arrays of len(targets) x n_points (dist 0:
+    not wanted).  Enqueued on `stream` (0 = the left extractor's stream) with no waits and no host synchronisation."""
+    L.check(L.lib().sivo_fuse_device(left._h, _nb_array(targets), len(targets), C.byref(cam), points_ptr, n_points, th, match_ptr,
+                                      dist_ptr, stream))
