@@ -1,28 +1,27 @@
 """ORBmatcher::Fuse on the device (sivo_fuse_device) at SearchInNeighbors' sizes: phase 1 at (targets, points) = (1, 2000),
 (10, 2000), (25, 2000) and (60, 2000), phase 2 at (1, 50000), and the host form (sivo_fuse) end to end at (10, 2000).  Each
 target holds 2000 keys, and about half of the points project near one of a target's keys with a few descriptor bits changed, so the
-windows and fold see real candidates.  Prints one JSON line with each call's median / p90 ms (CUDA events around each of 200 calls
-after warm-up; the host form: the host clock around each of 200 calls, which synchronise), the device form's equality with the
-host form on every configuration, and the GPU's name and power limit read in the same run.  The reference's host loop is not
-built here, so it is not measured."""
+windows and fold see real candidates.  Prints one JSON line with each call's median / p90 ms, timed as DESIGN.md §7 describes, and
+the device form's equality with the host form on every configuration.  The reference's host loop is not built here, so it is not
+measured.
+
+    python tools/fuse_bench.py [--steps 200] [--warmup 20]
+"""
+import argparse
 import json
-import os
-import subprocess
-import sys
-import time
 
 import numpy as np
 import torch
 
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
-from oracle.mapping_scene import rotation  # noqa: E402
-from oracle.track_oracle import gemm_neg_t  # noqa: E402
-from sivo_b200.mapping import FuseTarget, KeyframeKeys, fuse, fuse_device, make_fuse_camera, set_pose  # noqa: E402
-from sivo_b200.orb import KP_DTYPE, ORBextractor  # noqa: E402
-from sivo_b200.track import MAP_POINT_DTYPE  # noqa: E402
+from bench_support import add_common_args, card, device_ms, host_ms, require_cuda, stats  # puts the repository on sys.path
+from oracle.mapping_scene import rotation
+from oracle.track_oracle import gemm_neg_t
+from sivo_b200.mapping import FuseTarget, KeyframeKeys, fuse, fuse_device, make_fuse_camera, set_pose
+from sivo_b200.orb import KP_DTYPE, ORBextractor
+from sivo_b200.track import MAP_POINT_DTYPE
 
 FX, CX, CY, MBF, W, H = 718.856, 607.19, 185.22, 386.14, 1241.0, 376.0
-N_KEYS, CALLS, WARMUP = 2000, 200, 20
+N_KEYS = 2000
 
 
 def scene(n_targets, n_points, seed):
@@ -75,17 +74,16 @@ def device_targets(targets, cap):
     return keep, keys
 
 
-def stats(ms):
-    ms = np.sort(np.asarray(ms))
-    return {"median_ms": float(np.median(ms)), "p90_ms": float(ms[int(0.9 * (len(ms) - 1))])}
-
-
 def main():
+    ap = argparse.ArgumentParser()
+    add_common_args(ap, steps=200, warmup=20)
+    a = ap.parse_args()
+    require_cuda("fuse_bench.py")
     left = ORBextractor(N_KEYS, 1.2, 8, 20, 7)
     cap = left.capacity()
     cam = make_fuse_camera(FX, FX, CX, CY, MBF, (0.0, W, 0.0, H))
     stream = torch.cuda.Stream()
-    out = {"configs": []}
+    out = {"tool": "fuse_bench", "unit": "ms", **card(), "configs": []}
     for nt, npts in ((1, 2000), (10, 2000), (25, 2000), (60, 2000), (1, 50000)):
         targets, pts = scene(nt, npts, seed=nt * 7 + npts)
         keep, keys = device_targets(targets, cap)
@@ -94,39 +92,18 @@ def main():
         dist = torch.empty((nt, npts), dtype=torch.int32, device="cuda")
         torch.cuda.synchronize()
         call = lambda: fuse_device(left, keys, cam, d_pts.data_ptr(), npts, 3.0, match.data_ptr(), dist.data_ptr(), stream.cuda_stream)
-        for _ in range(WARMUP):
-            call()
-        ev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(CALLS)]
-        for a, b in ev:
-            a.record(stream)
-            call()
-            b.record(stream)
-        stream.synchronize()
-        ms = [a.elapsed_time(b) for a, b in ev]
+        ms = device_ms(call, stream, a.warmup, a.steps)
         host = [FuseTarget(kps, desc, ur, R, t, Ow) for kps, desc, ur, R, t, Ow in targets]
         hm, hd = fuse(left, host, cam, pts, 3.0)
-        entry = {"targets": nt, "points": npts, "device": stats(ms), "equal_to_host_form": bool(
+        entry = {"targets": nt, "points": npts, "device_call_ms": stats(ms), "equal_to_host_form": bool(
             np.array_equal(match.cpu().numpy(), hm) and np.array_equal(dist.cpu().numpy(), hd)),
             "matched_pairs": int((hm >= 0).sum())}
         if (nt, npts) == (10, 2000):
-            for _ in range(5):
-                fuse(left, host, cam, pts, 3.0)
-            t_host = []
-            for _ in range(CALLS):
-                t0 = time.perf_counter()
-                fuse(left, host, cam, pts, 3.0)
-                t_host.append((time.perf_counter() - t0) * 1e3)
-            entry["host_form_end_to_end"] = stats(t_host)
+            entry["host_call_ms"] = stats(host_ms(lambda: fuse(left, host, cam, pts, 3.0), 5, a.steps))
         out["configs"].append(entry)
         del keep
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
-    out["gpu"] = q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else torch.cuda.get_device_name()
     out["all_equal"] = all(c["equal_to_host_form"] for c in out["configs"])
-    line = json.dumps(out)
-    print(line)
-    if len(sys.argv) > 1:  # optional: also write the line to this file
-        with open(sys.argv[1], "w") as f:
-            f.write(line + "\n")
+    print(json.dumps(out))
 
 
 if __name__ == "__main__":

@@ -1,20 +1,19 @@
 """Map-point creation (sivo_create_map_points_device) at 2000 keys x 10 neighbours on a constructed scene: prints one JSON line with
-the device call's median / p90 ms (CUDA events, 200 calls after warm-up), the host form's end-to-end ms, and the GPU's name and
-power limit read in the same run.  The reference's host loop (LocalMapping::CreateNewMapPoints with OpenCV) is not built here, so it
-is not measured."""
+the device call's and the host form's median / p90 ms, timed as DESIGN.md §7 describes.  The reference's host loop
+(LocalMapping::CreateNewMapPoints with OpenCV) is not built here, so it is not measured.
+
+    python tools/mapping_bench.py [--steps 200] [--warmup 20]
+"""
+import argparse
 import json
-import os
-import subprocess
-import sys
-import time
 
 import numpy as np
 import torch
 
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
-from oracle import mapping_scene as S  # noqa: E402
-from sivo_b200.mapping import KeyframeKeys, create_map_points, create_map_points_device, HostKeyframe, make_params, set_pose  # noqa: E402
-from sivo_b200.orb import ORBextractor  # noqa: E402
+from bench_support import add_common_args, card, device_ms, host_ms, require_cuda, stats  # puts the repository on sys.path
+from oracle import mapping_scene as S
+from sivo_b200.mapping import KeyframeKeys, create_map_points, create_map_points_device, HostKeyframe, make_params, set_pose
+from sivo_b200.orb import ORBextractor
 
 
 def device_kf(kf, cap, keep):
@@ -30,6 +29,10 @@ def device_kf(kf, cap, keep):
 
 
 def main():
+    ap = argparse.ArgumentParser()
+    add_common_args(ap, steps=200, warmup=20)
+    a = ap.parse_args()
+    require_cuda("mapping_bench.py")
     p = S.EXTRACTOR
     left = ORBextractor(p.nfeatures, p.scale_factor, p.nlevels, 20, 7)
     cap = left.capacity()
@@ -45,31 +48,15 @@ def main():
     s = torch.cuda.Stream()
     torch.cuda.synchronize()
     call = lambda: create_map_points_device(left, d1, dn, prm, nb.data_ptr(), 0, world.data_ptr(), lst.data_ptr(), n.data_ptr(), s.cuda_stream)
-    for _ in range(20):
-        call()
-    s.synchronize()
-    ms = []
-    for _ in range(200):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record(s)
-        call()
-        b.record(s)
-        b.synchronize()
-        ms.append(a.elapsed_time(b))
+    ms = device_ms(call, s, a.warmup, a.steps)
     hk1 = HostKeyframe(kf1.kps, kf1.desc, kf1.u_right, kf1.depth, kf1.kp_class, kf1.kp_conf, kf1.kp_entropy, kf1.node, kf1.has_point,
                        kf1.Rcw, kf1.tcw, kf1.Ow)
     hn = [HostKeyframe(k.kps, k.desc, k.u_right, k.depth, k.kp_class, k.kp_conf, k.kp_entropy, k.node, k.has_point, k.Rcw, k.tcw, k.Ow)
           for k in nbs]
-    create_map_points(left, hk1, hn, prm)
-    host = []
-    for _ in range(20):
-        t0 = time.perf_counter()
-        r = create_map_points(left, hk1, hn, prm)
-        host.append(1e3 * (time.perf_counter() - t0))
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
-    print(json.dumps({"workload": "create_map_points 2000 keys x 10 neighbours", "device_ms_median": float(np.median(ms)),
-                      "device_ms_p90": float(np.percentile(ms, 90)), "host_form_ms_median": float(np.median(host)),
-                      "n_created": int(n.item()), "n_created_host": int(r["n_created"]), "gpu": q.stdout.strip().splitlines()[0] if q.stdout else "",
+    r = create_map_points(left, hk1, hn, prm)
+    host = host_ms(lambda: create_map_points(left, hk1, hn, prm), 0, 20)
+    print(json.dumps({"workload": "create_map_points 2000 keys x 10 neighbours", "unit": "ms", **card(), "device_call_ms": stats(ms),
+                      "host_call_ms": stats(host), "n_created": int(n.item()), "n_created_host": int(r["n_created"]),
                       "reference_host_loop": "not measured"}))
 
 

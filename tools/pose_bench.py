@@ -1,15 +1,15 @@
 #!/usr/bin/env python
 """Frame-pose benchmark: Optimizer::PoseOptimization on the device (sivo_pose_optimize_device).  Prints one JSON line
-{"metric": "pose optimisation", ...}.
+{"metric": "pose optimisation", ...}, timed as DESIGN.md §7 describes.
 
   python tools/pose_bench.py [--steps 30] [--warmup 5] [--blocks-of 10]
 
 Reports:
-  (a) device_call_ms: the device call at 100 / 500 / 1000 / 2000 edges with 0 / 30 % gross outliers, CUDA events around the call,
-      median / p90 over --steps calls.  The scenes are synthetic (keys at random pixels and depths seen from a known pose, 0.5 px
+  (a) device_call_ms: the device call at 100 / 500 / 1000 / 2000 edges with 0 / 30 % gross outliers, median / p90 over --steps
+      calls.  The scenes are synthetic (keys at random pixels and depths seen from a known pose, 0.5 px
       noise times the octave's scale, about 60 % stereo, the initial pose moved by up to 0.01 rad / 5 cm), because a 1024x352 frame
       holds fewer semantic keys with depth than the larger counts;
-  (b) host_call_ms: the host form on the same scenes, end to end (host wall time);
+  (b) host_call_ms: the host form on the same scenes, end to end;
   (c) frames/s of Tracking's device chain SegNet (Basic T=6) + ORB(2000) x2 + semantic keys + stereo + last-frame search +
       local-map search, without and with the two optimisations appended the way Tracking runs them: last-frame search -> gather
       -> pose -> the host reads the 512-byte result -> local-map search at that pose -> gather -> pose.  The host read makes
@@ -18,20 +18,13 @@ Reports:
       moved by 0.5-2 m), found by a first pass of the front end.  The two legs alternate in blocks.
 The g2o host loop the kernel replaces (Eigen + CHOLMOD) is not built here: not measured.  Writes nothing into the source tree."""
 import argparse
-import gc
 import json
-import os
-import sys
-import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-
-from bench import CROP_X, CROP_Y, NET_H, NET_W, frames, model_cache_dir, model_files  # noqa: E402
-from oracle.mapping_scene import rotation  # noqa: E402
+from bench_support import (CROP_X, CROP_Y, NET_H, NET_W, add_common_args, alternate, basic_front_end, card, chain_frames,
+                           check_device_trees, device_ms, host_ms, require_cuda, stats)
+from oracle.mapping_scene import rotation
 
 FX, CX, CY, MBF = 718.856, 607.1928 - CROP_X, 185.2157 - CROP_Y, 386.1448  # KITTI00-02.yaml, principal point in the crop
 MB = MBF / FX
@@ -68,31 +61,26 @@ def frame_map(kps, desc, depth, scale, rng):
 
 def run(args):
     import torch
-    from sivo_b200 import (BayesianSegNet, BayesianSegNetParams, KP_DTYPE, ORBextractor, make_frame, pose_gather_device, pose_optimize,
-                           pose_optimize_device, search_last_frame_device, search_local_points_device)
+    from sivo_b200 import (KP_DTYPE, make_frame, pose_gather_device, pose_optimize, pose_optimize_device, search_last_frame_device,
+                           search_local_points_device)
     from sivo_b200.frame import DeviceFrame
     from sivo_b200.pose import frame_from_result, result_from_bytes
-    if not torch.cuda.is_available():
-        raise SystemExit("pose_bench.py needs a CUDA device (there is no CPU fallback for the product path)")
-    dev = torch.device("cuda", 0)
-    el, er = (ORBextractor(args.nfeatures, 1.2, 8, 20, 7) for _ in range(2))
+    T = 6
+    seg, el, er = basic_front_end(args.nfeatures, T)
     cap = el.capacity()
-    u8, i32, i64, f32, f64 = torch.uint8, torch.int32, torch.int64, torch.float32, torch.float64
-    stream = torch.cuda.Stream(dev)
+    u8, i32, i64, f32 = torch.uint8, torch.int32, torch.int64, torch.float32
+    stream = torch.cuda.Stream()
     s = stream.cuda_stream
-    med = lambda v: float(np.median(v))
-    p90 = lambda v: float(np.percentile(v, 90))
     rng = np.random.default_rng(0)
 
     # (a) / (b)
-    kp_buf = torch.zeros(cap * 28, dtype=u8, device=dev)
-    n_buf = torch.zeros(1, dtype=i64, device=dev)
-    ur_buf = torch.zeros(cap, dtype=f32, device=dev)
-    xw_buf = torch.full((3 * cap,), float("nan"), dtype=f32, device=dev)
-    t_buf = torch.zeros(12, dtype=f32, device=dev)
-    res_buf = torch.zeros(512, dtype=u8, device=dev)
-    out_buf = torch.zeros(cap, dtype=u8, device=dev)
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    kp_buf = torch.zeros(cap * 28, dtype=u8, device="cuda")
+    n_buf = torch.zeros(1, dtype=i64, device="cuda")
+    ur_buf = torch.zeros(cap, dtype=f32, device="cuda")
+    xw_buf = torch.full((3 * cap,), float("nan"), dtype=f32, device="cuda")
+    t_buf = torch.zeros(12, dtype=f32, device="cuda")
+    res_buf = torch.zeros(512, dtype=u8, device="cuda")
+    out_buf = torch.zeros(cap, dtype=u8, device="cuda")
     calls = {}
     for n in EDGES:
         for frac in (0.0, 0.3):
@@ -104,47 +92,28 @@ def run(args):
             ur_buf[:len(kps)].copy_(torch.from_numpy(ur))
             xw_buf[:3 * len(kps)].copy_(torch.from_numpy(X.reshape(-1)))
             t_buf.copy_(torch.from_numpy(Tin.reshape(-1)))
-            torch.cuda.synchronize(dev)
-            dev_ms, host_ms = [], []
-            gc.collect()
-            gc.disable()
-            for i in range(args.warmup + args.steps):
-                e0.record(stream)
-                pose_optimize_device(el, kp_buf.data_ptr(), 0, n_buf.data_ptr(), ur_buf.data_ptr(), xw_buf.data_ptr(), FX, FX, CX, CY, MBF,
-                                     t_buf.data_ptr(), res_buf.data_ptr(), out_buf.data_ptr(), s)
-                e1.record(stream)
-                e1.synchronize()
-                t0 = time.perf_counter()
-                hres, _ = pose_optimize(el, kps, ur, X, Tin, FX, FX, CX, CY, MBF)
-                t1 = time.perf_counter()
-                if i >= args.warmup:
-                    dev_ms.append(e0.elapsed_time(e1))
-                    host_ms.append(1e3 * (t1 - t0))
-            gc.enable()
+            torch.cuda.synchronize()
+            dev_ms = device_ms(lambda: pose_optimize_device(el, kp_buf.data_ptr(), 0, n_buf.data_ptr(), ur_buf.data_ptr(), xw_buf.data_ptr(),
+                                                            FX, FX, CX, CY, MBF, t_buf.data_ptr(), res_buf.data_ptr(), out_buf.data_ptr(), s),
+                               stream, args.warmup, args.steps)
+            host = host_ms(lambda: pose_optimize(el, kps, ur, X, Tin, FX, FX, CX, CY, MBF), args.warmup, args.steps)
+            hres, _ = pose_optimize(el, kps, ur, X, Tin, FX, FX, CX, CY, MBF)
             dres = result_from_bytes(res_buf.cpu().numpy())
             calls[f"{n}_edges_{int(frac * 100)}pct_outliers"] = {
-                "device_call_ms": {"median": med(dev_ms), "p90": p90(dev_ms)}, "host_call_ms": {"median": med(host_ms), "p90": p90(host_ms)},
-                "n_good": int(dres.n_good), "device_equals_host": bytes(dres) == bytes(hres)}
+                "device_call_ms": stats(dev_ms), "host_call_ms": stats(host), "n_good": int(dres.n_good),
+                "device_equals_host": bytes(dres) == bytes(hres)}
 
     # (c) the chain
-    T = 6
-    _, proto, model, _ = model_files("basic", T, model_cache_dir())
-    seg = BayesianSegNet(BayesianSegNetParams(proto, model), seed=1234, T=T)
     bounds = (0.0, float(NET_W), 0.0, float(NET_H))
     frame0 = make_frame(FX, FX, CX, CY, MBF, bounds, rotation(0.001, -0.0015, 0.001), (0.01, -0.005, 0.01))
     T0 = np.concatenate([np.array(frame0.Rcw, np.float32).reshape(3, 3), np.array(frame0.tcw, np.float32)[:, None]], 1)
-    fr = frames(6)
-    B = []
-    for f in fr:
-        B.append({"in": [torch.from_numpy(np.ascontiguousarray(f[0][CROP_Y:CROP_Y + NET_H, CROP_X:CROP_X + NET_W])).to(dev), torch.from_numpy(f[1]).to(dev),
-                         torch.from_numpy(f[2]).to(dev)],
-                  "f": DeviceFrame(el, er, NET_H, NET_W), "m1": torch.empty(cap, dtype=i32, device=dev),
-                  "m2": torch.empty(cap, dtype=i32, device=dev), "nm": torch.empty(2, dtype=i64, device=dev),
-                  "view": torch.empty(cap, dtype=u8, device=dev), "xw": torch.empty(3 * cap, dtype=f32, device=dev),
-                  "T0": torch.from_numpy(T0.reshape(-1).copy()).to(dev), "r1": torch.empty(512, dtype=u8, device=dev),
-                  "r2": torch.empty(512, dtype=u8, device=dev), "o": torch.empty(cap, dtype=u8, device=dev),
-                  "r1_host": torch.empty(512, dtype=u8, pin_memory=True), "ev": torch.cuda.Event()})
-    torch.cuda.synchronize(dev)
+    B = [{"in": f, "f": DeviceFrame(el, er, NET_H, NET_W), "m1": torch.empty(cap, dtype=i32, device="cuda"),
+          "m2": torch.empty(cap, dtype=i32, device="cuda"), "nm": torch.empty(2, dtype=i64, device="cuda"),
+          "view": torch.empty(cap, dtype=u8, device="cuda"), "xw": torch.empty(3 * cap, dtype=f32, device="cuda"),
+          "T0": torch.from_numpy(T0.reshape(-1).copy()).cuda(), "r1": torch.empty(512, dtype=u8, device="cuda"),
+          "r2": torch.empty(512, dtype=u8, device="cuda"), "o": torch.empty(cap, dtype=u8, device="cuda"),
+          "r1_host": torch.empty(512, dtype=u8, pin_memory=True)} for f in chain_frames(6)]
+    torch.cuda.synchronize()
 
     def front(b):
         b["f"].extract(seg, *b["in"], s)  # the extractors first wait for the previous step's searches and optimisations
@@ -166,6 +135,7 @@ def run(args):
                              b["o"].data_ptr(), s)
 
     def step(b, with_pose):
+        nonlocal last_pose
         front(b)
         last_search(b)
         if with_pose:
@@ -180,58 +150,28 @@ def run(args):
             local_search(b, frame)
             pose_gather_device(el, b["m2"].data_ptr(), b["f"].n_keep, b["local"].data_ptr(), b["n_local"], b["xw"].data_ptr(), s)
             pose(b, b["r1"], b["r2"])
+            last_pose = b
         else:
             local_search(b, frame0)
-        b["ev"].record(stream)
 
+    last_pose = None
     for b in B:  # first pass: the network's graph is captured, and each frame's keys give its map
         front(b)
         stream.synchronize()
         _, kidx, _, depth = b["f"].host()
         kps, desc = (a[kidx] for a in b["f"].left.host())
         last, local = frame_map(kps, desc, depth, el.GetScaleFactors(), rng)
-        b["last"], b["local"] = (torch.from_numpy(p.view(np.uint8).reshape(-1).copy()).to(dev) for p in (last, local))
+        b["last"], b["local"] = (torch.from_numpy(p.view(np.uint8).reshape(-1).copy()).cuda() for p in (last, local))
         b["n_last"], b["n_local"] = len(last), len(local)
-    torch.cuda.synchronize(dev)
-    fps_blocks = {"without_pose": [], "with_two_poses": []}
-    total = {k: [0, 0.0] for k in fps_blocks}
-    n_blocks = max(1, -(-(args.warmup + args.steps) // args.blocks_of))
-    i = 0
-    gc.collect()
-    gc.disable()
-    for blk in range(n_blocks + 2):
-        for name in (("without_pose", "with_two_poses") if blk % 2 == 0 else ("with_two_poses", "without_pose")):
-            torch.cuda.synchronize(dev)
-            t0 = time.perf_counter()
-            for _ in range(args.blocks_of):
-                step(B[i % len(B)], name == "with_two_poses")
-                if (i & 3) == 3:
-                    B[(i - 1) % len(B)]["ev"].synchronize()
-                i += 1
-            torch.cuda.synchronize(dev)
-            dt = time.perf_counter() - t0
-            if blk >= 2:
-                fps_blocks[name].append(args.blocks_of / dt)
-                total[name][0] += args.blocks_of
-                total[name][1] += dt
-    gc.enable()
-    if el.device_status() or er.device_status():
-        raise SystemExit("a pyramid level exceeded the device quad tree's capacity: the asynchronous outputs are not valid")
-    r2 = result_from_bytes(B[(i - 1) % len(B)]["r2"].cpu().numpy())
+    torch.cuda.synchronize()
+    fps = alternate({"without_pose": lambda i, k: step(B[k], False), "with_two_poses": lambda i, k: step(B[k], True)}, stream, args.steps,
+                    args.warmup, args.blocks_of, len(B))
+    check_device_trees(el, er)
+    r2 = result_from_bytes(last_pose["r2"].cpu().numpy())
 
-    gpu, power = torch.cuda.get_device_name(dev), None
-    try:
-        import pynvml
-        pynvml.nvmlInit()
-        power = pynvml.nvmlDeviceGetEnforcedPowerLimit(pynvml.nvmlDeviceGetHandleByIndex(0)) / 1e3
-    except Exception:
-        pass
-    line = {"metric": "pose optimisation", "unit": "ms", "calls": calls,
-            "chain_fps": {name: {"overall": total[name][0] / total[name][1], "median_block": med(fps_blocks[name]),
-                                 "frames": total[name][0]} for name in fps_blocks},
+    line = {"metric": "pose optimisation", "unit": "ms", "calls": calls, "chain_fps": fps,
             "chain_last_second_optimisation": {"n_initial": int(r2.n_initial), "n_good": int(r2.n_good), "sigma_valid": int(r2.sigma_valid)},
-            "g2o_host_loop": "not measured (Eigen + CHOLMOD are not built here)", "calls_timed": args.steps, "warmup": args.warmup,
-            "gpu": gpu, "power_limit_w": power,
+            "g2o_host_loop": "not measured (Eigen + CHOLMOD are not built here)", "calls_timed": args.steps, "warmup": args.warmup, **card(),
             "workload": f"(a, b) synthetic scenes, 60 % stereo; (c) Bayesian SegNet Basic T={T} + ORB({args.nfeatures}) x2 + semantic keys + "
                         "stereo + last-frame search (th 7) + local-map search (th 1), with / without gather + pose after each search, "
                         "synthetic 1024x352 frames"}
@@ -240,13 +180,9 @@ def run(args):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--steps", type=int, default=30, help="timed calls / frames per measurement")
-    ap.add_argument("--warmup", type=int, default=5)
-    ap.add_argument("--blocks-of", type=int, default=10, help="frames per alternating block of the chain legs")
-    ap.add_argument("--nfeatures", type=int, default=2000)
+    add_common_args(ap, steps=30, warmup=5, chain=True)
     args = ap.parse_args()
-    if args.steps < 1 or args.blocks_of < 1:
-        ap.error("--steps and --blocks-of must be at least 1")
+    require_cuda("pose_bench.py")
     run(args)
 
 

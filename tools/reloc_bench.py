@@ -1,20 +1,21 @@
 """Times Relocalization's PnP RANSAC on the device: sivo_pnp_setup_device and one sivo_pnp_iterate_device(5) call (the first
 round of Tracking::Relocalization's loop) over 1 / 8 / 32 / 64 candidates x 15 / 200 / 2,000 correspondences each, 30 % outliers.
-Each repetition re-runs setup, which resets the state, so every timed iterate is a first round.  CUDA events around the calls,
-median of --reps.  Prints one JSON line per configuration with the card's name and power limit; writes nothing."""
+Each repetition re-runs setup, which resets the state, so every timed iterate is a first round.  Three CUDA events
+per repetition, around setup and around the iterate, median / p90 in ms over --steps repetitions after --warmup.  Prints one JSON
+line per configuration with the card's name and power limit read in the same run (DESIGN.md §7); writes nothing.
+
+    python tools/reloc_bench.py [--steps 30] [--warmup 3]
+"""
 import argparse
 import json
-import os
-import subprocess
-import sys
 
 import numpy as np
 import torch
 
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
-from sivo_b200 import reloc  # noqa: E402
-from sivo_b200.orb import KP_DTYPE, ORBextractor  # noqa: E402
-from sivo_b200.track import map_points  # noqa: E402
+from bench_support import add_common_args, card, require_cuda, stats  # puts the repository on sys.path
+from sivo_b200 import reloc
+from sivo_b200.orb import KP_DTYPE, ORBextractor
+from sivo_b200.track import map_points
 
 FX, FY, CX, CY = 718.856, 718.856, 607.1928, 185.2157
 
@@ -38,10 +39,10 @@ def scene(left, n_kf, N, outliers, seed):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--reps", type=int, default=30)
+    add_common_args(ap, steps=30, warmup=3)
     args = ap.parse_args()
-    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                          text=True).stdout.strip().splitlines()[0]
+    require_cuda("reloc_bench.py")
+    gpu = card()
     left = ORBextractor(2000, 1.2, 8, 20, 7)
     dev = torch.device("cuda")
     stream = torch.cuda.Stream()
@@ -60,7 +61,7 @@ def main():
             ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
             setup_ms, iter_ms = [], []
             torch.cuda.synchronize()
-            for rep in range(args.reps + 3):
+            for rep in range(args.warmup + args.steps):
                 s = stream.cuda_stream
                 ev[0].record(stream)
                 solver.setup_device(t[0].data_ptr(), 0, t[1].data_ptr(), t[2].data_ptr(), t[3].data_ptr(), t[4].data_ptr(), len(pts), ids,
@@ -70,12 +71,12 @@ def main():
                                       outs[2].data_ptr(), s)
                 ev[2].record(stream)
                 stream.synchronize()
-                if rep >= 3:
+                if rep >= args.warmup:
                     setup_ms.append(ev[0].elapsed_time(ev[1]))
                     iter_ms.append(ev[1].elapsed_time(ev[2]))
             solver.close()
-            print(json.dumps({"candidates": n_kf, "correspondences": N, "outliers": 0.3, "setup_ms": float(np.median(setup_ms)),
-                              "iterate5_ms": float(np.median(iter_ms)), "poses": int(outs[0].sum().item()), "card": card}), flush=True)
+            print(json.dumps({"candidates": n_kf, "correspondences": N, "outliers": 0.3, "unit": "ms", "setup_ms": stats(setup_ms),
+                              "iterate5_ms": stats(iter_ms), "poses": int(outs[0].sum().item()), **gpu}), flush=True)
 
 
 if __name__ == "__main__":
