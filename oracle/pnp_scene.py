@@ -4,9 +4,9 @@ per-hypothesis log, so a test can check both that a scene still reaches what it 
 every path in PATHS.
 
 A scene is one candidate's correspondences (p2d, p3d, octave) with its draw keys (seed, kf_id, frame_id) and a schedule of
-iterate(n) calls.  `embed` lays it out as sivo_pnp_setup_device's inputs: semantic keys in order, a permuted keep_idx into the
-extractor's slots, a match row into a permuted point array, and (optionally) rejected entries of every kind in between, so that
-the setup's compaction must return exactly the scene's correspondences.
+iterate(n) calls.  `embed` lays it out as sivo_pnp_setup_device's inputs: semantic keys in order, an oracle/keymap.py keep_idx
+into the extractor's slots, a match row into a permuted point array, and (optionally) rejected entries of every kind in
+between, so that the setup's compaction must return exactly the scene's correspondences.
 
   placed      every observation is computed from the pose it must agree with, in CheckInliers' own arithmetic: exact (error
               below 1e-3 px), at a chosen multiple of the threshold, or far off.  The hypothesis draws depend only on (seed,
@@ -25,7 +25,9 @@ from dataclasses import dataclass, field
 import numpy as np
 
 from oracle import pnp_oracle as P
+from oracle.keymap import SLACK, keymap, scatter
 from oracle.orb_oracle import ExtractorParams, Tables
+from sivo_b200.orb import KP_DTYPE
 
 F32, F64 = np.float32, np.float64
 KITTI = (718.856, 718.856, 607.1928, 185.2157)
@@ -309,70 +311,52 @@ class Frame:
     paths: set
 
 
-KP_DTYPE = np.dtype([("x", "<f4"), ("y", "<f4"), ("size", "<f4"), ("angle", "<f4"), ("response", "<f4"), ("octave", "<i4"),
-                     ("class_id", "<i4")])
-SLACK = 64
+REJECTS = ("keep_neg", "keep_cap", "match_neg5", "match_neg1", "match_np", "match_np1", "oct_neg", "oct_nlevels", "oct_127")
+FORCED = (255, 256, 511, 512)  # semantic keys whose entry is rejected: both sides of the 256-key chunk boundaries
 
 
 def embed(scene: Scene, cap: int, nlevels: int, rng, junk=None) -> Frame:
-    """sivo_pnp_setup_device's inputs for the scene: semantic key j's correspondences in order through a permuted keep_idx and
-    a permuted point array, with rejected keys between them (junk): keep_idx -1 and >= cap, match -5, -1, n_points and n_points
-    + 1, octaves -1, nlevels and 127, some at semantic keys 255, 256, 511 and 512.  Slack rows past cap, n_keep and n_points
-    hold keys and points that would be accepted if a bound were off by one."""
+    """sivo_pnp_setup_device's inputs for the scene: semantic key j's correspondences in order through an oracle/keymap.py map
+    and a permuted point array, with rejected keys between them (junk), some at semantic keys 255, 256, 511 and 512.  The
+    rejected entries cycle through REJECTS: the map's own rejected keep_idx (keep_neg or keep_cap by its sign), or a valid
+    slot whose match is -5, -1, n_points or n_points + 1 or whose key's octave is -1, nlevels or 127.  Slack rows past cap,
+    n_keep and n_points hold keys and points that would be accepted if a bound were off by one."""
     junk = scene.junk if junk is None else junk
     N = scene.N
-    kinds = ["keep_neg", "keep_cap", "match_neg5", "match_neg1", "match_np", "match_np1", "oct_neg", "oct_nlevels", "oct_127"]
-    n_junk = 0
-    if junk:
-        n_junk = min(cap - N, max(len(kinds), (cap - N) // 8 if N > 200 else 24))
-    n_keep = N + n_junk
-    assert n_keep <= cap, "the scene does not fit the capacity"
-    is_junk = np.zeros(n_keep, bool)
-    if n_junk:
-        forced = [j for j in (255, 256, 511, 512) if j < n_keep][:n_junk]
-        rest = rng.permutation(np.setdiff1d(np.arange(n_keep), forced))[:n_junk - len(forced)]
-        is_junk[forced] = True
-        is_junk[rest] = True
+    km = keymap(N, cap, rng, forced=FORCED, junk=junk)
+    n_keep, keep = km.n_keep, km.keep
     n_points = N + 7
     perm_pts = rng.permutation(n_points)
     points = np.zeros((n_points + SLACK, 3), F32)
     points[n_points:] = [1.0, 2.0, 10.0]  # slack: a point a bound one too wide would read
-    slots = rng.permutation(cap)
-    kps = np.zeros(cap + SLACK, KP_DTYPE)
+    points[perm_pts[:N]] = scene.p3d
+    points[perm_pts[N:]] = [3.0, -1.0, 20.0]
+    p2 = np.asarray(scene.p2d, F32).reshape(N, 2)
+    real = np.zeros(N, KP_DTYPE)
+    real["x"], real["y"], real["octave"] = p2[:, 0], p2[:, 1], scene.octave
+    kps = scatter(real, km.slots, cap, np.zeros(1, KP_DTYPE))
     kps["x"][cap:], kps["y"][cap:], kps["octave"][cap:] = 600.0, 180.0, 0  # slack: a key a bound one too wide would read
-    # keep_idx is read for every semantic key below min(*n_keep, cap), and a test may raise *n_keep to the capacity: cap + SLACK
-    # entries, those past n_keep valid slots (their match entries are -1, so a correct setup rejects them)
-    keep = np.zeros(max(n_keep, cap) + SLACK, np.int32)
-    keep[n_keep:] = slots[np.arange(len(keep) - n_keep) % cap]
+    # keep's entries past n_keep are valid slots, whose match entries are -1: a correct setup rejects them
     match = np.full(cap + SLACK, -1, np.int32)
     match[cap:] = 0
+    match[km.real] = perm_pts[:N]
+    free = np.setdiff1d(np.arange(cap), km.slots)
     paths = {"keep_permuted"} if cap > 1 else set()
-    c = 0
-    for j in range(n_keep):
-        keep[j] = slots[j]
-        if not is_junk[j]:
-            kps[slots[j]]["x"], kps[slots[j]]["y"] = scene.p2d[c]
-            kps[slots[j]]["octave"] = scene.octave[c]
-            points[perm_pts[c]] = scene.p3d[c]
-            match[j] = perm_pts[c]
-            c += 1
-            continue
-        kind = kinds[int(rng.integers(len(kinds)))] if j not in (255, 256, 511, 512) else kinds[(j + len(paths)) % len(kinds)]
-        kps[slots[j]]["x"], kps[slots[j]]["y"], kps[slots[j]]["octave"] = 600.0, 180.0, 0
+    for r, j in enumerate(np.flatnonzero(km.src < 0)):
+        kind = REJECTS[r % len(REJECTS)]
         match[j] = perm_pts[N + int(rng.integers(7))]
-        if kind == "keep_neg":
-            keep[j] = -1
-        elif kind == "keep_cap":
-            keep[j] = cap
-        elif kind.startswith("match"):
-            match[j] = {"match_neg5": -5, "match_neg1": -1, "match_np": n_points, "match_np1": n_points + 1}[kind]
+        if kind.startswith("keep"):
+            kind = "keep_neg" if keep[j] < 0 else "keep_cap"
         else:
-            kps[slots[j]]["octave"] = {"oct_neg": -1, "oct_nlevels": nlevels, "oct_127": 127}[kind]
+            keep[j] = s = free[r]
+            kps[s]["x"], kps[s]["y"], kps[s]["octave"] = 600.0, 180.0, 0
+            if kind.startswith("match"):
+                match[j] = {"match_neg5": -5, "match_neg1": -1, "match_np": n_points, "match_np1": n_points + 1}[kind]
+            else:
+                kps[s]["octave"] = {"oct_neg": -1, "oct_nlevels": nlevels, "oct_127": 127}[kind]
         paths.add(kind)
-        if j in (255, 256, 511, 512):
+        if j in FORCED:
             paths.add(f"reject_{j}")
-    points[perm_pts[N:]] = [3.0, -1.0, 20.0]
-    assert c == N
     return Frame(kps, keep, n_keep, match, points, n_points, paths)
 
 

@@ -12,6 +12,9 @@ both that a scene still reaches what it was built for and that the scenes togeth
   counts      3, 9, 10 and 11 edges; mono-only and stereo-only frames; every stereo edge gross, so rounds 1 - 3 have no edge; every
               point on the camera plane, so every edge is invalid.
   extremes    large finite intrinsics and near-zero depths (chi2 near 1e107, lambda near 1e238).
+
+Also the seeded frames of the pose tests (`scene`, and `exact_scene` at the identity), and `embed`, which lays a frame out per
+entry of a semantic-key map (oracle/keymap.py) for the device form.
 """
 from __future__ import annotations
 
@@ -19,14 +22,15 @@ import math
 from dataclasses import dataclass, field
 
 import numpy as np
+from scipy.linalg import expm
 
 from oracle import pose_oracle as P
+from sivo_b200.orb import KP_DTYPE
 
 F32, F64 = np.float32, np.float64
-KP_DTYPE = np.dtype([("x", "<f4"), ("y", "<f4"), ("size", "<f4"), ("angle", "<f4"), ("response", "<f4"), ("octave", "<i4"),
-                     ("class_id", "<i4")])
 INV_SIGMA2 = (F32(1) / np.array([F32(1.2 ** (2 * l)) for l in range(8)], F32)).astype(F32)  # ORBextractor(.., 1.2, 8, ..)
 KITTI = (718.856, 718.856, 498.1928, 174.2157, 386.1448)
+CAM = P.Camera(*KITTI)
 EXACT = (512.0, 512.0, 0.0, 0.0, 256.0)  # the fixed-point scenes' camera: cx = cy = 0, so a point on the axis projects to 0
 DSQR_MONO, DSQR_STEREO = P.DELTA_MONO * P.DELTA_MONO, P.DELTA_STEREO * P.DELTA_STEREO
 
@@ -89,6 +93,70 @@ def posed_scene(seed, R, C, n=120, mode="mixed", noise=0.5, outliers=0.0, motion
     dR = axis_rotation(rng.standard_normal(3), rng.uniform(0, motion[0]))
     dt = rng.uniform(-motion[1], motion[1], 3)
     return kps, ur, X, pose34(dR @ R, t + dt)
+
+
+# ---------------------------------------------------------------------------------------------------------- seeded frames
+def rotation(ax, ay, az):
+    return expm(np.array([[0, -az, ay], [az, 0, -ax], [-ay, ax, 0]], float))
+
+
+def scene(seed, n=300, mode="mixed", outliers=0.0, noise=0.5, motion=(0.01, 0.05), cam=CAM, size=(1024, 352)):
+    """A frame seen from a true pose: keys at random pixels and depths, their points placed in the world exactly, pixel noise
+    (sigma `noise` times the octave's scale), a fraction of the points replaced by gross outliers, and an initial pose moved by
+    `motion` (rotation rad, translation m).  mode: "mono" (u_right < 0), "stereo" or "mixed".  Returns (kps, u_right, xw,
+    Tcw_in, Tcw_true)."""
+    rng = np.random.default_rng(seed)
+    R = rotation(*rng.uniform(-0.2, 0.2, 3))
+    t = rng.uniform(-2, 2, 3)
+    u = rng.uniform(0, size[0], n)
+    v = rng.uniform(0, size[1], n)
+    z = rng.uniform(3, 40, n)
+    Pc = np.stack([(u - cam.cx) * z / cam.fx, (v - cam.cy) * z / cam.fy, z], 1)
+    X = ((Pc - t) @ R).astype(F32)
+    oct_ = rng.integers(0, 8, n)
+    sc = 1.2 ** oct_
+    kps = np.zeros(n, KP_DTYPE)
+    kps["x"] = u + noise * sc * rng.standard_normal(n)
+    kps["y"] = v + noise * sc * rng.standard_normal(n)
+    kps["octave"] = oct_
+    ur = (u - cam.mbf / z + noise * sc * rng.standard_normal(n)).astype(F32)
+    stereo = {"mono": np.zeros(n, bool), "stereo": np.ones(n, bool), "mixed": rng.uniform(size=n) < 0.6}[mode]
+    ur = np.where(stereo, np.maximum(ur, F32(0)), F32(-1)).astype(F32)
+    bad = rng.permutation(n)[:int(round(outliers * n))]
+    X[bad] = (X[bad] + rng.uniform(-5, 5, (len(bad), 3))).astype(F32)
+    dR = rotation(*rng.uniform(-motion[0], motion[0], 3))
+    dt = rng.uniform(-motion[1], motion[1], 3)
+    return kps, ur, X, pose34(dR @ R, t + dt), pose34(R, t)
+
+
+def exact_scene(mode):
+    """Observations that are exact floats of exact projections at the identity pose (fx = 512, power-of-two depths), so the
+    optimum is the identity."""
+    cam = P.Camera(512.0, 512.0, 320.0, 240.0, 256.0)
+    rng = np.random.default_rng(7)
+    n = 64
+    z = 2.0 ** rng.integers(1, 5, n)
+    x = rng.integers(-200, 200, n) / 64.0
+    y = rng.integers(-150, 150, n) / 64.0
+    kps = np.zeros(n, KP_DTYPE)
+    kps["x"] = (x / z) * 512 + 320
+    kps["y"] = (y / z) * 512 + 240
+    kps["octave"] = rng.integers(0, 8, n)
+    ur = (kps["x"] - 256 / z).astype(F32)
+    if mode == "mono":
+        ur[:] = -1
+    elif mode == "mixed":
+        ur[::3] = -1
+    X = np.stack([x, y, z], 1).astype(F32)
+    return cam, kps, ur, X
+
+
+def embed(km, kps, ur, X):
+    """Keys, u_right and points per entry of the map km (oracle/keymap.py): the real keys at their entries; a rejected entry holds
+    a point but no key, so it has no edge."""
+    K, U, W = np.zeros(km.n_keep, KP_DTYPE), np.zeros(km.n_keep, F32), np.ones((km.n_keep, 3), F32)
+    K[km.real], U[km.real], W[km.real] = kps, ur, X
+    return K, U, W
 
 
 # ---------------------------------------------------------------------------------------------------------- fixed points

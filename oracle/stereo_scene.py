@@ -15,10 +15,7 @@ from dataclasses import dataclass, field
 import numpy as np
 
 from oracle import orb_oracle as O
-
-# the record layout of sivo_keypoint (sivo_b200.orb.KP_DTYPE), restated so that the oracle does not import the product
-KP = np.dtype([("x", "<f4"), ("y", "<f4"), ("size", "<f4"), ("angle", "<f4"), ("response", "<f4"), ("octave", "<i4"),
-               ("class_id", "<i4")])
+from sivo_b200.orb import KP_DTYPE as KP
 ROWS, COLS = 240, 480
 f32 = np.float32
 

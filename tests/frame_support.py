@@ -1,6 +1,7 @@
 """What the GPU suites of the Frame tail share: the network's crop of a KITTI frame and its camera, synthetic stereo frames, the
-extractor pair, the Basic T=2 SegNet fixture, and one frame's front end and tail on the device (Tail).  A plain module the
-tests import, not a test module."""
+extractor pair and one cached extractor per parameter set, the Basic T=2 SegNet fixture, one frame's front end and tail on the
+device (Tail), and the device-test helpers (upload, sentinel outputs, int64 counts, bit equality).  A plain module the tests
+import, not a test module."""
 import os
 
 import numpy as np
@@ -10,7 +11,7 @@ import torch
 from oracle import info_oracle as I
 from oracle import pose_oracle as P
 from oracle.mapping_scene import rotation
-from sivo_b200 import BayesianSegNet, BayesianSegNetParams, ORBextractor, info_select_device, make_camera, stereo_match_device
+from sivo_b200 import BayesianSegNet, BayesianSegNetParams, KP_DTYPE, ORBextractor, info_select_device, make_camera, stereo_match_device
 from sivo_b200.frame import DeviceFrame
 from sivo_b200.synth import bgr_to_gray, stereo_frame
 
@@ -66,6 +67,35 @@ def upload(a):
     return t
 
 
+def sentinel(n, fill, dtype):
+    """n device entries at a sentinel value (one an output that was not written keeps), set before anything else is enqueued."""
+    t = torch.full((n,), fill, dtype=dtype, device="cuda")
+    torch.cuda.synchronize()
+    return t
+
+
+def i64(v):
+    """A device count (int64)."""
+    return sentinel(1, v, torch.int64)
+
+
+def same_bits(a, b):
+    """The same shape and the same bits, except that a NaN matches any NaN (the device's default NaN is not numpy's); 0.0 and
+    -0.0 differ.  Float values compare as float64, which keeps both."""
+    a, b = np.asarray(a), np.asarray(b)
+    if a.shape != b.shape:
+        return False
+    if a.dtype.kind != "f" and b.dtype.kind != "f":
+        return np.array_equal(a, b)
+    a, b = a.astype(np.float64), b.astype(np.float64)
+    return bool(((a.view(np.int64) == b.view(np.int64)) | (np.isnan(a) & np.isnan(b))).all())
+
+
+# a keyframe's per-key arrays (sivo_keyframe_keys) and their device layouts
+KF_FIELDS = {"kps": KP_DTYPE, "desc": np.uint8, "u_right": np.float32, "depth": np.float32, "kp_class": np.uint8, "kp_conf": np.float64,
+             "kp_entropy": np.float64, "node": np.int32, "has_point": np.uint8}
+
+
 def kp_matrix(kps):
     """Keypoint records as a float32 matrix of their seven fields, the layout of the golden files and the oracle."""
     return np.stack([kps["x"], kps["y"], kps["size"], kps["angle"], kps["response"], kps["octave"].astype(np.float32),
@@ -74,6 +104,17 @@ def kp_matrix(kps):
 
 def extractors(nf, nlevels=8):
     return ORBextractor(nf, 1.2, nlevels, 20, 7), ORBextractor(nf, 1.2, nlevels, 20, 7)
+
+
+_EXTRACTORS = {}
+
+
+def extractor(nfeatures=2000, scale_factor=1.2, nlevels=8, right=False):
+    """The process's one extractor of these parameters (right: a second one, the right side of a stereo pair)."""
+    key = (nfeatures, scale_factor, nlevels, right)
+    if key not in _EXTRACTORS:
+        _EXTRACTORS[key] = ORBextractor(nfeatures, scale_factor, nlevels, 20, 7)
+    return _EXTRACTORS[key]
 
 
 @pytest.fixture(scope="module")

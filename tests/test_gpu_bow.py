@@ -9,6 +9,7 @@ import torch
 from frame_support import extractors, upload
 from oracle import bow_oracle as B
 from oracle import bow_scene as S
+from oracle.keymap import keymap
 from sivo_b200 import _lib as L
 from sivo_b200.bow import Vocabulary, compute_bow, compute_bow_device, keyframe_keys, search_by_bow, search_by_bow_device
 from sivo_b200.orb import KP_DTYPE
@@ -120,13 +121,11 @@ def test_transform_edges_and_errors(ext, irregular):
     neg = device_bow(voc, el, desc, 4, count=-1)
     assert int(neg["len"][0]) == -1 and (neg["node"] == -7).all() and (neg["bwt"] == 7.0).all()
     # keep_idx: negative and out-of-capacity entries give -1, the rest take the extractor key
-    rng = np.random.default_rng(3)
-    n = 600
-    keep = rng.integers(0, cap, n).astype(np.int32)
-    keep[::7] = -1
-    keep[3::11] = cap + 5
-    k = device_bow(voc, el, desc, 4, keep=keep, count=n)
-    valid = (keep >= 0) & (keep < cap)
+    km = keymap(600, cap, np.random.default_rng(3), duplicates=True)
+    n = km.n_keep
+    keep = km.keep[:n]
+    k = device_bow(voc, el, desc, 4, keep=km.keep, count=n)
+    valid = km.src >= 0
     b2, _, node2, word2 = B.transform(tree, desc[np.where(valid, keep, 0)], 4)
     np.testing.assert_array_equal(k["node"][:n], np.where(valid, node2, -1))
     np.testing.assert_array_equal(k["word"][:n], np.where(valid, word2, -1))

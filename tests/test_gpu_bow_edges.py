@@ -4,35 +4,30 @@ descents through nodes of 40 children with ties across the lanes' two strides, w
 compared by position), key counts across the warp, block and power-of-two boundaries of the BowVector sort and at the 16,384-key
 capacity, frame runs at exact sorted positions, nodes 0 and 2^31 - 1, batches of 63-200 keyframes (later launches) with negative,
 zero and above-capacity counts, every NULL output combination of sivo_compute_bow_device, the capacity limits and 200 seeded fuzz
-scenes.  Every device call passes a permuted semantic-key map holding rejected (-1, capacity, past-capacity) and duplicate
-entries, and every buffer carries slack rows past its bound that a bound one too wide would read or write."""
+scenes.  Every device call passes an oracle/keymap.py semantic-key map holding rejected and duplicate entries, and every
+buffer carries slack rows past its bound that a bound one too wide would read or write."""
 import zlib
 
 import numpy as np
 import pytest
 import torch
 
-from frame_support import upload
+from frame_support import extractor, i64, same_bits, sentinel, upload
 from oracle import bow_oracle as B
 from oracle import bow_scene as S
+from oracle.keymap import SLACK, keymap, scatter
 from sivo_b200 import _lib as L
 from sivo_b200.bow import Vocabulary, compute_bow, compute_bow_device, keyframe_keys, search_by_bow, search_by_bow_device
 from sivo_b200.orb import KP_DTYPE, ORBextractor
 
 pytestmark = pytest.mark.gpu
-SLACK = 64
+FORCED = (0, 31, 32, -1)  # semantic keys whose entry is rejected: the first, both sides of a warp boundary, the last
 TRANSFORM = {c.name: c for c in S.transform_cases()}
 SEARCH = {c.name: c for c in S.search_cases()}
-_EXT, _VOC = {}, {}
+_VOC = {}
 
 
-def extractor(nfeatures=2000):
-    if nfeatures not in _EXT:
-        _EXT[nfeatures] = ORBextractor(nfeatures, 1.2, 8, 20, 7)
-    return _EXT[nfeatures]
-
-
-def extractor_for(n):
+def el_for(n):
     """The 2,000-feature extractor (capacity 2,096) when n keys and the rejected entries fit, else the 16,384-key one."""
     return extractor(2000) if n + 32 <= extractor(2000).capacity() else extractor(16288)
 
@@ -48,52 +43,8 @@ def case_rng(name):
     return np.random.default_rng(zlib.crc32(name.encode()))
 
 
-def same_f64(got, want):
-    """Bit for bit, except that a NaN matches a NaN (the device's default NaN is not numpy's)."""
-    got, want = np.asarray(got, np.float64), np.asarray(want, np.float64)
-    assert got.shape == want.shape
-    np.testing.assert_array_equal(np.isnan(got), np.isnan(want))
-    ok = ~np.isnan(want)
-    np.testing.assert_array_equal(got[ok].view(np.uint64), want[ok].view(np.uint64))
-
-
 def clamp(count, cap):
     return min(count, cap)
-
-
-# ---------------------------------------------------------------------------------------------------------- the embedding
-def embed(n, cap, rng, junk=True):
-    """Semantic key j -> an extractor slot: the n keys in order on a permutation of the slots, with rejected entries between them
-    (keep_idx -1, cap and cap + 7) and duplicates of earlier keys' slots.  Returns (keep, n_keep, src, dup, slots): src[j] is the
-    key whose slot entry j reads (-1: rejected), dup[j] marks the duplicates; keep has max(n_keep, cap) + SLACK entries, those
-    past n_keep valid slots."""
-    n_junk = max(0, min(cap - n, max(12, (cap - n) // 8))) if junk else 0
-    n_keep = n + n_junk
-    is_junk = np.zeros(n_keep, bool)
-    if n_junk:
-        forced = [j for j in (0, 31, 32, n_keep - 1) if j < n_keep][:n_junk]
-        rest = rng.permutation(np.setdiff1d(np.arange(n_keep), forced))[:n_junk - len(forced)]
-        is_junk[forced] = True
-        is_junk[rest] = True
-    slots = rng.permutation(cap)
-    keep = np.zeros(max(n_keep, cap) + SLACK, np.int32)
-    keep[n_keep:] = slots[rng.integers(0, cap, len(keep) - n_keep)]
-    src = np.full(n_keep, -1, np.int64)
-    dup = np.zeros(n_keep, bool)
-    c = 0
-    for j in range(n_keep):
-        if not is_junk[j]:
-            keep[j], src[j] = slots[c], c
-            c += 1
-            continue
-        kind = (j * 7 + c) % 4
-        if kind == 3 and c > 0:
-            i = int(rng.integers(c))
-            keep[j], src[j], dup[j] = slots[i], i, True  # a second semantic key on the same extractor key
-        else:
-            keep[j] = (-1, cap, cap + 7, -1)[kind]
-    assert c == n
-    return keep, n_keep, src, dup, slots[:n]
 
 
 def gathered(keep, count, cap):
@@ -108,13 +59,9 @@ def gathered(keep, count, cap):
 def device_bow(voc, el, slot_desc, keep, count, levelsup, want=(True,) * 5):
     """sivo_compute_bow_device with every output at capacity + SLACK (sentinels -7 / 7.0) or NULL where want is False."""
     cap = el.capacity()
-    t = [upload(slot_desc), upload(keep), upload(np.array([count], np.int64))]
-    out = dict(node=torch.full((cap + SLACK,), -7, dtype=torch.int32, device="cuda"),
-               word=torch.full((cap + SLACK,), -7, dtype=torch.int32, device="cuda"),
-               bw=torch.full((cap + SLACK,), -7, dtype=torch.int32, device="cuda"),
-               bwt=torch.full((cap + SLACK,), 7.0, dtype=torch.float64, device="cuda"),
-               len=torch.full((2,), -7, dtype=torch.int64, device="cuda"))
-    torch.cuda.synchronize()
+    t = [upload(slot_desc), upload(keep), i64(count)]
+    out = dict(node=sentinel(cap + SLACK, -7, torch.int32), word=sentinel(cap + SLACK, -7, torch.int32),
+               bw=sentinel(cap + SLACK, -7, torch.int32), bwt=sentinel(cap + SLACK, 7.0, torch.float64), len=sentinel(2, -7, torch.int64))
     ptrs = [v.data_ptr() if w else 0 for v, w in zip(out.values(), want)]
     compute_bow_device(voc, el, t[0].data_ptr(), t[1].data_ptr(), t[2].data_ptr(), levelsup, *ptrs)
     torch.cuda.synchronize()
@@ -122,12 +69,11 @@ def device_bow(voc, el, slot_desc, keep, count, levelsup, want=(True,) * 5):
 
 
 def transform_setup(case_desc, cap, rng, junk):
-    keep, n_keep, _, _, slots = embed(len(case_desc), cap, rng, junk)
-    slot_desc = rng.integers(0, 256, (cap + SLACK, 32), dtype=np.uint8)
-    slot_desc[slots] = case_desc
+    km = keymap(len(case_desc), cap, rng, FORCED, duplicates=True, junk=junk)
+    slot_desc = scatter(case_desc, km.slots, cap, rng.integers(0, 256, (cap + SLACK, 32), dtype=np.uint8))
     if len(case_desc):
         slot_desc[cap:] = case_desc[0]  # a key a bound one too wide would read
-    return slot_desc, keep, n_keep
+    return slot_desc, km.keep, km.n_keep
 
 
 def transform_want(tree, slot_desc, keep, count, cap, levelsup, same_as=None):
@@ -154,7 +100,7 @@ def check_device_bow(d, want, cap, want_mask=(True,) * 5):
             continue
         upto = m if k in ("node", "word") else n_bow
         if k == "bwt":
-            same_f64(got[:upto], w)
+            assert same_bits(got[:upto], w), k
         else:
             np.testing.assert_array_equal(got[:upto], w, err_msg=k)
         assert (got[upto:] == sentinel).all(), k
@@ -174,8 +120,8 @@ def test_transform_case(name):
     np.testing.assert_array_equal(h["node"], node)
     np.testing.assert_array_equal(h["word"], word)
     np.testing.assert_array_equal(h["bow_words"], words)
-    same_f64(h["bow_weights"], vals)
-    el = extractor_for(len(case.desc))
+    assert same_bits(h["bow_weights"], vals)
+    el = el_for(len(case.desc))
     cap = el.capacity()
     slot_desc, keep, n_keep = transform_setup(case.desc, cap, case_rng(name), case.junk)
     want = transform_want(tree, slot_desc, keep, n_keep, cap, case.levelsup, same_as=(bow, fv, node, word, case.desc))
@@ -211,12 +157,13 @@ class DeviceFrame:
     def __init__(self, f, cap, rng, junk=True, spare=-1):
         n = len(f["kps"])
         self.cap = cap
-        self.keep, self.n_keep, src, dup, slots = embed(n, cap, rng, junk)
+        km = keymap(n, cap, rng, FORCED, duplicates=True, junk=junk)
+        self.keep, self.n_keep, src, dup = km.keep, km.n_keep, km.src, km.dup
         live = int(f["node"][f["node"] >= 0][0]) if (f["node"] >= 0).any() else 3
-        self.kps = np.zeros(cap + SLACK, KP_DTYPE)
-        self.kps["angle"] = 100.0
-        self.desc = rng.integers(0, 256, (cap + SLACK, 32), dtype=np.uint8)
-        self.kps[slots], self.desc[slots] = f["kps"], f["desc"]
+        decoy = np.zeros(1, KP_DTYPE)
+        decoy["angle"] = 100.0
+        self.kps = scatter(f["kps"], km.slots, cap, decoy)
+        self.desc = scatter(f["desc"], km.slots, cap, rng.integers(0, 256, (cap + SLACK, 32), dtype=np.uint8))
         if n:
             self.kps[cap:], self.desc[cap:] = f["kps"][0], f["desc"][0]
         self.node = np.full(len(self.keep), live, np.int32)
@@ -248,17 +195,15 @@ def device_search(el, fr, kfs, counts, ratio, check, frame_count=None):
     """sivo_search_by_bow_device with n_kf rows of cap + SLACK sentinel (-7) entries and n_kf + 1 counts."""
     cap = el.capacity()
     n_kf = len(kfs)
-    hold = [upload(fr.kps), upload(fr.desc), upload(fr.keep), upload(np.array([fr.n_keep if frame_count is None else frame_count], np.int64)),
-            upload(fr.node)]
+    hold = [upload(fr.kps), upload(fr.desc), upload(fr.keep), i64(fr.n_keep if frame_count is None else frame_count), upload(fr.node)]
     keys, pts = [], []
     for kf, c in zip(kfs, counts):
-        a = [upload(kf["kps"]), upload(kf["desc"]), upload(kf["node"]), upload(kf["point"]), upload(np.array([c], np.int64))]
+        a = [upload(kf["kps"]), upload(kf["desc"]), upload(kf["node"]), upload(kf["point"]), i64(c)]
         hold += a
         keys.append(keyframe_keys(a[0].data_ptr(), a[1].data_ptr(), a[2].data_ptr(), a[4].data_ptr()))
         pts.append(a[3].data_ptr())
-    match = torch.full((n_kf * cap + SLACK,), -7, dtype=torch.int32, device="cuda")
-    nm = torch.full((n_kf + 1,), -7, dtype=torch.int64, device="cuda")
-    torch.cuda.synchronize()
+    match = sentinel(n_kf * cap + SLACK, -7, torch.int32)
+    nm = sentinel(n_kf + 1, -7, torch.int64)
     search_by_bow_device(el, hold[0].data_ptr(), hold[1].data_ptr(), hold[2].data_ptr(), hold[3].data_ptr(), hold[4].data_ptr(), keys,
                          pts, ratio, check, match.data_ptr(), nm.data_ptr())
     torch.cuda.synchronize()
@@ -319,7 +264,7 @@ def test_search_case(name):
     case = SEARCH[name]
     counts = counts_of(case)
     n = len(case.frame["kps"])
-    el = extractor_for(n)
+    el = el_for(n)
     want = check_host_search(el, case.frame, case.kfs, counts, case.ratio, case.check)
     check_device_search(el, case.frame, case.kfs, counts, case.ratio, case.check, case_rng(name), case.junk, same_as=want)
 
@@ -353,9 +298,8 @@ def test_capacity_limits():
     voc = vocabulary(case.tree)
     cap = over.capacity()
     slot_desc, keep, n_keep = transform_setup(case.desc, cap, case_rng("over"), True)
-    t = [upload(slot_desc), upload(keep), upload(np.array([n_keep], np.int64))]
-    outs = [torch.full((cap,), -7, dtype=torch.int32, device="cuda") for _ in range(3)] + \
-        [torch.full((cap,), 7.0, dtype=torch.float64, device="cuda"), torch.full((1,), -7, dtype=torch.int64, device="cuda")]
+    t = [upload(slot_desc), upload(keep), i64(n_keep)]
+    outs = [sentinel(cap, -7, torch.int32) for _ in range(3)] + [sentinel(cap, 7.0, torch.float64), sentinel(1, -7, torch.int64)]
     with pytest.raises(L.SivoError) as e:
         compute_bow_device(voc, over, t[0].data_ptr(), t[1].data_ptr(), t[2].data_ptr(), case.levelsup, *(o.data_ptr() for o in outs))
     assert e.value.code == L.ERANGE
@@ -363,11 +307,10 @@ def test_capacity_limits():
     assert all((o == (7.0 if o.dtype == torch.float64 else -7)).all() for o in outs)
     sc = SEARCH["decisions_070"]
     fr = DeviceFrame(sc.frame, cap, case_rng("over2"))
-    hold = [upload(fr.kps), upload(fr.desc), upload(fr.keep), upload(np.array([fr.n_keep], np.int64)), upload(fr.node)]
+    hold = [upload(fr.kps), upload(fr.desc), upload(fr.keep), i64(fr.n_keep), upload(fr.node)]
     pk = pad_keyframe(sc.kfs[0], cap)
-    a = [upload(pk["kps"]), upload(pk["desc"]), upload(pk["node"]), upload(pk["point"]), upload(np.array([len(sc.kfs[0]["kps"])], np.int64))]
-    match = torch.full((cap,), -7, dtype=torch.int32, device="cuda")
-    nm = torch.full((1,), -7, dtype=torch.int64, device="cuda")
+    a = [upload(pk["kps"]), upload(pk["desc"]), upload(pk["node"]), upload(pk["point"]), i64(len(sc.kfs[0]["kps"]))]
+    match, nm = sentinel(cap, -7, torch.int32), sentinel(1, -7, torch.int64)
     with pytest.raises(L.SivoError) as e:
         search_by_bow_device(over, *(h.data_ptr() for h in hold), [keyframe_keys(a[0].data_ptr(), a[1].data_ptr(), a[2].data_ptr(),
                                                                                  a[4].data_ptr())], [a[3].data_ptr()], sc.ratio, sc.check,

@@ -4,18 +4,15 @@ import numpy as np
 import pytest
 import torch
 
-from frame_support import H, MB, MBF, POSES, SIGMAS, W, InfoOut, cameras, ext, ptr, seg, synth, tails, upload  # noqa: F401
+from frame_support import H, MB, MBF, POSES, SIGMAS, W, InfoOut, cameras, ext, i64, ptr, same_bits, seg, synth, tails, upload  # noqa: F401
 from oracle import info_oracle as I
+from oracle.keymap import keymap
 from sivo_b200 import _lib as L
 from sivo_b200 import info_select, stereo_match
 from sivo_b200.frame import DeviceFrame
 from sivo_b200.info import info_terms
 
 pytestmark = pytest.mark.gpu
-
-
-def same_bits(a, b):
-    return a.shape == b.shape and a.tobytes() == b.tobytes()
 
 
 # ---------------------------------------------------------------------------------------------------------- against the oracle
@@ -81,6 +78,19 @@ def test_device_form_equals_the_host_form(tails, ext, sigma, pose):
         w, r, s, m = out.host(t.n_keep)
         assert same_bits(w, hw) and same_bits(r, hr) and same_bits(s, hs) and m == len(hs), f
         assert (out.red.cpu().numpy()[t.n_keep:] == 7.0).all() and (out.sel.cpu().numpy()[m:] == -7).all()
+        # the same keys through an oracle/keymap.py map: its rejected entries come out unselected
+        km = keymap(t.n_keep, t.f.left.cap, np.random.default_rng(t.n_keep))
+        keep = km.keep.copy()
+        keep[km.real] = t.keep
+        depth = np.full(len(keep), 10.0, np.float32)  # a rejected entry has a depth, but no key
+        depth[km.real] = t.depth
+        d_keep, d_n, d_depth = upload(keep), i64(km.n_keep), upload(depth)
+        out = InfoOut(t.f.left.cap)
+        out.run(el, t.f.kps, t.f.kp_entropy, ptr(d_keep), ptr(d_n), ptr(d_depth), cam, th, stream.cuda_stream)
+        stream.synchronize()
+        w, r, s, m = out.host(km.n_keep)
+        assert same_bits(w[km.real], hw) and same_bits(r[km.real], hr) and same_bits(s, km.real[hs].astype(np.int32)), f
+        assert m == len(hs) and not np.isin(s, np.flatnonzero(km.src < 0)).any()
         # keep_idx NULL: semantic key j is extractor key j (depth from the stereo call without keep_idx)
         n = len(t.kps_all)
         hw, hr, hs = info_select(el, t.kps_all, t.depth_all, t.ent_all, cam, th)
@@ -107,11 +117,6 @@ def test_device_form_edge_cases(tails, ext):
                 ptr(kw["depth"]) if "depth" in kw else t.f.depth, cam_, th, s, null)
         stream.synchronize()
         return out
-
-    def i64(v):
-        x = torch.tensor([v], dtype=torch.int64, device="cuda")
-        torch.cuda.synchronize()
-        return x
 
     # a negative count writes only n_selected = -1; a zero count writes only n_selected = 0
     for v in (-1, 0):

@@ -5,12 +5,14 @@ import numpy as np
 import pytest
 import torch
 
+from frame_support import KF_FIELDS, extractor, i64, upload
 from oracle import mapping_scene as S
 from oracle import mapping_oracle as MO
+from oracle.keymap import keymap, scatter
 from sivo_b200 import _lib as L
 from sivo_b200.mapping import HostKeyframe, KeyframeKeys, create_map_points, create_map_points_device, keyframe_gather_device, \
     make_params, set_pose
-from sivo_b200.orb import KP_DTYPE, ORBextractor
+from sivo_b200.orb import KP_DTYPE
 
 pytestmark = pytest.mark.gpu
 TH_CONF, TH_RED, MAX_CLASS = 0.5, 9.5, 8
@@ -19,7 +21,7 @@ TH_CONF, TH_RED, MAX_CLASS = 0.5, 9.5, 8
 @pytest.fixture(scope="module")
 def left():
     p = S.EXTRACTOR
-    return ORBextractor(p.nfeatures, p.scale_factor, p.nlevels, 20, 7)
+    return extractor(p.nfeatures, p.scale_factor, p.nlevels)
 
 
 def host_kf(kf: MO.KeyFrame, count=None) -> HostKeyframe:
@@ -110,18 +112,8 @@ def test_error_codes(left):
 
 def _device_kf(kf: MO.KeyFrame, cap, keep):
     n = len(kf.kps)
-    t = {}
-    pad = lambda a, dt: torch.from_numpy(np.concatenate([np.asarray(a, dt), np.zeros((cap - n,) + np.asarray(a).shape[1:], dt)])).cuda()
-    t["kps"] = pad(kf.kps.view(np.uint8).reshape(n, 28), np.uint8)
-    t["desc"] = pad(kf.desc, np.uint8)
-    t["u_right"] = pad(kf.u_right, np.float32)
-    t["depth"] = pad(kf.depth, np.float32)
-    t["kp_class"] = pad(kf.kp_class, np.uint8)
-    t["kp_conf"] = pad(kf.kp_conf, np.float64)
-    t["kp_entropy"] = pad(kf.kp_entropy, np.float64)
-    t["node"] = pad(kf.node, np.int32)
-    t["has_point"] = pad(kf.has_point, np.uint8)
-    t["count"] = torch.tensor([n], dtype=torch.int64, device="cuda")
+    t = {f: upload(scatter(np.asarray(getattr(kf, f), dt), np.arange(n), cap, 0)) for f, dt in KF_FIELDS.items()}
+    t["count"] = i64(n)
     keep.append(t)
     k = KeyframeKeys(*[t[f].data_ptr() for f in ("kps", "desc", "u_right", "depth", "kp_class", "kp_conf", "kp_entropy", "node",
                                                  "has_point", "count")])
@@ -174,16 +166,15 @@ def test_keyframe_gather(left):
     kps = np.zeros(cap, KP_DTYPE)
     kps["x"], kps["y"], kps["octave"] = rng.uniform(0, 900, cap), rng.uniform(0, 300, cap), rng.integers(0, 8, cap)
     desc = rng.integers(0, 256, (cap, 32), dtype=np.uint8)
-    keep_idx = np.sort(rng.choice(cap, n, replace=False)).astype(np.int32)
-    keep_idx[5] = cap + 3  # outside the capacity
+    km = keymap(n, cap, rng, forced=(5,))
+    n = km.n_keep
+    keep_idx = km.keep[:n]
     ur = rng.uniform(-1, 900, cap).astype(np.float32)
     depth = rng.uniform(-1, 40, cap).astype(np.float32)
     cls = rng.integers(0, 12, cap).astype(np.uint8)
     conf = rng.random(cap)
     ent = rng.random(cap)
-    dev = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()
-    src = [dev(kps.view(np.uint8)), dev(desc), dev(keep_idx), dev(np.array([n], np.int64)), dev(ur), dev(depth), dev(cls), dev(conf),
-           dev(ent)]
+    src = [upload(kps), upload(desc), upload(km.keep), i64(n), upload(ur), upload(depth), upload(cls), upload(conf), upload(ent)]
     out = dict(kps=torch.zeros(cap * 28, dtype=torch.uint8, device="cuda"), desc=torch.zeros(cap, 32, dtype=torch.uint8, device="cuda"),
                u_right=torch.zeros(cap, device="cuda"), depth=torch.zeros(cap, device="cuda"),
                kp_class=torch.zeros(cap, dtype=torch.uint8, device="cuda"), kp_conf=torch.zeros(cap, dtype=torch.float64, device="cuda"),
@@ -192,11 +183,11 @@ def test_keyframe_gather(left):
     keyframe_gather_device(left, *[s.data_ptr() for s in src], out)
     torch.cuda.synchronize()
     k = np.clip(keep_idx, 0, cap - 1)
-    good = keep_idx < cap
+    good = km.src >= 0
     got_kps = out["kps"].cpu().numpy().view(KP_DTYPE)
     assert int(out["count"][0]) == n
     np.testing.assert_array_equal(got_kps[:n][good], kps[k][good])
-    assert got_kps[5]["octave"] == -1
+    assert got_kps[5]["octave"] == -1 and (got_kps[:n][~good]["octave"] == -1).all()
     np.testing.assert_array_equal(out["desc"].cpu().numpy()[:n][good], desc[k][good])
     np.testing.assert_array_equal(out["u_right"].cpu().numpy()[:n], ur[:n])
     np.testing.assert_array_equal(out["depth"].cpu().numpy()[:n], depth[:n])

@@ -6,26 +6,18 @@ import numpy as np
 import pytest
 import torch
 
+from frame_support import KF_FIELDS, extractor, i64, upload
 from oracle import mapping_oracle as MO
 from oracle import mapping_scene as S
+from oracle.keymap import keymap, scatter
 from oracle.orb_oracle import ExtractorParams
 from sivo_b200.mapping import HostKeyframe, KeyframeKeys, create_map_points, create_map_points_device, keyframe_gather_device, \
     make_params, set_pose
-from sivo_b200.orb import KP_DTYPE, ORBextractor
+from sivo_b200.orb import KP_DTYPE
 
 pytestmark = pytest.mark.gpu
 SCENES = {sc.name: sc for sc in S.constructed_scenes()}
 FOUR = ExtractorParams(nfeatures=2000, scale_factor=1.5, nlevels=4)
-_EXT = {}
-
-
-def extractor(ext=S.EXTRACTOR):
-    key = (ext.nfeatures, ext.scale_factor, ext.nlevels)
-    if key not in _EXT:
-        _EXT[key] = ORBextractor(ext.nfeatures, ext.scale_factor, ext.nlevels, 20, 7)
-    return _EXT[key]
-
-
 def host_kf(kf: MO.KeyFrame) -> HostKeyframe:
     return HostKeyframe(kf.kps, kf.desc, kf.u_right, kf.depth, kf.kp_class, kf.kp_conf, kf.kp_entropy, kf.node, kf.has_point, kf.Rcw,
                         kf.tcw, kf.Ow)
@@ -39,11 +31,8 @@ def device_kf(kf: MO.KeyFrame, cap, keep, count=None):
     """The keyframe's keys in capacity-sized device buffers, padded with keys in no node."""
     n = len(kf.kps)
     assert n <= cap
-    pad = lambda a, dt, fill=0: torch.from_numpy(np.concatenate([np.asarray(a, dt), np.full((cap - n,) + np.asarray(a).shape[1:], fill, dt)])).cuda()
-    t = dict(kps=pad(kf.kps.view(np.uint8).reshape(n, 28), np.uint8), desc=pad(kf.desc, np.uint8), u_right=pad(kf.u_right, np.float32),
-             depth=pad(kf.depth, np.float32), kp_class=pad(kf.kp_class, np.uint8), kp_conf=pad(kf.kp_conf, np.float64),
-             kp_entropy=pad(kf.kp_entropy, np.float64), node=pad(kf.node, np.int32, -1), has_point=pad(kf.has_point, np.uint8),
-             count=torch.tensor([n if count is None else count], dtype=torch.int64, device="cuda"))
+    t = {f: upload(scatter(np.asarray(getattr(kf, f), dt), np.arange(n), cap, -1 if f == "node" else 0)) for f, dt in KF_FIELDS.items()}
+    t["count"] = i64(n if count is None else count)
     keep.append(t)
     k = KeyframeKeys(*[t[f].data_ptr() for f in ("kps", "desc", "u_right", "depth", "kp_class", "kp_conf", "kp_entropy", "node",
                                                  "has_point", "count")])
@@ -73,7 +62,7 @@ def as_result(o, n1):
 def all_forms(kf1, nbs, max_class=8, th_conf=0.5, th_red=-1e9, ext=S.EXTRACTOR, max_exempt=0, device=True):
     """The oracle, the debug and production host forms and the device form, each compared with mapping_scene.compare.  Returns
     (oracle result, debug result, exempt keys)."""
-    left = extractor(ext)
+    left = extractor(ext.nfeatures, ext.scale_factor, ext.nlevels)
     want = S.oracle_run(kf1, nbs, th_conf, th_red, max_class, ext)
     prm = params(max_class, th_conf, th_red)
     hk1, hn = host_kf(kf1), [host_kf(k) for k in nbs]
@@ -223,11 +212,10 @@ def test_keyframe_gather_edges():
     desc = rng.integers(0, 256, (cap, 32), dtype=np.uint8)
     ur, depth = rng.uniform(-1, 900, cap).astype(np.float32), rng.uniform(-1, 40, cap).astype(np.float32)
     cls, conf, ent = rng.integers(0, 12, cap).astype(np.uint8), rng.random(cap), rng.random(cap)
-    dev = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()
 
     def run(keep_idx, n_keep):
-        src = [dev(kps.view(np.uint8)), dev(desc), dev(keep_idx) if keep_idx is not None else None, dev(np.array([n_keep], np.int64)),
-               dev(ur), dev(depth), dev(cls), dev(conf), dev(ent)]
+        src = [upload(kps), upload(desc), upload(keep_idx) if keep_idx is not None else None, i64(n_keep), upload(ur), upload(depth),
+               upload(cls), upload(conf), upload(ent)]
         out = dict(kps=torch.full((cap * 28,), 0xAB, dtype=torch.uint8, device="cuda"),
                    desc=torch.full((cap, 32), 0xAB, dtype=torch.uint8, device="cuda"), u_right=torch.full((cap,), 7.0, device="cuda"),
                    depth=torch.full((cap,), 7.0, device="cuda"), kp_class=torch.full((cap,), 0xAB, dtype=torch.uint8, device="cuda"),
@@ -254,9 +242,9 @@ def test_keyframe_gather_edges():
         assert (o["kp_class"][n:] == 0xAB).all() and (o["u_right"][n:] == 7.0).all()
 
     check(run(None, 1000), None, 1000)  # keep_idx NULL: the identity
-    keep_idx = rng.permutation(cap).astype(np.int32)
-    keep_idx[[0, 5, 999]] = [-1, -(1 << 31), cap]
-    check(run(keep_idx, 1000), keep_idx, 1000)  # negative and out-of-capacity entries
+    km = keymap(1000, cap, rng, forced=(0, 5, 999))
+    keep_idx = km.keep
+    check(run(keep_idx, km.n_keep), keep_idx, km.n_keep)  # rejected entries
     check(run(keep_idx, cap + 50), keep_idx, cap)  # a count above the capacity: clamped
     o = run(keep_idx, -1)  # a negative count writes only the count
     assert int(o["count"][0]) == -1 and (o["kps"] == 0xAB).all() and (o["u_right"] == 7.0).all() and (o["kp_conf"] == 7.0).all()

@@ -5,9 +5,10 @@ import numpy as np
 import pytest
 import torch
 
+from frame_support import extractor, same_bits
 from oracle import pnp_oracle as P
 from sivo_b200 import reloc
-from sivo_b200.orb import KP_DTYPE, ORBextractor
+from sivo_b200.orb import KP_DTYPE
 from sivo_b200.track import map_points
 
 pytestmark = pytest.mark.gpu
@@ -17,11 +18,7 @@ SEED, FRAME = 0x5EED5EED1234, 77
 
 @pytest.fixture(scope="module")
 def left():
-    return ORBextractor(2000, 1.2, 8, 20, 7)
-
-
-def same(a, b):
-    return np.array_equal(np.asarray(a, np.float64), np.asarray(b, np.float64), equal_nan=True)
+    return extractor()
 
 
 def test_draws_match_the_oracle():
@@ -53,14 +50,14 @@ def test_refine_path_intermediates_match_the_oracle(n, planar):
         alphas, mask, cnt, d = reloc.compute_pose(p3, p2, err, FX, FY, CX, CY)
         fu, fv, uc, vc = (float(np.float32(x)) for x in (FX, FY, CX, CY))
         o = P.compute_pose(p3.astype(np.float64).tolist(), p2.astype(np.float64).tolist(), fu, fv, uc, vc, tree=True)
-        assert same(alphas, o.alphas)
-        assert same(d.cws, o.cws) and same(d.d, o.d) and same(d.ut, o.ut)
-        assert same(d.l_6x10, o.l_6x10) and same(d.rho, o.rho)
-        assert same(d.betas, [o.betas[b][i] for b in (1, 2, 3) for i in range(4)])
-        assert same(d.rep_errors, o.rep_errors[1:])
-        assert same(d.Rs, [x for b in (1, 2, 3) for row in o.Rs[b] for x in row])
-        assert same(d.ts, [x for b in (1, 2, 3) for x in o.ts[b]])
-        assert d.best == o.best and same(d.R, [x for row in o.R for x in row]) and same(d.t, o.t)
+        assert same_bits(alphas, o.alphas)
+        assert same_bits(d.cws, o.cws) and same_bits(d.d, o.d) and same_bits(d.ut, o.ut)
+        assert same_bits(d.l_6x10, o.l_6x10) and same_bits(d.rho, o.rho)
+        assert same_bits(d.betas, [o.betas[b][i] for b in (1, 2, 3) for i in range(4)])
+        assert same_bits(d.rep_errors, o.rep_errors[1:])
+        assert same_bits(d.Rs, [x for b in (1, 2, 3) for row in o.Rs[b] for x in row])
+        assert same_bits(d.ts, [x for b in (1, 2, 3) for x in o.ts[b]])
+        assert d.best == o.best and same_bits(d.R, [x for row in o.R for x in row]) and same_bits(d.t, o.t)
         om, oc = P.check_inliers(o.R, o.t, p3, p2, fu, fv, uc, vc, err)
         assert cnt == oc and np.array_equal(mask, om)
         if planar:
@@ -135,7 +132,7 @@ def run_and_compare(left, n_kf, N, outliers, seed, neg=(), n_keep=None, active0=
         for g in range(hyps):
             idx, dbg, mask, cnt = s.hypothesis(g)
             assert list(got["draws"][g]) == idx
-            assert same(got["R"][g], dbg.R) and same(got["t"][g], dbg.t)
+            assert same_bits(got["R"][g], dbg.R) and same_bits(got["t"][g], dbg.t)
             assert got["counts"][g] == cnt and np.array_equal(got["masks"][g][:s.N], mask)
     active = np.ones(n_kf, bool) if active0 is None else np.asarray(active0, bool).copy()
     Tcw = torch.full((n_kf, 12), float("nan"), dtype=torch.float32, device=dev)

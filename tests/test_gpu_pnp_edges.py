@@ -11,34 +11,21 @@ import numpy as np
 import pytest
 import torch
 
+from frame_support import extractor, i64, same_bits, sentinel, upload
 from oracle import bow_oracle as BO
 from oracle import bow_scene as BS
 from oracle import pnp_bounds as PB
 from oracle import pnp_oracle as P
 from oracle import pnp_scene as S
+from oracle.keymap import SLACK, keymap
 from oracle.orb_oracle import ExtractorParams, Tables
 from sivo_b200 import _lib as L
 from sivo_b200 import reloc
 from sivo_b200.bow import keyframe_keys, search_by_bow_device
-from sivo_b200.orb import ORBextractor
 from sivo_b200.track import map_points
 
 pytestmark = pytest.mark.gpu
 SCENES = {sc.name: sc for sc in S.constructed_scenes()}
-_EXT = {}
-
-
-def extractor(scale=1.2, nlevels=8):
-    if (scale, nlevels) not in _EXT:
-        _EXT[(scale, nlevels)] = ORBextractor(2000, scale, nlevels, 20, 7)
-    return _EXT[(scale, nlevels)]
-
-
-def dev(a, dtype=None):
-    a = np.ascontiguousarray(a)
-    return torch.from_numpy(a.view(np.uint8).reshape(-1).copy() if dtype is None else a.astype(dtype)).cuda()
-
-
 class Setup:
     """One embedded scene as device buffers: n_kf candidates sharing the frame (the same match row), kf_ids as given."""
 
@@ -53,10 +40,9 @@ class Setup:
         self.n_matches = np.full(n_kf, (self.fr.match[:self.fr.n_keep] >= 0).sum(), np.int64) if n_matches is None else \
             np.asarray(n_matches, np.int64)
         pts = map_points(np.zeros((len(self.fr.points), 32), np.uint8), self.fr.points, np.zeros_like(self.fr.points), 0.0, 1e9)
-        self.t = dict(kps=dev(self.fr.kps), keep=torch.from_numpy(self.fr.keep_idx.copy()).cuda(),
-                      nk=torch.tensor([self.n_keep], dtype=torch.int64, device="cuda"),
-                      match=torch.from_numpy(np.concatenate([rows.reshape(-1), np.zeros(S.SLACK, np.int32)])).cuda(),
-                      nm=torch.from_numpy(self.n_matches.copy()).cuda(), pts=dev(pts))
+        self.t = dict(kps=upload(self.fr.kps), keep=torch.from_numpy(self.fr.keep_idx.copy()).cuda(), nk=i64(self.n_keep),
+                      match=torch.from_numpy(np.concatenate([rows.reshape(-1), np.zeros(SLACK, np.int32)])).cuda(),
+                      nm=torch.from_numpy(self.n_matches.copy()).cuda(), pts=upload(pts))
 
     def call(self, solver, stream=0):
         t = self.t
@@ -150,7 +136,7 @@ def compare_pose(p3, p2, err, cam):
     alphas, mask, cnt, d = reloc.compute_pose(p3, p2, err, *cam)
     fu, fv, uc, vc = (float(np.float32(c)) for c in cam)
     o = P.compute_pose(p3.astype(np.float64).tolist(), p2.astype(np.float64).tolist(), fu, fv, uc, vc, tree=True)
-    same = lambda a, b: np.array_equal(np.asarray(a, np.float64).ravel(), np.asarray(b, np.float64).ravel(), equal_nan=True)
+    same = lambda a, b: same_bits(np.ravel(a), np.ravel(b))
     assert same(alphas, o.alphas) and same(d.cws, o.cws) and same(d.d, o.d) and same(d.ut, o.ut)
     assert same(d.l_6x10, o.l_6x10) and same(d.rho, o.rho)
     assert same(d.betas, [o.betas[b][i] for b in (1, 2, 3) for i in range(4)]) and same(d.rep_errors, o.rep_errors[1:])
@@ -355,7 +341,7 @@ def test_four_level_extractor():
     """4 levels at scale 1.5: the sigma2 table and the nlevels rejection (octave 4 among the rejected keys) differ from the
     default.  The scenes are re-octaved (octave % 4), so their thresholds change and the paths they were built for are not
     claimed here: this checks bit equality with the oracle on the 4-level tables, call by call."""
-    left = extractor(1.5, 4)
+    left = extractor(2000, 1.5, 4)
     assert np.array_equal(left._s2, Tables(ExtractorParams(nfeatures=2000, scale_factor=1.5, nlevels=4)).sigma2)
     for name in ("at_min_fail", "tie_worse_recover", "refine_257", "mask_33"):
         sc = SCENES[name]
@@ -449,7 +435,7 @@ class _Rows:
 
 
 def test_a_row_from_search_by_bow():
-    """sivo_search_by_bow_device on a permuted semantic-key map (with -1 and out-of-capacity entries), then its own keep_idx,
+    """sivo_search_by_bow_device on an oracle/keymap.py semantic-key map (rejected entries between the keys), then its own keep_idx,
     n_keep, match and n_matches buffers passed unchanged to sivo_pnp_setup_device; the points placed so that most matched
     (key, point) pairs agree with one pose.  Against bow_oracle.search_by_bow followed by pnp_oracle."""
     left = extractor()
@@ -459,61 +445,55 @@ def test_a_row_from_search_by_bow():
     for k, kf in enumerate(kfs):  # keyframe k's key i sees point k cap + i: a point is matched by at most one key per call
         kf["point"] = np.where(kf["point"] >= 0, k * cap + np.arange(len(kf["point"])), -1).astype(np.int32)
     rng = np.random.default_rng(5)
-    keep = np.zeros(cap + S.SLACK, np.int32)
-    keep[:n] = rng.permutation(cap)[:n]
-    keep[n:] = rng.integers(0, cap, len(keep) - n)
-    bad = rng.choice(n, 12, replace=False)
-    keep[bad[:6]], keep[bad[6:]] = -1, cap + 3
-    valid = (keep[:n] >= 0) & (keep[:n] < cap)
-    slots = np.zeros(cap + S.SLACK, f["kps"].dtype)
+    km = keymap(n, cap, rng)
+    keep, nk, src = km.keep, km.n_keep, km.src
+    key = np.maximum(src, 0)
+    slots = np.zeros(cap + SLACK, f["kps"].dtype)
     slots["x"][cap:], slots["y"][cap:] = 600.0, 180.0
-    desc = np.zeros((cap + S.SLACK, 32), np.uint8)
-    slots[keep[:n][valid]], desc[keep[:n][valid]] = f["kps"][valid], f["desc"][valid]
-    node = np.full(cap + S.SLACK, -1, np.int32)
-    node[:n] = f["node"]
-    # the oracle's frame: the keys outside the capacity are in no node
-    want = [BO.search_by_bow(f["kps"], f["desc"], np.where(valid, f["node"], -1), kf["kps"], kf["desc"], kf["node"], kf["point"], 0.75,
-                             True) for kf in kfs]
+    desc = np.zeros((cap + SLACK, 32), np.uint8)
+    slots[km.slots], desc[km.slots] = f["kps"], f["desc"]
+    node = np.full(cap + SLACK, -1, np.int32)
+    node[:nk] = np.where(src >= 0, f["node"][key], f["node"].max())  # a rejected entry carries a live node
+    # the oracle's frame, entry by entry: a rejected entry is in no node
+    want = [BO.search_by_bow(f["kps"][key], f["desc"][key], np.where(src >= 0, f["node"][key], -1), kf["kps"], kf["desc"], kf["node"],
+                             kf["point"], 0.75, True) for kf in kfs]
 
     def pad(a, fill=0):
         a = np.ascontiguousarray(a)
         out = np.zeros(cap, a.dtype) if a.dtype.names else np.full((cap,) + a.shape[1:], fill, a.dtype)
         out[:len(a)] = a
-        return dev(out) if a.dtype.names else torch.from_numpy(out).cuda()
+        return upload(out)
     hold, keys, pts = [], [], []
     for kf in kfs:
-        a = [pad(kf["kps"]), pad(kf["desc"]), pad(kf["node"], -1), pad(kf["point"], -1),
-             torch.tensor([len(kf["kps"])], dtype=torch.int64, device="cuda")]
+        a = [pad(kf["kps"]), pad(kf["desc"]), pad(kf["node"], -1), pad(kf["point"], -1), i64(len(kf["kps"]))]
         hold += a
         keys.append(keyframe_keys(a[0].data_ptr(), a[1].data_ptr(), a[2].data_ptr(), a[4].data_ptr()))
         pts.append(a[3].data_ptr())
-    t_kps, t_desc, t_keep, t_node = dev(slots), torch.from_numpy(desc).cuda(), torch.from_numpy(keep).cuda(), torch.from_numpy(node).cuda()
-    t_nk = torch.tensor([n], dtype=torch.int64, device="cuda")
-    t_match = torch.full((n_kf * cap + S.SLACK,), -7, dtype=torch.int32, device="cuda")
-    t_nm = torch.full((n_kf,), -7, dtype=torch.int64, device="cuda")
-    torch.cuda.synchronize()
+    t_kps, t_desc, t_keep, t_node, t_nk = upload(slots), upload(desc), upload(keep), upload(node), i64(nk)
+    t_match = sentinel(n_kf * cap + SLACK, -7, torch.int32)
+    t_nm = sentinel(n_kf, -7, torch.int64)
     search_by_bow_device(left, t_kps.data_ptr(), t_desc.data_ptr(), t_keep.data_ptr(), t_nk.data_ptr(), t_node.data_ptr(), keys, pts,
                          0.75, True, t_match.data_ptr(), t_nm.data_ptr())
     torch.cuda.synchronize()
     rows = t_match.cpu().numpy()[:n_kf * cap].reshape(n_kf, cap)
     for k, (m, c) in enumerate(want):
-        assert np.array_equal(rows[k, :n], m) and (rows[k, n:] == -1).all() and int(t_nm[k]) == c, k
+        assert np.array_equal(rows[k, :nk], m) and (rows[k, nk:] == -1).all() and int(t_nm[k]) == c, k
     assert sum(c for _, c in want) > 40
     # the points: a matched pair's point on its key's ray at 5 - 40 m under one pose (70 %), elsewhere at random
     R, C = S.rotation((0.2, 1, -0.1), 0.7), np.array([2.0, -0.5, 1.0])
     cam = S.KITTI
     n_points = n_kf * cap
-    points = np.zeros((n_points + S.SLACK, 3), np.float32)
+    points = np.zeros((n_points + SLACK, 3), np.float32)
     points[:] = rng.uniform(-30, 30, (len(points), 3)).astype(np.float32)
     for k in range(n_kf):
-        for j in np.nonzero(rows[k, :n] >= 0)[0]:
+        for j in np.nonzero(rows[k, :nk] >= 0)[0]:
             if rng.random() < 0.7:
                 kp = slots[keep[j]]
                 z = rng.uniform(5, 40)
                 Pc = np.array([(kp["x"] - cam[2]) * z / cam[0], (kp["y"] - cam[3]) * z / cam[1], z])
                 points[rows[k, j]] = (R.T @ Pc + C).astype(np.float32)
     mp_arr = map_points(np.zeros((len(points), 32), np.uint8), points, np.zeros_like(points), 0.0, 1e9)
-    t_pts = dev(mp_arr)
+    t_pts = upload(mp_arr)
     kf_ids = np.arange(n_kf, dtype=np.uint32) * 5 + 3
     solver = reloc.PnpSolver(left, n_kf, S.SEED)
     try:
@@ -521,8 +501,8 @@ def test_a_row_from_search_by_bow():
                             n_points, kf_ids, S.FRAME, *cam)
         oracles = []
         for k in range(n_kf):
-            p2, p3, s2, key = P.correspondences(slots, rows[k], n, points[:n_points], left._s2, keep_idx=keep, cap=cap)
-            oracles.append((P.Solver(p2, p3, s2, *cam, seed=S.SEED, kf_id=int(kf_ids[k]), frame_id=S.FRAME, log=True), key))
+            p2, p3, s2, ckey = P.correspondences(slots, rows[k], nk, points[:n_points], left._s2, keep_idx=keep, cap=cap)
+            oracles.append((P.Solver(p2, p3, s2, *cam, seed=S.SEED, kf_id=int(kf_ids[k]), frame_id=S.FRAME, log=True), ckey))
         check_state(solver, oracles)
         assert all(s.N >= s.min_inl for s, _ in oracles)
         out = Outputs(n_kf, cap)

@@ -7,12 +7,14 @@ import numpy as np
 import pytest
 import torch
 
+from frame_support import extractor
 from oracle import pose_oracle as P
+from oracle.keymap import keymap
+from oracle.pose_scene import CAM, embed, exact_scene, pose34, rotation, scene
 from sivo_b200 import _lib as L
-from sivo_b200 import ORBextractor, PoseResult, map_points, pose_gather_device, pose_optimize, pose_optimize_device
+from sivo_b200 import PoseResult, map_points, pose_gather_device, pose_optimize, pose_optimize_device
 from sivo_b200.orb import KP_DTYPE
 from sivo_b200.pose import camera_from_result, frame_from_result, pose_system, result_from_bytes
-from test_oracle_pose import CAM, exact_scene, pose34, rotation, scene
 
 pytestmark = pytest.mark.gpu
 
@@ -23,7 +25,7 @@ SCENES = [(seed, n, mode, out) for seed, (n, mode) in enumerate([(120, "mono"), 
 
 @pytest.fixture(scope="module")
 def ext():
-    return ORBextractor(2000, 1.2, 8, 20, 7)
+    return extractor()
 
 
 def inv_sigma2(ext):
@@ -142,8 +144,7 @@ def test_device_form_equals_the_host_form_and_repeats(ext, seed, n, mode, out):
     kps, ur, X, Tin, _ = scene(seed, n=n, mode=mode, outliers=out)
     res, outl = pose_optimize(ext, kps, ur, X, Tin, *INTR)
     b = Bufs(ext.capacity())
-    perm = np.random.default_rng(seed).permutation(ext.capacity())[:n].astype(np.int32)
-    b.load(kps, ur, X, Tin, keep=perm)
+    b.load(kps, ur, X, Tin, keep=keymap(n, ext.capacity(), np.random.default_rng(seed), junk=False).keep[:n])
     for _ in range(2):
         b.run(ext)
         r2, o2 = b.host(n)
@@ -195,18 +196,14 @@ def test_nan_rule_points_behind_and_on_the_camera_plane(ext):
 def test_keep_idx_with_negative_and_out_of_capacity_entries(ext):
     cap = ext.capacity()
     kps, ur, X, Tin, _ = scene(7, n=300, mode="mixed", outliers=0.1)
-    keep = np.random.default_rng(7).permutation(cap)[:300].astype(np.int32)
-    keep[::17] = -1
-    keep[5::23] = cap + 3
+    km = keymap(300, cap, np.random.default_rng(7))
     b = Bufs(cap)
-    b.load(kps, ur, X, Tin, keep=keep)
+    b.load(*embed(km, kps, ur, X), Tin, keep=km.keep[:km.n_keep])
     b.run(ext)
-    r, o = b.host(300)
-    Xh = X.copy()
-    Xh[(keep < 0) | (keep >= cap)] = np.nan
-    ref = P.pose_optimization(kps, ur, Xh, Tin, inv_sigma2(ext), CAM, order="device")
-    check_result(r, o, ref)
-    assert r.n_initial == int(((keep >= 0) & (keep < cap)).sum())
+    r, o = b.host(km.n_keep)
+    ref = P.pose_optimization(kps, ur, X, Tin, inv_sigma2(ext), CAM, order="device")
+    check_result(r, o[km.real], ref)
+    assert r.n_initial == 300 and not o[km.src < 0].any()
 
 
 def test_count_equal_to_capacity_and_the_minus_one_count(ext):

@@ -9,9 +9,11 @@ import pytest
 import torch
 from scipy.spatial.transform import Rotation
 
+from frame_support import extractor, i64, same_bits, sentinel, upload
 from oracle import pose_oracle as P
 from oracle import pose_scene as PS
-from sivo_b200 import ORBextractor, pose_optimize, pose_optimize_device
+from oracle.keymap import keymap, scatter
+from sivo_b200 import pose_optimize, pose_optimize_device
 from sivo_b200.pose import (TRACE_COS, TRACE_POW_RHO, TRACE_POW_THETA, TRACE_ROUND, TRACE_SIN, TRACE_TRIAL, pose_se3, pose_trace,
                             result_from_bytes)
 
@@ -30,7 +32,7 @@ CALLS = []  # every device transcendental value the tests saw: (kind, arg, value
 
 @pytest.fixture(scope="module")
 def ext():
-    return ORBextractor(2000, 1.2, 8, 20, 7)
+    return extractor()
 
 
 def records(rec):
@@ -41,25 +43,19 @@ def records(rec):
     return out
 
 
-def same(a, b) -> bool:
-    """Bit equality (NaN payloads aside: a NaN matches a NaN)."""
-    a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
-    return a.shape == b.shape and bool(np.all((a.view(np.int64) == b.view(np.int64)) | (np.isnan(a) & np.isnan(b))))
-
-
 def check_log(dev, ref):
     assert [d["kind"] for d in dev] == [r["kind"] for r in ref]
     for i, (d, r) in enumerate(zip(dev, ref)):
         for f in FIELDS["call" if d["kind"] not in ("trial", "round") else d["kind"]]:
-            assert same(d[f], r[f]), (i, d["kind"], f, d[f], r[f])
+            assert same_bits(d[f], r[f]), (i, d["kind"], f, d[f], r[f])
 
 
 def check_exact(res, outl, ref: P.Result):
-    assert np.array_equal(res.pose(), ref.Tcw) and same(res.q, ref.q) and same(res.t, ref.t)
+    assert np.array_equal(res.pose(), ref.Tcw) and same_bits(res.q, ref.q) and same_bits(res.t, ref.t)
     assert np.array_equal(np.array(res.Rcw, np.float32), ref.Rcw.reshape(-1))
     assert np.array_equal(np.array(res.tcw, np.float32), ref.tcw) and np.array_equal(np.array(res.Rwc, np.float32), ref.Rwc.reshape(-1))
     assert np.array_equal(np.array(res.Ow, np.float32), ref.Ow)
-    assert same(res.sigma(), ref.sigma) and bool(res.sigma_valid) == ref.sigma_valid
+    assert same_bits(res.sigma(), ref.sigma) and bool(res.sigma_valid) == ref.sigma_valid
     assert (res.n_initial, res.n_bad, res.n_good, res.rounds_run) == (ref.n_initial, ref.n_bad, ref.n_good, ref.rounds_run)
     assert np.array_equal(outl, ref.outlier)
 
@@ -82,43 +78,24 @@ def run_all(ext, kps, ur, X, Tin, cam, keep_device=True):
 
 
 def device_form(ext, kps, ur, X, Tin, intr, ref):
-    """Keys scattered over the extractor's slots, with two extra semantic keys whose keep_idx is -1 and the capacity: they have
-    no edge, so the result is the oracle's over the real keys."""
+    """Keys scattered over the extractor's slots by an oracle/keymap.py map, whose rejected entries have a point but no key slot:
+    they have no edge, so the result is the oracle's over the real keys."""
     cap = ext.capacity()
     n = len(kps)
     if n + 2 > cap:
         return
-    rng = np.random.default_rng(n)
-    keep = rng.permutation(cap)[:n + 2].astype(np.int32)
-    pos = rng.permutation(n + 2)
-    bad = pos[:2]
-    keep[bad[0]], keep[bad[1]] = -1, cap
-    real = np.sort(pos[2:])
-    K = np.zeros(n + 2, kps.dtype)
-    U = np.zeros(n + 2, np.float32)
-    W = np.zeros((n + 2, 3), np.float32)
-    K[real], U[real], W[real] = kps, ur, X
-    W[bad] = 1.0  # a point, but no key slot: no edge
-    slots = np.zeros(cap, kps.dtype)
-    ok = (keep >= 0) & (keep < cap)
-    slots[keep[ok]] = K[ok]
-    d = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a).view(dt).reshape(-1).copy()).cuda()
-    kb = d(slots, np.uint8)
-    kk = torch.from_numpy(keep).cuda()
-    nn = torch.tensor([n + 2], dtype=torch.int64, device="cuda")
-    ub = torch.from_numpy(U).cuda()
-    xb = torch.from_numpy(W.reshape(-1).copy()).cuda()
-    tb = torch.from_numpy(np.ascontiguousarray(Tin, np.float32).reshape(-1)[:12].copy()).cuda()
-    rb = torch.zeros(512, dtype=torch.uint8, device="cuda")
-    ob = torch.full((cap,), 7, dtype=torch.uint8, device="cuda")
-    torch.cuda.synchronize()
+    km = keymap(n, cap, np.random.default_rng(n))
+    _, U, W = PS.embed(km, kps, ur, X)
+    kb, kk, nn = upload(scatter(kps, km.slots, cap, np.zeros(1, kps.dtype))), upload(km.keep), i64(km.n_keep)
+    ub, xb, tb = upload(U), upload(W), upload(np.asarray(Tin, np.float32).reshape(-1)[:12])
+    rb, ob = sentinel(512, 0, torch.uint8), sentinel(cap, 7, torch.uint8)
     pose_optimize_device(ext, kb.data_ptr(), kk.data_ptr(), nn.data_ptr(), ub.data_ptr(), xb.data_ptr(), *intr, tb.data_ptr(),
                          rb.data_ptr(), ob.data_ptr())
     torch.cuda.synchronize()
     r = result_from_bytes(rb.cpu().numpy())
     o = ob.cpu().numpy()
-    check_exact(r, o[:n + 2][real].astype(bool), ref)
-    assert not o[bad].any() and (o[n + 2:] == 7).all()
+    check_exact(r, o[km.real].astype(bool), ref)
+    assert not o[:km.n_keep][km.src < 0].any() and (o[km.n_keep:] == 7).all()
 
 
 # ---------------------------------------------------------------------------------------------------------- constructed scenes
@@ -194,7 +171,7 @@ def test_se3_functions_bit_for_bit():
     for i in range(len(T)):
         m = T[i].reshape(3, 4).astype(np.float64)
         P0 = P.to_se3quat(T[i])
-        assert same(se3[i], np.r_[P0.q, P0.t]), i
+        assert same_bits(se3[i], np.r_[P0.q, P0.t]), i
         branches.add(PS.quat_branch(m[:, :3]).split("+")[0])
         flips_in += P.quat_from_matrix(m[:, :3])[3] < 0
         theta = tv[i, 0]
@@ -204,7 +181,7 @@ def test_se3_functions_bit_for_bit():
         tx = P.Transcendentals(replay)
         U = P.oplus(d[i], P0, tx)
         assert tx.used == len(replay)
-        assert same(up[i], np.r_[U.q, U.t]), i
+        assert same_bits(up[i], np.r_[U.q, U.t]), i
         E = P.se3_exp(d[i], P.Transcendentals(replay))
         flips_up += P.quat_mul(E.q, P0.q)[3] < 0
         R = P.rotation_matrix(U.q)

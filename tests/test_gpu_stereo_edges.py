@@ -1,5 +1,5 @@
 """-m gpu: Frame::ComputeStereoMatches on constructed worst cases (oracle/stereo_scene.py) through the oracle, the host form
-(sivo_stereo_match) and the device form (sivo_stereo_match_device, with a keep_idx holding negative and out-of-capacity entries),
+(sivo_stereo_match) and the device form (sivo_stereo_match_device, through an oracle/keymap.py map with rejected entries),
 bit for bit; the Hamming stage through sivo_stereo_hamming; the median cut alone through sivo_dbg_stereo_median_cut; the rule
 for keys outside the domain (also for the semantic keys); the refusals; the rule's inertness on extractor keys; 200 fuzz scenes."""
 import ctypes as C
@@ -9,9 +9,10 @@ import numpy as np
 import pytest
 import torch
 
-from frame_support import upload
+from frame_support import extractor, i64, sentinel, upload
 from oracle import orb_oracle as O
 from oracle import stereo_scene as S
+from oracle.keymap import keymap, scatter
 from sivo_b200 import KP_DTYPE, ORBextractor, stereo_hamming, stereo_match, stereo_match_device
 from sivo_b200 import _lib as L
 from sivo_b200.orb import stereo_median_cut
@@ -25,61 +26,30 @@ KITTI_MB = KITTI_MBF / 718.856
 f32 = np.float32
 
 
-def dev_buf(cap, rec, fill):
-    t = torch.full((cap * rec,), fill, dtype=torch.uint8, device="cuda")
-    torch.cuda.synchronize()
-    return t
+def pair(nfeatures, scale_factor, nlevels):
+    return extractor(nfeatures, scale_factor, nlevels), extractor(nfeatures, scale_factor, nlevels, right=True)
 
 
-_EXT = {}
-
-
-def extractors(nfeatures, scale_factor, nlevels):
-    key = (nfeatures, scale_factor, nlevels)
-    if key not in _EXT:
-        _EXT[key] = (ORBextractor(nfeatures, scale_factor, nlevels, 20, 7), ORBextractor(nfeatures, scale_factor, nlevels, 20, 7))
-    return _EXT[key]
-
-
-def device_form(el, er, kl, dl, kr, dr, mb, mbf, keep, n_left=None, n_right=None):
-    """sivo_stereo_match_device with keys in capacity-sized device buffers; returns the first len(keep) outputs (7.0 = unwritten)
-    and the untouched tail's check."""
+def device_form(el, er, km, kl, dl, kr, dr, mb, mbf, n_left=None, n_right=None):
+    """sivo_stereo_match_device with the left keys at the slots of the map km (oracle/keymap.py) and the right keys in order, in
+    capacity-sized device buffers; returns the left buffers as the device reads them and the outputs (7.0 = unwritten)."""
     cap_l, cap_r = el.capacity(), er.capacity()
-    assert len(kl) <= cap_l and len(kr) <= cap_r
-    bl, bdl = dev_buf(cap_l, 28, 0), dev_buf(cap_l, 32, 0)
-    br, bdr = dev_buf(cap_r, 28, 0), dev_buf(cap_r, 32, 0)
-    if len(kl):
-        bl[:len(kl) * 28] = upload(kl)
-        bdl[:len(kl) * 32] = upload(dl)
-    if len(kr):
-        br[:len(kr) * 28] = upload(kr)
-        bdr[:len(kr) * 32] = upload(dr)
-    d_keep = torch.from_numpy(np.ascontiguousarray(keep, np.int32)).cuda()
-    nl = torch.tensor([len(keep) if n_left is None else n_left], dtype=torch.int64, device="cuda")
-    nr = torch.tensor([len(kr) if n_right is None else n_right], dtype=torch.int64, device="cuda")
-    u = torch.full((cap_l,), 7.0, dtype=torch.float32, device="cuda")
-    z = torch.full((cap_l,), 7.0, dtype=torch.float32, device="cuda")
-    torch.cuda.synchronize()
+    assert len(kr) <= cap_r
+    none = np.zeros(1, KP_DTYPE)
+    sl, sdl = scatter(kl, km.slots, cap_l, none), scatter(dl, km.slots, cap_l, 0)
+    right = np.arange(len(kr))
+    bufs = [upload(a) for a in (sl, sdl, km.keep, scatter(kr, right, cap_r, none), scatter(dr, right, cap_r, 0))]
+    nl, nr = i64(km.n_keep if n_left is None else n_left), i64(len(kr) if n_right is None else n_right)
+    u, z = sentinel(cap_l, 7.0, torch.float32), sentinel(cap_l, 7.0, torch.float32)
     stream = torch.cuda.Stream()
-    stereo_match_device(el, er, bl.data_ptr(), bdl.data_ptr(), d_keep.data_ptr(), nl.data_ptr(), br.data_ptr(), bdr.data_ptr(),
-                        nr.data_ptr(), mb, mbf, u.data_ptr(), z.data_ptr(), stream.cuda_stream)
+    stereo_match_device(el, er, bufs[0].data_ptr(), bufs[1].data_ptr(), bufs[2].data_ptr(), nl.data_ptr(), bufs[3].data_ptr(),
+                        bufs[4].data_ptr(), nr.data_ptr(), mb, mbf, u.data_ptr(), z.data_ptr(), stream.cuda_stream)
     stream.synchronize()
-    return u.cpu().numpy(), z.cpu().numpy()
-
-
-def noisy_keep(n, cap, rng):
-    """Every key once in order, with negative and out-of-capacity entries in between (those outputs must be -1)."""
-    keep, bad = [], []
-    for i in range(n):
-        if rng.random() < 0.1 and len(keep) + 1 < cap - (n - i):
-            bad.append(len(keep))
-            keep.append(int(rng.choice([-1, -7, cap, cap + 5])))
-        keep.append(i)
-    return np.array(keep, np.int32), np.array(bad, np.int64)
+    return sl, sdl, u.cpu().numpy(), z.cpu().numpy()
 
 
 def check_scene(sc, seed=0, device=True):
-    el, er = extractors(500, sc.scale_factor, sc.nlevels)
+    el, er = pair(500, sc.scale_factor, sc.nlevels)
     el(sc.left, None)
     er(sc.right, None)
     ru, rz = O.compute_stereo_matches(sc.kl, sc.dl, sc.kr, sc.dr, el._bordered, er._bordered, el.GetScaleFactors(),
@@ -87,11 +57,11 @@ def check_scene(sc, seed=0, device=True):
     hu, hz = stereo_match(el, er, sc.kl, sc.dl, sc.kr, sc.dr, sc.mb, sc.mbf)
     assert hu.tobytes() == ru.tobytes() and hz.tobytes() == rz.tobytes(), (sc.name, np.nonzero((hu != ru) | (hz != rz))[0])
     if device:
-        keep, bad = noisy_keep(len(sc.kl), el.capacity(), np.random.default_rng(seed))
-        u, z = device_form(el, er, sc.kl, sc.dl, sc.kr, sc.dr, sc.mb, sc.mbf, keep)
-        good = np.setdiff1d(np.arange(len(keep)), bad)
-        assert u[good].tobytes() == hu.tobytes() and z[good].tobytes() == hz.tobytes(), sc.name
-        assert (u[bad] == -1).all() and (z[bad] == -1).all() and (u[len(keep):] == 7.0).all()
+        km = keymap(len(sc.kl), el.capacity(), np.random.default_rng(seed))
+        _, _, u, z = device_form(el, er, km, sc.kl, sc.dl, sc.kr, sc.dr, sc.mb, sc.mbf)
+        bad = np.flatnonzero(km.src < 0)
+        assert u[km.real].tobytes() == hu.tobytes() and z[km.real].tobytes() == hz.tobytes(), sc.name
+        assert (u[bad] == -1).all() and (z[bad] == -1).all() and (u[km.n_keep:] == 7.0).all()
     # the Hamming stage as sivo_stereo_hamming shows it, at the scene's window and with min_d > 0
     rows = sc.left.shape[0]
     for min_d in (0.0, 3.0):
@@ -106,7 +76,7 @@ def check_scene(sc, seed=0, device=True):
 def test_constructed_scene_oracle_host_device_and_hamming_agree(name):
     sc = {s.name: s for s in S.constructed_scenes()}[name]
     trace = []
-    el, er = extractors(500, sc.scale_factor, sc.nlevels)
+    el, er = pair(500, sc.scale_factor, sc.nlevels)
     el(sc.left, None)
     er(sc.right, None)
     O.compute_stereo_matches(sc.kl, sc.dl, sc.kr, sc.dr, el._bordered, er._bordered, el.GetScaleFactors(),
@@ -134,7 +104,7 @@ def test_hamming_99_and_100_and_the_20_bit_index():
         assert dist[0] == want and idx[0] == (0 if want < 100 else -1)
     # 2^20 - 1 right keys, the best at the last index: the index fills all 20 bits of the packed search word
     n = (1 << 20) - 1
-    el, er = extractors(500, sc.scale_factor, sc.nlevels)
+    el, er = pair(500, sc.scale_factor, sc.nlevels)
     el(sc.left, None)
     er(sc.right, None)
     kr = np.zeros(n, KP_DTYPE)
@@ -198,7 +168,7 @@ def test_median_cut_hook_equals_the_oracle():
 
 
 def test_median_cut_at_the_extractor_capacity():
-    el, _ = extractors(500, 1.2, 8)
+    el = extractor(500, 1.2, 8)
     for cap in (el.capacity(), 2000 + 4 * 8 + 64, 5000 + 4 * 8 + 64):
         rng = np.random.default_rng(cap)
         sad = np.where(rng.random(cap) < 0.8, rng.integers(0, 61711, cap), -1)
@@ -221,14 +191,10 @@ def refused_without_writing(el, er, sc, lib_msg):
 
 def device_refused_without_writing(el, er, sc, lib_msg):
     cap = el.capacity()
-    kps = dev_buf(cap, 28, 0)
-    desc = dev_buf(cap, 32, 0)
-    rk = dev_buf(max(len(sc.kr), 1), 28, 0)
-    rd = dev_buf(max(len(sc.kr), 1), 32, 0)
-    n = torch.tensor([len(sc.kl)], dtype=torch.int64, device="cuda")
-    u = torch.full((cap,), 7.0, dtype=torch.float32, device="cuda")
-    z = torch.full((cap,), 7.0, dtype=torch.float32, device="cuda")
-    torch.cuda.synchronize()
+    kps, desc = sentinel(cap * 28, 0, torch.uint8), sentinel(cap * 32, 0, torch.uint8)
+    rk, rd = sentinel(max(len(sc.kr), 1) * 28, 0, torch.uint8), sentinel(max(len(sc.kr), 1) * 32, 0, torch.uint8)
+    n = i64(len(sc.kl))
+    u, z = sentinel(cap, 7.0, torch.float32), sentinel(cap, 7.0, torch.float32)
     with pytest.raises(L.SivoError) as e:
         stereo_match_device(el, er, kps.data_ptr(), desc.data_ptr(), 0, n.data_ptr(), rk.data_ptr(), rd.data_ptr(), n.data_ptr(),
                             sc.mb, sc.mbf, u.data_ptr(), z.data_ptr(), 0)
@@ -239,7 +205,7 @@ def device_refused_without_writing(el, er, sc, lib_msg):
 
 def test_refusals():
     sc = S.sad_scene()
-    el, er = extractors(500, 1.2, 8)
+    el, er = pair(500, 1.2, 8)
     el(sc.left, None)
     # a right image 40 rows shorter, and a right extractor with another scale factor: different level tables
     er(np.ascontiguousarray(sc.right[:-40]), None)
@@ -295,15 +261,10 @@ def test_semantic_keys_of_non_finite_keys(seg):
     assert all(np.array_equal(g, w) for g, w in zip(got, want))
     # the device form
     cap = 64
-    buf = dev_buf(cap, 28, 0)
-    buf[:len(kps) * 28] = upload(kps)
-    cnt = torch.tensor([len(kps)], dtype=torch.int64, device="cuda")
-    cls = torch.full((cap,), 77, dtype=torch.uint8, device="cuda")
-    conf = torch.full((cap,), 7.0, dtype=torch.float64, device="cuda")
-    ent = torch.full((cap,), 7.0, dtype=torch.float64, device="cuda")
-    keep = torch.full((cap,), -7, dtype=torch.int32, device="cuda")
-    nk = torch.zeros(1, dtype=torch.int64, device="cuda")
-    torch.cuda.synchronize()
+    buf = upload(scatter(kps, np.arange(len(kps)), cap, np.zeros(1, KP_DTYPE)))
+    cnt = i64(len(kps))
+    cls, conf, ent = sentinel(cap, 77, torch.uint8), sentinel(cap, 7.0, torch.float64), sentinel(cap, 7.0, torch.float64)
+    keep, nk = sentinel(cap, -7, torch.int32), i64(0)
     seg.semantic_keys_device(buf.data_ptr(), cnt.data_ptr(), cap, 14, cls.data_ptr(), conf.data_ptr(), ent.data_ptr(), keep.data_ptr(),
                              nk.data_ptr(), side.cuda_stream)
     side.synchronize()
@@ -346,7 +307,7 @@ def test_the_rule_is_inert_on_extractor_keys(frame, cfg, kitti_gray_crop):
 def test_differential_fuzz(block):
     for seed in range(block * 20, block * 20 + 20):
         probe = S.fuzz_scene(seed)
-        el, er = extractors(200, probe.scale_factor, probe.nlevels)
+        el, er = pair(200, probe.scale_factor, probe.nlevels)
         ekl, edl = el(probe.left, None)
         ekr, edr = er(probe.right, None)
         rng = np.random.default_rng(seed)
@@ -362,13 +323,11 @@ def test_differential_fuzz(block):
         cap_l, cap_r = el.capacity(), er.capacity()
         nl, nr = min(len(sc.kl), cap_l), min(len(sc.kr), cap_r)
         kind = seed % 5
+        km = keymap(nl, cap_l, rng)
         if kind == 0:  # count -1: nothing written
-            u, z = device_form(el, er, sc.kl[:nl], sc.dl[:nl], sc.kr[:nr], sc.dr[:nr], sc.mb, sc.mbf, np.arange(nl), n_left=-1)
+            _, _, u, z = device_form(el, er, km, sc.kl[:nl], sc.dl[:nl], sc.kr[:nr], sc.dr[:nr], sc.mb, sc.mbf, n_left=-1)
             assert (u == 7.0).all() and (z == 7.0).all()
             continue
-        keep, bad = noisy_keep(nl, cap_l, rng)
-        keep = keep[:cap_l]
-        bad = bad[bad < len(keep)]
         kr, dr = sc.kr[:nr], sc.dr[:nr]
         n_right = None
         if kind == 1:  # a right count above the capacity reads the whole buffer
@@ -376,11 +335,12 @@ def test_differential_fuzz(block):
             kr = np.concatenate([kr, np.repeat(sc.kr[:1], pad)]) if pad and nr else kr
             dr = np.concatenate([dr, np.repeat(sc.dr[:1], pad, 0)]) if pad and nr else dr
             n_right = cap_r + 7
-        n_left = cap_l + 3 if kind == 2 and len(keep) == cap_l else None
-        u, z = device_form(el, er, sc.kl[:nl], sc.dl[:nl], kr, dr, sc.mb, sc.mbf, keep, n_left=n_left, n_right=n_right)
-        good = np.setdiff1d(np.arange(len(keep)), bad)
-        sel = keep[good]
-        wu, wz = O.compute_stereo_matches(sc.kl[sel], sc.dl[sel], kr, dr, el._bordered, er._bordered, el.GetScaleFactors(),
+        n_left = cap_l + 3 if kind == 2 else None  # clamped: the entries past n_keep are valid slots
+        sl, sdl, u, z = device_form(el, er, km, sc.kl[:nl], sc.dl[:nl], kr, dr, sc.mb, sc.mbf, n_left=n_left, n_right=n_right)
+        m = min(km.n_keep if n_left is None else n_left, cap_l)
+        keep = km.keep[:m]
+        good = (keep >= 0) & (keep < cap_l)
+        wu, wz = O.compute_stereo_matches(sl[keep[good]], sdl[keep[good]], kr, dr, el._bordered, er._bordered, el.GetScaleFactors(),
                                           el.GetInverseScaleFactors(), sc.mb, sc.mbf)
-        assert u[good].tobytes() == wu.tobytes() and z[good].tobytes() == wz.tobytes(), seed
-        assert (u[bad] == -1).all() and (u[len(keep):] == 7.0).all()
+        assert u[:m][good].tobytes() == wu.tobytes() and z[:m][good].tobytes() == wz.tobytes(), seed
+        assert (u[:m][~good] == -1).all() and (u[m:] == 7.0).all()

@@ -5,19 +5,20 @@ can fail: crowded windows whose column ranges span several 32-key chunks, exact 
 decision boundary hit exactly, the grid's bounds, the level clamps, the size limits and a seeded differential fuzz.
 
 Every comparison is the same: in_view, match and n_matches of both forms equal the oracle's.  The device form runs on
-extractor-sized buffers with a keep_idx permutation that also holds negative and out-of-capacity entries (keys in no cell),
-decoy records and a blocked mask; the host form on the gathered keys."""
+extractor-sized buffers through an oracle/keymap.py map whose rejected entries are keys in no cell, with decoy records and a
+blocked mask; the host form on the gathered keys."""
 import numpy as np
 import pytest
 import torch
 
-from frame_support import upload
+from frame_support import extractor, i64, sentinel, upload
 from oracle import track_oracle as T
+from oracle.keymap import SLACK, keymap, scatter
+from oracle.track_scene import MP, RESERVED, desc_with, keys, point_at
 from sivo_b200 import _lib as L
-from sivo_b200 import (KP_DTYPE, MAP_POINT_DTYPE, ORBextractor, make_frame, search_last_frame, search_last_frame_device,
+from sivo_b200 import (KP_DTYPE, make_frame, search_last_frame, search_last_frame_device,
                        search_local_points, search_local_points_device)
 from sivo_b200.track import features_in_area
-from test_oracle_track import KP, MP, desc_with, keys, point_at
 
 pytestmark = pytest.mark.gpu
 
@@ -36,21 +37,6 @@ def oframe(bounds=BOUNDS, R=np.eye(3), t=(0, 0, 0)):
     return T.Frame(FX, FX, CX, CY, MBF, bounds, R, t)
 
 
-def kp_records(k):
-    out = np.zeros(len(k), KP_DTYPE)
-    for name in KP.names:
-        out[name] = k[name]
-    return out
-
-
-def mp_records(pts):
-    out = np.zeros(len(pts), MAP_POINT_DTYPE)
-    for name in MP.names:
-        out[name] = pts[name]
-    out["reserved"] = -0x5A5A5A5B  # ignored by both searches
-    return out
-
-
 def point(pos, desc, observed=1, octave=0, angle=0.0, normal=None, max_distance=None):
     """A map point at world position pos (seen head-on from the origin unless a normal is given)."""
     p = np.zeros((), MP)
@@ -59,7 +45,7 @@ def point(pos, desc, observed=1, octave=0, angle=0.0, normal=None, max_distance=
     p["normal"] = p["pos"] / d if normal is None else np.asarray(normal, F32)
     p["max_distance"] = d if max_distance is None else max_distance
     p["min_distance"] = p["max_distance"] / F32(1.2) ** 7
-    p["desc"], p["observed"], p["octave"], p["angle"] = desc, observed, octave, angle
+    p["desc"], p["observed"], p["octave"], p["angle"], p["reserved"] = desc, observed, octave, angle, RESERVED
     return p
 
 
@@ -97,34 +83,23 @@ class Searcher:
         self.rng = np.random.default_rng(seed)
 
     def device(self, sc, last):
-        """The device form: semantic key j sits at a random record of a capacity-sized buffer of decoys; keep_idx also holds
-        invalid entries (negative, >= capacity) whose slots must stay unmatched, and blocked marks those slots."""
+        """The device form: semantic key j sits at its slot of an oracle/keymap.py map, in capacity-sized buffers whose other
+        records are decoys (copies of the scene's keys); the map's rejected entries must stay unmatched, and blocked marks them."""
         n, m, cap = len(sc.k), len(sc.pts), self.cap
-        assert n <= cap, "the device form takes at most the extractor's capacity of keys"
-        holes = min(cap - n, 3 + n // 8)
-        hole = np.zeros(n + holes, bool)
-        hole[self.rng.choice(n + holes, holes, replace=False)] = True
-        slot = np.flatnonzero(~hole)
-        keep = np.full(cap, -9, np.int64)
-        keep[slot] = self.rng.permutation(cap)[:n]
-        keep[np.flatnonzero(hole)] = self.rng.choice([-1, -7, -2 ** 31, cap, cap + 3, 2 ** 31 - 1], holes)
-        kps = np.zeros(cap, KP_DTYPE)
-        desc = self.rng.integers(0, 256, (cap, 32), dtype=np.uint8)
-        if n:
-            kps[:] = kp_records(sc.k)[self.rng.integers(0, n, cap)]
-            kps[keep[slot]] = kp_records(sc.k)
-            desc[keep[slot]] = sc.d
-        ur = self.rng.uniform(-5, 1030, cap).astype(F32)
-        ur[slot] = sc.ur
-        blocked = np.zeros(cap, np.uint8)
-        blocked[np.flatnonzero(hole)] = 1
+        km = keymap(n, cap, self.rng)
+        nk, real, rejected = km.n_keep, km.real, km.src < 0
+        decoy = sc.k[self.rng.integers(0, n, cap + SLACK)] if n else np.zeros(1, KP_DTYPE)
+        kps = scatter(sc.k, km.slots, cap, decoy)
+        desc = scatter(sc.d, km.slots, cap, self.rng.integers(0, 256, (cap + SLACK, 32), dtype=np.uint8))
+        ur = self.rng.uniform(-5, 1030, len(km.keep)).astype(F32)
+        ur[real] = sc.ur
+        blocked = np.zeros(len(km.keep), np.uint8)
+        blocked[np.flatnonzero(rejected)] = 1
         if sc.blocked is not None:
-            blocked[slot] = sc.blocked
-        bufs = [upload(a) for a in (kps, desc, keep.astype(np.int32), np.array([n + holes], np.int64), ur, blocked)]
-        pts = upload(mp_records(sc.pts)) if m else None
-        view = torch.full((max(m, 1),), 7, dtype=torch.uint8, device="cuda")
-        match = torch.full((cap,), -7, dtype=torch.int32, device="cuda")
-        nm = torch.full((1,), -7, dtype=torch.int64, device="cuda")
+            blocked[real] = sc.blocked
+        bufs = [upload(kps), upload(desc), upload(km.keep), i64(nk), upload(ur), upload(blocked)]
+        pts = upload(sc.pts) if m else None
+        view, match, nm = sentinel(max(m, 1), 7, torch.uint8), sentinel(cap, -7, torch.int32), sentinel(1, -7, torch.int64)
         frame, _ = sc.frames()
         p = [b.data_ptr() for b in bufs]
         pp = pts.data_ptr() if m else 0
@@ -137,14 +112,14 @@ class Searcher:
                                        match.data_ptr(), nm.data_ptr())
         torch.cuda.synchronize()
         mt, v = match.cpu().numpy(), view.cpu().numpy()
-        assert (mt[:n + holes][hole] == -1).all() and (mt[n + holes:] == -7).all()
+        assert (mt[:nk][rejected] == -1).all() and (mt[nk:] == -7).all()
         assert (v == 7).all() if last else set(np.unique(v[:m])) <= {0, 1}
-        return v[:m].astype(bool), mt[slot].copy(), int(nm.cpu()[0])
+        return v[:m].astype(bool), mt[real].copy(), int(nm.cpu()[0])
 
     def local(self, sc, per_point=None):
         frame, of = sc.frames()
         ov, om, on = T.search_local_points(sc.k, sc.d, sc.ur, sc.pts, of, self.scale, sc.th, sc.nnratio, sc.blocked, per_point)
-        hv, hm, hn = search_local_points(self.el, kp_records(sc.k), sc.d, sc.ur, mp_records(sc.pts), frame, sc.th, sc.nnratio,
+        hv, hm, hn = search_local_points(self.el, sc.k, sc.d, sc.ur, sc.pts, frame, sc.th, sc.nnratio,
                                          sc.blocked)
         assert np.array_equal(hv, ov) and np.array_equal(hm, om) and hn == on, "host form"
         dv, dm, dn = self.device(sc, False)
@@ -154,7 +129,7 @@ class Searcher:
     def last(self, sc):
         frame, of = sc.frames()
         om, on = T.search_last_frame(sc.k, sc.d, sc.ur, sc.pts, of, sc.Rlw, sc.tlw, self.scale, sc.th)
-        hm, hn = search_last_frame(self.el, kp_records(sc.k), sc.d, sc.ur, mp_records(sc.pts), frame, sc.Rlw, sc.tlw, sc.th)
+        hm, hn = search_last_frame(self.el, sc.k, sc.d, sc.ur, sc.pts, frame, sc.Rlw, sc.tlw, sc.th)
         assert np.array_equal(hm, om) and hn == on, "host form"
         _, dm, dn = self.device(sc, True)
         assert np.array_equal(dm, om) and dn == on, "device form"
@@ -163,12 +138,12 @@ class Searcher:
 
 @pytest.fixture(scope="module")
 def s8():
-    return Searcher(ORBextractor(1000, 1.2, 8, 20, 7), 1)
+    return Searcher(extractor(1000, 1.2, 8), 1)
 
 
 @pytest.fixture(scope="module")
 def s4():
-    return Searcher(ORBextractor(500, 1.5, 4, 20, 7), 2)
+    return Searcher(extractor(500, 1.5, 4), 2)
 
 
 def per_point_changes(s, sc):
@@ -272,7 +247,7 @@ def test_dense_windows_span_several_chunks_and_columns(s8):
         sc, k = dense_scene(seed)
         _, of = sc.frames()
         # the window of a point at the square's centre: some column's walk holds more than 32 candidates
-        got = features_in_area(s8.el, kp_records(k), BOUNDS, [(500.0, 150.0, 24.0, 0, 1)])[0]
+        got = features_in_area(s8.el, k, BOUNDS, [(500.0, 150.0, 24.0, 0, 1)])[0]
         per_col = np.bincount([T.pos_in_grid(k["x"][j], k["y"][j], of)[0] for j in got])
         assert per_col.max() > 64, per_col
         view, m, n = s8.local(sc)
@@ -415,7 +390,7 @@ def test_grid_at_half_cells_bounds_and_clipped_corners(s8):
     q = [(float(x), float(y), float(r), *lv) for x in (of.min_x, of.max_x, 500.3, ulp(of.min_x, DOWN), -30.0, 1060.0)
          for y in (of.min_y, of.max_y, 171.9, ulp(of.max_y, UP)) for r in (0.5, 7.9, 40.0) for lv in ((-1, -1), (0, 0), (2, -1))]
     q += [(float(x), float(y), float(rng.uniform(0.5, 50)), -1, -1) for x, y in xy[:200]]
-    got = features_in_area(s8.el, kp_records(k), ODD, q)
+    got = features_in_area(s8.el, k, ODD, q)
     total = 0
     for a, g in zip(q, got):
         want = T.get_features_in_area(grid, k, of, F32(a[0]), F32(a[1]), F32(a[2]), a[3], a[4])
@@ -558,14 +533,14 @@ def test_host_form_key_limit(s8):
     sc = Scene(k, d, pts, ur=ur, th=1)
     frame, of = sc.frames()
     ov, om, on = T.search_local_points(k, d, ur, pts, of, s8.scale, 1, 0.8)
-    hv, hm, hn = search_local_points(s8.el, kp_records(k), d, ur, mp_records(pts), frame, 1)
+    hv, hm, hn = search_local_points(s8.el, k, d, ur, pts, frame, 1)
     assert np.array_equal(hv, ov) and np.array_equal(hm, om) and hn == on > 100
     om, on = T.search_last_frame(k, d, ur, pts, of, np.eye(3), np.zeros(3), s8.scale, 7)
-    hm, hn = search_last_frame(s8.el, kp_records(k), d, ur, mp_records(pts), frame, np.eye(3), np.zeros(3), 7)
+    hm, hn = search_last_frame(s8.el, k, d, ur, pts, frame, np.eye(3), np.zeros(3), 7)
     assert np.array_equal(hm, om) and hn == on > 100
     k1, d1, u1 = np.concatenate([k, k[:1]]), np.concatenate([d, d[:1]]), np.concatenate([ur, ur[:1]])
-    for call in (lambda: search_local_points(s8.el, kp_records(k1), d1, u1, mp_records(pts), frame, 1),
-                 lambda: search_last_frame(s8.el, kp_records(k1), d1, u1, mp_records(pts), frame, np.eye(3), np.zeros(3), 7)):
+    for call in (lambda: search_local_points(s8.el, k1, d1, u1, pts, frame, 1),
+                 lambda: search_last_frame(s8.el, k1, d1, u1, pts, frame, np.eye(3), np.zeros(3), 7)):
         with pytest.raises(L.SivoError) as e:
             call()
         assert e.value.code == L.EINVAL
@@ -595,7 +570,7 @@ def test_fifty_thousand_points_on_a_handful_of_keys(s8):
     pts["pos"][::3, 2] *= -1  # a third behind the camera
     sc = Scene(k, d, pts, th=3)
     frame, of = sc.frames()
-    hv, hm, hn = search_local_points(s8.el, kp_records(k), d, sc.ur, mp_records(pts), frame, 3)
+    hv, hm, hn = search_local_points(s8.el, k, d, sc.ur, pts, frame, 3)
     dv, dm, dn = s8.device(sc, False)
     assert np.array_equal(dv, hv) and np.array_equal(dm, hm) and dn == hn
     lg = T.logf(s8.scale[1])
@@ -603,7 +578,7 @@ def test_fifty_thousand_points_on_a_handful_of_keys(s8):
     assert [T.is_in_frustum(pts[i], of, lg, 8) is not None for i in sample] == list(hv[sample])
     assert 0.4 < hv.mean() < 0.8
     s8.local(Scene(k, d, pts[:3000], th=3))
-    hm, hn = search_last_frame(s8.el, kp_records(k), d, sc.ur, mp_records(pts), frame, np.eye(3), np.zeros(3), 7)
+    hm, hn = search_last_frame(s8.el, k, d, sc.ur, pts, frame, np.eye(3), np.zeros(3), 7)
     _, dm, dn = s8.device(Scene(k, d, pts, th=7), True)
     assert np.array_equal(dm, hm) and dn == hn and hn > 0
     s8.last(Scene(k, d, pts[:3000], th=7))
@@ -626,8 +601,8 @@ def test_angle_rule_on_both_forms(s8):
         kb = k.copy()
         kb["angle"] = 0.0
         kb["angle"][3] = a
-        for call in (lambda: search_local_points(s8.el, kp_records(kb), d, np.full(n, -1, F32), mp_records(np.array(pts, MP)), frame, 1),
-                     lambda: search_last_frame(s8.el, kp_records(kb), d, np.full(n, -1, F32), mp_records(np.array(pts, MP)), frame,
+        for call in (lambda: search_local_points(s8.el, kb, d, np.full(n, -1, F32), np.array(pts, MP), frame, 1),
+                     lambda: search_last_frame(s8.el, kb, d, np.full(n, -1, F32), np.array(pts, MP), frame,
                                                np.eye(3), np.zeros(3), 7)):
             with pytest.raises(L.SivoError) as e:
                 call()
@@ -635,7 +610,7 @@ def test_angle_rule_on_both_forms(s8):
         pb = np.array(pts, MP)
         pb["angle"][3] = a
         with pytest.raises(L.SivoError) as e:
-            search_last_frame(s8.el, kp_records(k), d, np.full(n, -1, F32), mp_records(pb), frame, np.eye(3), np.zeros(3), 7)
+            search_last_frame(s8.el, k, d, np.full(n, -1, F32), pb, frame, np.eye(3), np.zeros(3), 7)
         assert e.value.code == L.ERANGE, a
         s8.local(Scene(k, d, pb))  # the local search does not read point angles
     # device forms: keys with bad angles are no candidates; last-frame points with bad angles are not searched

@@ -7,49 +7,9 @@ import pytest
 from scipy.linalg import expm
 
 from oracle import pose_oracle as P
+from oracle.pose_scene import CAM, INV_SIGMA2, exact_scene, pose34, rotation, scene
 
 F32 = np.float32
-KP_DTYPE = np.dtype([("x", "<f4"), ("y", "<f4"), ("size", "<f4"), ("angle", "<f4"), ("response", "<f4"), ("octave", "<i4"),
-                     ("class_id", "<i4")])
-INV_SIGMA2 = (F32(1) / np.array([F32(1.2 ** (2 * l)) for l in range(8)], F32)).astype(F32)
-CAM = P.Camera(718.856, 718.856, 498.1928, 174.2157, 386.1448)
-
-
-def rotation(ax, ay, az):
-    return expm(np.array([[0, -az, ay], [az, 0, -ax], [-ay, ax, 0]], float))
-
-
-def pose34(R, t):
-    return np.concatenate([np.asarray(R, float), np.asarray(t, float).reshape(3, 1)], 1).astype(F32)
-
-
-def scene(seed, n=300, mode="mixed", outliers=0.0, noise=0.5, motion=(0.01, 0.05), cam=CAM, size=(1024, 352)):
-    """A frame seen from a true pose: keys at random pixels and depths, their points placed in the world exactly, pixel noise
-    (sigma `noise` times the octave's scale), a fraction of the points replaced by gross outliers, and an initial pose moved by
-    `motion` (rotation rad, translation m).  mode: "mono" (u_right < 0), "stereo" or "mixed".  Returns (kps, u_right, xw,
-    Tcw_in, Tcw_true)."""
-    rng = np.random.default_rng(seed)
-    R = rotation(*rng.uniform(-0.2, 0.2, 3))
-    t = rng.uniform(-2, 2, 3)
-    u = rng.uniform(0, size[0], n)
-    v = rng.uniform(0, size[1], n)
-    z = rng.uniform(3, 40, n)
-    Pc = np.stack([(u - cam.cx) * z / cam.fx, (v - cam.cy) * z / cam.fy, z], 1)
-    X = ((Pc - t) @ R).astype(F32)
-    oct_ = rng.integers(0, 8, n)
-    sc = 1.2 ** oct_
-    kps = np.zeros(n, KP_DTYPE)
-    kps["x"] = u + noise * sc * rng.standard_normal(n)
-    kps["y"] = v + noise * sc * rng.standard_normal(n)
-    kps["octave"] = oct_
-    ur = (u - cam.mbf / z + noise * sc * rng.standard_normal(n)).astype(F32)
-    stereo = {"mono": np.zeros(n, bool), "stereo": np.ones(n, bool), "mixed": rng.uniform(size=n) < 0.6}[mode]
-    ur = np.where(stereo, np.maximum(ur, F32(0)), F32(-1)).astype(F32)
-    bad = rng.permutation(n)[:int(round(outliers * n))]
-    X[bad] = (X[bad] + rng.uniform(-5, 5, (len(bad), 3))).astype(F32)
-    dR = rotation(*rng.uniform(-motion[0], motion[0], 3))
-    dt = rng.uniform(-motion[1], motion[1], 3)
-    return kps, ur, X, pose34(dR @ R, t + dt), pose34(R, t)
 
 
 def rot_err(q, R):
@@ -149,28 +109,6 @@ def test_cholesky_refuses_a_singular_matrix():
 
 
 # ---------------------------------------------------------------------------------------------------------- whole optimisation
-def exact_scene(mode):
-    """Observations that are exact floats of exact projections at the identity pose (fx = 512, power-of-two depths), so the
-    optimum is the identity."""
-    cam = P.Camera(512.0, 512.0, 320.0, 240.0, 256.0)
-    rng = np.random.default_rng(7)
-    n = 64
-    z = 2.0 ** rng.integers(1, 5, n)
-    x = rng.integers(-200, 200, n) / 64.0
-    y = rng.integers(-150, 150, n) / 64.0
-    kps = np.zeros(n, KP_DTYPE)
-    kps["x"] = (x / z) * 512 + 320
-    kps["y"] = (y / z) * 512 + 240
-    kps["octave"] = rng.integers(0, 8, n)
-    ur = (kps["x"] - 256 / z).astype(F32)
-    if mode == "mono":
-        ur[:] = -1
-    elif mode == "mixed":
-        ur[::3] = -1
-    X = np.stack([x, y, z], 1).astype(F32)
-    return cam, kps, ur, X
-
-
 @pytest.mark.parametrize("mode", ["mono", "stereo", "mixed"])
 def test_noise_free_scenes_converge_to_the_true_pose(mode):
     cam, kps, ur, X = exact_scene(mode)

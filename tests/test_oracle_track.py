@@ -4,43 +4,13 @@ import cv2
 import numpy as np
 
 from oracle import track_oracle as T
+from oracle.track_scene import MP, SCALE, desc_with, keys, point_at
 
-KP = np.dtype([("x", np.float32), ("y", np.float32), ("size", np.float32), ("angle", np.float32), ("response", np.float32),
-               ("octave", np.int32), ("class_id", np.int32)])
-MP = np.dtype([("desc", np.uint8, 32), ("pos", np.float32, 3), ("normal", np.float32, 3), ("min_distance", np.float32),
-               ("max_distance", np.float32), ("observed", np.int32), ("octave", np.int32), ("angle", np.float32)])
-SCALE = np.float32(1.2) ** np.arange(8, dtype=np.float32)
 BOUNDS = (0.0, 1024.0, 0.0, 352.0)
 
 
 def frame(R=np.eye(3), t=(0, 0, 0)):
     return T.Frame(700.0, 700.0, 512.0, 176.0, 380.0, BOUNDS, R, t)
-
-
-def keys(xy, octave=0, angle=0.0):
-    k = np.zeros(len(xy), KP)
-    k["x"], k["y"] = np.asarray(xy, np.float32).T
-    k["octave"], k["angle"] = octave, angle
-    return k
-
-
-def desc_with(bits):
-    d = np.zeros(32, np.uint8)
-    for b in bits:
-        d[b // 8] |= 1 << (b % 8)
-    return d
-
-
-def point_at(f, u, v, z, desc, observed=1, octave=0, angle=0.0):
-    """A point that projects to (u, v) at depth z through the identity pose, seen head-on at its own distance."""
-    p = np.zeros((), MP)
-    x, y = (u - f.cx) * z / f.fx, (v - f.cy) * z / f.fy
-    p["pos"] = (x, y, z)
-    d = np.float32(np.sqrt(x * x + y * y + z * z))
-    p["normal"] = np.array([x, y, z], np.float32) / d
-    p["max_distance"], p["min_distance"] = d, d / SCALE[-1]
-    p["desc"], p["observed"], p["octave"], p["angle"] = desc, observed, octave, angle
-    return p
 
 
 def test_norm_and_pose_gemms_equal_cv2():
