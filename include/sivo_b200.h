@@ -880,6 +880,13 @@ int sivo_dbg_conv(int device, int engine, int precision, const float* in, int n,
  * NCHW [n][cout][2h][2w], cout <= 16, k = 7, no ReLU.  Equals sivo_dbg_unpool followed by sivo_dbg_conv bit for bit. */
 int sivo_dbg_conv_unpooled(int device, const float* pooled, const int* mask, int n, int mask_n, int h, int w, const float* weight,
                            const float* bias, const float* bn_scale, const float* bn_shift, int cout, int k, float* out);
+/* The 7x7 64 -> 64 half convolution (Basic's decoder layers: bias, no ReLU) over the max-unpool of `pooled` by `mask`
+ * (conventions as above): out = float NCHW [n][64][2h][2w].  drop_layer >= 0: the sampling dropout of that layer (seed,
+ * frame; image i is sample i, scale 2) is applied in its epilogue.  unpool_on_load = 1: the kernel expands the pooled input
+ * as it loads its input rows; 0: the unpool kernel writes the unpooled tensor and the same convolution reads it.  The two
+ * are equal bit for bit. */
+int sivo_dbg_conv64_unpooled(int device, const float* pooled, const int* mask, int n, int mask_n, int h, int w, const float* weight,
+                             const float* bias, int drop_layer, uint64_t seed, uint64_t frame, int unpool_on_load, float* out);
 int sivo_dbg_lrn(int device, const float* in, int n, int c, int h, int w, int size, float alpha, float beta,
                  float k, float* out);
 int sivo_dbg_mc_reduce(int device, const float* logits, int T, int c, int h, int w, uint8_t* classes,

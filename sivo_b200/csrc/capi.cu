@@ -1038,4 +1038,36 @@ int sivo_dbg_conv_unpooled(int device, const float* pooled, const int* mask, int
   });
 }
 
+int sivo_dbg_conv64_unpooled(int device, const float* pooled, const int* mask, int n, int mask_n, int h, int w, const float* weight,
+                             const float* bias, int drop_layer, uint64_t seed, uint64_t frame, int unpool_on_load, float* out) {
+  return guarded([&] {
+    if (!pooled || !mask || !weight || !out) fail(SIVO_EINVAL, "conv64_unpooled: null argument");
+    if (n < 1 || mask_n < 1 || mask_n > n || h < 1 || w < 1) fail(SIVO_EINVAL, "conv64_unpooled: needs n, h, w >= 1 and 1 <= mask_n <= n");
+    SIVO_CUDA(cudaSetDevice(device));
+    const size_t mask_cnt = static_cast<size_t>(mask_n) * 64 * h * w;
+    DevBuf bp, bu, bo, bm(mask_cnt), bmi(mask_cnt * sizeof(int)), bf(sizeof(uint64_t));
+    TensorView vp = make_view(bp, n, 64, h, w, 64, DType::F16);
+    TensorView vu = make_view(bu, n, 64, 2 * h, 2 * w, 64, DType::F16);
+    TensorView vo = make_view(bo, n, 64, 2 * h, 2 * w, 64, DType::F16);
+    upload_nchw(pooled, vp);
+    SIVO_CUDA(cudaMemcpy(bmi.p, mask, mask_cnt * sizeof(int), cudaMemcpyHostToDevice));
+    SIVO_CUDA(cudaMemcpy(bf.p, &frame, sizeof(uint64_t), cudaMemcpyHostToDevice));
+    launch_mask_from_nchw(bmi.as<int>(), mask_n, 64, h, w, bm.as<uint8_t>(), nullptr);
+    Op op;
+    op.kind = Op::Conv;
+    op.layer = "dbg_conv64_unpooled";
+    op.k = 7; op.pad = 3; op.cin = op.cin_p = 64; op.cout = op.cout_p = 64;
+    op.use_tc = true;
+    if (!conv_tc_supported(op, vu, vo)) fail(SIVO_EINVAL, "conv64_unpooled: shape not supported by the tensor-core kernel");
+    prepare_conv(op, DType::F16, weight, bias, nullptr, nullptr, vu, vo);
+    if (drop_layer >= 0) conv_tc_set_dropout(*op.tc, seed, bf.as<uint64_t>(), drop_layer, 2.f, 0);
+    if (unpool_on_load) conv_tc_set_unpool_input(*op.tc, vp.p, bm.as<uint8_t>(), mask_n, h, w);
+    else launch_unpool(vp, bm.as<uint8_t>(), mask_n, vu, nullptr);
+    launch_conv(op, vu, vo, nullptr);
+    SIVO_CUDA(cudaDeviceSynchronize());
+    download_nchw(vo, out);
+    SIVO_CUDA(cudaDeviceSynchronize());
+  });
+}
+
 }  // extern "C"

@@ -28,7 +28,7 @@
 //    shared-memory data path to the MMA operand reads.
 //  * The Cin = 64, 7x7 layers with 64-wide half output tiles (Basic's conv1 .. conv_decode2) run on k_conv_tn instead: the
 //    same producers and rings with the GEMM transposed -- the weights as M, all 128 pixels of a row as N -- and an
-//    epilogue staged through shared memory.
+//    epilogue staged through shared memory.  Fed by a max-unpool (Basic's decoder), it unpools as it loads its halo rows.
 //  * The 64 -> 16 float-logits layers (K = 3, 7) run on k_conv_stack instead: tap rows stacked along N, resident weights.
 //    Fed by a max-unpool (Basic's composed classifier), it unpools the pooled tensor as it loads its halo rows.
 #include <cuda.h>
@@ -92,8 +92,9 @@ struct TcParams {
   // written (pooling_layer.cpp:140-187: scan (0,0),(0,1),(1,0),(1,1), strict '>', so the first maximum wins)
   __half* pool_out;        // [N][H/2][W/2][cout_total]
   uint8_t* pool_mask;      // same shape
-  // k_conv_stack<K, true>: the input is the max-unpool of this pooled tensor [N][H/2][W/2][64] by unpool_mask (same shape,
-  // batch mask_n), expanded as the halo rows are loaded; the 2H x 2W unpooled tensor is never stored
+  // k_conv_stack<K, true>, k_conv_tn<7, 7, true>: the input is the max-unpool of this pooled tensor [N][H/2][W/2][64] by
+  // unpool_mask (same shape, batch mask_n), expanded as the halo rows are loaded; the H x W unpooled tensor is never
+  // stored, and the epilogue does not scatter (unpool_mask is the input's)
   const __half* unpool_in;
 };
 
@@ -467,9 +468,88 @@ __host__ __device__ constexpr int tc_stages(int K, bool roll, int n, int stage_b
   return 0;
 }
 
+// The halo-row producer of a convolution whose input is a max-unpool (k_conv_stack<K, true>, k_conv_tn<K, K, true>), run
+// by NT threads of warpgroup 0: each halo row -- input row y of the H x W unpooled tensor, pixels x0 - pad .. x0 + 127 + pad
+// -- is expanded from pooled row y / 2 straight into its ring slot.  Per pooled pixel j and 8-channel chunk c, one thread
+// loads the 16 bytes of values and the 8 mask bytes and writes the 16-byte chunks of pixels 2 j and 2 j + 1: each channel
+// keeps its value where its mask code is 2 (y & 1) + dx and is zero elsewhere, the select the unpool kernel makes, so the
+// slot holds the bits the unpooled tensor would.  Chunks go to their SWIZZLE_128B position (the slots are 1 KB aligned);
+// rows and pixels outside the image are written as zeros, since slots are reused (TMA's zero fill in the plain kernels).
+// A row's loads are issued before the wait for its slot, so their latency hides under the consumers' MMAs of the
+// previous row.
+template <int K, int NT>
+struct HaloUnpool {
+  static constexpr int kPad = (K - 1) / 2;
+  static constexpr int kHalo = 128 + K - 1;
+  static constexpr int kLeft = (kPad + 1) / 2;                  // pooled pixels the halo reaches left of x0 / 2
+  static constexpr int kPooled = kLeft + (127 + kPad) / 2 + 1;  // pooled pixels per halo row (68 for K = 7)
+  static constexpr int kJStep = NT / 8;                         // pooled pixels between a thread's consecutive steps
+  static constexpr int kSteps = (kPooled + kJStep - 1) / kJStep;  // (pixel, chunk) pairs per thread
+  static_assert(NT % 32 == 0 && kJStep % 4 == 0, "whole warps; steps 2 kJStep pixels apart keep the swizzle phase");
+  // thread tid: chunk c of pooled pixels j = jt + kJStep s (halo-relative jr = jr0 + kJStep s); the addresses of steps s
+  // differ by compile-time strides, so a row needs one pointer per tensor
+  const int c, jr0;
+  const int px0;  // halo pixel of (jr0, dx = 0): image pixel x0 - pad + px = 2 j + dx.  Its swizzle phase px & 7 is the same for every step.
+  int jt = 0;
+  uint32_t live = 0;  // steps whose pooled pixel is inside the image
+  long v_img = 0, m_img = 0;
+
+  __device__ __forceinline__ explicit HaloUnpool(int tid) : c(tid & 7), jr0(tid >> 3), px0(2 * (tid >> 3) + kPad - 2 * kLeft) {}
+
+  // the strip starting at pixel x0 of image img
+  __device__ __forceinline__ void strip(const TcParams& p, int img, int x0) {
+    const int Hp = p.H >> 1, Wp = p.W >> 1;
+    jt = (x0 >> 1) - kLeft + jr0;
+    live = 0;
+#pragma unroll
+    for (int s = 0; s < kSteps; ++s)
+      if (jr0 + kJStep * s < kPooled && jt + kJStep * s >= 0 && jt + kJStep * s < Wp) live |= 1u << s;
+    v_img = static_cast<long>(img) * Hp;
+    m_img = static_cast<long>(img % p.mask_n) * Hp;
+  }
+
+  // Input row y into slot `dst` once `empty` completes phase `parity`; every warp arrives on `full` once it has written its share.
+  __device__ __forceinline__ void row(const TcParams& p, int y, uint8_t* dst, uint64_t* full, uint64_t* empty, uint32_t parity) const {
+    const int Wp = p.W >> 1;
+    const uint32_t row_live = y >= 0 && y < p.H ? live : 0u;
+    const __half* const vp = p.unpool_in + ((v_img + (y >> 1)) * Wp + jt) * 64 + 8 * c;
+    const uint8_t* const mp = p.unpool_mask + ((m_img + (y >> 1)) * Wp + jt) * 64 + 8 * c;
+    uint4 v[kSteps];
+    uint2 m[kSteps];
+#pragma unroll
+    for (int s = 0; s < kSteps; ++s) {
+      v[s] = make_uint4(0u, 0u, 0u, 0u);
+      m[s] = make_uint2(0u, 0u);
+      if (row_live & (1u << s)) {
+        v[s] = __ldg(reinterpret_cast<const uint4*>(vp + s * kJStep * 64));
+        m[s] = __ldg(reinterpret_cast<const uint2*>(mp + s * kJStep * 64));
+      }
+    }
+    mbar_wait(empty, parity);
+#pragma unroll
+    for (int dx = 0; dx < 2; ++dx) {
+      const int px = px0 + dx;
+      uint8_t* const d = dst + px * 128 + ((c ^ (px & 7)) << 4);
+      const uint32_t code = 0x01010101u * static_cast<uint32_t>(2 * (y & 1) + dx);
+#pragma unroll
+      for (int s = 0; s < kSteps; ++s) {
+        if (jr0 + kJStep * s >= kPooled || px + 2 * kJStep * s < 0 || px + 2 * kJStep * s >= kHalo) continue;
+        const uint32_t lo = __vcmpeq4(m[s].x, code), hi = __vcmpeq4(m[s].y, code);  // 0xFF per matching byte
+        const uint4 o = make_uint4(v[s].x & __byte_perm(lo, 0u, 0x1100), v[s].y & __byte_perm(lo, 0u, 0x3322),
+                                   v[s].z & __byte_perm(hi, 0u, 0x1100), v[s].w & __byte_perm(hi, 0u, 0x3322));
+        *reinterpret_cast<uint4*>(d + s * 2 * kJStep * 128) = o;
+      }
+    }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes, read by wgmma
+    __syncwarp();
+    if ((threadIdx.x & 31) == 0) mbar_arrive(full);
+  }
+};
+
 // TcCta: what k_conv_tc and k_conv_tn share -- the CTA's shared-memory carve-up (see tc_smem_bytes), its place in the
 // (strip, row block, cout tile, image) grid, and warpgroup 0's producers that fill the two rings.
-template <int K, bool ROLL, int KW, bool PK2, int N>
+// UNPOOL (ROLL only): warps 0, 2 and 3 expand the halo rows from the pooled input (HaloUnpool) instead of warp 0's TMA.
+template <int K, bool ROLL, int KW, bool PK2, int N, bool UNPOOL = false>
 struct TcCta {
   static constexpr int RK = kRows + K - 1;           // halo rows one row block reads (per chunk)
   static constexpr int kSlots = tc_slots(K, ROLL);
@@ -477,6 +557,8 @@ struct TcCta {
   static constexpr int b_bytes = N * 128;
   static constexpr int b_stride = tc_b_stride(N);
   static constexpr int UPC = PK2 ? KW * RK : RK;     // halo units per (row block, chunk)
+  static_assert(!UNPOOL || (ROLL && KW == K), "the unpooled input is one 64-channel chunk, not window-folded");
+  static constexpr int kExpandThreads = 96;          // UNPOOL: warps 0, 2, 3
   uint8_t *a_slots, *b_stages, *stage;
   uint64_t *a_full, *a_empty, *b_full, *b_empty;   // [kSlots], [kSlots], [kBStages], [kBStages]
   int kBStages, n0, img, x0, NC, npairs, y_base, n_units;
@@ -503,18 +585,30 @@ struct TcCta {
   }
 
   __device__ __forceinline__ void init_barriers() const {
-    for (int i = 0; i < kSlots; ++i) { mbar_init(a_full + i, 1); mbar_init(a_empty + i, kEmptyArrivals); }
+    // UNPOOL: each expanding warp arrives once it has written its share of a halo row (no transaction bytes)
+    for (int i = 0; i < kSlots; ++i) { mbar_init(a_full + i, UNPOOL ? kExpandThreads / 32 : 1); mbar_init(a_empty + i, kEmptyArrivals); }
     for (int i = 0; i < kBStages; ++i) { mbar_init(b_full + i, 1); mbar_init(b_empty + i, kEmptyArrivals); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
 
   // Warpgroup 0: warp 0 streams the halo rows, warp 1 the weight tiles; the other producer threads have nothing to do.
+  // UNPOOL: warps 0, 2 and 3 expand the halo rows.
   __device__ __forceinline__ void produce(const CUtensorMap& map_a, const CUtensorMap& map_b, const TcParams& p, int warp, int lane) const {
     // 384 threads start with 168 registers each; the producers need few, the consumers (the accumulators, the split sums,
-    // the epilogue's packed outputs) many: 128 x 40 + 256 x 232 = 64 512 <= 65 536
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
-    if (warp == 0 && lane == 0) {
+    // the epilogue's packed outputs) many: 128 x 40 + 256 x 232 = 64 512 <= 65 536.  UNPOOL: the expanding producers keep a
+    // row's loads in flight (36 registers of values and masks per thread): 128 x 88 + 256 x 208 = 64 512
+    if constexpr (UNPOOL) asm volatile("setmaxnreg.dec.sync.aligned.u32 88;" ::: "memory");
+    else asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+    if (UNPOOL && warp != 1) {
+      // ===== halo-row expansion =====
+      HaloUnpool<K, kExpandThreads> h(threadIdx.x - (warp >= 2 ? 32 : 0));
+      h.strip(p, img, x0);
+      for (int u = 0; u < n_units; ++u) {
+        const int slot = u % kSlots;
+        h.row(p, y_base - kPad + u, a_slots + slot * kSlotBytes, a_full + slot, a_empty + slot, ((u / kSlots) & 1) ^ 1);
+      }
+    } else if (!UNPOOL && warp == 0 && lane == 0) {
       // ===== halo-row producer =====
       asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_a)) : "memory");
       for (int u = 0; u < n_units; ++u) {
@@ -738,8 +832,12 @@ k_conv_tc(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUt
 //    tile in SWIZZLE_128B chunk order (one 16-byte chunk = 8 channels of a pixel).  Once both rows are there (named barrier
 //    over the two consumers) the stores go out in 16-byte units (pixel, 8 channels), one slice per tap row of the next
 //    block right after its first MMA group is committed, the last block's at the end: a store, dropout (keep bits drawn
-//    once per pixel), the max-unpool scatter, or 2x2 max-pool + argmax over four staged pixels.  A second barrier before
-//    the next staging keeps the single tile safe.
+//    once per pixel) and a store, or 2x2 max-pool + argmax over four staged pixels.  A second barrier before the next
+//    staging keeps the single tile safe.  There is no max-unpool scatter: a max-unpool that follows is expanded by its
+//    consumer as it loads (UNPOOL below) or runs as its own kernel.
+//  * UNPOOL: the input is a max-unpool (Basic's upsample4 .. upsample2 -> conv_decode4 .. conv_decode2); warps 0, 2 and 3
+//    expand each halo row from the pooled tensor and its mask (HaloUnpool) instead of warp 0's TMA, so the unpooled
+//    tensor, three quarters zeros, is neither written nor read back.  The consumers are unchanged.
 constexpr int kTnStageBytes = kRows * 128 * 128;  // [kRows][128 px][64 ch] half
 constexpr int kTnUnits = kRows * 128 * 8 / 256;   // 16-byte store units per consumer thread per block (2x2 pool: 2)
 
@@ -758,11 +856,11 @@ __device__ __forceinline__ void consumers_sync() { asm volatile("bar.sync 1, 256
 __device__ __forceinline__ uint32_t tn_chunk(uint32_t s_base, int r, int px, int c) {
   return s_base + static_cast<uint32_t>(r * (128 * 128) + px * 128 + ((c ^ (px & 7)) << 4));
 }
-template <int K, int KW>
+template <int K, int KW, bool UNPOOL = false>
 __global__ void __launch_bounds__(kTcThreads, 1)
 k_conv_tn(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const __grid_constant__ TcParams p,
           const __grid_constant__ TcConsts cst) {
-  using Cta = TcCta<K, true, KW, false, 64>;
+  using Cta = TcCta<K, true, KW, false, 64, UNPOOL>;
   constexpr int kSlots = Cta::kSlots, b_stride = Cta::b_stride;
   static_assert(K >= kRows, "a block's own halo rows are released by its tap rows kh < kRows");
   static_assert(tc_stages(K, true, 64, kTnStageBytes) > 0, "halo ring + staging tile + 3 weight stages must fit in shared memory");
@@ -774,7 +872,8 @@ k_conv_tn(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUt
     cta.produce(map_a, map_b, p, warp, lane);
     return;
   }
-  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+  if constexpr (UNPOOL) asm volatile("setmaxnreg.inc.sync.aligned.u32 208;" ::: "memory");
+  else asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
   const int g = wg - 1;             // output row y0 + g of every block
   const int t = threadIdx.x - 128;  // consumer thread
   const int n0 = cta.n0, img = cta.img, x0 = cta.x0, kBStages = cta.kBStages;
@@ -782,12 +881,11 @@ k_conv_tn(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUt
   const bool releaser = lane == 0;
   const int c_lo = n0 + 16 * (warp & 3) + (lane >> 2);  // this thread's couts (rows of D^T): c_lo, c_lo + 8
 
-  // The staged block: its first row, and per store unit i of this thread -- chunk t % 8 of pixel t / 8 + 32 (i % 4) of
-  // row i / 4 (pool: pooled pixel t / 8 + 32 i) -- the unpool mask bytes.  Lane l draws the dropout keep bits of the
-  // pixel of unit l / 4 of lane 8 (l % 4) (two words: the tile's 64 channels) and shuffles them to its owners.
+  // The staged block's first row.  Store unit i of this thread is chunk t % 8 of pixel t / 8 + 32 (i % 4) of row i / 4
+  // (pool: pooled pixel t / 8 + 32 i).  Lane l draws the dropout keep bits of the pixel of unit l / 4 of lane 8 (l % 4)
+  // (two words: the tile's 64 channels) and shuffles them to its owners.
   int ys = 0;
   bool pending = false;
-  uint2 mk[kTnUnits] = {};
   uint32_t keep[2] = {0xFFFFFFFFu, 0xFFFFFFFFu};
   const int c = t & 7;
   auto flush_store = [&](int i) {
@@ -800,9 +898,8 @@ k_conv_tn(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUt
       v = make_uint4(drop_word(v.x, kb, 0, p.drop_scale), drop_word(v.y, kb, 2, p.drop_scale), drop_word(v.z, kb, 4, p.drop_scale),
                      drop_word(v.w, kb, 6, p.drop_scale));
     }
-    if (!(y < p.H && x < p.W)) return;
-    if (p.unpool_mask) unpool_store8(p, img, y, x, n0 + 8 * c, v, mk[i]);
-    else *reinterpret_cast<uint4*>(static_cast<__half*>(p.out) + ((static_cast<size_t>(img) * p.H + y) * p.W + x) * p.cout_total + n0 + 8 * c) = v;
+    if (y < p.H && x < p.W)
+      *reinterpret_cast<uint4*>(static_cast<__half*>(p.out) + ((static_cast<size_t>(img) * p.H + y) * p.W + x) * p.cout_total + n0 + 8 * c) = v;
   };
   auto flush_pool = [&](int i) {  // the window's four staged pixels, in scan order
     const int pp = (t >> 3) + 32 * i, x = x0 + 2 * pp;
@@ -898,15 +995,6 @@ k_conv_tn(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUt
     consumers_sync();  // both rows staged
     ys = cta.y_base + j * kRows;
     pending = true;
-    if (p.unpool_mask) {  // the mask loads are in flight under the next block's first MMAs
-#pragma unroll
-      for (int i = 0; i < kTnUnits; ++i) {
-        const int y = ys + (i >> 2), x = x0 + (t >> 3) + 32 * (i & 3);
-        mk[i] = make_uint2(0u, 0u);
-        if (y < p.H && x < p.W)
-          mk[i] = __ldg(reinterpret_cast<const uint2*>(p.unpool_mask + ((static_cast<size_t>(img % p.mask_n) * p.H + y) * p.W + x) * p.cout_total + n0 + 8 * c));
-      }
-    }
   }
   if (pending)
     for (int kh = 0; kh < K; ++kh) flush_slice(kh);
@@ -958,75 +1046,22 @@ __device__ __forceinline__ void stack_row(float (&acc)[K][8], uint32_t a_row, ui
   }
 }
 
-// The halo producer of k_conv_stack<K, true>, run by all four warps of warpgroup 0: each halo row -- input row y of the
-// 2H x 2W unpooled tensor, pixels x0 - pad .. x0 + 127 + pad -- is expanded from pooled row y / 2 straight into its ring
-// slot.  Per pooled pixel j and 8-channel chunk c, one thread loads the 16 bytes of values and the 8 mask bytes and writes
-// the 16-byte chunks of pixels 2 j and 2 j + 1: each channel keeps its value where its mask code is 2 (y & 1) + dx and is
-// zero elsewhere, the select epilogue_flush scatters with, so the slot holds the bits the unpooled tensor would.  Chunks go
-// to their SWIZZLE_128B position (the slots are 1 KB aligned); rows and pixels outside the image are written as zeros,
-// since slots are reused (TMA's zero fill in the plain kernel).  A row's loads are issued before the wait for its slot, so
-// their latency hides under the consumers' MMAs of the previous row.
+// The halo producer of k_conv_stack<K, true>, run by all four warps of warpgroup 0 (HaloUnpool): per run of output rows
+// within one strip, input rows y_start - pad .. y_end - 1 + pad.
 template <int K>
 __device__ __forceinline__ void stack_unpool_producer(const TcParams& p, uint8_t* a_slots, uint64_t* a_full, uint64_t* a_empty,
                                                       long t_begin, long t_end) {
   constexpr int kPad = (K - 1) / 2;
   constexpr int kSlots = stack_slots(K);
-  constexpr int kHalo = 128 + K - 1;
-  constexpr int kLeft = (kPad + 1) / 2;                  // pooled pixels the halo reaches left of x0 / 2
-  constexpr int kPooled = kLeft + (127 + kPad) / 2 + 1;  // pooled pixels per halo row (68 for K = 7)
-  constexpr int kSteps = (kPooled * 8 + 127) / 128;      // (pixel, chunk) pairs per thread
-  // thread: chunk c of pooled pixels j = jt + 16 s (halo-relative jr = jr0 + 16 s); the addresses of steps s differ by
-  // compile-time strides, so a row needs one pointer per tensor
-  const int tid = threadIdx.x, c = tid & 7, lane = tid & 31, jr0 = tid >> 3;
-  const int Hp = p.H >> 1, Wp = p.W >> 1;
-  // halo pixel of (jr0, dx): image pixel x0 - pad + px = 2 j + dx.  Its swizzle phase px & 7 is the same for every step.
-  const int px0 = 2 * jr0 + kPad - 2 * kLeft;
+  HaloUnpool<K, 128> h(threadIdx.x);
   uint32_t u = 0;
   for (long t = t_begin; t < t_end;) {
     const int col = static_cast<int>(t / p.H), y_start = static_cast<int>(t % p.H);
     const int n_out = static_cast<int>(min(static_cast<long>(p.H - y_start), t_end - t));
-    const int img = col / p.strips, jt = (col % p.strips) * 64 - kLeft + jr0;
-    uint32_t live = 0;  // steps whose pooled pixel is inside the image
-#pragma unroll
-    for (int s = 0; s < kSteps; ++s)
-      if (jr0 + 16 * s < kPooled && jt + 16 * s >= 0 && jt + 16 * s < Wp) live |= 1u << s;
-    const long v_img = static_cast<long>(img) * Hp, m_img = static_cast<long>(img % p.mask_n) * Hp;
+    h.strip(p, col / p.strips, (col % p.strips) * 128);
     for (int r = 0; r < n_out + K - 1; ++r, ++u) {
-      const int y = y_start - kPad + r;
-      const uint32_t row_live = y >= 0 && y < p.H ? live : 0u;
-      const __half* const vp = p.unpool_in + ((v_img + (y >> 1)) * Wp + jt) * 64 + 8 * c;
-      const uint8_t* const mp = p.unpool_mask + ((m_img + (y >> 1)) * Wp + jt) * 64 + 8 * c;
-      uint4 v[kSteps];
-      uint2 m[kSteps];
-#pragma unroll
-      for (int s = 0; s < kSteps; ++s) {
-        v[s] = make_uint4(0u, 0u, 0u, 0u);
-        m[s] = make_uint2(0u, 0u);
-        if (row_live & (1u << s)) {
-          v[s] = __ldg(reinterpret_cast<const uint4*>(vp + s * 16 * 64));
-          m[s] = __ldg(reinterpret_cast<const uint2*>(mp + s * 16 * 64));
-        }
-      }
       const int slot = u % kSlots;
-      mbar_wait(a_empty + slot, ((u / kSlots) & 1) ^ 1);
-      uint8_t* const dst = a_slots + slot * kSlotBytes;
-#pragma unroll
-      for (int dx = 0; dx < 2; ++dx) {
-        const int px = px0 + dx;
-        uint8_t* const d = dst + px * 128 + ((c ^ (px & 7)) << 4);
-        const uint32_t code = 0x01010101u * static_cast<uint32_t>(2 * (y & 1) + dx);
-#pragma unroll
-        for (int s = 0; s < kSteps; ++s) {
-          if (jr0 + 16 * s >= kPooled || px + 32 * s < 0 || px + 32 * s >= kHalo) continue;
-          const uint32_t lo = __vcmpeq4(m[s].x, code), hi = __vcmpeq4(m[s].y, code);  // 0xFF per matching byte
-          const uint4 o = make_uint4(v[s].x & __byte_perm(lo, 0u, 0x1100), v[s].y & __byte_perm(lo, 0u, 0x3322),
-                                     v[s].z & __byte_perm(hi, 0u, 0x1100), v[s].w & __byte_perm(hi, 0u, 0x3322));
-          *reinterpret_cast<uint4*>(d + s * 32 * 128) = o;
-        }
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes, read by wgmma
-      __syncwarp();
-      if (lane == 0) mbar_arrive(a_full + slot);
+      h.row(p, y_start - kPad + r, a_slots + slot * kSlotBytes, a_full + slot, a_empty + slot, ((u / kSlots) & 1) ^ 1);
     }
     t += n_out;
   }
@@ -1221,6 +1256,10 @@ bool tc_roll(const TcParams& p) { return p.chunks == 1 && !p.split; }
 // k_conv_stack: the 64 -> 16 float-logits layers, K = 3 / 7
 bool tc_stacked(const ConvTcPlan& plan) { return tc_roll(plan.p) && plan.p.n_tile == 16 && plan.k > 1; }
 // two images per 128-pixel M tile (PK2): chunked 3x3 layers at most 64 pixels wide
+// k_conv_tn: every Cin = 64, K = 7 layer with 64-wide half output tiles.  The K = 3 layers stay on k_conv_tc: on
+// k_conv_tn Standard's conv1_2_D (352 x 1024, T = 12) took 0.75 ms in one session and 1.77 ms in another, against
+// k_conv_tc's steady 1.35 ms (H100 80GB HBM3, 700 W).
+bool tc_tn(const ConvTcPlan& plan) { return tc_roll(plan.p) && plan.p.n_tile == 64 && plan.k == 7 && !plan.p.out_f32; }
 bool tc_pk2(const ConvTcPlan& plan) {
   const TcParams& p = plan.p;
   return !tc_roll(p) && !p.split && plan.k == 3 && p.W <= 64 && p.N_batch >= 2 && p.n_tile != 16;
@@ -1232,11 +1271,7 @@ bool tc_pk2(const ConvTcPlan& plan) {
 void tc_choose_kernel(ConvTcPlan& plan) {
   TcParams& p = plan.p;
   const int K = plan.k, n = p.n_tile;
-  const bool roll = tc_roll(p);
-  // k_conv_tn runs every Cin = 64, K = 7 layer with 64-wide half output tiles.  The K = 3 layers stay on k_conv_tc: on
-  // k_conv_tn Standard's conv1_2_D (352 x 1024, T = 12) took 0.75 ms in one session and 1.77 ms in another, against
-  // k_conv_tc's steady 1.35 ms (H100 80GB HBM3, 700 W).
-  const bool tn = roll && n == 64 && K == 7 && !p.out_f32;
+  const bool roll = tc_roll(p), tn = tc_tn(plan);
   // per (K, ROLL, KW, PK2): the three tile widths
   auto by_n = [n](TcKernel k16, TcKernel k64, TcKernel k128) { return n == 16 ? k16 : n == 64 ? k64 : k128; };
   if (tc_stacked(plan)) {
@@ -1247,7 +1282,7 @@ void tc_choose_kernel(ConvTcPlan& plan) {
       if (n == 16) plan.kern = K == 7 ? k_conv_tc<7, false, 7, false, 16, true> : K == 3 ? k_conv_tc<3, false, 3, false, 16, true> : k_conv_tc<1, false, 1, false, 16, true>;
       else plan.kern = K == 7 ? k_conv_tc<7, false, 7, false, 64, true> : K == 3 ? k_conv_tc<3, false, 3, false, 64, true> : k_conv_tc<1, false, 1, false, 64, true>;
     } else if (tn) {  // KW = 1: window-folded first layer
-      plan.kern = plan.kw == 7 ? k_conv_tn<7, 7> : k_conv_tn<7, 1>;
+      plan.kern = plan.kw == 1 ? k_conv_tn<7, 1> : p.unpool_in ? k_conv_tn<7, 7, true> : k_conv_tn<7, 7>;
     } else if (plan.kw == 1 && K == 3) {  // window-folded 3x3 first layer (3 x 1), 64-wide tiles
       plan.kern = k_conv_tc<3, true, 1, false, 64, false>;
     } else if (tc_pk2(plan)) {
@@ -1425,16 +1460,23 @@ void conv_tc_set_dropout(ConvTcPlan& plan, uint64_t seed, const uint64_t* frame_
   plan.p.drop_scale = scale;
 }
 
+bool conv_tc_can_fuse_unpool(const ConvTcPlan& plan) { return !tc_tn(plan) && !plan.p.unpool_in; }
+
 void conv_tc_set_unpool(ConvTcPlan& plan, const uint8_t* mask, int mask_n, void* out_2h_2w) {
+  if (!conv_tc_can_fuse_unpool(plan)) fail(SIVO_EINVAL, "conv_tc_set_unpool: this plan's kernel has no max-unpool scatter");
   plan.p.unpool_mask = mask;
   plan.p.mask_n = mask_n;
   plan.p.out = out_2h_2w;
 }
 
+bool conv_tc_can_unpool_input(const ConvTcPlan& plan) {
+  return plan.k == 7 && plan.kw == 7 && (tc_stacked(plan) || tc_tn(plan)) && !plan.p.unpool_mask;
+}
+
 void conv_tc_set_unpool_input(ConvTcPlan& plan, const void* pooled, const uint8_t* mask, int mask_n, int h, int w) {
-  if (!tc_stacked(plan) || plan.k != 7 || 2 * h != plan.p.H || 2 * w != plan.p.W || !pooled || !mask || mask_n < 1)
-    fail(SIVO_EINVAL, "conv_tc_set_unpool_input: needs a 7x7 float-logits plan over the %d x %d unpooled input (got %d x %d pooled)",
-         plan.p.H, plan.p.W, h, w);
+  if (!conv_tc_can_unpool_input(plan) || 2 * h != plan.p.H || 2 * w != plan.p.W || !pooled || !mask || mask_n < 1)
+    fail(SIVO_EINVAL, "conv_tc_set_unpool_input: needs a 7x7 float-logits or 64-wide half plan over the %d x %d unpooled input "
+                      "(got %d x %d pooled)", plan.p.H, plan.p.W, h, w);
   plan.p.unpool_in = static_cast<const __half*>(pooled);
   plan.p.unpool_mask = mask;
   plan.p.mask_n = mask_n;
@@ -1475,8 +1517,7 @@ void conv_tc_set_pool(ConvTcPlan& plan, void* pooled, uint8_t* mask) {
 }
 
 bool conv_tc_can_compose_classifier(const ConvTcPlan& plan) {
-  return tc_roll(plan.p) && plan.k == 7 && plan.kw == 7 && plan.p.n_tile == 64 && !plan.p.out_f32 && !plan.p.unpool_mask &&
-         !plan.p.has_drop && !plan.p.pool_out && !plan.p.relu && !plan.p.has_bn && plan.p.cout_total == 64;
+  return tc_tn(plan) && plan.kw == 7 && !plan.p.has_drop && !plan.p.pool_out && !plan.p.relu && !plan.p.has_bn && plan.p.cout_total == 64;
 }
 
 void conv_tc_set_composed_classifier(ConvTcPlan& plan, const Op& conv, const float* wc, const float* bc, int n_cls, float* logits) {

@@ -142,6 +142,35 @@ void SegNet::build(const NetSpec& net, const WeightMap& weights) {
                          "single-consumer chain (create the net with keep_blobs to run it unfused)", name.c_str());
     return it->second;
   };
+  // `conv` is a 7x7 convolution that can unpool on load, reading the max-unpool the last op writes -- an Unpool, or a
+  // sampling Dropout that writes its result unpooled (Basic's decoder: upsample4 .. upsample1).  The op is taken back: an
+  // Unpool is dropped, a DropoutUnpool writes the pooled tensor as a plain Dropout, and `conv` expands the pooled tensor as
+  // it loads its halo rows.  The unpooled tensor, three quarters zeros, is derived: never written.  The launch names stay
+  // those of the scattering build: the upsample is named with the launch that produces the values it places.
+  auto unpool_on_load = [&](Op& conv) {
+    Op& up = ops_.back();
+    int pooled;
+    if (up.kind == Op::Unpool && up.out == conv.in) pooled = up.in;
+    else if (up.kind == Op::DropoutUnpool && up.out2 == conv.in) pooled = up.out;
+    else return;
+    const Tensor& pt = *tensors_[pooled];
+    const Tensor& mt = *tensors_[up.in2];
+    conv_tc_set_unpool_input(*conv.tc, pt.v.p, mt.buf.as<uint8_t>(), mt.v.n, pt.v.h, pt.v.w);
+    Tensor& unpooled = *tensors_[conv.in];
+    unpooled.derived_from = pooled;
+    unpooled.derived_mask = up.in2;
+    unpooled.buf.release();
+    unpooled.v.p = nullptr;
+    if (up.kind == Op::Unpool) {
+      const std::string name = up.layer;
+      ops_.pop_back();
+      if (!ops_.empty() && ops_.back().out == pooled) ops_.back().layer += "+" + name;
+    } else {
+      up.kind = Op::Dropout;
+      tensors_[pooled]->elided = false;
+      up.in2 = up.out2 = -1;
+    }
+  };
   int drop_idx = 0;
   bool saw_softmax = false;
   for (size_t li = 0; li < net.layers.size(); ++li) {
@@ -246,24 +275,11 @@ void SegNet::build(const NetSpec& net, const WeightMap& weights) {
           conv.flops_exec = 2.0 * conv.cin * conv.k * conv.k * 16 * iv.h * iv.w * iv.n * conv_tc_rows_ratio(*conv.tc);
           conv.layer += "*" + ly.name;  // '*': composed, not merely fused
           Op* up = ops_.size() >= 2 ? &ops_[ops_.size() - 2] : nullptr;
-          if (up && up->kind == Op::Conv && up->use_tc && up->out2 == conv.in) {
-            // the input is scattered by the previous convolution's fused unpool (Basic: conv_decode2 -> upsample1), three
-            // quarters zeros: take that fusion back.  The previous convolution stores its own pooled-resolution output, and
-            // the composed kernel unpools it as it loads its halo rows.  The unpooled tensor is derived, never written.
-            Tensor& pooled = *tensors_[up->out];
-            Tensor& unpooled = *tensors_[conv.in];
-            const Tensor& mask = *tensors_[up->in2];
-            conv_tc_set_unpool(*up->tc, nullptr, 1, pooled.v.p);
-            pooled.elided = false;
-            conv_tc_set_unpool_input(*conv.tc, pooled.v.p, mask.buf.as<uint8_t>(), mask.v.n, pooled.v.h, pooled.v.w);
-            unpooled.derived_from = up->out;
-            unpooled.derived_mask = up->in2;
-            unpooled.buf.release();
-            unpooled.v.p = nullptr;
-            const size_t plus = up->layer.rfind('+');  // the unpool is the last layer fused into it
+          if (up && tensors_[conv.in]->derived_from == up->out) {
+            // the composed kernel unpools its input on load (Basic: conv_decode2 -> upsample1), and carries its name
+            const size_t plus = up->layer.rfind('+');  // the unpool is the last layer named with the producer
             conv.layer = up->layer.substr(plus + 1) + "+" + conv.layer;
             up->layer.erase(plus);
-            up->in2 = up->out2 = -1;
           }
           conv.flops += op.flops;  // algorithmic: the reference runs both layers
           tensors_[in]->elided = true;
@@ -283,6 +299,7 @@ void SegNet::build(const NetSpec& net, const WeightMap& weights) {
           fail(SIVO_EINVAL, "layer '%s': tcgen05 engine requested but the shape is not supported", ly.name.c_str());
         prepare_conv(op, act_, w, bias, bn ? (*bn)[0].data.data() : nullptr, bn ? (*bn)[1].data.data() : nullptr, civ, ov);
         op.flops_exec = op.split ? 3.0 * op.flops : op.flops * (op.use_tc ? conv_tc_rows_ratio(*op.tc) : 1.0);
+        if (!opt_.keep_blobs && op.use_tc && !ops_.empty() && conv_tc_can_unpool_input(*op.tc)) unpool_on_load(op);
         ops_.push_back(std::move(op));
         li = lj - 1;
         break;
@@ -320,24 +337,23 @@ void SegNet::build(const NetSpec& net, const WeightMap& weights) {
           fail(SIVO_EFORMAT, "layer '%s': mask blob '%s' does not match the input", ly.name.c_str(), ly.bottoms[1].c_str());
         const int up = add_tensor(ly.tops[0], iv.n, iv.c, iv.h * 2, iv.w * 2, iv.cs, act_);
         if (!opt_.keep_blobs && !ops_.empty() && ops_.back().kind == Op::Conv && ops_.back().use_tc && ops_.back().out == in &&
-            iv.dt == DType::F16 && iv.cs == iv.c) {
+            iv.dt == DType::F16 && iv.cs == iv.c && conv_tc_can_fuse_unpool(*ops_.back().tc)) {
           // the producing tensor-core convolution scatters straight into the unpooled tensor (its own output blob
           // is never materialised; keep_blobs keeps the two-kernel form so tests can read it)
           conv_tc_set_unpool(*ops_.back().tc, mt.buf.as<uint8_t>(), mt.v.n, tensors_[up]->v.p);
           tensors_[in]->elided = true;
           ops_.back().layer += "+" + ly.name;
-          ops_.back().in2 = m;  // recorded so that a consumer that unpools on load can take the fusion back
-          ops_.back().out2 = up;
           break;
         }
         if (!opt_.keep_blobs && !ops_.empty() && ops_.back().kind == Op::Dropout && ops_.back().out == in && iv.dt == DType::F16 &&
             iv.cs == iv.c && iv.cs % 8 == 0) {
-          // sampling Dropout feeding the upsample: one pass writes the unpooled tensor (the dropped blob is not materialised)
+          // sampling Dropout feeding the upsample: one pass writes the unpooled tensor out2 (the dropped blob `out` is not
+          // materialised)
           Op& d = ops_.back();
           tensors_[in]->elided = true;
           d.kind = Op::DropoutUnpool;
           d.in2 = m;
-          d.out = up;
+          d.out2 = up;
           d.layer += "+" + ly.name;
           break;
         }
@@ -487,7 +503,7 @@ void SegNet::enqueue(const uint8_t* bgr_dev, uint8_t* classes_dev, double* conf_
         d.layer = op.drop_layer;
         d.sample0 = s0_;
         const Tensor& mt = *tensors_[op.in2];
-        launch_dropout_unpool(tensors_[op.in]->v, ns_, mt.buf.as<uint8_t>(), mt.v.n, tensors_[op.out]->v, d, op.drop_scale, s);
+        launch_dropout_unpool(tensors_[op.in]->v, ns_, mt.buf.as<uint8_t>(), mt.v.n, tensors_[op.out2]->v, d, op.drop_scale, s);
         break;
       }
       case Op::Reduce: {

@@ -181,10 +181,14 @@ double conv_tc_rows_ratio(const ConvTcPlan& plan);
 // (sample0: global MC sample index of the batch's image 0, so that a shard handle draws the masks of its own samples)
 void conv_tc_set_dropout(ConvTcPlan& plan, uint64_t seed, const uint64_t* frame_dev, int layer, float scale, int sample0);
 // fuses the max-unpool (Upsample) that consumes the convolution's output into its epilogue; `out_2h_2w` is the
-// unpooled tensor the convolution then writes instead of its own output
+// unpooled tensor the convolution then writes instead of its own output.  k_conv_tn plans have no such epilogue: their
+// output is unpooled by its consumer (conv_tc_set_unpool_input) or by the unpool kernel.
+bool conv_tc_can_fuse_unpool(const ConvTcPlan& plan);
 void conv_tc_set_unpool(ConvTcPlan& plan, const uint8_t* mask, int mask_n, void* out_2h_2w);
-// makes a 7x7 float-logits (k_conv_stack) plan read the max-unpool of `pooled` ([n][h][w][64] half, the plan's input being
-// 2h x 2w) by `mask` (same layout, batch mask_n) instead of its input tensor: the unpool is done as the halo rows are loaded
+// makes a 7x7 float-logits (k_conv_stack) or 64-wide half (k_conv_tn) plan read the max-unpool of `pooled` ([n][h][w][64]
+// half, the plan's input being 2h x 2w) by `mask` (same layout, batch mask_n) instead of its input tensor: the unpool is
+// done as the halo rows are loaded
+bool conv_tc_can_unpool_input(const ConvTcPlan& plan);
 void conv_tc_set_unpool_input(ConvTcPlan& plan, const void* pooled, const uint8_t* mask, int mask_n, int h, int w);
 // fuses the 2x2/2 max pool (+ argmax mask) that consumes the convolution's output into its epilogue
 bool conv_tc_can_fuse_pool(const ConvTcPlan& plan);
